@@ -47,7 +47,29 @@ def parse_args():
     ap.add_argument("--reads", type=int, default=10000, help="reads per GPU")
     ap.add_argument("--events", type=int, default=4000, help="events per read")
     ap.add_argument("--no-cpu-baseline", action="store_true")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed path computed in its last step as DIR/<name>.npy (float32/float64; "
+                         "workloads scorereads, methylation, call_methylation and variants)")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.workload in ("abea", "events", "prologue", "eventalign"):
+        ap.error(f"--dump-outputs is not supported for --workload {args.workload}")
+    return args
+
+
+DUMP_LIMIT = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """Save {name: array} as out_dir/<name>.npy; integers and float32 as float32, float64 as float64, 64 MB at most in all."""
+    conv = {k: np.ascontiguousarray(v, np.float64 if v.dtype == np.float64 else np.float32) for k, v in arrays.items()}
+    total = sum(v.nbytes for v in conv.values())
+    if total > DUMP_LIMIT:
+        raise ValueError(f"--dump-outputs: {total} bytes exceed the {DUMP_LIMIT}-byte limit")
+    os.makedirs(out_dir, exist_ok=True)
+    for k, v in conv.items():
+        np.save(os.path.join(out_dir, k + ".npy"), v)
 
 
 def peaks():
@@ -57,7 +79,7 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s; not a measured figure)"
 
 
 def cpu_quota():
@@ -77,16 +99,15 @@ def cpu_quota():
 
 
 def cpu_threads():
-    """Threads for the CPU arm: every logical CPU, unless a cgroup quota makes that oversubscription — measured on the
-    B200 boxes (profiles/r01_cpu_threads.json): 128 threads under a 16-CPU quota run the reference 28 % slower than 32.
-    Twice the quota is the fastest setting there, so that is what the reference gets."""
+    """Threads for the CPU arm: every logical CPU, unless a cgroup quota makes that oversubscription (many more threads than
+    the quota allows run the reference slower); then twice the quota."""
     n = os.cpu_count() or 1
     q = cpu_quota()
     return n if not q else max(1, min(n, int(round(2 * q))))
 
 
 class ClockSampler:
-    """nvidia-smi sampled every 200 ms DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampled every 200 ms DURING the timed region (SM clock, power draw and throttle reasons)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -150,32 +171,6 @@ def build_workload(args, rank):
         rs = synth.gen_reads(args.reads, args.events, nuc, seed=seed, cpg_keep=0.3)
         jobs = synth.methylation_jobs(rs, model_id=1)
     return rs, jobs, models
-
-
-def k1_rooflines(args, jobs, kernel_ms, clocks):
-    """The two rooflines that do bound K1 (DESIGN.md section 3.4), from MEASURED counters: profiles/r02_k1_counters.json holds ncu's executed
-    warp instructions and shared-memory wavefronts of one pass of the forward kernels over this workload (same reads, same job list);
-    per block-cell they do not depend on the clock, so the live kernel time turns them into rates.
-      issue : warp instructions per second against 148 SMs x 4 schedulers x SM clock
-      shared: shared-memory wavefronts per second against 148 SMs x 1 wavefront per clock (the table look-ups replay on bank conflicts)"""
-    out = {}
-    try:
-        c = json.load(open(os.path.join(ROOT, "profiles", "r02_k1_counters.json"))).get(args.workload)
-    except Exception:
-        c = None
-    clk = ((clocks or {}).get("sm_mhz") or 1965.0) * 1e6
-    if c and c.get("reads") == args.reads and args.events == 4000:
-        inst_per_cell = c["inst_executed"] * 32.0 / float(jobs.block_cells)       # lane-instructions per block-cell, as ncu counted them
-        issue = c["inst_executed"] / (kernel_ms * 1e-3)
-        shared = c["lds_wavefronts"] / (kernel_ms * 1e-3)
-        out["issue"] = {"achieved": issue, "unit": "warp-instructions/s", "peak": 148 * 4 * clk, "frac": issue / (148 * 4 * clk),
-                        "instructions_per_block_cell": inst_per_cell, "source": "measured: smsp__inst_executed (profiles/r02_k1_counters.json) / live kernel time"}
-        out["shared_memory"] = {"achieved": shared, "unit": "wavefronts/s", "peak": 148 * clk, "frac": shared / (148 * clk),
-                                "bank_conflict_share": c["lds_conflict_wavefronts"] / c["lds_wavefronts"],
-                                "source": "measured: l1tex__data_pipe_lsu_wavefronts_mem_shared / live kernel time"}
-        if c.get("dram_bytes"):
-            out["traffic"] = c["dram_bytes"]
-    return out
 
 
 def algorithmic_bytes(jobs, k=6):
@@ -284,7 +279,7 @@ def workload_config(args, jobs, reads_override=None):
                            else "cpg model, CpG-group windows u/m pairs, flags PRE|POST"),
             "reads_per_gpu": reads_override or args.reads, "events_per_read": args.events,
             "mean_E": float(E.mean()), "mean_K": float(j["n_kmers"].mean()),
-            "parallelism": f"read-shard x{args.gpus}", "l2": "inputs larger than L2 (levels+ranks+scratch > 126 MB)"}
+            "parallelism": f"read-shard x{args.gpus}", "l2": "inputs larger than L2 (levels+ranks+scratch > 50 MB)"}
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -297,7 +292,7 @@ class _DevBytes:
         self.__cuda_array_interface__ = {"shape": (nbytes,), "typestr": "|u1", "data": (ptr, False), "version": 2}
 
 
-def call_methylation_block(args, rank, world, local, steps, warmup):
+def call_methylation_block(args, rank, world, local, steps, warmup, dump=None):
     """One step = nph_methylation_run over the resident batch (motif scan, grouping, event bounds, k-mer ranks, schedule,
     both forward scores per group, site records) and, at N > 1, ONE variable-length NCCL gather of the site records to
     rank 0 straight from device memory.  e2e = the C++ host's flat entry (libnph_host.so nphh_call_methylation_flat): page-locked
@@ -360,11 +355,14 @@ def call_methylation_block(args, rank, world, local, steps, warmup):
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     total_ms = float(t.item())
     n_sites, n_jobs, scored = eng.methylation_counts()
+    site_off, sites = eng.methylation_fetch()
+    if dump is not None:
+        dump.update({"meth_site_start": sites["start_position"], "meth_site_ll_unmethylated": sites["ll_unmethylated"],
+                     "meth_site_ll_methylated": sites["ll_methylated"]})
     kern = []
     for _ in range(5):
         eng.methylation_run(); eng.sync(); kern.append(eng.last_kernel_ms())
     kernel_ms, launches = float(np.mean([k[0] for k in kern])), int(kern[-1][1])
-    site_off, sites = eng.methylation_fetch()
     tot = torch.tensor([float(scored), float(n_sites), float(n_reads)], dtype=torch.float64, device=dev)
     if world > 1:
         dist.all_reduce(tot)
@@ -414,7 +412,7 @@ def call_methylation_block(args, rank, world, local, steps, warmup):
     for _ in range(2):
         tsv_bytes = e2e_step()
     barrier()
-    e2e_steps = max(3, min(steps, 10))
+    e2e_steps = steps
     stage = np.zeros(2)
     t0 = time.perf_counter()
     for _ in range(e2e_steps):
@@ -447,7 +445,7 @@ def call_methylation_block(args, rank, world, local, steps, warmup):
                           "reads_per_gpu": n_reads, "reads_total": reads_all, "events_per_read": args.events, "sites_per_step": sites_all,
                           "jobs_per_gpu": n_jobs, "scored_events_per_step": scored_all, "parallelism": f"read-shard x{world}",
                           "multi_gpu": "one variable-length NCCL gather of the 24-byte site records to rank 0 per step" if world > 1 else None,
-                          "l2": "inputs larger than L2 (levels + event alignments + reference > 126 MB)"},
+                          "l2": "inputs larger than L2 (levels + event alignments + reference > 50 MB)"},
                "e2e": {"value": scored_all * e2e_steps / e2e_s, "unit": UNIT, "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": int(d2h),
                        "steps": e2e_steps, "tsv_bytes_per_step": tsv_bytes, "ms_per_step": e2e_s / e2e_steps * 1e3,
                        "stage_ms": {"device_call": float(stage[0] / e2e_steps * 1e3), "host_side": float(stage[1] / e2e_steps * 1e3)},
@@ -524,7 +522,7 @@ def call_methylation_cpu(rs, recs, ref, pairs, site_off, sites, tsv_ours):
 # variants --consensus candidate screening (BASELINE configs[4]): every single-base edit of every position of a region scored
 # against the pile-up with the reference's early-exit rule; enumeration, rounds and accumulation on the device.
 # ------------------------------------------------------------------------------------------------------------------
-def variants_block(args, rank, world, local, steps, warmup):
+def variants_block(args, rank, world, local, steps, warmup, dump=None):
     """One step = nph_screen_run over the resident pile-up (windows' event sequences, edited-window ranks, rounds of
     reads_per_round reads with the early exit applied between rounds, qualities) + fetch of the 9 qualities per position; at N > 1
     the region is cut into one slice per rank (positions are independent: no data-path collective) and the slices' qualities are
@@ -583,6 +581,8 @@ def variants_block(args, rank, world, local, steps, warmup):
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     total_ms = float(t.item())
+    if dump is not None:
+        dump.update({"screen_qualities": q, "screen_reads": nr})
     cnt = eng.screen_counts()
     kernel_ms, launches = float(np.mean([k[0] for k in kms])), int(kms[-1][1])
     tot = torch.tensor([float(cnt["reference_events"]), float(cnt["scored_events"]), float(cnt["jobs"]), float(cnt["jobs_without_exit"])],
@@ -598,7 +598,7 @@ def variants_block(args, rank, world, local, steps, warmup):
     for _ in range(2):
         e2e_step()
     barrier()
-    e2e_steps = max(3, min(steps, 10))
+    e2e_steps = steps
     t0 = time.perf_counter()
     for _ in range(e2e_steps):
         q2, nr2, _ = e2e_step()
@@ -629,7 +629,7 @@ def variants_block(args, rank, world, local, steps, warmup):
                           "reference_dp_rows_per_step": ref_events_all, "our_dp_rows_per_step": our_rows_all, "jobs_per_step": jobs_all,
                           "jobs_without_early_exit": jobs_noexit_all, "parallelism": f"region-slice x{world}",
                           "multi_gpu": "positions are independent: one region slice per rank, one NCCL gather of the qualities" if world > 1 else None,
-                          "l2": "inputs larger than L2 (events + rank pool > 126 MB)"},
+                          "l2": "inputs larger than L2 (events + rank pool > 50 MB)"},
                "e2e": {"value": ref_events_all * e2e_steps / e2e_s, "unit": UNIT, "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": int(d2h),
                        "steps": e2e_steps, "ms_per_step": e2e_s / e2e_steps * 1e3, "api": "nph_screen_edits_batch (host buffers in, qualities out)"},
                "gpu_launches": launches * steps,
@@ -922,16 +922,10 @@ def run_aux(args, rank, world, local, saved_stdout):
                 "gpu_launches": 2 * args.steps,
                 "roofline": {"bound": "hbm", "achieved": b_alg / (t * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
                              "frac": b_alg / (t * 1e-3) / 1e9 / peak,
-                             # DRAM bytes of the two kernels for the 4 096-read shape (profiles/r02_events_summary.md: 1.07 GB + 1.35 GB)
-                             "traffic": 2.42e9 if reads.shape[0] == 4096 else None, "peak_source": peak_src,
+                             "traffic": None, "peak_source": peak_src,
                              "kernel": "ed_fused_kernel + ed_events_kernel",
                              "note": "algorithmic bytes = 4 B/sample in + 24 B/event out; the fused kernel is bound by the float<->double "
-                                     "conversion unit and FP64 latency, not by HBM (DESIGN.md section 11)",
-                             # compute_tstat needs >= 24 conversions per sample position (after staging each sample once), 8.5 clk per
-                             # warp instruction and sub-partition (profiles/r02_ubench_cvt.txt), x 1.11 for the 128-sample warm-ups
-                             "conversion_unit": {"floor_ms": raw.shape[0] / 32 * 24 * 1.11 * 8.5 / (148 * 4 * 1.965e6),
-                                                 "frac": raw.shape[0] / 32 * 24 * 1.11 * 8.5 / (148 * 4 * 1.965e6) / t,
-                                                 "unit": "share of the step the conversion unit alone would need"}}}
+                                     "conversion unit and FP64 latency, not by HBM (DESIGN.md section 11)"}}
     emit(line, saved_stdout)
     eng.close()
 
@@ -963,8 +957,11 @@ def main():
         sampler = ClockSampler(local)
         if rank == 0:
             sampler.start()
-        blk = variants_block(args, rank, world, local, args.steps, args.warmup)
+        dump = {} if args.dump_outputs else None
+        blk = variants_block(args, rank, world, local, args.steps, args.warmup, dump)
         if rank == 0:
+            if dump is not None:
+                dump_outputs(args.dump_outputs, dump)
             blk["clocks"] = sampler.stop()
             emit(blk, saved_stdout)
         if world > 1:
@@ -980,8 +977,11 @@ def main():
         sampler = ClockSampler(local)
         if rank == 0:
             sampler.start()
-        blk = call_methylation_block(args, rank, world, local, args.steps, args.warmup)
+        dump = {} if args.dump_outputs else None
+        blk = call_methylation_block(args, rank, world, local, args.steps, args.warmup, dump)
         if rank == 0:
+            if dump is not None:
+                dump_outputs(args.dump_outputs, dump)
             blk.update({"higher_is_better": True, "vs_baseline": None, "clocks": sampler.stop()})
             emit(blk, saved_stdout)
         if world > 1:
@@ -1062,6 +1062,7 @@ def main():
     e1.record()
     barrier()
     total_ms = e0.elapsed_time(e1)
+    dump = {"scores": scores[:n_jobs].cpu().numpy()} if args.dump_outputs else None
     km, launches_per_step = eng.last_kernel_ms()
     t = torch.tensor([total_ms], dtype=torch.float64, device=dev)
     if world > 1:
@@ -1091,10 +1092,12 @@ def main():
         e2e_step()
     barrier()
     t0 = time.perf_counter()
-    e2e_steps = max(3, min(args.steps, 10))
+    e2e_steps = args.steps
     for _ in range(e2e_steps):
         e2e_step()
     torch.cuda.synchronize()
+    if dump is not None:
+        dump["e2e_scores"] = h_out.copy()
     e2e_s = time.perf_counter() - t0
     t = torch.tensor([e2e_s], dtype=torch.float64, device=dev)
     if world > 1:
@@ -1110,7 +1113,6 @@ def main():
         peak, peak_src = peaks()
         b_alg = algorithmic_bytes(jobs)
         achieved = b_alg / (kernel_ms * 1e-3) / 1e9
-        traffic = None          # filled from profiles/r02_k1_counters.json by k1_rooflines when the workload matches the capture
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps,
             "warmup": max(3, args.warmup), "ms_per_step": total_ms / args.steps, "higher_is_better": True,
@@ -1122,13 +1124,12 @@ def main():
                     "steps": e2e_steps, "api": "nph_hmm_score_batch_seq (host buffers in: events + 1 B/base sequence codes + jobs; host scores out)"},
             "gpu_launches": int(launches_per_step) * args.steps,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": traffic, "peak_source": peak_src, "kernel": "hmm_forward_kernel<C>",
+                         "traffic": None, "peak_source": peak_src, "kernel": "hmm_forward_kernel<C>",
                          "kernel_ms": kernel_ms, "algorithmic_bytes_per_step": b_alg,
                          "note": "scalar log-semiring DP: issue/shared-memory bound, not HBM bound (DESIGN.md); "
                                  "block-cells/s below is the figure that moves",
                          "block_cells_per_sec_per_gpu": float(jobs.block_cells) / (kernel_ms * 1e-3)},
         }
-        line["roofline"].update(k1_rooflines(args, jobs, kernel_ms, clocks))
         if world == 1 and not args.no_cpu_baseline:
             try:
                 arm = CpuArm(rs, jobs, models)
@@ -1142,12 +1143,14 @@ def main():
     cm = None
     if not args.no_call_methylation:
         try:
-            cm = call_methylation_block(args, rank, world, local, max(3, min(args.steps, 10)), args.warmup)
+            cm = call_methylation_block(args, rank, world, local, args.steps, args.warmup, dump)
         except Exception as ex:          # never lose the headline line over the extra block
             cm = {"error": f"{type(ex).__name__}: {ex}"} if rank == 0 else None
     if rank == 0:
         if cm is not None:
             line["configs"] = {"call_methylation": cm}
+        if dump is not None:
+            dump_outputs(args.dump_outputs, dump)
         emit(line, saved_stdout)
     if world > 1:
         dist.barrier()

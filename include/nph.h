@@ -1,4 +1,4 @@
-/* nph.h — C ABI of the B200-native nanopolish HMM engine (libnph.so).
+/* nph.h — C ABI of the H100-native nanopolish HMM engine (libnph.so).
  *
  * This is the drop-in boundary for the ONE hot path this repository accelerates
  * (SURVEY.md section 8):

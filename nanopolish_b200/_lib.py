@@ -26,7 +26,7 @@ def load() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise FileNotFoundError(
             f"{LIB_PATH} is not built; the engine has no CPU path. Build it with "
-            f"`make -C {os.path.join(HERE, 'csrc')}` (nvcc, sm_100a).")
+            f"`make -C {os.path.join(HERE, 'csrc')}` (nvcc, sm_90a).")
     lib = C.CDLL(LIB_PATH)
     vp, sz, u32, dbl = C.c_void_p, C.c_size_t, C.c_uint32, C.c_double
     lib.nph_strerror.restype = C.c_char_p

@@ -1,4 +1,4 @@
-// abea.cu — K2: adaptive banded event-to-sequence alignment on sm_100a, and the method-of-moments
+// abea.cu — K2: adaptive banded event-to-sequence alignment on sm_90a, and the method-of-moments
 // scaling estimate that prepares its input.
 //
 // Replaces, for a batch of reads:

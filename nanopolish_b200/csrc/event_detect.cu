@@ -288,7 +288,7 @@ constexpr int kPeakWarps = 4;
 // exactness guard rides along on the samples the warp touches anyway.
 //   * what bounds it is not HBM but the float<->double conversion unit: compute_tstat needs >= 10 conversions per
 //     window and position however it is arranged (float sums, float means, float variance, double quotient), and a
-//     conversion costs 8.5 clk per warp instruction (scripts/ubench_cvt.cu, profiles/r02_ubench_cvt.txt)
+//     conversion issues at a fraction of the FP32 rate (scripts/ubench_cvt.cu measures it)
 //   * divisions by the window length are Markstein divisions by a cached reciprocal (exact_math.cuh); the final
 //     |delta| / sqrt(v) is D * rsqrt(v) in FP64 (<= 2 ulp) rounded to float, accepted only when that FP64 value is
 //     more than 2^10 ulps away from a float rounding boundary (so the correctly rounded chain dsqrt -> ddiv -> float
@@ -349,8 +349,8 @@ __device__ __noinline__ float tstat_windows_exact(float combined_var, float delt
 
 // A row of the tile: the 32 positions [p0 + w2, p0 + w2 + 32) of one lane's range.  The warp first stages the row and its
 // halo (32 + 2*w2 samples from p0; zeros outside the read) in shared memory as doubles — x and the float product x*x,
-// each sample converted ONCE (the float->double conversion is the scarce resource here: 8.5 clk per warp instruction,
-// profiles/r02_ubench_cvt.txt) — and feeds the exactness guard with the samples it touches.
+// each sample converted ONCE (the float->double conversion is the scarce resource here) — and feeds the exactness guard
+// with the samples it touches.
 constexpr int kFusedMaxW2 = 14;                   // scrappie: 6 (DNA), 14 (RNA); wider windows take the streaming kernel
 constexpr int kRowBuf = 32 + 2 * kFusedMaxW2;
 

@@ -27,7 +27,7 @@
 struct LogsumTable {
     uint32_t biased_base;   // shared-window byte address of entry 0, minus 4 * 0x4B000000 (mod 2^32)
     uint32_t scale;         // 4, as a RUNTIME value: bits * scale + base then stays one IMAD on the FMA pipe; with a literal 4 ptxas
-                            // picks LEA, which issues on the half-rate ALU pipe that FMNMX already loads (profiles/r02_*)
+                            // picks LEA, which issues on the half-rate ALU pipe that FMNMX already loads
 };
 
 // `bias` must be NPH_LOGSUM_ADDR_BIAS and must reach the kernel as a RUNTIME value (a kernel parameter):
@@ -74,53 +74,4 @@ __device__ __forceinline__ float div_by_cached_rcp(float a, float b, float y)
     const float q1 = __fmaf_rn(r0, y, q0);
     const float r1 = __fmaf_rn(-q1, b, a);
     return __fmaf_rn(r1, y, q1);
-}
-
-// ---- sm_100 packed FP32 (add/sub/mul/fma .f32x2: SASS FADD2 / FMUL2 / FFMA2) ------------------------------------
-// Two IEEE-754 binary32 operations per issue slot on a 64-bit register pair; each half is rounded exactly like the
-// scalar instruction (round-to-nearest-even, or toward -inf for the .rm form), so results stay bit-identical to the
-// reference's scalar arithmetic.  The pipe still spends two cycles on a packed instruction (measured:
-// profiles/r02_ubench_f32x2.txt, 31.5 vs 29.3 lane-ops/clk/SMSP), the gain is in ISSUE slots, which is what bounds K1.
-// max/min have no packed form and the table load is per element: those stay scalar on the halves of the pair (a pair's
-// halves are ordinary 32-bit registers, no move is needed to use them one by one).
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 pk2(float lo, float hi) { f32x2 r; asm("mov.b64 %0, {%1,%2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
-__device__ __forceinline__ f32x2 bc2(float x) { return pk2(x, x); }
-__device__ __forceinline__ float lo2(f32x2 a) { return __uint_as_float((unsigned int)(a & 0xffffffffull)); }
-__device__ __forceinline__ float hi2(f32x2 a) { return __uint_as_float((unsigned int)(a >> 32)); }
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) { f32x2 r; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ f32x2 sub2(f32x2 a, f32x2 b) { f32x2 r; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { f32x2 r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { f32x2 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r; }
-__device__ __forceinline__ f32x2 add2_rd(f32x2 a, f32x2 b) { f32x2 r; asm("add.rm.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-
-// two quantised log-sums at once: (a.lo (+) b.lo, a.hi (+) b.hi); 12 issue slots instead of 16.
-// |d| * 1000 is formed as |d * 1000| (RN is sign-symmetric), the abs riding on the FMNMX source modifier.
-__device__ __forceinline__ f32x2 lsum2(f32x2 a, f32x2 b, const LogsumTable tb)
-{
-    const f32x2 mx = pk2(fmaxf(lo2(a), lo2(b)), fmaxf(hi2(a), hi2(b)));
-    const f32x2 t = mul2(sub2(a, b), bc2(1000.0f));
-    const f32x2 tc = pk2(fminf(fabsf(lo2(t)), (float)NPH_LOGSUM_CUT), fminf(fabsf(hi2(t)), (float)NPH_LOGSUM_CUT));
-    const f32x2 u = add2_rd(tc, bc2(8388608.0f));
-#ifdef NPH_LSUM_LEA
-    const uint32_t a0 = (uint32_t)__float_as_int(lo2(u)) * 4u + tb.biased_base;
-    const uint32_t a1 = (uint32_t)__float_as_int(hi2(u)) * 4u + tb.biased_base;
-#else
-    const uint32_t a0 = (uint32_t)__float_as_int(lo2(u)) * tb.scale + tb.biased_base;
-    const uint32_t a1 = (uint32_t)__float_as_int(hi2(u)) * tb.scale + tb.biased_base;
-#endif
-    float v0, v1;
-    asm("ld.shared.f32 %0, [%1];" : "=f"(v0) : "r"(a0));
-    asm("ld.shared.f32 %0, [%1];" : "=f"(v1) : "r"(a1));
-    return add2(mx, pk2(v0, v1));
-}
-
-// Markstein division of both halves; nb = -b (fma(-q, b, a) == fma(q, -b, a) exactly), y = RN(1/b)
-__device__ __forceinline__ f32x2 div2_by_cached_rcp(f32x2 a, f32x2 nb, f32x2 y)
-{
-    const f32x2 q0 = mul2(a, y);
-    const f32x2 r0 = fma2(q0, nb, a);
-    const f32x2 q1 = fma2(r0, y, q0);
-    const f32x2 r1 = fma2(q1, nb, a);
-    return fma2(r1, y, q1);
 }

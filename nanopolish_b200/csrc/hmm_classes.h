@@ -2,9 +2,8 @@
 //
 // A class is (C columns per lane, W lanes per job); 32/W jobs share a warp.  W < 32 classes hold
 // single-strip jobs (K <= W*C); W == 32 also chains strips for wide jobs.  A job goes to the class that
-// minimises modelled issue slots = steps x (per-step overhead + C x per-cell cost) x W/32, with the
-// constants measured by ncu (profiles/): ~96 per warp step, ~88 instructions per block-cell for odd C and ~66 for
-// even C (whose columns run pairwise on sm_100's packed FP32 instructions).
+// minimises modelled issue slots = steps x (per-step overhead + C x per-cell cost) x W/32: ~96 per warp step and
+// ~88 instructions per block-cell.
 #pragma once
 #include <stdint.h>
 
@@ -35,18 +34,10 @@ NPH_HD uint32_t nph_class_steps(uint32_t K, uint32_t E, int C, uint32_t W)
     return (n_strips - 1) * P + E + (last_cols - 1) / (uint32_t)C;
 }
 
-// per-step cost: ~96 issue slots of per-step work plus the row update, ~88 per column in the scalar form.  Even C runs the row
-// update pairwise on sm_100's packed FP32 instructions (~66 issue slots per column), which pays where the kernel is issue
-// bound — the sub-warp classes of short windows (measured: call-methylation windows 2.09 -> 1.97 ms) — and does not in the
-// full-warp classes, where the 16 warps of a CTA keep the shared-memory pipe ~80 % busy with the table look-ups' bank conflicts
-// (2.6 wavefronts per LDS) and packed C = 10 only adds padding over scalar C = 9 (profiles/r02_k1_variants.md).
-#ifndef NPH_EVEN_CELL_COST
-#define NPH_EVEN_CELL_COST 66.0f
-#endif
+// per-step cost: ~96 issue slots of per-step work plus the row update, ~88 per column
 NPH_HD float nph_class_cost(uint32_t steps, int C, uint32_t W)
 {
-    const float cell = ((C & 1) || W == 32u) ? 88.0f : NPH_EVEN_CELL_COST;
-    return (float)steps * (96.0f + cell * C) * (W * (1.0f / 32.0f));
+    return (float)steps * (96.0f + 88.0f * C) * (W * (1.0f / 32.0f));
 }
 
 // returns class index; *steps_out = steps in that class

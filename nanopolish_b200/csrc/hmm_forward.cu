@@ -75,7 +75,6 @@ int nph_launch_hmm_forward(nph_ctx* ctx, float* scores_dev)
     p.c = ctx->consts;
     p.lsum_bias = NPH_LOGSUM_ADDR_BIAS;
     p.lsum_scale = 4u;
-    p.neg_zero = -0.0f;
     p.progress = (ctx->levels_inflight && ctx->level_chunk_events) ? ctx->d_progress : nullptr;
     p.chunk_events = (uint32_t)ctx->level_chunk_events;
     const size_t slice = scratch_slice_bytes(ctx);

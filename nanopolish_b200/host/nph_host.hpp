@@ -358,8 +358,8 @@ size_t format_fixed(char* dst, double v, int prec);
 
 // Threads the host-side batch loops use (chain building, record scatter, TSV formatting): $NPH_HOST_THREADS if set,
 // else min(omp_get_max_threads(), 32) — GPU nodes expose many more logical CPUs than a container's CPU quota covers
-// (the B200 boxes of this project: 128 logical CPUs, cgroup quota 16), and a parallel region that oversubscribes them pays
-// for it at every barrier; short bursts of 32-64 threads still fit one quota period (measured: profiles/r01_host_threads.md).
+// (e.g. 128 logical CPUs under a cgroup quota of 16), and a parallel region that oversubscribes them pays for it at every
+// barrier; short bursts of 32-64 threads still fit one quota period.
 int host_threads();
 
 namespace detail {

@@ -487,7 +487,7 @@ void MethylationCaller::run(Engine& engine, double indel_bias)
 // one TSV row (write_methylation_results_as_tsv, call_methylation.cpp:532-550): chromosome, strand, start, end, read_name,
 // log_lik_ratio %.2lf, log_lik_methylated %.2lf, log_lik_unmethylated %.2lf, num_calling_strands, num_motifs, sequence.
 // Rows are written straight into a growing character buffer: "%d" by a reversed-digit loop, "%.2lf" by format_fixed (exact
-// integer arithmetic, nph_host.cpp) — no printf and no per-field string appends (19 -> 4 ms per 350 000 rows on the B200 box).
+// integer arithmetic, nph_host.cpp) — no printf and no per-field string appends.
 namespace {
 struct RowBuffer {
     std::unique_ptr<char[]> p;
@@ -700,7 +700,7 @@ size_t call_methylation_flat(Engine& engine, const FlatMethylationBatch& b, cons
     for (size_t r = 0; identity && r < n; ++r)
         identity = b.records[r].read == r && (r == 0 || (b.reads[r].event_off == b.reads[r - 1].event_off + b.reads[r - 1].n_events &&
                                                          b.records[r].ref_off == b.records[r - 1].ref_off + b.records[r - 1].ref_len));
-    // Measured on the B200 box (10 000 reads): four pipelined sub-batches 21.8 ms against 13.0 ms for one call — every sub-batch pays the
+    // One call rather than pipelined sub-batches: every sub-batch pays the
     // call's fixed costs (two read-backs, ten class launches, the scheduler) and the formatter's thread teams compete with the driver
     // thread for the container's CPU quota.  One call it is; the sub-batch path stays behind $NPH_METH_PIPELINE for larger batches.
     static const bool want_pipeline = std::getenv("NPH_METH_PIPELINE") != nullptr;

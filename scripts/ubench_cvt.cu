@@ -34,10 +34,11 @@ template <int OP> __global__ void k(float* out, float seed, long long* clk)
 }
 template <int OP> void run(const char* name, int per_iter)
 {
-    float* out; long long* clk; cudaMalloc(&out, 148 * 1024 * 4); cudaMalloc(&clk, 8);
+    int sms = 0; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+    float* out; long long* clk; cudaMalloc(&out, sms * 1024 * 4); cudaMalloc(&clk, 8);
     for (int warps = 4; warps <= 32; warps *= 2) {          // warps per SM (1..8 per sub-partition)
-        k<OP><<<148, warps * 32>>>(out, 1.5f, clk); cudaDeviceSynchronize();
-        k<OP><<<148, warps * 32>>>(out, 1.5f, clk); cudaDeviceSynchronize();
+        k<OP><<<sms, warps * 32>>>(out, 1.5f, clk); cudaDeviceSynchronize();
+        k<OP><<<sms, warps * 32>>>(out, 1.5f, clk); cudaDeviceSynchronize();
         long long c; cudaMemcpy(&c, clk, 8, cudaMemcpyDeviceToHost);
         printf("%-28s warps/SMSP %d : %.3f warp-instr/clk/SMSP\n", name, warps / 4, (double)per_iter * N_ITER * (warps / 4) / (double)c);
     }

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
 
 
 @pytest.fixture(scope="session")
@@ -19,11 +19,34 @@ def port_oracle():
 
 
 @pytest.fixture(scope="session")
-def ref_oracle():
+def _ref_session():
+    """(live RefOracle or None, recorded calls, record path or None); see tests/ref_calls.py"""
     from oracle.oracle_py import RefOracle
-    if not RefOracle.available():
-        pytest.skip("compiled reference (oracle/_ref/libnpref.so) not present on this box")
-    return RefOracle()
+    from tests import ref_calls
+    path = os.environ.get("NPH_REF_RECORD")
+    live = RefOracle() if RefOracle.available() else None
+    if path and live is None:
+        pytest.fail("NPH_REF_RECORD needs the compiled reference (oracle/_ref/libnpref.so)")
+    calls = ref_calls.load()
+    yield live, calls, path
+    if path:
+        ref_calls.save(calls, path)
+
+
+@pytest.fixture
+def ref_oracle(request, _ref_session):
+    """The compiled reference: live where oracle/_ref/libnpref.so exists, else its recorded answers for this test."""
+    from tests import ref_calls
+    live, calls, path = _ref_session
+    key = ref_calls.test_key(request.node)
+    if path:
+        calls[key] = []
+        return ref_calls.Recorder(live, calls[key])
+    if live is not None:
+        return live
+    if key not in calls:
+        pytest.fail(f"no recorded reference answers for {key} (tests/golden/ref_calls.pkl.xz)")
+    return ref_calls.Replay(key, calls[key])
 
 
 @pytest.fixture(scope="session")
