@@ -1,7 +1,7 @@
 // check_tsv_format — tsv_format.cuh against the C library: printf("%.2lf") on random and adversarial doubles (values the
 // call-methylation rows hold: float scores widened and their differences; exact halves at the second decimal; tiny, huge,
 // negative zero), and %d on the integer range; the same inputs through the device copies of the functions.
-// Build: nvcc -O2 -gencode arch=compute_90a,code=sm_90a -I nanopolish_b200/csrc tests/cuda/check_tsv_format.cu -o tests/cuda/check_tsv_format
+// Build: nvcc -O2 -gencode arch=compute_90a,code=sm_90a -I nanopolish_b200/csrc tests/cuda/check_tsv_format.cu -o build/checks/check_tsv_format
 // Usage: check_tsv_format [--host-only]
 #include "tsv_format.cuh"
 #include <cstdio>

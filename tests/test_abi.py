@@ -72,10 +72,10 @@ def test_dist_library_exports():
 
 @pytest.mark.gpu
 def test_dist_gather_on_visible_gpus():
-    """tests/cuda/dist_gather_check: one host thread per visible GPU, variable-length gather to rank 0, the too-small-root case
+    """dist_gather_check (tests/cuda/dist_gather_check.cu, built into build/checks/): one host thread per visible GPU, variable-length gather to rank 0, the too-small-root case
     (every rank fails alike, nobody hangs) and the f64 reduce — a C++ caller sharding without Python."""
     import subprocess
-    exe = os.path.join(ROOT, "tests", "cuda", "dist_gather_check")
+    exe = os.path.join(ROOT, "build", "checks", "dist_gather_check")
     r = subprocess.run([exe], capture_output=True, text=True, timeout=120)
     assert r.returncode == 0, r.stdout + r.stderr
     assert "ok" in r.stdout
@@ -84,7 +84,7 @@ def test_dist_gather_on_visible_gpus():
 def test_tsv_number_formatting_on_host():
     """the host copy of csrc/tsv_format.cuh against snprintf (the device copy runs in the gpu tests)"""
     import subprocess
-    exe = os.path.join(ROOT, "tests", "cuda", "check_tsv_format")
+    exe = os.path.join(ROOT, "build", "checks", "check_tsv_format")
     r = subprocess.run([exe, "--host-only"], capture_output=True, text=True, timeout=600)
     assert r.returncode == 0, r.stdout + r.stderr
     assert ", 0 bad" in r.stdout

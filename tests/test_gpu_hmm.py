@@ -115,7 +115,7 @@ def test_invalid_jobs_are_rejected(engine, models):
 def test_exact_math_primitives_on_device():
     """div_by_cached_rcp == __fdiv_rn and the 8-instruction logsum == p7_FLogsum, bit for bit (2e8 pairs each)."""
     import subprocess
-    exe = os.path.join(os.path.dirname(os.path.abspath(__file__)), "cuda", "check_exact_math")
+    exe = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "build", "checks", "check_exact_math")
     r = subprocess.run([exe, "200"], capture_output=True, text=True, timeout=300)
     assert r.returncode == 0, r.stdout + r.stderr
     assert "0 mismatches" in r.stdout
