@@ -75,3 +75,17 @@ __device__ __forceinline__ float div_by_cached_rcp(float a, float b, float y)
     const float r1 = __fmaf_rn(-q1, b, a);
     return __fmaf_rn(r1, y, q1);
 }
+
+// ---- the Gaussian's last two operations in one FMUL + one FFMA ---------------------------------
+// The reference forms cc + (-0.5f*a)*a (emissions.h:54): three roundings.  Scaling by 2^-1 commutes with
+// round-to-nearest while the result stays normal, so RN(RN(-0.5a)*a) = -0.5*RN(a*a) whenever
+// 0.5*a*a >= 2^-126; the FMA's product RN(a*a)*(-0.5) is then exact and only the final add rounds, as in
+// the reference.  Below that (|a| < 2^-62.5, a != 0) both forms add less than half an ulp of cc and return cc,
+// unless |cc| < 2^-100.  For a nonzero a = RN((x - mu)/sigma) the first case needs |x - mu| < 2^-54 * sigma, which
+// two pA levels cannot give, and cc = log(1/sqrt(2pi)) - log(sigma) is 0 or at least 2^-25 in magnitude.  a == 0
+// gives cc + (-0) in both forms; |a| stays far below the 2^63 where a*a would overflow (|x - mu| < 2^12, sigma > 2^-8).
+// tests/cuda/check_emission_fold.cu compares it with the literal form on the device.
+__device__ __forceinline__ float add_neg_half_square(float cc, float a)
+{
+    return __fmaf_rn(__fmul_rn(a, a), -0.5f, cc);
+}

@@ -25,6 +25,7 @@
 #include "nph_internal.cuh"
 #include "exact_math.cuh"
 #include <math_constants.h>
+#include <climits>
 
 namespace nph_fwd {
 
@@ -81,12 +82,14 @@ __global__ void __launch_bounds__(CtaShape<C, W>::warps * 32, 1) hmm_forward_ker
     const int warp_global = blockIdx.x * kWarpsPerCta + (threadIdx.x >> 5);
     float4* const my_params = p.scratch_params + (size_t)warp_global * p.kpad_stride + (W < 32 ? grp * STRIP : 0);
     float* const edge_m = p.scratch_edge + (size_t)warp_global * 3 * p.edge_stride;
-    float* const edge_b = edge_m + p.edge_stride;
-    float* const edge_k = edge_b + p.edge_stride;
+    float* const edge_t = edge_m + p.edge_stride;   // lp3 + B of the edge column
+    float* const edge_k = edge_t + p.edge_stride;
 
     const float NEG = -CUDART_INF_F;
-    const float lp_mk = p.c.lp_mk, lp_mb = p.c.lp_mb, lp_bb = p.c.lp_bb, lp_bk = p.c.lp_bk;
-    const float lp_bm_next = p.c.lp_bm_next, lp_bm_self = p.c.lp_bm_self, lp_kk = p.c.lp_kk, lp_km = p.c.lp_km;
+    // lp_bk, lp_bm_next and lp_bm_self are all log(p_third) (nph_api.cu checks that they are bitwise equal), so
+    // lp3 + B is one float that serves K-skip at (r, c+1), M-self at (r+1, c) and M-next at (r+1, c+1)
+    const float lp_mk = p.c.lp_mk, lp_mb = p.c.lp_mb, lp_bb = p.c.lp_bb, lp3 = p.c.lp_bk;
+    const float lp_kk = p.c.lp_kk, lp_km = p.c.lp_km;
 
     for (;;) {
         uint32_t base = 0;
@@ -153,36 +156,52 @@ __global__ void __launch_bounds__(CtaShape<C, W>::warps * 32, 1) hmm_forward_ker
         // lanes beyond end_lane own no column of the last strip; the warp runs until its slowest group is done
         const int my_steps = has_job ? last_strip * P + E + end_lane : 0;
         const int total_steps = (W == 32) ? my_steps : __reduce_max_sync(kFull, my_steps);
+        // the soft-clip fold touches column 0 only at row 1 (step 0) unless a job of this warp allows pre-clipping;
+        // elsewhere its operand is -inf, and x (+) -inf == x, so the warp skips it
+        const bool any_pre_clip = __any_sync(kFull, pre_clip);
 
         float mu[C], sd[C], cc[C], ry[C];
-        float Mp[C], Bp[C], Kp[C];
+        float Mp[C], Bp[C], Kp[C], Tp[C];   // Tp[c] = lp3 + Bp[c]
 #pragma unroll
-        for (int c = 0; c < C; ++c) { mu[c] = 0.f; sd[c] = 1.f; cc[c] = 0.f; ry[c] = 1.f; Mp[c] = NEG; Bp[c] = NEG; Kp[c] = NEG; }
-        float Lm_prev = NEG, Lb_prev = NEG, Lk_prev = NEG;
+        for (int c = 0; c < C; ++c) { mu[c] = 0.f; sd[c] = 1.f; cc[c] = 0.f; ry[c] = 1.f; Mp[c] = NEG; Bp[c] = NEG; Kp[c] = NEG; Tp[c] = NEG; }
+        if (!CHAIN && gl * C < K) {
+            // one strip: each lane's columns are fixed for the whole job
+#pragma unroll
+            for (int c = 0; c < C; ++c) {
+                const float4 g4 = my_params[gl * C + c];
+                mu[c] = g4.x; sd[c] = g4.y; cc[c] = g4.z; ry[c] = g4.w;
+            }
+        }
+        float Lm_prev = NEG, Lt_prev = NEG, Lk_prev = NEG;
         float lp_end = NEG;
         int r = 1 - gl;        // row of this lane at the current step (rows 1..P; <1 = not started)
-        int s = 0;             // strip of this lane
+        int s = 0;             // strip of this lane (always 0 without CHAIN: rows past E are simply not live)
         float x_next = 0.f;
         if (r == 1 && E >= 1) x_next = lv[e_first];
-        float em_next = NEG, eb_next = NEG, ek_next = NEG;   // group lane 0: prefetched right edge of the previous strip
+        float em_next = NEG, et_next = NEG, ek_next = NEG;   // group lane 0: prefetched right edge of the previous strip
+        // one strip: address of the level of row r + 1, stepped by one IMAD.WIDE (unsigned, so rows < 1 wrap harmlessly)
+        const long long x_step = (long long)stride * (long long)sizeof(float);
+        unsigned long long x_addr = (unsigned long long)(lv + e_first) + (unsigned long long)((long long)r * x_step);
+        // the end fold runs on the lane holding the last k-mer, from row 1 with post-clipping and at row E without
+        const int end_row = (gl == end_lane) ? (post_clip ? 1 : E) : INT_MAX;
 
         for (int g = 0; g < total_steps; ++g) {
             // left neighbour's newest row (its row == my row, computed one step ago)
             float Lm = __shfl_up_sync(kFull, Mp[C - 1], 1, W);
-            float Lb = __shfl_up_sync(kFull, Bp[C - 1], 1, W);
+            float Lt = __shfl_up_sync(kFull, Tp[C - 1], 1, W);
             float Lk = __shfl_up_sync(kFull, Kp[C - 1], 1, W);
-            if (gl == 0) { Lm = CHAIN ? em_next : NEG; Lb = CHAIN ? eb_next : NEG; Lk = CHAIN ? ek_next : NEG; }
+            if (gl == 0) { Lm = CHAIN ? em_next : NEG; Lt = CHAIN ? et_next : NEG; Lk = CHAIN ? ek_next : NEG; }
 
-            const bool in_strip = (r >= 1) && (s < n_strips);
-            const int col0 = s * STRIP + gl * C;
+            const bool in_strip = (r >= 1) && (!CHAIN || s < n_strips);
+            const int col0 = (CHAIN ? s * STRIP : 0) + gl * C;
             const bool live = in_strip && (r <= E) && (col0 < K);
             const float x = x_next;
 
-            if (in_strip && r == 1) {
+            if (CHAIN && in_strip && r == 1) {
                 // entering a strip: row 0 and the start column are -inf
 #pragma unroll
-                for (int c = 0; c < C; ++c) { Mp[c] = NEG; Bp[c] = NEG; Kp[c] = NEG; }
-                Lm_prev = NEG; Lb_prev = NEG; Lk_prev = NEG;
+                for (int c = 0; c < C; ++c) { Mp[c] = NEG; Bp[c] = NEG; Kp[c] = NEG; Tp[c] = NEG; }
+                Lm_prev = NEG; Lt_prev = NEG; Lk_prev = NEG;
                 if (col0 < K) {
 #pragma unroll
                     for (int c = 0; c < C; ++c) {
@@ -195,66 +214,69 @@ __global__ void __launch_bounds__(CtaShape<C, W>::warps * 32, 1) hmm_forward_ker
             // prefetch for the next step: event level and (group lane 0, chained strips) the stored right edge
             {
                 int rn = r + 1, sn = s;
-                if (rn > P) { rn = 1; sn = s + 1; }
-                if (rn >= 1 && rn <= E && sn < n_strips) {
-                    x_next = lv[e_first + (long long)(rn - 1) * stride];
-                    if (CHAIN && gl == 0 && sn > 0) { em_next = edge_m[rn]; eb_next = edge_b[rn]; ek_next = edge_k[rn]; }
+                if (CHAIN && rn > P) { rn = 1; sn = s + 1; }
+                if (rn >= 1 && rn <= E && (!CHAIN || sn < n_strips)) {
+                    x_next = CHAIN ? lv[e_first + (long long)(rn - 1) * stride] : __ldca(reinterpret_cast<const float*>(x_addr));
+                    if (CHAIN && gl == 0 && sn > 0) { em_next = edge_m[rn]; et_next = edge_t[rn]; ek_next = edge_k[rn]; }
                 }
             }
 
             if (live) {
-                float soft = NEG;
-                if (col0 == 0 && (r == 1 || pre_clip)) soft = p.flank[r - 1];
-                float post = 0.f;
-                const bool do_end = (s == last_strip) && (gl == end_lane) && (post_clip || r == E);
-                if (do_end) post = p.flank[E - r];
-                float Me, Be, Ke;                                                  // states of the last k-mer's column (do_end)
+                const bool do_end = (!CHAIN || s == last_strip) && r >= end_row;
 
-                float lm_prev = Lm_prev, lb_prev = Lb_prev, lk_prev = Lk_prev;   // left column, row r-1
-                float lm_cur = Lm, lb_cur = Lb, lk_cur = Lk;                      // left column, row r
-#pragma unroll
-                for (int c = 0; c < C; ++c) {
+                float lm_prev = Lm_prev, lt_prev = Lt_prev, lk_prev = Lk_prev;   // left column, row r-1
+                float lm_cur = Lm, lt_cur = Lt, lk_cur = Lk;                      // left column, row r
+                auto cell = [&](const int c, const bool with_soft) {
                     // Gaussian log-density, reference operation order (emissions.h:51-55)
                     const float a = div_by_cached_rcp(__fsub_rn(x, mu[c]), sd[c], ry[c]);
-                    const float em = __fadd_rn(cc[c], __fmul_rn(__fmul_rn(-0.5f, a), a));
+                    const float em = add_neg_half_square(cc[c], a);
                     // match: left fold over {same M, prev M, same B, prev B, prev K, soft}
                     float m = __fadd_rn(lp_mm_self, Mp[c]);
                     m = lsum(m, __fadd_rn(lp_mm_next, lm_prev), tb);
-                    m = lsum(m, __fadd_rn(lp_bm_self, Bp[c]), tb);
-                    m = lsum(m, __fadd_rn(lp_bm_next, lb_prev), tb);
+                    m = lsum(m, Tp[c], tb);
+                    m = lsum(m, lt_prev, tb);
                     m = lsum(m, __fadd_rn(lp_km, lk_prev), tb);
-                    if (c == 0) m = lsum(m, soft, tb);
+                    if (with_soft) m = lsum(m, (col0 == 0 && (r == 1 || pre_clip)) ? p.flank[r - 1] : NEG, tb);
                     m = __fadd_rn(m, em);
                     // bad event: {same M, same B}
                     const float b = lsum(__fadd_rn(lp_mb, Mp[c]), __fadd_rn(lp_bb, Bp[c]), tb);
                     // k-mer skip: {prev M, prev B, prev K} of the SAME row
-                    float kk = lsum(__fadd_rn(lp_mk, lm_cur), __fadd_rn(lp_bk, lb_cur), tb);
+                    float kk = lsum(__fadd_rn(lp_mk, lm_cur), lt_cur, tb);
                     kk = lsum(kk, __fadd_rn(lp_kk, lk_cur), tb);
+                    const float t = __fadd_rn(lp3, b);
 
-                    lm_prev = Mp[c]; lb_prev = Bp[c]; lk_prev = Kp[c];
-                    lm_cur = m; lb_cur = b; lk_cur = kk;
-                    Mp[c] = m; Bp[c] = b; Kp[c] = kk;
-                }
-                Me = Mp[0]; Be = Bp[0]; Ke = Kp[0];
+                    lm_prev = Mp[c]; lt_prev = Tp[c]; lk_prev = Kp[c];
+                    lm_cur = m; lt_cur = t; lk_cur = kk;
+                    Mp[c] = m; Bp[c] = b; Kp[c] = kk; Tp[c] = t;
+                };
+                // two copies of column 0, so that the usual step branches past the soft fold instead of predicating it
+                if (any_pre_clip || g == 0) cell(0, true);
+                else cell(0, false);
 #pragma unroll
-                for (int c = 1; c < C; ++c) if (c == end_slot) { Me = Mp[c]; Be = Bp[c]; Ke = Kp[c]; }
-                Lm_prev = Lm; Lb_prev = Lb; Lk_prev = Lk;
+                for (int c = 1; c < C; ++c) cell(c, false);
+                Lm_prev = Lm; Lt_prev = Lt; Lk_prev = Lk;
 
                 if (do_end) {
+                    // states of the last k-mer's column; with flags 0 this runs once per job
+                    float Me = Mp[0], Be = Bp[0], Ke = Kp[0];
+#pragma unroll
+                    for (int c = 1; c < C; ++c) if (c == end_slot) { Me = Mp[c]; Be = Bp[c]; Ke = Kp[c]; }
+                    const float post = p.flank[E - r];
                     lp_end = lsum(lp_end, __fadd_rn(Me, post), tb);
                     lp_end = lsum(lp_end, __fadd_rn(Be, post), tb);
                     lp_end = lsum(lp_end, __fadd_rn(Ke, post), tb);
                 }
                 if (CHAIN && gl == W - 1 && s < last_strip) {
                     edge_m[r] = Mp[C - 1];
-                    edge_b[r] = Bp[C - 1];
+                    edge_t[r] = Tp[C - 1];
                     edge_k[r] = Kp[C - 1];
                 }
             }
 
             // advance
             r += 1;
-            if (r > P) { r = 1; s += 1; }
+            if (!CHAIN) x_addr += x_step;
+            if (CHAIN && r > P) { r = 1; s += 1; }
             if (CHAIN && n_strips > 1) __syncwarp();   // orders lane 31's edge stores before lane 0's later loads
         }
 

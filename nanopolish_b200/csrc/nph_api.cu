@@ -149,6 +149,9 @@ int create_common(nph_ctx** out, int device, bool own_stream, cudaStream_t strea
     if (cudaMalloc((void**)&ctx->d_logsum, sizeof(float) * NPH_TBL_SMEM) != cudaSuccess) return fail(NPH_ERR_NOMEM);
     if (cudaMemcpy(ctx->d_logsum, tbl.data(), sizeof(float) * NPH_TBL_SMEM, cudaMemcpyHostToDevice) != cudaSuccess) return fail(NPH_ERR_CUDA);
     const_transitions(ctx->consts);
+    // the forward kernel computes lp + B once for all three bad-state transitions (hmm_forward_kernel.cuh)
+    if (std::memcmp(&ctx->consts.lp_bk, &ctx->consts.lp_bm_next, sizeof(float)) != 0 ||
+        std::memcmp(&ctx->consts.lp_bk, &ctx->consts.lp_bm_self, sizeof(float)) != 0) return fail(NPH_ERR_STATE);
     if (nph_reserve(ctx, ctx->d_counters, NPH_NUM_COUNTERS) != NPH_OK) return fail(NPH_ERR_NOMEM);
     if (ensure_flank(ctx, 4096) != NPH_OK) return fail(NPH_ERR_CUDA);
     *out = ctx;
