@@ -529,25 +529,6 @@ std::vector<uint32_t> HmmBatch::ranks() const
     return out;
 }
 
-void HmmBatch::append(HmmBatch&& other)
-{
-    const uint64_t rank_base = m_codes.size();
-    std::vector<uint32_t> remap(other.m_reads.size());
-    for (size_t i = 0; i < other.m_reads.size(); ++i) {
-        auto it = m_read_index.find(other.m_reads[i]);
-        if (it == m_read_index.end()) {
-            it = m_read_index.insert({other.m_reads[i], (uint32_t)m_reads.size()}).first;
-            m_reads.push_back(other.m_reads[i]);
-        }
-        remap[i] = it->second;
-    }
-    m_jobs.reserve(m_jobs.size() + other.m_jobs.size());
-    for (nph_hmm_job j : other.m_jobs) { j.read = remap[j.read]; j.rank_off += rank_base; m_jobs.push_back(j); }
-    m_codes.insert(m_codes.end(), other.m_codes.begin(), other.m_codes.end());
-    m_job_models.insert(m_job_models.end(), other.m_job_models.begin(), other.m_job_models.end());
-    other.clear();
-}
-
 void HmmBatch::clear()
 {
     m_read_index.clear(); m_reads.clear(); m_job_models.clear(); m_jobs.clear(); m_codes.clear();

@@ -394,9 +394,6 @@ public:
     size_t size() const { return m_jobs.size(); }
     void clear();
     std::vector<float> run(Engine& engine, double indel_bias = hmm_indel_bias_factor);
-    // Move the jobs of `other` behind this batch's (job j of other becomes job size() + j); other is left empty.
-    // Lets worker threads enumerate into private batches and the owner splice them in a fixed order.
-    void append(HmmBatch&& other);
     const std::vector<nph_hmm_job>& jobs() const { return m_jobs; }
     // the k-mer ranks of the queued jobs, ranks()[job.rank_off + i] = get_kmer_rank(i, k, rc) — derived from the codes on request
     // (the batch itself ships one byte per base; for inspection and tests)

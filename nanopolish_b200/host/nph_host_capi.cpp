@@ -353,7 +353,6 @@ long long nphh_call_methylation_timed(int n_reads, const int32_t* read, const ch
 }
 
 // call-methylation from flat host buffers (the C-ABI layout) to TSV bytes: what bench.py's end-to-end arm times.
-// host_mode != 0 runs the host-side enumerator instead (reads registered with nphh_read_create; the cross-check path).
 long long nphh_call_methylation_flat(const void* reads, size_t n_reads, const float* ev_mean, const double* ev_start_time, size_t n_events,
                                      const char* ref_bases, size_t n_ref, const void* aligned_events, size_t n_pairs,
                                      const int16_t* event_deltas, const int32_t* first_event, void* records, size_t n_records,
@@ -419,47 +418,6 @@ long long nphh_modbam_tags(const char* seq, int ref_pos, int flag, const uint32_
         n = (long long)t.ml.size();
     });
     return rc ? rc : n;
-}
-
-// enumeration only (no device): seconds spent in MethylationCaller::add_read over all reads, and the job count
-// parallel != 0: MethylationCaller::add_reads (host_threads() workers); jobs_out / ranks_out (optional) receive the job list
-double nphh_methylation_enumerate_seconds(int n_reads, const int32_t* read, const char** read_names, const uint8_t* is_rev, const uint8_t* rc,
-                                          const int32_t* ref_start, const char** ref_seqs, const int32_t* pairs, const uint64_t* pair_off,
-                                          const char* contig, uint64_t* n_jobs_out, int parallel, void* jobs_out, size_t cap_jobs,
-                                          uint32_t* ranks_out, size_t cap_ranks, uint64_t* n_ranks_out)
-{
-    double secs = -1.0;
-    guard([&] {
-        MethylationCallingParameters params;
-        MethylationCaller caller(params, MethylationCaller::Mode::HostEnumeration);
-        std::vector<EventAlignedRead> rs(n_reads);
-        for (int i = 0; i < n_reads; ++i) {
-            EventAlignedRead& r = rs[i];
-            r.read = g_reads[read[i]].get();
-            r.read_name = read_names[i];
-            r.is_reverse = is_rev[i];
-            r.contig = contig;
-            r.ref_start_pos = ref_start[i];
-            r.ref_seq = ref_seqs[i];
-            r.aligned_events[0].reserve(pair_off[i + 1] - pair_off[i]);
-            for (uint64_t p = pair_off[i]; p < pair_off[i + 1]; ++p) r.aligned_events[0].push_back(AlignedPair{pairs[2 * p], pairs[2 * p + 1]});
-            r.rc[0] = rc[i];
-        }
-        const auto t0 = std::chrono::steady_clock::now();
-        if (parallel) caller.add_reads(rs);
-        else for (int i = 0; i < n_reads; ++i) caller.add_read(rs[i]);
-        secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-        *n_jobs_out = caller.num_jobs();
-        if (jobs_out && ranks_out) {
-            const HmmBatch& b = caller.batch();
-            const std::vector<uint32_t> rk = b.ranks();
-            if (b.jobs().size() > cap_jobs || rk.size() > cap_ranks) throw Error(NPH_ERR_INVALID, "dump buffers too small");
-            std::memcpy(jobs_out, b.jobs().data(), sizeof(nph_hmm_job) * b.jobs().size());
-            std::memcpy(ranks_out, rk.data(), sizeof(uint32_t) * rk.size());
-            *n_ranks_out = rk.size();
-        }
-    });
-    return secs;
 }
 
 // ---- N4: load_from_raw over a batch -----------------------------------------------------------

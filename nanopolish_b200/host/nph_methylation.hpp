@@ -1,5 +1,5 @@
 // nph_methylation.hpp — SURVEY.md section 8(f) row N3: call-methylation's per-read logic split into
-// enumerate / one batched launch / scatter, plus the TSV writer.
+// staging / one batched launch / scatter, plus the TSV writer.
 //
 //   calculate_methylation_for_read      ref: src/basemods/nanopolish_basemods.cpp:238-457
 //   ScoredSite, MethylationCallingParameters   ref: src/basemods/nanopolish_basemods.h:45-77
@@ -15,8 +15,6 @@
 // the grouping, the window / event-bound tests, the methylated / unmethylated k-mer ranks and the two scores per group
 // all happen on the device (csrc/methylation.cu); what comes back is one 24-byte record per scored group, from which
 // the ScoredSites and the TSV rows (write_methylation_results_as_tsv) are formed.
-// A host-side enumerator with the same results (Mode::HostEnumeration: jobs queued into an HmmBatch read by read, the
-// round-1 path) is kept as the cross-check of the device enumerator.
 #pragma once
 #include <cstdio>
 #include "nph_host.hpp"
@@ -74,8 +72,6 @@ ModbamTags modbam_tags(const std::string& bam_seq, const std::vector<AlignedPair
 ModbamTags reference_modbam_tags(const std::string& ref_seq, int ref_start_pos, const std::map<int, ScoredSite>& calls,
                                  const MethylationCallingParameters& params);
 
-bool find_by_ref_bounds(const std::vector<AlignedPair>& pairs, int ref_start, int ref_stop, int& read_start, int& read_stop);
-
 // nph_meth_params (include/nph.h) for these calling parameters, model k-mer size and output window
 nph_meth_params make_meth_params(const MethylationCallingParameters& params, uint32_t k, int region_start, int region_end);
 
@@ -120,25 +116,21 @@ size_t call_methylation_flat(Engine& engine, const FlatMethylationBatch& batch, 
 
 class MethylationCaller {
 public:
-    enum class Mode { DeviceEnumeration, HostEnumeration };
-    explicit MethylationCaller(const MethylationCallingParameters& params, Mode mode = Mode::DeviceEnumeration);
-    // enumerate the read's motif groups and queue their jobs; returns the read's index in this batch.
+    explicit MethylationCaller(const MethylationCallingParameters& params);
+    // stage the read's reference substring and event alignments for run(); returns the read's index in this batch.
     // region_start/region_end = -1 for no window restriction (the reference's -w option).
     size_t add_read(const EventAlignedRead& r, int region_start = -1, int region_end = -1);
-    // The same for a whole BamProcessor batch, enumerated by host_threads() workers into private job lists that are
-    // spliced in read order (so job order, scores and output equal add_read called read by read).  Returns the index of
-    // the first read.  The reference runs this enumeration inside its per-read OpenMP loop too.
+    // The same for a whole BamProcessor batch, staged by host_threads() workers.  Returns the index of the first read.
     size_t add_reads(const std::vector<EventAlignedRead>& reads, int region_start = -1, int region_end = -1);
-    void run(Engine& engine, double indel_bias = hmm_indel_bias_factor);       // one launch for every queued group
-    const std::map<int, ScoredSite>& sites(size_t read_idx) const;            // (device mode: built from the site records on first use)
+    void run(Engine& engine, double indel_bias = hmm_indel_bias_factor);       // one device call for every staged read
+    const std::map<int, ScoredSite>& sites(size_t read_idx) const;            // (built from the site records on first use)
     size_t num_reads() const { return m_reads.size(); }
-    // forward jobs of the batch: queued so far (host mode) / scored by the last run() (device mode: two per group)
-    size_t num_jobs() const { return m_mode == Mode::HostEnumeration ? m_batch.size() : (size_t)(2 * m_n_sites); }
-    uint64_t scored_events() const { return m_scored_events; }                // device mode, after run()
-    // every read's rows back to back in one buffer (device mode: formatted straight from the site records by
-    // host_threads() workers); returns the byte count, or the required size when cap is too small
+    // forward jobs scored by the last run(): two per group
+    size_t num_jobs() const { return (size_t)(2 * m_n_sites); }
+    uint64_t scored_events() const { return m_scored_events; }                // after run()
+    // every read's rows back to back in one buffer (formatted straight from the site records by host_threads() workers);
+    // returns the byte count, or the required size when cap is too small
     size_t tsv_all(char* out, size_t cap) const;
-    const HmmBatch& batch() const { return m_batch; }      // the queued jobs (read-only; for inspection and tests)
     void write_tsv(FILE* fp, size_t read_idx) const;
     std::string tsv(size_t read_idx) const;
     std::vector<std::string> tsv_batch() const;            // every read's rows, formatted by host_threads() workers
@@ -151,26 +143,20 @@ public:
     void clear();
 
 private:
-    struct Pending { size_t read; int site_key; size_t strand; size_t job_u, job_m; };
     struct ReadEntry {
         std::string name; bool is_reverse = false;
         mutable std::map<int, ScoredSite> sites; mutable bool sites_built = false;
-        // device mode
         std::string contig; size_t ref_off = 0, ref_len = 0; int ref_start_pos = 0; uint32_t k = 0;
         size_t first_record = 0, n_records = 0;
     };
     struct Record { const SquiggleRead* read; const PoreModel* model; uint8_t strand; };
-    size_t add_read_host(const EventAlignedRead& r, int region_start, int region_end);
     void stage(const EventAlignedRead* const* reads, size_t n, int region_start, int region_end);
     void build_sites(size_t read_idx) const;
     void append_rows(std::string& out, size_t read_idx) const;
     void put_rows(void* row_buffer, size_t read_idx) const;          // the same into the writer's growing character buffer
-    Mode m_mode;
     MethylationCallingParameters m_params;
-    HmmBatch m_batch;
-    std::vector<Pending> m_pending;
     std::vector<ReadEntry> m_reads;
-    // device mode: the flat batch (page-locked) and its results
+    // the flat batch (page-locked) and its results
     PinnedArray<char> m_ref;
     PinnedArray<nph_aligned_pair> m_pairs;
     PinnedArray<int16_t> m_deltas;            // compact event alignments, parallel to m_ref (built next to m_pairs; used unless a step overflowed)

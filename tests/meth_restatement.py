@@ -1,5 +1,5 @@
 """Plain-Python restatement of call-methylation's per-read enumeration — test infrastructure (the checker of
-csrc/methylation.cu and of the host enumerator), never imported by the product.
+csrc/methylation.cu and the expectation of the host caller's TSV), never imported by the product.
 
 Follows calculate_methylation_for_read, src/basemods/nanopolish_basemods.cpp:301-417, with the pieces it calls:
   Alphabet::match_to_site / is_motif_match / methylate / reverse_complement   src/common/nanopolish_alphabet.h:108-330

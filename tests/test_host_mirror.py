@@ -105,6 +105,20 @@ def test_kmer_ranks_match_compiled_reference(host, ref_oracle):
             assert np.array_equal(out[:k], ref_oracle.kmer_ranks(hc, m.encode(), bool(rc)))
 
 
+def test_rolling_ranks_equal_get_kmer_rank(host):
+    """HmmBatch::add fills the ranks by one rolling pass; they must be HMMInputSequence::get_kmer_rank's, both strands,
+    plain and methylation alphabets (the rc strand of a methylated sequence is not a per-base complement)."""
+    rng = np.random.default_rng(12)
+    for alphabet, sym in (("nucleotide", "ACGT"), ("cpg", "ACGT")):
+        for rep in range(20):
+            seq = "".join(sym[c] for c in rng.integers(0, 4, int(rng.integers(6, 260))))
+            if alphabet == "cpg" and rep % 2:
+                seq = seq.replace("CG", "MG")
+            for rc in (0, 1):
+                assert host.nphh_kmer_ranks_rolling_check(alphabet.encode(), seq.encode(), 6, rc) == 0, (alphabet, seq, rc)
+    assert host.nphh_kmer_ranks_rolling_check(b"nucleotide", b"ACG", 6, 0) == 0
+
+
 # ---- GPU: the reference's free functions through the mirror -----------------------------------
 def _register(host, model):
     mean = np.ascontiguousarray(model.level_mean); sd = np.ascontiguousarray(model.level_stdv)
