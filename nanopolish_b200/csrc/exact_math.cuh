@@ -7,13 +7,49 @@
 #ifndef NPH_LOGSUM_CUT
 #define NPH_LOGSUM_CUT 15700
 #endif
+// lsum_sat's index reaches 2^14: its table has 16385 entries, and entries NPH_LOGSUM_CUT .. 2^14 hold 0.0f
+#define NPH_LOGSUM_TBL_LEN 16385
 
 // ---- quantised log-sum ---------------------------------------------------------------------
 // Reference (src/common/logsum.h:55-66):
 //     max = a > b ? a : b;  min = a < b ? a : b;
 //     (min == -inf || max - min >= 15.7f) ? max : max + tbl[(int)((max - min) * 1000.f)]
-//
-// Here, in 8 SASS instructions (2 ALU-pipe, 5 FMA-pipe, 1 LDS):
+// Two forms, which return the same float for every pair of operands (both read entry floor(RN(|d| * 1000)) wherever the
+// reference reads the table, and a 0.0f entry or -inf + log 2 = -inf everywhere else):
+//   * lsum, 8 instructions: the index clamped to the zero entry NPH_LOGSUM_CUT; a table of NPH_LOGSUM_CUT + 1 entries or more.
+//   * lsum_sat, 7 instructions: the clamp folded into the multiply; a table of NPH_LOGSUM_TBL_LEN entries.  The forward kernel
+//     uses this one.  tests/cuda/check_lsum_saturated.cu compares it with the reference and with lsum on the device.
+struct LogsumTable {
+    uint32_t biased_base;   // shared-window byte address of entry 0, minus 4 * (bit pattern of the floor's offset) (mod 2^32)
+    uint32_t scale;         // 4, as a RUNTIME value: bits * scale + base then stays one IMAD on the FMA pipe; with a literal 4 ptxas
+                            // picks LEA, which issues on the half-rate ALU pipe that FMNMX already loads
+};
+
+// `bias` must be NPH_LOGSUM_ADDR_BIAS (lsum) or NPH_LOGSUM_SAT_ADDR_BIAS (lsum_sat) and must reach the kernel as a RUNTIME
+// value (a kernel parameter): when ptxas can see the constant it re-associates (bits*4 + base) - const into two instructions.
+#define NPH_LOGSUM_ADDR_BIAS (0u - 4u * 0x4B000000u)
+#define NPH_LOGSUM_SAT_ADDR_BIAS (0u - 4u * 0x44000000u)
+__device__ __forceinline__ LogsumTable make_logsum_table(const float* smem_tbl, uint32_t bias, uint32_t scale = 4u)
+{
+    LogsumTable t;
+    t.biased_base = (uint32_t)__cvta_generic_to_shared(smem_tbl) + bias;
+    t.scale = scale;
+    return t;
+}
+
+__device__ __forceinline__ float lsum_lookup(float mx, float u, const LogsumTable tb)
+{
+#ifdef NPH_LSUM_LEA
+    const uint32_t adr = (uint32_t)__float_as_int(u) * 4u + tb.biased_base;          // A/B: literal 4 -> LEA on the ALU pipe
+#else
+    const uint32_t adr = (uint32_t)__float_as_int(u) * tb.scale + tb.biased_base;
+#endif
+    float v;
+    asm("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(adr));
+    return __fadd_rn(mx, v);
+}
+
+// lsum, in 8 SASS instructions (2 ALU-pipe, 5 FMA-pipe, 1 LDS):
 //     mx  = fmaxf(a, b)                                   FMNMX
 //     d   = a - b                 (|d| == max - min exactly: RN is sign-symmetric)   FADD
 //     t   = fminf(|d| * 1000, 15700)                      FMUL (|.| is a free source modifier), FMNMX
@@ -24,37 +60,40 @@
 // max - min >= 15.7f (15.7f * 1000.f rounds to exactly 15700.0f, and every smaller float maps to an
 // index <= 15699), for min == -inf (difference +inf), and for both -inf (difference NaN: fminf
 // returns the non-NaN operand, and -inf + 0 = -inf).
-struct LogsumTable {
-    uint32_t biased_base;   // shared-window byte address of entry 0, minus 4 * 0x4B000000 (mod 2^32)
-    uint32_t scale;         // 4, as a RUNTIME value: bits * scale + base then stays one IMAD on the FMA pipe; with a literal 4 ptxas
-                            // picks LEA, which issues on the half-rate ALU pipe that FMNMX already loads
-};
-
-// `bias` must be NPH_LOGSUM_ADDR_BIAS and must reach the kernel as a RUNTIME value (a kernel parameter):
-// when ptxas can see the constant it re-associates (bits*4 + base) - const into two instructions.
-#define NPH_LOGSUM_ADDR_BIAS (0u - 4u * 0x4B000000u)
-__device__ __forceinline__ LogsumTable make_logsum_table(const float* smem_tbl, uint32_t bias, uint32_t scale = 4u)
-{
-    LogsumTable t;
-    t.biased_base = (uint32_t)__cvta_generic_to_shared(smem_tbl) + bias;
-    t.scale = scale;
-    return t;
-}
-
 __device__ __forceinline__ float lsum(float a, float b, const LogsumTable tb)
 {
     const float mx = fmaxf(a, b);
     const float d = __fsub_rn(a, b);
     const float t = fminf(__fmul_rn(fabsf(d), 1000.0f), (float)NPH_LOGSUM_CUT);
-    const float u = __fadd_rd(t, 8388608.0f);
-#ifdef NPH_LSUM_LEA
-    const uint32_t adr = (uint32_t)__float_as_int(u) * 4u + tb.biased_base;          // A/B: literal 4 -> LEA on the ALU pipe
-#else
-    const uint32_t adr = (uint32_t)__float_as_int(u) * tb.scale + tb.biased_base;
-#endif
-    float v;
-    asm("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(adr));
-    return __fadd_rn(mx, v);
+    return lsum_lookup(mx, __fadd_rd(t, 8388608.0f), tb);
+}
+
+// lsum_sat, in 7 SASS instructions (1 ALU-pipe, 5 FMA-pipe, 1 LDS):
+//     mx  = fmaxf(a, b)                                   FMNMX
+//     d   = a - b                                         FADD
+//     t   = sat(|d| * (1000 * 2^-14))                     FMUL.SAT (|.| is a free source modifier)
+//     u   = t +(round-down) 2^9   -> bits = 0x44000000 + floor(t * 2^14)              FADD.RM
+//     adr = bits * 4 + (table_base - 4 * 0x44000000)      IMAD   (mod 2^32)
+//     r   = mx + shared[adr]                              LDS, FADD
+// Why the index is the reference's, entries >= 15700 being 0.0f:
+//   * 1000 * 2^-14 = 0.06103515625 is exact, and scaling by a power of two commutes with round-to-nearest
+//     while the result is normal: RN(|d| * 1000 * 2^-14) = RN(|d| * 1000) * 2^-14.  Saturation clamps to [0, 1],
+//     so t * 2^14 = min(RN(|d| * 1000), 16384).  If the scaled product is subnormal (|d| * 1000 < 2^-112) both
+//     forms give index 0.
+//   * t lies in [0, 1] and the spacing of floats in [512, 1024) is 2^-14, so t + 512 rounded down is
+//     512 + floor(t * 2^14) * 2^-14, whose bit pattern is 0x44000000 + floor(t * 2^14) (at most 0x44004000 = 513.0f).
+//   * max - min >= 15.7f: 15.7f * 1000.f rounds to exactly 15700.0f and every smaller float maps to an index
+//     <= 15699, so exactly these differences read an entry in 15700 .. 16384, which holds 0.0f: "return max".
+//   * min == -inf, max finite: |d| = +inf, saturates to 1, entry 16384 (0.0f).  Both -inf: d is NaN, which
+//     saturation turns into 0, entry 0 (log 2); -inf + log 2 = -inf.
+// Without lsum's clamp onto one zero word, a difference in [15.7, 16.384) reads its own zero word: slightly more bank
+// conflicts for one instruction less (DESIGN §3.4).
+__device__ __forceinline__ float lsum_sat(float a, float b, const LogsumTable tb)
+{
+    const float mx = fmaxf(a, b);
+    const float d = __fsub_rn(a, b);
+    const float t = __saturatef(__fmul_rn(fabsf(d), 0.06103515625f));
+    return lsum_lookup(mx, __fadd_rd(t, 512.0f), tb);
 }
 
 // ---- correctly rounded float division with a precomputed reciprocal --------------------------

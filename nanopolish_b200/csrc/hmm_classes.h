@@ -3,7 +3,7 @@
 // A class is (C columns per lane, W lanes per job); 32/W jobs share a warp.  W < 32 classes hold
 // single-strip jobs (K <= W*C); W == 32 also chains strips for wide jobs.  A job goes to the class that
 // minimises modelled issue slots = steps x (per-step overhead + C x per-cell cost) x W/32: 46 per warp step and
-// 74 instructions per block-cell (the steady-state step of hmm_forward_kernel<9|10, 32, false> in cuobjdump -sass,
+// 67 instructions per block-cell (the steady-state step of hmm_forward_kernel<9|10, 32, false> in cuobjdump -sass,
 // scripts/k1_bounds.py).
 #pragma once
 #include <stdint.h>
@@ -35,10 +35,10 @@ NPH_HD uint32_t nph_class_steps(uint32_t K, uint32_t E, int C, uint32_t W)
     return (n_strips - 1) * P + E + (last_cols - 1) / (uint32_t)C;
 }
 
-// per-step cost: 46 issue slots of per-step work plus the row update, 74 per column
+// per-step cost: 46 issue slots of per-step work plus the row update, 67 per column
 NPH_HD float nph_class_cost(uint32_t steps, int C, uint32_t W)
 {
-    return (float)steps * (46.0f + 74.0f * C) * (W * (1.0f / 32.0f));
+    return (float)steps * (46.0f + 67.0f * C) * (W * (1.0f / 32.0f));
 }
 
 // returns class index; *steps_out = steps in that class

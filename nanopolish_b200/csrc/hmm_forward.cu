@@ -73,7 +73,7 @@ int nph_launch_hmm_forward(nph_ctx* ctx, float* scores_dev)
     p.kpad_stride = ctx->max_kpad;
     p.edge_stride = ctx->max_period + 8;
     p.c = ctx->consts;
-    p.lsum_bias = NPH_LOGSUM_ADDR_BIAS;
+    p.lsum_bias = NPH_LOGSUM_SAT_ADDR_BIAS;
     p.lsum_scale = 4u;
     p.progress = (ctx->levels_inflight && ctx->level_chunk_events) ? ctx->d_progress : nullptr;
     p.chunk_events = (uint32_t)ctx->level_chunk_events;

@@ -17,7 +17,7 @@
 //   * W == 32 only: jobs wider than 32*C columns are cut into strips chained back-to-back (lane 0 starts
 //     strip s+1 while lane 31 is still finishing strip s); only the strip's right-edge column (3 floats
 //     per row) goes through an L1-resident scratch line.  W < 32 classes hold single-strip jobs (K <= W*C).
-//   * the 62.8 KB quantised log-sum table lives in shared memory (exact_math.cuh: 8 instructions per sum).
+//   * the 65.5 KB quantised log-sum table lives in shared memory (exact_math.cuh: 7 instructions per sum).
 //   * every float operation is issued in the reference's order with explicit round-to-nearest
 //     intrinsics (no FMA contraction), IEEE division included, so scores are bit-identical.
 //   * persistent CTAs (one per SM); warps pull 32/W jobs at a time, longest first, from an atomic counter.
@@ -28,6 +28,8 @@
 #include <climits>
 
 namespace nph_fwd {
+
+static_assert(NPH_TBL_SMEM == NPH_LOGSUM_TBL_LEN, "the shared table must cover every index lsum_sat can form");
 
 // Warps per persistent CTA (one CTA per SM).  The full-warp classes hold 16 warps at up to 128 registers; the sub-warp classes of short
 // windows need fewer registers (80 at C = 4) and are latency bound on their per-step loads, so they run 24 (C <= 4) or 20 (C <= 6)
@@ -54,7 +56,7 @@ struct FwdParams {
     float* scratch_edge;          // per warp: 3 * edge_stride floats (W == 32 classes)
     uint32_t kpad_stride;
     uint32_t edge_stride;
-    uint32_t lsum_bias;           // NPH_LOGSUM_ADDR_BIAS, passed at run time on purpose (exact_math.cuh)
+    uint32_t lsum_bias;           // NPH_LOGSUM_SAT_ADDR_BIAS, passed at run time on purpose (exact_math.cuh)
     uint32_t lsum_scale;          // 4, at run time for the same reason (keeps the table address an IMAD)
     const uint32_t* progress;     // one-shot call: number of level chunks landed so far (nullptr: all resident)
     uint32_t chunk_events;        // events per level chunk (multiple of 32)
@@ -232,17 +234,17 @@ __global__ void __launch_bounds__(CtaShape<C, W>::warps * 32, 1) hmm_forward_ker
                     const float em = add_neg_half_square(cc[c], a);
                     // match: left fold over {same M, prev M, same B, prev B, prev K, soft}
                     float m = __fadd_rn(lp_mm_self, Mp[c]);
-                    m = lsum(m, __fadd_rn(lp_mm_next, lm_prev), tb);
-                    m = lsum(m, Tp[c], tb);
-                    m = lsum(m, lt_prev, tb);
-                    m = lsum(m, __fadd_rn(lp_km, lk_prev), tb);
-                    if (with_soft) m = lsum(m, (col0 == 0 && (r == 1 || pre_clip)) ? p.flank[r - 1] : NEG, tb);
+                    m = lsum_sat(m, __fadd_rn(lp_mm_next, lm_prev), tb);
+                    m = lsum_sat(m, Tp[c], tb);
+                    m = lsum_sat(m, lt_prev, tb);
+                    m = lsum_sat(m, __fadd_rn(lp_km, lk_prev), tb);
+                    if (with_soft) m = lsum_sat(m, (col0 == 0 && (r == 1 || pre_clip)) ? p.flank[r - 1] : NEG, tb);
                     m = __fadd_rn(m, em);
                     // bad event: {same M, same B}
-                    const float b = lsum(__fadd_rn(lp_mb, Mp[c]), __fadd_rn(lp_bb, Bp[c]), tb);
+                    const float b = lsum_sat(__fadd_rn(lp_mb, Mp[c]), __fadd_rn(lp_bb, Bp[c]), tb);
                     // k-mer skip: {prev M, prev B, prev K} of the SAME row
-                    float kk = lsum(__fadd_rn(lp_mk, lm_cur), lt_cur, tb);
-                    kk = lsum(kk, __fadd_rn(lp_kk, lk_cur), tb);
+                    float kk = lsum_sat(__fadd_rn(lp_mk, lm_cur), lt_cur, tb);
+                    kk = lsum_sat(kk, __fadd_rn(lp_kk, lk_cur), tb);
                     const float t = __fadd_rn(lp3, b);
 
                     lm_prev = Mp[c]; lt_prev = Tp[c]; lk_prev = Kp[c];
@@ -262,9 +264,9 @@ __global__ void __launch_bounds__(CtaShape<C, W>::warps * 32, 1) hmm_forward_ker
 #pragma unroll
                     for (int c = 1; c < C; ++c) if (c == end_slot) { Me = Mp[c]; Be = Bp[c]; Ke = Kp[c]; }
                     const float post = p.flank[E - r];
-                    lp_end = lsum(lp_end, __fadd_rn(Me, post), tb);
-                    lp_end = lsum(lp_end, __fadd_rn(Be, post), tb);
-                    lp_end = lsum(lp_end, __fadd_rn(Ke, post), tb);
+                    lp_end = lsum_sat(lp_end, __fadd_rn(Me, post), tb);
+                    lp_end = lsum_sat(lp_end, __fadd_rn(Be, post), tb);
+                    lp_end = lsum_sat(lp_end, __fadd_rn(Ke, post), tb);
                 }
                 if (CHAIN && gl == W - 1 && s < last_strip) {
                     edge_m[r] = Mp[C - 1];

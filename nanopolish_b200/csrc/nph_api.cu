@@ -143,9 +143,9 @@ int create_common(nph_ctx** out, int device, bool own_stream, cudaStream_t strea
     }
 
     // quantised log-sum table, built exactly like p7_FLogsumInit (ref: src/common/logsum.cpp:57-69)
-    std::vector<float> tbl(NPH_TBL_SMEM);
+    // entries NPH_LOGSUM_CUT .. NPH_TBL_SMEM - 1 are 0.0f: every difference >= 15.7f returns max
+    std::vector<float> tbl(NPH_TBL_SMEM, 0.0f);
     for (int i = 0; i < NPH_LOGSUM_CUT; ++i) tbl[i] = (float)log(1. + exp((double)-i / 1000.f));
-    tbl[NPH_LOGSUM_CUT] = 0.0f;
     if (cudaMalloc((void**)&ctx->d_logsum, sizeof(float) * NPH_TBL_SMEM) != cudaSuccess) return fail(NPH_ERR_NOMEM);
     if (cudaMemcpy(ctx->d_logsum, tbl.data(), sizeof(float) * NPH_TBL_SMEM, cudaMemcpyHostToDevice) != cudaSuccess) return fail(NPH_ERR_CUDA);
     const_transitions(ctx->consts);

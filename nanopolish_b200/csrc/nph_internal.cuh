@@ -9,8 +9,8 @@
 #include "../../include/nph.h"
 
 #define NPH_LOGSUM_TBL 16000        // ref: p7_LOGSUM_TBL, src/common/logsum.h:20
-#define NPH_LOGSUM_CUT 15700        // (max-min) >= 15.7f returns max: entries >= 15700 are never read
-#define NPH_TBL_SMEM   (NPH_LOGSUM_CUT + 1)   // +1: a zero entry that the clamped index lands on
+#define NPH_LOGSUM_CUT 15700        // (max-min) >= 15.7f returns max: entries >= 15700 hold 0.0f
+#define NPH_TBL_SMEM   16385        // = NPH_LOGSUM_TBL_LEN: the saturated index of lsum_sat (exact_math.cuh) reaches 2^14
 #define NPH_NUM_COUNTERS 64          // work-queue counters: one per forward class (<= 40) + ABEA (last)
 
 // Per-read record on the device (what the kernels need of nph_read after the prologue).

@@ -12,9 +12,13 @@ the step loop's body that performs at least 7*C table look-ups (every lane live,
 soft-clip fold).  Its opcode histogram for C = 9 and C = 10 gives the per-column and per-step costs.
 
 Shared-memory side: the kernel's lockstep schedule replayed on a sample of bench.py's own scorereads jobs.
-At step g lane j owns row g - j + 1 and columns j*C .. j*C + C - 1; every look-up index
-min(floor(|a - b| * 1000), 15700) comes from a float32 restatement of the recurrence in the kernel's
-(= oracle/np_oracle.c's) operation order.
+At step g lane j owns row g - j + 1 and columns j*C .. j*C + C - 1; every look-up index comes from a float32
+restatement of the recurrence in the kernel's (= oracle/np_oracle.c's) operation order.  Three index forms are
+replayed on the same look-ups, per site (m1..m4 the match fold, b the bad state, k1 k2 the skip fold):
+  * cut:       min(floor(|a - b| * 1000), 15700), NaN -> 15700 (exact_math.cuh's lsum, 8 instructions)
+  * saturated: min(floor(|a - b| * 1000), 16384), NaN -> 0      (exact_math.cuh's lsum_sat, 7 instructions)
+  * ideal:     the saturated form with every look-up that leaves the sum unchanged (mx + tbl[i] == mx) sent to one
+               word; a bound on what a sink word for no-op look-ups could give, not a form the kernel has.
 
 Usage: python scripts/k1_bounds.py [--jobs N] [--object path/to/hmm_forward_w32.o]
 """
@@ -33,15 +37,17 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 CSRC = os.path.join(ROOT, "nanopolish_b200", "csrc")
 LOGSUM_CUT = 15700
+SAT_INDEX = 16384          # the saturated index's largest value; the table holds 16385 entries
+SITES = ("m1", "m2", "m3", "m4", "b", "k1", "k2")
 
-# Steady-state warp step of the parent revision's kernels (cuobjdump -sass, CUDA 12.9, sm_90a), before the
-# shared bad-state sums, the folded emission multiply, the end-state select moved under do_end and the
-# single-strip loop trimmed.  Recorded here because the script compiles only the current source.
+# Steady-state warp step of the parent revision's kernels (cuobjdump -sass, CUDA 12.9, sm_90a), with the
+# 8-instruction log-sum (FMUL, FMNMX clamp to 15700) instead of the saturated 7-instruction one.  Recorded here
+# because the script compiles only the current source.
 BEFORE = {
-    9: {"total": 776, "ops": {"FADD": 245, "FADD.RM": 64, "FMNMX": 128, "FMUL": 91, "FFMA": 36, "IMAD/LEA": 68, "LDS": 64,
-                              "SHFL": 3, "SEL/MOV": 25, "SETP/LOP": 17, "IADD": 8, "LDG": 2, "BRA/BSSY": 12, "other": 13}},
-    10: {"total": 853, "ops": {"FADD": 272, "FADD.RM": 71, "FMNMX": 142, "FMUL": 101, "FFMA": 40, "IMAD/LEA": 75, "LDS": 71,
-                               "SHFL": 3, "SEL/MOV": 26, "SETP/LOP": 17, "IADD": 8, "LDG": 2, "BRA/BSSY": 12, "other": 13}},
+    9: {"total": 712, "ops": {"FADD": 216, "FADD.RM": 63, "FMNMX": 126, "FMUL": 81, "FFMA": 45, "IMAD/LEA": 65, "LDS": 63,
+                              "SHFL": 3, "SEL/MOV": 19, "SETP/LOP": 9, "IADD": 3, "LDG": 1, "BRA/BSSY": 7, "other": 11}},
+    10: {"total": 786, "ops": {"FADD": 240, "FADD.RM": 70, "FMNMX": 140, "FMUL": 90, "FFMA": 50, "IMAD/LEA": 72, "LDS": 70,
+                               "SHFL": 3, "SEL/MOV": 20, "SETP/LOP": 9, "IADD": 3, "LDG": 1, "BRA/BSSY": 7, "other": 11}},
 }
 
 
@@ -173,17 +179,24 @@ def issue_side(obj: str) -> dict[int, dict]:
 # ---------------------------------------------------------------------------------------------------------
 # shared-memory side
 def _lsum(a, b, tbl):
-    """kernel's lsum in float32; returns (result, table index)"""
+    """kernel's lsum in float32; returns (result, index per form).  Both forms give the same sum: entries 15700..16384
+    of the table are 0.0f, and the NaN difference (both operands -inf) adds log 2 or 0 to -inf."""
     with np.errstate(invalid="ignore", over="ignore"):
         mx = np.maximum(a, b)
         d = np.abs(a - b) * np.float32(1000.0)
-        d = np.where(np.isnan(d), np.float32(LOGSUM_CUT), np.minimum(d, np.float32(LOGSUM_CUT)))
-        idx = np.floor(d).astype(np.int32)
-        return (mx + tbl[idx]).astype(np.float32), idx
+        nan = np.isnan(d)
+        cut = np.floor(np.where(nan, np.float32(LOGSUM_CUT), np.minimum(d, np.float32(LOGSUM_CUT)))).astype(np.int32)
+        sat = np.floor(np.where(nan, np.float32(0.0), np.minimum(d, np.float32(SAT_INDEX)))).astype(np.int32)
+        r = (mx + tbl[sat]).astype(np.float32)
+        ideal = np.where(r == mx, LOGSUM_CUT, sat)   # one sink word for no-op look-ups (mx = -inf included)
+        return r, {"cut": cut, "saturated": sat, "ideal": ideal}
+
+
+FORMS = ("cut", "saturated", "ideal")
 
 
 def job_indices(rs, jobs, j, model, tbl, consts):
-    """look-up indices of every cell of job j: array [site, row, column] (sites: m1..m4, b, k1, k2; -1 unused)"""
+    """look-up indices of every cell of job j, per form: array [site, row, column] (sites: m1..m4, b, k1, k2; -1 unused)"""
     job = jobs.jobs[j]
     rd = rs.reads[job["read"]]
     ranks = jobs.kmer_ranks[job["rank_off"]:job["rank_off"] + job["n_kmers"]].astype(np.int64)
@@ -199,28 +212,34 @@ def job_indices(rs, jobs, j, model, tbl, consts):
     lp_mm_self, lp_mm_next = consts["trans"][job["read"]]
     f32 = np.float32
     NEG = f32(-np.inf)
-    idx = np.full((7, E, K), -1, np.int32)
+    idx = {f: np.full((7, E, K), -1, np.int32) for f in FORMS}
+
+    def put(site, r, ix, c=slice(None)):
+        for f in FORMS:
+            idx[f][site, r, c] = ix[f]
+
     Mp = np.full(K, NEG, f32); Bp = Mp.copy(); Kp = Mp.copy()
     for r in range(E):
         a = ((f32(x[r]) - mu) / sd).astype(f32)
         em = (cc + (f32(-0.5) * a) * a).astype(f32)
         Ml = np.concatenate(([NEG], Mp[:-1])); Bl = np.concatenate(([NEG], Bp[:-1])); Kl = np.concatenate(([NEG], Kp[:-1]))
         m = (f32(lp_mm_self) + Mp).astype(f32)
-        m, idx[0, r] = _lsum(m, f32(lp_mm_next) + Ml, tbl)
-        m, idx[1, r] = _lsum(m, consts["lp3"] + Bp, tbl)
-        m, idx[2, r] = _lsum(m, consts["lp3"] + Bl, tbl)
-        m, idx[3, r] = _lsum(m, consts["lp_km"] + Kl, tbl)
+        m, ix = _lsum(m, f32(lp_mm_next) + Ml, tbl); put(0, r, ix)
+        m, ix = _lsum(m, consts["lp3"] + Bp, tbl); put(1, r, ix)
+        m, ix = _lsum(m, consts["lp3"] + Bl, tbl); put(2, r, ix)
+        m, ix = _lsum(m, consts["lp_km"] + Kl, tbl); put(3, r, ix)
         if r == 0:
             m[:1] = _lsum(m[:1], consts["flank"][:1], tbl)[0]       # soft-clip fold, column 0 of row 1
         m = (m + em).astype(f32)
-        b, idx[4, r] = _lsum(consts["lp_mb"] + Mp, consts["lp_bb"] + Bp, tbl)
-        kk1, idx[5, r] = _lsum(consts["lp_mk"] + np.concatenate(([NEG], m[:-1])), consts["lp3"] + np.concatenate(([NEG], b[:-1])), tbl)
+        b, ix = _lsum(consts["lp_mb"] + Mp, consts["lp_bb"] + Bp, tbl); put(4, r, ix)
+        kk1, ix = _lsum(consts["lp_mk"] + np.concatenate(([NEG], m[:-1])), consts["lp3"] + np.concatenate(([NEG], b[:-1])), tbl)
+        put(5, r, ix)
         kk = np.empty(K, f32)
         prev = NEG
         lp_kk = consts["lp_kk"]
         for c in range(K):
-            v, i = _lsum(kk1[c:c + 1], np.array([lp_kk + prev], f32), tbl)
-            kk[c] = v[0]; idx[6, r, c] = i[0]
+            v, ix = _lsum(kk1[c:c + 1], np.array([lp_kk + prev], f32), tbl)
+            kk[c] = v[0]; put(6, r, {f: ix[f][0] for f in FORMS}, c)
             prev = kk[c]
         Mp, Bp, Kp = m, b, kk
     return idx
@@ -241,12 +260,12 @@ def levels_of(rs, read):
 
 
 def wavefronts(idx, C: int):
-    """replay lane j = row g - j + 1, columns j*C..: wavefronts per (step, slot, site), and the steps"""
+    """replay lane j = row g - j + 1, columns j*C..: wavefronts per site (summed over steps and slots), and the steps"""
     S, E, K = idx.shape
     lanes = np.arange(32)
     end_lane = (K - 1) // C
     steps = E + end_lane
-    total = 0
+    total = np.zeros(S, np.int64)
     g = np.arange(steps)[:, None]
     row = g - lanes[None, :]                                   # 0-based row of lane j at step g
     valid_row = (row >= 0) & (row < E)
@@ -264,7 +283,7 @@ def wavefronts(idx, C: int):
             bank = np.where(first, v & 31, 32)
             counts = np.zeros((steps, 33), np.int32)
             np.add.at(counts, (np.repeat(np.arange(steps), 32), bank.ravel()), 1)
-            total += counts[:, :32].max(axis=1).sum()
+            total[s] += counts[:, :32].max(axis=1).sum()
     return total, steps
 
 
@@ -273,7 +292,8 @@ def smem_side(n_jobs: int):
     nuc = synth.load_model("nucleotide")
     rs = synth.gen_reads(max(1, n_jobs // 6 + 1), 4000, nuc, seed=42)      # bench.py: gen_reads(reads, 4000, seed=42 + ...)
     jobs = synth.scorereads_jobs(rs, 500, model_id=0)
-    tbl = np.array([np.float32(np.log(1. + np.exp(-i / np.float32(1000.)))) for i in range(LOGSUM_CUT)] + [0.0], np.float32)
+    tbl = np.array([np.float32(np.log(1. + np.exp(-i / np.float32(1000.)))) for i in range(LOGSUM_CUT)]
+                   + [0.0] * (SAT_INDEX + 1 - LOGSUM_CUT), np.float32)
     f = np.float32
     p_third = f((f(1.0) - f(0.001)) / f(3))
     consts = {"lp_mk": f(np.log(f(0.0025))), "lp_mb": f(np.log(f(0.001))), "lp_bb": f(np.log(f(0.001))),
@@ -288,16 +308,18 @@ def smem_side(n_jobs: int):
     consts["trans"] = trans
     out = {}
     for C in (9, 10):
-        out[C] = {"wavefronts": 0, "steps": 0, "jobs": 0, "lookups": 0}
+        out[C] = {"wavefronts": {f: np.zeros(len(SITES), np.int64) for f in FORMS}, "steps": 0, "jobs": 0, "lookups": 0}
     for j in range(min(n_jobs, len(jobs.jobs))):
         K = int(jobs.jobs[j]["n_kmers"])
         C = 9 if K <= 288 else 10
         if K > 320:
             continue
         idx = job_indices(rs, jobs, j, nuc, tbl, consts)
-        w, st = wavefronts(idx, C)
         o = out[C]
-        o["wavefronts"] += int(w); o["steps"] += st; o["jobs"] += 1; o["lookups"] += 7 * C * st
+        for f in FORMS:
+            w, st = wavefronts(idx[f], C)
+            o["wavefronts"][f] += w
+        o["steps"] += st; o["jobs"] += 1; o["lookups"] += 7 * C * st
     return out
 
 
@@ -325,16 +347,26 @@ def main():
 
     sm = smem_side(args.jobs)
     print(f"\nShared-memory side: look-up wavefronts, lockstep replay of bench scorereads jobs (seed 42)")
-    print(f"{'class':>14s} {'jobs':>5s} {'steps/job':>9s} {'LDS/step':>8s} {'wavefronts/LDS':>14s} "
-          f"{'smem clk/step':>13s} {'issue clk/step before':>21s} {'after':>6s}")
     for C in (9, 10):
         o = sm[C]
         if not o["jobs"]:
             continue
-        wf_step = o["wavefronts"] / o["steps"]
-        lds = 7 * C
-        print(f"{'<%d,32,false>' % C:>14s} {o['jobs']:5d} {o['steps'] / o['jobs']:9.1f} {lds:8d} {o['wavefronts'] / o['lookups']:14.2f} "
-              f"{wf_step:13.1f} {BEFORE[C]['total'] / 4:21.1f} {after[C]['total'] / 4:6.1f}")
+        site_lookups = o["lookups"] / len(SITES)
+        print(f"  <{C},32,false>: {o['jobs']} jobs, {o['steps'] / o['jobs']:.1f} steps/job, {7 * C} LDS/step; wavefronts per LDS by site:")
+        print("    " + f"{'form':10s}" + "".join(f"{s:>6s}" for s in SITES) + f"{'all':>6s}{'smem clk/step':>15s}")
+        for f in FORMS:
+            w = o["wavefronts"][f]
+            print("    " + f"{f:10s}" + "".join(f"{x / site_lookups:6.2f}" for x in w)
+                  + f"{w.sum() / o['lookups']:6.2f}{w.sum() / o['steps']:15.1f}")
+    print("\nBound per warp step, per SM clock (max of issue and shared memory):")
+    for C in (9, 10):
+        o = sm[C]
+        if not o["jobs"]:
+            continue
+        before = (BEFORE[C]["total"] / 4, o["wavefronts"]["cut"].sum() / o["steps"])
+        now = (after[C]["total"] / 4, o["wavefronts"]["saturated"].sum() / o["steps"])
+        print(f"  <{C},32,false>: before issue {before[0]:.1f}, smem {before[1]:.1f} -> {max(before):.1f};"
+              f"  after issue {now[0]:.1f}, smem {now[1]:.1f} -> {max(now):.1f}  ({100 * (1 - max(now) / max(before)):.1f}% fewer clocks)")
     print("(per SM: 4 sub-partitions issue one warp instruction each per clock; shared memory serves one wavefront per clock;\n"
           " the look-ups at the fill/drain edges, where fewer lanes are live, are counted at what they cost)")
 
