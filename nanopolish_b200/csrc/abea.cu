@@ -27,8 +27,6 @@
 #include <cmath>
 #include <vector>
 
-#define NPH_TRY(expr) do { int rc__ = (expr); if (rc__ != NPH_OK) return rc__; } while (0)
-
 namespace {
 
 #ifndef NPH_ABEA_WARPS
@@ -108,13 +106,7 @@ __global__ void __launch_bounds__(kThreads, 1) abea_kernel(const AbeaParams p)
         // ---- prologue: read-scaled Gaussian of every k-mer (FP64 like the reference, then narrowed)
         {
             const uint32_t* rk = p.ranks + job.rank_off;
-            for (int i = lane; i < K; i += 32) {
-                const uint32_t r = rk[i];
-                const float mu = (float)__dadd_rn(__dmul_rn(rd.scale, mv.mean[r]), rd.shift);
-                const float sd = (float)__dmul_rn(mv.stdv[r], rd.var);
-                const float lsd = (float)__dadd_rn(mv.log_stdv[r], rd.log_var);
-                prm[i] = make_float4(mu, sd, __fsub_rn(p.log_inv_sqrt_2pi, lsd), __frcp_rn(sd));
-            }
+            for (int i = lane; i < K; i += 32) prm[i] = nph_scaled_gaussian(mv, rd, rk[i], p.log_inv_sqrt_2pi);
         }
         __syncwarp();
 
@@ -429,6 +421,14 @@ int validate_abea_jobs(nph_ctx* ctx, const nph_abea_job* jobs, size_t n_jobs, si
     return NPH_OK;
 }
 
+// per warp: kmax Gaussians, then trace_stride bytes of band trace
+void scratch_layout(const nph_ctx* ctx, NphArena& a, float4** params, uint8_t** trace)
+{
+    const size_t warps = (size_t)ctx->sm_count * kWarps;
+    *params = a.take<float4>((size_t)ctx->abea_kmax * warps);
+    *trace = a.take<uint8_t>(ctx->abea_trace_stride * warps);
+}
+
 } // namespace
 
 int nph_launch_abea(nph_ctx* ctx)
@@ -445,11 +445,10 @@ int nph_launch_abea(nph_ctx* ctx)
     p.counter = ctx->d_counters.p + (NPH_NUM_COUNTERS - 1);
     p.pairs = ctx->d_pairs.p;
     p.results = ctx->d_abea_res.p;
-    const int warps = ctx->sm_count * kWarps;
     p.kmax_stride = ctx->abea_kmax;
     p.trace_stride = ctx->abea_trace_stride;
-    p.scratch_params = reinterpret_cast<float4*>(ctx->d_abea_scratch.p);
-    p.scratch_trace = ctx->d_abea_scratch.p + sizeof(float4) * (size_t)p.kmax_stride * warps;
+    NphArena scratch{ctx->d_abea_scratch.p};
+    scratch_layout(ctx, scratch, &p.scratch_params, &p.scratch_trace);
     p.consts = reinterpret_cast<const AbeaJobConsts*>(ctx->d_abea_consts.p);
     p.lp_skip = log(1e-10);
     p.lp_trim = log(0.01);
@@ -463,15 +462,13 @@ int nph_launch_abea(nph_ctx* ctx)
     abea_kernel<<<grid, kThreads, 0, ctx->stream>>>(p);
     NPH_CUDA(ctx, cudaGetLastError());
     NPH_CUDA(ctx, cudaEventRecord(ctx->ev1, ctx->stream));
-    ctx->last_launches = 1;
-    ctx->timing_valid = true;
+    nph_timing_events(ctx, 1);
     return NPH_OK;
 }
 
 // estimate_scalings_using_mom over the loaded ABEA jobs (reads, ranks and jobs already on the device)
 int nph_launch_mom(nph_ctx* ctx, double* d_shift_scale_out, bool reversed)
 {
-    if (!ctx->ev_mean_resident) return NPH_ERR_STATE;      // the pipelined one-shot score leaves only d_level behind
     MomParams p{};
     p.reversed = reversed ? 1 : 0;
     p.ev_mean = ctx->d_ev_mean.p; p.reads = ctx->d_reads.p; p.models = ctx->d_models.p; p.model_id = ctx->abea_model;
@@ -494,7 +491,7 @@ int nph_abea_jobs_load(nph_ctx* ctx, const uint32_t* kmer_ranks, size_t n_ranks_
 
     // per-job transition penalties, evaluated with the host libm in FP64 exactly as raw_loader.cpp:95-108
     std::vector<AbeaJobConsts> consts(n_jobs);
-    std::vector<std::pair<uint64_t, uint32_t>> keyed(n_jobs);
+    std::vector<uint64_t> bands(n_jobs);
     uint32_t kmax = 1;
     uint64_t max_bands = 4;
     const double lp_skip = log(1e-10);
@@ -504,21 +501,15 @@ int nph_abea_jobs_load(nph_ctx* ctx, const uint32_t* kmer_ranks, size_t n_ranks_
         const double p_stay = 1 - (1 / (events_per_kmer + 1));
         consts[j].lp_stay = log(p_stay);
         consts[j].lp_step = log(1.0 - exp(lp_skip) - exp(consts[j].lp_stay));
-        const uint64_t bands = (uint64_t)ctx->h_read_n_events[jobs[j].read] + jobs[j].n_kmers + 2;
-        keyed[j] = {bands, (uint32_t)j};
+        bands[j] = (uint64_t)ctx->h_read_n_events[jobs[j].read] + jobs[j].n_kmers + 2;
         kmax = std::max(kmax, jobs[j].n_kmers);
-        max_bands = std::max(max_bands, bands);
+        max_bands = std::max(max_bands, bands[j]);
     }
-    std::sort(keyed.begin(), keyed.end(), [](const std::pair<uint64_t, uint32_t>& a, const std::pair<uint64_t, uint32_t>& b) {
-        return a.first != b.first ? a.first > b.first : a.second < b.second; });   // longest reads first
-    std::vector<uint32_t> order(n_jobs);
-    for (size_t j = 0; j < n_jobs; ++j) order[j] = keyed[j].second;
+    const std::vector<uint32_t> order = nph_longest_first(bands);     // longest reads first
 
-    const int warps = ctx->sm_count * kWarps;
     ctx->abea_kmax = kmax;
     ctx->abea_trace_stride = 32 * (max_bands + kTraceBlockRows);
-    const size_t scratch = (sizeof(float4) * (size_t)kmax + ctx->abea_trace_stride) * warps;
-    NPH_TRY(nph_reserve(ctx, ctx->d_abea_scratch, scratch));
+    NPH_TRY(nph_reserve(ctx, ctx->d_abea_scratch, nph_layout_bytes([&](NphArena& a) { float4* q; uint8_t* t; scratch_layout(ctx, a, &q, &t); })));
     NPH_TRY(nph_reserve(ctx, ctx->d_abea_jobs, n_jobs));
     NPH_TRY(nph_reserve(ctx, ctx->d_abea_ranks, n_ranks_total));
     NPH_TRY(nph_reserve(ctx, ctx->d_abea_order, n_jobs));

@@ -22,8 +22,6 @@
 #include <vector>
 #include <cstdlib>
 
-#define NPH_TRY(expr) do { int rc__ = (expr); if (rc__ != NPH_OK) return rc__; } while (0)
-
 namespace {
 
 constexpr int kThreads = 128;
@@ -648,15 +646,25 @@ __global__ void __launch_bounds__(256) ed_events_kernel(const FastParams p)
 
 } // namespace
 
-static inline size_t ed_al(size_t v) { return (v + 255) / 256 * 256; }
-
-// Scratch the detector needs next to the raw samples (which the caller keeps on the device).
-size_t nph_ed_scratch_bytes(size_t n_samples_total, size_t n_reads, size_t events_total)
+// The detector's scratch next to the raw samples (which the caller keeps on the device); nothing per sample: the
+// t-statistics never leave the SM.  overflow is 64 words: the flag, then the statistics counters.
+struct EdScratch { nph_raw_read* reads; uint32_t* order; nph_event* events; uint32_t* n_events; int* overflow; uint32_t* peaks; uint32_t* n_peaks; uint8_t* exact; };
+static void ed_layout(NphArena& a, size_t n_reads, size_t events_total, EdScratch& e)
 {
-    (void)n_samples_total;                 // nothing per sample any more: the t-statistics never leave the SM
-    const size_t b_n = ed_al(sizeof(uint32_t) * n_reads);
-    return ed_al(sizeof(nph_raw_read) * n_reads) + b_n /*order*/ + ed_al(sizeof(nph_event) * events_total) + 2 * b_n /*n_events, n_peaks*/ + 256 +
-           ed_al(sizeof(uint32_t) * events_total) /*peaks*/ + ed_al(n_reads) /*exact*/;
+    e.reads = a.take<nph_raw_read>(n_reads);
+    e.order = a.take<uint32_t>(n_reads);
+    e.events = a.take<nph_event>(events_total);
+    e.n_events = a.take<uint32_t>(n_reads);
+    e.overflow = a.take<int>(64);
+    e.peaks = a.take<uint32_t>(events_total);
+    e.n_peaks = a.take<uint32_t>(n_reads);
+    e.exact = a.take<uint8_t>(n_reads);
+}
+
+size_t nph_ed_scratch_bytes(size_t n_reads, size_t events_total)
+{
+    EdScratch e;
+    return nph_layout_bytes([&](NphArena& a) { ed_layout(a, n_reads, events_total, e); });
 }
 
 // Event detection over reads whose samples are already on the device.  Leaves the events (at each read's event_off)
@@ -667,32 +675,29 @@ int nph_detect_events_device(nph_ctx* ctx, const float* d_raw, size_t n_samples_
                              nph_event** d_events_out, uint32_t** d_n_events_out, std::vector<uint32_t>& h_n_events, int* launches_out)
 {
     if (params->window_length2 > kMaxW2 || params->window_length1 > params->window_length2 || params->window_length1 == 0) return NPH_ERR_UNSUPPORTED;
-    std::vector<std::pair<uint32_t, uint32_t>> keyed(n_reads);
+    std::vector<uint32_t> n_samples(n_reads);
     for (size_t i = 0; i < n_reads; ++i) {
         const nph_raw_read& r = reads[i];
         if (r.n_samples == 0 || r.sample_off + r.n_samples > n_samples_total || r.event_off + r.event_cap > events_total || r.event_cap == 0)
             return NPH_ERR_INVALID;
         if (r.n_samples > 0xFFFFFF00u) return NPH_ERR_UNSUPPORTED;      // position arithmetic is 32-bit with a 2*w2 halo
-        keyed[i] = {r.n_samples, (uint32_t)i};
+        n_samples[i] = r.n_samples;
     }
     // threads of a warp walk reads of similar length: longest first
-    std::sort(keyed.begin(), keyed.end(), [](const std::pair<uint32_t, uint32_t>& a, const std::pair<uint32_t, uint32_t>& b) {
-        return a.first != b.first ? a.first > b.first : a.second < b.second; });
-    std::vector<uint32_t> order(n_reads);
-    for (size_t i = 0; i < n_reads; ++i) order[i] = keyed[i].second;
+    const std::vector<uint32_t> order = nph_longest_first(n_samples);
 
-    const size_t b_reads = ed_al(sizeof(nph_raw_read) * n_reads), b_n = ed_al(sizeof(uint32_t) * n_reads);
-    const size_t b_ev = ed_al(sizeof(nph_event) * events_total), b_pk = ed_al(sizeof(uint32_t) * events_total);
-    uint8_t* base = scratch;
+    EdScratch e;
+    NphArena arena{scratch};
+    ed_layout(arena, n_reads, events_total, e);
+    nph_raw_read* d_reads = e.reads;
+    uint32_t* d_order = e.order;
+    uint32_t* d_peaks = e.peaks;
+    uint32_t* d_npeaks = e.n_peaks;
+    uint8_t* d_exact = e.exact;
     DetParams p{};
-    nph_raw_read* d_reads = reinterpret_cast<nph_raw_read*>(base); base += b_reads;
-    uint32_t* d_order = reinterpret_cast<uint32_t*>(base); base += b_n;
-    p.events = reinterpret_cast<nph_event*>(base); base += b_ev;
-    p.n_events = reinterpret_cast<uint32_t*>(base); base += b_n;
-    p.overflow = reinterpret_cast<int*>(base); base += 256;
-    uint32_t* d_peaks = reinterpret_cast<uint32_t*>(base); base += b_pk;
-    uint32_t* d_npeaks = reinterpret_cast<uint32_t*>(base); base += b_n;
-    uint8_t* d_exact = reinterpret_cast<uint8_t*>(base);
+    p.events = e.events;
+    p.n_events = e.n_events;
+    p.overflow = e.overflow;
     p.raw = d_raw; p.reads = d_reads; p.order = d_order; p.n_reads = (uint32_t)n_reads;
     p.w1 = params->window_length1; p.w2 = params->window_length2;
     p.t1 = params->threshold1; p.t2 = params->threshold2; p.peak_height = params->peak_height;
@@ -721,7 +726,7 @@ int nph_detect_events_device(nph_ctx* ctx, const float* d_raw, size_t n_samples_
         // with 1 / 2 / 4), more for small batches (512 reads: 1.46 / 1.02 / 0.86 ms) as long as a segment stays >= 2 warm-ups long
         int wpr = 1;
         const size_t want = (size_t)ctx->sm_count * 20;
-        while (wpr < 4 && n_reads * wpr < want && keyed[0].first / (64u * wpr) >= 2 * f.warm) wpr *= 2;
+        while (wpr < 4 && n_reads * wpr < want && n_samples[order[0]] / (64u * wpr) >= 2 * f.warm) wpr *= 2;
         if (getenv("NPH_EVENTS_WPR")) wpr = atoi(getenv("NPH_EVENTS_WPR"));
         if (wpr >= 4) launch_fused<4>(f, tc, n_reads, ctx->stream);
         else if (wpr == 2) launch_fused<2>(f, tc, n_reads, ctx->stream);
@@ -769,22 +774,24 @@ extern "C" int nph_detect_events_batch(nph_ctx* ctx, const float* raw, size_t n_
     if (n_reads == 0) return NPH_OK;
     if (!raw || !reads || !events_out || !n_events_out) return NPH_ERR_INVALID;
     NPH_CUDA(ctx, cudaSetDevice(ctx->device));
-    const size_t b_raw = ed_al(sizeof(float) * n_samples_total);
-    NPH_TRY(nph_reserve(ctx, ctx->d_abea_scratch, b_raw + nph_ed_scratch_bytes(n_samples_total, n_reads, events_total)));
+    float* d_raw;
+    uint8_t* scratch;
+    NPH_TRY(nph_carve(ctx, ctx->d_abea_scratch, [&](NphArena& a) {
+        d_raw = a.take<float>(n_samples_total);
+        scratch = a.take<uint8_t>(nph_ed_scratch_bytes(n_reads, events_total));
+    }));
     ctx->abea_loaded = false;     // the arena is shared with the ABEA trace
-    float* d_raw = reinterpret_cast<float*>(ctx->d_abea_scratch.p);
     NPH_CUDA(ctx, cudaMemcpyAsync(d_raw, raw, sizeof(float) * n_samples_total, cudaMemcpyHostToDevice, ctx->stream));
     NPH_CUDA(ctx, cudaEventRecord(ctx->ev0, ctx->stream));
     nph_event* d_events = nullptr;
     uint32_t* d_n = nullptr;
     std::vector<uint32_t> counts;
     int launches = 0;
-    const int rc = nph_detect_events_device(ctx, d_raw, n_samples_total, reads, n_reads, params, ctx->d_abea_scratch.p + b_raw, events_total,
+    const int rc = nph_detect_events_device(ctx, d_raw, n_samples_total, reads, n_reads, params, scratch, events_total,
                                             &d_events, &d_n, counts, &launches);
     if (rc != NPH_OK && rc != NPH_ERR_UNSUPPORTED) return rc;
     if (!d_events) return rc;                       // parameters refused before anything ran
-    ctx->last_launches = launches;
-    ctx->timing_valid = true;
+    nph_timing_events(ctx, launches);
     // only the events that exist cross PCIe: a read's room (n_samples / 2 in practice) is ~4.5 x what it fills, and the room of a
     // 4 096-read batch is 1.8 GB.  One copy per read when that saves more than the copies' launch cost, else the whole arena.
     size_t used = 0;

@@ -20,17 +20,18 @@
 #define NPH_STEP_BUCKETS 1024         // step key: exact below 768, then 32-step bins
 #define NPH_CHUNK_BUCKETS 8           // level chunk of the job's read (one-shot call), major key
 #define NPH_KEY_BUCKETS (NPH_STEP_BUCKETS * NPH_CHUNK_BUCKETS)
+#define NPH_MIN_PERIOD 40             // chained strips (forward and Viterbi): the right edge of row r must be written >32 steps before it is read
 
 NPH_HD uint32_t nph_class_width(int wi) { return wi >= 3 ? 32u : (4u << wi); }   // 4, 8, 16, 32, 32 (chained)
 NPH_HD bool nph_class_chained(int wi) { return wi == 4; }
 NPH_HD int nph_class_index(int C, int wi) { return wi * NPH_MAX_COLS + (C - 1); }
 
-// warp steps one job takes in class (C, W): chained strips of W*C columns, period max(E, 40) when chained
+// warp steps one job takes in class (C, W): chained strips of W*C columns, period max(E, NPH_MIN_PERIOD) when chained
 NPH_HD uint32_t nph_class_steps(uint32_t K, uint32_t E, int C, uint32_t W)
 {
     const uint32_t strip = W * (uint32_t)C;
     const uint32_t n_strips = (K + strip - 1) / strip;
-    const uint32_t P = n_strips > 1 ? (E > 40u ? E : 40u) : E;
+    const uint32_t P = n_strips > 1 ? (E > (uint32_t)NPH_MIN_PERIOD ? E : (uint32_t)NPH_MIN_PERIOD) : E;
     const uint32_t last_cols = K - (n_strips - 1) * strip;
     return (n_strips - 1) * P + E + (last_cols - 1) / (uint32_t)C;
 }

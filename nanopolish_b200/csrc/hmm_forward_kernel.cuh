@@ -23,6 +23,7 @@
 //   * persistent CTAs (one per SM); warps pull 32/W jobs at a time, longest first, from an atomic counter.
 #pragma once
 #include "nph_internal.cuh"
+#include "hmm_classes.h"
 #include "exact_math.cuh"
 #include <math_constants.h>
 #include <climits>
@@ -37,7 +38,6 @@ static_assert(NPH_TBL_SMEM == NPH_LOGSUM_TBL_LEN, "the shared table must cover e
 constexpr int kMaxWarpsPerCta = 24;
 template <int C, int W> struct CtaShape { static constexpr int warps = (W == 32) ? 16 : (C <= 4 ? 24 : (C <= 6 ? 20 : 16)); };
 constexpr unsigned kFull = 0xffffffffu;
-constexpr int kMinPeriod = 40;   // chained strips: the right edge of row r must be written >32 steps before it is read
 
 struct FwdParams {
     const float* level;           // drift-scaled event levels, all reads
@@ -127,7 +127,7 @@ __global__ void __launch_bounds__(CtaShape<C, W>::warps * 32, 1) hmm_forward_ker
         const bool post_clip = (job.flags & NPH_HAF_ALLOW_POST_CLIP) != 0;
         const int n_strips = CHAIN ? (K + STRIP - 1) / STRIP : 1;
         const int kpad = n_strips * STRIP;
-        const int P = n_strips > 1 ? max(E, kMinPeriod) : E;
+        const int P = n_strips > 1 ? max(E, NPH_MIN_PERIOD) : E;
 
         // ---- per-job prologue: read-scaled Gaussian of every k-mer, formed in FP64 exactly as
         // get_scaled_gaussian_from_pore_model_state does, then narrowed; plus RN(1/sigma') ----
@@ -135,13 +135,7 @@ __global__ void __launch_bounds__(CtaShape<C, W>::warps * 32, 1) hmm_forward_ker
             const uint32_t* rk = p.ranks + job.rank_off;
             for (int i = gl; i < kpad; i += W) {
                 float4 g = make_float4(0.f, 1.f, 0.f, 1.f);
-                if (i < K) {
-                    const uint32_t r = rk[i];
-                    const float mu = (float)__dadd_rn(__dmul_rn(rd.scale, mv.mean[r]), rd.shift);
-                    const float sd = (float)__dmul_rn(mv.stdv[r], rd.var);
-                    const float lsd = (float)__dadd_rn(mv.log_stdv[r], rd.log_var);
-                    g = make_float4(mu, sd, __fsub_rn(p.c.log_inv_sqrt_2pi, lsd), __frcp_rn(sd));
-                }
+                if (i < K) g = nph_scaled_gaussian(mv, rd, rk[i], p.c.log_inv_sqrt_2pi);
                 my_params[i] = g;
             }
         }

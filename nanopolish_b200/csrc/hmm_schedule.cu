@@ -97,7 +97,7 @@ __global__ void classify_kernel(const nph_hmm_job* __restrict__ jobs, uint32_t n
         if (ok) {
             const uint32_t strip = W * C;
             atomicMax(&s_kpad, ((K + strip - 1) / strip) * strip);
-            atomicMax(&s_period, E > 40u ? E : 40u);
+            atomicMax(&s_period, E > (uint32_t)NPH_MIN_PERIOD ? E : (uint32_t)NPH_MIN_PERIOD);
             atomicMax(&s_E, E);
         }
     }
@@ -184,14 +184,15 @@ __global__ void scatter_kernel(uint32_t n_jobs, const uint8_t* __restrict__ cls,
 
 // Runs on ctx->stream after the jobs are on the device.  Fills ctx->classes, max_kpad/max_period, returns
 // NPH_ERR_INVALID if any job failed validation.  One stream synchronisation (the summary read-back).
-int nph_schedule_hmm_jobs(nph_ctx* ctx, size_t n_jobs, size_t n_ranks_total, uint32_t* max_E_out)
+int nph_schedule_hmm_jobs(nph_ctx* ctx, size_t n_jobs, size_t n_ranks_total, NphJobSource src, uint32_t* max_E_out)
 {
+    const bool codes = src == NphJobSource::HostCodes;
     const size_t hist_n = (size_t)NPH_NUM_CLASSES * NPH_KEY_BUCKETS;
     int rc;
     if ((rc = nph_reserve(ctx, ctx->d_sched_cls, n_jobs)) != NPH_OK) return rc;
     if ((rc = nph_reserve(ctx, ctx->d_sched_bkt, n_jobs)) != NPH_OK) return rc;
     if ((rc = nph_reserve(ctx, ctx->d_sched_hist, 2 * hist_n + 1024)) != NPH_OK) return rc;
-    if (ctx->codes_mode && (rc = nph_reserve(ctx, ctx->d_rank_base, n_jobs)) != NPH_OK) return rc;
+    if (codes && (rc = nph_reserve(ctx, ctx->d_rank_base, n_jobs)) != NPH_OK) return rc;
     unsigned int* hist = ctx->d_sched_hist.p;
     unsigned int* offs = hist + hist_n;
     SchedSummary* d_sum = reinterpret_cast<SchedSummary*>(offs + hist_n);
@@ -201,10 +202,10 @@ int nph_schedule_hmm_jobs(nph_ctx* ctx, size_t n_jobs, size_t n_ranks_total, uin
     int blocks = (int)std::min<size_t>((n_jobs + threads - 1) / threads, (size_t)ctx->sm_count * 8);
     if (blocks < 1) blocks = 1;
     classify_kernel<<<blocks, threads, 0, ctx->stream>>>(ctx->d_jobs.p, (uint32_t)n_jobs, ctx->d_reads.p, (uint32_t)ctx->n_reads,
-                                                        ctx->d_models.p, ctx->d_ranks.p, ctx->codes_mode ? ctx->d_codes.p : nullptr, (uint32_t)ctx->models.size(), (uint64_t)n_ranks_total,
+                                                        ctx->d_models.p, ctx->d_ranks.p, codes ? ctx->d_codes.p : nullptr, (uint32_t)ctx->models.size(), (uint64_t)n_ranks_total,
                                                         (uint32_t)(ctx->levels_inflight ? ctx->level_chunk_events : 0), ctx->d_sched_cls.p,
-                                                        ctx->d_sched_bkt.p, hist, d_sum, ctx->codes_mode ? ctx->d_rank_base.p : nullptr,
-                                                        ctx->jobs_trusted ? 1 : 0);
+                                                        ctx->d_sched_bkt.p, hist, d_sum, codes ? ctx->d_rank_base.p : nullptr,
+                                                        src == NphJobSource::DeviceRanks ? 1 : 0);
     NPH_CUDA(ctx, cudaGetLastError());
     scan_kernel<<<NPH_NUM_CLASSES, 1024, 0, ctx->stream>>>(hist, offs, d_sum);
     NPH_CUDA(ctx, cudaGetLastError());
@@ -217,7 +218,7 @@ int nph_schedule_hmm_jobs(nph_ctx* ctx, size_t n_jobs, size_t n_ranks_total, uin
         ctx->last_error = "job " + std::to_string(h.error - 1) + " fails validation (read/model index, event range, stride, rank range or a k-mer rank outside the model)";
         return NPH_ERR_INVALID;
     }
-    if (ctx->codes_mode) {
+    if (codes) {
         // the ranks the kernels read: formed here, once, from the codes (the jobs' device copies now index d_ranks)
         if ((rc = nph_reserve(ctx, ctx->d_ranks, (size_t)h.rank_cursor)) != NPH_OK) return rc;
         const int wblocks = (int)std::min<size_t>((n_jobs + 7) / 8, (size_t)ctx->sm_count * 8);
@@ -232,7 +233,7 @@ int nph_schedule_hmm_jobs(nph_ctx* ctx, size_t n_jobs, size_t n_ranks_total, uin
         first += (size_t)h.class_count[c];
     }
     ctx->max_kpad = std::max<uint32_t>(h.max_kpad, 32 * NPH_MAX_COLS);
-    ctx->max_period = std::max<uint32_t>(h.max_period, 40);
+    ctx->max_period = std::max<uint32_t>(h.max_period, NPH_MIN_PERIOD);
     *max_E_out = std::max<uint32_t>(h.max_E, 1);
     return NPH_OK;
 }

@@ -24,8 +24,6 @@
 #include <string>
 #include <vector>
 
-#define NPH_TRY(expr) do { int rc__ = (expr); if (rc__ != NPH_OK) return rc__; } while (0)
-
 namespace {
 
 constexpr int kWarps = 16;
@@ -123,13 +121,6 @@ int launch_vit(nph_ctx* ctx, const VitParams& base, const uint32_t* order, size_
 const int kVitCols[] = {1, 2, 3, 4, 6, 8};
 const int kNumVit = 6;
 
-inline uint32_t vit_steps(uint32_t K, uint32_t E, int C)
-{
-    const uint32_t strip = 32u * C, n_strips = (K + strip - 1) / strip;
-    const uint32_t P = n_strips > 1 ? std::max<uint32_t>(E, kMinPeriod) : E;
-    return (n_strips - 1) * P + E + ((K - (n_strips - 1) * strip) - 1) / C;
-}
-
 } // namespace
 
 extern "C" int nph_hmm_align_batch(nph_ctx* ctx,
@@ -156,9 +147,10 @@ extern "C" int nph_hmm_align(nph_ctx* ctx,
     // jobs, ranks, transitions and validation go through the forward path's loader (same job semantics)
     NPH_TRY(nph_hmm_jobs_load(ctx, kmer_ranks, n_ranks_total, jobs, n_jobs, indel_bias));
 
-    // class per job (columns per lane) and schedule, longest first
-    std::vector<std::vector<std::pair<uint32_t, uint32_t>>> per(kNumVit);
-    uint32_t max_kpad = 32, max_period = kMinPeriod;
+    // class per job (columns per lane) and schedule: class by class, longest first inside each
+    std::vector<uint64_t> key(n_jobs);
+    size_t first[kNumVit + 1] = {};
+    uint32_t max_kpad = 32, max_period = NPH_MIN_PERIOD;
     uint64_t max_trace = 1;
     for (size_t j = 0; j < n_jobs; ++j) {
         const nph_hmm_job& jb = jobs[j];
@@ -167,26 +159,19 @@ extern "C" int nph_hmm_align(nph_ctx* ctx,
         if (states_off[j + 1] < states_off[j]) return NPH_ERR_INVALID;
         double best = 1e300; int bi = 0; uint32_t bsteps = 0;
         for (int i = 0; i < kNumVit; ++i) {
-            const uint32_t st = vit_steps(K, E, kVitCols[i]);
+            const uint32_t st = nph_class_steps(K, E, kVitCols[i], 32);
             const double cost = (double)st * (120.0 + 70.0 * kVitCols[i]);
             if (cost < best) { best = cost; bi = i; bsteps = st; }
         }
-        per[bi].push_back({bsteps, (uint32_t)j});
+        key[j] = (uint64_t)(kNumVit - 1 - bi) << 32 | bsteps;
+        ++first[bi + 1];
         const uint32_t strip = 32u * kVitCols[bi], n_strips = (K + strip - 1) / strip;
         max_kpad = std::max(max_kpad, n_strips * strip);
-        max_period = std::max(max_period, std::max<uint32_t>(E, kMinPeriod));
+        max_period = std::max(max_period, std::max<uint32_t>(E, NPH_MIN_PERIOD));
         max_trace = std::max<uint64_t>(max_trace, (uint64_t)(bsteps + 1) * strip);
     }
-    std::vector<uint32_t> order;
-    order.reserve(n_jobs);
-    size_t first[kNumVit + 1];
-    for (int i = 0; i < kNumVit; ++i) {
-        first[i] = order.size();
-        std::sort(per[i].begin(), per[i].end(), [](const std::pair<uint32_t, uint32_t>& a, const std::pair<uint32_t, uint32_t>& b) {
-            return a.first != b.first ? a.first > b.first : a.second < b.second; });
-        for (auto& e : per[i]) order.push_back(e.second);
-    }
-    first[kNumVit] = order.size();
+    const std::vector<uint32_t> order = nph_longest_first(key);
+    for (int i = 0; i < kNumVit; ++i) first[i + 1] += first[i];
 
     // The movement trace is per resident warp and sized by the batch's largest job ((steps + 1) x strip uint16 entries),
     // so one long window must not multiply by every warp of the chip: the number of resident CTAs is capped so that
@@ -202,29 +187,23 @@ extern "C" int nph_hmm_align(nph_ctx* ctx,
     const int max_ctas = (int)std::min<uint64_t>((uint64_t)ctx->sm_count, std::max<uint64_t>(1, kTraceBudget / per_cta));
     const int warps = max_ctas * kWarps;
     const size_t total_states = (size_t)states_off[n_jobs];
-    const size_t b_params = sizeof(float4) * (size_t)max_kpad * warps;
-    const size_t b_edge = sizeof(float) * 3 * ((size_t)max_period + 8) * warps;
-    const size_t b_trace = sizeof(uint16_t) * trace_stride * warps;
-    const size_t b_states = sizeof(nph_align_state) * total_states;
-    const size_t b_off = sizeof(uint64_t) * (n_jobs + 1);
-    const size_t b_n = sizeof(uint32_t) * n_jobs;
-    auto al = [](size_t v) { return (v + 255) / 256 * 256; };
-    const size_t need = al(b_params) + al(b_edge) + al(b_trace) + al(b_states) + al(b_off) + al(b_n) + al(sizeof(uint32_t) * n_jobs);
-    NPH_TRY(nph_reserve(ctx, ctx->d_abea_scratch, need));      // shares the alignment scratch arena with ABEA
-    uint8_t* base = ctx->d_abea_scratch.p;
     VitParams p{};
-    p.scratch_params = reinterpret_cast<float4*>(base); base += al(b_params);
-    p.scratch_edge = reinterpret_cast<float*>(base); base += al(b_edge);
-    p.scratch_trace = reinterpret_cast<uint16_t*>(base); base += al(b_trace);
-    p.states = reinterpret_cast<nph_align_state*>(base); base += al(b_states);
-    uint64_t* d_off = reinterpret_cast<uint64_t*>(base); base += al(b_off);
-    p.n_states = reinterpret_cast<uint32_t*>(base); base += al(b_n);
-    uint32_t* d_order = reinterpret_cast<uint32_t*>(base);
+    uint64_t* d_off = nullptr;
+    uint32_t* d_order = nullptr;
+    NPH_TRY(nph_carve(ctx, ctx->d_abea_scratch, [&](NphArena& a) {      // shares the alignment scratch arena with ABEA
+        p.scratch_params = a.take<float4>((size_t)max_kpad * warps);
+        p.scratch_edge = a.take<float>(3 * ((size_t)max_period + 8) * warps);
+        p.scratch_trace = a.take<uint16_t>(trace_stride * warps);
+        p.states = a.take<nph_align_state>(total_states);
+        d_off = a.take<uint64_t>(n_jobs + 1);
+        p.n_states = a.take<uint32_t>(n_jobs);
+        d_order = a.take<uint32_t>(n_jobs);
+    }));
     p.states_off = d_off;
     p.level = ctx->d_level.p; p.reads = ctx->d_reads.p; p.trans = ctx->d_trans.p; p.models = ctx->d_models.p;
     p.ranks = ctx->d_ranks.p; p.jobs = ctx->d_jobs.p; p.flank = ctx->d_flank.p; p.scores = ctx->d_scores.p;
     p.kpad_stride = max_kpad; p.edge_stride = max_period + 8; p.trace_stride = trace_stride; p.c = ctx->consts;
-    NPH_CUDA(ctx, cudaMemcpyAsync(d_off, states_off, b_off, cudaMemcpyHostToDevice, ctx->stream));
+    NPH_CUDA(ctx, cudaMemcpyAsync(d_off, states_off, sizeof(uint64_t) * (n_jobs + 1), cudaMemcpyHostToDevice, ctx->stream));
     NPH_CUDA(ctx, cudaMemcpyAsync(d_order, order.data(), sizeof(uint32_t) * n_jobs, cudaMemcpyHostToDevice, ctx->stream));
     NPH_CUDA(ctx, cudaMemsetAsync(ctx->d_counters.p, 0, sizeof(unsigned int) * NPH_NUM_COUNTERS, ctx->stream));
     NPH_CUDA(ctx, cudaEventRecord(ctx->ev0, ctx->stream));
@@ -245,10 +224,9 @@ extern "C" int nph_hmm_align(nph_ctx* ctx,
         ++launches;
     }
     NPH_CUDA(ctx, cudaEventRecord(ctx->ev1, ctx->stream));
-    ctx->last_launches = launches;
-    ctx->timing_valid = true;
-    NPH_CUDA(ctx, cudaMemcpyAsync(states_out, p.states, b_states, cudaMemcpyDeviceToHost, ctx->stream));
-    NPH_CUDA(ctx, cudaMemcpyAsync(n_states_out, p.n_states, b_n, cudaMemcpyDeviceToHost, ctx->stream));
+    nph_timing_events(ctx, launches);
+    NPH_CUDA(ctx, cudaMemcpyAsync(states_out, p.states, sizeof(nph_align_state) * total_states, cudaMemcpyDeviceToHost, ctx->stream));
+    NPH_CUDA(ctx, cudaMemcpyAsync(n_states_out, p.n_states, sizeof(uint32_t) * n_jobs, cudaMemcpyDeviceToHost, ctx->stream));
     if (scores_out) NPH_CUDA(ctx, cudaMemcpyAsync(scores_out, ctx->d_scores.p, sizeof(float) * n_jobs, cudaMemcpyDeviceToHost, ctx->stream));
     NPH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     ctx->abea_loaded = false;   // the arena was reused

@@ -5,13 +5,13 @@
 //   ProfileHMMViterbiOutputR9     ref: src/hmm/nanopolish_profile_hmm_r9.inl:130-197
 #pragma once
 #include "nph_internal.cuh"
+#include "hmm_classes.h"
 #include "exact_math.cuh"
 #include <math_constants.h>
 
 namespace nph_vit {
 
 constexpr unsigned kFull = 0xffffffffu;
-constexpr int kMinPeriod = 40;
 enum { MV_SAME_M = 0, MV_PREV_M = 1, MV_SAME_B = 2, MV_PREV_B = 3, MV_PREV_K = 4, MV_SOFT = 5 };
 
 // one profile_hmm_align call, as the warp sees it
@@ -66,18 +66,12 @@ __device__ __forceinline__ int viterbi_align(const HmmConsts& c, const float* __
     uint16_t* const trace = sc.trace;
     const int n_strips = (K + STRIP - 1) / STRIP;
     const int kpad = n_strips * STRIP;
-    const int P = n_strips > 1 ? max(E, kMinPeriod) : E;
+    const int P = n_strips > 1 ? max(E, NPH_MIN_PERIOD) : E;
     {
         const uint32_t* rk = j.rk;
         for (int i = lane; i < kpad; i += 32) {
             float4 g = make_float4(0.f, 1.f, 0.f, 1.f);
-            if (i < K) {
-                const uint32_t r = rk[i];
-                const float mu = (float)__dadd_rn(__dmul_rn(rd.scale, mv.mean[r]), rd.shift);
-                const float sd = (float)__dmul_rn(mv.stdv[r], rd.var);
-                const float lsd = (float)__dadd_rn(mv.log_stdv[r], rd.log_var);
-                g = make_float4(mu, sd, __fsub_rn(c.log_inv_sqrt_2pi, lsd), __frcp_rn(sd));
-            }
+            if (i < K) g = nph_scaled_gaussian(mv, rd, rk[i], c.log_inv_sqrt_2pi);
             my_params[i] = g;
         }
     }

@@ -16,13 +16,9 @@
 #include <cstdlib>
 #include <vector>
 
-#define NPH_TRY(expr) do { int rc__ = (expr); if (rc__ != NPH_OK) return rc__; } while (0)
-
 namespace {
 
 constexpr int kConvWarps = 8;
-
-inline size_t al256(size_t v) { return (v + 255) / 256 * 256; }
 
 struct ConvParams {
     const nph_event* events;         // capacity layout: read t at cap_off[t]
@@ -123,13 +119,15 @@ extern "C" int nph_load_from_raw_batch(nph_ctx* ctx, const float* raw, size_t n_
     std::vector<nph_raw_read> rr(n_jobs);
     size_t cap_total = 0;
     for (size_t j = 0; j < n_jobs; ++j) { rr[j] = nph_raw_read{jobs[j].sample_off, 0, jobs[j].n_samples, 0}; cap_total += jobs[j].n_samples / 2 + 8; }
-    const size_t b_raw = al256(sizeof(float) * n_samples_total);
-    const size_t b_trim = nph_trim_scratch_bytes(rr.data(), n_jobs, 100);
-    const size_t b_ed = nph_ed_scratch_bytes(n_samples_total, n_jobs, cap_total);
-    const size_t b_small = al256(sizeof(uint64_t) * n_jobs) * 2 + al256(sizeof(uint32_t) * n_jobs) + al256(sizeof(double) * n_jobs);
-    NPH_TRY(nph_reserve(ctx, ctx->d_abea_scratch, b_raw + std::max(b_trim, b_ed + b_small)));
-    float* d_raw = reinterpret_cast<float*>(ctx->d_abea_scratch.p);
-    uint8_t* arena = ctx->d_abea_scratch.p + b_raw;
+    // raw samples | the trim's scratch, later the detector's (its events are read after it returns) | small per-read arrays
+    float* d_raw; uint8_t* arena; uint64_t* d_cap_off; uint64_t* d_out_off; double* d_rate;
+    NPH_TRY(nph_carve(ctx, ctx->d_abea_scratch, [&](NphArena& a) {
+        d_raw = a.take<float>(n_samples_total);
+        arena = a.take<uint8_t>(std::max(nph_trim_scratch_bytes(rr.data(), n_jobs, 100), nph_ed_scratch_bytes(n_jobs, cap_total)));
+        d_cap_off = a.take<uint64_t>(n_jobs);
+        d_out_off = a.take<uint64_t>(n_jobs);
+        d_rate = a.take<double>(n_jobs);
+    }));
     NPH_CUDA(ctx, cudaMemcpyAsync(d_raw, raw, sizeof(float) * n_samples_total, cudaMemcpyHostToDevice, ctx->stream));
     NPH_CUDA(ctx, cudaEventRecord(ctx->ev0, ctx->stream));
     int launches = 0;
@@ -153,7 +151,7 @@ extern "C" int nph_load_from_raw_batch(nph_ctx* ctx, const float* raw, size_t n_
     if (live.empty()) {
         if (base_to_event_out) for (size_t i = 0; i < n_ranks_total; ++i) base_to_event_out[i] = nph_event_range{-1, -1};
         for (size_t j = 0; j <= n_jobs; ++j) event_off_out[j] = 0;
-        ctx->last_launches = launches; ctx->staged_ms = staged_ms; ctx->timing_valid = 2;
+        nph_timing_staged(ctx, staged_ms, launches);
         return NPH_OK;
     }
     const size_t nl = live.size();
@@ -202,28 +200,20 @@ extern "C" int nph_load_from_raw_batch(nph_ctx* ctx, const float* raw, size_t n_
     }
     (void)n_live_ranks;
     NPH_TRY(nph_reserve(ctx, ctx->d_ev_mean, n_events_total));
-    ctx->ev_mean_resident = true;
     NPH_TRY(nph_reserve(ctx, ctx->d_ev_time, n_events_total));
     NPH_TRY(nph_reserve(ctx, ctx->d_level, n_events_total));
     NPH_TRY(nph_reserve(ctx, ctx->d_reads, nl));
-    const size_t b_ev4 = al256(sizeof(float) * n_events_total), b_mom = al256(sizeof(double) * 2 * nl), b_views = al256(sizeof(nph_read) * nl);
-    const size_t b_b2e = al256(sizeof(nph_event_range) * n_ranks_total), b_cal = al256(sizeof(nph_calibration) * nl);
-    NPH_TRY(nph_reserve(ctx, ctx->d_prep, 2 * b_ev4 + b_mom + b_views + b_b2e + b_cal + 256));
-    uint8_t* pb = ctx->d_prep.p;
-    float* d_stdv = reinterpret_cast<float*>(pb); pb += b_ev4;
-    float* d_dur = reinterpret_cast<float*>(pb); pb += b_ev4;
-    double* d_mom = reinterpret_cast<double*>(pb); pb += b_mom;
-    nph_read* d_views = reinterpret_cast<nph_read*>(pb); pb += b_views;
-    nph_event_range* d_b2e = reinterpret_cast<nph_event_range*>(pb); pb += b_b2e;
-    nph_calibration* d_cal = reinterpret_cast<nph_calibration*>(pb); pb += b_cal;
-    int* d_bad = reinterpret_cast<int*>(pb);
+    float* d_stdv; float* d_dur; double* d_mom; nph_read* d_views; nph_event_range* d_b2e; nph_calibration* d_cal; int* d_bad;
+    NPH_TRY(nph_carve(ctx, ctx->d_prep, [&](NphArena& a) {
+        d_stdv = a.take<float>(n_events_total);
+        d_dur = a.take<float>(n_events_total);
+        d_mom = a.take<double>(2 * nl);
+        d_views = a.take<nph_read>(nl);
+        d_b2e = a.take<nph_event_range>(n_ranks_total);
+        d_cal = a.take<nph_calibration>(nl);
+        d_bad = a.take<int>(1);
+    }));
     {
-        // small per-read arrays behind the detector's scratch (still alive: the events are read from it)
-        uint8_t* sb = arena + b_ed;
-        uint64_t* d_cap_off = reinterpret_cast<uint64_t*>(sb); sb += al256(sizeof(uint64_t) * n_jobs);
-        uint64_t* d_out_off = reinterpret_cast<uint64_t*>(sb); sb += al256(sizeof(uint64_t) * n_jobs);
-        sb += al256(sizeof(uint32_t) * n_jobs);
-        double* d_rate = reinterpret_cast<double*>(sb);
         std::vector<double> rate(nl);
         for (size_t t = 0; t < nl; ++t) rate[t] = jobs[live[t]].sample_rate;
         NPH_CUDA(ctx, cudaMemcpyAsync(d_cap_off, cap_off.data(), sizeof(uint64_t) * nl, cudaMemcpyHostToDevice, ctx->stream));
@@ -250,7 +240,7 @@ extern "C" int nph_load_from_raw_batch(nph_ctx* ctx, const float* raw, size_t n_
     ctx->n_reads = nl;
     ctx->n_events_total = n_events_total;
     ctx->h_read_n_events.assign(counts.begin(), counts.end());
-    ctx->reads_loaded = true;                      // for the staged ABEA calls below; cleared again before returning
+    nph_reads_resident(ctx);                       // for the staged ABEA calls below; cleared again before returning
     int rc = nph_abea_jobs_load(ctx, kmer_ranks, n_ranks_total, aj.data(), nl, model_id, pairs_total);
     if (rc == NPH_OK) rc = nph_launch_mom(ctx, d_mom, params->reverse_events != 0);
     if (rc == NPH_OK) {
@@ -279,9 +269,7 @@ extern "C" int nph_load_from_raw_batch(nph_ctx* ctx, const float* raw, size_t n_
     for (size_t t = 0; t < nl; ++t) calibrations_out[live[t]] = cal[t];
     NPH_CUDA(ctx, cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1)); staged_ms += ms;     // ev0 was recorded at the ABEA launch
     if (verbose) fprintf(stderr, "  abea+calibration %.2f ms  (total %.2f ms, %zu of %zu reads aligned)\n", ms, staged_ms, nl, n_jobs);
-    ctx->last_launches = launches;
-    ctx->staged_ms = staged_ms;
-    ctx->timing_valid = 2;
+    nph_timing_staged(ctx, staged_ms, launches);
     return NPH_OK;
 }
 

@@ -29,8 +29,6 @@
 #include <string>
 #include <vector>
 
-#define NPH_TRY(expr) do { int rc__ = (expr); if (rc__ != NPH_OK) return rc__; } while (0)
-
 namespace {
 
 constexpr int kWarps = 8;
@@ -550,23 +548,18 @@ extern "C" int nph_methylation_run(nph_ctx* ctx)
     }
     m.n_sites = h.n_sites; m.n_ranks = h.n_ranks; m.n_scored_events = h.n_events;
     const size_t n_jobs = 2 * (size_t)h.n_sites;
-    ctx->n_jobs = 0; ctx->jobs_loaded = false; ctx->codes_mode = false;       // the enumerator emits k-mer ranks
+    ctx->n_jobs = 0; ctx->jobs_loaded = false;
     if (n_jobs == 0) { ctx->classes.clear(); ctx->jobs_loaded = true; m.ran = true; return NPH_OK; }
     NPH_TRY(nph_reserve(ctx, ctx->d_ranks, (size_t)h.n_ranks));
-    NPH_TRY(nph_reserve(ctx, ctx->d_jobs, n_jobs));
-    NPH_TRY(nph_reserve(ctx, ctx->d_order, n_jobs));
-    NPH_TRY(nph_reserve(ctx, ctx->d_scores, n_jobs));
     NPH_TRY(nph_reserve(ctx, m.d_sites, (size_t)h.n_sites));
-    NPH_TRY(nph_upload_read_transitions(ctx, m.indel_bias));
-    EmitArgs ea{m.d_ref.p, m.d_records.p, m.d_prov_off.p, reinterpret_cast<const MethGroup*>(m.d_prov.p), counts, site_off, rank_off,
-                ctx->d_jobs.p, ctx->d_ranks.p, m.d_sites.p, n};
-    meth_emit_kernel<<<grid, kThreads, 0, ctx->stream>>>(ea, d);
-    NPH_CUDA(ctx, cudaGetLastError());
-    ctx->jobs_trusted = true;                                     // meth_emit_kernel wrote these ranks: the scheduler need not walk them
-    const int rc_sched = nph_jobs_schedule(ctx, n_jobs, (size_t)h.n_ranks);   // read-back 2 of 2: validation + schedule summary
-    ctx->jobs_trusted = false;
-    NPH_TRY(rc_sched);
-    NPH_TRY(nph_launch_hmm_forward(ctx, nullptr));
+    // meth_emit_kernel writes the jobs and their k-mer ranks; the schedule is read-back 2 of 2
+    NPH_TRY(nph_score_device_jobs(ctx, n_jobs, (size_t)h.n_ranks, m.indel_bias, [&]() -> int {
+        EmitArgs ea{m.d_ref.p, m.d_records.p, m.d_prov_off.p, reinterpret_cast<const MethGroup*>(m.d_prov.p), counts, site_off, rank_off,
+                    ctx->d_jobs.p, ctx->d_ranks.p, m.d_sites.p, n};
+        meth_emit_kernel<<<grid, kThreads, 0, ctx->stream>>>(ea, d);
+        NPH_CUDA(ctx, cudaGetLastError());
+        return NPH_OK;
+    }));
     const int fgrid = (int)std::min<size_t>(((size_t)h.n_sites + 255) / 256, (size_t)ctx->sm_count * 8);
     meth_fill_kernel<<<fgrid, 256, 0, ctx->stream>>>(m.d_sites.p, ctx->d_scores.p, h.n_sites);
     NPH_CUDA(ctx, cudaGetLastError());
@@ -719,21 +712,24 @@ extern "C" int nph_methylation_tsv(nph_ctx* ctx, const char* contig, const char*
     const size_t n = m.n_records, contig_len = std::strlen(contig), names_len = name_off[n];
     for (size_t r = 0; r < n; ++r) if (name_off[r] > name_off[r + 1]) { ctx->last_error = "name_off must ascend"; return NPH_ERR_INVALID; }
     // one staging block: contig | names | name offsets | strand flags
-    auto al = [](size_t v) { return (v + 15) / 16 * 16; };
-    const size_t o_names = al(contig_len + 1), o_noff = o_names + al(names_len + 1), o_rev = o_noff + al(sizeof(uint32_t) * (n + 1));
-    NPH_TRY(nph_reserve(ctx, m.d_tsv_in, o_rev + al(n)));
+    char* d_contig; char* d_names; uint32_t* d_noff; uint8_t* d_rev;
+    NPH_TRY(nph_carve(ctx, m.d_tsv_in, [&](NphArena& a) {
+        d_contig = a.take<char>(contig_len + 1);
+        d_names = a.take<char>(names_len + 1);
+        d_noff = a.take<uint32_t>(n + 1);
+        d_rev = a.take<uint8_t>(n);
+    }));
     NPH_TRY(nph_reserve(ctx, m.d_tsv_off, 2 * n + 4));
-    uint8_t* in = m.d_tsv_in.p;
-    NPH_CUDA(ctx, cudaMemcpyAsync(in, contig, contig_len, cudaMemcpyHostToDevice, ctx->stream));
-    NPH_CUDA(ctx, cudaMemcpyAsync(in + o_names, read_names, names_len, cudaMemcpyHostToDevice, ctx->stream));
-    NPH_CUDA(ctx, cudaMemcpyAsync(in + o_noff, name_off, sizeof(uint32_t) * (n + 1), cudaMemcpyHostToDevice, ctx->stream));
-    NPH_CUDA(ctx, cudaMemcpyAsync(in + o_rev, is_reverse, n, cudaMemcpyHostToDevice, ctx->stream));
+    NPH_CUDA(ctx, cudaMemcpyAsync(d_contig, contig, contig_len, cudaMemcpyHostToDevice, ctx->stream));
+    NPH_CUDA(ctx, cudaMemcpyAsync(d_names, read_names, names_len, cudaMemcpyHostToDevice, ctx->stream));
+    NPH_CUDA(ctx, cudaMemcpyAsync(d_noff, name_off, sizeof(uint32_t) * (n + 1), cudaMemcpyHostToDevice, ctx->stream));
+    NPH_CUDA(ctx, cudaMemcpyAsync(d_rev, is_reverse, n, cudaMemcpyHostToDevice, ctx->stream));
     uint64_t* rec_bytes = m.d_tsv_off.p;
     uint64_t* rec_off = rec_bytes + n;                                  // n + 1 entries
     int* d_refused = reinterpret_cast<int*>(rec_off + n + 1);
     NPH_CUDA(ctx, cudaMemsetAsync(d_refused, 0, sizeof(int), ctx->stream));
-    TsvArgs a{m.d_sites.p, m.d_counts.p + 3 * n, m.d_records.p, m.d_ref.p, reinterpret_cast<const char*>(in), (uint32_t)contig_len,
-              reinterpret_cast<const char*>(in + o_names), reinterpret_cast<const uint32_t*>(in + o_noff), in + o_rev, m.params.k, (uint32_t)n,
+    TsvArgs a{m.d_sites.p, m.d_counts.p + 3 * n, m.d_records.p, m.d_ref.p, d_contig, (uint32_t)contig_len,
+              d_names, d_noff, d_rev, m.params.k, (uint32_t)n,
               rec_bytes, rec_off, nullptr, d_refused};
     const int grid = (int)std::min<size_t>((n + kWarps - 1) / kWarps, (size_t)ctx->sm_count * 8);
     meth_tsv_kernel<false><<<grid, kThreads, 0, ctx->stream>>>(a);
@@ -818,14 +814,11 @@ extern "C" int nph_methylation_batch_compact(nph_ctx* ctx,
 {
     if (!ctx || !site_off_out) return NPH_ERR_INVALID;
     if (n_records == 0) { site_off_out[0] = 0; if (n_scored_events_out) *n_scored_events_out = 0; return NPH_OK; }
-    ctx->levels_inflight = false;
-    int rc = nph_reads_load_impl(ctx, reads, n_reads, ev_mean, ev_start_time, n_events_total, true);
-    if (rc == NPH_OK) { ctx->reads_loaded = true; ctx->jobs_loaded = false; ctx->abea_loaded = false; }
-    if (rc == NPH_OK) rc = nph_methylation_load_compact(ctx, ref_bases, event_deltas, n_ref_total, first_event, records, n_records, params, indel_bias);
-    if (rc == NPH_OK && ctx->levels_inflight) rc = nph_upload_level_chunks(ctx, ev_mean);
+    int rc = nph_oneshot_begin(ctx, reads, n_reads, ev_mean, ev_start_time, n_events_total, [&] {
+        return nph_methylation_load_compact(ctx, ref_bases, event_deltas, n_ref_total, first_event, records, n_records, params, indel_bias); });
     if (rc == NPH_OK) rc = nph_methylation_run(ctx);
     if (rc == NPH_OK) rc = nph_methylation_fetch(ctx, site_off_out, sites_out, sites_cap);
-    nph_finish_level_upload(ctx);
+    nph_oneshot_finish(ctx);
     if (rc == NPH_OK && n_scored_events_out) *n_scored_events_out = ctx->meth.n_scored_events;
     return rc;
 }
@@ -846,14 +839,11 @@ extern "C" int nph_methylation_batch_compact_tsv(nph_ctx* ctx,
     if (n_sites_out) *n_sites_out = 0;
     if (n_scored_events_out) *n_scored_events_out = 0;
     if (n_records == 0) return NPH_OK;
-    ctx->levels_inflight = false;
-    int rc = nph_reads_load_impl(ctx, reads, n_reads, ev_mean, ev_start_time, n_events_total, true);
-    if (rc == NPH_OK) { ctx->reads_loaded = true; ctx->jobs_loaded = false; ctx->abea_loaded = false; }
-    if (rc == NPH_OK) rc = nph_methylation_load_compact(ctx, ref_bases, event_deltas, n_ref_total, first_event, records, n_records, params, indel_bias);
-    if (rc == NPH_OK && ctx->levels_inflight) rc = nph_upload_level_chunks(ctx, ev_mean);
+    int rc = nph_oneshot_begin(ctx, reads, n_reads, ev_mean, ev_start_time, n_events_total, [&] {
+        return nph_methylation_load_compact(ctx, ref_bases, event_deltas, n_ref_total, first_event, records, n_records, params, indel_bias); });
     if (rc == NPH_OK) rc = nph_methylation_run(ctx);
     if (rc == NPH_OK) rc = nph_methylation_tsv(ctx, contig, read_names, name_off, is_reverse, tsv_out, cap, n_bytes_out);
-    nph_finish_level_upload(ctx);
+    nph_oneshot_finish(ctx);
     if (n_sites_out) *n_sites_out = ctx->meth.n_sites;
     if (n_scored_events_out) *n_scored_events_out = ctx->meth.n_scored_events;
     return rc;
@@ -871,17 +861,11 @@ extern "C" int nph_methylation_batch(nph_ctx* ctx,
 {
     if (!ctx || !site_off_out) return NPH_ERR_INVALID;
     if (n_records == 0) { site_off_out[0] = 0; if (n_scored_events_out) *n_scored_events_out = 0; return NPH_OK; }
-    // Order of issue: read records first (small), then the reference bases / event alignments / records the enumeration
-    // needs, then the event levels in chunks on the copy stream — the enumeration and the scheduler run while the levels
-    // are still crossing PCIe, and the forward kernels wait per job on the chunk that holds their read.
-    ctx->levels_inflight = false;
-    int rc = nph_reads_load_impl(ctx, reads, n_reads, ev_mean, ev_start_time, n_events_total, true);
-    if (rc == NPH_OK) { ctx->reads_loaded = true; ctx->jobs_loaded = false; ctx->abea_loaded = false; }
-    if (rc == NPH_OK) rc = nph_methylation_load(ctx, ref_bases, n_ref_total, aligned_events, n_pairs_total, records, n_records, params, indel_bias);
-    if (rc == NPH_OK && ctx->levels_inflight) rc = nph_upload_level_chunks(ctx, ev_mean);
+    int rc = nph_oneshot_begin(ctx, reads, n_reads, ev_mean, ev_start_time, n_events_total, [&] {
+        return nph_methylation_load(ctx, ref_bases, n_ref_total, aligned_events, n_pairs_total, records, n_records, params, indel_bias); });
     if (rc == NPH_OK) rc = nph_methylation_run(ctx);
     if (rc == NPH_OK) rc = nph_methylation_fetch(ctx, site_off_out, sites_out, sites_cap);
-    nph_finish_level_upload(ctx);
+    nph_oneshot_finish(ctx);
     if (rc == NPH_OK && n_scored_events_out) *n_scored_events_out = ctx->meth.n_scored_events;
     return rc;
 }

@@ -19,40 +19,9 @@ int nph_set_cuda_error(nph_ctx* ctx, cudaError_t e, const char* what)
     return NPH_ERR_CUDA;
 }
 
-template <typename T>
-int nph_reserve(nph_ctx* ctx, DevBuf<T>& b, size_t n)
-{
-    if (n <= b.cap && b.p) return NPH_OK;
-    if (b.p) { NPH_CUDA(ctx, cudaFree(b.p)); b.p = nullptr; b.cap = 0; }
-    size_t want = n + n / 8 + 16;
-    NPH_CUDA(ctx, cudaMalloc((void**)&b.p, want * sizeof(T)));
-    b.cap = want;
-    return NPH_OK;
-}
-template int nph_reserve<float>(nph_ctx*, DevBuf<float>&, size_t);
-template int nph_reserve<double>(nph_ctx*, DevBuf<double>&, size_t);
-template int nph_reserve<uint32_t>(nph_ctx*, DevBuf<uint32_t>&, size_t);
-template int nph_reserve<uint8_t>(nph_ctx*, DevBuf<uint8_t>&, size_t);
-template int nph_reserve<uint16_t>(nph_ctx*, DevBuf<uint16_t>&, size_t);
-template int nph_reserve<DevRead>(nph_ctx*, DevBuf<DevRead>&, size_t);
-template int nph_reserve<DevModelView>(nph_ctx*, DevBuf<DevModelView>&, size_t);
-template int nph_reserve<nph_hmm_job>(nph_ctx*, DevBuf<nph_hmm_job>&, size_t);
-template int nph_reserve<float2>(nph_ctx*, DevBuf<float2>&, size_t);
-template int nph_reserve<nph_abea_job>(nph_ctx*, DevBuf<nph_abea_job>&, size_t);
-template int nph_reserve<nph_aligned_pair>(nph_ctx*, DevBuf<nph_aligned_pair>&, size_t);
-template int nph_reserve<nph_abea_result>(nph_ctx*, DevBuf<nph_abea_result>&, size_t);
-template int nph_reserve<uint64_t>(nph_ctx*, DevBuf<uint64_t>&, size_t);
-template int nph_reserve<nph_meth_record>(nph_ctx*, DevBuf<nph_meth_record>&, size_t);
-template int nph_reserve<nph_meth_site>(nph_ctx*, DevBuf<nph_meth_site>&, size_t);
-
-#define NPH_TRY(expr) do { int rc__ = (expr); if (rc__ != NPH_OK) return rc__; } while (0)
-
 extern "C" int nph_destroy(nph_ctx* ctx);
 
 namespace {
-
-template <typename T>
-void free_buf(DevBuf<T>& b) { if (b.p) cudaFree(b.p); b.p = nullptr; b.cap = 0; }
 
 // clip-penalty table (see np_oracle.c:npo_flank_table for the derivation; ref profile_hmm_r9.inl:200-260)
 int ensure_flank(nph_ctx* ctx, size_t n)
@@ -131,12 +100,12 @@ int create_common(nph_ctx** out, int device, bool own_stream, cudaStream_t strea
         cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&ctx->ev_reset, cudaEventDisableTiming) != cudaSuccess ||
         cudaStreamCreateWithFlags(&ctx->cstream, cudaStreamNonBlocking) != cudaSuccess) return fail(NPH_ERR_CUDA);
-    if (cudaMalloc((void**)&ctx->d_progress, sizeof(uint32_t)) != cudaSuccess) return fail(NPH_ERR_NOMEM);
-    if (cudaMallocHost((void**)&ctx->h_progress_vals, sizeof(uint32_t) * (nph_ctx::kLevelChunks + 1)) != cudaSuccess) {
-        ctx->h_progress_vals = nullptr;
+    if (nph_reserve(ctx, ctx->d_progress, 1) != NPH_OK) return fail(NPH_ERR_NOMEM);
+    if (cudaMallocHost((void**)&ctx->h_progress_vals.p, sizeof(uint32_t) * (nph_ctx::kLevelChunks + 1)) != cudaSuccess) {
+        ctx->h_progress_vals.p = nullptr;
         return fail(NPH_ERR_NOMEM);
     }
-    for (int i = 0; i <= nph_ctx::kLevelChunks; ++i) ctx->h_progress_vals[i] = (uint32_t)(i + 1);
+    for (int i = 0; i <= nph_ctx::kLevelChunks; ++i) ctx->h_progress_vals.p[i] = (uint32_t)(i + 1);
     for (int i = 0; i < nph_ctx::kSideStreams; ++i) {
         if (cudaStreamCreateWithFlags(&ctx->side[i], cudaStreamNonBlocking) != cudaSuccess ||
             cudaEventCreateWithFlags(&ctx->ev_join[i], cudaEventDisableTiming) != cudaSuccess) return fail(NPH_ERR_CUDA);
@@ -146,8 +115,8 @@ int create_common(nph_ctx** out, int device, bool own_stream, cudaStream_t strea
     // entries NPH_LOGSUM_CUT .. NPH_TBL_SMEM - 1 are 0.0f: every difference >= 15.7f returns max
     std::vector<float> tbl(NPH_TBL_SMEM, 0.0f);
     for (int i = 0; i < NPH_LOGSUM_CUT; ++i) tbl[i] = (float)log(1. + exp((double)-i / 1000.f));
-    if (cudaMalloc((void**)&ctx->d_logsum, sizeof(float) * NPH_TBL_SMEM) != cudaSuccess) return fail(NPH_ERR_NOMEM);
-    if (cudaMemcpy(ctx->d_logsum, tbl.data(), sizeof(float) * NPH_TBL_SMEM, cudaMemcpyHostToDevice) != cudaSuccess) return fail(NPH_ERR_CUDA);
+    if (nph_reserve(ctx, ctx->d_logsum, NPH_TBL_SMEM) != NPH_OK) return fail(NPH_ERR_NOMEM);
+    if (cudaMemcpy(ctx->d_logsum.p, tbl.data(), sizeof(float) * NPH_TBL_SMEM, cudaMemcpyHostToDevice) != cudaSuccess) return fail(NPH_ERR_CUDA);
     const_transitions(ctx->consts);
     // the forward kernel computes lp + B once for all three bad-state transitions (hmm_forward_kernel.cuh)
     if (std::memcmp(&ctx->consts.lp_bk, &ctx->consts.lp_bm_next, sizeof(float)) != 0 ||
@@ -162,7 +131,7 @@ int create_common(nph_ctx** out, int device, bool own_stream, cudaStream_t strea
 
 int nph_upload_read_transitions(nph_ctx* ctx, double indel_bias)
 {
-    std::vector<float2>& trans = ctx->h_stage_trans;
+    std::vector<float2>& trans = ctx->h_stage_trans;      // host staging: outlives the async copy
     trans.resize(ctx->n_reads);
     for (size_t i = 0; i < ctx->n_reads; ++i) trans[i] = read_transitions(ctx->h_events_per_base[i], indel_bias);
     NPH_TRY(nph_reserve(ctx, ctx->d_trans, ctx->n_reads));
@@ -201,27 +170,14 @@ int nph_destroy(nph_ctx* ctx)
     if (!ctx) return NPH_ERR_INVALID;
     cudaSetDevice(ctx->device);
     if (ctx->stream || !ctx->own_stream) cudaStreamSynchronize(ctx->stream);
-    if (ctx->d_logsum) cudaFree(ctx->d_logsum);
-    free_buf(ctx->d_flank); free_buf(ctx->d_models); free_buf(ctx->d_reads); free_buf(ctx->d_ev_mean);
-    free_buf(ctx->d_ev_time); free_buf(ctx->d_level); free_buf(ctx->d_drift); free_buf(ctx->d_ranks); free_buf(ctx->d_codes); free_buf(ctx->d_rank_base);
-    free_buf(ctx->d_jobs); free_buf(ctx->d_trans); free_buf(ctx->d_order); free_buf(ctx->d_scores);
-    free_buf(ctx->d_counters); free_buf(ctx->d_sched_cls); free_buf(ctx->d_sched_bkt); free_buf(ctx->d_sched_hist); free_buf(ctx->d_scratch); free_buf(ctx->d_abea_jobs); free_buf(ctx->d_abea_ranks);
-    free_buf(ctx->d_pairs); free_buf(ctx->d_abea_res); free_buf(ctx->d_abea_scratch); free_buf(ctx->d_abea_order); free_buf(ctx->d_abea_consts); free_buf(ctx->d_prep);
-    free_buf(ctx->meth.d_ref); free_buf(ctx->meth.d_pairs); free_buf(ctx->meth.d_records); free_buf(ctx->meth.d_prov_off); free_buf(ctx->meth.d_prov);
-    free_buf(ctx->meth.d_counts); free_buf(ctx->meth.d_sites); free_buf(ctx->meth.d_tsv_in); free_buf(ctx->meth.d_tsv_off); free_buf(ctx->meth.d_tsv); free_buf(ctx->meth.d_deltas); free_buf(ctx->meth.d_dense);
-    free_buf(ctx->screen.d_ref); free_buf(ctx->screen.d_deltas); free_buf(ctx->screen.d_dense); free_buf(ctx->screen.d_records);
-    free_buf(ctx->screen.d_pos_off); free_buf(ctx->screen.d_pos_reads); free_buf(ctx->screen.d_state); free_buf(ctx->screen.d_job_off);
-    for (auto& m : ctx->models) { cudaFree(m.mean); cudaFree(m.stdv); cudaFree(m.log_stdv); }
     if (ctx->ev0) cudaEventDestroy(ctx->ev0);
     if (ctx->ev1) cudaEventDestroy(ctx->ev1);
     if (ctx->ev_fork) cudaEventDestroy(ctx->ev_fork);
     if (ctx->ev_reset) cudaEventDestroy(ctx->ev_reset);
     if (ctx->cstream) { cudaStreamSynchronize(ctx->cstream); cudaStreamDestroy(ctx->cstream); }
-    if (ctx->d_progress) cudaFree(ctx->d_progress);
-    if (ctx->h_progress_vals) cudaFreeHost(ctx->h_progress_vals);
     for (int i = 0; i < nph_ctx::kSideStreams; ++i) { if (ctx->ev_join[i]) cudaEventDestroy(ctx->ev_join[i]); if (ctx->side[i]) cudaStreamDestroy(ctx->side[i]); }
     if (ctx->own_stream && ctx->stream) cudaStreamDestroy(ctx->stream);
-    delete ctx;
+    delete ctx;                                  // the buffers free themselves
     return NPH_OK;
 }
 
@@ -243,19 +199,19 @@ int nph_model_upload(nph_ctx* ctx, const double* level_mean, const double* level
     for (uint32_t i = 0; i < k; ++i) expect *= alphabet_size;
     if (expect != n_states || k == 0 || k > 16 || alphabet_size == 0 || alphabet_size > 255) return NPH_ERR_INVALID;   // ref asserts states.size() == alphabet^k (profile_hmm_r9.inl:305)
     NPH_CUDA(ctx, cudaSetDevice(ctx->device));
-    DevModel m;
+    DevModel m;                                  // freed on every early return below
     const size_t bytes = sizeof(double) * n_states;
-    NPH_CUDA(ctx, cudaMalloc((void**)&m.mean, bytes));
-    NPH_CUDA(ctx, cudaMalloc((void**)&m.stdv, bytes));
-    NPH_CUDA(ctx, cudaMalloc((void**)&m.log_stdv, bytes));
-    NPH_CUDA(ctx, cudaMemcpyAsync(m.mean, level_mean, bytes, cudaMemcpyHostToDevice, ctx->stream));
-    NPH_CUDA(ctx, cudaMemcpyAsync(m.stdv, level_stdv, bytes, cudaMemcpyHostToDevice, ctx->stream));
-    NPH_CUDA(ctx, cudaMemcpyAsync(m.log_stdv, level_log_stdv, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    NPH_TRY(nph_reserve(ctx, m.mean, n_states));
+    NPH_TRY(nph_reserve(ctx, m.stdv, n_states));
+    NPH_TRY(nph_reserve(ctx, m.log_stdv, n_states));
+    NPH_CUDA(ctx, cudaMemcpyAsync(m.mean.p, level_mean, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    NPH_CUDA(ctx, cudaMemcpyAsync(m.stdv.p, level_stdv, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    NPH_CUDA(ctx, cudaMemcpyAsync(m.log_stdv.p, level_log_stdv, bytes, cudaMemcpyHostToDevice, ctx->stream));
     m.n_states = n_states; m.k = k; m.alphabet_size = alphabet_size;
-    ctx->models.push_back(m);
+    ctx->models.push_back(std::move(m));
     std::vector<DevModelView> views(ctx->models.size());
     for (size_t i = 0; i < views.size(); ++i)
-        views[i] = DevModelView{ctx->models[i].mean, ctx->models[i].stdv, ctx->models[i].log_stdv, ctx->models[i].n_states,
+        views[i] = DevModelView{ctx->models[i].mean.p, ctx->models[i].stdv.p, ctx->models[i].log_stdv.p, ctx->models[i].n_states,
                                 (uint16_t)ctx->models[i].k, (uint16_t)ctx->models[i].alphabet_size};
     NPH_TRY(nph_reserve(ctx, ctx->d_models, views.size()));
     NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_models.p, views.data(), sizeof(DevModelView) * views.size(), cudaMemcpyHostToDevice, ctx->stream));
@@ -264,11 +220,16 @@ int nph_model_upload(nph_ctx* ctx, const double* level_mean, const double* level
     return NPH_OK;
 }
 
+} // extern "C"
+
+namespace {
+
 // Shared by the staged call (pipelined = false: everything on the context's stream, synchronous) and by the
 // one-shot call (pipelined = true: read records on the main stream, event levels in chunks on the copy stream,
 // each chunk followed by a progress word the forward kernel polls — so scoring starts while levels still arrive).
-int nph_reads_load_impl(nph_ctx* ctx, const nph_read* reads, size_t n_reads,
-                           const float* ev_mean, const double* ev_start_time, size_t n_events_total, bool pipelined)
+// ctx->levels_inflight says whether the chunked path was taken; upload_level_chunks() then queues the chunks.
+int reads_load_impl(nph_ctx* ctx, const nph_read* reads, size_t n_reads,
+                    const float* ev_mean, const double* ev_start_time, size_t n_events_total, bool pipelined)
 {
     if (!ctx || !reads || !ev_mean || n_reads == 0) return NPH_ERR_INVALID;
     NPH_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -303,15 +264,14 @@ int nph_reads_load_impl(nph_ctx* ctx, const nph_read* reads, size_t n_reads,
         size_t chunk = (n_events_total + nph_ctx::kLevelChunks - 1) / nph_ctx::kLevelChunks;
         chunk = (chunk + 31) / 32 * 32;                       // 128-byte lines never straddle two chunks
         ctx->level_chunk_events = chunk;
-        NPH_CUDA(ctx, cudaMemsetAsync(ctx->d_progress, 0, sizeof(uint32_t), ctx->cstream));
+        NPH_CUDA(ctx, cudaMemsetAsync(ctx->d_progress.p, 0, sizeof(uint32_t), ctx->cstream));
         NPH_CUDA(ctx, cudaEventRecord(ctx->ev_reset, ctx->cstream));
         NPH_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_reset, 0));
         ctx->levels_inflight = true;
-        ctx->ev_mean_resident = false;                        // only d_level is filled on this path
+        nph_reads_resident(ctx);
         return NPH_OK;                                         // chunks are queued by upload_level_chunks()
     }
     NPH_TRY(nph_reserve(ctx, ctx->d_ev_mean, n_events_total));
-    ctx->ev_mean_resident = true;
     NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_drift.p, hd.data(), sizeof(double) * n_reads, cudaMemcpyHostToDevice, ctx->stream));
     NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_ev_mean.p, ev_mean, sizeof(float) * n_events_total, cudaMemcpyHostToDevice, ctx->stream));
     if (any_drift) {
@@ -324,22 +284,52 @@ int nph_reads_load_impl(nph_ctx* ctx, const nph_read* reads, size_t n_reads,
         NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_level.p, ctx->d_ev_mean.p, sizeof(float) * n_events_total, cudaMemcpyDeviceToDevice, ctx->stream));
     }
     NPH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    nph_reads_resident(ctx);
     return NPH_OK;
 }
 
-int nph_upload_level_chunks(nph_ctx* ctx, const float* ev_mean)
+int upload_level_chunks(nph_ctx* ctx, const float* ev_mean)
 {
     const size_t chunk = ctx->level_chunk_events, total = ctx->n_events_total;
     uint32_t c = 0;
     for (size_t off = 0; off < total; off += chunk, ++c) {
         const size_t n = std::min(chunk, total - off);
         NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_level.p + off, ev_mean + off, sizeof(float) * n, cudaMemcpyHostToDevice, ctx->cstream));
-        NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_progress, ctx->h_progress_vals + c, sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->cstream));
+        NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_progress.p, ctx->h_progress_vals.p + c, sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->cstream));
     }
     return NPH_OK;
 }
 
-void nph_finish_level_upload(nph_ctx* ctx)
+// kmer_ranks != nullptr: ranks (uint32 per k-mer); else seq_codes (uint8 per base) — n_total counts whichever it is
+int jobs_upload_async(nph_ctx* ctx, const uint32_t* kmer_ranks, const uint8_t* seq_codes, size_t n_ranks_total,
+                      const nph_hmm_job* jobs, size_t n_jobs, double indel_bias)
+{
+    if ((!kmer_ranks && !seq_codes) || !jobs) return NPH_ERR_INVALID;
+    NPH_CUDA(ctx, cudaSetDevice(ctx->device));
+    if (!kmer_ranks) NPH_TRY(nph_reserve(ctx, ctx->d_codes, n_ranks_total + 16));
+    else NPH_TRY(nph_reserve(ctx, ctx->d_ranks, n_ranks_total));
+    NPH_TRY(nph_reserve(ctx, ctx->d_jobs, n_jobs));
+    NPH_TRY(nph_reserve(ctx, ctx->d_order, n_jobs));
+    NPH_TRY(nph_reserve(ctx, ctx->d_scores, n_jobs));
+    NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_jobs.p, jobs, sizeof(nph_hmm_job) * n_jobs, cudaMemcpyHostToDevice, ctx->stream));
+    if (!kmer_ranks) NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_codes.p, seq_codes, n_ranks_total, cudaMemcpyHostToDevice, ctx->stream));
+    else NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_ranks.p, kmer_ranks, sizeof(uint32_t) * n_ranks_total, cudaMemcpyHostToDevice, ctx->stream));
+    return nph_upload_read_transitions(ctx, indel_bias);
+}
+
+} // namespace
+
+int nph_oneshot_begin(nph_ctx* ctx, const nph_read* reads, size_t n_reads, const float* ev_mean, const double* ev_start_time,
+                      size_t n_events_total, const std::function<int()>& upload)
+{
+    ctx->levels_inflight = false;
+    NPH_TRY(reads_load_impl(ctx, reads, n_reads, ev_mean, ev_start_time, n_events_total, true));
+    NPH_TRY(upload());
+    if (ctx->levels_inflight) NPH_TRY(upload_level_chunks(ctx, ev_mean));
+    return NPH_OK;
+}
+
+void nph_oneshot_finish(nph_ctx* ctx)
 {
     if (!ctx->levels_inflight) return;
     cudaStreamSynchronize(ctx->cstream);
@@ -347,53 +337,37 @@ void nph_finish_level_upload(nph_ctx* ctx)
     ctx->level_chunk_events = 0;
 }
 
-int nph_reads_load(nph_ctx* ctx, const nph_read* reads, size_t n_reads,
-                   const float* ev_mean, const double* ev_start_time, size_t n_events_total)
-{
-    NPH_TRY(nph_reads_load_impl(ctx, reads, n_reads, ev_mean, ev_start_time, n_events_total, false));
-    ctx->reads_loaded = true;
-    ctx->jobs_loaded = false;
-    ctx->abea_loaded = false;
-    return NPH_OK;
-}
-
-// kmer_ranks != nullptr: ranks (uint32 per k-mer); else seq_codes (uint8 per base) — n_total counts whichever it is
-static int jobs_upload_async(nph_ctx* ctx, const uint32_t* kmer_ranks, const uint8_t* seq_codes, size_t n_ranks_total,
-                             const nph_hmm_job* jobs, size_t n_jobs, double indel_bias)
-{
-    if ((!kmer_ranks && !seq_codes) || !jobs) return NPH_ERR_INVALID;
-    ctx->codes_mode = kmer_ranks == nullptr;
-    NPH_CUDA(ctx, cudaSetDevice(ctx->device));
-
-    // per-read transition pair (2 logf with the host libm, see read_transitions)
-    std::vector<float2>& trans = ctx->h_stage_trans;
-    trans.resize(ctx->n_reads);
-    for (size_t i = 0; i < ctx->n_reads; ++i) trans[i] = read_transitions(ctx->h_events_per_base[i], indel_bias);
-
-    if (ctx->codes_mode) NPH_TRY(nph_reserve(ctx, ctx->d_codes, n_ranks_total + 16));
-    else NPH_TRY(nph_reserve(ctx, ctx->d_ranks, n_ranks_total));
-    NPH_TRY(nph_reserve(ctx, ctx->d_jobs, n_jobs));
-    NPH_TRY(nph_reserve(ctx, ctx->d_order, n_jobs));
-    NPH_TRY(nph_reserve(ctx, ctx->d_trans, ctx->n_reads));
-    NPH_TRY(nph_reserve(ctx, ctx->d_scores, n_jobs));
-    NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_jobs.p, jobs, sizeof(nph_hmm_job) * n_jobs, cudaMemcpyHostToDevice, ctx->stream));
-    if (ctx->codes_mode) NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_codes.p, seq_codes, n_ranks_total, cudaMemcpyHostToDevice, ctx->stream));
-    else NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_ranks.p, kmer_ranks, sizeof(uint32_t) * n_ranks_total, cudaMemcpyHostToDevice, ctx->stream));
-    NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_trans.p, trans.data(), sizeof(float2) * ctx->n_reads, cudaMemcpyHostToDevice, ctx->stream));
-    return NPH_OK;
-}
-
-int nph_jobs_schedule(nph_ctx* ctx, size_t n_jobs, size_t n_ranks_total)
+int nph_jobs_schedule(nph_ctx* ctx, size_t n_jobs, size_t n_ranks_total, NphJobSource src)
 {
     // validate + classify + schedule on the device (hmm_schedule.cu); synchronises the stream once
     uint32_t max_E = 1;
-    NPH_TRY(nph_schedule_hmm_jobs(ctx, n_jobs, n_ranks_total, &max_E));
+    NPH_TRY(nph_schedule_hmm_jobs(ctx, n_jobs, n_ranks_total, src, &max_E));
     NPH_TRY(ensure_flank(ctx, (size_t)max_E + 2));
-    NPH_TRY(nph_reserve(ctx, ctx->d_scratch, nph_hmm_scratch_bytes(ctx, nullptr)));
+    NPH_TRY(nph_reserve(ctx, ctx->d_scratch, nph_hmm_scratch_bytes(ctx)));
     ctx->n_jobs = n_jobs;
     ctx->n_ranks = n_ranks_total;
     ctx->jobs_loaded = true;
     return NPH_OK;
+}
+
+int nph_score_device_jobs(nph_ctx* ctx, size_t n_jobs, size_t n_ranks_total, double indel_bias, const std::function<int()>& emit)
+{
+    ctx->jobs_loaded = false;
+    NPH_TRY(nph_reserve(ctx, ctx->d_jobs, n_jobs));
+    NPH_TRY(nph_reserve(ctx, ctx->d_order, n_jobs));
+    NPH_TRY(nph_reserve(ctx, ctx->d_scores, n_jobs));
+    NPH_TRY(nph_upload_read_transitions(ctx, indel_bias));
+    NPH_TRY(emit());
+    NPH_TRY(nph_jobs_schedule(ctx, n_jobs, n_ranks_total, NphJobSource::DeviceRanks));
+    return nph_launch_hmm_forward(ctx, nullptr);
+}
+
+extern "C" {
+
+int nph_reads_load(nph_ctx* ctx, const nph_read* reads, size_t n_reads,
+                   const float* ev_mean, const double* ev_start_time, size_t n_events_total)
+{
+    return reads_load_impl(ctx, reads, n_reads, ev_mean, ev_start_time, n_events_total, false);
 }
 
 int nph_hmm_jobs_load(nph_ctx* ctx, const uint32_t* kmer_ranks, size_t n_ranks_total,
@@ -403,7 +377,7 @@ int nph_hmm_jobs_load(nph_ctx* ctx, const uint32_t* kmer_ranks, size_t n_ranks_t
     if (n_jobs == 0) { ctx->n_jobs = 0; ctx->classes.clear(); ctx->jobs_loaded = true; return NPH_OK; }   // empty batch: nothing to score
     if (!ctx->reads_loaded) return NPH_ERR_STATE;
     NPH_TRY(jobs_upload_async(ctx, kmer_ranks, nullptr, n_ranks_total, jobs, n_jobs, indel_bias));
-    return nph_jobs_schedule(ctx, n_jobs, n_ranks_total);
+    return nph_jobs_schedule(ctx, n_jobs, n_ranks_total, NphJobSource::HostRanks);
 }
 
 int nph_hmm_jobs_load_seq(nph_ctx* ctx, const uint8_t* seq_codes, size_t n_codes_total,
@@ -414,7 +388,7 @@ int nph_hmm_jobs_load_seq(nph_ctx* ctx, const uint8_t* seq_codes, size_t n_codes
     if (!ctx->reads_loaded) return NPH_ERR_STATE;
     if (!seq_codes) return NPH_ERR_INVALID;
     NPH_TRY(jobs_upload_async(ctx, nullptr, seq_codes, n_codes_total, jobs, n_jobs, indel_bias));
-    return nph_jobs_schedule(ctx, n_jobs, n_codes_total);
+    return nph_jobs_schedule(ctx, n_jobs, n_codes_total, NphJobSource::HostCodes);
 }
 
 int nph_hmm_score(nph_ctx* ctx, float* scores_dev)
@@ -450,22 +424,18 @@ static int hmm_score_batch_impl(nph_ctx* ctx,
     const double t0 = now();
     if (!ctx) return NPH_ERR_INVALID;
     if (n_jobs == 0) return NPH_OK;                              // empty batch
-    // Order of issue matters: small read records + jobs + ranks first (the scheduler needs only those), then the
-    // event levels in chunks on the copy stream; the forward kernels start as soon as the schedule exists and wait
-    // per job on the progress word of the chunk that holds their read (hmm_forward_kernel.cuh).
-    ctx->levels_inflight = false;
-    int rc = nph_reads_load_impl(ctx, reads, n_reads, ev_mean, ev_start_time, n_events_total, true);
-    if (rc == NPH_OK) { ctx->reads_loaded = true; ctx->jobs_loaded = false; ctx->abea_loaded = false; }
+    // the scheduler needs only the read records, jobs and ranks; the forward kernels start as soon as the schedule exists and
+    // wait per job on the progress word of the level chunk that holds their read (hmm_forward_kernel.cuh)
+    int rc = nph_oneshot_begin(ctx, reads, n_reads, ev_mean, ev_start_time, n_events_total,
+                               [&] { return jobs_upload_async(ctx, kmer_ranks, seq_codes, n_ranks_total, jobs, n_jobs, indel_bias); });
     const double t1 = now();
-    if (rc == NPH_OK) rc = jobs_upload_async(ctx, kmer_ranks, seq_codes, n_ranks_total, jobs, n_jobs, indel_bias);
-    if (rc == NPH_OK && ctx->levels_inflight) rc = nph_upload_level_chunks(ctx, ev_mean);
-    if (rc == NPH_OK) rc = nph_jobs_schedule(ctx, n_jobs, n_ranks_total);
+    if (rc == NPH_OK) rc = nph_jobs_schedule(ctx, n_jobs, n_ranks_total, kmer_ranks ? NphJobSource::HostRanks : NphJobSource::HostCodes);
     const double t2 = now();
     if (rc == NPH_OK) rc = nph_hmm_score(ctx, nullptr);
     if (rc == NPH_OK) rc = nph_hmm_scores_fetch(ctx, scores_out, n_jobs);
-    nph_finish_level_upload(ctx);                                // also on error paths: never leave copies in flight
+    nph_oneshot_finish(ctx);                                     // also on error paths: never leave copies in flight
     const double t3 = now();
-    if (timing) fprintf(stderr, "[nph] reads %.2f ms  jobs+schedule %.2f ms  score+fetch %.2f ms\n", t1 - t0, t2 - t1, t3 - t2);
+    if (timing) fprintf(stderr, "[nph] reads+jobs %.2f ms  schedule %.2f ms  score+fetch %.2f ms\n", t1 - t0, t2 - t1, t3 - t2);
     return rc;
 }
 
@@ -522,8 +492,8 @@ int nph_score_set_combine(const float* scores, size_t n_groups, uint32_t n_alt, 
 int nph_last_kernel_ms(nph_ctx* ctx, float* ms_out, int* launches_out)
 {
     if (!ctx || !ms_out) return NPH_ERR_INVALID;
-    if (!ctx->timing_valid) return NPH_ERR_STATE;
-    if (ctx->timing_valid == 2) *ms_out = ctx->staged_ms;
+    if (ctx->timing == nph_ctx::Timing::None) return NPH_ERR_STATE;
+    if (ctx->timing == nph_ctx::Timing::Staged) *ms_out = ctx->staged_ms;
     else {
         NPH_CUDA(ctx, cudaEventSynchronize(ctx->ev1));
         NPH_CUDA(ctx, cudaEventElapsedTime(ms_out, ctx->ev0, ctx->ev1));

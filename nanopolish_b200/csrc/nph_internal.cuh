@@ -6,6 +6,8 @@
 #include <string>
 #include <vector>
 #include <algorithm>
+#include <functional>
+#include <utility>
 #include "../../include/nph.h"
 
 #define NPH_LOGSUM_TBL 16000        // ref: p7_LOGSUM_TBL, src/common/logsum.h:20
@@ -28,20 +30,35 @@ struct HmmConsts {
     float log_inv_sqrt_2pi;
 };
 
-struct DevModel {
-    double* mean = nullptr;
-    double* stdv = nullptr;
-    double* log_stdv = nullptr;
-    uint32_t n_states = 0, k = 0, alphabet_size = 0;
-};
-
 // Device-side view of the models for kernels (array of pointers)
 struct DevModelView { const double* mean; const double* stdv; const double* log_stdv; uint32_t n_states; uint16_t k; uint16_t alphabet_size; };
 
+// Device memory that frees itself: move-only, released when the owner (the context, a model) goes away.
 template <typename T>
 struct DevBuf {
     T* p = nullptr;
     size_t cap = 0;   // elements
+    DevBuf() = default;
+    DevBuf(DevBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+    DevBuf& operator=(DevBuf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); return *this; }
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { if (p) cudaFree(p); }
+};
+
+// Page-locked host memory that frees itself.
+template <typename T>
+struct PinnedBuf {
+    T* p = nullptr;
+    PinnedBuf() = default;
+    PinnedBuf(const PinnedBuf&) = delete;
+    PinnedBuf& operator=(const PinnedBuf&) = delete;
+    ~PinnedBuf() { if (p) cudaFreeHost(p); }
+};
+
+struct DevModel {
+    DevBuf<double> mean, stdv, log_stdv;
+    uint32_t n_states = 0, k = 0, alphabet_size = 0;
 };
 
 struct nph_ctx {
@@ -52,7 +69,7 @@ struct nph_ctx {
     std::string last_error;
 
     // constant tables
-    float* d_logsum = nullptr;       // NPH_TBL_SMEM floats
+    DevBuf<float> d_logsum;          // NPH_TBL_SMEM floats
     DevBuf<float> d_flank;           // clip-penalty table, grown on demand
     std::vector<float> h_flank;
     HmmConsts consts;
@@ -71,15 +88,11 @@ struct nph_ctx {
     std::vector<double> h_events_per_base;
     std::vector<uint32_t> h_read_n_events;
     bool reads_loaded = false;
-    bool ev_mean_resident = false;   // d_ev_mean holds this batch's raw event means (false after the pipelined one-shot score, which fills d_level only)
 
     // resident HMM jobs
     size_t n_jobs = 0, n_ranks = 0;
     DevBuf<uint32_t> d_ranks;
     DevBuf<uint8_t> d_codes;         // jobs loaded through the *_seq calls: base codes instead of k-mer ranks (jobs' rank_off index this)
-    bool codes_mode = false;
-    bool jobs_trusted = false;       // the resident jobs and their ranks were written by a kernel of ours (methylation.cu, variants.cu): the
-                                     // scheduler validates the jobs' read / event ranges but does not walk their ranks again
     DevBuf<uint64_t> d_rank_base;    // base-code jobs: where each job's ranks start in d_ranks (hmm_schedule.cu)
     DevBuf<nph_hmm_job> d_jobs;
     DevBuf<float2> d_trans;          // per read: (lp_mm_self, lp_mm_next)
@@ -158,15 +171,15 @@ struct nph_ctx {
     cudaStream_t side[4] = {nullptr, nullptr, nullptr, nullptr};
     cudaEvent_t ev_fork = nullptr, ev_join[4] = {nullptr, nullptr, nullptr, nullptr};
     int last_launches = 0;
-    int timing_valid = 0;            // 0 none, 1 = ev0..ev1, 2 = staged_ms (a call with host round trips between its kernels)
+    enum class Timing { None, Events, Staged } timing = Timing::None;   // set by nph_timing_events / nph_timing_staged
     float staged_ms = 0.0f;
 
     // pipelined level upload of the one-shot call: copy stream, progress word polled by the forward kernel
     static const int kLevelChunks = 8;
     cudaStream_t cstream = nullptr;
     cudaEvent_t ev_reset = nullptr;
-    uint32_t* d_progress = nullptr;          // number of level chunks that have landed
-    uint32_t* h_progress_vals = nullptr;     // pinned {1, 2, ...}: sources of the progress writes
+    DevBuf<uint32_t> d_progress;             // number of level chunks that have landed
+    PinnedBuf<uint32_t> h_progress_vals;     // {1, 2, ...}: sources of the progress writes
     size_t level_chunk_events = 0;           // 0 = levels fully resident, kernels do not poll
     bool levels_inflight = false;
     std::vector<DevRead> h_stage_reads;      // host staging that must outlive async copies
@@ -178,35 +191,111 @@ struct nph_ctx {
 
 int nph_set_cuda_error(nph_ctx* ctx, cudaError_t e, const char* what);
 #define NPH_CUDA(ctx, call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) return nph_set_cuda_error((ctx), e__, #call); } while (0)
+#define NPH_TRY(expr) do { int rc__ = (expr); if (rc__ != NPH_OK) return rc__; } while (0)
 
+// Grows b to hold at least n elements (with room for n / 8 + 16 more); the old contents are not kept, and the old
+// allocation is freed before the new one is made.
 template <typename T>
-int nph_reserve(nph_ctx* ctx, DevBuf<T>& b, size_t n);
+int nph_reserve(nph_ctx* ctx, DevBuf<T>& b, size_t n)
+{
+    if (n <= b.cap && b.p) return NPH_OK;
+    if (b.p) { NPH_CUDA(ctx, cudaFree(b.p)); b.p = nullptr; b.cap = 0; }
+    const size_t want = n + n / 8 + 16;
+    NPH_CUDA(ctx, cudaMalloc((void**)&b.p, want * sizeof(T)));
+    b.cap = want;
+    return NPH_OK;
+}
+
+// One scratch layout.  A layout function lists every slice once, in order, through take(); run over an arena without a
+// base it only adds up the bytes, run over a reserved buffer it hands out the pointers.  Every slice starts on 256 bytes.
+struct NphArena {
+    uint8_t* base = nullptr;
+    size_t used = 0;
+    template <typename T> T* take(size_t n)
+    {
+        T* q = base ? reinterpret_cast<T*>(base + used) : nullptr;
+        used += (sizeof(T) * n + 255) / 256 * 256;
+        return q;
+    }
+};
+template <typename Layout>
+size_t nph_layout_bytes(Layout&& layout) { NphArena a; layout(a); return a.used; }
+// reserve buf for the layout, then carve it
+template <typename Layout>
+int nph_carve(nph_ctx* ctx, DevBuf<uint8_t>& buf, Layout&& layout)
+{
+    NPH_TRY(nph_reserve(ctx, buf, nph_layout_bytes(layout)));
+    NphArena a{buf.p};
+    layout(a);
+    return NPH_OK;
+}
+
+// Indices 0 .. n-1 by key, largest first; equal keys keep index order.
+template <typename K>
+std::vector<uint32_t> nph_longest_first(const std::vector<K>& key)
+{
+    std::vector<uint32_t> order(key.size());
+    for (size_t i = 0; i < order.size(); ++i) order[i] = (uint32_t)i;
+    std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return key[a] > key[b]; });
+    return order;
+}
+
+// What nph_last_kernel_ms reports: the time between ctx->ev0 and ctx->ev1, or the summed device time of a call with host
+// round trips between its kernels.
+inline void nph_timing_events(nph_ctx* ctx, int launches) { ctx->last_launches = launches; ctx->timing = nph_ctx::Timing::Events; }
+inline void nph_timing_staged(nph_ctx* ctx, float ms, int launches)
+{
+    ctx->staged_ms = ms; ctx->last_launches = launches; ctx->timing = nph_ctx::Timing::Staged;
+}
+
+// A new read batch is resident: the HMM and ABEA jobs of the previous one no longer apply.
+inline void nph_reads_resident(nph_ctx* ctx) { ctx->reads_loaded = true; ctx->jobs_loaded = false; ctx->abea_loaded = false; }
+
+#ifdef __CUDACC__
+// get_scaled_gaussian_from_pore_model_state (ref: src/nanopolish_squiggle_read.h:217-226) of k-mer rank r, formed in FP64 and
+// narrowed: {mu', sigma', log(1/sqrt(2pi)) - log sigma', RN(1/sigma')}
+__device__ __forceinline__ float4 nph_scaled_gaussian(const DevModelView& mv, const DevRead& rd, uint32_t r, float log_inv_sqrt_2pi)
+{
+    const float mu = (float)__dadd_rn(__dmul_rn(rd.scale, mv.mean[r]), rd.shift);
+    const float sd = (float)__dmul_rn(mv.stdv[r], rd.var);
+    const float lsd = (float)__dadd_rn(mv.log_stdv[r], rd.log_var);
+    return make_float4(mu, sd, __fsub_rn(log_inv_sqrt_2pi, lsd), __frcp_rn(sd));
+}
+#endif
+
+// where the HMM jobs in ctx->d_jobs and their ranks come from
+enum class NphJobSource {
+    HostRanks,      // k-mer ranks from the caller: every rank is checked against the model
+    HostCodes,      // base codes from the caller (the *_seq calls): every code is checked, then turned into ranks
+    DeviceRanks,    // ranks a kernel of ours wrote (call-methylation, variant screening): job ranges are checked, ranks are not walked
+};
 
 // kernels (defined in hmm_forward.cu / abea.cu)
 int nph_launch_read_prologue(nph_ctx* ctx);
 int nph_launch_hmm_forward(nph_ctx* ctx, float* scores_dev);
-size_t nph_hmm_scratch_bytes(const nph_ctx* ctx, int* warps_total_out);
+size_t nph_hmm_scratch_bytes(const nph_ctx* ctx);
 int nph_launch_abea(nph_ctx* ctx);
-int nph_schedule_hmm_jobs(nph_ctx* ctx, size_t n_jobs, size_t n_ranks_total, uint32_t* max_E_out);
+int nph_schedule_hmm_jobs(nph_ctx* ctx, size_t n_jobs, size_t n_ranks_total, NphJobSource src, uint32_t* max_E_out);
 // per-read (lp_mm_self, lp_mm_next) of the resident reads into ctx->d_trans (host libm, like calculate_transitions)
 int nph_upload_read_transitions(nph_ctx* ctx, double indel_bias);
 // compact event alignments -> event index per reference base (methylation.cu): dense[ref_off + o] (INT32_MIN: no entry), first_valid[record]
 int nph_expand_event_maps(nph_ctx* ctx, const int16_t* d_deltas, const int32_t* d_first_event, const nph_meth_record* d_records, uint32_t n_records,
                           int32_t* d_dense, int32_t* d_first_valid);
-extern "C" {   // defined inside nph_api.cu's extern "C" block (internal all the same: not in include/nph.h)
 // validate + classify + schedule the n_jobs jobs already sitting in ctx->d_jobs / d_ranks (one stream sync), size the scratch
-int nph_jobs_schedule(nph_ctx* ctx, size_t n_jobs, size_t n_ranks_total);
-// nph_reads_load's body; pipelined = true (one-shot calls) leaves the event levels to nph_upload_level_chunks, which queues them
-// on the copy stream behind progress words the forward kernel polls (ctx->levels_inflight says whether that path was taken)
-int nph_reads_load_impl(nph_ctx* ctx, const nph_read* reads, size_t n_reads, const float* ev_mean, const double* ev_start_time, size_t n_events_total, bool pipelined);
-int nph_upload_level_chunks(nph_ctx* ctx, const float* ev_mean);
-// after a one-shot call: wait for the copy stream and leave the pipelined mode
-void nph_finish_level_upload(nph_ctx* ctx);
-}
+int nph_jobs_schedule(nph_ctx* ctx, size_t n_jobs, size_t n_ranks_total, NphJobSource src);
+// Scores n_jobs jobs that emit() writes into ctx->d_jobs (ranks already in ctx->d_ranks, written by a kernel of ours): reserves
+// the job, order and score arrays, uploads the read transitions, runs emit(), schedules and launches the forward kernels.
+int nph_score_device_jobs(nph_ctx* ctx, size_t n_jobs, size_t n_ranks_total, double indel_bias, const std::function<int()>& emit);
+// One-shot calls (read batch, work and results in one call).  Begin: read records on the main stream, then upload() (the
+// jobs or records), then the event levels in chunks on the copy stream behind progress words the forward kernel polls —
+// enumeration and scheduling run while the levels still cross PCIe.  Finish, on every path: wait for the copy stream.
+int nph_oneshot_begin(nph_ctx* ctx, const nph_read* reads, size_t n_reads, const float* ev_mean, const double* ev_start_time,
+                      size_t n_events_total, const std::function<int()>& upload);
+void nph_oneshot_finish(nph_ctx* ctx);
 
 // ---- device-level pieces of the raw-read prologue (event_detect.cu, squiggle_prep.cu, abea.cu), chained by
 // load_from_raw.cu without leaving the device.  Inputs named d_* are device pointers; everything runs on ctx->stream.
-size_t nph_ed_scratch_bytes(size_t n_samples_total, size_t n_reads, size_t events_total);
+size_t nph_ed_scratch_bytes(size_t n_reads, size_t events_total);
 int nph_detect_events_device(nph_ctx* ctx, const float* d_raw, size_t n_samples_total, const nph_raw_read* reads, size_t n_reads,
                              const nph_event_params* params, uint8_t* scratch, size_t events_total,
                              nph_event** d_events_out, uint32_t** d_n_events_out, std::vector<uint32_t>& h_n_events, int* launches_out);

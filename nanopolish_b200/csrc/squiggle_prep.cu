@@ -16,8 +16,6 @@
 #include <cstdlib>
 #include <cstring>
 
-#define NPH_TRY(expr) do { int rc__ = (expr); if (rc__ != NPH_OK) return rc__; } while (0)
-
 namespace {
 
 constexpr unsigned kFull = 0xffffffffu;
@@ -363,7 +361,14 @@ __global__ void __launch_bounds__(kCalWarps * 32) recalibrate_kernel(const CalPa
     }
 }
 
-inline size_t al256(size_t v) { return (v + 255) / 256 * 256; }
+// the trim's scratch: read records, per-read chunk offsets, the chunks' MADs, the ranges
+void trim_layout(NphArena& a, size_t n_reads, uint64_t n_chunks, nph_raw_read** reads, uint64_t** mad_off, TrimParams& p)
+{
+    *reads = a.take<nph_raw_read>(n_reads);
+    *mad_off = a.take<uint64_t>(n_reads);
+    p.mad = a.take<float>(n_chunks + 1);
+    p.out = a.take<nph_raw_range>(n_reads);
+}
 
 } // namespace
 
@@ -371,8 +376,8 @@ size_t nph_trim_scratch_bytes(const nph_raw_read* reads, size_t n_reads, int32_t
 {
     uint64_t n_chunks = 0;
     for (size_t i = 0; i < n_reads; ++i) n_chunks += reads[i].n_samples / (uint32_t)varseg_chunk;
-    return al256(sizeof(nph_raw_read) * n_reads) + al256(sizeof(uint64_t) * n_reads) + al256(sizeof(float) * (n_chunks + 1)) +
-           al256(sizeof(nph_raw_range) * n_reads);
+    nph_raw_read* r; uint64_t* o; TrimParams p;
+    return nph_layout_bytes([&](NphArena& a) { trim_layout(a, n_reads, n_chunks, &r, &o, p); });
 }
 
 // trim_and_segment_raw over reads whose samples are on the device; the ranges come back to the host (one sync).
@@ -389,12 +394,11 @@ int nph_trim_device(nph_ctx* ctx, const float* d_raw, size_t n_samples_total, co
         mad_off[i] = n_chunks;
         n_chunks += reads[i].n_samples / (uint32_t)varseg_chunk;
     }
-    uint8_t* base = scratch;
     TrimParams p{};
-    nph_raw_read* d_reads = reinterpret_cast<nph_raw_read*>(base); base += al256(sizeof(nph_raw_read) * n_reads);
-    uint64_t* d_off = reinterpret_cast<uint64_t*>(base); base += al256(sizeof(uint64_t) * n_reads);
-    p.mad = reinterpret_cast<float*>(base); base += al256(sizeof(float) * (n_chunks + 1));
-    p.out = reinterpret_cast<nph_raw_range*>(base);
+    nph_raw_read* d_reads;
+    uint64_t* d_off;
+    NphArena arena{scratch};
+    trim_layout(arena, n_reads, n_chunks, &d_reads, &d_off, p);
     p.raw = d_raw; p.reads = d_reads; p.mad_off = d_off; p.n_reads = (uint32_t)n_reads;
     p.trim_start = trim_start; p.trim_end = trim_end; p.chunk = varseg_chunk; p.perc = varseg_thresh;
     NPH_CUDA(ctx, cudaMemcpyAsync(d_reads, reads, sizeof(nph_raw_read) * n_reads, cudaMemcpyHostToDevice, ctx->stream));
@@ -428,16 +432,18 @@ extern "C" int nph_trim_raw_batch(nph_ctx* ctx, const float* raw, size_t n_sampl
     if (!raw || !reads || !ranges_out) return NPH_ERR_INVALID;
     if (varseg_chunk < 2) return NPH_ERR_INVALID;
     NPH_CUDA(ctx, cudaSetDevice(ctx->device));
-    const size_t b_raw = al256(sizeof(float) * n_samples_total);
-    NPH_TRY(nph_reserve(ctx, ctx->d_abea_scratch, b_raw + nph_trim_scratch_bytes(reads, n_reads, varseg_chunk)));
+    float* d_raw;
+    uint8_t* scratch;
+    NPH_TRY(nph_carve(ctx, ctx->d_abea_scratch, [&](NphArena& a) {
+        d_raw = a.take<float>(n_samples_total);
+        scratch = a.take<uint8_t>(nph_trim_scratch_bytes(reads, n_reads, varseg_chunk));
+    }));
     ctx->abea_loaded = false;       // the arena is shared with the ABEA trace
-    float* d_raw = reinterpret_cast<float*>(ctx->d_abea_scratch.p);
     NPH_CUDA(ctx, cudaMemcpyAsync(d_raw, raw, sizeof(float) * n_samples_total, cudaMemcpyHostToDevice, ctx->stream));
     NPH_CUDA(ctx, cudaEventRecord(ctx->ev0, ctx->stream));
     NPH_TRY(nph_trim_device(ctx, d_raw, n_samples_total, reads, n_reads, trim_start, trim_end, varseg_chunk, varseg_thresh,
-                            ctx->d_abea_scratch.p + b_raw, ranges_out));
-    ctx->last_launches = 1;
-    ctx->timing_valid = true;
+                            scratch, ranges_out));
+    nph_timing_events(ctx, 1);
     return NPH_OK;
 }
 
@@ -461,23 +467,20 @@ extern "C" int nph_recalibrate_batch(nph_ctx* ctx, const nph_read* reads, size_t
     for (size_t i = 0; i < n_ranks_total; ++i)
         if (kmer_ranks[i] >= n_states) return NPH_ERR_INVALID;
     NPH_CUDA(ctx, cudaSetDevice(ctx->device));
-    const size_t b_ev = al256(sizeof(float) * n_events_total), b_reads = al256(sizeof(nph_read) * n_reads);
-    const size_t b_rk = al256(sizeof(uint32_t) * n_ranks_total), b_jobs = al256(sizeof(nph_abea_job) * n_jobs);
-    const size_t b_res = al256(sizeof(nph_abea_result) * n_jobs), b_pairs = al256(sizeof(nph_aligned_pair) * (pairs_total + 1));
-    const size_t b_b2e = al256(sizeof(nph_event_range) * n_ranks_total), b_cal = al256(sizeof(nph_calibration) * n_jobs);
-    NPH_TRY(nph_reserve(ctx, ctx->d_abea_scratch, b_ev + b_reads + b_rk + b_jobs + b_res + b_pairs + b_b2e + b_cal + 256));
-    ctx->abea_loaded = false;
-    uint8_t* base = ctx->d_abea_scratch.p;
     NphCalArgs a{};
-    float* d_ev = reinterpret_cast<float*>(base); base += b_ev;
-    nph_read* d_reads = reinterpret_cast<nph_read*>(base); base += b_reads;
-    uint32_t* d_rk = reinterpret_cast<uint32_t*>(base); base += b_rk;
-    nph_abea_job* d_jobs = reinterpret_cast<nph_abea_job*>(base); base += b_jobs;
-    nph_abea_result* d_res = reinterpret_cast<nph_abea_result*>(base); base += b_res;
-    nph_aligned_pair* d_pairs = reinterpret_cast<nph_aligned_pair*>(base); base += b_pairs;
-    a.b2e = reinterpret_cast<nph_event_range*>(base); base += b_b2e;
-    a.out = reinterpret_cast<nph_calibration*>(base); base += b_cal;
-    a.bad_input = reinterpret_cast<int*>(base);
+    float* d_ev; nph_read* d_reads; uint32_t* d_rk; nph_abea_job* d_jobs; nph_abea_result* d_res; nph_aligned_pair* d_pairs;
+    NPH_TRY(nph_carve(ctx, ctx->d_abea_scratch, [&](NphArena& ar) {
+        d_ev = ar.take<float>(n_events_total);
+        d_reads = ar.take<nph_read>(n_reads);
+        d_rk = ar.take<uint32_t>(n_ranks_total);
+        d_jobs = ar.take<nph_abea_job>(n_jobs);
+        d_res = ar.take<nph_abea_result>(n_jobs);
+        d_pairs = ar.take<nph_aligned_pair>(pairs_total + 1);
+        a.b2e = ar.take<nph_event_range>(n_ranks_total);
+        a.out = ar.take<nph_calibration>(n_jobs);
+        a.bad_input = ar.take<int>(1);
+    }));
+    ctx->abea_loaded = false;
     a.ev_mean = d_ev; a.reads = d_reads; a.model_id = model_id; a.ranks = d_rk; a.jobs = d_jobs;
     a.results = d_res; a.pairs = d_pairs; a.n_jobs = (uint32_t)n_jobs;
     NPH_CUDA(ctx, cudaMemcpyAsync(d_ev, ev_mean, sizeof(float) * n_events_total, cudaMemcpyHostToDevice, ctx->stream));
@@ -489,8 +492,7 @@ extern "C" int nph_recalibrate_batch(nph_ctx* ctx, const nph_read* reads, size_t
     NPH_CUDA(ctx, cudaEventRecord(ctx->ev0, ctx->stream));
     NPH_TRY(nph_launch_recalibrate(ctx, a));
     NPH_CUDA(ctx, cudaEventRecord(ctx->ev1, ctx->stream));
-    ctx->last_launches = 1;
-    ctx->timing_valid = true;
+    nph_timing_events(ctx, 1);
     int bad = 0;
     NPH_CUDA(ctx, cudaMemcpyAsync(calibrations_out, a.out, sizeof(nph_calibration) * n_jobs, cudaMemcpyDeviceToHost, ctx->stream));
     if (base_to_event_out)

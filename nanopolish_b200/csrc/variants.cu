@@ -25,8 +25,6 @@
 #include <string>
 #include <vector>
 
-#define NPH_TRY(expr) do { int rc__ = (expr); if (rc__ != NPH_OK) return rc__; } while (0)
-
 int nph_launch_hmm_forward(nph_ctx* ctx, float* scores_dev);
 
 namespace {
@@ -451,8 +449,6 @@ extern "C" int nph_screen_run(nph_ctx* ctx)
     const long long n_thr = (long long)n_pos * kSeqs;
     var_ranks_kernel<<<(unsigned)((n_thr + kBlock - 1) / kBlock), kBlock, 0, st>>>(d, m.d_ref.p, ctx->d_ranks.p, state, m.d_pos_off.p);
     NPH_CUDA(ctx, cudaGetLastError());
-    NPH_TRY(nph_upload_read_transitions(ctx, m.indel_bias));
-    ctx->codes_mode = false;
     // what the same screening costs without the early exit: every read of every candidate (+ the base per candidate, as the reference scores it)
     // counted on the host side from the totals: sum over positions of reads x (1 + candidates) — filled at the end from the state
     unsigned long long* d_events = reinterpret_cast<unsigned long long*>(m.d_state.p + sizeof(PosState) * (size_t)n_pos);
@@ -469,17 +465,12 @@ extern "C" int nph_screen_run(nph_ctx* ctx)
         NPH_CUDA(ctx, cudaMemcpyAsync(&n_jobs, job_off + n_pos, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
         NPH_CUDA(ctx, cudaStreamSynchronize(st));                         // read-back: the round's job count
         if (n_jobs == 0) break;
-        NPH_TRY(nph_reserve(ctx, ctx->d_jobs, (size_t)n_jobs));
-        NPH_TRY(nph_reserve(ctx, ctx->d_order, (size_t)n_jobs));
-        NPH_TRY(nph_reserve(ctx, ctx->d_scores, (size_t)n_jobs));
-        var_emit_kernel<<<pgrid, kBlock, 0, st>>>(d, state, m.d_pos_off.p, pos_reads, m.d_records.p, job_off, ctx->d_jobs.p, d_events);
-        NPH_CUDA(ctx, cudaGetLastError());
-        ctx->jobs_loaded = false;
-        ctx->jobs_trusted = true;                                         // var_ranks_kernel wrote the pool: the scheduler need not walk it every round
-        const int rc_sched = nph_jobs_schedule(ctx, (size_t)n_jobs, pool); // validation + schedule (one more read-back)
-        ctx->jobs_trusted = false;
-        NPH_TRY(rc_sched);
-        NPH_TRY(nph_launch_hmm_forward(ctx, nullptr));
+        // var_emit_kernel writes the round's jobs over the pool var_ranks_kernel wrote; the schedule is one more read-back
+        NPH_TRY(nph_score_device_jobs(ctx, (size_t)n_jobs, pool, m.indel_bias, [&]() -> int {
+            var_emit_kernel<<<pgrid, kBlock, 0, st>>>(d, state, m.d_pos_off.p, pos_reads, m.d_records.p, job_off, ctx->d_jobs.p, d_events);
+            NPH_CUDA(ctx, cudaGetLastError());
+            return NPH_OK;
+        }));
         NPH_CUDA(ctx, cudaMemsetAsync(d_any, 0, sizeof(unsigned int), st));
         var_accumulate_kernel<<<pgrid, kBlock, 0, st>>>(d, state, job_off, ctx->d_scores.p, d_any, m.d_pos_off.p, pos_reads, d_events + 2);
         NPH_CUDA(ctx, cudaGetLastError());
@@ -493,7 +484,7 @@ extern "C" int nph_screen_run(nph_ctx* ctx)
     NPH_CUDA(ctx, cudaStreamSynchronize(st));
     m.n_scored_events = ev[0];
     m.n_reference_events = ev[2];
-    ctx->staged_ms = kernel_ms_total; ctx->timing_valid = 2; ctx->last_launches = launches_total;
+    nph_timing_staged(ctx, kernel_ms_total, launches_total);
     m.ran = true;
     return NPH_OK;
 }
@@ -520,14 +511,15 @@ extern "C" int nph_screen_fetch(nph_ctx* ctx, double* qualities_out, uint32_t* n
     VarDev d;
     NPH_TRY(make_dev(ctx, m.params, m.n_ref, d));
     const uint32_t n_pos = (uint32_t)m.n_pos;
-    // outputs staged in the (now idle) score buffer region: 9 doubles + 1 uint32 per position
-    DevBuf<uint8_t>& scratch = ctx->d_prep;
+    // outputs staged in the (now idle) prologue buffer: per position the slot qualities, reference rows and read count
     const size_t b_q = sizeof(double) * NPH_SCREEN_SLOTS * (size_t)n_pos, b_n = sizeof(uint32_t) * (size_t)n_pos;
     const size_t b_r = sizeof(unsigned long long) * (size_t)n_pos;
-    NPH_TRY(nph_reserve(ctx, scratch, b_q + b_r + b_n + 256));
-    double* d_q = reinterpret_cast<double*>(scratch.p);
-    unsigned long long* d_r = reinterpret_cast<unsigned long long*>(scratch.p + b_q);
-    uint32_t* d_n = reinterpret_cast<uint32_t*>(scratch.p + b_q + b_r);
+    double* d_q; unsigned long long* d_r; uint32_t* d_n;
+    NPH_TRY(nph_carve(ctx, ctx->d_prep, [&](NphArena& a) {
+        d_q = a.take<double>(NPH_SCREEN_SLOTS * (size_t)n_pos);
+        d_r = a.take<unsigned long long>(n_pos);
+        d_n = a.take<uint32_t>(n_pos);
+    }));
     var_output_kernel<<<(n_pos + kBlock - 1) / kBlock, kBlock, 0, ctx->stream>>>(d, reinterpret_cast<const PosState*>(m.d_state.p), m.d_pos_off.p, d_q, d_n, d_r);
     NPH_CUDA(ctx, cudaGetLastError());
     NPH_CUDA(ctx, cudaMemcpyAsync(qualities_out, d_q, b_q, cudaMemcpyDeviceToHost, ctx->stream));
