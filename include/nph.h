@@ -447,7 +447,7 @@ int nph_methylation_batch_compact_tsv(nph_ctx* ctx,
  * threshold get jobs in the next round (a candidate that leaves it mid-round ignores the rest of that round, exactly like the
  * sequential loop).  Window enumeration, the k-mer ranks of the ten sequences per position and strand, job emission, the
  * forward scores and the accumulation all run on the device; the host drives the rounds (one count read-back per round).
- * No methylation alternatives (opt::methylation_types empty, the default).
+ * No methylation alternatives (opt::methylation_types empty, the default); nph_screen_edits_batch_methylation below takes -q types.
  * Records: nph_meth_record with ref_off = offset of the record's compact event alignment in event_deltas[] (ref_len entries,
  * entry o <-> reference position ref_start_pos + o; NPH_METH_NO_PAIR / steps as in nph_methylation_batch_compact),
  * pair_off / n_pairs unused, model_id = the read's base model.  Record order = AlignmentDB's m_event_records order.
@@ -489,6 +489,39 @@ int nph_screen_counts(nph_ctx* ctx, uint32_t* n_rounds_out, uint64_t* n_jobs_out
                       uint64_t* n_reference_events_out);
 /* reference_rows_out (optional, one per position): the position's share of nph_screen_counts' n_reference_events */
 int nph_screen_fetch(nph_ctx* ctx, double* qualities_out, uint32_t* n_reads_out, uint64_t* reference_rows_out);
+
+/* Methylation-aware screening (`variants -q cpg`, `-q dam,dcm`): opt::methylation_types non-empty.  Every sequence the screening
+ * scores (the base window and its nine edited versions) becomes profile_hmm_score_set's set (src/common/nanopolish_variant.cpp:158-178):
+ * the sequence itself, then for each type in -q order Alphabet::methylate of it where that changes it (sites matched on the
+ * window's characters: an N never completes one), scored against the read's model of that type; the set is folded with log(n)
+ * penalties through the table log-sum.  An edit can create or destroy a site, so a candidate and its base can have different
+ * numbers of alternatives.  Qualities are those of score_variant_thresholded(..., methylation_types); n_reference_events counts
+ * (n(base) + n(variant)) x E per (candidate, read) added, n(s) = 1 + alternatives of s.  With n_types = 0 this is nph_screen_*. */
+#define NPH_SCREEN_MAX_TYPES 4
+typedef struct {
+    uint32_t n_types;                                  /* opt::methylation_types.size() */
+    uint32_t reserved;
+    nph_meth_params alphabets[NPH_SCREEN_MAX_TYPES];   /* get_alphabet_by_name(type t), in -q order; only k, alphabet_size, bases, complements,
+                                                          n_sites, site_len and the three site arrays are read */
+} nph_screen_methylation;                              /* 616 bytes */
+/* nph_screen_load plus the types.  alt_model_ids: n_records x n_types, entry r * n_types + t = read->get_model(strand, type t) of
+ * record r.  NPH_ERR_INVALID: n_types > NPH_SCREEN_MAX_TYPES, a malformed alphabet, an alphabet whose k is not params.k, a model id out of
+ * range or whose model's k / alphabet size differ from its alphabet's; NPH_ERR_UNSUPPORTED: recognition sites that can overlap each
+ * other.  A refused load leaves nph_screen_run at NPH_ERR_STATE.  nph_screen_run / _counts / _fetch serve both loads. */
+int nph_screen_load_methylation(nph_ctx* ctx, const char* ref_bases, size_t n_ref_bases, const int16_t* event_deltas, size_t n_deltas_total,
+                                const int32_t* first_event, const nph_meth_record* records, size_t n_records,
+                                const nph_screen_params* params, double indel_bias,
+                                const nph_screen_methylation* meth, const uint32_t* alt_model_ids);
+/* One-shot form: nph_screen_edits_batch with the types. */
+int nph_screen_edits_batch_methylation(nph_ctx* ctx,
+                                       const nph_read* reads, size_t n_reads,
+                                       const float* ev_mean, const double* ev_start_time, size_t n_events_total,
+                                       const char* ref_bases, size_t n_ref_bases,
+                                       const int16_t* event_deltas, size_t n_deltas_total, const int32_t* first_event,
+                                       const nph_meth_record* records, size_t n_records,
+                                       const nph_screen_params* params, double indel_bias,
+                                       const nph_screen_methylation* meth, const uint32_t* alt_model_ids,
+                                       double* qualities_out, uint32_t* n_reads_out, uint64_t* n_scored_events_out);
 
 /* ---- event detection (section 8f N4: the step before ABEA) --------------------------------------
  * scrappie's detect_events as load_from_raw calls it: t-statistics over two windows on prefix sums, a short/long

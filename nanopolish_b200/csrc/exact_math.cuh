@@ -2,6 +2,7 @@
 // bit-identical to the reference's IEEE-754 arithmetic while costing as few issue slots as possible.
 #pragma once
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
 
 #ifndef NPH_LOGSUM_CUT
@@ -94,6 +95,25 @@ __device__ __forceinline__ float lsum_sat(float a, float b, const LogsumTable tb
     const float d = __fsub_rn(a, b);
     const float t = __saturatef(__fmul_rn(fabsf(d), 0.06103515625f));
     return lsum_lookup(mx, __fadd_rd(t, 512.0f), tb);
+}
+
+// ---- profile_hmm_score_set's fold of one group of scores (ref: src/hmm/nanopolish_profile_hmm.cpp:32-56) --------------------
+// s[0] is the nucleotide sequence's score, s[1 .. n-1] those of its methylated alternatives; pen = log(n) from host libm.
+//     score = s[0] - pen;  per alternative: add_logs((float)score, (float)(s[i] - pen)) -> score (double)
+// with add_logs the table log-sum of src/common/logsum.h:55-66.  tbl needs the reference's entries below NPH_LOGSUM_CUT (the host's
+// own table or the context's device copy).  Every operation is a single IEEE operation (no multiply feeds an add), so host and
+// device round alike.  !(d < 15.7f) also catches NaN / inf differences (a NaN or +inf score): no out-of-range table index.
+__host__ __device__ inline float nph_score_set_fold(const float* s, uint32_t n, double pen, const float* tbl)
+{
+    double score = (double)s[0] - pen;
+    for (uint32_t i = 1; i < n; ++i) {
+        const double alt = (double)s[i] - pen;
+        const float a = (float)score, b = (float)alt;
+        const float mx = a > b ? a : b, mn = a < b ? a : b;
+        const float d = mx - mn;
+        score = (mn == -INFINITY || !(d < 15.7f)) ? mx : mx + tbl[(int)(d * 1000.f)];
+    }
+    return (float)score;
 }
 
 // ---- correctly rounded float division with a precomputed reciprocal --------------------------

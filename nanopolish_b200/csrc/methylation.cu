@@ -23,6 +23,7 @@
 // then hmm_schedule.cu + the forward kernels run unchanged, and meth_fill_kernel copies the two scores of each group
 // into its site record.  The host sees O(records) work only.
 #include "nph_internal.cuh"
+#include "meth_dev.cuh"
 #include "tsv_format.cuh"
 #include <algorithm>
 #include <cstring>
@@ -48,30 +49,6 @@ struct MethSummary {
     int error;                // 0, or 1 + index of a record with a window shorter than k
     int pad;
 };
-
-// the alphabet and site tables as the kernels use them (ranks, not characters)
-struct MethDev {
-    int32_t min_separation, min_flank, max_span, min_event_span, region_start, region_end;
-    uint32_t k, asize, n_sites, site_len;
-    uint8_t rank_of[256];                                              // Alphabet::rank (unknown symbols rank 0)
-    uint8_t comp_rank_of[256];                                         // rank(complement(symbol))
-    char    site[NPH_METH_MAX_SITES][NPH_METH_MAX_SITE_LEN];           // recognition sites, characters
-    uint8_t site_m_rank[NPH_METH_MAX_SITES][NPH_METH_MAX_SITE_LEN];    // ranks of the methylated site
-    uint8_t site_mrc_rank[NPH_METH_MAX_SITES][NPH_METH_MAX_SITE_LEN];  // ranks of what stands on the other strand: reverse(methylated complement)
-};
-
-// does a complete recognition site start at ref[i]?  (is_motif_match reports complete sites only; the partial
-// matches match_to_site also knows — string end, string inside a site — never have the full length for len >= site_len)
-__device__ __forceinline__ int site_at(const MethDev& d, const uint8_t* __restrict__ ref, int i, int n)
-{
-    if (i < 0 || i + (int)d.site_len > n) return -1;
-    for (uint32_t s = 0; s < d.n_sites; ++s) {
-        bool eq = true;
-        for (uint32_t t = 0; t < d.site_len; ++t) eq = eq && (ref[i + t] == (uint8_t)d.site[s][t]);
-        if (eq) return (int)s;
-    }
-    return -1;
-}
 
 // std::lower_bound(pairs, pairs + n, v, ref_pos < v) as a 32-ary search by the whole warp: every round the lanes probe
 // 32 evenly spaced entries and the ballot tells which interval holds the boundary (3 rounds for a 4 000-event read
@@ -363,19 +340,27 @@ __global__ void meth_fill_kernel(nph_meth_site* __restrict__ sites, const float*
 
 int build_dev_params(nph_ctx* ctx, const nph_meth_params& p, MethDev& d)
 {
-    auto bad = [&](const char* what) { ctx->last_error = std::string("nph_meth_params: ") + what; return NPH_ERR_INVALID; };
-    if (p.min_separation < 0 || p.min_flank < 0 || p.max_span < 0) return bad("negative window parameter");
-    if (p.k == 0 || p.k > 12) return bad("k");
-    if (p.alphabet_size == 0 || p.alphabet_size > 8) return bad("alphabet_size");
-    if (p.n_sites == 0 || p.n_sites > NPH_METH_MAX_SITES) return bad("n_sites");
-    if (p.site_len == 0 || p.site_len >= NPH_METH_MAX_SITE_LEN) return bad("site_len");
+    if (p.min_separation < 0 || p.min_flank < 0 || p.max_span < 0) { ctx->last_error = "nph_meth_params: negative window parameter"; return NPH_ERR_INVALID; }
+    NPH_TRY(nph_meth_alphabet(ctx, p, d));
     if ((long long)p.max_span + 2ll * p.min_flank + 1 > NPH_METH_MAX_WINDOW) {
         ctx->last_error = "max_span + 2 * min_flank + 1 exceeds NPH_METH_MAX_WINDOW";
         return NPH_ERR_UNSUPPORTED;
     }
-    std::memset(&d, 0, sizeof(d));
     d.min_separation = p.min_separation; d.min_flank = p.min_flank; d.max_span = p.max_span; d.min_event_span = p.min_event_span;
     d.region_start = p.region_start; d.region_end = p.region_end;
+    return NPH_OK;
+}
+
+} // namespace
+
+int nph_meth_alphabet(nph_ctx* ctx, const nph_meth_params& p, MethDev& d)
+{
+    auto bad = [&](const char* what) { ctx->last_error = std::string("nph_meth_params: ") + what; return NPH_ERR_INVALID; };
+    if (p.k == 0 || p.k > 12) return bad("k");
+    if (p.alphabet_size == 0 || p.alphabet_size > 8) return bad("alphabet_size");
+    if (p.n_sites == 0 || p.n_sites > NPH_METH_MAX_SITES) return bad("n_sites");
+    if (p.site_len == 0 || p.site_len >= NPH_METH_MAX_SITE_LEN) return bad("site_len");
+    std::memset(&d, 0, sizeof(d));
     d.k = p.k; d.asize = p.alphabet_size; d.n_sites = p.n_sites; d.site_len = p.site_len;
     int rank_of[256];
     for (int c = 0; c < 256; ++c) rank_of[c] = -1;
@@ -411,8 +396,6 @@ int build_dev_params(nph_ctx* ctx, const nph_meth_params& p, MethDev& d)
     }
     return NPH_OK;
 }
-
-} // namespace
 
 // event alignments either as pair lists (aligned_events) or in compact form (event_deltas + first_event)
 static int meth_load(nph_ctx* ctx, const char* ref_bases, size_t n_ref_total,

@@ -1,6 +1,7 @@
 // nph_api.cu — the C ABI of libnph.so (include/nph.h): context, uploads, scheduling, fetches.
 // All device work is launched from here; there is no CPU implementation of any entry point.
 #include "nph_internal.cuh"
+#include "exact_math.cuh"
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
@@ -472,20 +473,8 @@ int nph_score_set_combine(const float* scores, size_t n_groups, uint32_t n_alt, 
         Table() { for (int i = 0; i < NPH_LOGSUM_TBL; ++i) v[i] = (float)log(1. + exp((double)-i / 1000.f)); }
     };
     static const Table table;
-    const float* tbl = table.v;
     const double pen = log((double)n_alt);
-    for (size_t g = 0; g < n_groups; ++g) {
-        double score = scores[g * n_alt] - pen;
-        for (uint32_t i = 1; i < n_alt; ++i) {
-            const double alt = scores[g * n_alt + i] - pen;
-            const float a = (float)score, b = (float)alt;
-            const float mx = a > b ? a : b, mn = a < b ? a : b;
-            // !(d < 15.7f) also catches NaN / inf differences (a NaN or +inf score): no out-of-range table index, like the device path's clamp
-            const float d = mx - mn;
-            score = (mn == -INFINITY || !(d < 15.7f)) ? mx : mx + tbl[(int)(d * 1000.f)];
-        }
-        out[g] = (float)score;
-    }
+    for (size_t g = 0; g < n_groups; ++g) out[g] = nph_score_set_fold(scores + g * n_alt, n_alt, pen, table.v);
     return NPH_OK;
 }
 

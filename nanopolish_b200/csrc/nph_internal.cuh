@@ -160,8 +160,13 @@ struct nph_ctx {
         DevBuf<nph_meth_record> d_records;
         DevBuf<uint64_t> d_pos_off;        // n_pos + 1: where each position's bounded reads start
         DevBuf<uint8_t> d_pos_reads;       // {record, e1, e2} per bounded read
-        DevBuf<uint8_t> d_state;           // per position: totals (9 doubles), alive mask, reads done, valid mask
+        DevBuf<uint8_t> d_state;           // per position: totals (9 doubles), alive mask, reads done, valid mask; then the counters and
+                                           // per position the methylated-alternatives mask
         DevBuf<uint64_t> d_job_off;        // per position: first job of the round (+ totals)
+        uint32_t n_types = 0;              // methylation types (nph_screen_load_methylation)
+        std::vector<uint8_t> h_meth;       // their MethDev tables (meth_dev.cuh), the source of d_meth's upload
+        DevBuf<uint8_t> d_meth;
+        DevBuf<uint32_t> d_alt_models;     // n_records x n_types model ids
     } screen;
 
     // measurement

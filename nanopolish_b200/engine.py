@@ -123,19 +123,31 @@ class Engine:
         return site_off, sites[:n_sites]
 
     # ---- variants: candidate screening on the device (include/nph.h, section N2) ----
-    def screen_edits_batch(self, reads, ev_mean, ev_start_time, ref_bases, deltas, first_event, records, params, indel_bias: float = 1.0):
-        """nph_screen_edits_batch: returns (qualities f8[n_pos, 9], n_reads u4[n_pos], scored_events)."""
+    def screen_edits_batch(self, reads, ev_mean, ev_start_time, ref_bases, deltas, first_event, records, params, indel_bias: float = 1.0,
+                           methylation=None):
+        """nph_screen_edits_batch: returns (qualities f8[n_pos, 9], n_reads u4[n_pos], scored_events).  methylation = (SCREEN_METH_DT[1],
+        alt_model_ids u4[n_records, n_types]): nph_screen_edits_batch_methylation (`variants -q ...`)."""
         n_pos = int(ref_bases.shape[0]) - 1
         q = np.zeros((n_pos, 9), np.float64); nr = np.zeros(n_pos, np.uint32)
         scored = C.c_uint64()
-        self._check(self.lib.nph_screen_edits_batch(self.ctx, _p(reads), reads.shape[0], _p(ev_mean), _p(ev_start_time), ev_mean.shape[0],
-                                                    _p(ref_bases), ref_bases.shape[0], _p(deltas), deltas.shape[0], _p(first_event), _p(records),
-                                                    records.shape[0], _p(params), indel_bias, _p(q), _p(nr), C.byref(scored)), "nph_screen_edits_batch")
+        head = (self.ctx, _p(reads), reads.shape[0], _p(ev_mean), _p(ev_start_time), ev_mean.shape[0], _p(ref_bases), ref_bases.shape[0],
+                _p(deltas), deltas.shape[0], _p(first_event), _p(records), records.shape[0], _p(params), indel_bias)
+        if methylation is None:
+            self._check(self.lib.nph_screen_edits_batch(*head, _p(q), _p(nr), C.byref(scored)), "nph_screen_edits_batch")
+        else:
+            meth, ids = methylation[0], np.ascontiguousarray(methylation[1], np.uint32)
+            self._check(self.lib.nph_screen_edits_batch_methylation(*head, _p(meth), _p(ids), _p(q), _p(nr), C.byref(scored)),
+                        "nph_screen_edits_batch_methylation")
         return q, nr, int(scored.value)
 
-    def screen_load(self, ref_bases, deltas, first_event, records, params, indel_bias: float = 1.0):
-        self._check(self.lib.nph_screen_load(self.ctx, _p(ref_bases), ref_bases.shape[0], _p(deltas), deltas.shape[0], _p(first_event), _p(records),
-                                             records.shape[0], _p(params), indel_bias), "nph_screen_load")
+    def screen_load(self, ref_bases, deltas, first_event, records, params, indel_bias: float = 1.0, methylation=None):
+        head = (self.ctx, _p(ref_bases), ref_bases.shape[0], _p(deltas), deltas.shape[0], _p(first_event), _p(records), records.shape[0], _p(params),
+                indel_bias)
+        if methylation is None:
+            self._check(self.lib.nph_screen_load(*head), "nph_screen_load")
+        else:
+            meth, ids = methylation[0], np.ascontiguousarray(methylation[1], np.uint32)
+            self._check(self.lib.nph_screen_load_methylation(*head, _p(meth), _p(ids)), "nph_screen_load_methylation")
         self._screen_n = int(ref_bases.shape[0]) - 1
 
     def screen_run(self):

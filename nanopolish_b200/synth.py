@@ -582,12 +582,14 @@ def screen_params(region_start: int, k: int = 6, flank: int = 10, threshold: int
 
 
 def gen_pileup(ref_len: int, depth: int, read_bases: int, model: PoreModel, seed: int = 42, region_start: int = 5000, n_true_variants: int = 0,
-               rc_every: int = 2):
+               rc_every: int = 2, sequences=None, read_levels=None):
     """A draft reference of ref_len bases and ~depth-fold coverage by reads of read_bases bases sampled from the TRUTH (the draft with
     n_true_variants substitutions), aligned base for base (CIGAR all M) — the input shape of `variants --consensus` screening
     (SURVEY.md 8d, config 5).  Returns (ref_codes u1, ReadSet, records METH_RECORD_DT, pairs PAIR_DT): record r = read r, its
     EventAlignmentRecord::aligned_events built like src/alignment/nanopolish_alignment_db.cpp:50-91 (ref_off = offset of the record's
-    slice in the compact event alignment, see compact_event_alignment)."""
+    slice in the compact event alignment, see compact_event_alignment).
+    sequences(draft, truth) -> (draft, truth) may rewrite the two sequences; read_levels(r, rc, codes) -> (level_mean, level_stdv) per k-mer,
+    or None for `model`'s levels of the read's k-mers (gen_pileup_methylated uses both)."""
     rng = np.random.default_rng(seed)
     k = model.k
     ref = rng.integers(0, 4, ref_len, dtype=np.uint8)
@@ -595,6 +597,8 @@ def gen_pileup(ref_len: int, depth: int, read_bases: int, model: PoreModel, seed
     if n_true_variants:
         pos = rng.choice(np.arange(40, ref_len - 40), n_true_variants, replace=False)
         truth[pos] = (truth[pos] + rng.integers(1, 4, n_true_variants)) % 4
+    if sequences is not None:
+        ref, truth = sequences(ref, truth)
     n_reads = max(1, int(round(depth * ref_len / read_bases)))
     starts = np.sort(rng.integers(0, ref_len - read_bases + 1, n_reads))
     reads = np.zeros(n_reads, READ_DT)
@@ -609,14 +613,17 @@ def gen_pileup(ref_len: int, depth: int, read_bases: int, model: PoreModel, seed
         rc = 1 if (rc_every and r % rc_every == rc_every - 1) else 0
         codes = (3 - seg[::-1]).astype(np.uint8) if rc else seg.copy()          # the bases as the pore saw them
         nk = codes.shape[0] - k + 1
-        ranks = kmer_ranks_from_codes(codes, k, 4)
+        levels = read_levels(r, rc, codes) if read_levels is not None else None
+        if levels is None:
+            ranks = kmer_ranks_from_codes(codes, k, 4)
+            levels = (model.level_mean[ranks], model.level_stdv[ranks])
         nev = rr.choice(4, nk, p=p_nev)
         nev[0] = max(nev[0], 1); nev[-1] = max(nev[-1], 1)
         which = np.repeat(np.arange(nk, dtype=np.int32), nev)
         E = which.shape[0]
         shift, scale, var = rr.uniform(-5.0, 5.0), rr.uniform(0.9, 1.1), rr.uniform(0.9, 1.3)
         t = np.arange(E, dtype=np.float64) * 0.002 + rr.uniform(0.0, 100.0)
-        m = (scale * model.level_mean[ranks[which]] + shift + var * model.level_stdv[ranks[which]] * rr.standard_normal(E)).astype(np.float32)
+        m = (scale * levels[0][which] + shift + var * levels[1][which] * rr.standard_normal(E)).astype(np.float32)
         reads[r] = (eoff, E, 0, scale, shift, 0.0, var, np.log(var), E / float(nk))
         _, _, closest = closest_event_map(which, nk)
         q = np.arange(k, read_bases - k)
@@ -632,3 +639,87 @@ def gen_pileup(ref_len: int, depth: int, read_bases: int, model: PoreModel, seed
         eoff += E; doff += read_bases; poff += pr.shape[0]
     rs = ReadSet(reads, np.concatenate(means), np.concatenate(times), seqs, evk, kfe, k)
     return ref, rs, recs, np.concatenate(prs)
+
+
+# ---- methylation-aware screening (`variants -q cpg`, `-q dam,dcm`) -------------------------------------------------------
+SCREEN_METH_DT = np.dtype([("n_types", "<u4"), ("reserved", "<u4"), ("alphabets", METH_PARAMS_DT, 4)], align=True)
+assert SCREEN_METH_DT.itemsize == 616
+
+
+def screen_methylation(types, k: int = 6) -> np.ndarray:
+    """nph_screen_methylation for opt::methylation_types = types (-q order)"""
+    m = np.zeros(1, SCREEN_METH_DT)
+    m[0]["n_types"] = len(types)
+    for t, name in enumerate(types):
+        m[0]["alphabets"][t] = meth_params(name, k)[0]
+    return m
+
+
+def _methylate_codes(alphabet: str, seq: bytes, rc: bool) -> np.ndarray:
+    """ACGMT codes of Alphabet::methylate(seq) (every recognition site replaced; the reference's sites never overlap), or of
+    Alphabet::reverse_complement of it: a methylated site on the other strand is its methylated complement back to front"""
+    bases, comps, sites, sm, smc = _METH_ALPHABETS[alphabet]
+    rl = len(sites[0])
+    out = bytearray(seq)
+    hits = []
+    for si, site in enumerate(sites):
+        q = seq.find(site)
+        while q >= 0:
+            out[q:q + rl] = sm[si]
+            hits.append((q, si))
+            q = seq.find(site, q + 1)
+    if rc:
+        comp = dict(zip(bases, comps))
+        out = bytearray(comp[c] for c in reversed(seq))
+        L = len(seq)
+        for q, si in hits:
+            out[L - q - rl:L - q] = smc[si]
+    return encode(bytes(out), "cpg")
+
+
+def gen_pileup_methylated(ref_len: int, depth: int, read_bases: int, model: PoreModel, types, type_models: dict, seed: int = 42,
+                          region_start: int = 5000, n_true_variants: int = 8, rc_every: int = 2, methylated_fraction: float = 0.5,
+                          site_spacing: int = 24):
+    """gen_pileup over a draft with planted recognition sites of every type in `types` (about one per site_spacing bases), and
+    n_true_variants true substitutions placed inside sites: half destroy a site of the draft in the truth, half complete in the truth a
+    site the draft lacks, so the candidates that correct them change the number of methylated alternatives.  A methylated_fraction of
+    the reads (cycling through the types) take their levels from type_models[type] over the methylated k-mers of the truth.
+    Returns what gen_pileup returns."""
+    sites = [(name, s) for name in types for s in _METH_ALPHABETS[name][2]]
+    k = model.k
+
+    def plant(draft, truth):
+        rng = np.random.default_rng(seed * 104729 + 17)
+        draft = draft.copy()
+        starts = []
+        p = 30
+        while p < ref_len - 40:
+            _, site = sites[int(rng.integers(len(sites)))]
+            draft[p:p + len(site)] = encode(site, "nucleotide")
+            starts.append((p, len(site)))
+            p += len(site) + int(rng.integers(site_spacing // 2, site_spacing * 3 // 2))
+        truth = draft.copy()
+        chosen = rng.choice(len(starts), min(n_true_variants, len(starts)), replace=False)
+        for n, c in enumerate(chosen):
+            p, ln = starts[int(c)]
+            o = p + int(rng.integers(ln))
+            other = (int(draft[o]) + int(rng.integers(1, 4))) % 4
+            if n % 2 == 0:
+                truth[o] = other            # the truth lacks the site: the correcting candidate destroys it
+            else:
+                draft[o] = other            # the draft lacks it: the correcting candidate creates it
+        return draft, truth
+
+    def levels(r, rc, codes):
+        pick = np.random.default_rng(seed * 15485863 + r).random()
+        if pick >= methylated_fraction:
+            return None
+        name = types[r % len(types)]
+        tm = type_models[name]
+        truth_seq = _CODE2DNA[(3 - codes[::-1]).astype(np.uint8) if rc else codes].tobytes()     # the reference strand of the read
+        mc = _methylate_codes(name, truth_seq, bool(rc))
+        ranks = kmer_ranks_from_codes(mc, k, 5)
+        return tm.level_mean[ranks], tm.level_stdv[ranks]
+
+    return gen_pileup(ref_len, depth, read_bases, model, seed=seed, region_start=region_start, n_true_variants=0, rc_every=rc_every,
+                      sequences=plant, read_levels=levels)

@@ -5,6 +5,8 @@ Run in the build container (where /root/reference exists):  python scripts/make_
 Outputs (small, committed):
   tests/golden/r9.4_450bps.{nucleotide,cpg}.6mer.template.npz  pore-model tables dumped from the
       reference's PoreModelSet (k, level_mean, level_stdv, level_log_stdv as float64)
+  tests/golden/r9.4_450bps.{dam,dcm}.6mer.template.npz  the same for `variants -q dam,dcm`
+      [python scripts/make_golden.py models dam dcm: writes only the models named]
   tests/golden/hmm_golden.npz   inputs (seeds + job lists) and the reference's profile_hmm_score floats
   tests/golden/abea_golden.npz  inputs (seeds) and the reference's AlignedPair lists / verdicts
   tests/golden/eventalign_golden.npz  the reference's align_read_to_ref + emit_event_alignment_tsv output (TSV bytes,
@@ -25,8 +27,8 @@ from nanopolish_b200 import synth  # noqa: E402
 GOLD = os.path.join(ROOT, "tests", "golden")
 
 
-def dump_models(ref):
-    for alphabet in ("nucleotide", "cpg"):
+def dump_models(ref, alphabets=("nucleotide", "cpg")):
+    for alphabet in alphabets:
         h = ref.builtin_model(alphabet)
         k, a, mean, sd, lsd = ref.model_dump(h)
         np.savez_compressed(os.path.join(GOLD, f"r9.4_450bps.{alphabet}.6mer.template.npz"),
@@ -60,6 +62,9 @@ def main():
     ref = RefOracle()
     if sys.argv[1:] == ["eventalign"]:
         eventalign_golden(ref)
+        return
+    if sys.argv[1:2] == ["models"]:
+        dump_models(ref, sys.argv[2:])
         return
     dump_models(ref)
     from tests.golden_cases import make_hmm_cases, make_abea_cases   # shared with the tests
