@@ -3,8 +3,8 @@
 // call-methylation batches hold ~10^6 tiny jobs; doing the per-job bookkeeping on the host cost more
 // than scoring them.  Three small kernels replace it: (1) validate each job against its read exactly
 // where the reference would assert or read out of bounds (profile_hmm_r9.inl:275, :305), choose its
-// kernel class (hmm_classes.h) and histogram (class, step-count) keys; (2) one-block exclusive scan,
-// longest jobs first inside each class; (3) scatter job indices into the schedule.  The host reads
+// kernel class (hmm_classes.h) and histogram (class, step-count) keys; (2) exclusive scan of the histogram,
+// a block per class, longest jobs first inside each class; (3) scatter job indices into the schedule.  The host reads
 // back one small summary (error flag, per-class counts and costs, scratch sizes).
 #include "nph_internal.cuh"
 #include "hmm_classes.h"
@@ -115,7 +115,7 @@ __global__ void __launch_bounds__(1024) scan_kernel(const unsigned int* __restri
 {
     constexpr int T = 1024;
     constexpr int PER = (NPH_KEY_BUCKETS + T - 1) / T;
-    __shared__ unsigned int s_part[T];
+    __shared__ unsigned int s_warp[32];
     const int c = blockIdx.x, t = threadIdx.x;
     unsigned int base = 0;
     for (int k = 0; k < c; ++k) base += (unsigned int)sum->class_count[k];
@@ -125,15 +125,7 @@ __global__ void __launch_bounds__(1024) scan_kernel(const unsigned int* __restri
     const int lo = t * PER, hi = min((int)NPH_KEY_BUCKETS, lo + PER);
     unsigned int s = 0;
     for (int i = lo; i < hi; ++i) s += h[i];
-    s_part[t] = s;
-    __syncthreads();
-    for (int d = 1; d < T; d <<= 1) {                          // Hillis-Steele inclusive scan over the 1024 partials
-        unsigned int v = (t >= d) ? s_part[t - d] : 0u;
-        __syncthreads();
-        s_part[t] += v;
-        __syncthreads();
-    }
-    unsigned int run = base + ((t == 0) ? 0u : s_part[t - 1]);
+    unsigned int run = base + nph_block_scan_incl(s, s_warp, t) - s;      // exclusive over the 1024 partials
     for (int i = lo; i < hi; ++i) { o[i] = run; run += h[i]; }
 }
 
@@ -188,16 +180,18 @@ int nph_schedule_hmm_jobs(nph_ctx* ctx, size_t n_jobs, size_t n_ranks_total, Nph
 {
     const bool codes = src == NphJobSource::HostCodes;
     const size_t hist_n = (size_t)NPH_NUM_CLASSES * NPH_KEY_BUCKETS;
-    int rc;
-    if ((rc = nph_reserve(ctx, ctx->d_sched_cls, n_jobs)) != NPH_OK) return rc;
-    if ((rc = nph_reserve(ctx, ctx->d_sched_bkt, n_jobs)) != NPH_OK) return rc;
-    if ((rc = nph_reserve(ctx, ctx->d_sched_hist, 2 * hist_n + 1024)) != NPH_OK) return rc;
-    if (codes && (rc = nph_reserve(ctx, ctx->d_rank_base, n_jobs)) != NPH_OK) return rc;
-    unsigned int* hist = ctx->d_sched_hist.p;
-    unsigned int* offs = hist + hist_n;
-    SchedSummary* d_sum = reinterpret_cast<SchedSummary*>(offs + hist_n);
-    static_assert(sizeof(SchedSummary) <= 1024 * sizeof(unsigned int), "summary fits the tail of the buffer");
-    NPH_CUDA(ctx, cudaMemsetAsync(hist, 0, sizeof(unsigned int) * (2 * hist_n + 1024), ctx->stream));
+    NPH_TRY(nph_reserve(ctx, ctx->d_sched_cls, n_jobs));
+    NPH_TRY(nph_reserve(ctx, ctx->d_sched_bkt, n_jobs));
+    if (codes) NPH_TRY(nph_reserve(ctx, ctx->d_rank_base, n_jobs));
+    unsigned int* hist; unsigned int* offs; SchedSummary* d_sum;
+    auto layout = [&](NphArena& a) {
+        hist = a.take<unsigned int>(hist_n);
+        offs = a.take<unsigned int>(hist_n);
+        d_sum = a.take<SchedSummary>(1);
+    };
+    const size_t bytes = nph_layout_bytes(layout);           // (before the carve: sizing leaves the pointers null)
+    NPH_TRY(nph_carve(ctx, ctx->d_sched_hist, layout));
+    NPH_CUDA(ctx, cudaMemsetAsync(hist, 0, bytes, ctx->stream));
     const int threads = 256;
     int blocks = (int)std::min<size_t>((n_jobs + threads - 1) / threads, (size_t)ctx->sm_count * 8);
     if (blocks < 1) blocks = 1;
@@ -220,7 +214,7 @@ int nph_schedule_hmm_jobs(nph_ctx* ctx, size_t n_jobs, size_t n_ranks_total, Nph
     }
     if (codes) {
         // the ranks the kernels read: formed here, once, from the codes (the jobs' device copies now index d_ranks)
-        if ((rc = nph_reserve(ctx, ctx->d_ranks, (size_t)h.rank_cursor)) != NPH_OK) return rc;
+        NPH_TRY(nph_reserve(ctx, ctx->d_ranks, (size_t)h.rank_cursor));
         const int wblocks = (int)std::min<size_t>((n_jobs + 7) / 8, (size_t)ctx->sm_count * 8);
         codes_to_ranks_kernel<<<wblocks, 256, 0, ctx->stream>>>(ctx->d_jobs.p, (uint32_t)n_jobs, ctx->d_models.p, ctx->d_codes.p, ctx->d_rank_base.p, ctx->d_ranks.p);
         NPH_CUDA(ctx, cudaGetLastError());

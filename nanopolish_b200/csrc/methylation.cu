@@ -11,11 +11,12 @@
 //   Alphabet::methylate / reverse_complement and HMMInputSequence::get_kmer_rank over the window
 //                                        ref: nanopolish_alphabet.h:146-330, src/hmm/nanopolish_hmm_input_sequence.h:76-91
 //
-// Three small kernels around K1:
+// Two small kernels around K1:
 //   meth_scan_kernel   a warp per record: ballot scan for recognition sites 32 bases at a time, groups closed as the
 //                      sites stream by, the two lower_bounds as 32-ary warp searches over the event alignment; writes a
-//                      provisional row per surviving group and the record's group / k-mer-rank / scored-event counts
-//   meth_prefix_kernel exclusive prefix sums of those counts over the records (site, job and rank offsets) + totals
+//                      provisional row per surviving group, the record's group and k-mer-rank counts, and adds its scored
+//                      events to the summary
+//   (nph_scan_exclusive, scan.cu: the site and rank offsets of the records, exclusive prefixes of those two counts)
 //   meth_emit_kernel   a warp per record: per group, the window as alphabet ranks in shared memory (forward, or the
 //                      reverse complement the way Alphabet::reverse_complement builds it), methylated copy with every
 //                      complete recognition site replaced, rolling k-mer ranks by all lanes, two nph_hmm_job records and
@@ -45,10 +46,25 @@ struct MethGroup {
 };
 
 struct MethSummary {
-    unsigned long long n_sites, n_ranks, n_events;
+    unsigned long long n_events;
     int error;                // 0, or 1 + index of a record with a window shorter than k
-    int pad;
 };
+
+// d_counts: per record its groups and k-mer ranks (meth_scan_kernel), their exclusive prefixes (n + 1 entries each: the site
+// and rank offsets), the scans' scratch, the summary
+struct MethCounts { uint64_t* groups; uint64_t* ranks; uint64_t* site_off; uint64_t* rank_off; uint64_t* scratch; MethSummary* sum; };
+MethCounts meth_counts_layout(NphArena& a, size_t n)
+{
+    MethCounts c;
+    c.groups = a.take<uint64_t>(n);
+    c.ranks = a.take<uint64_t>(n);
+    c.site_off = a.take<uint64_t>(n + 1);
+    c.rank_off = a.take<uint64_t>(n + 1);
+    c.scratch = a.take<uint64_t>(nph_scan_scratch(n));
+    c.sum = a.take<MethSummary>(1);
+    return c;
+}
+MethCounts meth_counts(const nph_ctx::MethState& m) { NphArena a{m.d_counts.p}; return meth_counts_layout(a, m.ev.n_records); }
 
 // std::lower_bound(pairs, pairs + n, v, ref_pos < v) as a 32-ary search by the whole warp: every round the lanes probe
 // 32 evenly spaced entries and the ballot tells which interval holds the boundary (3 rounds for a 4 000-event read
@@ -70,46 +86,12 @@ __device__ __forceinline__ int warp_lower_bound(const nph_aligned_pair* __restri
     return lo + __popc(__ballot_sync(kFull, less));
 }
 
-constexpr int kNoEvent = INT32_MIN;
-
-// compact event alignments: per record, a prefix sum over its int16 deltas rebuilds the event index of every reference base that
-// has an aligned_events entry (kNoEvent elsewhere) and notes the first such base
-__global__ void __launch_bounds__(kThreads) meth_expand_kernel(const int16_t* __restrict__ deltas, const int32_t* __restrict__ first_event,
-                                                               const nph_meth_record* __restrict__ records, uint32_t n_records,
-                                                               int32_t* __restrict__ dense, int32_t* __restrict__ first_valid)
-{
-    const int lane = threadIdx.x & 31;
-    const uint32_t warp = blockIdx.x * kWarps + (threadIdx.x >> 5);
-    const uint32_t n_warps = gridDim.x * kWarps;
-    for (uint32_t rec = warp; rec < n_records; rec += n_warps) {
-        const nph_meth_record R = records[rec];
-        const int16_t* dl = deltas + R.ref_off;
-        int32_t* out = dense + R.ref_off;
-        const int n = (int)R.ref_len;
-        int running = first_event[rec];
-        int fv = n;
-        for (int base = 0; base < n; base += 32) {
-            const int o = base + lane;
-            const int dv = o < n ? (int)dl[o] : NPH_METH_NO_PAIR;
-            const bool valid = dv != NPH_METH_NO_PAIR;
-            int v = valid ? dv : 0;
-#pragma unroll
-            for (int sft = 1; sft < 32; sft <<= 1) { const int t = __shfl_up_sync(kFull, v, sft); if (lane >= sft) v += t; }
-            if (o < n) out[o] = valid ? running + v : kNoEvent;
-            running += __shfl_sync(kFull, v, 31);
-            const unsigned m = __ballot_sync(kFull, valid);
-            if (m && fv == n) fv = base + (__ffs(m) - 1);
-        }
-        if (lane == 0) first_valid[rec] = fv;
-    }
-}
-
 // first offset >= from with an aligned_events entry (n: none): the dense counterpart of std::lower_bound on ref_pos
 __device__ __forceinline__ int warp_first_valid(const int32_t* __restrict__ dense, int n, int from, int lane)
 {
     for (int base = from < 0 ? 0 : from; base < n; base += 32) {
         const int o = base + lane;
-        const unsigned m = __ballot_sync(kFull, o < n && dense[o] != kNoEvent);
+        const unsigned m = __ballot_sync(kFull, o < n && dense[o] != NPH_NO_EVENT);
         if (m) return base + (__ffs(m) - 1);
     }
     return n;
@@ -123,7 +105,8 @@ struct ScanArgs {
     const nph_meth_record* records;
     const uint64_t* prov_off;
     MethGroup* prov;
-    uint64_t* counts;          // [3 * n_records]: groups, ranks, scored events per record
+    uint64_t* groups;          // per record
+    uint64_t* ranks;
     MethSummary* sum;
     uint32_t n_records;
 };
@@ -198,52 +181,11 @@ __global__ void __launch_bounds__(kThreads) meth_scan_kernel(const ScanArgs a, c
         }
         if (g_count > 0) close_group();
         if (lane == 0) {
-            a.counts[3 * (size_t)rec] = n_groups;
-            a.counts[3 * (size_t)rec + 1] = n_ranks;
-            a.counts[3 * (size_t)rec + 2] = n_events;
+            a.groups[rec] = n_groups;
+            a.ranks[rec] = n_ranks;
             if (bad) atomicCAS(&a.sum->error, 0, (int)(rec + 1));
+            if (n_events) atomicAdd(&a.sum->n_events, n_events);
         }
-    }
-}
-
-// exclusive prefix sums over the records: site_off (n + 1 entries) and rank_off (n entries), plus the totals.
-// One block; the record count of a batch is 10^3..10^6, i.e. at most ~1000 rounds of a 1024-wide scan.
-__global__ void __launch_bounds__(1024) meth_prefix_kernel(const uint64_t* __restrict__ counts, uint32_t n_records,
-                                                           uint64_t* __restrict__ site_off, uint64_t* __restrict__ rank_off,
-                                                           MethSummary* __restrict__ sum)
-{
-    __shared__ unsigned long long s_a[1024], s_b[1024];
-    __shared__ unsigned long long carry_a, carry_b, carry_e;
-    const int t = threadIdx.x;
-    if (t == 0) { carry_a = 0; carry_b = 0; carry_e = 0; }
-    __syncthreads();
-    unsigned long long ev = 0;
-    for (uint32_t base = 0; base < n_records; base += 1024) {
-        const uint32_t r = base + t;
-        const unsigned long long va = r < n_records ? counts[3 * (size_t)r] : 0ull;
-        const unsigned long long vb = r < n_records ? counts[3 * (size_t)r + 1] : 0ull;
-        if (r < n_records) ev += counts[3 * (size_t)r + 2];
-        s_a[t] = va; s_b[t] = vb;
-        __syncthreads();
-        for (int dlt = 1; dlt < 1024; dlt <<= 1) {
-            const unsigned long long xa = t >= dlt ? s_a[t - dlt] : 0ull, xb = t >= dlt ? s_b[t - dlt] : 0ull;
-            __syncthreads();
-            s_a[t] += xa; s_b[t] += xb;
-            __syncthreads();
-        }
-        if (r < n_records) { site_off[r] = carry_a + s_a[t] - va; rank_off[r] = carry_b + s_b[t] - vb; }
-        __syncthreads();
-        if (t == 1023) { carry_a += s_a[1023]; carry_b += s_b[1023]; }
-        __syncthreads();
-    }
-    // scored events: plain block reduction
-    s_a[t] = ev;
-    __syncthreads();
-    for (int dlt = 512; dlt > 0; dlt >>= 1) { if (t < dlt) s_a[t] += s_a[t + dlt]; __syncthreads(); }
-    if (t == 0) {
-        carry_e = s_a[0];
-        site_off[n_records] = carry_a;
-        sum->n_sites = carry_a; sum->n_ranks = carry_b; sum->n_events = carry_e;
     }
 }
 
@@ -252,7 +194,7 @@ struct EmitArgs {
     const nph_meth_record* records;
     const uint64_t* prov_off;
     const MethGroup* prov;
-    const uint64_t* counts;
+    const uint64_t* groups;
     const uint64_t* site_off;
     const uint64_t* rank_off;
     nph_hmm_job* jobs;
@@ -277,7 +219,7 @@ __global__ void __launch_bounds__(kThreads) meth_emit_kernel(const EmitArgs a, c
         const nph_meth_record R = a.records[rec];
         const uint8_t* ref = a.ref + R.ref_off;
         const MethGroup* grp = a.prov + a.prov_off[rec];
-        const int n_groups = (int)a.counts[3 * (size_t)rec];
+        const int n_groups = (int)a.groups[rec];
         const uint64_t site0 = a.site_off[rec];
         uint64_t roff = a.rank_off[rec];
         for (int g = 0; g < n_groups; ++g) {
@@ -397,6 +339,103 @@ int nph_meth_alphabet(nph_ctx* ctx, const nph_meth_params& p, MethDev& d)
     return NPH_OK;
 }
 
+// ---- the event-aligned records of both device callers (call-methylation here, candidate screening in variants.cu) ----
+namespace {
+
+// compact event alignments: per record, a prefix sum over its int16 deltas rebuilds the event index of every reference base that
+// has an aligned_events entry (NPH_NO_EVENT elsewhere) and notes the first such base
+__global__ void __launch_bounds__(kThreads) meth_expand_kernel(const int16_t* __restrict__ deltas, const int32_t* __restrict__ first_event,
+                                                               const nph_meth_record* __restrict__ records, uint32_t n_records,
+                                                               int32_t* __restrict__ dense, int32_t* __restrict__ first_valid)
+{
+    const int lane = threadIdx.x & 31;
+    const uint32_t warp = blockIdx.x * kWarps + (threadIdx.x >> 5);
+    const uint32_t n_warps = gridDim.x * kWarps;
+    for (uint32_t rec = warp; rec < n_records; rec += n_warps) {
+        const nph_meth_record R = records[rec];
+        const int16_t* dl = deltas + R.ref_off;
+        int32_t* out = dense + R.ref_off;
+        const int n = (int)R.ref_len;
+        int running = first_event[rec];
+        int fv = n;
+        for (int base = 0; base < n; base += 32) {
+            const int o = base + lane;
+            const int dv = o < n ? (int)dl[o] : NPH_METH_NO_PAIR;
+            const bool valid = dv != NPH_METH_NO_PAIR;
+            int v = valid ? dv : 0;
+#pragma unroll
+            for (int sft = 1; sft < 32; sft <<= 1) { const int t = __shfl_up_sync(kFull, v, sft); if (lane >= sft) v += t; }
+            if (o < n) out[o] = valid ? running + v : NPH_NO_EVENT;
+            running += __shfl_sync(kFull, v, 31);
+            const unsigned m = __ballot_sync(kFull, valid);
+            if (m && fv == n) fv = base + (__ffs(m) - 1);
+        }
+        if (lane == 0) first_valid[rec] = fv;
+    }
+}
+
+// d_dense: event index per base | per record its first event (uploaded) | per record its first base with an entry
+struct DenseMap { int32_t* dense; int32_t* first_event; int32_t* first_valid; };
+DenseMap dense_layout(NphArena& a, const NphEventRecords& ev)
+{
+    DenseMap m;
+    m.dense = a.take<int32_t>(ev.n_map);
+    m.first_event = a.take<int32_t>(ev.n_records);
+    m.first_valid = a.take<int32_t>(ev.n_records);
+    return m;
+}
+
+} // namespace
+
+int nph_event_records_load(nph_ctx* ctx, NphEventRecords& ev, const char* ref, size_t n_ref, size_t n_map, bool compact,
+                           const int16_t* deltas, const int32_t* first_event, const nph_aligned_pair* pairs, size_t n_pairs,
+                           const nph_meth_record* records, size_t n_records, uint32_t max_len,
+                           const std::function<int(size_t, const nph_meth_record&)>& check)
+{
+    for (size_t r = 0; r < n_records; ++r) {
+        const nph_meth_record& R = records[r];
+        const bool ok = R.read < ctx->n_reads && R.model_id < ctx->models.size() && R.ref_len <= n_map && R.ref_off <= n_map - R.ref_len &&
+                        R.ref_len <= max_len && (compact || (R.n_pairs <= n_pairs && R.pair_off <= n_pairs - R.n_pairs));
+        if (!ok) { ctx->last_error = "record " + std::to_string(r) + " is out of range (read, model, reference or event-alignment slice)"; return NPH_ERR_INVALID; }
+        NPH_TRY(check(r, R));
+    }
+    NPH_CUDA(ctx, cudaSetDevice(ctx->device));
+    ev.n_records = n_records; ev.n_ref = n_ref; ev.n_map = n_map; ev.compact = compact;
+    NPH_TRY(nph_reserve(ctx, ev.d_ref, n_ref + 16));
+    NPH_TRY(nph_reserve(ctx, ev.d_records, n_records));
+    DenseMap dm{};
+    if (compact) {
+        NPH_TRY(nph_reserve(ctx, ev.d_deltas, n_map + 16));
+        NPH_TRY(nph_carve(ctx, ev.d_dense, [&](NphArena& a) { dm = dense_layout(a, ev); }));
+    } else {
+        NPH_TRY(nph_reserve(ctx, ev.d_pairs, n_pairs + 1));
+    }
+    NPH_CUDA(ctx, cudaMemcpyAsync(ev.d_ref.p, ref, n_ref, cudaMemcpyHostToDevice, ctx->stream));
+    if (n_records) NPH_CUDA(ctx, cudaMemcpyAsync(ev.d_records.p, records, sizeof(nph_meth_record) * n_records, cudaMemcpyHostToDevice, ctx->stream));
+    if (compact) {
+        if (n_map) NPH_CUDA(ctx, cudaMemcpyAsync(ev.d_deltas.p, deltas, sizeof(int16_t) * n_map, cudaMemcpyHostToDevice, ctx->stream));
+        if (n_records) NPH_CUDA(ctx, cudaMemcpyAsync(dm.first_event, first_event, sizeof(int32_t) * n_records, cudaMemcpyHostToDevice, ctx->stream));
+    } else if (n_pairs) {
+        NPH_CUDA(ctx, cudaMemcpyAsync(ev.d_pairs.p, pairs, sizeof(nph_aligned_pair) * n_pairs, cudaMemcpyHostToDevice, ctx->stream));
+    }
+    return NPH_OK;
+}
+
+int nph_event_records_expand(nph_ctx* ctx, NphEventRecords& ev, const int32_t** dense, const int32_t** first_valid)
+{
+    *dense = nullptr; *first_valid = nullptr;
+    if (!ev.compact) return NPH_OK;
+    NphArena a{ev.d_dense.p};
+    const DenseMap dm = dense_layout(a, ev);
+    *dense = dm.dense; *first_valid = dm.first_valid;
+    if (ev.n_records == 0) return NPH_OK;
+    const int grid = (int)std::min<size_t>((ev.n_records + kWarps - 1) / kWarps, (size_t)ctx->sm_count * 8);
+    meth_expand_kernel<<<grid, kThreads, 0, ctx->stream>>>(reinterpret_cast<const int16_t*>(ev.d_deltas.p), dm.first_event, ev.d_records.p,
+                                                           (uint32_t)ev.n_records, dm.dense, dm.first_valid);
+    NPH_CUDA(ctx, cudaGetLastError());
+    return NPH_OK;
+}
+
 // event alignments either as pair lists (aligned_events) or in compact form (event_deltas + first_event)
 static int meth_load(nph_ctx* ctx, const char* ref_bases, size_t n_ref_total,
                      const nph_aligned_pair* aligned_events, size_t n_pairs_total,
@@ -408,67 +447,36 @@ static int meth_load(nph_ctx* ctx, const char* ref_bases, size_t n_ref_total,
     nph_ctx::MethState& m = ctx->meth;
     m.loaded = false; m.ran = false;
     const bool compact = event_deltas != nullptr;
-    if (n_records == 0) { m.n_records = 0; m.loaded = true; return NPH_OK; }
+    if (n_records == 0) { m.ev.n_records = 0; m.loaded = true; return NPH_OK; }
     if (!ref_bases || !records || (!compact && !aligned_events && n_pairs_total) || (compact && !first_event)) return NPH_ERR_INVALID;
     if (!ctx->reads_loaded) return NPH_ERR_STATE;
     MethDev d;
     NPH_TRY(build_dev_params(ctx, *params, d));
-    // O(records) validation and the provisional layout: a record has at most ref_len / (min_separation + 1) + 1 groups
-    // (consecutive groups start more than min_separation bases apart)
+    // records index the reference: the compact form has one delta per reference base
+    NPH_TRY(nph_event_records_load(ctx, m.ev, ref_bases, n_ref_total, n_ref_total, compact, event_deltas, first_event, aligned_events, n_pairs_total,
+                                   records, n_records, 0x7fffffffu, [&](size_t r, const nph_meth_record& R) {
+        const DevModel& mod = ctx->models[R.model_id];
+        if (mod.k == params->k && mod.alphabet_size == params->alphabet_size) return NPH_OK;
+        ctx->last_error = "methylation record " + std::to_string(r) + ": its model's k / alphabet differ from nph_meth_params";
+        return NPH_ERR_INVALID;
+    }));
+    // the provisional layout: a record has at most ref_len / (min_separation + 1) + 1 groups (consecutive groups start more
+    // than min_separation bases apart)
     std::vector<uint64_t>& po = m.h_prov_off;
     po.resize(n_records + 1);
     uint64_t prov = 0;
     for (size_t r = 0; r < n_records; ++r) {
-        const nph_meth_record& R = records[r];
-        const bool ok = R.read < ctx->n_reads && R.model_id < ctx->models.size() && R.ref_len <= n_ref_total && R.ref_off <= n_ref_total - R.ref_len &&
-                        R.ref_len <= 0x7fffffffu && (compact || (R.n_pairs <= n_pairs_total && R.pair_off <= n_pairs_total - R.n_pairs));
-        if (!ok) { ctx->last_error = "methylation record " + std::to_string(r) + " is out of range (read, model, reference or event-alignment slice)"; return NPH_ERR_INVALID; }
-        const DevModel& mod = ctx->models[R.model_id];
-        if (mod.k != params->k || mod.alphabet_size != params->alphabet_size) {
-            ctx->last_error = "methylation record " + std::to_string(r) + ": its model's k / alphabet differ from nph_meth_params";
-            return NPH_ERR_INVALID;
-        }
         po[r] = prov;
-        prov += (uint64_t)R.ref_len / (uint64_t)(params->min_separation + 1) + 2;
+        prov += (uint64_t)records[r].ref_len / (uint64_t)(params->min_separation + 1) + 2;
     }
     po[n_records] = prov;
-    NPH_CUDA(ctx, cudaSetDevice(ctx->device));
-    NPH_TRY(nph_reserve(ctx, m.d_ref, n_ref_total + 16));
-    if (compact) {
-        NPH_TRY(nph_reserve(ctx, m.d_deltas, n_ref_total + 16));
-        NPH_TRY(nph_reserve(ctx, m.d_dense, n_ref_total + 2 * n_records + 16));
-    } else {
-        NPH_TRY(nph_reserve(ctx, m.d_pairs, n_pairs_total + 1));
-    }
-    NPH_TRY(nph_reserve(ctx, m.d_records, n_records));
     NPH_TRY(nph_reserve(ctx, m.d_prov_off, n_records + 1));
     NPH_TRY(nph_reserve(ctx, m.d_prov, (size_t)prov * sizeof(MethGroup)));
-    // counts (3 per record) | site_off (n + 1) | rank_off (n) | summary
-    NPH_TRY(nph_reserve(ctx, m.d_counts, 5 * n_records + 1 + (sizeof(MethSummary) + 7) / 8 + 8));
-    NPH_CUDA(ctx, cudaMemcpyAsync(m.d_records.p, records, sizeof(nph_meth_record) * n_records, cudaMemcpyHostToDevice, ctx->stream));
+    NPH_TRY(nph_carve(ctx, m.d_counts, [&](NphArena& a) { meth_counts_layout(a, n_records); }));
     NPH_CUDA(ctx, cudaMemcpyAsync(m.d_prov_off.p, po.data(), sizeof(uint64_t) * (n_records + 1), cudaMemcpyHostToDevice, ctx->stream));
-    NPH_CUDA(ctx, cudaMemcpyAsync(m.d_ref.p, ref_bases, n_ref_total, cudaMemcpyHostToDevice, ctx->stream));
-    if (compact) {
-        // first_event goes behind the dense array: [n_ref] event indices | [n_records] first_event | [n_records] first valid offset
-        NPH_CUDA(ctx, cudaMemcpyAsync(m.d_deltas.p, event_deltas, sizeof(int16_t) * n_ref_total, cudaMemcpyHostToDevice, ctx->stream));
-        NPH_CUDA(ctx, cudaMemcpyAsync(m.d_dense.p + n_ref_total, first_event, sizeof(int32_t) * n_records, cudaMemcpyHostToDevice, ctx->stream));
-    } else if (n_pairs_total) {
-        NPH_CUDA(ctx, cudaMemcpyAsync(m.d_pairs.p, aligned_events, sizeof(nph_aligned_pair) * n_pairs_total, cudaMemcpyHostToDevice, ctx->stream));
-    }
-    m.compact = compact;
-    m.n_records = n_records; m.n_ref = n_ref_total; m.n_pairs = compact ? 0 : n_pairs_total; m.prov_total = (size_t)prov;
+    m.prov_total = (size_t)prov;
     m.params = *params; m.indel_bias = indel_bias;
     m.loaded = true;
-    return NPH_OK;
-}
-
-int nph_expand_event_maps(nph_ctx* ctx, const int16_t* d_deltas, const int32_t* d_first_event, const nph_meth_record* d_records, uint32_t n_records,
-                          int32_t* d_dense, int32_t* d_first_valid)
-{
-    if (n_records == 0) return NPH_OK;
-    const int grid = (int)std::min<size_t>(((size_t)n_records + kWarps - 1) / kWarps, (size_t)ctx->sm_count * 8);
-    meth_expand_kernel<<<grid, kThreads, 0, ctx->stream>>>(d_deltas, d_first_event, d_records, n_records, d_dense, d_first_valid);
-    NPH_CUDA(ctx, cudaGetLastError());
     return NPH_OK;
 }
 
@@ -495,58 +503,53 @@ extern "C" int nph_methylation_run(nph_ctx* ctx)
     if (!m.loaded) return NPH_ERR_STATE;
     m.ran = false;
     m.n_sites = m.n_ranks = m.n_scored_events = 0;
-    if (m.n_records == 0) { m.ran = true; return NPH_OK; }
+    if (m.ev.n_records == 0) { m.ran = true; return NPH_OK; }
     if (!ctx->reads_loaded) return NPH_ERR_STATE;
     NPH_CUDA(ctx, cudaSetDevice(ctx->device));
     MethDev d;
     NPH_TRY(build_dev_params(ctx, m.params, d));
-    const uint32_t n = (uint32_t)m.n_records;
-    uint64_t* counts = m.d_counts.p;
-    uint64_t* site_off = counts + 3 * (size_t)n;
-    uint64_t* rank_off = site_off + n + 1;
-    MethSummary* d_sum = reinterpret_cast<MethSummary*>(rank_off + n);
-    NPH_CUDA(ctx, cudaMemsetAsync(d_sum, 0, sizeof(MethSummary), ctx->stream));
-    const int grid = (int)std::min<size_t>((m.n_records + kWarps - 1) / kWarps, (size_t)ctx->sm_count * 8);
-    int32_t* dense = nullptr;
-    int32_t* first_valid = nullptr;
-    if (m.compact) {
-        dense = reinterpret_cast<int32_t*>(m.d_dense.p);
-        const int32_t* d_first_event = dense + m.n_ref;
-        first_valid = dense + m.n_ref + m.n_records;
-        meth_expand_kernel<<<grid, kThreads, 0, ctx->stream>>>(reinterpret_cast<const int16_t*>(m.d_deltas.p), d_first_event, m.d_records.p, n, dense, first_valid);
-        NPH_CUDA(ctx, cudaGetLastError());
-    }
-    ScanArgs sa{m.d_ref.p, dense, first_valid, m.compact ? nullptr : m.d_pairs.p, m.d_records.p, m.d_prov_off.p,
-                reinterpret_cast<MethGroup*>(m.d_prov.p), counts, d_sum, n};
+    const NphEventRecords& ev = m.ev;
+    const uint32_t n = (uint32_t)ev.n_records;
+    const MethCounts c = meth_counts(m);
+    NPH_CUDA(ctx, cudaMemsetAsync(c.sum, 0, sizeof(MethSummary), ctx->stream));
+    const int grid = (int)std::min<size_t>((ev.n_records + kWarps - 1) / kWarps, (size_t)ctx->sm_count * 8);
+    const int32_t* dense;
+    const int32_t* first_valid;
+    NPH_TRY(nph_event_records_expand(ctx, m.ev, &dense, &first_valid));
+    ScanArgs sa{ev.d_ref.p, dense, first_valid, ev.compact ? nullptr : ev.d_pairs.p, ev.d_records.p, m.d_prov_off.p,
+                reinterpret_cast<MethGroup*>(m.d_prov.p), c.groups, c.ranks, c.sum, n};
     meth_scan_kernel<<<grid, kThreads, 0, ctx->stream>>>(sa, d);
     NPH_CUDA(ctx, cudaGetLastError());
-    meth_prefix_kernel<<<1, 1024, 0, ctx->stream>>>(counts, n, site_off, rank_off, d_sum);
-    NPH_CUDA(ctx, cudaGetLastError());
+    NPH_TRY(nph_scan_exclusive(ctx, c.groups, n, c.site_off, c.scratch));
+    NPH_TRY(nph_scan_exclusive(ctx, c.ranks, n, c.rank_off, c.scratch));
     MethSummary h{};
-    NPH_CUDA(ctx, cudaMemcpyAsync(&h, d_sum, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
+    uint64_t n_sites = 0, n_ranks = 0;
+    NPH_CUDA(ctx, cudaMemcpyAsync(&h, c.sum, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
+    NPH_CUDA(ctx, cudaMemcpyAsync(&n_sites, c.site_off + n, sizeof(n_sites), cudaMemcpyDeviceToHost, ctx->stream));
+    NPH_CUDA(ctx, cudaMemcpyAsync(&n_ranks, c.rank_off + n, sizeof(n_ranks), cudaMemcpyDeviceToHost, ctx->stream));
     NPH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));          // read-back 1 of 2: the counts that size the job arrays
     if (h.error) {
         ctx->last_error = "methylation record " + std::to_string(h.error - 1) + ": a window cut by the end of the reference is shorter than k";
         return NPH_ERR_INVALID;
     }
-    m.n_sites = h.n_sites; m.n_ranks = h.n_ranks; m.n_scored_events = h.n_events;
-    const size_t n_jobs = 2 * (size_t)h.n_sites;
+    m.n_sites = n_sites; m.n_ranks = n_ranks; m.n_scored_events = h.n_events;
+    const size_t n_jobs = 2 * (size_t)n_sites;
     ctx->n_jobs = 0; ctx->jobs_loaded = false;
     if (n_jobs == 0) { ctx->classes.clear(); ctx->jobs_loaded = true; m.ran = true; return NPH_OK; }
-    NPH_TRY(nph_reserve(ctx, ctx->d_ranks, (size_t)h.n_ranks));
-    NPH_TRY(nph_reserve(ctx, m.d_sites, (size_t)h.n_sites));
+    NPH_TRY(nph_reserve(ctx, ctx->d_ranks, (size_t)n_ranks));
+    NPH_TRY(nph_reserve(ctx, m.d_sites, (size_t)n_sites));
     // meth_emit_kernel writes the jobs and their k-mer ranks; the schedule is read-back 2 of 2
-    NPH_TRY(nph_score_device_jobs(ctx, n_jobs, (size_t)h.n_ranks, m.indel_bias, [&]() -> int {
-        EmitArgs ea{m.d_ref.p, m.d_records.p, m.d_prov_off.p, reinterpret_cast<const MethGroup*>(m.d_prov.p), counts, site_off, rank_off,
+    NPH_TRY(nph_score_device_jobs(ctx, n_jobs, (size_t)n_ranks, m.indel_bias, [&]() -> int {
+        EmitArgs ea{ev.d_ref.p, ev.d_records.p, m.d_prov_off.p, reinterpret_cast<const MethGroup*>(m.d_prov.p), c.groups, c.site_off, c.rank_off,
                     ctx->d_jobs.p, ctx->d_ranks.p, m.d_sites.p, n};
         meth_emit_kernel<<<grid, kThreads, 0, ctx->stream>>>(ea, d);
         NPH_CUDA(ctx, cudaGetLastError());
         return NPH_OK;
     }));
-    const int fgrid = (int)std::min<size_t>(((size_t)h.n_sites + 255) / 256, (size_t)ctx->sm_count * 8);
-    meth_fill_kernel<<<fgrid, 256, 0, ctx->stream>>>(m.d_sites.p, ctx->d_scores.p, h.n_sites);
+    const int fgrid = (int)std::min<size_t>(((size_t)n_sites + 255) / 256, (size_t)ctx->sm_count * 8);
+    meth_fill_kernel<<<fgrid, 256, 0, ctx->stream>>>(m.d_sites.p, ctx->d_scores.p, n_sites);
     NPH_CUDA(ctx, cudaGetLastError());
-    ctx->last_launches += 6;                                     // scan, prefix, emit, classify/scan/scatter are counted with the forward classes' launches: 3 + 3
+    ctx->last_launches += 11;        // counted with the forward classes' launches: meth_scan, two 3-launch offset scans, emit, classify/scan/scatter
     m.ran = true;
     return NPH_OK;
 }
@@ -653,33 +656,6 @@ __global__ void __launch_bounds__(kThreads) meth_tsv_kernel(const TsvArgs a)
     }
 }
 
-// exclusive prefix of the per-record byte counts (one block; n + 1 entries out)
-__global__ void __launch_bounds__(1024) meth_tsv_prefix_kernel(const uint64_t* __restrict__ bytes, uint32_t n, uint64_t* __restrict__ off)
-{
-    __shared__ unsigned long long s_a[1024];
-    __shared__ unsigned long long carry;
-    const int t = threadIdx.x;
-    if (t == 0) carry = 0;
-    __syncthreads();
-    for (uint32_t base = 0; base < n; base += 1024) {
-        const uint32_t r = base + t;
-        const unsigned long long v = r < n ? bytes[r] : 0ull;
-        s_a[t] = v;
-        __syncthreads();
-        for (int dlt = 1; dlt < 1024; dlt <<= 1) {
-            const unsigned long long x = t >= dlt ? s_a[t - dlt] : 0ull;
-            __syncthreads();
-            s_a[t] += x;
-            __syncthreads();
-        }
-        if (r < n) off[r] = carry + s_a[t] - v;
-        __syncthreads();
-        if (t == 1023) carry += s_a[1023];
-        __syncthreads();
-    }
-    if (t == 0) off[n] = carry;
-}
-
 } // namespace
 
 extern "C" int nph_methylation_tsv(nph_ctx* ctx, const char* contig, const char* read_names, const uint32_t* name_off,
@@ -689,10 +665,10 @@ extern "C" int nph_methylation_tsv(nph_ctx* ctx, const char* contig, const char*
     nph_ctx::MethState& m = ctx->meth;
     if (!m.ran) return NPH_ERR_STATE;
     *n_bytes_out = 0;
-    if (m.n_records == 0 || m.n_sites == 0) return NPH_OK;
+    if (m.ev.n_records == 0 || m.n_sites == 0) return NPH_OK;
     if (!contig || !read_names || !name_off || !is_reverse) return NPH_ERR_INVALID;
     NPH_CUDA(ctx, cudaSetDevice(ctx->device));
-    const size_t n = m.n_records, contig_len = std::strlen(contig), names_len = name_off[n];
+    const size_t n = m.ev.n_records, contig_len = std::strlen(contig), names_len = name_off[n];
     for (size_t r = 0; r < n; ++r) if (name_off[r] > name_off[r + 1]) { ctx->last_error = "name_off must ascend"; return NPH_ERR_INVALID; }
     // one staging block: contig | names | name offsets | strand flags
     char* d_contig; char* d_names; uint32_t* d_noff; uint8_t* d_rev;
@@ -702,23 +678,25 @@ extern "C" int nph_methylation_tsv(nph_ctx* ctx, const char* contig, const char*
         d_noff = a.take<uint32_t>(n + 1);
         d_rev = a.take<uint8_t>(n);
     }));
-    NPH_TRY(nph_reserve(ctx, m.d_tsv_off, 2 * n + 4));
+    uint64_t* rec_bytes; uint64_t* rec_off; uint64_t* scratch; int* d_refused;
+    NPH_TRY(nph_carve(ctx, m.d_tsv_off, [&](NphArena& a) {
+        rec_bytes = a.take<uint64_t>(n);
+        rec_off = a.take<uint64_t>(n + 1);
+        scratch = a.take<uint64_t>(nph_scan_scratch(n));
+        d_refused = a.take<int>(1);
+    }));
     NPH_CUDA(ctx, cudaMemcpyAsync(d_contig, contig, contig_len, cudaMemcpyHostToDevice, ctx->stream));
     NPH_CUDA(ctx, cudaMemcpyAsync(d_names, read_names, names_len, cudaMemcpyHostToDevice, ctx->stream));
     NPH_CUDA(ctx, cudaMemcpyAsync(d_noff, name_off, sizeof(uint32_t) * (n + 1), cudaMemcpyHostToDevice, ctx->stream));
     NPH_CUDA(ctx, cudaMemcpyAsync(d_rev, is_reverse, n, cudaMemcpyHostToDevice, ctx->stream));
-    uint64_t* rec_bytes = m.d_tsv_off.p;
-    uint64_t* rec_off = rec_bytes + n;                                  // n + 1 entries
-    int* d_refused = reinterpret_cast<int*>(rec_off + n + 1);
     NPH_CUDA(ctx, cudaMemsetAsync(d_refused, 0, sizeof(int), ctx->stream));
-    TsvArgs a{m.d_sites.p, m.d_counts.p + 3 * n, m.d_records.p, m.d_ref.p, d_contig, (uint32_t)contig_len,
+    TsvArgs a{m.d_sites.p, meth_counts(m).site_off, m.ev.d_records.p, m.ev.d_ref.p, d_contig, (uint32_t)contig_len,
               d_names, d_noff, d_rev, m.params.k, (uint32_t)n,
               rec_bytes, rec_off, nullptr, d_refused};
     const int grid = (int)std::min<size_t>((n + kWarps - 1) / kWarps, (size_t)ctx->sm_count * 8);
     meth_tsv_kernel<false><<<grid, kThreads, 0, ctx->stream>>>(a);
     NPH_CUDA(ctx, cudaGetLastError());
-    meth_tsv_prefix_kernel<<<1, 1024, 0, ctx->stream>>>(rec_bytes, (uint32_t)n, rec_off);
-    NPH_CUDA(ctx, cudaGetLastError());
+    NPH_TRY(nph_scan_exclusive(ctx, rec_bytes, (uint32_t)n, rec_off, scratch));
     uint64_t total = 0;
     int refused = 0;
     NPH_CUDA(ctx, cudaMemcpyAsync(&total, rec_off + n, sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
@@ -743,7 +721,7 @@ extern "C" int nph_methylation_tsv(nph_ctx* ctx, const char* contig, const char*
     NPH_CUDA(ctx, cudaGetLastError());
     NPH_CUDA(ctx, cudaMemcpyAsync(tsv_out, m.d_tsv.p, (size_t)total, cudaMemcpyDeviceToHost, ctx->stream));
     NPH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    ctx->last_launches += 3;
+    ctx->last_launches += 5;
     return NPH_OK;
 }
 
@@ -771,14 +749,13 @@ extern "C" int nph_methylation_fetch(nph_ctx* ctx, uint64_t* site_off_out, nph_m
     if (!ctx || !site_off_out) return NPH_ERR_INVALID;
     nph_ctx::MethState& m = ctx->meth;
     if (!m.ran) return NPH_ERR_STATE;
-    if (m.n_records == 0) { site_off_out[0] = 0; return NPH_OK; }
+    if (m.ev.n_records == 0) { site_off_out[0] = 0; return NPH_OK; }
     if (m.n_sites > sites_cap) {
         ctx->last_error = "sites_cap too small: " + std::to_string(m.n_sites) + " site records";
         return NPH_ERR_INVALID;
     }
     if (m.n_sites && !sites_out) return NPH_ERR_INVALID;
-    const uint64_t* site_off = m.d_counts.p + 3 * m.n_records;
-    NPH_CUDA(ctx, cudaMemcpyAsync(site_off_out, site_off, sizeof(uint64_t) * (m.n_records + 1), cudaMemcpyDeviceToHost, ctx->stream));
+    NPH_CUDA(ctx, cudaMemcpyAsync(site_off_out, meth_counts(m).site_off, sizeof(uint64_t) * (m.ev.n_records + 1), cudaMemcpyDeviceToHost, ctx->stream));
     if (m.n_sites)
         NPH_CUDA(ctx, cudaMemcpyAsync(sites_out, m.d_sites.p, sizeof(nph_meth_site) * (size_t)m.n_sites, cudaMemcpyDeviceToHost, ctx->stream));
     NPH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));

@@ -61,6 +61,18 @@ struct DevModel {
     uint32_t n_states = 0, k = 0, alphabet_size = 0;
 };
 
+// The event-aligned records of a call-methylation or screening batch: reference bytes, each record's event alignment as a pair
+// list or in compact form, the records.  Each record's [ref_off, ref_off + ref_len) indexes the n_map bases of the event map.
+struct NphEventRecords {
+    size_t n_records = 0, n_ref = 0, n_map = 0;
+    bool compact = false;                  // int16 deltas per base + first_event per record, expanded by nph_event_records_expand
+    DevBuf<uint8_t> d_ref;
+    DevBuf<nph_aligned_pair> d_pairs;      // pair form
+    DevBuf<uint16_t> d_deltas;             // compact form: n_map int16 deltas
+    DevBuf<uint8_t> d_dense;               // compact form: event index per base, first_event and first valid base per record
+    DevBuf<nph_meth_record> d_records;
+};
+
 struct nph_ctx {
     int device = 0;
     cudaStream_t stream = nullptr;
@@ -101,7 +113,7 @@ struct nph_ctx {
     DevBuf<unsigned int> d_counters;
     DevBuf<uint8_t> d_sched_cls;     // per job: kernel class
     DevBuf<uint16_t> d_sched_bkt;    // per job: schedule key bucket
-    DevBuf<unsigned int> d_sched_hist;   // histogram + offsets + summary
+    DevBuf<uint8_t> d_sched_hist;    // histogram, offsets, summary (hmm_schedule.cu)
     DevBuf<uint8_t> d_scratch;
     struct ClassLaunch { int cols_per_lane; int group_width; bool chained; size_t first; size_t count; double cost; };
     std::vector<ClassLaunch> classes;
@@ -126,22 +138,17 @@ struct nph_ctx {
     // resident call-methylation batch (methylation.cu)
     struct MethState {
         bool loaded = false, ran = false;
-        size_t n_records = 0, n_ref = 0, n_pairs = 0, prov_total = 0;
+        size_t prov_total = 0;
         nph_meth_params params{};
         double indel_bias = 1.0;
         uint64_t n_sites = 0, n_ranks = 0, n_scored_events = 0;
-        DevBuf<uint8_t> d_ref;
-        DevBuf<nph_aligned_pair> d_pairs;
-        bool compact = false;              // event alignments came as int16 deltas per reference base (nph_methylation_load_compact)
-        DevBuf<uint16_t> d_deltas;         // int16 deltas, n_ref entries
-        DevBuf<uint32_t> d_dense;          // int32 event index per reference base after the prefix sum (INT32_MIN: no pair), then per record: first_event, first valid offset
-        DevBuf<nph_meth_record> d_records;
+        NphEventRecords ev;                // pair lists (nph_methylation_load) or compact form (nph_methylation_load_compact)
         DevBuf<uint64_t> d_prov_off;       // n_records + 1: where each record's provisional group rows start
         DevBuf<uint8_t> d_prov;            // provisional group rows (MethGroup)
-        DevBuf<uint64_t> d_counts;         // per record: groups, ranks (2 x n_records), then the prefix arrays and the summary
+        DevBuf<uint8_t> d_counts;          // meth_counts_layout: per-record groups and ranks, their offsets, the summary
         DevBuf<nph_meth_site> d_sites;
         DevBuf<uint8_t> d_tsv_in;          // nph_methylation_tsv: contig, read names, name offsets, strand flags
-        DevBuf<uint64_t> d_tsv_off;        // bytes of each record's rows, then their exclusive prefix (n_records + 1) and the flags word
+        DevBuf<uint8_t> d_tsv_off;         // bytes of each record's rows, their exclusive prefix, the refusal flag
         DevBuf<uint8_t> d_tsv;             // the rows
         std::vector<uint64_t> h_prov_off;
     } meth;
@@ -151,18 +158,14 @@ struct nph_ctx {
         bool loaded = false, ran = false;
         nph_screen_params params{};
         double indel_bias = 1.0;
-        size_t n_pos = 0, n_records = 0, n_ref = 0, n_deltas = 0;
+        size_t n_pos = 0;
         uint32_t n_rounds = 0;
         uint64_t n_jobs = 0, n_scored_events = 0, n_jobs_no_exit = 0, n_reference_events = 0;
-        DevBuf<uint8_t> d_ref;
-        DevBuf<uint16_t> d_deltas;
-        DevBuf<uint32_t> d_dense;          // event index per reference base of every record, then first_event, first valid
-        DevBuf<nph_meth_record> d_records;
+        NphEventRecords ev;                // region reference, compact event alignments over n_map bases
         DevBuf<uint64_t> d_pos_off;        // n_pos + 1: where each position's bounded reads start
         DevBuf<uint8_t> d_pos_reads;       // {record, e1, e2} per bounded read
-        DevBuf<uint8_t> d_state;           // per position: totals (9 doubles), alive mask, reads done, valid mask; then the counters and
-                                           // per position the methylated-alternatives mask
-        DevBuf<uint64_t> d_job_off;        // per position: first job of the round (+ totals)
+        DevBuf<uint8_t> d_state;           // screen_state_layout: per-position state, counters, methylated-alternatives masks
+        DevBuf<uint8_t> d_job_off;         // per position: job count and first job of the round, scan scratch
         uint32_t n_types = 0;              // methylation types (nph_screen_load_methylation)
         std::vector<uint8_t> h_meth;       // their MethDev tables (meth_dev.cuh), the source of d_meth's upload
         DevBuf<uint8_t> d_meth;
@@ -266,6 +269,26 @@ __device__ __forceinline__ float4 nph_scaled_gaussian(const DevModelView& mv, co
     const float lsd = (float)__dadd_rn(mv.log_stdv[r], rd.log_var);
     return make_float4(mu, sd, __fsub_rn(log_inv_sqrt_2pi, lsd), __frcp_rn(sd));
 }
+
+// Inclusive sum of v over the block (blockDim.x a multiple of 32; every thread calls it), s: 32 values of shared memory.
+// Each warp scans by shuffles, then warp 0 scans the warp totals.
+template <typename T>
+__device__ __forceinline__ T nph_block_scan_incl(T v, T* s, int t)
+{
+    const int lane = t & 31, w = t >> 5;
+    for (int o = 1; o < 32; o <<= 1) { const T x = __shfl_up_sync(0xffffffffu, v, o); if (lane >= o) v += x; }
+    if (lane == 31) s[w] = v;
+    __syncthreads();
+    if (w == 0) {
+        T x = s[lane];
+        for (int o = 1; o < 32; o <<= 1) { const T y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
+        s[lane] = x;
+    }
+    __syncthreads();
+    if (w > 0) v += s[w - 1];
+    __syncthreads();
+    return v;
+}
 #endif
 
 // where the HMM jobs in ctx->d_jobs and their ranks come from
@@ -283,9 +306,20 @@ int nph_launch_abea(nph_ctx* ctx);
 int nph_schedule_hmm_jobs(nph_ctx* ctx, size_t n_jobs, size_t n_ranks_total, NphJobSource src, uint32_t* max_E_out);
 // per-read (lp_mm_self, lp_mm_next) of the resident reads into ctx->d_trans (host libm, like calculate_transitions)
 int nph_upload_read_transitions(nph_ctx* ctx, double indel_bias);
-// compact event alignments -> event index per reference base (methylation.cu): dense[ref_off + o] (INT32_MIN: no entry), first_valid[record]
-int nph_expand_event_maps(nph_ctx* ctx, const int16_t* d_deltas, const int32_t* d_first_event, const nph_meth_record* d_records, uint32_t n_records,
-                          int32_t* d_dense, int32_t* d_first_valid);
+// Checks every record (read and model index, its slice of the n_map bases, its pair-list slice, ref_len <= max_len, then
+// check(r, R)) and uploads the batch into ev (methylation.cu).  compact: deltas (n_map) and first_event; else pairs.
+int nph_event_records_load(nph_ctx* ctx, NphEventRecords& ev, const char* ref, size_t n_ref, size_t n_map, bool compact,
+                           const int16_t* deltas, const int32_t* first_event, const nph_aligned_pair* pairs, size_t n_pairs,
+                           const nph_meth_record* records, size_t n_records, uint32_t max_len,
+                           const std::function<int(size_t, const nph_meth_record&)>& check);
+// Compact form: the event index of every base (NPH_NO_EVENT: no entry) at dense[ref_off + o] and each record's first base with
+// an entry (ref_len: none) at first_valid[record].  Pair form: both nullptr, nothing launched.
+int nph_event_records_expand(nph_ctx* ctx, NphEventRecords& ev, const int32_t** dense, const int32_t** first_valid);
+constexpr int32_t NPH_NO_EVENT = INT32_MIN;
+// Exclusive prefix sum over n values on ctx->stream (scan.cu): out[0..n) the prefix, out[n] the total.  scratch holds
+// nph_scan_scratch(n) values from the caller's arena.
+size_t nph_scan_scratch(size_t n);
+int nph_scan_exclusive(nph_ctx* ctx, const uint64_t* in, uint32_t n, uint64_t* out, uint64_t* scratch);
 // validate + classify + schedule the n_jobs jobs already sitting in ctx->d_jobs / d_ranks (one stream sync), size the scratch
 int nph_jobs_schedule(nph_ctx* ctx, size_t n_jobs, size_t n_ranks_total, NphJobSource src);
 // Scores n_jobs jobs that emit() writes into ctx->d_jobs (ranks already in ctx->d_ranks, written by a kernel of ours): reserves

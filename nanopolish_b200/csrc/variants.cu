@@ -29,11 +29,8 @@
 #include <string>
 #include <vector>
 
-int nph_launch_hmm_forward(nph_ctx* ctx, float* scores_dev);
-
 namespace {
 
-constexpr int kNoEvent = INT32_MIN;
 constexpr int kSeqs = NPH_SCREEN_SLOTS + 1;      // nine candidates + the base haplotype (slot 9)
 constexpr int kBlock = 256;
 constexpr int kListCap = 2048;                   // records overlapping one block of positions, kept in shared memory
@@ -81,7 +78,7 @@ __device__ __forceinline__ uint64_t pool_slot(const VarDev& d, int pi, int seq, 
 // first offset >= from with an event-alignment entry (n: none)
 __device__ __forceinline__ int first_valid_from(const int32_t* __restrict__ dense, int n, int from)
 {
-    for (int o = from < 0 ? 0 : from; o < n; ++o) if (dense[o] != kNoEvent) return o;
+    for (int o = from < 0 ? 0 : from; o < n; ++o) if (dense[o] != NPH_NO_EVENT) return o;
     return n;
 }
 
@@ -160,70 +157,6 @@ __global__ void __launch_bounds__(kBlock) var_bounds_kernel(const VarDev d, cons
         }
     }
     if (!FILL) counts[pi] = cnt;
-}
-
-// exclusive prefix over n values: out[i], out[n] = total.  Three small launches (per-block sums, a one-block scan of the
-// sums, per-block scan with the block's base) instead of one block walking the whole array: 200 000 positions took 0.36 ms
-// per call in the one-block form, ten calls per screening.
-constexpr int kScanBlock = 1024;
-__device__ __forceinline__ unsigned long long block_scan_incl(unsigned long long v, unsigned long long* s /* 32 */, int t)
-{
-    const int lane = t & 31, w = t >> 5;
-    for (int o = 1; o < 32; o <<= 1) { const unsigned long long x = __shfl_up_sync(0xffffffffu, v, o); if (lane >= o) v += x; }
-    if (lane == 31) s[w] = v;
-    __syncthreads();
-    if (w == 0) {
-        unsigned long long x = s[lane];
-        for (int o = 1; o < 32; o <<= 1) { const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-        s[lane] = x;
-    }
-    __syncthreads();
-    if (w > 0) v += s[w - 1];
-    __syncthreads();
-    return v;
-}
-__global__ void __launch_bounds__(kScanBlock) prefix_sums_kernel(const uint64_t* __restrict__ in, uint32_t n, uint64_t* __restrict__ block_sum)
-{
-    __shared__ unsigned long long s[32];
-    const uint32_t i = blockIdx.x * kScanBlock + threadIdx.x;
-    const unsigned long long incl = block_scan_incl(i < n ? in[i] : 0ull, s, threadIdx.x);
-    if (threadIdx.x == kScanBlock - 1) block_sum[blockIdx.x] = incl;
-}
-__global__ void __launch_bounds__(kScanBlock) prefix_top_kernel(uint64_t* __restrict__ block_sum, uint32_t n_blocks, uint64_t* __restrict__ total)
-{
-    __shared__ unsigned long long s[32];
-    __shared__ unsigned long long carry;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
-    for (uint32_t base = 0; base < n_blocks; base += kScanBlock) {
-        const uint32_t i = base + threadIdx.x;
-        const unsigned long long v = i < n_blocks ? block_sum[i] : 0ull;
-        const unsigned long long incl = block_scan_incl(v, s, threadIdx.x);
-        if (i < n_blocks) block_sum[i] = carry + incl - v;
-        __syncthreads();
-        if (threadIdx.x == kScanBlock - 1) carry += incl;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *total = carry;
-}
-__global__ void __launch_bounds__(kScanBlock) prefix_apply_kernel(const uint64_t* __restrict__ in, uint32_t n, const uint64_t* __restrict__ block_base,
-                                                                  uint64_t* __restrict__ out)
-{
-    __shared__ unsigned long long s[32];
-    const uint32_t i = blockIdx.x * kScanBlock + threadIdx.x;
-    const unsigned long long v = i < n ? in[i] : 0ull;
-    const unsigned long long incl = block_scan_incl(v, s, threadIdx.x);
-    if (i < n) out[i] = block_base[blockIdx.x] + incl - v;
-}
-// scratch: (n + 1023) / 1024 entries
-static int prefix_exclusive(nph_ctx* ctx, const uint64_t* in, uint32_t n, uint64_t* out, uint64_t* scratch, cudaStream_t st)
-{
-    const uint32_t nb = (n + kScanBlock - 1) / kScanBlock;
-    prefix_sums_kernel<<<nb, kScanBlock, 0, st>>>(in, n, scratch);
-    prefix_top_kernel<<<1, kScanBlock, 0, st>>>(scratch, nb, out + n);
-    prefix_apply_kernel<<<nb, kScanBlock, 0, st>>>(in, n, scratch, out);
-    if (cudaGetLastError() != cudaSuccess) { ctx->last_error = "prefix kernels failed to launch"; return NPH_ERR_CUDA; }
-    return NPH_OK;
 }
 
 // the sequence of slot `seq` at a position: the window (characters) with the slot's edit applied, length returned.
@@ -452,7 +385,7 @@ __global__ void var_output_kernel(const VarDev d, const PosState* __restrict__ s
     if ((threadIdx.x & 31) == 0 && full) atomicAdd(no_exit, full);
 }
 
-int make_dev(nph_ctx* ctx, const nph_screen_params& p, size_t n_ref, VarDev& d)
+int make_dev(nph_ctx* ctx, const nph_screen_params& p, size_t n_ref, uint32_t n_types, VarDev& d)
 {
     if (p.flank < 1 || 2 * p.flank + 3 > NPH_SCREEN_MAX_WINDOW) { ctx->last_error = "nph_screen_params: flank outside 1..30"; return NPH_ERR_UNSUPPORTED; }
     if (p.k < 1 || (int)p.k > 2 * p.flank + 1 || p.reads_per_round == 0 || n_ref < 2 || n_ref > 0x7fffffffu) return NPH_ERR_INVALID;
@@ -460,8 +393,22 @@ int make_dev(nph_ctx* ctx, const nph_screen_params& p, size_t n_ref, VarDev& d)
     d.k = (int)p.k; d.rpr = (int)p.reads_per_round; d.flags = p.alignment_flags; d.threshold = p.score_threshold;
     d.win = 2 * p.flank + 2;
     d.stride = d.win + 1 - d.k + 1;
-    d.T = 0;
+    d.T = (int)n_types;
     return NPH_OK;
+}
+
+// the counters of a screening: scored events, the reference's scored events, whether any position has reads left
+struct ScreenCounters { unsigned long long events, ref_events; unsigned int any_left; };
+
+// d_state: per-position state | the counters | per position the methylated-alternatives mask
+struct ScreenStateLayout { PosState* state; ScreenCounters* counters; unsigned long long* alts; };
+ScreenStateLayout screen_state_layout(NphArena& a, size_t n_pos)
+{
+    ScreenStateLayout l;
+    l.state = a.take<PosState>(n_pos);
+    l.counters = a.take<ScreenCounters>(1);
+    l.alts = a.take<unsigned long long>(n_pos);
+    return l;
 }
 
 } // namespace
@@ -477,7 +424,7 @@ extern "C" int nph_screen_load_methylation(nph_ctx* ctx, const char* ref_bases, 
     if (!meth) return NPH_ERR_INVALID;
     if (!ctx->reads_loaded) return NPH_ERR_STATE;
     VarDev d;
-    NPH_TRY(make_dev(ctx, *params, n_ref_bases, d));
+    NPH_TRY(make_dev(ctx, *params, n_ref_bases, meth->n_types, d));
     const uint32_t T = meth->n_types;
     if (T > NPH_SCREEN_MAX_TYPES) { ctx->last_error = "nph_screen_methylation: more than NPH_SCREEN_MAX_TYPES types"; return NPH_ERR_INVALID; }
     if (T && n_records && !alt_model_ids) return NPH_ERR_INVALID;
@@ -486,11 +433,9 @@ extern "C" int nph_screen_load_methylation(nph_ctx* ctx, const char* ref_bases, 
         NPH_TRY(nph_meth_alphabet(ctx, meth->alphabets[t], md[t]));
         if (md[t].k != params->k) { ctx->last_error = "nph_screen_methylation: type " + std::to_string(t) + " has k != params.k"; return NPH_ERR_INVALID; }
     }
-    for (size_t r = 0; r < n_records; ++r) {
-        const nph_meth_record& R = records[r];
-        const bool ok = R.read < ctx->n_reads && R.model_id < ctx->models.size() && R.ref_len <= n_deltas_total && R.ref_off <= n_deltas_total - R.ref_len &&
-                        R.ref_len <= 0x3fffffffu;
-        if (!ok) { ctx->last_error = "screening record " + std::to_string(r) + " is out of range (read, model or event-alignment slice)"; return NPH_ERR_INVALID; }
+    // records index the event deltas, not the region's reference
+    NPH_TRY(nph_event_records_load(ctx, m.ev, ref_bases, n_ref_bases, n_deltas_total, true, event_deltas, first_event, nullptr, 0,
+                                   records, n_records, 0x3fffffffu, [&](size_t r, const nph_meth_record& R) {
         const DevModel& mod = ctx->models[R.model_id];
         if (mod.k != params->k || mod.alphabet_size != 4) { ctx->last_error = "screening record " + std::to_string(r) + ": its model is not a nucleotide model of k = params.k"; return NPH_ERR_INVALID; }
         for (uint32_t t = 0; t < T; ++t) {
@@ -501,12 +446,8 @@ extern "C" int nph_screen_load_methylation(nph_ctx* ctx, const char* ref_bases, 
                 return NPH_ERR_INVALID;
             }
         }
-    }
-    NPH_CUDA(ctx, cudaSetDevice(ctx->device));
-    NPH_TRY(nph_reserve(ctx, m.d_ref, n_ref_bases + 16));
-    NPH_TRY(nph_reserve(ctx, m.d_deltas, n_deltas_total + 16));
-    NPH_TRY(nph_reserve(ctx, m.d_dense, n_deltas_total + 2 * n_records + 16));
-    NPH_TRY(nph_reserve(ctx, m.d_records, n_records + 1));
+        return NPH_OK;
+    }));
     m.h_meth.resize(sizeof(MethDev) * T);
     if (T) {
         std::memcpy(m.h_meth.data(), md.data(), m.h_meth.size());
@@ -516,14 +457,8 @@ extern "C" int nph_screen_load_methylation(nph_ctx* ctx, const char* ref_bases, 
         if (n_records) NPH_CUDA(ctx, cudaMemcpyAsync(m.d_alt_models.p, alt_model_ids, sizeof(uint32_t) * n_records * T, cudaMemcpyHostToDevice, ctx->stream));
     }
     m.n_types = T;
-    NPH_CUDA(ctx, cudaMemcpyAsync(m.d_ref.p, ref_bases, n_ref_bases, cudaMemcpyHostToDevice, ctx->stream));
-    if (n_records) {
-        NPH_CUDA(ctx, cudaMemcpyAsync(m.d_records.p, records, sizeof(nph_meth_record) * n_records, cudaMemcpyHostToDevice, ctx->stream));
-        if (n_deltas_total) NPH_CUDA(ctx, cudaMemcpyAsync(m.d_deltas.p, event_deltas, sizeof(int16_t) * n_deltas_total, cudaMemcpyHostToDevice, ctx->stream));
-        NPH_CUDA(ctx, cudaMemcpyAsync(m.d_dense.p + n_deltas_total, first_event, sizeof(int32_t) * n_records, cudaMemcpyHostToDevice, ctx->stream));
-    }
     m.params = *params; m.indel_bias = indel_bias;
-    m.n_pos = (size_t)d.n_pos; m.n_records = n_records; m.n_ref = n_ref_bases; m.n_deltas = n_deltas_total;
+    m.n_pos = (size_t)d.n_pos;
     m.loaded = true;
     return NPH_OK;
 }
@@ -545,80 +480,80 @@ extern "C" int nph_screen_run(nph_ctx* ctx)
     m.ran = false; m.n_rounds = 0; m.n_jobs = 0; m.n_scored_events = 0; m.n_jobs_no_exit = 0; m.n_reference_events = 0;
     NPH_CUDA(ctx, cudaSetDevice(ctx->device));
     VarDev d;
-    NPH_TRY(make_dev(ctx, m.params, m.n_ref, d));
-    d.T = (int)m.n_types;
-    const uint32_t n_pos = (uint32_t)m.n_pos, n_rec = (uint32_t)m.n_records;
+    NPH_TRY(make_dev(ctx, m.params, m.ev.n_ref, m.n_types, d));
+    const uint32_t n_pos = (uint32_t)m.n_pos, n_rec = (uint32_t)m.ev.n_records;
+    const nph_meth_record* records = m.ev.d_records.p;
     cudaStream_t st = ctx->stream;
-    int32_t* dense = reinterpret_cast<int32_t*>(m.d_dense.p);
-    int32_t* first_valid = dense + m.n_deltas + m.n_records;
-    NPH_TRY(nph_expand_event_maps(ctx, reinterpret_cast<const int16_t*>(m.d_deltas.p), dense + m.n_deltas, m.d_records.p, n_rec, dense, first_valid));
+    const int32_t* dense;
+    const int32_t* first_valid;
+    NPH_TRY(nph_event_records_expand(ctx, m.ev, &dense, &first_valid));
     // per position: its event sequences
     NPH_TRY(nph_reserve(ctx, m.d_pos_off, (size_t)n_pos + 1));
-    NPH_TRY(nph_reserve(ctx, m.d_job_off, 2 * ((size_t)n_pos + 1) + 8 + ((size_t)n_pos + 1023) / 1024 + 1));
-    uint64_t* counts = m.d_job_off.p;                         // scratch: per-position counts, then per-round job counts / offsets
-    uint64_t* job_off = m.d_job_off.p + (size_t)n_pos + 1;
-    uint64_t* scan_scratch = job_off + (size_t)n_pos + 1 + 8;
+    uint64_t* counts; uint64_t* job_off; uint64_t* scan_scratch;     // per-position counts (reads, then each round's jobs) and job offsets
+    NPH_TRY(nph_carve(ctx, m.d_job_off, [&](NphArena& a) {
+        counts = a.take<uint64_t>(n_pos);
+        job_off = a.take<uint64_t>((size_t)n_pos + 1);
+        scan_scratch = a.take<uint64_t>(nph_scan_scratch(n_pos));
+    }));
     const int pgrid = (int)((n_pos + kBlock - 1) / kBlock);
-    var_bounds_kernel<false><<<pgrid, kBlock, 0, st>>>(d, m.d_records.p, n_rec, dense, first_valid, counts, nullptr, nullptr);
+    var_bounds_kernel<false><<<pgrid, kBlock, 0, st>>>(d, records, n_rec, dense, first_valid, counts, nullptr, nullptr);
     NPH_CUDA(ctx, cudaGetLastError());
-    NPH_TRY(prefix_exclusive(ctx, counts, n_pos, m.d_pos_off.p, scan_scratch, st));
+    NPH_TRY(nph_scan_exclusive(ctx, counts, n_pos, m.d_pos_off.p, scan_scratch));
     uint64_t n_pos_reads = 0;
     NPH_CUDA(ctx, cudaMemcpyAsync(&n_pos_reads, m.d_pos_off.p + n_pos, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
     NPH_CUDA(ctx, cudaStreamSynchronize(st));
     NPH_TRY(nph_reserve(ctx, m.d_pos_reads, sizeof(PosRead) * ((size_t)n_pos_reads + 1)));
     PosRead* pos_reads = reinterpret_cast<PosRead*>(m.d_pos_reads.p);
-    var_bounds_kernel<true><<<pgrid, kBlock, 0, st>>>(d, m.d_records.p, n_rec, dense, first_valid, nullptr, m.d_pos_off.p, pos_reads);
+    var_bounds_kernel<true><<<pgrid, kBlock, 0, st>>>(d, records, n_rec, dense, first_valid, nullptr, m.d_pos_off.p, pos_reads);
     NPH_CUDA(ctx, cudaGetLastError());
     // rank pool (K1's d_ranks for this batch: per position, sequence and alternative both strands) and position state
     const size_t pool = (size_t)n_pos * kSeqs * (size_t)(1 + d.T) * 2 * (size_t)d.stride;
     NPH_TRY(nph_reserve(ctx, ctx->d_ranks, pool));
-    // + the counters (our DP rows, a flag, the reference's DP rows) in 64 bytes, then the alternatives mask per position
-    NPH_TRY(nph_reserve(ctx, m.d_state, sizeof(PosState) * (size_t)n_pos + 64 + sizeof(unsigned long long) * (size_t)n_pos));
-    PosState* state = reinterpret_cast<PosState*>(m.d_state.p);
+    ScreenStateLayout sl;
+    NPH_TRY(nph_carve(ctx, m.d_state, [&](NphArena& a) { sl = screen_state_layout(a, n_pos); }));
+    PosState* state = sl.state;
     VarMeth vm{};
     vm.types = reinterpret_cast<const MethDev*>(m.d_meth.p);
     vm.alt_model = m.d_alt_models.p;
-    vm.alts = reinterpret_cast<unsigned long long*>(m.d_state.p + sizeof(PosState) * (size_t)n_pos + 64);
+    vm.alts = sl.alts;
     vm.tbl = ctx->d_logsum.p;
     for (int n = 1; n <= 1 + d.T; ++n) vm.pen[n - 1] = log((double)n);      // profile_hmm_score_set's log(num_models), host libm
     NPH_CUDA(ctx, cudaMemsetAsync(ctx->d_ranks.p, 0, sizeof(uint32_t) * pool, st));
     if (d.T) NPH_CUDA(ctx, cudaMemsetAsync(vm.alts, 0, sizeof(unsigned long long) * (size_t)n_pos, st));
     const long long n_thr = (long long)n_pos * kSeqs * (1 + d.T);
-    var_ranks_kernel<<<(unsigned)((n_thr + kBlock - 1) / kBlock), kBlock, 0, st>>>(d, m.d_ref.p, ctx->d_ranks.p, state, m.d_pos_off.p, vm);
+    var_ranks_kernel<<<(unsigned)((n_thr + kBlock - 1) / kBlock), kBlock, 0, st>>>(d, m.ev.d_ref.p, ctx->d_ranks.p, state, m.d_pos_off.p, vm);
     NPH_CUDA(ctx, cudaGetLastError());
-    unsigned long long* d_events = reinterpret_cast<unsigned long long*>(m.d_state.p + sizeof(PosState) * (size_t)n_pos);
-    unsigned int* d_any = reinterpret_cast<unsigned int*>(d_events + 1);
-    NPH_CUDA(ctx, cudaMemsetAsync(d_events, 0, 24, st));
+    ScreenCounters* ctr = sl.counters;
+    NPH_CUDA(ctx, cudaMemsetAsync(ctr, 0, sizeof(ScreenCounters), st));
     float kernel_ms_total = 0.f;
     int launches_total = 0;
     for (;;) {
         var_round_count_kernel<<<pgrid, kBlock, 0, st>>>(d, state, m.d_pos_off.p, counts, vm.alts);
         NPH_CUDA(ctx, cudaGetLastError());
-        NPH_TRY(prefix_exclusive(ctx, counts, n_pos, job_off, scan_scratch, st));
-        NPH_CUDA(ctx, cudaGetLastError());
+        NPH_TRY(nph_scan_exclusive(ctx, counts, n_pos, job_off, scan_scratch));
         uint64_t n_jobs = 0;
         NPH_CUDA(ctx, cudaMemcpyAsync(&n_jobs, job_off + n_pos, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
         NPH_CUDA(ctx, cudaStreamSynchronize(st));                         // read-back: the round's job count
         if (n_jobs == 0) break;
         // var_emit_kernel writes the round's jobs over the pool var_ranks_kernel wrote; the schedule is one more read-back
         NPH_TRY(nph_score_device_jobs(ctx, (size_t)n_jobs, pool, m.indel_bias, [&]() -> int {
-            var_emit_kernel<<<pgrid, kBlock, 0, st>>>(d, state, m.d_pos_off.p, pos_reads, m.d_records.p, job_off, ctx->d_jobs.p, d_events, vm);
+            var_emit_kernel<<<pgrid, kBlock, 0, st>>>(d, state, m.d_pos_off.p, pos_reads, records, job_off, ctx->d_jobs.p, &ctr->events, vm);
             NPH_CUDA(ctx, cudaGetLastError());
             return NPH_OK;
         }));
-        NPH_CUDA(ctx, cudaMemsetAsync(d_any, 0, sizeof(unsigned int), st));
-        var_accumulate_kernel<<<pgrid, kBlock, 0, st>>>(d, state, job_off, ctx->d_scores.p, d_any, m.d_pos_off.p, pos_reads, d_events + 2, vm);
+        NPH_CUDA(ctx, cudaMemsetAsync(&ctr->any_left, 0, sizeof(unsigned int), st));
+        var_accumulate_kernel<<<pgrid, kBlock, 0, st>>>(d, state, job_off, ctx->d_scores.p, &ctr->any_left, m.d_pos_off.p, pos_reads, &ctr->ref_events, vm);
         NPH_CUDA(ctx, cudaGetLastError());
         float ms = 0.f; int nl = 0;
         if (nph_last_kernel_ms(ctx, &ms, &nl) == NPH_OK) { kernel_ms_total += ms; launches_total += nl + 6; }
         m.n_rounds += 1;
         m.n_jobs += n_jobs;
     }
-    unsigned long long ev[3] = {0, 0, 0};
-    NPH_CUDA(ctx, cudaMemcpyAsync(ev, d_events, sizeof(ev), cudaMemcpyDeviceToHost, st));
+    ScreenCounters h{};
+    NPH_CUDA(ctx, cudaMemcpyAsync(&h, ctr, sizeof(h), cudaMemcpyDeviceToHost, st));
     NPH_CUDA(ctx, cudaStreamSynchronize(st));
-    m.n_scored_events = ev[0];
-    m.n_reference_events = ev[2];
+    m.n_scored_events = h.events;
+    m.n_reference_events = h.ref_events;
     nph_timing_staged(ctx, kernel_ms_total, launches_total);
     m.ran = true;
     return NPH_OK;
@@ -644,8 +579,7 @@ extern "C" int nph_screen_fetch(nph_ctx* ctx, double* qualities_out, uint32_t* n
     nph_ctx::ScreenState& m = ctx->screen;
     if (!m.ran) return NPH_ERR_STATE;
     VarDev d;
-    NPH_TRY(make_dev(ctx, m.params, m.n_ref, d));
-    d.T = (int)m.n_types;
+    NPH_TRY(make_dev(ctx, m.params, m.ev.n_ref, m.n_types, d));
     const uint32_t n_pos = (uint32_t)m.n_pos;
     // outputs staged in the (now idle) prologue buffer: per position the slot qualities, reference rows and read count
     const size_t b_q = sizeof(double) * NPH_SCREEN_SLOTS * (size_t)n_pos, b_n = sizeof(uint32_t) * (size_t)n_pos;
@@ -657,10 +591,10 @@ extern "C" int nph_screen_fetch(nph_ctx* ctx, double* qualities_out, uint32_t* n
         d_n = a.take<uint32_t>(n_pos);
         d_full = a.take<unsigned long long>(1);
     }));
-    const unsigned long long* alts = reinterpret_cast<const unsigned long long*>(m.d_state.p + sizeof(PosState) * (size_t)n_pos + 64);
+    NphArena sa{m.d_state.p};
+    const ScreenStateLayout sl = screen_state_layout(sa, n_pos);
     NPH_CUDA(ctx, cudaMemsetAsync(d_full, 0, sizeof(unsigned long long), ctx->stream));
-    var_output_kernel<<<(n_pos + kBlock - 1) / kBlock, kBlock, 0, ctx->stream>>>(d, reinterpret_cast<const PosState*>(m.d_state.p), m.d_pos_off.p, d_q, d_n, d_r,
-                                                                                 alts, d_full);
+    var_output_kernel<<<(n_pos + kBlock - 1) / kBlock, kBlock, 0, ctx->stream>>>(d, sl.state, m.d_pos_off.p, d_q, d_n, d_r, sl.alts, d_full);
     NPH_CUDA(ctx, cudaGetLastError());
     NPH_CUDA(ctx, cudaMemcpyAsync(qualities_out, d_q, b_q, cudaMemcpyDeviceToHost, ctx->stream));
     if (n_reads_out) NPH_CUDA(ctx, cudaMemcpyAsync(n_reads_out, d_n, b_n, cudaMemcpyDeviceToHost, ctx->stream));

@@ -25,9 +25,13 @@ def _expected(port_oracle, rs, models, ref_bases, pairs, records, alphabet, **kw
     return site_rows, jobs, scores
 
 
-def _check(engine, port_oracle, rs, models, ref_bases, pairs, records, alphabet, **kw):
+def _check(engine, port_oracle, rs, models, ref_bases, pairs, records, alphabet, compact=False, **kw):
     params = synth.meth_params(alphabet, K, **kw)
-    site_off, sites, scored = engine.methylation_batch(rs.reads, rs.ev_mean, rs.ev_start_time, ref_bases, pairs, records, params)
+    if compact:
+        deltas, first = synth.compact_event_alignment(records, pairs, ref_bases.shape[0])
+        site_off, sites, scored = engine.methylation_batch_compact(rs.reads, rs.ev_mean, rs.ev_start_time, ref_bases, deltas, first, records, params)
+    else:
+        site_off, sites, scored = engine.methylation_batch(rs.reads, rs.ev_mean, rs.ev_start_time, ref_bases, pairs, records, params)
     rows, jobs, scores = _expected(port_oracle, rs, models, ref_bases, pairs, records, alphabet, **kw)
     assert sites.shape[0] == len(rows)
     want_off = np.zeros(records.shape[0] + 1, np.uint64)
@@ -118,6 +122,22 @@ def test_dam_alphabet(port_oracle):
         assert sites.shape[0] > 100
     finally:
         e.close()
+
+
+@pytest.mark.parametrize("compact", [False, True])
+@pytest.mark.parametrize("n_records", [1, 1023, 1024, 1025, 3073])
+def test_record_counts_around_the_scan_block(eng2, port_oracle, n_records, compact):
+    """The site and rank offsets are exclusive scans over the records in blocks of 1 024: short records, one to three blocks
+    and a record past them; the TSV byte offsets are the same scan over the records."""
+    rs, models, ref, pairs, recs = _batch(n_records, 200, 501 + n_records)
+    sites = _check(eng2, port_oracle, rs, models, ref, pairs, recs, "cpg", compact=compact)
+    assert sites.shape[0] > 0
+    if n_records == 3073:
+        site_off = np.zeros(n_records + 1, np.uint64)
+        site_off[1:] = np.cumsum(np.bincount(sites["record"], minlength=n_records))
+        names = ["r%d" % i for i in range(n_records)]
+        is_rev = (np.arange(n_records) % 2).astype(np.uint8)
+        assert eng2.methylation_tsv("chr20", names, is_rev).decode() == _expected_rows(sites, site_off, recs, ref, names, is_rev, "chr20", K)
 
 
 def test_staged_form_matches_one_shot(eng2):
