@@ -433,6 +433,41 @@ int nph_methylation_batch_compact_tsv(nph_ctx* ctx,
                                       char* tsv_out, size_t cap, uint64_t* n_bytes_out,
                                       uint64_t* n_sites_out, uint64_t* n_scored_events_out);
 
+/* ---- call-methylation: per-site methylation frequency accumulated on the device ------------------------------------------
+ * The table the reference's scripts/calculate_methylation_frequency.py builds from methylation_calls.tsv (chromosome, start, end,
+ * num_motifs_in_group, called_sites, called_sites_methylated, methylated_frequency, group_sequence), kept on the device while
+ * batches are scored, so that a caller who wants frequencies needs neither the TSV nor the script.  Folding the batches in order
+ * gives the script's output for the concatenation of the batches' TSV rows, byte for byte:
+ *   a row is skipped when abs(llr) < call_threshold * num_motifs (llr: the row's printed "%.2lf" log_lik_ratio, as the script
+ *   parses it) and is methylated when llr > 0; it counts num_motifs calls at (chromosome, start, end), or, with split_groups and
+ *   num_motifs > 1, one call per "CG" of its sequence column (overlapping matches too) at (chromosome, start + offset of that CG
+ *   from the first, same) with group size 1 and sequence "split-group"; a key keeps the group size and sequence of the first row
+ *   that created it.
+ * The accumulator belongs to the context (freed by nph_destroy) and grows on the device as keys arrive. */
+typedef struct {
+    double   call_threshold;  /* -c (2.0) */
+    uint32_t split_groups;    /* -s: nonzero splits multi-site groups into their CpGs */
+    uint32_t reserved;
+} nph_methfreq_params;
+/* Empties the accumulator and sets its parameters (NULL: the script's defaults, 2.0 and no split).  A context starts with an
+ * empty accumulator and the defaults. */
+int nph_methfreq_reset(nph_ctx* ctx, const nph_methfreq_params* params);
+/* Folds the rows of the most recent call-methylation run on this context (the rows nph_methylation_tsv would write, in its
+ * order; the same one-strand contract) under contig_id (< 2^20; its name is given to nph_methfreq_tsv).  Call it before the
+ * next run on the context: the run replaces the site records.  One small read-back; no per-site work on the host.
+ * NPH_ERR_STATE without a run.  A refused batch leaves the accumulator unchanged: NPH_ERR_UNSUPPORTED for a likelihood that is
+ * not finite or beyond 2^52, a printed ratio of 2^53 / 100 or more, a negative start or a group spanning 2^13 bases or more;
+ * NPH_ERR_INVALID for a group whose sequence column would start before its record's reference (as nph_methylation_tsv). */
+int nph_methfreq_add(nph_ctx* ctx, uint32_t contig_id);
+/* distinct keys, calls counted (rows that passed the threshold; one per CpG of a split group), rows skipped by the threshold */
+int nph_methfreq_counts(nph_ctx* ctx, uint64_t* n_keys_out, uint64_t* n_calls_out, uint64_t* n_ambiguous_out);
+/* The frequency table so far: the header and one row per key, sorted by (name, start, end) as Python sorts them (names bytewise).
+ * names + name_off (n_contigs + 1 offsets into names, no terminators): the name of each contig id.  out receives *n_bytes_out
+ * bytes (no terminator); the accumulator is kept, so folding may go on.  NPH_ERR_INVALID with *n_bytes_out set if cap was too
+ * small; NPH_ERR_INVALID for duplicate names or a folded contig id without a name. */
+int nph_methfreq_tsv(nph_ctx* ctx, const char* names, const uint32_t* name_off, uint32_t n_contigs,
+                     char* out, size_t cap, uint64_t* n_bytes_out);
+
 /* ---- variants: candidate screening on the device (section 8f N2, BASELINE configs[4]) -----------------------------
  * generate_candidate_single_base_edits (src/nanopolish_call_variants.cpp:288-361) for a reference region: at every position i
  * the window [i - flank, i + 1 + flank] (22 bases for flank 10), up to nine candidate edits of base i — for j in ACGT order

@@ -70,6 +70,10 @@ def load() -> C.CDLL:
     lib.nph_methylation_fetch.argtypes = [vp, vp, vp, sz]
     lib.nph_methylation_sites_dev.argtypes = [vp, vp, vp]
     lib.nph_methylation_tsv.argtypes = [vp, C.c_char_p, vp, vp, vp, vp, C.c_size_t, vp]
+    lib.nph_methfreq_reset.argtypes = [vp, vp]
+    lib.nph_methfreq_add.argtypes = [vp, u32]
+    lib.nph_methfreq_counts.argtypes = [vp, vp, vp, vp]
+    lib.nph_methfreq_tsv.argtypes = [vp, vp, vp, u32, vp, sz, vp]
     lib.nph_screen_edits_batch.argtypes = [vp, vp, sz, vp, vp, sz, vp, sz, vp, sz, vp, vp, sz, vp, dbl, vp, vp, vp]
     lib.nph_screen_load.argtypes = [vp, vp, sz, vp, sz, vp, vp, sz, vp, dbl]
     lib.nph_screen_run.argtypes = [vp]
@@ -89,5 +93,5 @@ EXPORTS = [
     "nph_sync", "nph_stream", "nph_model_upload", "nph_hmm_score_batch", "nph_hmm_score_batch_seq", "nph_hmm_jobs_load_seq", "nph_reads_load",
     "nph_hmm_jobs_load", "nph_hmm_score", "nph_hmm_scores_fetch", "nph_score_set_combine",
     "nph_abea_batch", "nph_abea_jobs_load", "nph_abea_run", "nph_abea_fetch", "nph_mom_batch",
-    "nph_hmm_align_batch", "nph_hmm_align", "nph_eventalign_chain", "nph_detect_events_batch", "nph_trim_raw_batch", "nph_recalibrate_batch", "nph_load_from_raw_batch", "nph_last_trim_ranges", "nph_methylation_batch", "nph_methylation_batch_compact", "nph_methylation_load", "nph_methylation_load_compact", "nph_methylation_run", "nph_methylation_counts", "nph_methylation_fetch", "nph_methylation_sites_dev", "nph_methylation_tsv", "nph_methylation_batch_compact_tsv", "nph_screen_edits_batch", "nph_screen_load", "nph_screen_run", "nph_screen_counts", "nph_screen_fetch", "nph_screen_load_methylation", "nph_screen_edits_batch_methylation", "nph_last_kernel_ms", "nph_host_alloc", "nph_host_free",
+    "nph_hmm_align_batch", "nph_hmm_align", "nph_eventalign_chain", "nph_detect_events_batch", "nph_trim_raw_batch", "nph_recalibrate_batch", "nph_load_from_raw_batch", "nph_last_trim_ranges", "nph_methylation_batch", "nph_methylation_batch_compact", "nph_methylation_load", "nph_methylation_load_compact", "nph_methylation_run", "nph_methylation_counts", "nph_methylation_fetch", "nph_methylation_sites_dev", "nph_methylation_tsv", "nph_methylation_batch_compact_tsv", "nph_methfreq_reset", "nph_methfreq_add", "nph_methfreq_counts", "nph_methfreq_tsv", "nph_screen_edits_batch", "nph_screen_load", "nph_screen_run", "nph_screen_counts", "nph_screen_fetch", "nph_screen_load_methylation", "nph_screen_edits_batch_methylation", "nph_last_kernel_ms", "nph_host_alloc", "nph_host_free",
 ]

@@ -25,7 +25,6 @@
 // into its site record.  The host sees O(records) work only.
 #include "nph_internal.cuh"
 #include "meth_dev.cuh"
-#include "tsv_format.cuh"
 #include <algorithm>
 #include <cstring>
 #include <string>
@@ -578,25 +577,6 @@ struct TsvArgs {
     char* out;
     int* refused;                      // set when a value needs the C library (non-finite, |v| >= 2^52)
 };
-
-struct RowNums { nph_tsv::Fixed2 diff, m, u; uint32_t seq_b, seq_len; bool seq_ok; };
-
-__device__ __forceinline__ RowNums row_numbers(const nph_meth_site& ms, const nph_meth_record& R, uint32_t k)
-{
-    RowNums r;
-    // ScoredSite: ll_*[strand] = the float score, the other strand 0.0; the writer sums the two strands in double
-    const double sum_m = __dadd_rn((double)ms.ll_methylated, 0.0), sum_u = __dadd_rn((double)ms.ll_unmethylated, 0.0);
-    r.diff = nph_tsv::fixed2_of(__dsub_rn(sum_m, sum_u));
-    r.m = nph_tsv::fixed2_of(sum_m);
-    r.u = nph_tsv::fixed2_of(sum_u);
-    // the sequence column starts k - 1 bases before the first site: a window parameter set that lets a group start closer to the
-    // beginning of the record's reference than that makes the reference's substr throw; here the call is refused
-    const int bs = (ms.start_position - R.ref_start_pos) - (int)k + 1;
-    const uint32_t e = min((uint32_t)(ms.end_position - R.ref_start_pos) + k, R.ref_len);
-    r.seq_ok = bs >= 0 && (uint32_t)bs <= e;
-    r.seq_b = r.seq_ok ? (uint32_t)bs : 0u; r.seq_len = r.seq_ok ? e - (uint32_t)bs : 0u;
-    return r;
-}
 
 __device__ __forceinline__ uint32_t row_len(const TsvArgs& a, const nph_meth_site& ms, const RowNums& r, uint32_t name_len)
 {

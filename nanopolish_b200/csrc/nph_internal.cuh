@@ -153,6 +153,19 @@ struct nph_ctx {
         std::vector<uint64_t> h_prov_off;
     } meth;
 
+    // per-site methylation frequency accumulated over call-methylation batches (meth_frequency.cu)
+    struct FreqState {
+        nph_methfreq_params params{2.0, 0, 0};
+        size_t slots = 0;                  // hash table slots, a power of two (0: no accumulator yet)
+        uint32_t n_batches = 0;            // folds so far: the batch part of the first-row ordinals
+        uint64_t n_calls = 0, n_ambiguous = 0;
+        DevBuf<uint8_t> d_summary;         // the accumulator's key and pool counters, the fold's batch counts
+        DevBuf<uint8_t> d_table;           // keys, first-row ordinals, called, methylated, sequence offsets, group info per slot
+        DevBuf<uint8_t> d_pool;            // sequence bytes of the keys' first rows
+        DevBuf<uint8_t> d_work;            // nph_methfreq_tsv: names, ranks, compaction, sort and row offsets
+        DevBuf<uint8_t> d_out;             // nph_methfreq_tsv: the rows
+    } freq;
+
     // resident variant-screening batch (variants.cu)
     struct ScreenState {
         bool loaded = false, ran = false;

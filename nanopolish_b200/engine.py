@@ -10,7 +10,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from .synth import ABEA_RES_DT, ALIGN_STATE_DT, CALIBRATION_DT, EVENT_DT, EVENT_RANGE_DT, METH_SITE_DT, PAIR_DT, RAW_RANGE_DT
+from .synth import ABEA_RES_DT, ALIGN_STATE_DT, CALIBRATION_DT, EVENT_DT, EVENT_RANGE_DT, METH_SITE_DT, METHFREQ_PARAMS_DT, PAIR_DT, RAW_RANGE_DT
 
 
 def _p(a):
@@ -121,6 +121,39 @@ class Engine:
         site_off, sites = out if out is not None else (np.zeros(self._meth_n + 1, np.uint64), np.zeros(max(n_sites, 1), METH_SITE_DT))
         self._check(self.lib.nph_methylation_fetch(self.ctx, _p(site_off), _p(sites), sites.shape[0]), "nph_methylation_fetch")
         return site_off, sites[:n_sites]
+
+    # ---- call-methylation: per-site methylation frequency on the device (calculate_methylation_frequency.py) ----
+    def methylation_frequency_reset(self, call_threshold: float = 2.0, split_groups: bool = False):
+        """nph_methfreq_reset: an empty accumulator with the script's -c / -s."""
+        p = np.zeros(1, METHFREQ_PARAMS_DT)
+        p[0]["call_threshold"], p[0]["split_groups"] = call_threshold, 1 if split_groups else 0
+        self._check(self.lib.nph_methfreq_reset(self.ctx, _p(p)), "nph_methfreq_reset")
+
+    def methylation_frequency_add(self, contig_id: int):
+        """nph_methfreq_add: fold the rows of the last methylation run under contig_id."""
+        self._check(self.lib.nph_methfreq_add(self.ctx, contig_id), "nph_methfreq_add")
+
+    def methylation_frequency_counts(self):
+        """(distinct keys, calls counted, rows skipped by the threshold)"""
+        a, b, c = C.c_uint64(), C.c_uint64(), C.c_uint64()
+        self._check(self.lib.nph_methfreq_counts(self.ctx, C.byref(a), C.byref(b), C.byref(c)), "nph_methfreq_counts")
+        return int(a.value), int(b.value), int(c.value)
+
+    def methylation_frequency_tsv(self, contigs: list, cap: int | None = None) -> bytes:
+        """nph_methfreq_tsv: the frequency table so far; contigs[i] is the name of contig id i."""
+        blob = np.frombuffer("".join(contigs).encode() or b"\0", np.uint8)
+        off = np.zeros(len(contigs) + 1, np.uint32)
+        off[1:] = np.cumsum([len(c.encode()) for c in contigs])
+        n = C.c_uint64()
+        if cap is None:              # a guess, then the size the call reports when the guess was short
+            cap = 4096 + (256 + max((len(c.encode()) for c in contigs), default=0)) * self.methylation_frequency_counts()[0]
+            out = np.empty(cap, np.uint8)
+            if self.lib.nph_methfreq_tsv(self.ctx, _p(blob), _p(off), len(contigs), _p(out), cap, C.byref(n)) == 0:
+                return out[:int(n.value)].tobytes()
+            cap = max(cap, int(n.value))
+        out = np.empty(max(cap, 1), np.uint8)
+        self._check(self.lib.nph_methfreq_tsv(self.ctx, _p(blob), _p(off), len(contigs), _p(out), cap, C.byref(n)), "nph_methfreq_tsv")
+        return out[:int(n.value)].tobytes()
 
     # ---- variants: candidate screening on the device (include/nph.h, section N2) ----
     def screen_edits_batch(self, reads, ev_mean, ev_start_time, ref_bases, deltas, first_event, records, params, indel_bias: float = 1.0,

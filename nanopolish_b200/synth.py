@@ -67,6 +67,7 @@ METH_PARAMS_DT = np.dtype([("min_separation", "<i4"), ("min_flank", "<i4"), ("ma
                            ("region_start", "<i4"), ("region_end", "<i4"), ("k", "<u4"), ("alphabet_size", "<u4"),
                            ("bases", "S8"), ("complements", "S8"), ("n_sites", "<u4"), ("site_len", "<u4"),
                            ("sites", "S8", 4), ("sites_methylated", "S8", 4), ("sites_methylated_complement", "S8", 4)], align=True)
+METHFREQ_PARAMS_DT = np.dtype([("call_threshold", "<f8"), ("split_groups", "<u4"), ("reserved", "<u4")], align=True)
 assert METH_RECORD_DT.itemsize == 40 and METH_SITE_DT.itemsize == 24 and METH_PARAMS_DT.itemsize == 152
 assert ALIGN_STATE_DT.itemsize == 16
 assert READ_DT.itemsize == 64 and HMM_JOB_DT.itemsize == 32 and ABEA_JOB_DT.itemsize == 32
