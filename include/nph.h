@@ -233,11 +233,15 @@ int nph_mom_batch(nph_ctx* ctx, const nph_read* reads, size_t n_reads,
 /* ---- profile_hmm_align (Viterbi; section 8f N1) ------------------------------------------
  * states_out receives, for job j, n_states_out[j] HMMAlignmentStates at states_out + states_off[j] in ascending
  * event order; states_off has n_jobs + 1 entries and states_off[j+1] - states_off[j] is the room for job j
- * (n_events + n_kmers always suffices).  n_states_out[j] == 0 where the reference would trip an assert (fewer
- * than two events, or the best path runs into a -inf cell).  scores_out (optional) = l_fm of the last state.
- * Limit: the movement trace of the batch's largest window, 2 * (E + K/C + 1) * 32*C bytes per warp (C = 1..8 columns per
- * lane), is kept for every resident warp; the number of resident warps shrinks so that the arena stays within 16 GiB, and a
- * window that needs more than that for a single CTA of 16 warps (E*K beyond ~1.6e7) returns NPH_ERR_UNSUPPORTED.
+ * (n_events + n_kmers always suffices).  n_states_out[j] == 0 and scores_out[j] == -inf where the reference would
+ * trip an assert (fewer than two events, or the best path runs into a -inf cell) and where the room is shorter than the
+ * path.  Offsets must not decrease (NPH_ERR_INVALID); states_out before states_off[0] is left untouched.
+ * scores_out (optional) = l_fm of the last state.
+ * Limit: the movement trace of the batch's largest window, 2 * (steps + 1) * 32*C bytes per warp (C = 1..8 columns per
+ * lane, steps ~ E * ceil(K / 32C) + K/C), is kept for every resident warp; the number of resident CTAs shrinks so that the
+ * traces stay within 16 GiB, and a batch whose largest window needs more than that for a single CTA of 16 warps returns
+ * NPH_ERR_UNSUPPORTED: about E*K > 5.4e8, from K = E = 23 046 on for a square window.  On a 132-SM H100 the cap starts
+ * at about K = E = 1 983.
  * ref: profile_hmm_align_r9, src/hmm/nanopolish_profile_hmm_r9.cpp:73-204. */
 int nph_hmm_align_batch(nph_ctx* ctx,
                         const nph_read* reads, size_t n_reads,

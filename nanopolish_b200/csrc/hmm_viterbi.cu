@@ -225,7 +225,9 @@ extern "C" int nph_hmm_align(nph_ctx* ctx,
     }
     NPH_CUDA(ctx, cudaEventRecord(ctx->ev1, ctx->stream));
     nph_timing_events(ctx, launches);
-    NPH_CUDA(ctx, cudaMemcpyAsync(states_out, p.states, sizeof(nph_align_state) * total_states, cudaMemcpyDeviceToHost, ctx->stream));
+    // only the jobs' slices go back: states_out[0 .. states_off[0]) belongs to the caller
+    NPH_CUDA(ctx, cudaMemcpyAsync(states_out + states_off[0], p.states + states_off[0], sizeof(nph_align_state) * (total_states - states_off[0]),
+                                  cudaMemcpyDeviceToHost, ctx->stream));
     NPH_CUDA(ctx, cudaMemcpyAsync(n_states_out, p.n_states, sizeof(uint32_t) * n_jobs, cudaMemcpyDeviceToHost, ctx->stream));
     if (scores_out) NPH_CUDA(ctx, cudaMemcpyAsync(scores_out, ctx->d_scores.p, sizeof(float) * n_jobs, cudaMemcpyDeviceToHost, ctx->stream));
     NPH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));

@@ -226,7 +226,8 @@ double npref_score_batch(size_t n_jobs, const int32_t* read_h, const int32_t* mo
 }
 
 // profile_hmm_align on one job; out = (event_idx, kmer_idx) u32 pairs, l_fm floats, state chars.
-// Guards the conditions the reference asserts on so the harness does not abort the test process.
+// Guards nothing: the reference is built with its asserts on, so a job with fewer than two events or a path that enters a
+// -inf cell aborts the calling process (tests/test_viterbi_edges_oracle.py runs such jobs in a forked child).
 int npref_align(int read_h, int model_h, const char* seq, uint32_t e_start, uint32_t e_stop, int rc, uint32_t flags,
                 double indel_bias, uint32_t* ev_kmer_out, float* lfm_out, char* state_out, uint32_t cap)
 {
