@@ -1,10 +1,8 @@
 // meth_dev.cuh — a methylation alphabet and its recognition sites as the device kernels use them (ranks, not characters).
 // Built and validated once by nph_meth_alphabet (methylation.cu); read by call-methylation (methylation.cu) and by the
-// methylation-aware variant screening (variants.cu).  Also the numbers of one methylation_calls.tsv row, shared by the device
-// writer of those rows (methylation.cu) and the per-site frequency accumulator that reads them (meth_frequency.cu).
+// methylation-aware variant screening (variants.cu).
 #pragma once
 #include "nph_internal.cuh"
-#include "tsv_format.cuh"
 
 struct MethDev {
     int32_t min_separation, min_flank, max_span, min_event_span, region_start, region_end;   // call-methylation's window (variants.cu: unused)
@@ -32,26 +30,5 @@ __device__ __forceinline__ int site_at(const MethDev& d, const uint8_t* __restri
         if (eq) return (int)q;
     }
     return -1;
-}
-
-// The printed numbers and the sequence column of the methylation_calls.tsv row of site record ms (a 1D read: the other
-// strand's entries are 0): the three "%.2lf" likelihoods, and the sequence as [seq_b, seq_b + seq_len) of the record's reference.
-struct RowNums { nph_tsv::Fixed2 diff, m, u; uint32_t seq_b, seq_len; bool seq_ok; };
-
-__device__ __forceinline__ RowNums row_numbers(const nph_meth_site& ms, const nph_meth_record& R, uint32_t k)
-{
-    RowNums r;
-    // ScoredSite: ll_*[strand] = the float score, the other strand 0.0; the writer sums the two strands in double
-    const double sum_m = __dadd_rn((double)ms.ll_methylated, 0.0), sum_u = __dadd_rn((double)ms.ll_unmethylated, 0.0);
-    r.diff = nph_tsv::fixed2_of(__dsub_rn(sum_m, sum_u));
-    r.m = nph_tsv::fixed2_of(sum_m);
-    r.u = nph_tsv::fixed2_of(sum_u);
-    // the sequence column starts k - 1 bases before the first site: a window parameter set that lets a group start closer to the
-    // beginning of the record's reference than that makes the reference's substr throw; here the call is refused
-    const int bs = (ms.start_position - R.ref_start_pos) - (int)k + 1;
-    const uint32_t e = min((uint32_t)(ms.end_position - R.ref_start_pos) + k, R.ref_len);
-    r.seq_ok = bs >= 0 && (uint32_t)bs <= e;
-    r.seq_b = r.seq_ok ? (uint32_t)bs : 0u; r.seq_len = r.seq_ok ? e - (uint32_t)bs : 0u;
-    return r;
 }
 #endif

@@ -8,7 +8,7 @@
 //   and a key keeps the group size and sequence of the first row that created it, in input order.
 // The table is the script's output: a header, then one row per key in the order Python sorts (str, int, int) tuples.
 //
-// Exactness: the "%.2lf" text of a row is the integer D = fixed2_of(llr_m - llr_u) (tsv_format.cuh, the same arithmetic the
+// Exactness: the "%.2lf" text of a row is the integer D = fixed_of<2>(llr_m - llr_u) (tsv_format.cuh, the same arithmetic the
 // row writer prints), so Python's float() of it is the correctly rounded D / 100, which (double)D / 100.0 is as long as D is
 // a double (D < 2^53; larger values are refused).  is_methylated (llr > 0) is D > 0 with a '+' sign: "-0.00" is not.  Counts
 // are 64-bit integer atomics and the first row of a key is an atomicMin over (batch, row) ordinals, so the table does not
@@ -21,6 +21,7 @@
 // span), cub radix sort, row lengths -> scan -> rows (one read-back between), one D2H copy.
 #include "nph_internal.cuh"
 #include "meth_dev.cuh"
+#include "tsv_format.cuh"
 #include <cub/device/device_radix_sort.cuh>
 #include <algorithm>
 #include <cstring>
@@ -137,7 +138,7 @@ __device__ __forceinline__ FreqRow freq_row(const FoldArgs& a, uint64_t i)
 {
     const nph_meth_site ms = a.sites[i];
     const nph_meth_record R = a.records[ms.record];
-    const RowNums r = row_numbers(ms, R, a.k);
+    const nph_tsv::RowNums r = nph_tsv::row_numbers(ms, R, a.k);
     FreqRow f;
     f.refused = 0;
     if (!(r.diff.ok && r.m.ok && r.u.ok) || r.diff.q >= (1ull << 53)) f.refused |= kRefuseNumber;
@@ -327,7 +328,7 @@ extern "C" int nph_methfreq_add(nph_ctx* ctx, uint32_t contig_id)
     NPH_CUDA(ctx, cudaMemcpyAsync(&h, d_sum, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
     NPH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));            // the fold's one read-back
     if (h.refused & kRefuseSeq) {
-        ctx->last_error = "a group starts fewer than k - 1 bases into its record's reference: the sequence column of its row is undefined (min_flank too small for k)";
+        ctx->last_error = nph_tsv::kSeqRefused;
         return NPH_ERR_INVALID;
     }
     if (h.refused) {

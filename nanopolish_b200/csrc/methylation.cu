@@ -25,6 +25,7 @@
 // into its site record.  The host sees O(records) work only.
 #include "nph_internal.cuh"
 #include "meth_dev.cuh"
+#include "tsv_format.cuh"
 #include <algorithm>
 #include <cstring>
 #include <string>
@@ -578,13 +579,6 @@ struct TsvArgs {
     int* refused;                      // set when a value needs the C library (non-finite, |v| >= 2^52)
 };
 
-__device__ __forceinline__ uint32_t row_len(const TsvArgs& a, const nph_meth_site& ms, const RowNums& r, uint32_t name_len)
-{
-    return a.contig_len + 3u + (uint32_t)nph_tsv::int_len(ms.start_position) + 1u + (uint32_t)nph_tsv::int_len(ms.end_position) + 1u + name_len + 1u +
-           (uint32_t)nph_tsv::fixed2_len(r.diff) + 1u + (uint32_t)nph_tsv::fixed2_len(r.m) + 1u + (uint32_t)nph_tsv::fixed2_len(r.u) + 1u + 2u +
-           (uint32_t)nph_tsv::ndigits(ms.n_motif) + 1u + r.seq_len + 1u;
-}
-
 // pass 1 (WRITE = false): bytes per record; pass 2 (WRITE = true): the rows at rec_off[record]
 template <bool WRITE>
 __global__ void __launch_bounds__(kThreads) meth_tsv_kernel(const TsvArgs a)
@@ -601,35 +595,20 @@ __global__ void __launch_bounds__(kThreads) meth_tsv_kernel(const TsvArgs a)
         for (uint64_t base = s0; base < s1; base += 32) {
             const uint64_t s = base + lane;
             const bool have = s < s1;
-            nph_meth_site ms{};
-            RowNums r{};
+            nph_tsv::MethRow row{};
             uint32_t len = 0;
             if (have) {
-                ms = a.sites[s];
-                r = row_numbers(ms, R, a.k);
+                const nph_meth_site ms = a.sites[s];
+                const nph_tsv::RowNums r = nph_tsv::row_numbers(ms, R, a.k);
                 if (!(r.diff.ok && r.m.ok && r.u.ok)) atomicMax(a.refused, 1);
                 if (!r.seq_ok) atomicMax(a.refused, 2);
-                len = row_len(a, ms, r, name_len);
+                row = {a.contig, a.contig_len, a.is_reverse[rec] ? '-' : '+', ms.start_position, ms.end_position, a.names + nb, name_len,
+                       r.diff, r.m, r.u, 1, (int)ms.n_motif, reinterpret_cast<const char*>(a.ref + R.ref_off + r.seq_b), r.seq_len};
+                len = nph_tsv::meth_row_len(row);
             }
             uint32_t incl = len;
             for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(kFull, incl, o); if (lane >= o) incl += v; }
-            if (WRITE && have) {
-                char* o = a.out + run + (incl - len);
-                for (uint32_t i = 0; i < a.contig_len; ++i) *o++ = a.contig[i];
-                *o++ = '\t'; *o++ = a.is_reverse[rec] ? '-' : '+'; *o++ = '\t';
-                o = nph_tsv::put_int(o, ms.start_position); *o++ = '\t';
-                o = nph_tsv::put_int(o, ms.end_position); *o++ = '\t';
-                for (uint32_t i = 0; i < name_len; ++i) *o++ = a.names[nb + i];
-                *o++ = '\t';
-                o = nph_tsv::put_fixed2(o, r.diff); *o++ = '\t';
-                o = nph_tsv::put_fixed2(o, r.m); *o++ = '\t';
-                o = nph_tsv::put_fixed2(o, r.u); *o++ = '\t';
-                *o++ = '1'; *o++ = '\t';
-                o = nph_tsv::put_u64(o, ms.n_motif); *o++ = '\t';
-                const uint8_t* sq = a.ref + R.ref_off + r.seq_b;
-                for (uint32_t i = 0; i < r.seq_len; ++i) *o++ = (char)sq[i];
-                *o++ = '\n';
-            }
+            if (WRITE && have) nph_tsv::put_meth_row(a.out + run + (incl - len), row);
             run += __shfl_sync(kFull, incl, 31);
         }
         if (!WRITE && lane == 0) a.rec_bytes[rec] = run;
@@ -683,7 +662,7 @@ extern "C" int nph_methylation_tsv(nph_ctx* ctx, const char* contig, const char*
     NPH_CUDA(ctx, cudaMemcpyAsync(&refused, d_refused, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
     NPH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     if (refused == 2) {
-        ctx->last_error = "a group starts fewer than k - 1 bases into its record's reference: the sequence column of its row is undefined (min_flank too small for k)";
+        ctx->last_error = nph_tsv::kSeqRefused;
         return NPH_ERR_INVALID;
     }
     if (refused) {

@@ -1,5 +1,6 @@
 // nph_eventalign.cpp — see nph_eventalign.hpp (SURVEY.md section 8f, row N1).
 #include "nph_eventalign.hpp"
+#include "../csrc/tsv_format.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -570,16 +571,7 @@ size_t EventAligner::run(Engine& engine, double indel_bias)
 // ---------------------------------------------------------------------------------------------
 // writers
 // ---------------------------------------------------------------------------------------------
-static inline char* put_int(char* o, long long v)
-{
-    char tmp[24];
-    int n = 0;
-    unsigned long long u = v < 0 ? 0ull - (unsigned long long)v : (unsigned long long)v;
-    do { tmp[n++] = (char)('0' + u % 10); u /= 10; } while (u);
-    if (v < 0) *o++ = '-';
-    while (n) *o++ = tmp[--n];
-    return o;
-}
+using nph_tsv::put_i64;
 static inline char* put_str(char* o, const char* s, size_t n) { std::memcpy(o, s, n); return o + n; }
 
 std::string EventAligner::tsv_header(const EventalignOptions& opt)
@@ -624,7 +616,7 @@ std::string EventAligner::tsv(size_t read_idx, const EventalignOptions& opt) con
         kmers_at(rs, r, ref_kmer, model_kmer);
         // contig, position, reference_kmer, read, strand
         o = put_str(o, ref_name.data(), ref_name.size()); *o++ = '\t';
-        o = put_int(o, r.ref_position); *o++ = '\t';
+        o = put_i64(o, r.ref_position); *o++ = '\t';
         o = put_str(o, ref_kmer, std::strlen(ref_kmer)); *o++ = '\t';
         o = put_str(o, who_s.data(), who_s.size()); *o++ = '\t';
         *o++ = "tc"[strand]; *o++ = '\t';
@@ -650,7 +642,7 @@ std::string EventAligner::tsv(size_t read_idx, const EventalignOptions& opt) con
         // float difference over a double product, narrowed to float (a 'B' state divides by zero: inf, like the reference)
         const float standard_level = (float)((event_mean - model_mean) / (sqrt_var * model_stdv));
         // event_index %d, event_level_mean %.2lf, event_stdv %.3lf, event_length %.5lf
-        o = put_int(o, r.event_idx); *o++ = '\t';
+        o = put_i64(o, r.event_idx); *o++ = '\t';
         o += format_fixed(o, event_mean, 2); *o++ = '\t';
         o += format_fixed(o, event_stdv, 3); *o++ = '\t';
         o += format_fixed(o, event_duration, 5); *o++ = '\t';
@@ -661,7 +653,7 @@ std::string EventAligner::tsv(size_t read_idx, const EventalignOptions& opt) con
         o += format_fixed(o, standard_level, 2);
         if (opt.write_signal_index) {
             const std::pair<size_t, size_t> si = sr.get_event_sample_idx(strand, r.event_idx);
-            *o++ = '\t'; o = put_int(o, (long long)si.first); *o++ = '\t'; o = put_int(o, (long long)si.second);
+            *o++ = '\t'; o = put_i64(o, (int64_t)si.first); *o++ = '\t'; o = put_i64(o, (int64_t)si.second);
         }
         if (opt.write_samples) {
             // the reference streams the floats through an ostream (%g, 6 significant digits) with ',' after each and

@@ -1,5 +1,6 @@
 // nph_host.cpp — implementation of the C++ host mirror (see nph_host.hpp).
 #include "nph_host.hpp"
+#include "../csrc/tsv_format.cuh"
 #ifdef _OPENMP
 #include <omp.h>
 #endif
@@ -283,98 +284,41 @@ uint32_t Engine::model_id(const PoreModel* model)
 // ---------------------------------------------------------------------------------------------
 // Batches
 // ---------------------------------------------------------------------------------------------
-// printf("%.<prec>lf", (double)v) for a float v, prec <= 5, without going through the C library's arbitrary-precision
-// path: v = m * 2^e exactly with m < 2^24, so v * 10^prec = (m * 10^prec) * 2^e fits 64-bit integer arithmetic with an
-// exact remainder, and round-half-to-even on it is the decimal string glibc prints (it rounds the exact value, in the
-// default rounding mode).  Magnitudes of 2^39 and above and non-finite values take snprintf.  Returns the length.
-size_t format_fixed(char* dst, float v, int prec)
+// format_fixed: csrc/tsv_format.cuh's exact formatter where it takes the value and the precision, snprintf elsewhere
+namespace {
+template <int N, typename T>
+size_t fixed_or_printf(char* dst, T v)
 {
-    static const uint64_t pow10[6] = {1, 10, 100, 1000, 10000, 100000};
-    uint32_t bits;
-    std::memcpy(&bits, &v, 4);
-    const uint32_t expo = (bits >> 23) & 0xff;
-    if (expo == 0xff || expo >= 127 + 39 || prec < 0 || prec > 5) return (size_t)snprintf(dst, 64, "%.*lf", prec, (double)v);
-    uint64_t m = bits & 0x7fffff;
-    int e;                                   // v = m * 2^e
-    if (expo == 0) e = -149; else { m |= 0x800000; e = (int)expo - 150; }
-    uint64_t q;
-    const uint64_t N = m * pow10[prec];      // < 2^24 * 10^5 < 2^41
-    if (e >= 0) {
-        q = N << e;                          // e <= 15 here: < 2^56
-    } else {
-        const int sft = -e;
-        if (sft > 62) q = 0;                 // N < 2^41 is far below half an ulp of the last printed digit
-        else {
-            q = N >> sft;
-            const uint64_t rem = N & (((uint64_t)1 << sft) - 1), half = (uint64_t)1 << (sft - 1);
-            if (rem > half || (rem == half && (q & 1))) q += 1;
-        }
-    }
-    char tmp[32];
-    int n = 0;
-    uint64_t ip = q / pow10[prec], fp = q % pow10[prec];
-    do { tmp[n++] = (char)('0' + ip % 10); ip /= 10; } while (ip);
-    char* o = dst;
-    if (bits >> 31) *o++ = '-';
-    while (n) *o++ = tmp[--n];
-    if (prec) {
-        *o++ = '.';
-        for (int i = prec - 1; i >= 0; --i) { o[i] = (char)('0' + fp % 10); fp /= 10; }
-        o += prec;
-    }
+    const nph_tsv::Fixed f = nph_tsv::fixed_of<N>(v);
+    if (!f.ok) return (size_t)snprintf(dst, 400, "%.*lf", N, (double)v);
+    char* const o = nph_tsv::put_fixed<N>(dst, f);
     *o = 0;
     return (size_t)(o - dst);
 }
+} // namespace
 
-// the same for a double: m < 2^53 and 10^prec <= 10^3 keep m * 10^prec below 2^63
+size_t format_fixed(char* dst, float v, int prec)
+{
+    switch (prec) {
+    case 0: return fixed_or_printf<0>(dst, v);
+    case 1: return fixed_or_printf<1>(dst, v);
+    case 2: return fixed_or_printf<2>(dst, v);
+    case 3: return fixed_or_printf<3>(dst, v);
+    case 4: return fixed_or_printf<4>(dst, v);
+    case 5: return fixed_or_printf<5>(dst, v);
+    }
+    return (size_t)snprintf(dst, 64, "%.*lf", prec, (double)v);
+}
+
 size_t format_fixed(char* dst, double v, int prec)
 {
-    static const uint64_t pow10[4] = {1, 10, 100, 1000};
-    uint64_t bits;
-    std::memcpy(&bits, &v, 8);
-    const uint32_t expo = (uint32_t)((bits >> 52) & 0x7ff);
-    if (expo == 0x7ff || expo >= 1075 || prec < 0 || prec > 3) return (size_t)snprintf(dst, 400, "%.*lf", prec, v);
-    uint64_t m = bits & 0xfffffffffffffull;
-    int sft;                                 // v = m * 2^-sft, sft >= 1
-    if (expo == 0) sft = 1074; else { m |= (uint64_t)1 << 52; sft = 1075 - (int)expo; }
-    const uint64_t N = m * pow10[prec];      // < 2^53 * 1000 < 2^63
-    uint64_t q = 0;
-    if (sft <= 63) {
-        q = N >> sft;
-        const uint64_t rem = N & (((uint64_t)1 << sft) - 1), half = (uint64_t)1 << (sft - 1);
-        if (rem > half || (rem == half && (q & 1))) q += 1;
-    }                                        // sft >= 64: N < 2^63 is below half a unit of the last printed digit
-    char* o = dst;
-    if (bits >> 63) *o++ = '-';
-    if (prec == 2 && q < 4000000000ull) {
-        // the call-methylation / eventalign fast path: constant divisors (multiply-shift), 32-bit arithmetic, two digits at a time
-        static const char kPairs[201] =
-            "0001020304050607080910111213141516171819202122232425262728293031323334353637383940414243444546474849"
-            "5051525354555657585960616263646566676869707172737475767778798081828384858687888990919293949596979899";
-        const uint32_t q32 = (uint32_t)q;
-        uint32_t ip32 = q32 / 100u;
-        const uint32_t fp32 = q32 % 100u;
-        char tmp2[12];
-        int m = 0;
-        while (ip32 >= 100u) { const uint32_t r = ip32 % 100u; ip32 /= 100u; tmp2[m++] = kPairs[2 * r + 1]; tmp2[m++] = kPairs[2 * r]; }
-        if (ip32 >= 10u) { tmp2[m++] = kPairs[2 * ip32 + 1]; tmp2[m++] = kPairs[2 * ip32]; } else tmp2[m++] = (char)('0' + ip32);
-        while (m) *o++ = tmp2[--m];
-        *o++ = '.'; *o++ = kPairs[2 * fp32]; *o++ = kPairs[2 * fp32 + 1];
-        *o = 0;
-        return (size_t)(o - dst);
+    switch (prec) {
+    case 0: return fixed_or_printf<0>(dst, v);
+    case 1: return fixed_or_printf<1>(dst, v);
+    case 2: return fixed_or_printf<2>(dst, v);
+    case 3: return fixed_or_printf<3>(dst, v);
     }
-    char tmp[32];
-    int n = 0;
-    uint64_t ip = q / pow10[prec], fp = q % pow10[prec];
-    do { tmp[n++] = (char)('0' + ip % 10); ip /= 10; } while (ip);
-    while (n) *o++ = tmp[--n];
-    if (prec) {
-        *o++ = '.';
-        for (int i = prec - 1; i >= 0; --i) { o[i] = (char)('0' + fp % 10); fp /= 10; }
-        o += prec;
-    }
-    *o = 0;
-    return (size_t)(o - dst);
+    return (size_t)snprintf(dst, 400, "%.*lf", prec, v);
 }
 
 int host_threads()

@@ -351,8 +351,9 @@ private:
 };
 
 // == snprintf(dst, ..., "%.<prec>lf", v), byte for byte, by exact integer arithmetic on the binary value (round half to
-// even on the exact quotient — what glibc prints in the default rounding mode).  float: prec <= 5; double: prec <= 3.
-// Magnitudes of 2^39 (float) / 2^52 (double) and above and non-finite values take snprintf.  Returns the length.
+// even on the exact quotient — what glibc prints in the default rounding mode; csrc/tsv_format.cuh).  float: prec <= 5;
+// double: prec <= 3.  Other precisions, magnitudes of 2^39 (float) / 2^52 (double) and above and non-finite values take
+// snprintf.  Returns the length.
 size_t format_fixed(char* dst, float v, int prec);
 size_t format_fixed(char* dst, double v, int prec);
 

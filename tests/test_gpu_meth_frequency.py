@@ -177,10 +177,10 @@ def test_refusals(eng, batches):
 
 
 def test_frequency_number_formatting_on_device():
-    """fixed_of<3> == printf("%.3f") of every m / n, n <= 5000, and fixed2_of unchanged, on the device"""
+    """fixed_of<3> == printf("%.3f") of every m / n, n <= 5000, and fixed_of<2> unchanged, on the device"""
     import os
     import subprocess
-    exe = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "build", "checks", "check_freq_format")
+    exe = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "build", "checks", "check_tsv_format")
     r = subprocess.run([exe], capture_output=True, text=True, timeout=600)
     assert r.returncode == 0, r.stdout + r.stderr
     assert "device: 0 bad" in r.stdout

@@ -318,7 +318,8 @@ def test_tsv_rows_formatted_on_the_device(eng2):
 
 def test_tsv_number_formatting_on_device():
     """csrc/tsv_format.cuh == printf("%.2lf") / printf("%d") on 6.6e6 doubles (scores, differences, exact halves at the second decimal,
-    every binade, random bit patterns, refusals beyond 2^52) — host and device copies of the same functions."""
+    every binade, random bit patterns, refusals beyond 2^52), floats at "%.0lf" .. "%.5lf", and put_meth_row == the reference's row
+    format — host and device copies of the same functions."""
     import os, subprocess
     exe = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "build", "checks", "check_tsv_format")
     r = subprocess.run([exe], capture_output=True, text=True, timeout=600)

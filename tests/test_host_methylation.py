@@ -119,3 +119,12 @@ def test_flat_call_formats_its_rows_on_the_device(host):
     assert got >= 0, host.nphh_last_error()
     assert int(ns.value) == sites.shape[0] and int(se.value) == scored
     assert buf[:got].tobytes().decode() == want
+    # the pair-list form of the same batch: its rows are formatted on the host, by the same row writer
+    pairs_c = np.ascontiguousarray(pairs)
+    buf[:] = 0
+    got = host.nphh_call_methylation_flat(vp(rs.reads), C.c_size_t(n), vp(rs.ev_mean), None, C.c_size_t(rs.ev_mean.shape[0]),
+                                          vp(ref), C.c_size_t(ref.shape[0]), vp(pairs_c), C.c_size_t(pairs_c.shape[0]), None, None,
+                                          vp(recs2), C.c_size_t(n), mh, names, vp(is_rev), b"chr1", C.c_double(1.0),
+                                          vp(buf), C.c_size_t(buf.shape[0]), C.byref(ns), C.byref(se), vp(secs))
+    assert got >= 0, host.nphh_last_error()
+    assert buf[:got].tobytes().decode() == want

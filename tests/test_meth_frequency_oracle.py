@@ -132,9 +132,9 @@ def test_crafted_inputs_cover_the_rules():
 
 
 def test_frequency_number_formatting_on_host():
-    """the host copy of tsv_format.cuh's fixed_of<3> against snprintf("%.3f") of every m / n, n <= 5000, and fixed2_of unchanged on
-    the same values (the device copy runs in the gpu tests)"""
-    exe = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "build", "checks", "check_freq_format")
+    """the host copy of tsv_format.cuh's fixed_of<3> against snprintf("%.3f") of every m / n, n <= 5000, and fixed_of<2> unchanged
+    on the same values (the device copy runs in the gpu tests)"""
+    exe = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "build", "checks", "check_tsv_format")
     r = subprocess.run([exe, "--host-only"], capture_output=True, text=True, timeout=600)
     assert r.returncode == 0, r.stdout + r.stderr
     assert ", 0 bad" in r.stdout
