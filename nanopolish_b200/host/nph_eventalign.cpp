@@ -14,37 +14,9 @@ namespace nph {
 // ---------------------------------------------------------------------------------------------
 size_t AlignBatch::add(const HMMInputSequence& sequence, const HMMInputData& data, uint32_t flags)
 {
-    if (!data.read || !data.pore_model) throw Error(NPH_ERR_INVALID, "HMMInputData without read or pore_model");
-    if (data.read->pore_type != PORETYPE_R9) throw Error(NPH_ERR_UNSUPPORTED, "only R9 reads are supported (load_from_raw always makes R9)");
-    const uint32_t k = data.pore_model->k;
-    if (data.pore_model->states.size() != sequence.get_num_kmer_ranks(k))
-        throw Error(NPH_ERR_INVALID, "sequence alphabet does not match the pore model's state space");
-    if (!((data.rc && data.event_stride == -1) || (!data.rc && data.event_stride == 1)))
-        throw Error(NPH_ERR_INVALID, "rc and event_stride disagree");                                       // ref asserts (profile_hmm_r9.inl:275)
-    if (sequence.length() < k) throw Error(NPH_ERR_INVALID, "sequence shorter than k");
-    ReadKey key{data.read, data.strand};
-    auto it = m_read_index.find(key);
-    uint32_t ridx;
-    if (it == m_read_index.end()) {
-        ridx = (uint32_t)m_reads.size();
-        m_read_index[key] = ridx;
-        m_reads.push_back(key);
-    } else {
-        ridx = it->second;
-    }
-    const uint32_t n_kmers = (uint32_t)(sequence.length() - k + 1);
-    nph_hmm_job j;
+    nph_hmm_job j = detail::make_hmm_job(sequence, data, flags, m_reads);
     j.rank_off = m_ranks.size();
-    j.read = ridx;
-    j.model_id = 0;   // resolved against the engine in run()
-    j.event_start = data.event_start_idx;
-    j.event_stop = data.event_stop_idx;
-    j.n_kmers = n_kmers;
-    j.stride = data.event_stride;
-    j.rc = data.rc;
-    j.flags = (uint8_t)flags;
-    j.reserved = 0;
-    sequence.append_kmer_ranks(k, data.rc != 0, m_ranks);
+    sequence.append_kmer_ranks(data.pore_model->k, data.rc != 0, m_ranks);
     m_jobs.push_back(j);
     m_job_models.push_back(data.pore_model);
     return m_jobs.size() - 1;
@@ -58,18 +30,16 @@ void AlignBatch::clear_jobs()
 void AlignBatch::clear()
 {
     clear_jobs();
-    m_read_index.clear(); m_reads.clear(); m_reads_uploaded = 0;
+    m_reads.clear(); m_reads_uploaded = 0;
 }
 
 std::vector<std::vector<HMMAlignmentState>> AlignBatch::run(Engine& engine, double indel_bias, bool reads_resident)
 {
     std::vector<std::vector<HMMAlignmentState>> out(m_jobs.size());
     if (m_jobs.empty()) return out;
-    for (size_t j = 0; j < m_jobs.size(); ++j) m_jobs[j].model_id = engine.model_id(m_job_models[j]);
+    detail::resolve_model_ids(engine, m_job_models, m_jobs);
     if (!reads_resident || m_reads_uploaded != m_reads.size()) {
-        std::vector<std::pair<const SquiggleRead*, uint8_t>> rl;
-        for (auto& r : m_reads) rl.push_back({r.read, r.strand});
-        const detail::FlatReads fr = detail::flatten_reads(engine, rl);
+        const detail::FlatReads fr = detail::flatten_reads(engine, m_reads);
         engine.check(nph_reads_load(engine.ctx(), fr.reads.data(), fr.reads.size(), fr.mean, fr.time, fr.n_events), "nph_reads_load");
         m_reads_uploaded = m_reads.size();
     }
@@ -392,49 +362,27 @@ std::vector<EventAlignment> EventAligner::alignment(size_t read_idx) const
     return out;
 }
 
-// ranks of every k-mer of seq by one rolling pass: rank(pos + 1) = (rank(pos) mod A^(k-1)) * A + rank(seq[pos + k])
-void rolling_kmer_ranks(const Alphabet* alphabet, const std::string& seq, uint32_t k, uint32_t* out)
-{
-    const size_t n = seq.size();
-    if (n < k) return;
-    uint64_t top = 1;
-    for (uint32_t i = 1; i < k; ++i) top *= alphabet->size();
-    uint64_t r = 0;
-    for (uint32_t i = 0; i < k; ++i) r = r * alphabet->size() + alphabet->rank(seq[i]);
-    out[0] = (uint32_t)r;
-    for (size_t pos = 1; pos + k <= n; ++pos) {
-        r = (r % top) * alphabet->size() + alphabet->rank(seq[pos + k - 1]);
-        out[pos] = (uint32_t)r;
-    }
-}
-
 size_t EventAligner::run(Engine& engine, double indel_bias)
 {
     const size_t nr = m_reads.size();
     // ---- phase 1 (parallel over reads): trims and start/stop events of every BAM segment, up to the first segment
     //      that trims to nothing (where the reference returns from align_read_to_ref) ----
     std::vector<std::vector<SegmentStart>> starts(nr);
-    std::vector<std::string> errors(nr);
-#pragma omp parallel for schedule(dynamic, 8) num_threads(host_threads())
-    for (long long i = 0; i < (long long)nr; ++i) {
+    parallel_for(nr, host_threads(), 8, [&](size_t i) {
         ReadState& rs = m_reads[i];
-        if (rs.done) continue;
-        try {
-            if (rs.k >= 64) throw Error(NPH_ERR_UNSUPPORTED, "k-mer length");
-            for (size_t sidx = 0; sidx < rs.segments.size(); ++sidx) {
-                SegmentStart st;
-                if (!setup_segment(rs, sidx, st)) break;
-                starts[i].push_back(st);
-            }
-        } catch (const std::exception& e) { errors[i] = e.what(); }
-    }
-    for (size_t i = 0; i < nr; ++i) if (!errors[i].empty()) throw Error(NPH_ERR_INVALID, errors[i]);
+        if (rs.done) return;
+        if (rs.k >= 64) throw Error(NPH_ERR_UNSUPPORTED, "k-mer length");
+        for (size_t sidx = 0; sidx < rs.segments.size(); ++sidx) {
+            SegmentStart st;
+            if (!setup_segment(rs, sidx, st)) break;
+            starts[i].push_back(st);
+        }
+    });
 
     // ---- phase 2 (serial, O(reads)): read table, offsets ----
-    struct Slot { uint32_t read_index; uint64_t map_off; };
-    std::vector<std::pair<const SquiggleRead*, uint8_t>> read_table;
-    std::map<std::pair<const SquiggleRead*, uint8_t>, Slot> read_slot;
-    std::vector<Slot> slot_of(nr);
+    detail::ReadTable read_table;
+    std::vector<uint64_t> map_off;                          // per read_table entry: where its base-to-event map starts
+    std::vector<uint32_t> read_of(nr, 0);                   // per read: its read_table entry
     std::vector<char> fills_map(nr, 0);
     std::vector<uint64_t> rank_off(nr, 0), chain_first(nr + 1, 0);
     std::vector<uint32_t> model_of(nr, 0);
@@ -444,15 +392,12 @@ size_t EventAligner::run(Engine& engine, double indel_bias)
         if (starts[i].empty()) continue;
         const ReadState& rs = m_reads[i];
         const EventAlignmentParameters& p = rs.params;
-        const auto key = std::make_pair((const SquiggleRead*)p.sr, (uint8_t)p.strand_idx);
-        auto it = read_slot.find(key);
-        if (it == read_slot.end()) {
-            it = read_slot.insert({key, Slot{(uint32_t)read_table.size(), n_map}}).first;
-            read_table.push_back(key);
+        read_of[i] = read_table.index(p.sr, (uint8_t)p.strand_idx);
+        if (read_of[i] == map_off.size()) {
+            map_off.push_back(n_map);
             n_map += p.sr->base_to_event_map.size();
             fills_map[i] = 1;
         }
-        slot_of[i] = it->second;
         rank_off[i] = n_ranks;
         n_ranks += rs.ref_seq.size() >= rs.k ? rs.ref_seq.size() - rs.k + 1 : 0;
         model_of[i] = engine.model_id(rs.pore_model);
@@ -488,31 +433,26 @@ size_t EventAligner::run(Engine& engine, double indel_bias)
         const ReadState& rs = m_reads[i];
         const EventAlignmentParameters& p = rs.params;
         if (fills_map[i]) {
-            int32_t* m = map_start.data() + slot_of[i].map_off;
+            int32_t* m = map_start.data() + map_off[read_of[i]];
             const std::vector<EventRangeForBase>& b2e = p.sr->base_to_event_map;
             for (size_t j = 0; j < b2e.size(); ++j) m[j] = b2e[j].indices[p.strand_idx].start;
         }
         const size_t n = rs.ref_seq.size();
-        if (n >= rs.k) {
-            const size_t nk = n - rs.k + 1;
-            rolling_kmer_ranks(rs.pore_model->pmalphabet, rs.ref_seq, rs.k, ranks_fwd.data() + rank_off[i]);
-            // entry pos of the rc table = rank of rc_ref_seq's k-mer at n - pos - k (what get_kmer_rank(ki, k, true) resolves to)
-            std::vector<uint32_t> tmp(nk);
-            rolling_kmer_ranks(rs.pore_model->pmalphabet, rs.rc_ref_seq, rs.k, tmp.data());
-            uint32_t* rc = ranks_rc.data() + rank_off[i];
-            for (size_t pos = 0; pos < nk; ++pos) rc[pos] = tmp[nk - 1 - pos];
-        }
+        const Alphabet& alphabet = *rs.pore_model->pmalphabet;
+        kmer_ranks(alphabet, rs.ref_seq.data(), n, rs.k, false, ranks_fwd.data() + rank_off[i]);
+        // entry pos of the rc table = rank of rc_ref_seq's k-mer at n - pos - k (what get_kmer_rank(ki, k, true) resolves to)
+        kmer_ranks(alphabet, rs.rc_ref_seq.data(), rs.rc_ref_seq.size(), rs.k, true, ranks_rc.data() + rank_off[i]);
         for (size_t sidx = 0; sidx < starts[i].size(); ++sidx) {
             const SegmentStart& st = starts[i][sidx];
             nph_ea_chain& c = chains[chain_first[i] + sidx];
             nph_aligned_pair* dst = pairs.data() + c.pair_off;
             const AlignedSegment& seg = rs.segments[sidx];
             for (size_t j = 0; j < seg.size(); ++j) dst[j] = nph_aligned_pair{seg[j].ref_pos, seg[j].read_pos};
-            c.map_off = slot_of[i].map_off;
+            c.map_off = map_off[read_of[i]];
             c.map_len = (uint32_t)p.sr->base_to_event_map.size();
             c.rank_off = rank_off[i];
             c.ref_len = (uint32_t)n;
-            c.read = slot_of[i].read_index;
+            c.read = read_of[i];
             c.model_id = model_of[i];
             c.read_seq_len = (uint32_t)p.sr->read_sequence.size();
             c.ref_offset = p.ref_pos;
@@ -527,7 +467,8 @@ size_t EventAligner::run(Engine& engine, double indel_bias)
     // ---- the device: reads up, one launch, records back ----
     const detail::FlatReads fr = detail::flatten_reads(engine, read_table);
     engine.check(nph_reads_load(engine.ctx(), fr.reads.data(), fr.reads.size(), fr.mean, fr.time, fr.n_events), "nph_reads_load");
-    nph_ea_record* const records = static_cast<nph_ea_record*>(engine.pinned(0, sizeof(nph_ea_record) * std::max<uint64_t>(records_total, 1)));
+    nph_ea_record* const records = static_cast<nph_ea_record*>(
+        engine.pinned(Engine::Staging::EventalignRecords, sizeof(nph_ea_record) * std::max<uint64_t>(records_total, 1)));
     std::vector<nph_ea_result> results(n_chains);
     engine.check(nph_eventalign_chain(engine.ctx(), pairs.data(), pairs.size(), map_start.data(), map_start.size(), ranks_fwd.data(),
                                       ranks_rc.data(), ranks_fwd.size(), chains.data(), n_chains, indel_bias, records, records_total,
@@ -675,8 +616,7 @@ std::vector<std::string> EventAligner::tsv_batch(const EventalignOptions& opt) c
 {
     std::vector<std::string> out(m_reads.size());
     // rows of different reads are independent; the reference formats them one read at a time inside an omp critical
-#pragma omp parallel for schedule(dynamic, 4) num_threads(host_threads())
-    for (long long i = 0; i < (long long)m_reads.size(); ++i) out[i] = tsv((size_t)i, opt);
+    parallel_for(m_reads.size(), host_threads(), 4, [&](size_t i) { out[i] = tsv(i, opt); });
     return out;
 }
 

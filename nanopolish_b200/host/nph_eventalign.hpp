@@ -50,12 +50,10 @@ public:
     // the flat job list, for callers that drive the rounds themselves
     const std::vector<nph_hmm_job>& jobs() const { return m_jobs; }
     const std::vector<uint32_t>& ranks() const { return m_ranks; }
-    const SquiggleRead* job_read(size_t j) const { return m_reads[m_jobs[j].read].read; }
+    const SquiggleRead* job_read(size_t j) const { return m_reads.reads()[m_jobs[j].read].first; }
 
 private:
-    struct ReadKey { const SquiggleRead* read; uint8_t strand; bool operator<(const ReadKey& o) const { return read != o.read ? read < o.read : strand < o.strand; } };
-    std::map<ReadKey, uint32_t> m_read_index;
-    std::vector<ReadKey> m_reads;
+    detail::ReadTable m_reads;
     std::vector<const PoreModel*> m_job_models;
     std::vector<nph_hmm_job> m_jobs;
     std::vector<uint32_t> m_ranks;
@@ -194,9 +192,8 @@ private:
 };
 
 std::vector<uint32_t> event_alignment_to_cigar(const std::vector<EventAlignment>& alignments);
-// out[pos] = alphabet->kmer_rank(seq + pos, k) for every k-mer of seq, in one rolling pass
-void rolling_kmer_ranks(const Alphabet* alphabet, const std::string& seq, uint32_t k, uint32_t* out);
-// (format_fixed, the exact %.Nlf replacement the writers use, lives in nph_host.hpp)
+// (format_fixed, the exact %.Nlf replacement the writers use, and kmer_ranks, the rolling pass that builds the chains' rank
+// tables, live in nph_host.hpp)
 std::string cigar_ops_to_string(const std::vector<uint32_t>& ops);
 
 } // namespace nph

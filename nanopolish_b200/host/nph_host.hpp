@@ -89,6 +89,10 @@ extern const Alphabet gDNAAlphabet, gMCpGAlphabet, gMethylGpCAlphabet, gMethylDa
 const Alphabet* get_alphabet_by_name(const std::string& name);   // throws nph::Error for an unknown name
 const Alphabet* best_alphabet(const char* bases);
 
+// out[i] = alphabet.kmer_rank(s + i, k) for the n = len - k + 1 k-mers of s (nothing when len < k), in one rolling pass;
+// reversed stores them back to front, out[n - 1 - i]
+void kmer_ranks(const Alphabet& alphabet, const char* s, size_t len, uint32_t k, bool reversed, uint32_t* out);
+
 // ---------------------------------------------------------------------------------------------
 // Pore model
 // ---------------------------------------------------------------------------------------------
@@ -340,14 +344,15 @@ public:
     void forget_model(const PoreModel* model) { m_models.erase(model); }   // after a model was edited in place
     static Engine& thread_default();                  // lazily created, device from $NPH_DEVICE (default 0)
     void check(int status, const char* what) const;
-    // page-locked host staging owned by the engine, grown on demand and reused across calls (slot = one buffer per use)
-    void* pinned(int slot, size_t bytes);
+    // page-locked host staging owned by the engine, grown on demand and reused across calls: one buffer per use
+    enum class Staging { EventalignRecords, EventMeans, StartTimes, MethylationSites, Count };
+    void* pinned(Staging use, size_t bytes);
 
 private:
     nph_ctx* m_ctx = nullptr;
     std::unordered_map<const PoreModel*, uint32_t> m_models;
     struct Pinned { void* p = nullptr; size_t bytes = 0; };
-    Pinned m_pinned[4];
+    Pinned m_pinned[(int)Staging::Count];
 };
 
 // == snprintf(dst, ..., "%.<prec>lf", v), byte for byte, by exact integer arithmetic on the binary value (round half to
@@ -363,19 +368,66 @@ size_t format_fixed(char* dst, double v, int prec);
 // barrier; short bursts of 32-64 threads still fit one quota period.
 int host_threads();
 
+// body(i) for every i in [0, n) on `threads` workers, handed out `chunk` indices at a time.  An exception must not leave an
+// OpenMP region (that terminates the process): the message of the lowest index that threw is rethrown after the loop.
+template <typename Body>
+void parallel_for(size_t n, int threads, int chunk, const Body& body)
+{
+    long long failed = (long long)n;
+    std::string what;
+#pragma omp parallel for schedule(dynamic, chunk) num_threads(threads) if (threads > 1)
+    for (long long i = 0; i < (long long)n; ++i) {
+        try {
+            body((size_t)i);
+        } catch (const std::exception& e) {
+#pragma omp critical(nph_parallel_for_error)
+            if (i < failed) { failed = i; what = e.what(); }
+        }
+    }
+    if (failed < (long long)n) throw Error(NPH_ERR_INVALID, what);
+}
+
 namespace detail {
-// (read, strand) list -> the flat nph_read records + event arrays the C ABI takes.  The arrays live in the engine's
-// page-locked staging (slots 1 and 2: no page faults after the first batch, full-speed H2D) and stay valid until the next
-// flatten on the same engine; time is nullptr when no read has a drift term (the start times are then not needed).
+// The distinct (read, strand) pairs of a batch, numbered in the order they were first seen: the nph_read index the jobs
+// and records of the C ABI carry.
+class ReadTable {
+public:
+    typedef std::pair<const SquiggleRead*, uint8_t> Key;
+    uint32_t index(const SquiggleRead* read, uint8_t strand)
+    {
+        const Key key(read, strand);
+        if (!m_reads.empty() && m_reads.back() == key) return (uint32_t)m_reads.size() - 1;   // consecutive jobs of one read: the common case
+        auto it = m_index.find(key);
+        if (it != m_index.end()) return it->second;
+        m_index.emplace(key, (uint32_t)m_reads.size());
+        m_reads.push_back(key);
+        return (uint32_t)m_reads.size() - 1;
+    }
+    const std::vector<Key>& reads() const { return m_reads; }
+    size_t size() const { return m_reads.size(); }
+    void clear() { m_index.clear(); m_reads.clear(); }
+
+private:
+    std::map<Key, uint32_t> m_index;
+    std::vector<Key> m_reads;
+};
+
+// The table's reads -> the flat nph_read records + event arrays the C ABI takes.  The arrays live in the engine's
+// page-locked staging (no page faults after the first batch, full-speed H2D) and stay valid until the next flatten on the
+// same engine; time is nullptr when no read has a drift term (the start times are then not needed).
 struct FlatReads {
     std::vector<nph_read> reads;
     const float* mean = nullptr;
     const double* time = nullptr;
     size_t n_events = 0;
 };
-}
-namespace detail {
-FlatReads flatten_reads(Engine& engine, const std::vector<std::pair<const SquiggleRead*, uint8_t>>& reads);
+FlatReads flatten_reads(Engine& engine, const ReadTable& table);
+
+// What profile_hmm_score / profile_hmm_align check of one job, and the job: read resolved through `reads`; rank_off and
+// model_id are the caller's to fill.
+nph_hmm_job make_hmm_job(const HMMInputSequence& sequence, const HMMInputData& data, uint32_t flags, ReadTable& reads);
+// jobs[j].model_id = engine.model_id(models[j])
+void resolve_model_ids(Engine& engine, const std::vector<const PoreModel*>& models, std::vector<nph_hmm_job>& jobs);
 }
 
 // A batch of profile_hmm_score calls.  add() returns the index of the job's score in run()'s result.
@@ -402,9 +454,7 @@ public:
     const std::vector<uint8_t>& codes() const { return m_codes; }
 
 private:
-    struct ReadKey { const SquiggleRead* read; uint8_t strand; bool operator<(const ReadKey& o) const { return read != o.read ? read < o.read : strand < o.strand; } };
-    std::map<ReadKey, uint32_t> m_read_index;
-    std::vector<ReadKey> m_reads;
+    detail::ReadTable m_reads;
     std::vector<const PoreModel*> m_job_models;
     std::vector<nph_hmm_job> m_jobs;
     std::vector<uint8_t> m_codes;           // per distinct (sequence, strand): its symbols' alphabet ranks; jobs' rank_off index this
@@ -419,7 +469,7 @@ public:
     std::vector<std::vector<AlignedPair>> run(Engine& engine);
 
 private:
-    std::vector<const SquiggleRead*> m_reads;
+    detail::ReadTable m_reads;
     const PoreModel* m_model = nullptr;
     std::vector<nph_abea_job> m_jobs;
     std::vector<uint32_t> m_ranks;

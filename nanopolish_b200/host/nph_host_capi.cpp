@@ -22,6 +22,20 @@ bool g_raw_is_rna = false;
 uint32_t g_load_flags = 0;
 thread_local std::string g_err;
 template <typename F> int guard(F f) { try { f(); return 0; } catch (const Error& e) { g_err = e.what(); return e.status; } catch (const std::exception& e) { g_err = e.what(); return NPH_ERR_INVALID; } }
+
+// a job over events [e_start, e_stop] of strand 0 of a registered read, read backwards on the rc strand
+HMMInputData input_data(int read, const PoreModel* model, uint32_t e_start, uint32_t e_stop, int rc)
+{
+    HMMInputData data;
+    data.read = g_reads[read].get();
+    data.pore_model = model;
+    data.event_start_idx = e_start;
+    data.event_stop_idx = e_stop;
+    data.strand = 0;
+    data.rc = (uint8_t)rc;
+    data.event_stride = rc ? -1 : 1;
+    return data;
+}
 }
 
 extern "C" {
@@ -62,7 +76,7 @@ int nphh_lexicographic_next(const char* alphabet, const char* in, char* out)
     return (int)s.size();
 }
 
-// HMMInputSequence::append_kmer_ranks (the rolling pass HmmBatch::add uses) against get_kmer_rank: mismatching positions
+// HMMInputSequence::append_kmer_ranks (the rolling pass AlignBatch::add uses) against get_kmer_rank: mismatching positions
 int nphh_kmer_ranks_rolling_check(const char* alphabet, const char* seq, uint32_t k, int rc)
 {
     int bad = -1;
@@ -137,15 +151,7 @@ int nphh_profile_hmm_score(int read, int model, const char* seq, uint32_t e_star
     return guard([&] {
         const PoreModel* pm = g_models[model].get();
         HMMInputSequence sequence(std::string(seq), pm->pmalphabet);
-        HMMInputData data;
-        data.read = g_reads[read].get();
-        data.pore_model = pm;
-        data.event_start_idx = e_start;
-        data.event_stop_idx = e_stop;
-        data.strand = 0;
-        data.rc = rc;
-        data.event_stride = rc ? -1 : 1;
-        *out = profile_hmm_score(sequence, data, flags);
+        *out = profile_hmm_score(sequence, input_data(read, pm, e_start, e_stop, rc), flags);
     });
 }
 
@@ -158,15 +164,7 @@ int nphh_profile_hmm_score_many(size_t n, const int32_t* read, const int32_t* mo
         for (size_t j = 0; j < n; ++j) {
             const PoreModel* pm = g_models[model[j]].get();
             HMMInputSequence sequence(std::string(seq_buf + seq_off[j], seq_buf + seq_off[j + 1]), pm->pmalphabet);
-            HMMInputData data;
-            data.read = g_reads[read[j]].get();
-            data.pore_model = pm;
-            data.event_start_idx = e_start[j];
-            data.event_stop_idx = e_stop[j];
-            data.strand = 0;
-            data.rc = rc[j];
-            data.event_stride = rc[j] ? -1 : 1;
-            b.add(sequence, data, flags[j]);
+            b.add(sequence, input_data(read[j], pm, e_start[j], e_stop[j], rc[j]), flags[j]);
         }
         std::vector<float> s = b.run(Engine::thread_default());
         std::memcpy(out, s.data(), sizeof(float) * n);
@@ -180,15 +178,7 @@ int nphh_profile_hmm_score_set(int read, int model, int n_seqs, const char** seq
     return guard([&] {
         std::vector<HMMInputSequence> ss;
         for (int i = 0; i < n_seqs; ++i) ss.emplace_back(std::string(seqs[i]), get_alphabet_by_name(alphabets[i]));
-        HMMInputData data;
-        data.read = g_reads[read].get();
-        data.pore_model = g_models[model].get();
-        data.event_start_idx = e_start;
-        data.event_stop_idx = e_stop;
-        data.strand = 0;
-        data.rc = rc;
-        data.event_stride = rc ? -1 : 1;
-        *out = profile_hmm_score_set(ss, data, flags);
+        *out = profile_hmm_score_set(ss, input_data(read, g_models[model].get(), e_start, e_stop, rc), flags);
     });
 }
 
@@ -234,15 +224,7 @@ int nphh_score_variants_thresholded(int n_reads, const int32_t* read, const uint
 {
     return guard([&] {
         std::vector<HMMInputData> input(n_reads);
-        for (int j = 0; j < n_reads; ++j) {
-            input[j].read = g_reads[read[j]].get();
-            input[j].pore_model = g_models[model].get();
-            input[j].event_start_idx = e_start[j];
-            input[j].event_stop_idx = e_stop[j];
-            input[j].strand = 0;
-            input[j].rc = rc[j];
-            input[j].event_stride = rc[j] ? -1 : 1;
-        }
+        for (int j = 0; j < n_reads; ++j) input[j] = input_data(read[j], g_models[model].get(), e_start[j], e_stop[j], rc[j]);
         std::vector<Variant> vars(n_var);
         for (int i = 0; i < n_var; ++i) { vars[i].ref_name = "ctg"; vars[i].ref_position = pos[i]; vars[i].ref_seq = ref_seq[i]; vars[i].alt_seq = alt_seq[i]; }
         std::vector<std::string> mt;
@@ -263,15 +245,7 @@ long long nphh_score_variant_group(int n_reads, const int32_t* read, const uint3
     long long n = -1;
     int st = guard([&] {
         std::vector<HMMInputData> input(n_reads);
-        for (int j = 0; j < n_reads; ++j) {
-            input[j].read = g_reads[read[j]].get();
-            input[j].pore_model = g_models[model].get();
-            input[j].event_start_idx = e_start[j];
-            input[j].event_stop_idx = e_stop[j];
-            input[j].strand = 0;
-            input[j].rc = rc[j];
-            input[j].event_stride = rc[j] ? -1 : 1;
-        }
+        for (int j = 0; j < n_reads; ++j) input[j] = input_data(read[j], g_models[model].get(), e_start[j], e_stop[j], rc[j]);
         std::vector<Variant> vars(n_var);
         for (int i = 0; i < n_var; ++i) { vars[i].ref_name = "ctg"; vars[i].ref_position = pos[i]; vars[i].ref_seq = ref_seq[i]; vars[i].alt_seq = alt_seq[i]; }
         std::vector<std::string> mt;
@@ -291,10 +265,11 @@ long long nphh_score_variant_group(int n_reads, const int32_t* read, const uint3
 }
 
 // ---- N3: call-methylation for a batch of reads; returns the concatenated TSV ------------------------------
-// aligned pairs are (ref_pos, event_idx) interleaved, pair_off[n_reads+1]
-static long long call_methylation_impl(int n_reads, const int32_t* read, const char** read_names, const uint8_t* is_rev, const uint8_t* rc,
-                                       const int32_t* ref_start, const char** ref_seqs, const int32_t* pairs, const uint64_t* pair_off,
-                                       const char* contig, double indel_bias, char* tsv_out, size_t cap, uint64_t* n_jobs_out, double* secs4)
+// aligned pairs are (ref_pos, event_idx) interleaved, pair_off[n_reads+1].  secs4 (optional): the seconds spent in {staging
+// (add_reads), flatten + device call, TSV formatting, the shim's own marshalling}
+long long nphh_call_methylation_timed(int n_reads, const int32_t* read, const char** read_names, const uint8_t* is_rev, const uint8_t* rc,
+                                      const int32_t* ref_start, const char** ref_seqs, const int32_t* pairs, const uint64_t* pair_off,
+                                      const char* contig, double indel_bias, char* tsv_out, size_t cap, uint64_t* n_jobs_out, double* secs4)
 {
     long long n = -1;
     auto now = [] { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
@@ -340,16 +315,8 @@ long long nphh_call_methylation(int n_reads, const int32_t* read, const char** r
                                 const int32_t* ref_start, const char** ref_seqs, const int32_t* pairs, const uint64_t* pair_off,
                                 const char* contig, double indel_bias, char* tsv_out, size_t cap, uint64_t* n_jobs_out)
 {
-    return call_methylation_impl(n_reads, read, read_names, is_rev, rc, ref_start, ref_seqs, pairs, pair_off, contig, indel_bias, tsv_out, cap,
-                                 n_jobs_out, nullptr);
-}
-// the same, with the seconds spent in {staging (add_reads), flatten + device call, TSV formatting, the shim's own marshalling}: secs4[4]
-long long nphh_call_methylation_timed(int n_reads, const int32_t* read, const char** read_names, const uint8_t* is_rev, const uint8_t* rc,
-                                      const int32_t* ref_start, const char** ref_seqs, const int32_t* pairs, const uint64_t* pair_off,
-                                      const char* contig, double indel_bias, char* tsv_out, size_t cap, uint64_t* n_jobs_out, double* secs3)
-{
-    return call_methylation_impl(n_reads, read, read_names, is_rev, rc, ref_start, ref_seqs, pairs, pair_off, contig, indel_bias, tsv_out, cap,
-                                 n_jobs_out, secs3);
+    return nphh_call_methylation_timed(n_reads, read, read_names, is_rev, rc, ref_start, ref_seqs, pairs, pair_off, contig, indel_bias, tsv_out,
+                                       cap, n_jobs_out, nullptr);
 }
 
 // call-methylation from flat host buffers (the C-ABI layout) to TSV bytes: what bench.py's end-to-end arm times.
@@ -581,11 +548,11 @@ long long nphh_ea_text(int idx, int what, char* out, size_t cap)
 }
 
 // every read's TSV rows concatenated in read order, formatted in parallel (EventAligner::tsv_batch)
-long long nphh_ea_tsv_all(char* out, size_t cap)
+static long long ea_tsv_all(const EventalignOptions& opt, char* out, size_t cap)
 {
     long long n = -1;
     int rc = guard([&] {
-        const std::vector<std::string> parts = g_aligner.tsv_batch();
+        const std::vector<std::string> parts = g_aligner.tsv_batch(opt);
         size_t total = 0;
         for (const std::string& s : parts) total += s.size();
         n = (long long)total;
@@ -596,6 +563,16 @@ long long nphh_ea_tsv_all(char* out, size_t cap)
         *o = 0;
     });
     return rc ? rc : n;
+}
+
+long long nphh_ea_tsv_all(char* out, size_t cap) { return ea_tsv_all(EventalignOptions(), out, cap); }
+
+// the same with --signal-index --samples (every read needs its raw samples)
+long long nphh_ea_tsv_all_samples(char* out, size_t cap)
+{
+    EventalignOptions opt;
+    opt.write_signal_index = opt.write_samples = true;
+    return ea_tsv_all(opt, out, cap);
 }
 
 // format_fixed against the C library on n float bit patterns drawn from `seed` (uniform bit patterns, then values
@@ -639,7 +616,7 @@ long long nphh_format_fixed_check(uint64_t seed, size_t n)
     return bad;
 }
 
-// rolling_kmer_ranks against Alphabet::kmer_rank on every k-mer of seq: number of mismatches
+// kmer_ranks against Alphabet::kmer_rank on every k-mer of seq: number of mismatches
 long long nphh_rolling_ranks_check(const char* alphabet, const char* seq, uint32_t k)
 {
     long long bad = -1;
@@ -647,7 +624,7 @@ long long nphh_rolling_ranks_check(const char* alphabet, const char* seq, uint32
         const Alphabet* a = get_alphabet_by_name(alphabet);
         const std::string s(seq);
         std::vector<uint32_t> r(s.size() >= k ? s.size() - k + 1 : 0);
-        rolling_kmer_ranks(a, s, k, r.data());
+        kmer_ranks(*a, s.data(), s.size(), k, false, r.data());
         bad = 0;
         for (size_t i = 0; i < r.size(); ++i) bad += r[i] != a->kmer_rank(s.c_str() + i, k);
     });

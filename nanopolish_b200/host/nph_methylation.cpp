@@ -290,26 +290,17 @@ void MethylationCaller::run(Engine& engine, double indel_bias)
     for (ReadEntry& re : m_reads) { re.sites.clear(); re.sites_built = false; }
     m_ran = true;
     if (m_records.empty()) return;
-    // one nph_read per distinct (SquiggleRead, strand); consecutive records of one read are the common case
-    std::vector<std::pair<const SquiggleRead*, uint8_t>> uniq;
-    std::map<std::pair<const SquiggleRead*, uint8_t>, uint32_t> index;
+    // one nph_read per distinct (SquiggleRead, strand)
+    detail::ReadTable reads;
     uint32_t k = 0;
     for (size_t i = 0; i < m_records.size(); ++i) {
         const Record& rm = m_record_meta[i];
-        const std::pair<const SquiggleRead*, uint8_t> key(rm.read, rm.strand);
-        uint32_t ridx;
-        if (!uniq.empty() && uniq.back() == key) ridx = (uint32_t)uniq.size() - 1;
-        else {
-            auto it = index.find(key);
-            if (it == index.end()) { ridx = (uint32_t)uniq.size(); index[key] = ridx; uniq.push_back(key); }
-            else ridx = it->second;
-        }
-        m_records[i].read = ridx;
+        m_records[i].read = reads.index(rm.read, rm.strand);
         m_records[i].model_id = engine.model_id(rm.model);
         if (k && rm.model->k != k) throw Error(NPH_ERR_UNSUPPORTED, "models with different k in one call-methylation batch");
         k = rm.model->k;
     }
-    const detail::FlatReads fr = detail::flatten_reads(engine, uniq);
+    const detail::FlatReads fr = detail::flatten_reads(engine, reads);
     const nph_meth_params mp = make_meth_params(m_params, k, m_region_start, m_region_end);
     size_t cap = 0;
     for (const nph_meth_record& r : m_records) cap += r.ref_len / (size_t)(m_params.min_separation + 1) + 2;
@@ -452,12 +443,8 @@ std::string MethylationCaller::tsv(size_t read_idx) const
 
 std::vector<std::string> MethylationCaller::tsv_batch() const
 {
-    std::vector<std::string> out(m_reads.size()), errors(m_reads.size());
-#pragma omp parallel for schedule(dynamic, 16) num_threads(host_threads()) if (m_reads.size() > 64)
-    for (long long i = 0; i < (long long)m_reads.size(); ++i) {
-        try { out[i] = tsv((size_t)i); } catch (const std::exception& ex) { errors[i] = ex.what(); }
-    }
-    for (const std::string& e : errors) if (!e.empty()) throw Error(NPH_ERR_INVALID, e);
+    std::vector<std::string> out(m_reads.size());
+    parallel_for(m_reads.size(), m_reads.size() > 64 ? host_threads() : 1, 16, [&](size_t i) { out[i] = tsv(i); });
     return out;
 }
 
@@ -467,16 +454,11 @@ size_t MethylationCaller::tsv_all(char* out, size_t cap) const
     const size_t n = m_reads.size();
     const int T = (int)std::max<size_t>(1, std::min<size_t>((size_t)host_threads(), (n + 63) / 64));
     std::vector<RowBuffer> parts((size_t)T);
-    std::vector<std::string> errors((size_t)T);
-#pragma omp parallel for schedule(static, 1) num_threads(T) if (T > 1)
-    for (int t = 0; t < T; ++t) {
-        const size_t b = n * (size_t)t / (size_t)T, e = n * ((size_t)t + 1) / (size_t)T;
-        try {
-            parts[t].room((e - b) * 4096);
-            for (size_t i = b; i < e; ++i) put_rows(&parts[t], i);
-        } catch (const std::exception& ex) { errors[t] = ex.what(); }
-    }
-    for (const std::string& e : errors) if (!e.empty()) throw Error(NPH_ERR_INVALID, e);
+    parallel_for((size_t)T, T, 1, [&](size_t t) {
+        const size_t b = n * t / (size_t)T, e = n * (t + 1) / (size_t)T;
+        parts[t].room((e - b) * 4096);
+        for (size_t i = b; i < e; ++i) put_rows(&parts[t], i);
+    });
     std::vector<size_t> off((size_t)T + 1, 0);
     for (int t = 0; t < T; ++t) off[t + 1] = off[t] + parts[t].n;
     if (off[T] > cap || !out) return off[T];
@@ -496,21 +478,16 @@ void format_records(const FlatMethylationBatch& b, uint32_t k, const uint64_t* s
     parts.clear();
     parts.resize((size_t)T);
     const std::string contig(b.contig ? b.contig : "");
-    std::vector<std::string> errors((size_t)T);
-#pragma omp parallel for schedule(static, 1) num_threads(T) if (T > 1)
-    for (int t = 0; t < T; ++t) {
-        const size_t lo = n * (size_t)t / (size_t)T, hi = n * ((size_t)t + 1) / (size_t)T;
+    parallel_for((size_t)T, T, 1, [&](size_t t) {
+        const size_t lo = n * t / (size_t)T, hi = n * (t + 1) / (size_t)T;
         RowBuffer& out = parts[t];
-        try {
-            out.room((size_t)(site_off[hi] - site_off[lo]) * 96 + 64);
-            for (size_t r = lo; r < hi; ++r) {
-                const char* name = b.read_names[r];
-                append_record_rows(out, contig, b.is_reverse[r] != 0, name, std::strlen(name), b.ref_bases, b.records[r], k, sites + site_off[r],
-                                   (size_t)(site_off[r + 1] - site_off[r]));
-            }
-        } catch (const std::exception& ex) { errors[t] = ex.what(); }
-    }
-    for (const std::string& e : errors) if (!e.empty()) throw Error(NPH_ERR_INVALID, e);
+        out.room((size_t)(site_off[hi] - site_off[lo]) * 96 + 64);
+        for (size_t r = lo; r < hi; ++r) {
+            const char* name = b.read_names[r];
+            append_record_rows(out, contig, b.is_reverse[r] != 0, name, std::strlen(name), b.ref_bases, b.records[r], k, sites + site_off[r],
+                               (size_t)(site_off[r + 1] - site_off[r]));
+        }
+    });
 }
 } // namespace
 
@@ -544,7 +521,8 @@ size_t call_methylation_flat(Engine& engine, const FlatMethylationBatch& b, cons
     }
     size_t site_cap = 0;
     for (size_t r = 0; r < n; ++r) site_cap += b.records[r].ref_len / (size_t)(params.min_separation + 1) + 2;
-    nph_meth_site* sites = static_cast<nph_meth_site*>(engine.pinned(3, sizeof(nph_meth_site) * std::max<size_t>(site_cap, 1)));
+    nph_meth_site* sites =
+        static_cast<nph_meth_site*>(engine.pinned(Engine::Staging::MethylationSites, sizeof(nph_meth_site) * std::max<size_t>(site_cap, 1)));
     std::vector<uint64_t> site_off(n + 1, 0);
     uint64_t scored = 0;
     const double td = now();

@@ -98,7 +98,8 @@ std::vector<std::unique_ptr<SquiggleRead>> load_from_raw(Engine& engine, const P
         if (raw[i].samples.empty() || seq.size() < k || !(raw[i].sample_rate > 0.0)) { ++st.empty_after_trim; continue; }
         const uint32_t n_kmers = (uint32_t)(seq.size() - k + 1);
         jobs.push_back(nph_raw_job{total, ranks.size(), (uint32_t)raw[i].samples.size(), n_kmers, raw[i].sample_rate});
-        for (uint32_t j = 0; j < n_kmers; ++j) ranks.push_back(base_model.pmalphabet->kmer_rank(seq.c_str() + j, k));
+        ranks.resize(ranks.size() + n_kmers);
+        kmer_ranks(*base_model.pmalphabet, seq.data(), seq.size(), k, false, ranks.data() + jobs.back().rank_off);
         total += raw[i].samples.size();
         sent.push_back((uint32_t)i);
     }

@@ -203,6 +203,44 @@ def test_host_chaining_logic_on_cpu(host, cases, restated, golden, port_oracle):
     host.nphh_ea_begin()
 
 
+_MISSING_SAMPLES = r"""
+import ctypes as C, sys
+import numpy as np
+host = C.CDLL(sys.argv[1])
+host.nphh_last_error.restype = C.c_char_p
+host.nphh_ea_tsv_all.restype = host.nphh_ea_tsv_all_samples.restype = C.c_longlong
+p = lambda a: a.ctypes.data_as(C.c_void_p)
+mean, sd = np.linspace(60.0, 120.0, 1024), np.full(1024, 2.0)
+mh = host.nphh_model_create(b"nucleotide", 5, 1024, p(mean), p(sd), None)
+ev, t = np.full(50, 90.0, np.float32), np.arange(50, dtype=np.float64) / 1000.0
+reads = [host.nphh_read_create(50, p(ev), p(t), C.c_double(0.0), C.c_double(1.0), C.c_double(0.0), C.c_double(1.0), C.c_double(1.5), mh)
+         for _ in range(2)]
+smp = np.zeros(400, np.float32)
+assert host.nphh_read_set_samples(reads[0], p(smp), C.c_size_t(400), C.c_double(4000.0)) == 0          # the second read has none
+host.nphh_ea_begin()
+cigar = np.zeros(1, np.uint32)
+for i, r in enumerate(reads):
+    assert host.nphh_ea_add_read(r, b"ctg", 0, 4, 0, p(cigar), 0, b"ACGTACGTAC", i, -1, -1) == i
+buf = C.create_string_buffer(1 << 16)
+print(host.nphh_ea_tsv_all(buf, C.c_size_t(1 << 16)))
+print(host.nphh_ea_tsv_all_samples(buf, C.c_size_t(1 << 16)))
+print(host.nphh_last_error().decode())
+"""
+
+
+def test_tsv_batch_reports_a_read_without_samples():
+    """--samples rows for a batch in which one read kept no raw samples: tsv() throws for that read inside tsv_batch's
+    parallel loop, and the batch must return an error status instead of terminating the process (run in a child)."""
+    import subprocess
+    import sys
+    from tests.test_host_mirror import HOST_SO
+    r = subprocess.run([sys.executable, "-c", _MISSING_SAMPLES, HOST_SO], capture_output=True, text=True, timeout=120)
+    assert r.returncode == 0, r.stderr
+    plain, with_samples, err = r.stdout.splitlines()
+    assert int(plain) == 0                                 # without the sample columns both reads format (unmapped: no rows)
+    assert int(with_samples) < 0 and "--samples" in err
+
+
 def _drive_rounds(host, cs, rs, model, port_oracle):
     """pull every round's jobs out of the C++ cursors and feed back the plain-C Viterbi's paths"""
     jobs = np.zeros(max(len(cs), 1), synth.HMM_JOB_DT)
