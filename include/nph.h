@@ -210,7 +210,8 @@ int nph_score_set_combine(const float* scores, size_t n_groups, uint32_t n_alt, 
 
 /* ---- adaptive_banded_simple_event_align -------------------------------------------------
  * One-shot, host buffers (synchronous). pairs_out receives, for job j, results[j].n_pairs
- * AlignedPairs at pairs_out + jobs[j].pairs_off in the reference's order (ascending). */
+ * AlignedPairs at pairs_out + jobs[j].pairs_off in the reference's order (ascending).
+ * Both forms return NPH_ERR_INVALID for a k-mer rank >= the model's n_states. */
 int nph_abea_batch(nph_ctx* ctx,
                    const nph_read* reads, size_t n_reads,
                    const float* ev_mean, const double* ev_start_time, size_t n_events_total,
@@ -224,7 +225,8 @@ int nph_abea_run(nph_ctx* ctx);
 int nph_abea_fetch(nph_ctx* ctx, nph_aligned_pair* pairs_out, size_t pairs_total,
                    nph_abea_result* results, size_t n_jobs);
 
-/* estimate_scalings_using_mom for each job's read/sequence: out[j] = {shift, scale} (drift 0, var 1). */
+/* estimate_scalings_using_mom for each job's read/sequence: out[j] = {shift, scale} (drift 0, var 1).
+ * NPH_ERR_INVALID for a k-mer rank >= the model's n_states. */
 int nph_mom_batch(nph_ctx* ctx, const nph_read* reads, size_t n_reads,
                   const float* ev_mean, size_t n_events_total,
                   const uint32_t* kmer_ranks, size_t n_ranks_total,
@@ -637,7 +639,8 @@ int nph_recalibrate_batch(nph_ctx* ctx, const nph_read* reads, size_t n_reads, c
  * SquiggleEvent::log_stdv = logf(stdv) is left to the caller's libm), calibrations_out[j] (status != 0: the reference
  * clears the read's events; the arrays still hold them), base_to_event_out[rank_off + ki] (optional).
  * A read that trims to nothing (the reference aborts on it) gets no events and NPH_CAL_EMPTY_AFTER_TRIM.
- * NPH_ERR_UNSUPPORTED if events_cap is too small (n_samples_total / 3 always suffices). */
+ * NPH_ERR_UNSUPPORTED if events_cap is too small (n_samples_total / 3 always suffices).  NPH_ERR_INVALID for a k-mer rank
+ * >= the model's n_states, before any step runs. */
 #define NPH_CAL_EMPTY_AFTER_TRIM 16
 typedef struct {
     uint64_t sample_off;      /* first raw sample (picoamps, float) of this read in raw[] */

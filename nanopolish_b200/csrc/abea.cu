@@ -408,17 +408,11 @@ __global__ void __launch_bounds__(kThreads) mom_kernel(const MomParams p)
     }
 }
 
-int validate_abea_jobs(nph_ctx* ctx, const nph_abea_job* jobs, size_t n_jobs, size_t n_ranks_total, uint32_t model_id,
-                       size_t pairs_total)
+// nph_check_ranks: *bad = 1 if a rank is not a state of the model
+__global__ void check_ranks_kernel(const uint32_t* ranks, size_t n, uint32_t n_states, unsigned int* bad)
 {
-    if (model_id >= ctx->models.size()) return NPH_ERR_INVALID;
-    for (size_t j = 0; j < n_jobs; ++j) {
-        const nph_abea_job& jb = jobs[j];
-        if (jb.read >= ctx->n_reads || jb.n_kmers == 0) return NPH_ERR_INVALID;
-        if (jb.n_kmers > n_ranks_total || jb.rank_off > n_ranks_total - jb.n_kmers) return NPH_ERR_INVALID;      // overflow-safe
-        if (jb.pairs_cap > pairs_total || jb.pairs_off > pairs_total - jb.pairs_cap) return NPH_ERR_INVALID;
-    }
-    return NPH_OK;
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+        if (ranks[i] >= n_states) *bad = 1u;
 }
 
 // per warp: kmax Gaussians, then trace_stride bytes of band trace
@@ -447,7 +441,7 @@ int nph_launch_abea(nph_ctx* ctx)
     p.results = ctx->d_abea_res.p;
     p.kmax_stride = ctx->abea_kmax;
     p.trace_stride = ctx->abea_trace_stride;
-    NphArena scratch{ctx->d_abea_scratch.p};
+    NphArena scratch{ctx->d_align_scratch.p};
     scratch_layout(ctx, scratch, &p.scratch_params, &p.scratch_trace);
     p.consts = reinterpret_cast<const AbeaJobConsts*>(ctx->d_abea_consts.p);
     p.lp_skip = log(1e-10);
@@ -466,16 +460,67 @@ int nph_launch_abea(nph_ctx* ctx)
     return NPH_OK;
 }
 
-// estimate_scalings_using_mom over the loaded ABEA jobs (reads, ranks and jobs already on the device)
-int nph_launch_mom(nph_ctx* ctx, double* d_shift_scale_out, bool reversed)
+int nph_launch_mom(nph_ctx* ctx, const nph_abea_job* d_jobs, const uint32_t* d_ranks, size_t n_jobs, uint32_t model_id, double* d_out, bool reversed)
 {
     MomParams p{};
     p.reversed = reversed ? 1 : 0;
-    p.ev_mean = ctx->d_ev_mean.p; p.reads = ctx->d_reads.p; p.models = ctx->d_models.p; p.model_id = ctx->abea_model;
-    p.ranks = ctx->d_abea_ranks.p; p.jobs = ctx->d_abea_jobs.p; p.n_jobs = (uint32_t)ctx->n_abea_jobs; p.out = d_shift_scale_out;
-    const int grid = (int)std::min<size_t>((ctx->n_abea_jobs + kWarps - 1) / kWarps, (size_t)ctx->sm_count * 4);
+    p.ev_mean = ctx->d_ev_mean.p; p.reads = ctx->d_reads.p; p.models = ctx->d_models.p; p.model_id = model_id;
+    p.ranks = d_ranks; p.jobs = d_jobs; p.n_jobs = (uint32_t)n_jobs; p.out = d_out;
+    const int grid = (int)std::min<size_t>((n_jobs + kWarps - 1) / kWarps, (size_t)ctx->sm_count * 4);
     mom_kernel<<<grid, kThreads, 0, ctx->stream>>>(p);
     NPH_CUDA(ctx, cudaGetLastError());
+    return NPH_OK;
+}
+
+int nph_check_ranks(nph_ctx* ctx, const uint32_t* d_ranks, size_t n, uint32_t n_states)
+{
+    unsigned int* flag = ctx->d_counters.p + (NPH_NUM_COUNTERS - 2);
+    unsigned int bad = 0;
+    NPH_CUDA(ctx, cudaMemsetAsync(flag, 0, sizeof(unsigned int), ctx->stream));
+    if (n) check_ranks_kernel<<<(unsigned)std::min<size_t>((n + 255) / 256, (size_t)ctx->sm_count * 8), 256, 0, ctx->stream>>>(d_ranks, n, n_states, flag);
+    NPH_CUDA(ctx, cudaGetLastError());
+    NPH_CUDA(ctx, cudaMemcpyAsync(&bad, flag, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));
+    NPH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if (bad) { ctx->last_error = "a k-mer rank is not a state of the model"; return NPH_ERR_INVALID; }
+    return NPH_OK;
+}
+
+int nph_abea_stage(nph_ctx* ctx, const uint32_t* n_events, const nph_abea_job* jobs, size_t n_jobs, size_t n_ranks_total, uint32_t model_id,
+                   size_t pairs_total)
+{
+    // per-job transition penalties, evaluated with the host libm in FP64 exactly as raw_loader.cpp:95-108
+    std::vector<AbeaJobConsts> consts(n_jobs);
+    std::vector<uint64_t> bands(n_jobs);
+    uint32_t kmax = 1;
+    uint64_t max_bands = 4;
+    const double lp_skip = log(1e-10);
+    for (size_t j = 0; j < n_jobs; ++j) {
+        const double events_per_kmer = (double)n_events[jobs[j].read] / jobs[j].n_kmers;
+        const double p_stay = 1 - (1 / (events_per_kmer + 1));
+        consts[j].lp_stay = log(p_stay);
+        consts[j].lp_step = log(1.0 - exp(lp_skip) - exp(consts[j].lp_stay));
+        bands[j] = (uint64_t)n_events[jobs[j].read] + jobs[j].n_kmers + 2;
+        kmax = std::max(kmax, jobs[j].n_kmers);
+        max_bands = std::max(max_bands, bands[j]);
+    }
+    const std::vector<uint32_t> order = nph_longest_first(bands);     // longest reads first
+
+    ctx->abea_kmax = kmax;
+    ctx->abea_trace_stride = 32 * (max_bands + kTraceBlockRows);
+    NPH_TRY(nph_reserve(ctx, ctx->d_align_scratch, nph_layout_bytes([&](NphArena& a) { float4* q; uint8_t* t; scratch_layout(ctx, a, &q, &t); })));
+    NPH_TRY(nph_reserve(ctx, ctx->d_abea_jobs, n_jobs));
+    NPH_TRY(nph_reserve(ctx, ctx->d_abea_ranks, n_ranks_total));
+    NPH_TRY(nph_reserve(ctx, ctx->d_abea_order, n_jobs));
+    NPH_TRY(nph_reserve(ctx, ctx->d_abea_consts, 2 * n_jobs));
+    NPH_TRY(nph_reserve(ctx, ctx->d_pairs, pairs_total));
+    NPH_TRY(nph_reserve(ctx, ctx->d_abea_res, n_jobs));
+    // copies from pageable memory: the runtime has taken order and consts before each call returns
+    NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_abea_jobs.p, jobs, sizeof(nph_abea_job) * n_jobs, cudaMemcpyHostToDevice, ctx->stream));
+    NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_abea_order.p, order.data(), sizeof(uint32_t) * n_jobs, cudaMemcpyHostToDevice, ctx->stream));
+    NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_abea_consts.p, consts.data(), sizeof(AbeaJobConsts) * n_jobs, cudaMemcpyHostToDevice, ctx->stream));
+    ctx->n_abea_jobs = n_jobs;
+    ctx->abea_pairs_total = pairs_total;
+    ctx->abea_model = model_id;
     return NPH_OK;
 }
 
@@ -486,46 +531,18 @@ int nph_abea_jobs_load(nph_ctx* ctx, const uint32_t* kmer_ranks, size_t n_ranks_
 {
     if (!ctx || !kmer_ranks || !jobs || n_jobs == 0) return NPH_ERR_INVALID;
     if (!ctx->reads_loaded) return NPH_ERR_STATE;
-    NPH_CUDA(ctx, cudaSetDevice(ctx->device));
-    NPH_TRY(validate_abea_jobs(ctx, jobs, n_jobs, n_ranks_total, model_id, pairs_total));
-
-    // per-job transition penalties, evaluated with the host libm in FP64 exactly as raw_loader.cpp:95-108
-    std::vector<AbeaJobConsts> consts(n_jobs);
-    std::vector<uint64_t> bands(n_jobs);
-    uint32_t kmax = 1;
-    uint64_t max_bands = 4;
-    const double lp_skip = log(1e-10);
-    for (size_t j = 0; j < n_jobs; ++j) {
-        const double n_events = (double)ctx->h_read_n_events[jobs[j].read];
-        const double events_per_kmer = n_events / jobs[j].n_kmers;
-        const double p_stay = 1 - (1 / (events_per_kmer + 1));
-        consts[j].lp_stay = log(p_stay);
-        consts[j].lp_step = log(1.0 - exp(lp_skip) - exp(consts[j].lp_stay));
-        bands[j] = (uint64_t)ctx->h_read_n_events[jobs[j].read] + jobs[j].n_kmers + 2;
-        kmax = std::max(kmax, jobs[j].n_kmers);
-        max_bands = std::max(max_bands, bands[j]);
-    }
-    const std::vector<uint32_t> order = nph_longest_first(bands);     // longest reads first
-
-    ctx->abea_kmax = kmax;
-    ctx->abea_trace_stride = 32 * (max_bands + kTraceBlockRows);
-    NPH_TRY(nph_reserve(ctx, ctx->d_abea_scratch, nph_layout_bytes([&](NphArena& a) { float4* q; uint8_t* t; scratch_layout(ctx, a, &q, &t); })));
-    NPH_TRY(nph_reserve(ctx, ctx->d_abea_jobs, n_jobs));
-    NPH_TRY(nph_reserve(ctx, ctx->d_abea_ranks, n_ranks_total));
-    NPH_TRY(nph_reserve(ctx, ctx->d_abea_order, n_jobs));
-    NPH_TRY(nph_reserve(ctx, ctx->d_abea_consts, 2 * n_jobs));
-    NPH_TRY(nph_reserve(ctx, ctx->d_pairs, pairs_total));
-    NPH_TRY(nph_reserve(ctx, ctx->d_abea_res, n_jobs));
-    NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_abea_jobs.p, jobs, sizeof(nph_abea_job) * n_jobs, cudaMemcpyHostToDevice, ctx->stream));
-    NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_abea_ranks.p, kmer_ranks, sizeof(uint32_t) * n_ranks_total, cudaMemcpyHostToDevice, ctx->stream));
-    NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_abea_order.p, order.data(), sizeof(uint32_t) * n_jobs, cudaMemcpyHostToDevice, ctx->stream));
-    NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_abea_consts.p, consts.data(), sizeof(AbeaJobConsts) * n_jobs, cudaMemcpyHostToDevice, ctx->stream));
-    NPH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    ctx->n_abea_jobs = n_jobs;
-    ctx->abea_pairs_total = pairs_total;
-    ctx->abea_model = model_id;
-    ctx->abea_loaded = true;
-    return NPH_OK;
+    if (model_id >= ctx->models.size()) return NPH_ERR_INVALID;
+    for (size_t j = 0; j < n_jobs; ++j)
+        if (!nph_abea_job_ok(jobs[j], ctx->n_reads, n_ranks_total, jobs[j].pairs_cap, pairs_total)) return NPH_ERR_INVALID;
+    auto stage = [&]() -> int {
+        NPH_CUDA(ctx, cudaSetDevice(ctx->device));
+        NPH_TRY(nph_abea_stage(ctx, ctx->h_read_n_events.data(), jobs, n_jobs, n_ranks_total, model_id, pairs_total));
+        NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_abea_ranks.p, kmer_ranks, sizeof(uint32_t) * n_ranks_total, cudaMemcpyHostToDevice, ctx->stream));
+        return nph_check_ranks(ctx, ctx->d_abea_ranks.p, n_ranks_total, ctx->models[model_id].n_states);   // the call's one sync
+    };
+    const int rc = stage();
+    ctx->abea_loaded = rc == NPH_OK;      // from the first upload on, the ABEA buffers hold this batch
+    return rc;
 }
 
 int nph_abea_run(nph_ctx* ctx)
@@ -569,23 +586,18 @@ int nph_mom_batch(nph_ctx* ctx, const nph_read* reads, size_t n_reads,
     // scalings are what this call estimates: load the reads with whatever the caller has (only events are used)
     NPH_TRY(nph_reads_load(ctx, reads, n_reads, ev_mean, nullptr, n_events_total));
     if (model_id >= ctx->models.size()) return NPH_ERR_INVALID;
-    for (size_t j = 0; j < n_jobs; ++j) {
-        if (jobs[j].read >= n_reads || jobs[j].n_kmers == 0 || jobs[j].n_kmers > n_ranks_total || jobs[j].rank_off > n_ranks_total - jobs[j].n_kmers) return NPH_ERR_INVALID;
-    }
+    for (size_t j = 0; j < n_jobs; ++j)
+        if (!nph_abea_job_ok(jobs[j], n_reads, n_ranks_total)) return NPH_ERR_INVALID;
+    ctx->abea_loaded = false;         // the ABEA job, rank and transition buffers are overwritten below
     NPH_TRY(nph_reserve(ctx, ctx->d_abea_jobs, n_jobs));
     NPH_TRY(nph_reserve(ctx, ctx->d_abea_ranks, n_ranks_total));
     NPH_TRY(nph_reserve(ctx, ctx->d_abea_consts, 2 * n_jobs));
     NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_abea_jobs.p, jobs, sizeof(nph_abea_job) * n_jobs, cudaMemcpyHostToDevice, ctx->stream));
     NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_abea_ranks.p, kmer_ranks, sizeof(uint32_t) * n_ranks_total, cudaMemcpyHostToDevice, ctx->stream));
-    MomParams p{};
-    p.ev_mean = ctx->d_ev_mean.p; p.reads = ctx->d_reads.p; p.models = ctx->d_models.p; p.model_id = model_id;
-    p.ranks = ctx->d_abea_ranks.p; p.jobs = ctx->d_abea_jobs.p; p.n_jobs = (uint32_t)n_jobs; p.out = ctx->d_abea_consts.p;
-    int grid = (int)std::min<size_t>((n_jobs + kWarps - 1) / kWarps, (size_t)ctx->sm_count * 4);
-    mom_kernel<<<grid, kThreads, 0, ctx->stream>>>(p);
-    NPH_CUDA(ctx, cudaGetLastError());
+    NPH_TRY(nph_check_ranks(ctx, ctx->d_abea_ranks.p, n_ranks_total, ctx->models[model_id].n_states));
+    NPH_TRY(nph_launch_mom(ctx, ctx->d_abea_jobs.p, ctx->d_abea_ranks.p, n_jobs, model_id, ctx->d_abea_consts.p, false));
     NPH_CUDA(ctx, cudaMemcpyAsync(shift_scale_out, ctx->d_abea_consts.p, sizeof(double) * 2 * n_jobs, cudaMemcpyDeviceToHost, ctx->stream));
     NPH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    ctx->abea_loaded = false;
     return NPH_OK;
 }
 

@@ -678,7 +678,8 @@ int nph_detect_events_device(nph_ctx* ctx, const float* d_raw, size_t n_samples_
     std::vector<uint32_t> n_samples(n_reads);
     for (size_t i = 0; i < n_reads; ++i) {
         const nph_raw_read& r = reads[i];
-        if (r.n_samples == 0 || r.sample_off + r.n_samples > n_samples_total || r.event_off + r.event_cap > events_total || r.event_cap == 0)
+        if (r.n_samples == 0 || r.event_cap == 0 || !nph_slice_ok(r.sample_off, r.n_samples, n_samples_total) ||
+            !nph_slice_ok(r.event_off, r.event_cap, events_total))
             return NPH_ERR_INVALID;
         if (r.n_samples > 0xFFFFFF00u) return NPH_ERR_UNSUPPORTED;      // position arithmetic is 32-bit with a 2*w2 halo
         n_samples[i] = r.n_samples;
@@ -776,11 +777,10 @@ extern "C" int nph_detect_events_batch(nph_ctx* ctx, const float* raw, size_t n_
     NPH_CUDA(ctx, cudaSetDevice(ctx->device));
     float* d_raw;
     uint8_t* scratch;
-    NPH_TRY(nph_carve(ctx, ctx->d_abea_scratch, [&](NphArena& a) {
+    NPH_TRY(nph_carve_align_scratch(ctx, [&](NphArena& a) {
         d_raw = a.take<float>(n_samples_total);
         scratch = a.take<uint8_t>(nph_ed_scratch_bytes(n_reads, events_total));
     }));
-    ctx->abea_loaded = false;     // the arena is shared with the ABEA trace
     NPH_CUDA(ctx, cudaMemcpyAsync(d_raw, raw, sizeof(float) * n_samples_total, cudaMemcpyHostToDevice, ctx->stream));
     NPH_CUDA(ctx, cudaEventRecord(ctx->ev0, ctx->stream));
     nph_event* d_events = nullptr;

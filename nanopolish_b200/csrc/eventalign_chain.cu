@@ -266,7 +266,7 @@ extern "C" int nph_eventalign_chain(nph_ctx* ctx,
     nph_aligned_pair* d_pairs; int32_t* d_map; uint32_t* d_rf; uint32_t* d_rr; nph_ea_chain* d_chains; uint32_t* d_order;
     nph_ea_record* d_rec; nph_ea_result* d_res;
     ChainParams p{};
-    NPH_TRY(nph_carve(ctx, ctx->d_abea_scratch, [&](NphArena& a) {      // shares the alignment scratch arena with ABEA / K3
+    NPH_TRY(nph_carve_align_scratch(ctx, [&](NphArena& a) {
         d_pairs = a.take<nph_aligned_pair>(n_pairs_total);
         d_map = a.take<int32_t>(n_map_total);
         d_rf = a.take<uint32_t>(n_ranks_total);
@@ -279,7 +279,6 @@ extern "C" int nph_eventalign_chain(nph_ctx* ctx,
         p.scratch_trace = a.take<uint16_t>(trace_stride * warps);
         p.scratch_states = a.take<nph_align_state>((size_t)states_stride * warps);
     }));
-    ctx->abea_loaded = false;
     p.trace_stride = trace_stride; p.states_stride = states_stride; p.e_cap = e_cap;
     p.level = ctx->d_level.p; p.reads = ctx->d_reads.p; p.trans = ctx->d_trans.p; p.models = ctx->d_models.p; p.flank = ctx->d_flank.p;
     p.pairs = d_pairs; p.map_start = d_map; p.ranks_fwd = d_rf; p.ranks_rc = d_rr; p.chains = d_chains; p.order = d_order;

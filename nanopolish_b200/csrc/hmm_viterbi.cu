@@ -190,7 +190,7 @@ extern "C" int nph_hmm_align(nph_ctx* ctx,
     VitParams p{};
     uint64_t* d_off = nullptr;
     uint32_t* d_order = nullptr;
-    NPH_TRY(nph_carve(ctx, ctx->d_abea_scratch, [&](NphArena& a) {      // shares the alignment scratch arena with ABEA
+    NPH_TRY(nph_carve_align_scratch(ctx, [&](NphArena& a) {
         p.scratch_params = a.take<float4>((size_t)max_kpad * warps);
         p.scratch_edge = a.take<float>(3 * ((size_t)max_period + 8) * warps);
         p.scratch_trace = a.take<uint16_t>(trace_stride * warps);
@@ -231,6 +231,5 @@ extern "C" int nph_hmm_align(nph_ctx* ctx,
     NPH_CUDA(ctx, cudaMemcpyAsync(n_states_out, p.n_states, sizeof(uint32_t) * n_jobs, cudaMemcpyDeviceToHost, ctx->stream));
     if (scores_out) NPH_CUDA(ctx, cudaMemcpyAsync(scores_out, ctx->d_scores.p, sizeof(float) * n_jobs, cudaMemcpyDeviceToHost, ctx->stream));
     NPH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    ctx->abea_loaded = false;   // the arena was reused
     return NPH_OK;
 }

@@ -11,9 +11,6 @@
 // per-read transition log-probabilities).
 #include "nph_internal.cuh"
 
-#include <cmath>
-#include <cstdio>
-#include <cstdlib>
 #include <vector>
 
 namespace {
@@ -103,31 +100,30 @@ extern "C" int nph_load_from_raw_batch(nph_ctx* ctx, const float* raw, size_t n_
     if (!raw || !kmer_ranks || !jobs || !event_off_out || !ev_mean_out || !ev_stdv_out || !ev_start_time_out || !ev_duration_out || !calibrations_out)
         return NPH_ERR_INVALID;
     if (model_id >= ctx->models.size()) return NPH_ERR_INVALID;
-    const uint32_t n_states = ctx->models[model_id].n_states;
     for (size_t j = 0; j < n_jobs; ++j) {
         const nph_raw_job& jb = jobs[j];
-        if (jb.sample_off + jb.n_samples > n_samples_total || jb.n_kmers == 0 || jb.rank_off + jb.n_kmers > n_ranks_total || !(jb.sample_rate > 0.0))
+        if (!nph_slice_ok(jb.sample_off, jb.n_samples, n_samples_total) || !nph_kmers_ok(jb.rank_off, jb.n_kmers, n_ranks_total) || !(jb.sample_rate > 0.0))
             return NPH_ERR_INVALID;
     }
-    uint32_t max_rank = 0;
-    for (size_t i = 0; i < n_ranks_total; ++i) max_rank = std::max(max_rank, kmer_ranks[i]);     // branch-free: vectorises
-    if (max_rank >= n_states) return NPH_ERR_INVALID;
     NPH_CUDA(ctx, cudaSetDevice(ctx->device));
-    ctx->reads_loaded = false; ctx->jobs_loaded = false; ctx->abea_loaded = false;    // resident batches are replaced
 
-    // ---- 1. raw samples up once; trim (defaults hard-coded at the reference's call site) ----
+    // ---- 1. raw samples and ranks up once, ranks checked; trim (defaults hard-coded at the reference's call site) ----
     std::vector<nph_raw_read> rr(n_jobs);
     size_t cap_total = 0;
     for (size_t j = 0; j < n_jobs; ++j) { rr[j] = nph_raw_read{jobs[j].sample_off, 0, jobs[j].n_samples, 0}; cap_total += jobs[j].n_samples / 2 + 8; }
     // raw samples | the trim's scratch, later the detector's (its events are read after it returns) | small per-read arrays
     float* d_raw; uint8_t* arena; uint64_t* d_cap_off; uint64_t* d_out_off; double* d_rate;
-    NPH_TRY(nph_carve(ctx, ctx->d_abea_scratch, [&](NphArena& a) {
+    NPH_TRY(nph_carve_align_scratch(ctx, [&](NphArena& a) {
         d_raw = a.take<float>(n_samples_total);
         arena = a.take<uint8_t>(std::max(nph_trim_scratch_bytes(rr.data(), n_jobs, 100), nph_ed_scratch_bytes(n_jobs, cap_total)));
         d_cap_off = a.take<uint64_t>(n_jobs);
         d_out_off = a.take<uint64_t>(n_jobs);
         d_rate = a.take<double>(n_jobs);
     }));
+    NPH_TRY(nph_reserve(ctx, ctx->d_abea_ranks, n_ranks_total));       // where MoM, ABEA and the calibration read them
+    NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_abea_ranks.p, kmer_ranks, sizeof(uint32_t) * n_ranks_total, cudaMemcpyHostToDevice, ctx->stream));
+    NPH_TRY(nph_check_ranks(ctx, ctx->d_abea_ranks.p, n_ranks_total, ctx->models[model_id].n_states));
+    ctx->reads_loaded = false; ctx->jobs_loaded = false;    // the resident reads are replaced
     NPH_CUDA(ctx, cudaMemcpyAsync(d_raw, raw, sizeof(float) * n_samples_total, cudaMemcpyHostToDevice, ctx->stream));
     NPH_CUDA(ctx, cudaEventRecord(ctx->ev0, ctx->stream));
     int launches = 0;
@@ -136,8 +132,6 @@ extern "C" int nph_load_from_raw_batch(nph_ctx* ctx, const float* raw, size_t n_
     NPH_TRY(nph_trim_device(ctx, d_raw, n_samples_total, rr.data(), n_jobs, 200, 10, 100, 0.0f, arena, range.data())); ++launches;
     ctx->h_last_trim = range;                   // for nph_last_trim_ranges (SRF_LOAD_RAW_SAMPLES keeps rt.raw[rt.start .. rt.end))
     NPH_CUDA(ctx, cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1)); staged_ms += ms;
-    const bool verbose = getenv("NPH_TIMING") != nullptr;
-    if (verbose) fprintf(stderr, "[nph] load_from_raw: trim %.2f ms", ms);
 
     // outputs of the reads that do not get as far as alignment
     for (size_t j = 0; j < n_jobs; ++j) {
@@ -174,7 +168,6 @@ extern "C" int nph_load_from_raw_batch(nph_ctx* ctx, const float* raw, size_t n_
     NPH_TRY(nph_detect_events_device(ctx, d_raw, n_samples_total, tr.data(), nl, params, arena, room, &d_events, &d_counts, counts, &ed_launches));
     launches += ed_launches;
     NPH_CUDA(ctx, cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1)); staged_ms += ms;
-    if (verbose) fprintf(stderr, "  events %.2f ms", ms);
 
     // ---- 3. compact layout, SquiggleEvent conversion, outputs of the event arrays ----
     std::vector<uint64_t> out_off(nl + 1, 0);
@@ -190,15 +183,13 @@ extern "C" int nph_load_from_raw_batch(nph_ctx* ctx, const float* raw, size_t n_
         event_off_out[n_jobs] = acc;
     }
     if (n_events_total > events_cap) { ctx->last_error = "nph_load_from_raw_batch: events_cap too small (n_samples_total / 3 always suffices)"; return NPH_ERR_UNSUPPORTED; }
-    uint64_t n_live_ranks = 0, pairs_total = 0;
+    uint64_t pairs_total = 0;
     std::vector<nph_abea_job> aj(nl);
     for (size_t t = 0; t < nl; ++t) {
         const nph_raw_job& jb = jobs[live[t]];
         aj[t] = nph_abea_job{jb.rank_off, pairs_total, (uint32_t)t, jb.n_kmers, counts[t] + jb.n_kmers, 0};
         pairs_total += aj[t].pairs_cap;
-        n_live_ranks += jb.n_kmers;
     }
-    (void)n_live_ranks;
     NPH_TRY(nph_reserve(ctx, ctx->d_ev_mean, n_events_total));
     NPH_TRY(nph_reserve(ctx, ctx->d_ev_time, n_events_total));
     NPH_TRY(nph_reserve(ctx, ctx->d_level, n_events_total));
@@ -233,25 +224,15 @@ extern "C" int nph_load_from_raw_batch(nph_ctx* ctx, const float* raw, size_t n_
         NPH_CUDA(ctx, cudaMemcpyAsync(ev_duration_out, d_dur, sizeof(float) * n_events_total, cudaMemcpyDeviceToHost, ctx->stream));
         NPH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
         NPH_CUDA(ctx, cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1)); staged_ms += ms;
-        if (verbose) fprintf(stderr, "  convert %.2f ms", ms);
     }
 
-    // ---- 4. MoM scalings and event alignment (the arena becomes ABEA's band storage) ----
-    ctx->n_reads = nl;
-    ctx->n_events_total = n_events_total;
-    ctx->h_read_n_events.assign(counts.begin(), counts.end());
-    nph_reads_resident(ctx);                       // for the staged ABEA calls below; cleared again before returning
-    int rc = nph_abea_jobs_load(ctx, kmer_ranks, n_ranks_total, aj.data(), nl, model_id, pairs_total);
-    if (rc == NPH_OK) rc = nph_launch_mom(ctx, d_mom, params->reverse_events != 0);
-    if (rc == NPH_OK) {
-        apply_mom_kernel<<<(unsigned)((nl + 127) / 128), 128, 0, ctx->stream>>>(d_mom, ctx->d_reads.p, d_views, (uint32_t)nl);
-        launches += 2;
-        if (cudaGetLastError() != cudaSuccess) rc = NPH_ERR_CUDA;
-    }
-    if (rc == NPH_OK) { rc = nph_launch_abea(ctx); ++launches; }
-    ctx->reads_loaded = false;
-    ctx->abea_loaded = false;
-    if (rc != NPH_OK) return rc;
+    // ---- 4. MoM scalings and event alignment (the arena becomes ABEA's band storage; no ABEA batch is left staged) ----
+    NPH_TRY(nph_abea_stage(ctx, counts.data(), aj.data(), nl, n_ranks_total, model_id, pairs_total));
+    NPH_TRY(nph_launch_mom(ctx, ctx->d_abea_jobs.p, ctx->d_abea_ranks.p, nl, model_id, d_mom, params->reverse_events != 0));
+    apply_mom_kernel<<<(unsigned)((nl + 127) / 128), 128, 0, ctx->stream>>>(d_mom, ctx->d_reads.p, d_views, (uint32_t)nl);
+    NPH_CUDA(ctx, cudaGetLastError());
+    NPH_TRY(nph_launch_abea(ctx));
+    launches += 3;
 
     // ---- 5. base_to_event_map, events_per_base, recalibration, QC ----
     NPH_CUDA(ctx, cudaMemsetAsync(d_b2e, 0xff, sizeof(nph_event_range) * n_ranks_total, ctx->stream));
@@ -268,7 +249,6 @@ extern "C" int nph_load_from_raw_batch(nph_ctx* ctx, const float* raw, size_t n_
     NPH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     for (size_t t = 0; t < nl; ++t) calibrations_out[live[t]] = cal[t];
     NPH_CUDA(ctx, cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1)); staged_ms += ms;     // ev0 was recorded at the ABEA launch
-    if (verbose) fprintf(stderr, "  abea+calibration %.2f ms  (total %.2f ms, %zu of %zu reads aligned)\n", ms, staged_ms, nl, n_jobs);
     nph_timing_staged(ctx, staged_ms, launches);
     return NPH_OK;
 }

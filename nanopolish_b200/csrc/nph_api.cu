@@ -4,10 +4,7 @@
 #include "exact_math.cuh"
 #include <algorithm>
 #include <cmath>
-#include <cstdio>
 #include <cstring>
-#include <chrono>
-#include <cstdlib>
 #include <new>
 
 int nph_set_cuda_error(nph_ctx* ctx, cudaError_t e, const char* what)
@@ -420,23 +417,16 @@ static int hmm_score_batch_impl(nph_ctx* ctx,
                                 const nph_hmm_job* jobs, size_t n_jobs,
                                 double indel_bias, float* scores_out)
 {
-    static const bool timing = getenv("NPH_TIMING") != nullptr;   // development aid: per-phase host wall time on stderr
-    auto now = [] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
-    const double t0 = now();
     if (!ctx) return NPH_ERR_INVALID;
     if (n_jobs == 0) return NPH_OK;                              // empty batch
     // the scheduler needs only the read records, jobs and ranks; the forward kernels start as soon as the schedule exists and
     // wait per job on the progress word of the level chunk that holds their read (hmm_forward_kernel.cuh)
     int rc = nph_oneshot_begin(ctx, reads, n_reads, ev_mean, ev_start_time, n_events_total,
                                [&] { return jobs_upload_async(ctx, kmer_ranks, seq_codes, n_ranks_total, jobs, n_jobs, indel_bias); });
-    const double t1 = now();
     if (rc == NPH_OK) rc = nph_jobs_schedule(ctx, n_jobs, n_ranks_total, kmer_ranks ? NphJobSource::HostRanks : NphJobSource::HostCodes);
-    const double t2 = now();
     if (rc == NPH_OK) rc = nph_hmm_score(ctx, nullptr);
     if (rc == NPH_OK) rc = nph_hmm_scores_fetch(ctx, scores_out, n_jobs);
     nph_oneshot_finish(ctx);                                     // also on error paths: never leave copies in flight
-    const double t3 = now();
-    if (timing) fprintf(stderr, "[nph] reads+jobs %.2f ms  schedule %.2f ms  score+fetch %.2f ms\n", t1 - t0, t2 - t1, t3 - t2);
     return rc;
 }
 

@@ -13,7 +13,7 @@
 #define NPH_LOGSUM_TBL 16000        // ref: p7_LOGSUM_TBL, src/common/logsum.h:20
 #define NPH_LOGSUM_CUT 15700        // (max-min) >= 15.7f returns max: entries >= 15700 hold 0.0f
 #define NPH_TBL_SMEM   16385        // = NPH_LOGSUM_TBL_LEN: the saturated index of lsum_sat (exact_math.cuh) reaches 2^14
-#define NPH_NUM_COUNTERS 64          // work-queue counters: one per forward class (<= 40) + ABEA (last)
+#define NPH_NUM_COUNTERS 64          // work-queue counters: one per forward class (<= 40), nph_check_ranks' flag, ABEA (last)
 
 // Per-read record on the device (what the kernels need of nph_read after the prologue).
 struct DevRead {
@@ -127,7 +127,7 @@ struct nph_ctx {
     DevBuf<uint32_t> d_abea_ranks;
     DevBuf<nph_aligned_pair> d_pairs;
     DevBuf<nph_abea_result> d_abea_res;
-    DevBuf<uint8_t> d_abea_scratch;
+    DevBuf<uint8_t> d_align_scratch; // ABEA's band trace, and the scratch of every other alignment-prologue call (nph_carve_align_scratch)
     DevBuf<uint32_t> d_abea_order;
     DevBuf<double> d_abea_consts;    // per job (lp_stay, lp_step); also the MoM output buffer
     DevBuf<uint8_t> d_prep;          // load_from_raw: event SoA staging, MoM output, calibration buffers
@@ -250,6 +250,23 @@ int nph_carve(nph_ctx* ctx, DevBuf<uint8_t>& buf, Layout&& layout)
     layout(a);
     return NPH_OK;
 }
+// Carve the alignment scratch for a call other than ABEA: the staged ABEA batch keeps its band trace there, so it is dropped.
+template <typename Layout>
+int nph_carve_align_scratch(nph_ctx* ctx, Layout&& layout)
+{
+    ctx->abea_loaded = false;
+    return nph_carve(ctx, ctx->d_align_scratch, layout);
+}
+
+// off + len <= total, in a form that cannot wrap
+inline bool nph_slice_ok(uint64_t off, uint64_t len, uint64_t total) { return len <= total && off <= total - len; }
+// A job's k-mers: at least one, with ranks [rank_off, rank_off + n_kmers) inside the call's n_ranks
+inline bool nph_kmers_ok(uint64_t rank_off, uint32_t n_kmers, uint64_t n_ranks) { return n_kmers > 0 && nph_slice_ok(rank_off, n_kmers, n_ranks); }
+// An ABEA-shaped job (ABEA, MoM, calibration): its read is one of the call's n_reads, its k-mers are nph_kmers_ok and its
+// n_pairs pairs from pairs_off lie inside pairs_total (the defaults: a call without pairs).  The ranks themselves are checked
+// on the device by nph_check_ranks.
+inline bool nph_abea_job_ok(const nph_abea_job& jb, size_t n_reads, uint64_t n_ranks, uint64_t n_pairs = 0, uint64_t pairs_total = UINT64_MAX)
+{ return jb.read < n_reads && nph_kmers_ok(jb.rank_off, jb.n_kmers, n_ranks) && nph_slice_ok(jb.pairs_off, n_pairs, pairs_total); }
 
 // Indices 0 .. n-1 by key, largest first; equal keys keep index order.
 template <typename K>
@@ -368,4 +385,12 @@ struct NphCalArgs {
     int* bad_input;
 };
 int nph_launch_recalibrate(nph_ctx* ctx, const NphCalArgs& args);
-int nph_launch_mom(nph_ctx* ctx, double* d_shift_scale_out, bool reversed = false);     // over the loaded ABEA jobs: 2 doubles per job
+// estimate_scalings_using_mom of n_jobs jobs over the resident reads' event means: 2 doubles (shift, scale) per job
+int nph_launch_mom(nph_ctx* ctx, const nph_abea_job* d_jobs, const uint32_t* d_ranks, size_t n_jobs, uint32_t model_id, double* d_out, bool reversed);
+// Stages n_jobs checked ABEA jobs over reads on the device with n_events[read] events: transition terms, longest-first order,
+// band trace room, every ABEA buffer reserved (the caller fills ctx->d_abea_ranks), uploads.  Sets no residency flag and does
+// not synchronise.
+int nph_abea_stage(nph_ctx* ctx, const uint32_t* n_events, const nph_abea_job* jobs, size_t n_jobs, size_t n_ranks_total, uint32_t model_id,
+                   size_t pairs_total);
+// NPH_ERR_INVALID unless every rank of d_ranks[0, n) is below n_states: one kernel, one flag copied back (a stream sync).
+int nph_check_ranks(nph_ctx* ctx, const uint32_t* d_ranks, size_t n, uint32_t n_states);

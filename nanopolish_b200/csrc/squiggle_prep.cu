@@ -390,7 +390,7 @@ int nph_trim_device(nph_ctx* ctx, const float* d_raw, size_t n_samples_total, co
     std::vector<uint64_t> mad_off(n_reads);
     uint64_t n_chunks = 0;
     for (size_t i = 0; i < n_reads; ++i) {
-        if (reads[i].sample_off + reads[i].n_samples > n_samples_total) return NPH_ERR_INVALID;
+        if (!nph_slice_ok(reads[i].sample_off, reads[i].n_samples, n_samples_total)) return NPH_ERR_INVALID;
         mad_off[i] = n_chunks;
         n_chunks += reads[i].n_samples / (uint32_t)varseg_chunk;
     }
@@ -434,11 +434,10 @@ extern "C" int nph_trim_raw_batch(nph_ctx* ctx, const float* raw, size_t n_sampl
     NPH_CUDA(ctx, cudaSetDevice(ctx->device));
     float* d_raw;
     uint8_t* scratch;
-    NPH_TRY(nph_carve(ctx, ctx->d_abea_scratch, [&](NphArena& a) {
+    NPH_TRY(nph_carve_align_scratch(ctx, [&](NphArena& a) {
         d_raw = a.take<float>(n_samples_total);
         scratch = a.take<uint8_t>(nph_trim_scratch_bytes(reads, n_reads, varseg_chunk));
     }));
-    ctx->abea_loaded = false;       // the arena is shared with the ABEA trace
     NPH_CUDA(ctx, cudaMemcpyAsync(d_raw, raw, sizeof(float) * n_samples_total, cudaMemcpyHostToDevice, ctx->stream));
     NPH_CUDA(ctx, cudaEventRecord(ctx->ev0, ctx->stream));
     NPH_TRY(nph_trim_device(ctx, d_raw, n_samples_total, reads, n_reads, trim_start, trim_end, varseg_chunk, varseg_thresh,
@@ -456,20 +455,15 @@ extern "C" int nph_recalibrate_batch(nph_ctx* ctx, const nph_read* reads, size_t
     if (n_jobs == 0) return NPH_OK;
     if (!reads || !ev_mean || !kmer_ranks || !jobs || !results || !calibrations_out || (!pairs && pairs_total)) return NPH_ERR_INVALID;
     if (model_id >= ctx->models.size()) return NPH_ERR_INVALID;
-    const uint32_t n_states = ctx->models[model_id].n_states;
     for (size_t i = 0; i < n_reads; ++i)
-        if (reads[i].event_off + reads[i].n_events > n_events_total) return NPH_ERR_INVALID;
-    for (size_t j = 0; j < n_jobs; ++j) {
-        const nph_abea_job& jb = jobs[j];
-        if (jb.read >= n_reads || jb.n_kmers == 0 || jb.rank_off + jb.n_kmers > n_ranks_total) return NPH_ERR_INVALID;
-        if (results[j].n_pairs > jb.pairs_cap || jb.pairs_off + results[j].n_pairs > pairs_total) return NPH_ERR_INVALID;
-    }
-    for (size_t i = 0; i < n_ranks_total; ++i)
-        if (kmer_ranks[i] >= n_states) return NPH_ERR_INVALID;
+        if (!nph_slice_ok(reads[i].event_off, reads[i].n_events, n_events_total)) return NPH_ERR_INVALID;
+    for (size_t j = 0; j < n_jobs; ++j)     // the pairs a job has are the n_pairs its result reports
+        if (results[j].n_pairs > jobs[j].pairs_cap || !nph_abea_job_ok(jobs[j], n_reads, n_ranks_total, results[j].n_pairs, pairs_total))
+            return NPH_ERR_INVALID;
     NPH_CUDA(ctx, cudaSetDevice(ctx->device));
     NphCalArgs a{};
     float* d_ev; nph_read* d_reads; uint32_t* d_rk; nph_abea_job* d_jobs; nph_abea_result* d_res; nph_aligned_pair* d_pairs;
-    NPH_TRY(nph_carve(ctx, ctx->d_abea_scratch, [&](NphArena& ar) {
+    NPH_TRY(nph_carve_align_scratch(ctx, [&](NphArena& ar) {
         d_ev = ar.take<float>(n_events_total);
         d_reads = ar.take<nph_read>(n_reads);
         d_rk = ar.take<uint32_t>(n_ranks_total);
@@ -480,7 +474,6 @@ extern "C" int nph_recalibrate_batch(nph_ctx* ctx, const nph_read* reads, size_t
         a.out = ar.take<nph_calibration>(n_jobs);
         a.bad_input = ar.take<int>(1);
     }));
-    ctx->abea_loaded = false;
     a.ev_mean = d_ev; a.reads = d_reads; a.model_id = model_id; a.ranks = d_rk; a.jobs = d_jobs;
     a.results = d_res; a.pairs = d_pairs; a.n_jobs = (uint32_t)n_jobs;
     NPH_CUDA(ctx, cudaMemcpyAsync(d_ev, ev_mean, sizeof(float) * n_events_total, cudaMemcpyHostToDevice, ctx->stream));
@@ -489,6 +482,7 @@ extern "C" int nph_recalibrate_batch(nph_ctx* ctx, const nph_read* reads, size_t
     NPH_CUDA(ctx, cudaMemcpyAsync(d_jobs, jobs, sizeof(nph_abea_job) * n_jobs, cudaMemcpyHostToDevice, ctx->stream));
     NPH_CUDA(ctx, cudaMemcpyAsync(d_res, results, sizeof(nph_abea_result) * n_jobs, cudaMemcpyHostToDevice, ctx->stream));
     if (pairs_total) NPH_CUDA(ctx, cudaMemcpyAsync(d_pairs, pairs, sizeof(nph_aligned_pair) * pairs_total, cudaMemcpyHostToDevice, ctx->stream));
+    NPH_TRY(nph_check_ranks(ctx, d_rk, n_ranks_total, ctx->models[model_id].n_states));
     NPH_CUDA(ctx, cudaEventRecord(ctx->ev0, ctx->stream));
     NPH_TRY(nph_launch_recalibrate(ctx, a));
     NPH_CUDA(ctx, cudaEventRecord(ctx->ev1, ctx->stream));

@@ -10,6 +10,7 @@ from nanopolish_b200.engine import Engine
 
 pytestmark = pytest.mark.gpu
 K = 6
+NPH_ERR_INVALID = -3        # include/nph.h: bad argument
 NPH_ERR_STATE = -5          # include/nph.h: call sequence error
 
 
@@ -76,7 +77,7 @@ def _raw_batch(model, seed):
     return raw, np.concatenate(ranks).astype(np.uint32), jobs
 
 
-def _between(ctx, rs, which):
+def _between(ctx, rs, which, abea_out):
     if which == "hmm_align":
         jobs = synth.scorereads_jobs(rs, 300)
         ctx.hmm_align(jobs.kmer_ranks, jobs.jobs)
@@ -91,9 +92,19 @@ def _between(ctx, rs, which):
     elif which == "load_from_raw_batch":
         raw, ranks, jobs = _raw_batch(synth.load_model("nucleotide"), 21)
         ctx.load_from_raw_batch(raw, ranks, jobs, 0, synth.event_params(False))
+    elif which == "trim_raw_batch":
+        raw, rr = synth.gen_raw(2, 12000, synth.load_model("nucleotide"), seed=21)
+        ctx.trim_raw_batch(raw, rr)
+    elif which == "detect_events_batch":
+        raw, rr = synth.gen_raw(2, 12000, synth.load_model("nucleotide"), seed=21)
+        ctx.detect_events_batch(raw, rr, synth.event_params(False))
+    elif which == "recalibrate_batch":
+        jobs, ranks, _ = synth.abea_jobs(rs)
+        ctx.recalibrate_batch(rs.reads, rs.ev_mean, ranks, jobs, 0, *abea_out)
 
 
-@pytest.mark.parametrize("which", [None, "hmm_align", "eventalign_chain", "mom_batch", "reads_load", "load_from_raw_batch"])
+@pytest.mark.parametrize("which", [None, "hmm_align", "eventalign_chain", "mom_batch", "reads_load", "load_from_raw_batch",
+                                   "trim_raw_batch", "detect_events_batch", "recalibrate_batch"])
 def test_staged_abea_is_dropped_by_calls_that_reuse_its_buffers(ctx, which):
     rs = _reads(3, 1500, seed=8)
     jobs, ranks, total = synth.abea_jobs(rs)
@@ -106,9 +117,61 @@ def test_staged_abea_is_dropped_by_calls_that_reuse_its_buffers(ctx, which):
         assert pairs.tobytes() == want_pairs.tobytes() and res.tobytes() == want_res.tobytes()
         assert (res["n_pairs"] > 0).all()
         return
-    _between(ctx, rs, which)
+    _between(ctx, rs, which, (want_pairs, want_res))
     assert _status(ctx.abea_run) == NPH_ERR_STATE
     assert _status(ctx.abea_fetch) == NPH_ERR_STATE
+
+
+def _prologue_outputs(e, rs, abea, raw_batch):
+    """every output of the ABEA-shaped calls on one good batch: one-shot and staged ABEA, MoM, calibration, load_from_raw"""
+    jobs, ranks, total = abea
+    pairs, res = e.abea_batch(rs.reads, rs.ev_mean, rs.ev_start_time, ranks, jobs, 0, total)
+    e.reads_load(rs.reads, rs.ev_mean, rs.ev_start_time)
+    e.abea_jobs_load(ranks, jobs, 0, total)
+    e.abea_run()
+    staged = e.abea_fetch()
+    mom = e.mom_batch(rs.reads, rs.ev_mean, ranks, jobs, 0)
+    b2e, cal = e.recalibrate_batch(rs.reads, rs.ev_mean, ranks, jobs, 0, pairs, res)
+    raw, raw_ranks, raw_jobs = raw_batch
+    return [pairs, res, *staged, mom, b2e, cal, *e.load_from_raw_batch(raw, raw_ranks, raw_jobs, 0, synth.event_params(False))]
+
+
+def test_bad_ranks_and_wrapping_offsets_are_refused(ctx):
+    """A rank outside the model (4096 of a 6-mer model's 4^6 states) and a job slice whose offset is 2^64 - 1 are refused
+    with NPH_ERR_INVALID by every ABEA-shaped call; afterwards the context computes a good batch exactly as a fresh one."""
+    rs = _reads(3, 1500, seed=8)
+    abea = jobs, ranks, total = synth.abea_jobs(rs)
+    raw_batch = raw, raw_ranks, raw_jobs = _raw_batch(synth.load_model("nucleotide"), 21)
+    fresh = _fresh()
+    try:
+        want = _prologue_outputs(fresh, rs, abea, raw_batch)
+    finally:
+        fresh.close()
+    pairs, res = want[0], want[1]
+    bad_ranks = ranks.copy()
+    bad_ranks[int(jobs[1]["rank_off"]) + 5] = 4096
+    wrapped = jobs.copy()
+    wrapped[1]["rank_off"] = 2**64 - 1
+    calls = [lambda r, j: ctx.abea_batch(rs.reads, rs.ev_mean, rs.ev_start_time, r, j, 0, total),
+             lambda r, j: (ctx.reads_load(rs.reads, rs.ev_mean, rs.ev_start_time), ctx.abea_jobs_load(r, j, 0, total)),
+             lambda r, j: ctx.mom_batch(rs.reads, rs.ev_mean, r, j, 0),
+             lambda r, j: ctx.recalibrate_batch(rs.reads, rs.ev_mean, r, j, 0, pairs, res)]
+    for call in calls:
+        assert _status(call, bad_ranks, jobs) == NPH_ERR_INVALID
+        assert _status(call, ranks, wrapped) == NPH_ERR_INVALID
+    bad_raw_ranks = raw_ranks.copy()
+    bad_raw_ranks[-1] = 4096
+    prm = synth.event_params(False)
+    assert _status(ctx.load_from_raw_batch, raw, bad_raw_ranks, raw_jobs, 0, prm) == NPH_ERR_INVALID
+    for field in ("sample_off", "rank_off"):
+        wrapped_raw = raw_jobs.copy()
+        wrapped_raw[0][field] = 2**64 - 1
+        assert _status(ctx.load_from_raw_batch, raw, raw_ranks, wrapped_raw, 0, prm) == NPH_ERR_INVALID
+    got = _prologue_outputs(ctx, rs, abea, raw_batch)
+    assert len(got) == len(want)
+    for g, w in zip(got, want):
+        assert g.tobytes() == w.tobytes()
+    assert (want[1]["n_pairs"] > 0).all() and (want[-1]["status"] == 0).any()
 
 
 def _meth_inputs(rs):
