@@ -8,12 +8,9 @@
 // discarded there, so the whole signal is segmented).
 //
 // The reference makes five passes over each read and mallocs five arrays (two FP64 prefix sums, two t-statistic
-// vectors, a peak list).  The prefix sums are strictly sequential FP64 accumulations, so the result is only
-// reproducible by walking each read in order; parallelism is across reads.  One thread streams one read in a single
-// pass: the running sums live in registers, a (2*w2+1)-deep ring of the last prefix values per thread lives in shared
-// memory (the two t-statistics at position i only need sums at i-w..i+w), the short/long peak detector is a register
-// state machine, and each boundary emits its event from the sums captured when the peak was set.  HBM traffic is the
-// algorithmic minimum: 4 B per sample in, 24 B per event out.  Every float/double operation mirrors the C source's
+// vectors, a peak list).  Here reads whose prefix sums are provably exact take the fast path (ed_fused_kernel, then
+// ed_events_kernel) and the others the streaming fallback (detect_events_stream_kernel).  Both step the same peak detector
+// (peak_step) and build events with the same arithmetic (event_of).  Every float/double operation mirrors the C source's
 // promotions (float products, double quotient, double sqrt) so boundaries, means and stdvs are bit-identical.
 #include "nph_internal.cuh"
 #include "exact_math.cuh"
@@ -27,174 +24,14 @@ namespace {
 constexpr int kThreads = 128;
 constexpr int kMaxW2 = 16;
 
-struct DetParams {
+// The parameters of all three kernels, filled once by the host.  The fused kernel's fields come first, in the order that
+// fixes its constant-bank offsets; `ring` fills the alignment hole after n_reads.
+struct EdParams {
     const float* raw;
     const nph_raw_read* reads;
-    const uint32_t* order;
+    const uint32_t* order;       // reads sorted by length (desc); the fallback's reads in the streaming kernel
     uint32_t n_reads;
-    nph_event* events;
-    uint32_t* n_events;
-    int* overflow;
-    uint32_t w1, w2;
-    float t1, t2, peak_height;
-    uint32_t ring;         // 2*w2 + 1
-};
-
-struct Detector {
-    float threshold;
-    unsigned long long window_length;
-    unsigned long long masked_to;
-    long long peak_pos;
-    float peak_value;
-    bool valid_peak;
-    double s_at_peak, q_at_peak;      // prefix sums at peak_pos, captured when the peak is set
-};
-
-// t-statistic at position i from prefix values (compute_tstat's loop body, same promotions)
-__device__ __forceinline__ float tstat_at(double s_lo, double q_lo, double s_mid, double q_mid, double s_hi, double q_hi, float wf)
-{
-    const double sum1 = __dsub_rn(s_mid, s_lo);
-    const double sumsq1 = __dsub_rn(q_mid, q_lo);
-    const float sum2 = (float)__dsub_rn(s_hi, s_mid);
-    const float sumsq2 = (float)__dsub_rn(q_hi, q_mid);
-    const float mean1 = (float)__ddiv_rn(sum1, (double)wf);
-    const float mean2 = __fdiv_rn(sum2, wf);
-    double cv = __dsub_rn(__ddiv_rn(sumsq1, (double)wf), (double)__fmul_rn(mean1, mean1));
-    cv = __dadd_rn(cv, (double)__fdiv_rn(sumsq2, wf));
-    cv = __dsub_rn(cv, (double)__fmul_rn(mean2, mean2));
-    float combined_var = fmaxf((float)cv, FLT_MIN);
-    const float delta_mean = __fsub_rn(mean2, mean1);
-    return (float)__ddiv_rn(fabs((double)delta_mean), __dsqrt_rn((double)__fdiv_rn(combined_var, wf)));
-}
-
-__device__ __forceinline__ void emit_event(nph_event* out, uint32_t& count, uint32_t cap, unsigned long long start, unsigned long long end,
-                                           double s0, double q0, double s1, double q1)
-{
-    if (count < cap) {
-        nph_event e;
-        e.start = start;
-        e.length = (float)(end - start);                             // size_t difference, as in create_event
-        e.mean = __fdiv_rn((float)__dsub_rn(s1, s0), e.length);
-        const float deltasqr = (float)__dsub_rn(q1, q0);
-        const float var = __fsub_rn(__fdiv_rn(deltasqr, e.length), __fmul_rn(e.mean, e.mean));
-        e.stdv = __fsqrt_rn(fmaxf(var, 0.0f));
-        e.reserved = 0;
-        out[count] = e;
-    }
-    ++count;
-}
-
-// Fallback for reads whose prefix sums are not provably exact (the guard of ed_fused_kernel): one thread streams one read.
-__global__ void __launch_bounds__(kThreads) detect_events_stream_kernel(const DetParams p)
-{
-    extern __shared__ double s_ring[];                                // [2][ring][kThreads]: S then Q
-    const uint32_t slot_idx = blockIdx.x * kThreads + threadIdx.x;
-    if (slot_idx >= p.n_reads) return;
-    const uint32_t ridx = p.order[slot_idx];
-    const nph_raw_read rd = p.reads[ridx];
-    const float* __restrict__ raw = p.raw + rd.sample_off;
-    const unsigned long long n = rd.n_samples;
-    nph_event* out = p.events + rd.event_off;
-    const uint32_t R = p.ring;
-    double* ringS = s_ring + threadIdx.x;
-    double* ringQ = s_ring + (size_t)R * kThreads + threadIdx.x;
-#define RS(slot) ringS[(size_t)(slot) * kThreads]
-#define RQ(slot) ringQ[(size_t)(slot) * kThreads]
-
-    const uint32_t w1 = p.w1, w2 = p.w2;
-    const float wf1 = (float)w1, wf2 = (float)w2;
-    const bool on1 = !(n < 2ull * w1 || w1 < 2), on2 = !(n < 2ull * w2 || w2 < 2);
-    Detector d0{p.t1, w1, 0ull, -1, FLT_MAX, false, 0.0, 0.0};
-    Detector d1{p.t2, w2, 0ull, -1, FLT_MAX, false, 0.0, 0.0};
-
-    double S = 0.0, Q = 0.0;
-    unsigned long long consumed = 0;          // prefix index available: S == prefix[consumed]
-    RS(0) = 0.0; RQ(0) = 0.0;                 // prefix[0]
-    uint32_t slot_w = 0;                      // ring slot of prefix[consumed]
-    // ring slots of prefix[i - w2], [i - w1], [i], [i + w1], [i + w2]; negative indices are never read
-    int sl_m2 = -(int)w2, sl_m1 = -(int)w1, sl_0 = 0, sl_p1 = (int)w1, sl_p2 = (int)w2;
-    sl_p1 %= (int)R; sl_p2 %= (int)R;
-
-    uint32_t count = 0;
-    unsigned long long prev_pos = 0;
-    double prev_s = 0.0, prev_q = 0.0;
-
-    for (unsigned long long i = 0; i < n; ++i) {
-        // make prefix[min(n, i + w2)] available
-        const unsigned long long need = (i + w2 < n) ? i + w2 : n;
-        while (consumed < need) {
-            const float x = raw[consumed];
-            S = __dadd_rn(S, (double)x);
-            Q = __dadd_rn(Q, (double)__fmul_rn(x, x));
-            ++consumed;
-            slot_w = (slot_w + 1 == R) ? 0 : slot_w + 1;
-            RS(slot_w) = S; RQ(slot_w) = Q;
-        }
-        const double s_mid = RS(sl_0), q_mid = RQ(sl_0);
-        float ts1 = 0.0f, ts2 = 0.0f;
-        if (on1 && i >= w1 && i <= n - w1) ts1 = tstat_at(RS(sl_m1), RQ(sl_m1), s_mid, q_mid, RS(sl_p1), RQ(sl_p1), wf1);
-        if (on2 && i >= w2 && i <= n - w2) ts2 = tstat_at(RS(sl_m2), RQ(sl_m2), s_mid, q_mid, RS(sl_p2), RQ(sl_p2), wf2);
-
-        // short_long_peak_detector, iteration i: short detector first, then long
-#pragma unroll
-        for (int k = 0; k < 2; ++k) {
-            Detector& d = k == 0 ? d0 : d1;
-            if (d.masked_to >= i) continue;
-            const float cur = k == 0 ? ts1 : ts2;
-            if (d.peak_pos == -1) {
-                if (cur < d.peak_value) {
-                    d.peak_value = cur;
-                } else if (__fsub_rn(cur, d.peak_value) > p.peak_height) {
-                    d.peak_value = cur; d.peak_pos = (long long)i; d.s_at_peak = s_mid; d.q_at_peak = q_mid;
-                }
-            } else {
-                if (cur > d.peak_value) { d.peak_value = cur; d.peak_pos = (long long)i; d.s_at_peak = s_mid; d.q_at_peak = q_mid; }
-                if (k == 0 && d.peak_value > d.threshold) {
-                    d1.masked_to = (unsigned long long)d.peak_pos + d.window_length;
-                    d1.peak_pos = -1; d1.peak_value = FLT_MAX; d1.valid_peak = false;
-                }
-                if (__fsub_rn(d.peak_value, cur) > p.peak_height && d.peak_value > d.threshold) d.valid_peak = true;
-                if (d.valid_peak && (i - (unsigned long long)d.peak_pos) > d.window_length / 2) {
-                    const unsigned long long pk = (unsigned long long)d.peak_pos;
-                    emit_event(out, count, rd.event_cap, prev_pos, pk, prev_s, prev_q, d.s_at_peak, d.q_at_peak);
-                    prev_pos = pk; prev_s = d.s_at_peak; prev_q = d.q_at_peak;
-                    d.peak_pos = -1; d.peak_value = cur; d.valid_peak = false;
-                }
-            }
-        }
-        // advance the five ring cursors
-        sl_m2 = (sl_m2 + 1 == (int)R) ? 0 : sl_m2 + 1;
-        sl_m1 = (sl_m1 + 1 == (int)R) ? 0 : sl_m1 + 1;
-        sl_0 = (sl_0 + 1 == (int)R) ? 0 : sl_0 + 1;
-        sl_p1 = (sl_p1 + 1 == (int)R) ? 0 : sl_p1 + 1;
-        sl_p2 = (sl_p2 + 1 == (int)R) ? 0 : sl_p2 + 1;
-    }
-    // last event: previous boundary to the end of the signal (a signal without peaks is one event)
-    emit_event(out, count, rd.event_cap, prev_pos, n, prev_s, prev_q, S, Q);
-    if (count > rd.event_cap) { *p.overflow = 1; p.n_events[ridx] = 0; }
-    else p.n_events[ridx] = count;
-#undef RS
-#undef RQ
-}
-
-
-// =============================================================================================================
-// Fast path.  The reference accumulates FP64 prefix sums of the samples (and of their float squares) sequentially,
-// which no parallel algorithm reproduces in general.  But when every partial sum is EXACTLY representable nothing
-// is ever rounded, so any summation order gives the same doubles, and every quantity the detector derives from
-// the prefix arrays (window sums of the t-statistics, segment sums of the events) equals the exact sum of the
-// samples involved.  The guard proves that per read: all samples are integer multiples of 2^L (L = smallest ulp
-// exponent present) and |partial sum| <= n * max|x| < 2^(ceil(log2 n) + Emax + 1); if that span fits 53 bits (and
-// likewise for the float squares) the read takes the parallel path, otherwise the streaming fallback above.
-// Real traces (40-200 pA) pass with ~10 bits to spare.
-//   ed_fused_kernel : guard + both t-statistics + the short/long peak detector in ONE pass over the samples
-//   ed_events_kernel: thread per event, exact FP64 segment sums -> start / length / mean / stdv
-// =============================================================================================================
-struct FastParams {
-    const float* raw;
-    const nph_raw_read* reads;
-    const uint32_t* order;       // reads sorted by length (desc)
-    uint32_t n_reads;
+    uint32_t ring;               // streaming kernel only: 2*w2 + 1 prefix values per thread
     uint32_t* peaks;             // per read at event_off, event_cap entries
     uint32_t* n_peaks;           // per read
     uint8_t* exact;              // per read: 1 = fast path
@@ -206,6 +43,38 @@ struct FastParams {
     float t1, t2, peak_height;
     uint32_t warm;
 };
+
+// create_event's arithmetic (event_detection.c:216-235) from the segment's sums, sums[end] - sums[start]
+__device__ __forceinline__ nph_event event_of(unsigned long long start, unsigned long long end, double ds, double dq)
+{
+    nph_event e;
+    e.start = start;
+    e.length = (float)(end - start);                             // size_t difference, as in create_event
+    e.mean = __fdiv_rn((float)ds, e.length);
+    const float var = __fsub_rn(__fdiv_rn((float)dq, e.length), __fmul_rn(e.mean, e.mean));
+    e.stdv = __fsqrt_rn(fmaxf(var, 0.0f));
+    e.reserved = 0;
+    return e;
+}
+
+// the last step of compute_tstat: |delta| / sqrt(v / w), double quotient and double sqrt narrowed to float
+__device__ __forceinline__ float tstat_quotient(float combined_var, float delta_mean, float wf)
+{
+    return (float)__ddiv_rn(fabs((double)delta_mean), __dsqrt_rn((double)__fdiv_rn(combined_var, wf)));
+}
+
+// =============================================================================================================
+// Fast path.  The reference accumulates FP64 prefix sums of the samples (and of their float squares) sequentially,
+// which no parallel algorithm reproduces in general.  But when every partial sum is EXACTLY representable nothing
+// is ever rounded, so any summation order gives the same doubles, and every quantity the detector derives from
+// the prefix arrays (window sums of the t-statistics, segment sums of the events) equals the exact sum of the
+// samples involved.  The guard proves that per read: all samples are integer multiples of 2^L (L = smallest ulp
+// exponent present) and |partial sum| <= n * max|x| < 2^(ceil(log2 n) + Emax + 1); if that span fits 53 bits (and
+// likewise for the float squares) the read takes the parallel path, otherwise the streaming fallback below.
+// Real traces (40-200 pA) pass with ~10 bits to spare.
+//   ed_fused_kernel : guard + both t-statistics + the short/long peak detector in ONE pass over the samples
+//   ed_events_kernel: thread per event, exact FP64 segment sums -> start / length / mean / stdv
+// =============================================================================================================
 
 // ---- peak detector -------------------------------------------------------------------------------------------
 // short_long_peak_detector (event_detection.c:122-201) is a sequential state machine over the two t-statistic
@@ -232,6 +101,8 @@ __device__ __forceinline__ bool same_state(const PeakState& a, const PeakState& 
 }
 
 struct PeakConsts { float thr0, thr1, ph; uint32_t w0, half0, half1; };
+
+__device__ __forceinline__ PeakConsts peak_consts(const EdParams& p) { return PeakConsts{p.t1, p.t2, p.peak_height, p.w1, p.w1 / 2, p.w2 / 2}; }
 
 // one step at position i; returns the boundaries emitted (0, 1 or 2) in e0 (short detector) / e1 (long detector)
 __device__ __forceinline__ void peak_step(PeakState& st, const PeakConsts& k, uint32_t i, float ts1, float ts2, int& e0, int& e1)
@@ -342,7 +213,7 @@ __device__ __forceinline__ TsCand tstat_windows(double sl, double ql, double sr,
 
 __device__ __noinline__ float tstat_windows_exact(float combined_var, float delta_mean, float wf)
 {
-    return (float)__ddiv_rn(fabs((double)delta_mean), __dsqrt_rn((double)__fdiv_rn(combined_var, wf)));
+    return tstat_quotient(combined_var, delta_mean, wf);
 }
 
 // A row of the tile: the 32 positions [p0 + w2, p0 + w2 + 32) of one lane's range.  The warp first stages the row and its
@@ -479,7 +350,7 @@ __device__ __forceinline__ void read_barrier(int id, int threads) { asm volatile
 // WPR warps walk one read as 32*WPR segments (a CTA of kPeakWarps warps holds kPeakWarps / WPR reads): small batches
 // and the tail of a large one get WPR times the parallelism for warm / segment more work.
 template <int W1, int W2, int WPR>
-__global__ void __launch_bounds__(kPeakWarps * 32, NPH_ED_CTAS) ed_fused_kernel(const FastParams p, const TsConsts tc)
+__global__ void __launch_bounds__(kPeakWarps * 32, NPH_ED_CTAS) ed_fused_kernel(const EdParams p, const TsConsts tc)
 {
     constexpr int LANES = 32 * WPR;
     __shared__ FusedSmem s_mem[kPeakWarps];
@@ -498,7 +369,7 @@ __global__ void __launch_bounds__(kPeakWarps * 32, NPH_ED_CTAS) ed_fused_kernel(
     const uint32_t R = cap_peaks / LANES;                                 // a lane's slice of the peak array
     const uint32_t gl = (uint32_t)part * 32u + (uint32_t)lane;             // lane within the read
     uint32_t* region = peaks + (size_t)gl * R;
-    const PeakConsts k{p.t1, p.t2, p.peak_height, p.w1, p.w1 / 2, p.w2 / 2};
+    const PeakConsts k = peak_consts(p);
 
     const uint32_t seg = ((n + LANES - 1) / LANES + 31) / 32 * 32;         // segment length, multiple of 32
     const uint32_t b0 = (unsigned long long)gl * seg < n ? gl * seg : n, b1 = min(n, b0 + seg);
@@ -601,10 +472,10 @@ __global__ void __launch_bounds__(kPeakWarps * 32, NPH_ED_CTAS) ed_fused_kernel(
 }
 
 template <int WPR>
-static void launch_fused(const FastParams& f, const TsConsts& tc, size_t n_reads, cudaStream_t stream)
+static void launch_fused(const EdParams& f, const TsConsts& tc, size_t n_reads, cudaStream_t stream)
 {
     const unsigned blocks = (unsigned)((n_reads + kPeakWarps / WPR - 1) / (kPeakWarps / WPR));
-    void (*kern)(const FastParams, const TsConsts) = ed_fused_kernel<0, 0, WPR>;
+    void (*kern)(const EdParams, const TsConsts) = ed_fused_kernel<0, 0, WPR>;
     if (f.w1 == 3 && f.w2 == 6) kern = ed_fused_kernel<3, 6, WPR>;
     else if (f.w1 == 7 && f.w2 == 14) kern = ed_fused_kernel<7, 14, WPR>;
     // five CTAs per SM need the large shared-memory carve-out (static shared memory alone does not ask for it)
@@ -613,7 +484,7 @@ static void launch_fused(const FastParams& f, const TsConsts& tc, size_t n_reads
 }
 
 // block per read, thread per event
-__global__ void __launch_bounds__(256) ed_events_kernel(const FastParams p)
+__global__ void __launch_bounds__(256) ed_events_kernel(const EdParams p)
 {
     for (uint32_t r = blockIdx.x; r < p.n_reads; r += gridDim.x) {
         if (!p.exact[r]) continue;
@@ -632,16 +503,111 @@ __global__ void __launch_bounds__(256) ed_events_kernel(const FastParams p)
             double s = 0.0, q = 0.0;
             for (unsigned long long j = lo; j < hi; ++j) { const float v = x[j]; s = __dadd_rn(s, (double)v); q = __dadd_rn(q, (double)__fmul_rn(v, v)); }
             if (end < start) { s = -s; q = -q; }
-            nph_event e;
-            e.start = start;
-            e.length = (float)(end - start);
-            e.mean = __fdiv_rn((float)s, e.length);
-            const float var = __fsub_rn(__fdiv_rn((float)q, e.length), __fmul_rn(e.mean, e.mean));
-            e.stdv = __fsqrt_rn(fmaxf(var, 0.0f));
-            e.reserved = 0;
-            out[ev] = e;
+            out[ev] = event_of(start, end, s, q);
         }
     }
+}
+
+// =============================================================================================================
+// Streaming fallback, for reads the guard refuses and for windows wider than kFusedMaxW2: one thread streams one read in
+// a single pass, the running FP64 prefix sums in registers and a (2*w2+1)-deep ring of the last prefix values in shared
+// memory (the t-statistics at position i only need sums at i-w..i+w).  Each event's sums are the difference of the
+// prefix sums at its two boundaries, as in the reference.
+// =============================================================================================================
+__device__ __forceinline__ void emit_event(nph_event* out, uint32_t& count, uint32_t cap, unsigned long long start, unsigned long long end,
+                                           double s0, double q0, double s1, double q1)
+{
+    if (count < cap) out[count] = event_of(start, end, __dsub_rn(s1, s0), __dsub_rn(q1, q0));
+    ++count;
+}
+
+// t-statistic at position i from prefix values (compute_tstat's loop body, same promotions)
+__device__ __forceinline__ float tstat_at(double s_lo, double q_lo, double s_mid, double q_mid, double s_hi, double q_hi, float wf)
+{
+    const double sum1 = __dsub_rn(s_mid, s_lo);
+    const double sumsq1 = __dsub_rn(q_mid, q_lo);
+    const float sum2 = (float)__dsub_rn(s_hi, s_mid);
+    const float sumsq2 = (float)__dsub_rn(q_hi, q_mid);
+    const float mean1 = (float)__ddiv_rn(sum1, (double)wf);
+    const float mean2 = __fdiv_rn(sum2, wf);
+    double cv = __dsub_rn(__ddiv_rn(sumsq1, (double)wf), (double)__fmul_rn(mean1, mean1));
+    cv = __dadd_rn(cv, (double)__fdiv_rn(sumsq2, wf));
+    cv = __dsub_rn(cv, (double)__fmul_rn(mean2, mean2));
+    return tstat_quotient(fmaxf((float)cv, FLT_MIN), __fsub_rn(mean2, mean1), wf);
+}
+
+__global__ void __launch_bounds__(kThreads) detect_events_stream_kernel(const EdParams p)
+{
+    extern __shared__ double s_ring[];                                // [2][ring][kThreads]: S then Q
+    const uint32_t slot_idx = blockIdx.x * kThreads + threadIdx.x;
+    if (slot_idx >= p.n_reads) return;
+    const uint32_t ridx = p.order[slot_idx];
+    const nph_raw_read rd = p.reads[ridx];
+    const float* __restrict__ raw = p.raw + rd.sample_off;
+    const unsigned long long n = rd.n_samples;
+    nph_event* out = p.events + rd.event_off;
+    const uint32_t R = p.ring;
+    double* ringS = s_ring + threadIdx.x;
+    double* ringQ = s_ring + (size_t)R * kThreads + threadIdx.x;
+#define RS(slot) ringS[(size_t)(slot) * kThreads]
+#define RQ(slot) ringQ[(size_t)(slot) * kThreads]
+
+    const uint32_t w1 = p.w1, w2 = p.w2;
+    const float wf1 = (float)w1, wf2 = (float)w2;
+    const bool on1 = !(n < 2ull * w1 || w1 < 2), on2 = !(n < 2ull * w2 || w2 < 2);
+    const PeakConsts k = peak_consts(p);
+    PeakState st = fresh_state();
+    double s0 = 0.0, q0 = 0.0, s1 = 0.0, q1 = 0.0;                  // prefix sums at the peaks st.pp0 / st.pp1
+
+    double S = 0.0, Q = 0.0;
+    unsigned long long consumed = 0;          // prefix index available: S == prefix[consumed]
+    RS(0) = 0.0; RQ(0) = 0.0;                 // prefix[0]
+    uint32_t slot_w = 0;                      // ring slot of prefix[consumed]
+    // ring slots of prefix[i - w2], [i - w1], [i], [i + w1], [i + w2]; negative indices are never read
+    int sl_m2 = -(int)w2, sl_m1 = -(int)w1, sl_0 = 0, sl_p1 = (int)w1, sl_p2 = (int)w2;
+    sl_p1 %= (int)R; sl_p2 %= (int)R;
+
+    uint32_t count = 0;
+    unsigned long long prev_pos = 0;
+    double prev_s = 0.0, prev_q = 0.0;
+
+    for (unsigned long long i = 0; i < n; ++i) {
+        // make prefix[min(n, i + w2)] available
+        const unsigned long long need = (i + w2 < n) ? i + w2 : n;
+        while (consumed < need) {
+            const float x = raw[consumed];
+            S = __dadd_rn(S, (double)x);
+            Q = __dadd_rn(Q, (double)__fmul_rn(x, x));
+            ++consumed;
+            slot_w = (slot_w + 1 == R) ? 0 : slot_w + 1;
+            RS(slot_w) = S; RQ(slot_w) = Q;
+        }
+        const double s_mid = RS(sl_0), q_mid = RQ(sl_0);
+        float ts1 = 0.0f, ts2 = 0.0f;
+        if (on1 && i >= w1 && i <= n - w1) ts1 = tstat_at(RS(sl_m1), RQ(sl_m1), s_mid, q_mid, RS(sl_p1), RQ(sl_p1), wf1);
+        if (on2 && i >= w2 && i <= n - w2) ts2 = tstat_at(RS(sl_m2), RQ(sl_m2), s_mid, q_mid, RS(sl_p2), RQ(sl_p2), wf2);
+
+        // peak_step's positions are int: the host refuses reads of more than 0x7FFFFF00 samples
+        int e0, e1;
+        peak_step(st, k, (uint32_t)i, ts1, ts2, e0, e1);
+        // a peak set at i cannot be emitted at i (that needs i - peak > w/2 >= 0), so this captures every peak's sums
+        if (st.pp0 == (int)i) { s0 = s_mid; q0 = q_mid; }
+        if (st.pp1 == (int)i) { s1 = s_mid; q1 = q_mid; }
+        if (e0 >= 0) { emit_event(out, count, rd.event_cap, prev_pos, (uint32_t)e0, prev_s, prev_q, s0, q0); prev_pos = (uint32_t)e0; prev_s = s0; prev_q = q0; }
+        if (e1 >= 0) { emit_event(out, count, rd.event_cap, prev_pos, (uint32_t)e1, prev_s, prev_q, s1, q1); prev_pos = (uint32_t)e1; prev_s = s1; prev_q = q1; }
+        // advance the five ring cursors
+        sl_m2 = (sl_m2 + 1 == (int)R) ? 0 : sl_m2 + 1;
+        sl_m1 = (sl_m1 + 1 == (int)R) ? 0 : sl_m1 + 1;
+        sl_0 = (sl_0 + 1 == (int)R) ? 0 : sl_0 + 1;
+        sl_p1 = (sl_p1 + 1 == (int)R) ? 0 : sl_p1 + 1;
+        sl_p2 = (sl_p2 + 1 == (int)R) ? 0 : sl_p2 + 1;
+    }
+    // last event: previous boundary to the end of the signal (a signal without peaks is one event)
+    emit_event(out, count, rd.event_cap, prev_pos, n, prev_s, prev_q, S, Q);
+    if (count > rd.event_cap) { *p.overflow = 1; p.n_events[ridx] = 0; }
+    else p.n_events[ridx] = count;
+#undef RS
+#undef RQ
 }
 
 } // namespace
@@ -681,7 +647,7 @@ int nph_detect_events_device(nph_ctx* ctx, const float* d_raw, size_t n_samples_
         if (r.n_samples == 0 || r.event_cap == 0 || !nph_slice_ok(r.sample_off, r.n_samples, n_samples_total) ||
             !nph_slice_ok(r.event_off, r.event_cap, events_total))
             return NPH_ERR_INVALID;
-        if (r.n_samples > 0xFFFFFF00u) return NPH_ERR_UNSUPPORTED;      // position arithmetic is 32-bit with a 2*w2 halo
+        if (r.n_samples > 0x7FFFFF00u) return NPH_ERR_UNSUPPORTED;      // peak positions are int (PeakState), with a 2*w2 halo
         n_samples[i] = r.n_samples;
     }
     // threads of a warp walk reads of similar length: longest first
@@ -690,61 +656,50 @@ int nph_detect_events_device(nph_ctx* ctx, const float* d_raw, size_t n_samples_
     EdScratch e;
     NphArena arena{scratch};
     ed_layout(arena, n_reads, events_total, e);
-    nph_raw_read* d_reads = e.reads;
-    uint32_t* d_order = e.order;
-    uint32_t* d_peaks = e.peaks;
-    uint32_t* d_npeaks = e.n_peaks;
-    uint8_t* d_exact = e.exact;
-    DetParams p{};
-    p.events = e.events;
-    p.n_events = e.n_events;
-    p.overflow = e.overflow;
-    p.raw = d_raw; p.reads = d_reads; p.order = d_order; p.n_reads = (uint32_t)n_reads;
+    EdParams p{};
+    p.raw = d_raw; p.reads = e.reads; p.order = e.order; p.n_reads = (uint32_t)n_reads;
+    p.peaks = e.peaks; p.n_peaks = e.n_peaks; p.exact = e.exact;
+    p.events = e.events; p.n_events = e.n_events; p.overflow = e.overflow;
+    p.stats = reinterpret_cast<uint32_t*>(e.overflow) + 2;
     p.w1 = params->window_length1; p.w2 = params->window_length2;
     p.t1 = params->threshold1; p.t2 = params->threshold2; p.peak_height = params->peak_height;
+    p.warm = getenv("NPH_EVENTS_WARMUP") ? ((uint32_t)atoi(getenv("NPH_EVENTS_WARMUP")) + 31u) / 32u * 32u : kFusedWarm;
     p.ring = 2 * p.w2 + 1;
-    NPH_CUDA(ctx, cudaMemcpyAsync(d_reads, reads, sizeof(nph_raw_read) * n_reads, cudaMemcpyHostToDevice, ctx->stream));
-    NPH_CUDA(ctx, cudaMemcpyAsync(d_order, order.data(), sizeof(uint32_t) * n_reads, cudaMemcpyHostToDevice, ctx->stream));
+    NPH_CUDA(ctx, cudaMemcpyAsync(e.reads, reads, sizeof(nph_raw_read) * n_reads, cudaMemcpyHostToDevice, ctx->stream));
+    NPH_CUDA(ctx, cudaMemcpyAsync(e.order, order.data(), sizeof(uint32_t) * n_reads, cudaMemcpyHostToDevice, ctx->stream));
     NPH_CUDA(ctx, cudaMemsetAsync(p.overflow, 0, 64, ctx->stream));
     // fast path first (fused guard + t-statistics + peaks, then events); reads that fail the exactness guard take the stream kernel
-    FastParams f{};
-    f.raw = d_raw; f.reads = d_reads; f.order = d_order; f.n_reads = (uint32_t)n_reads;
-    f.peaks = d_peaks; f.n_peaks = d_npeaks; f.exact = d_exact;
-    f.events = p.events; f.n_events = p.n_events; f.overflow = p.overflow;
-    f.stats = reinterpret_cast<uint32_t*>(p.overflow) + 2;
-    f.w1 = p.w1; f.w2 = p.w2; f.t1 = p.t1; f.t2 = p.t2; f.peak_height = p.peak_height;
     int launches = 0;
     if (p.w2 > (uint32_t)kFusedMaxW2) {
-        NPH_CUDA(ctx, cudaMemsetAsync(d_exact, 0, n_reads, ctx->stream));   // windows wider than the staged row: every read streams
+        NPH_CUDA(ctx, cudaMemsetAsync(p.exact, 0, n_reads, ctx->stream));   // windows wider than the staged row: every read streams
     } else {
         // one pass over the samples: guard + t-statistics + peaks (ed_fused_kernel)
         TsConsts tc{};
         tc.w1 = p.w1; tc.w2 = p.w2;
         tc.w1f = (float)p.w1; tc.w2f = (float)p.w2; tc.r1f = 1.0f / tc.w1f; tc.r2f = 1.0f / tc.w2f;
         tc.w1d = (double)p.w1; tc.w2d = (double)p.w2; tc.r1d = 1.0 / tc.w1d; tc.r2d = 1.0 / tc.w2d;
-        f.warm = getenv("NPH_EVENTS_WARMUP") ? ((uint32_t)atoi(getenv("NPH_EVENTS_WARMUP")) + 31u) / 32u * 32u : kFusedWarm;
         // warps per read: one when the batch alone fills the machine (20 resident warps per SM; measured 4 096 reads: 4.3 / 4.8 / 5.0 ms
         // with 1 / 2 / 4), more for small batches (512 reads: 1.46 / 1.02 / 0.86 ms) as long as a segment stays >= 2 warm-ups long
         int wpr = 1;
         const size_t want = (size_t)ctx->sm_count * 20;
-        while (wpr < 4 && n_reads * wpr < want && n_samples[order[0]] / (64u * wpr) >= 2 * f.warm) wpr *= 2;
+        while (wpr < 4 && n_reads * wpr < want && n_samples[order[0]] / (64u * wpr) >= 2 * p.warm) wpr *= 2;
         if (getenv("NPH_EVENTS_WPR")) wpr = atoi(getenv("NPH_EVENTS_WPR"));
-        if (wpr >= 4) launch_fused<4>(f, tc, n_reads, ctx->stream);
-        else if (wpr == 2) launch_fused<2>(f, tc, n_reads, ctx->stream);
-        else launch_fused<1>(f, tc, n_reads, ctx->stream);
+        if (wpr >= 4) launch_fused<4>(p, tc, n_reads, ctx->stream);
+        else if (wpr == 2) launch_fused<2>(p, tc, n_reads, ctx->stream);
+        else launch_fused<1>(p, tc, n_reads, ctx->stream);
         ++launches;
         NPH_CUDA(ctx, cudaGetLastError());
     }
-    ed_events_kernel<<<(unsigned)std::min<size_t>(n_reads, (size_t)ctx->sm_count * 16), 256, 0, ctx->stream>>>(f); ++launches;
+    ed_events_kernel<<<(unsigned)std::min<size_t>(n_reads, (size_t)ctx->sm_count * 16), 256, 0, ctx->stream>>>(p); ++launches;
     NPH_CUDA(ctx, cudaGetLastError());
     // fallback list
     std::vector<uint8_t> exact(n_reads);
-    NPH_CUDA(ctx, cudaMemcpyAsync(exact.data(), d_exact, n_reads, cudaMemcpyDeviceToHost, ctx->stream));
+    NPH_CUDA(ctx, cudaMemcpyAsync(exact.data(), p.exact, n_reads, cudaMemcpyDeviceToHost, ctx->stream));
     NPH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     std::vector<uint32_t> slow;
     for (size_t t = 0; t < n_reads; ++t) if (!exact[order[t]] || getenv("NPH_EVENTS_FORCE_STREAM")) slow.push_back(order[t]);
     if (!slow.empty()) {
-        NPH_CUDA(ctx, cudaMemcpyAsync(d_order, slow.data(), sizeof(uint32_t) * slow.size(), cudaMemcpyHostToDevice, ctx->stream));
+        NPH_CUDA(ctx, cudaMemcpyAsync(e.order, slow.data(), sizeof(uint32_t) * slow.size(), cudaMemcpyHostToDevice, ctx->stream));
         p.n_reads = (uint32_t)slow.size();
         const size_t smem = sizeof(double) * 2 * p.ring * kThreads;
         NPH_CUDA(ctx, cudaFuncSetAttribute(detect_events_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -753,15 +708,15 @@ int nph_detect_events_device(nph_ctx* ctx, const float* d_raw, size_t n_samples_
     }
     NPH_CUDA(ctx, cudaEventRecord(ctx->ev1, ctx->stream));
     int overflow = 0;
+    uint32_t stats[2] = {0, 0};
+    const bool report = getenv("NPH_EVENTS_STATS") != nullptr;
     h_n_events.resize(n_reads);
     NPH_CUDA(ctx, cudaMemcpyAsync(h_n_events.data(), p.n_events, sizeof(uint32_t) * n_reads, cudaMemcpyDeviceToHost, ctx->stream));
     NPH_CUDA(ctx, cudaMemcpyAsync(&overflow, p.overflow, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    if (report) NPH_CUDA(ctx, cudaMemcpyAsync(stats, p.stats, sizeof(stats), cudaMemcpyDeviceToHost, ctx->stream));
     NPH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    if (getenv("NPH_EVENTS_STATS")) {
-        uint32_t st[2] = {0, 0};
-        cudaMemcpy(st, f.stats, sizeof(st), cudaMemcpyDeviceToHost);
-        fprintf(stderr, "[nph events] reads %zu  repair walks %u  streaming fallback %zu (guard/slice %u)\n", n_reads, st[0], slow.size(), st[1]);
-    }
+    if (report)
+        fprintf(stderr, "[nph events] reads %zu  repair walks %u  streaming fallback %zu (guard/slice %u)\n", n_reads, stats[0], slow.size(), stats[1]);
     *d_events_out = p.events;
     *d_n_events_out = p.n_events;
     if (launches_out) *launches_out = launches;
