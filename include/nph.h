@@ -662,6 +662,49 @@ int nph_load_from_raw_batch(nph_ctx* ctx, const float* raw, size_t n_samples_tot
  * --samples / --signal-index read back.  NPH_ERR_STATE if n_jobs is not that call's job count. */
 int nph_last_trim_ranges(nph_ctx* ctx, nph_raw_range* ranges_out, size_t n_jobs);
 
+/* ---- poly(A) tail segmentation and length (nanopolish polya) ---------------------------------------------
+ * Per read, what estimate_polya_for_single_read computes after loading (src/nanopolish_polya_estimator.cpp:786-813):
+ * SegmentationHMM(scale, shift, var).segment_squiggle over the read's samples (:204-509: the 6-state Viterbi over every raw
+ * sample, its backtrack and the region boundaries), estimate_unaligned_duration_profile (:564-599: 1 / the median per-k-mer
+ * duration), estimate_polya_length (:638-662) and the three QC checks with their priority (:672-722, :803-813).
+ * Inputs follow nph_load_from_raw_batch's outputs: ev_duration[event_off + e] is the read's SquiggleEvent::duration,
+ * base_to_event[rank_off + ki] its base_to_event_map[ki].indices[0].  raw[sample_off ..] is the read's WHOLE raw signal
+ * (SquiggleRead::samples with SRF_LOAD_RAW_SAMPLES, acquisition order, not reversed for direct RNA).
+ * A job with loaded == 0 (the read is missing from the index) or n_events == 0 (load_from_raw cleared its events: any
+ * NPH_CAL_* status != 0) is not computed: its result carries NPH_POLYA_READ_FAILED_LOAD and -1 values (:760-777).  NPH_ERR_INVALID, before anything runs, for a loaded job with fewer than 2 samples
+ * (the reference's backtrack loop wraps), no k-mer, a sample, event or map slice outside the call's arrays, or a map entry
+ * other than {-1, *} or {start, stop} with 0 <= start <= stop < n_events (the reference asserts).  Secondary records and the
+ * suffix clip (the length of the record's LAST CIGAR operation, whatever its type) are the caller's to take from the BAM. */
+#define NPH_POLYA_PASS             0
+#define NPH_POLYA_NOREGION         1   /* fewer than 200 adapter or poly(A) samples */
+#define NPH_POLYA_ADAPTER          2   /* estimated adapter length > 300 nt */
+#define NPH_POLYA_SUFFCLIP         3   /* suffix_clip > 200 */
+#define NPH_POLYA_READ_FAILED_LOAD 4
+typedef struct {
+    uint64_t sample_off;      /* first raw sample (picoamps, float) of the read in raw[] */
+    uint64_t event_off;       /* first event duration of the read in ev_duration[] */
+    uint64_t rank_off;        /* first base_to_event entry of the read in base_to_event[] */
+    uint32_t n_samples;       /* SquiggleRead::samples.size() */
+    uint32_t n_kmers;         /* base_to_event_map.size() = read_sequence.length() - k + 1 */
+    uint32_t n_events;        /* events[0].size() */
+    uint32_t suffix_clip;     /* bam_cigar_oplen of the record's last CIGAR operation */
+    double   sample_rate;
+    double   scale, shift, var;   /* scalings[0]; the HMM takes them as floats */
+    uint32_t loaded;          /* 0: READ_FAILED_LOAD (the read is not in the index) */
+    uint32_t reserved;
+} nph_polya_job;
+typedef struct {
+    uint64_t start, leader, adapter, polya;   /* Segmentation: final sample index of START, LEADER, ADAPTER, POLYA/CLIFF */
+    uint64_t cliffs;                          /* CLIFF samples on the path */
+    double   read_rate;                       /* 1 / median per-k-mer duration (may be inf) */
+    double   polya_length;                    /* max(0, duration * rate - 5) */
+    int32_t  qc;                              /* NPH_POLYA_* */
+    uint32_t reserved;
+} nph_polya_result;
+int nph_polya_batch(nph_ctx* ctx, const float* raw, size_t n_samples_total, const nph_polya_job* jobs, size_t n_jobs,
+                    const float* ev_duration, size_t n_events_total, const nph_event_range* base_to_event, size_t n_ranks_total,
+                    nph_polya_result* results_out);
+
 /* ---- measurement hooks (used by bench.py; not part of the reference surface) ------------- */
 /* Device time in ms of the most recent nph_hmm_score / nph_abea_run kernel sequence, measured
  * with CUDA events on the context's stream (valid after a sync), and the number of kernel

@@ -10,7 +10,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from .synth import ABEA_RES_DT, ALIGN_STATE_DT, CALIBRATION_DT, EVENT_DT, EVENT_RANGE_DT, METH_SITE_DT, METHFREQ_PARAMS_DT, PAIR_DT, RAW_RANGE_DT
+from .synth import ABEA_RES_DT, ALIGN_STATE_DT, CALIBRATION_DT, EVENT_DT, EVENT_RANGE_DT, METH_SITE_DT, METHFREQ_PARAMS_DT, PAIR_DT, POLYA_RES_DT, RAW_RANGE_DT
 
 
 def _p(a):
@@ -388,6 +388,17 @@ class Engine:
                     "nph_load_from_raw_batch")
         tot = int(off[-1])
         return off, mean[:tot], stdv[:tot], start[:tot], dur[:tot], b2e, cal
+
+    def polya_batch(self, raw, jobs, ev_duration, base_to_event):
+        """nanopolish polya's per-read estimate (segmentation, read rate, tail length, QC) for a batch in one call.
+        raw: float32 whole raw signals; jobs: POLYA_JOB_DT; ev_duration: float32 event durations; base_to_event:
+        EVENT_RANGE_DT (the layout of load_from_raw_batch's outputs).  Returns POLYA_RES_DT[n_jobs];
+        nanopolish_b200.polya.rows() turns it into the reference's TSV rows."""
+        n = jobs.shape[0]
+        out = np.zeros(n, POLYA_RES_DT)
+        self._check(self.lib.nph_polya_batch(self.ctx, _p(raw), raw.shape[0], _p(jobs), n, _p(ev_duration), ev_duration.shape[0],
+                                             _p(base_to_event), base_to_event.shape[0], _p(out)), "nph_polya_batch")
+        return out
 
     # ---- measurement ----------------------------------------------------------------------
     def last_trim_ranges(self, n_jobs: int) -> np.ndarray:

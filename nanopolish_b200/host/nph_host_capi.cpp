@@ -6,6 +6,7 @@
 #include "nph_raw.hpp"
 #include "nph_eventalign.hpp"
 #include "nph_scorereads.hpp"
+#include "nph_polya.hpp"
 #include <cmath>
 #include <chrono>
 #include <cstring>
@@ -428,6 +429,41 @@ int nphh_load_from_raw(int model, int n, const float* samples, const uint64_t* s
         }
     });
     return rc ? rc : first;
+}
+
+// ---- polya over a batch of BAM records ------------------------------------------------------------------
+// Record i: name / contig / pos / flag, CIGAR words cigar[cigar_off[i] .. cigar_off[i+1]), read handle read[i] (-1: not in
+// the index) with its whole raw signal samples[sample_off[i] .. sample_off[i+1]) at sample_rate[i].  One device call; the
+// TSV (header included) goes to tsv_out.  Returns its length, or a negative status (NPH_ERR_INVALID with the length needed in
+// *n_needed if cap is too small).
+long long nphh_polya(int n, const char** names, const char** contigs, const int32_t* pos, const uint16_t* flag, const uint32_t* cigar,
+                     const uint64_t* cigar_off, const int32_t* read, const float* samples, const uint64_t* sample_off,
+                     const double* sample_rate, char* tsv_out, size_t cap, size_t* n_needed)
+{
+    std::string tsv;
+    int rc = guard([&] {
+        std::vector<RawRead> raw(n);
+        PolyaBatch batch;
+        for (int i = 0; i < n; ++i) {
+            PolyaRecord r;
+            r.read_name = names[i]; r.contig = contigs[i]; r.pos = pos[i]; r.flag = flag[i];
+            r.cigar.assign(cigar + cigar_off[i], cigar + cigar_off[i + 1]);
+            if (read[i] >= 0) {
+                raw[i].samples.assign(samples + sample_off[i], samples + sample_off[i + 1]);
+                raw[i].sample_rate = sample_rate[i];
+                r.read = g_reads.at(read[i]).get();
+                r.raw = &raw[i];
+            }
+            batch.add(r);
+        }
+        batch.run(Engine::thread_default());
+        tsv = batch.tsv(true);
+    });
+    if (rc) return rc;
+    *n_needed = tsv.size();
+    if (tsv.size() > cap) return NPH_ERR_INVALID;
+    memcpy(tsv_out, tsv.data(), tsv.size());
+    return (long long)tsv.size();
 }
 
 // ---- N1: eventalign (segment chaining around the Viterbi kernel) -------------------------------------------

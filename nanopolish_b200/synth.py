@@ -59,6 +59,13 @@ assert EVENT_DT.itemsize == 24 and RAW_READ_DT.itemsize == 24 and EVENT_PARAMS_D
 RAW_JOB_DT = np.dtype([("sample_off", "<u8"), ("rank_off", "<u8"), ("n_samples", "<u4"), ("n_kmers", "<u4"), ("sample_rate", "<f8")], align=True)
 assert RAW_JOB_DT.itemsize == 32
 assert RAW_RANGE_DT.itemsize == 8 and EVENT_RANGE_DT.itemsize == 8 and CALIBRATION_DT.itemsize == 48
+# nph_polya_job / nph_polya_result (include/nph.h)
+POLYA_JOB_DT = np.dtype([("sample_off", "<u8"), ("event_off", "<u8"), ("rank_off", "<u8"), ("n_samples", "<u4"), ("n_kmers", "<u4"),
+                         ("n_events", "<u4"), ("suffix_clip", "<u4"), ("sample_rate", "<f8"), ("scale", "<f8"), ("shift", "<f8"),
+                         ("var", "<f8"), ("loaded", "<u4"), ("reserved", "<u4")], align=True)
+POLYA_RES_DT = np.dtype([("start", "<u8"), ("leader", "<u8"), ("adapter", "<u8"), ("polya", "<u8"), ("cliffs", "<u8"),
+                         ("read_rate", "<f8"), ("polya_length", "<f8"), ("qc", "<i4"), ("reserved", "<u4")], align=True)
+assert POLYA_JOB_DT.itemsize == 80 and POLYA_RES_DT.itemsize == 64
 METH_RECORD_DT = np.dtype([("ref_off", "<u8"), ("pair_off", "<u8"), ("read", "<u4"), ("model_id", "<u4"), ("ref_len", "<u4"),
                            ("n_pairs", "<u4"), ("ref_start_pos", "<i4"), ("rc", "u1"), ("strand", "u1"), ("reserved", "u1", 2)], align=True)
 METH_SITE_DT = np.dtype([("start_position", "<i4"), ("end_position", "<i4"), ("n_motif", "<u4"), ("record", "<u4"),
