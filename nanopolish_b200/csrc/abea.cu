@@ -90,9 +90,7 @@ __global__ void __launch_bounds__(kThreads, 1) abea_kernel(const AbeaParams p)
     const DevModelView mv = p.models[p.model_id];
 
     for (;;) {
-        uint32_t slot_idx = 0;
-        if (lane == 0) slot_idx = atomicAdd(p.counter, 1u);
-        slot_idx = __shfl_sync(kFull, slot_idx, 0);
+        const uint32_t slot_idx = nph_warp_pop(p.counter, 1u, lane);
         if (slot_idx >= p.n_jobs) break;
         const uint32_t job_idx = p.order[slot_idx];
         const nph_abea_job job = p.jobs[job_idx];
@@ -143,7 +141,7 @@ __global__ void __launch_bounds__(kThreads, 1) abea_kernel(const AbeaParams p)
         const int uK = K + 128;
         const int laneK = uK & 31, slotK = (uK >> 5) & 3;
 
-        float4 g_next = (lo + 128 <= K) ? prm[lo + 128 - 1] : make_float4(0.f, 1.f, 0.f, 1.f);   // Gaussian of the next column to enter a slot
+        float4 g_next = (lo + 128 <= K) ? prm[lo + 128 - 1] : nph_pad_gaussian();   // Gaussian of the next column to enter a slot
         float x_down = lv[min(max(1 - lo, 0), E - 1)];       // level the lowest column meets in band 2 (already loaded above: a down move rewrites the same value)
         for (int bi = 2; bi < n_bands; ++bi) {
             // Suzuki's rule on the two ends of band bi-1 (offset 0 = column lo, offset 99 = column lo+99)
@@ -181,7 +179,7 @@ __global__ void __launch_bounds__(kThreads, 1) abea_kernel(const AbeaParams p)
                 }
 #undef NPH_ABEA_NEW_COLUMN
                 lo += 1;
-                g_next = (lo + 128 <= K) ? prm[lo + 128 - 1] : make_float4(0.f, 1.f, 0.f, 1.f);
+                g_next = (lo + 128 <= K) ? prm[lo + 128 - 1] : nph_pad_gaussian();
             } else {
                 // the band moved down: its lowest column meets a new event (fetched one band ahead); every other column's event
                 // level came from its left neighbour, and after a right move the column that entered the window got its own that way
@@ -204,8 +202,7 @@ __global__ void __launch_bounds__(kThreads, 1) abea_kernel(const AbeaParams p)
                 const bool cell = ((unsigned)e < (unsigned)E) && ((unsigned)(c - 1) < col_lim);
                 const float x = xn[s];
                 // emission (emissions.h:51-55) — computed for every slot, used where the cell exists
-                const float a = div_by_cached_rcp(__fsub_rn(x, mu[s]), sd[s], ry[s]);
-                const float em = __fadd_rn(cc[s], __fmul_rn(__fmul_rn(-0.5f, a), a));
+                const float em = log_gauss(x, mu[s], sd[s], cc[s], ry[s]);
                 const double emd = (double)em;
                 const float score_d = (float)__dadd_rn(__dadd_rn(dgd[s], lp_step), emd);
                 const float score_u = (float)__dadd_rn(__dadd_rn(b1d[s], lp_stay), emd);
@@ -304,8 +301,7 @@ __global__ void __launch_bounds__(kThreads, 1) abea_kernel(const AbeaParams p)
                     const unsigned long long raw = __ldcg(reinterpret_cast<const unsigned long long*>(out + (cap - 1 - i)));
                     const int pk = (int)(uint32_t)(raw & 0xffffffffull), pe = (int)(uint32_t)(raw >> 32);   // {ref_pos, read_pos}
                     const float4 g = prm[pk];
-                    const float a = div_by_cached_rcp(__fsub_rn(lv[pe], g.x), g.y, g.w);
-                    em = __fadd_rn(g.z, __fmul_rn(__fmul_rn(-0.5f, a), a));
+                    em = log_gauss(lv[pe], g.x, g.y, g.z, g.w);
                 }
                 s_em[wib][lane] = em;
                 __syncwarp();

@@ -44,7 +44,7 @@ struct ChainParams {
     unsigned int* counter;
     nph_ea_record* records;
     nph_ea_result* results;
-    float4* scratch_params;          // 32*C per warp
+    float4* scratch_params;          // 32*C per warp (one strip: no edge rows)
     uint16_t* scratch_trace;         // trace_stride per warp
     nph_align_state* scratch_states; // states_stride per warp
     uint64_t trace_stride;
@@ -94,15 +94,13 @@ __global__ void __launch_bounds__(kThreads, 1) eventalign_chain_kernel(const Cha
     __shared__ uint16_t s_tile[kWarps][32 * 32];
     VitScratch sc;
     sc.tile = s_tile[threadIdx.x >> 5];
-    sc.params = p.scratch_params + (size_t)warp_global * STRIP;
-    sc.edge_m = nullptr; sc.edge_b = nullptr; sc.edge_k = nullptr;       // single strip: never touched
+    sc.params = warp_params(p.scratch_params, STRIP, warp_global);
+    sc.edge = EdgeRows{nullptr, nullptr, nullptr};                       // single strip: never touched
     sc.trace = p.scratch_trace + (size_t)warp_global * p.trace_stride;
     nph_align_state* const states = p.scratch_states + (size_t)warp_global * p.states_stride;
 
     for (;;) {
-        uint32_t slot = 0;
-        if (lane == 0) slot = atomicAdd(p.counter, 1u);
-        slot = __shfl_sync(kFull, slot, 0);
+        const uint32_t slot = nph_warp_pop(p.counter, 1u, lane);
         if (slot >= p.n_chains) break;
         const uint32_t chain_idx = p.order[slot];
         const nph_ea_chain ch = p.chains[chain_idx];

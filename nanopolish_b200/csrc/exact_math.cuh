@@ -5,9 +5,7 @@
 #include <math.h>
 #include <stdint.h>
 
-#ifndef NPH_LOGSUM_CUT
-#define NPH_LOGSUM_CUT 15700
-#endif
+#define NPH_LOGSUM_CUT 15700        // (max - min) >= 15.7f returns max: table entries from here on hold 0.0f
 // lsum_sat's index reaches 2^14: its table has 16385 entries, and entries NPH_LOGSUM_CUT .. 2^14 hold 0.0f
 #define NPH_LOGSUM_TBL_LEN 16385
 
@@ -40,11 +38,7 @@ __device__ __forceinline__ LogsumTable make_logsum_table(const float* smem_tbl, 
 
 __device__ __forceinline__ float lsum_lookup(float mx, float u, const LogsumTable tb)
 {
-#ifdef NPH_LSUM_LEA
-    const uint32_t adr = (uint32_t)__float_as_int(u) * 4u + tb.biased_base;          // A/B: literal 4 -> LEA on the ALU pipe
-#else
     const uint32_t adr = (uint32_t)__float_as_int(u) * tb.scale + tb.biased_base;
-#endif
     float v;
     asm("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(adr));
     return __fadd_rn(mx, v);
@@ -147,4 +141,11 @@ __device__ __forceinline__ float div_by_cached_rcp(float a, float b, float y)
 __device__ __forceinline__ float add_neg_half_square(float cc, float a)
 {
     return __fmaf_rn(__fmul_rn(a, a), -0.5f, cc);
+}
+
+// Gaussian log-density of level x under a column's {mu, sd, cc = log(1/sqrt(2pi)) - log sd, ry = RN(1/sd)} (emissions.h:51-55).  The Viterbi
+// replay calls the function its fill called, so it reproduces the fill's values bit for bit.
+__device__ __forceinline__ float log_gauss(float x, float mu, float sd, float cc, float ry)
+{
+    return add_neg_half_square(cc, div_by_cached_rcp(__fsub_rn(x, mu), sd, ry));
 }

@@ -7,6 +7,7 @@
 // scripts/k1_bounds.py).
 #pragma once
 #include <stdint.h>
+#include "../../include/nph.h"
 
 #ifdef __CUDACC__
 #define NPH_HD __host__ __device__ __forceinline__
@@ -20,20 +21,42 @@
 #define NPH_STEP_BUCKETS 1024         // step key: exact below 768, then 32-step bins
 #define NPH_CHUNK_BUCKETS 8           // level chunk of the job's read (one-shot call), major key
 #define NPH_KEY_BUCKETS (NPH_STEP_BUCKETS * NPH_CHUNK_BUCKETS)
-#define NPH_MIN_PERIOD 40             // chained strips (forward and Viterbi): the right edge of row r must be written >32 steps before it is read
+#define NPH_MIN_PERIOD 40             // least rows between chained strips: the last lane writes the right edge of row r, and lane 0 reads it P - 32 steps later (hmm_wavefront.cuh)
 
 NPH_HD uint32_t nph_class_width(int wi) { return wi >= 3 ? 32u : (4u << wi); }   // 4, 8, 16, 32, 32 (chained)
 NPH_HD bool nph_class_chained(int wi) { return wi == 4; }
 NPH_HD int nph_class_index(int C, int wi) { return wi * NPH_MAX_COLS + (C - 1); }
 
-// warp steps one job takes in class (C, W): chained strips of W*C columns, period max(E, NPH_MIN_PERIOD) when chained
-NPH_HD uint32_t nph_class_steps(uint32_t K, uint32_t E, int C, uint32_t W)
+// events of a job's window, both ends included
+NPH_HD int nph_job_events(const nph_hmm_job& jb)
 {
-    const uint32_t strip = W * (uint32_t)C;
-    const uint32_t n_strips = (K + strip - 1) / strip;
-    const uint32_t P = n_strips > 1 ? (E > (uint32_t)NPH_MIN_PERIOD ? E : (uint32_t)NPH_MIN_PERIOD) : E;
-    const uint32_t last_cols = K - (n_strips - 1) * strip;
-    return (n_strips - 1) * P + E + (last_cols - 1) / (uint32_t)C;
+    return (int)(jb.event_stop > jb.event_start ? jb.event_stop - jb.event_start : jb.event_start - jb.event_stop) + 1;
+}
+
+// How K k-mer columns and E event rows lie on the systolic wavefront of a class (C columns per lane, W lanes per job): the one
+// statement of the strip rules for the forward and Viterbi kernels, the scheduler and the host-side scratch sizing.  A chained class
+// cuts the columns into strips of W*C that follow each other every P rows.
+struct nph_wave_geom {
+    int K, E, C, strip;
+    int n_strips;
+    int kpad;           // columns the strips cover
+    int P;              // rows between strip starts (one strip: E)
+    NPH_HD bool multi_strip() const { return kpad > strip; }
+    NPH_HD int last_strip() const { return n_strips - 1; }
+    // lane of the group, and column of that lane, that hold k-mer K - 1 in the last strip
+    NPH_HD int end_lane() const { return ((K - 1) - last_strip() * strip) / C; }
+    NPH_HD int end_slot() const { return ((K - 1) - last_strip() * strip) % C; }
+    NPH_HD int total_steps() const { return last_strip() * P + E + end_lane(); }   // until end_lane has done row E of the last strip
+};
+// may_chain = false only spares the single-strip kernels the division: a job that fits one strip has one strip either way
+NPH_HD nph_wave_geom nph_wave_geometry(int K, int E, int C, int W, bool may_chain)
+{
+    nph_wave_geom g;
+    g.K = K; g.E = E; g.C = C; g.strip = W * C;
+    g.n_strips = may_chain ? (K + g.strip - 1) / g.strip : 1;
+    g.kpad = g.n_strips * g.strip;
+    g.P = g.multi_strip() ? (E > NPH_MIN_PERIOD ? E : NPH_MIN_PERIOD) : E;
+    return g;
 }
 
 // per-step cost: 46 issue slots of per-step work plus the row update, 67 per column
@@ -53,7 +76,7 @@ NPH_HD int nph_choose_class(uint32_t K, uint32_t E, uint32_t* steps_out)
         for (int C = 1; C <= NPH_MAX_COLS; ++C) {
             const bool fits = K <= W * (uint32_t)C;
             if (nph_class_chained(wi) ? fits : !fits) continue;       // single-strip classes take jobs that fit, the chained class the rest
-            const uint32_t steps = nph_class_steps(K, E, C, W);
+            const uint32_t steps = (uint32_t)nph_wave_geometry((int)K, (int)E, C, (int)W, true).total_steps();   // a job that fits one strip has one strip
             const float cost = nph_class_cost(steps, C, W);
             if (cost < best) { best = cost; best_cls = nph_class_index(C, wi); best_steps = steps; }
         }

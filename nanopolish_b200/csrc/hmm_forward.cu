@@ -32,14 +32,11 @@ __global__ void read_prologue_kernel(const DevRead* __restrict__ reads, const do
 } // namespace
 
 // One slice per side stream: classes running concurrently on different SMs index their per-warp scratch by
-// (block, warp) and must not share it.  Per warp: kpad float4 Gaussians and three strip-edge rows.
+// (block, warp) and must not share it.
 static void scratch_layout(const nph_ctx* ctx, NphArena& a, float4** params, float** edge)
 {
     const size_t warps = (size_t)ctx->sm_count * kMaxWarpsPerCta;
-    for (int si = 0; si < nph_ctx::kSideStreams; ++si) {
-        params[si] = a.take<float4>((size_t)ctx->max_kpad * warps);
-        edge[si] = a.take<float>(3 * ((size_t)ctx->max_period + 8) * warps);
-    }
+    for (int si = 0; si < nph_ctx::kSideStreams; ++si) nph_wave_scratch(a, ctx->max_kpad, ctx->max_period, warps, &params[si], &edge[si]);
 }
 
 size_t nph_hmm_scratch_bytes(const nph_ctx* ctx)
@@ -73,7 +70,7 @@ int nph_launch_hmm_forward(nph_ctx* ctx, float* scores_dev)
     p.flank = ctx->d_flank.p;
     p.scores = scores_dev ? scores_dev : ctx->d_scores.p;
     p.kpad_stride = ctx->max_kpad;
-    p.edge_stride = ctx->max_period + 8;
+    p.edge_stride = nph_edge_stride(ctx->max_period);
     p.c = ctx->consts;
     p.lsum_bias = NPH_LOGSUM_SAT_ADDR_BIAS;
     p.lsum_scale = 4u;

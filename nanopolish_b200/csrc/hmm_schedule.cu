@@ -68,7 +68,7 @@ __global__ void classify_kernel(const nph_hmm_job* __restrict__ jobs, uint32_t n
         uint32_t key = 0xffffffffu, steps = 0, K = jb.n_kmers, E = 0;
         int c = 0;
         if (ok) {
-            E = (jb.event_stop > jb.event_start ? jb.event_stop - jb.event_start : jb.event_start - jb.event_stop) + 1;
+            E = (uint32_t)nph_job_events(jb);
             if (codes) rank_base[j] = atomicAdd(&sum->rank_cursor, (unsigned long long)K);     // where this job's ranks will live
             c = nph_choose_class(K, E, &steps);
             const uint32_t b = nph_key_bucket(steps, chunk);
@@ -95,9 +95,9 @@ __global__ void classify_kernel(const nph_hmm_job* __restrict__ jobs, uint32_t n
             atomicAdd(&s_cost[c], cost);
         }
         if (ok) {
-            const uint32_t strip = W * C;
-            atomicMax(&s_kpad, ((K + strip - 1) / strip) * strip);
-            atomicMax(&s_period, E > (uint32_t)NPH_MIN_PERIOD ? E : (uint32_t)NPH_MIN_PERIOD);
+            const nph_wave_geom geo = nph_wave_geometry((int)K, (int)E, C, (int)W, true);
+            atomicMax(&s_kpad, (unsigned int)geo.kpad);
+            atomicMax(&s_period, (unsigned int)geo.P);
             atomicMax(&s_E, E);
         }
     }

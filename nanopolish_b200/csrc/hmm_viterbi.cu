@@ -5,8 +5,8 @@
 //   ProfileHMMViterbiOutputR9     ref: src/hmm/nanopolish_profile_hmm_r9.inl:130-197
 //   (the fill itself is profile_hmm_fill_generic_r9, .inl:265-433, shared with the forward score)
 //
-// Same systolic mapping as the forward kernel (hmm_forward_kernel.cuh): a warp per job, lane j owns C
-// k-mer columns, strips of 32*C columns chained.  Differences:
+// The systolic wavefront of hmm_wavefront.cuh, which the forward kernel also walks: a warp per job, lane j owns C
+// k-mer columns, strips of 32*C columns chained.  What differs from the forward score is the cell:
 //   * (+) is max with the reference's argmax rule — a compare chain over the six movement types in
 //     index order where a LATER index wins ties (`from = max == x[i] ? i : from`), so an all -inf cell
 //     records FROM_SOFT like the reference does;
@@ -56,24 +56,18 @@ struct VitParams {
 template <int C>
 __global__ void __launch_bounds__(kThreads, 1) hmm_viterbi_kernel(const VitParams p)
 {
-    constexpr int STRIP = 32 * C;
     const int lane = threadIdx.x & 31;
     const int warp_global = blockIdx.x * kWarps + (threadIdx.x >> 5);
     __shared__ uint16_t s_tile[kWarps][32 * 32];
     VitScratch sc;
     sc.tile = s_tile[threadIdx.x >> 5];
-    sc.params = p.scratch_params + (size_t)warp_global * p.kpad_stride;
-    sc.edge_m = p.scratch_edge + (size_t)warp_global * 3 * p.edge_stride;
-    sc.edge_b = sc.edge_m + p.edge_stride;
-    sc.edge_k = sc.edge_b + p.edge_stride;
+    sc.params = warp_params(p.scratch_params, p.kpad_stride, warp_global);
+    sc.edge = warp_edge_rows(p.scratch_edge, p.edge_stride, warp_global);
     sc.trace = p.scratch_trace + (size_t)warp_global * p.trace_stride;
     const float NEG = -CUDART_INF_F;
-    (void)STRIP;
 
     for (;;) {
-        uint32_t slot = 0;
-        if (lane == 0) slot = atomicAdd(p.counter, 1u);
-        slot = __shfl_sync(kFull, slot, 0);
+        const uint32_t slot = nph_warp_pop(p.counter, 1u, lane);
         if (slot >= p.n_jobs) break;
         const uint32_t job_idx = p.order[slot];
         const nph_hmm_job job = p.jobs[job_idx];
@@ -84,7 +78,7 @@ __global__ void __launch_bounds__(kThreads, 1) hmm_viterbi_kernel(const VitParam
         j.lv = p.level + j.rd.event_off;
         j.rk = p.ranks + job.rank_off;
         j.K = (int)job.n_kmers;
-        j.E = (int)(job.event_stop > job.event_start ? job.event_stop - job.event_start : job.event_start - job.event_stop) + 1;
+        j.E = nph_job_events(job);
         j.stride = job.stride;
         j.e_first = (long long)job.event_start;
         j.pre_clip = (job.flags & NPH_HAF_ALLOW_PRE_CLIP) != 0;
@@ -154,21 +148,21 @@ extern "C" int nph_hmm_align(nph_ctx* ctx,
     uint64_t max_trace = 1;
     for (size_t j = 0; j < n_jobs; ++j) {
         const nph_hmm_job& jb = jobs[j];
-        const uint32_t E = (jb.event_stop > jb.event_start ? jb.event_stop - jb.event_start : jb.event_start - jb.event_stop) + 1;
+        const uint32_t E = (uint32_t)nph_job_events(jb);
         const uint32_t K = jb.n_kmers;
         if (states_off[j + 1] < states_off[j]) return NPH_ERR_INVALID;
         double best = 1e300; int bi = 0; uint32_t bsteps = 0;
+        nph_wave_geom geo{};
         for (int i = 0; i < kNumVit; ++i) {
-            const uint32_t st = nph_class_steps(K, E, kVitCols[i], 32);
-            const double cost = (double)st * (120.0 + 70.0 * kVitCols[i]);
-            if (cost < best) { best = cost; bi = i; bsteps = st; }
+            const nph_wave_geom g = nph_wave_geometry((int)K, (int)E, kVitCols[i], 32, true);
+            const double cost = (double)g.total_steps() * (120.0 + 70.0 * kVitCols[i]);
+            if (cost < best) { best = cost; bi = i; bsteps = (uint32_t)g.total_steps(); geo = g; }
         }
         key[j] = (uint64_t)(kNumVit - 1 - bi) << 32 | bsteps;
         ++first[bi + 1];
-        const uint32_t strip = 32u * kVitCols[bi], n_strips = (K + strip - 1) / strip;
-        max_kpad = std::max(max_kpad, n_strips * strip);
-        max_period = std::max(max_period, std::max<uint32_t>(E, NPH_MIN_PERIOD));
-        max_trace = std::max<uint64_t>(max_trace, (uint64_t)(bsteps + 1) * strip);
+        max_kpad = std::max(max_kpad, (uint32_t)geo.kpad);
+        max_period = std::max(max_period, (uint32_t)geo.P);
+        max_trace = std::max<uint64_t>(max_trace, (uint64_t)(bsteps + 1) * geo.strip);
     }
     const std::vector<uint32_t> order = nph_longest_first(key);
     for (int i = 0; i < kNumVit; ++i) first[i + 1] += first[i];
@@ -191,8 +185,7 @@ extern "C" int nph_hmm_align(nph_ctx* ctx,
     uint64_t* d_off = nullptr;
     uint32_t* d_order = nullptr;
     NPH_TRY(nph_carve_align_scratch(ctx, [&](NphArena& a) {
-        p.scratch_params = a.take<float4>((size_t)max_kpad * warps);
-        p.scratch_edge = a.take<float>(3 * ((size_t)max_period + 8) * warps);
+        nph_wave_scratch(a, max_kpad, max_period, warps, &p.scratch_params, &p.scratch_edge);
         p.scratch_trace = a.take<uint16_t>(trace_stride * warps);
         p.states = a.take<nph_align_state>(total_states);
         d_off = a.take<uint64_t>(n_jobs + 1);
@@ -202,7 +195,7 @@ extern "C" int nph_hmm_align(nph_ctx* ctx,
     p.states_off = d_off;
     p.level = ctx->d_level.p; p.reads = ctx->d_reads.p; p.trans = ctx->d_trans.p; p.models = ctx->d_models.p;
     p.ranks = ctx->d_ranks.p; p.jobs = ctx->d_jobs.p; p.flank = ctx->d_flank.p; p.scores = ctx->d_scores.p;
-    p.kpad_stride = max_kpad; p.edge_stride = max_period + 8; p.trace_stride = trace_stride; p.c = ctx->consts;
+    p.kpad_stride = max_kpad; p.edge_stride = nph_edge_stride(max_period); p.trace_stride = trace_stride; p.c = ctx->consts;
     NPH_CUDA(ctx, cudaMemcpyAsync(d_off, states_off, sizeof(uint64_t) * (n_jobs + 1), cudaMemcpyHostToDevice, ctx->stream));
     NPH_CUDA(ctx, cudaMemcpyAsync(d_order, order.data(), sizeof(uint32_t) * n_jobs, cudaMemcpyHostToDevice, ctx->stream));
     NPH_CUDA(ctx, cudaMemsetAsync(ctx->d_counters.p, 0, sizeof(unsigned int) * NPH_NUM_COUNTERS, ctx->stream));

@@ -4,10 +4,8 @@
 //   profile_hmm_align_r9          ref: src/hmm/nanopolish_profile_hmm_r9.cpp:73-204
 //   ProfileHMMViterbiOutputR9     ref: src/hmm/nanopolish_profile_hmm_r9.inl:130-197
 #pragma once
-#include "nph_internal.cuh"
-#include "hmm_classes.h"
+#include "hmm_wavefront.cuh"
 #include "exact_math.cuh"
-#include <math_constants.h>
 
 namespace nph_vit {
 
@@ -25,11 +23,11 @@ struct VitJob {
     long long e_first;        // HMMInputData::event_start_idx
     bool pre_clip;
 };
-// per-warp scratch: Gaussians (kpad float4), strip-edge columns (3 x edge_stride floats; untouched for one strip),
+// per-warp scratch: Gaussians (kpad float4), strip-edge columns M, B, K (untouched for one strip),
 // movement codes ((steps + 1) * 32 * C uint16) in global memory; a 2 KB tile in shared memory
 struct VitScratch {
     float4* params;
-    float* edge_m; float* edge_b; float* edge_k;
+    EdgeRows edge;
     uint16_t* trace;
     uint16_t* tile;           // shared memory, 32 x 32 movement codes: the backtrack's staging corner
 };
@@ -57,37 +55,25 @@ __device__ __forceinline__ int viterbi_align(const HmmConsts& c, const float* __
     const float lp_mk = c.lp_mk, lp_mb = c.lp_mb, lp_bb = c.lp_bb, lp_bk = c.lp_bk;
     const float lp_bm_next = c.lp_bm_next, lp_bm_self = c.lp_bm_self, lp_kk = c.lp_kk, lp_km = c.lp_km;
     const float lp_mm_self = j.tr.x, lp_mm_next = j.tr.y;
-    const DevRead& rd = j.rd;
-    const DevModelView& mv = j.mv;
     const int K = j.K, E = j.E, stride = j.stride;
     const bool pre_clip = j.pre_clip;
     float4* const my_params = sc.params;
-    float* const edge_m = sc.edge_m; float* const edge_b = sc.edge_b; float* const edge_k = sc.edge_k;
     uint16_t* const trace = sc.trace;
-    const int n_strips = (K + STRIP - 1) / STRIP;
-    const int kpad = n_strips * STRIP;
-    const int P = n_strips > 1 ? max(E, NPH_MIN_PERIOD) : E;
-    {
-        const uint32_t* rk = j.rk;
-        for (int i = lane; i < kpad; i += 32) {
-            float4 g = make_float4(0.f, 1.f, 0.f, 1.f);
-            if (i < K) g = nph_scaled_gaussian(mv, rd, rk[i], c.log_inv_sqrt_2pi);
-            my_params[i] = g;
-        }
-    }
+    const nph_wave_geom geo = nph_wave_geometry(K, E, C, 32, true);
+    const int P = geo.P;
+    fill_job_gaussians<32>(my_params, j.mv, j.rd, j.rk, K, geo.kpad, lane, c.log_inv_sqrt_2pi);
     __syncwarp();
 
     const float* lv = j.lv;
     const long long e_first = j.e_first;
-    const int last_strip = n_strips - 1;
-    const int end_lane = ((K - 1) - last_strip * STRIP) / C;
-    const int total_steps = last_strip * P + E + end_lane;
+    const int total_steps = geo.total_steps();
 
     // ---------------------------------- fill ----------------------------------
     float mu[C], sd[C], cc[C], ry[C], Mp[C], Bp[C], Kp[C];
 #pragma unroll
     for (int c = 0; c < C; ++c) { mu[c] = 0.f; sd[c] = 1.f; cc[c] = 0.f; ry[c] = 1.f; Mp[c] = NEG; Bp[c] = NEG; Kp[c] = NEG; }
     float Lm_prev = NEG, Lb_prev = NEG, Lk_prev = NEG;
+    const int n_strips = geo.n_strips, last_strip = geo.last_strip();
     int r = 1 - lane, s = 0;
     float x_next = 0.f;
     if (r == 1) x_next = lv[e_first];
@@ -106,17 +92,14 @@ __device__ __forceinline__ int viterbi_align(const HmmConsts& c, const float* __
 #pragma unroll
             for (int c = 0; c < C; ++c) { Mp[c] = NEG; Bp[c] = NEG; Kp[c] = NEG; }
             Lm_prev = NEG; Lb_prev = NEG; Lk_prev = NEG;
-            if (col0 < K) {
-#pragma unroll
-                for (int c = 0; c < C; ++c) { const float4 g4 = my_params[col0 + c]; mu[c] = g4.x; sd[c] = g4.y; cc[c] = g4.z; ry[c] = g4.w; }
-            }
+            if (col0 < K) load_columns<C>(my_params, col0, mu, sd, cc, ry);
         }
         {
             int rn = r + 1, sn = s;
             if (rn > P) { rn = 1; sn = s + 1; }
             if (rn >= 1 && rn <= E && sn < n_strips) {
                 x_next = lv[e_first + (long long)(rn - 1) * stride];
-                if (lane == 0 && sn > 0) { em_next = edge_m[rn]; eb_next = edge_b[rn]; ek_next = edge_k[rn]; }
+                if (lane == 0 && sn > 0) { em_next = sc.edge.a[rn]; eb_next = sc.edge.b[rn]; ek_next = sc.edge.c[rn]; }
             }
         }
         uint16_t tcode[C];
@@ -129,8 +112,7 @@ __device__ __forceinline__ int viterbi_align(const HmmConsts& c, const float* __
             float lm_cur = Lm, lb_cur = Lb, lk_cur = Lk;
 #pragma unroll
             for (int c = 0; c < C; ++c) {
-                const float a = div_by_cached_rcp(__fsub_rn(x, mu[c]), sd[c], ry[c]);
-                const float em = __fadd_rn(cc[c], __fmul_rn(__fmul_rn(-0.5f, a), a));
+                const float em = log_gauss(x, mu[c], sd[c], cc[c], ry[c]);
                 // MATCH: six candidates in movement order
                 float m = __fadd_rn(lp_mm_self, Mp[c]);
                 int fm = MV_SAME_M;
@@ -164,7 +146,7 @@ __device__ __forceinline__ int viterbi_align(const HmmConsts& c, const float* __
                 tcode[c] = (uint16_t)(fm | (fb << 3) | (fk << 6));
             }
             Lm_prev = Lm; Lb_prev = Lb; Lk_prev = Lk;
-            if (lane == 31 && s < last_strip) { edge_m[r] = Mp[C - 1]; edge_b[r] = Bp[C - 1]; edge_k[r] = Kp[C - 1]; }
+            if (lane == 31 && s < last_strip) { sc.edge.a[r] = Mp[C - 1]; sc.edge.b[r] = Bp[C - 1]; sc.edge.c[r] = Kp[C - 1]; }
         }
         // trace line of this step: one contiguous 64*C bytes per warp
 #pragma unroll
@@ -259,8 +241,7 @@ __device__ __forceinline__ int viterbi_align(const HmmConsts& c, const float* __
                                   : mvt == MV_PREV_B ? lp_bm_next : lp_km;
                 t = (mvt == MV_SOFT) ? x5 : __fadd_rn(tr_, v);
                 const float4 g4 = my_params[a.kmer_idx];
-                const float aa = div_by_cached_rcp(__fsub_rn(lv[a.event_idx], g4.x), g4.y, g4.w);
-                t = __fadd_rn(t, __fadd_rn(g4.z, __fmul_rn(__fmul_rn(-0.5f, aa), aa)));
+                t = __fadd_rn(t, log_gauss(lv[a.event_idx], g4.x, g4.y, g4.z, g4.w));
             } else if (a.state == 'B') {
                 t = __fadd_rn(mvt == MV_SAME_M ? lp_mb : lp_bb, v);
             } else {

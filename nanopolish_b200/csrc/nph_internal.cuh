@@ -11,7 +11,6 @@
 #include "../../include/nph.h"
 
 #define NPH_LOGSUM_TBL 16000        // ref: p7_LOGSUM_TBL, src/common/logsum.h:20
-#define NPH_LOGSUM_CUT 15700        // (max-min) >= 15.7f returns max: entries >= 15700 hold 0.0f
 #define NPH_TBL_SMEM   16385        // = NPH_LOGSUM_TBL_LEN: the saturated index of lsum_sat (exact_math.cuh) reaches 2^14
 #define NPH_NUM_COUNTERS 64          // work-queue counters: one per forward class (<= 40), nph_check_ranks' flag, ABEA (last)
 
@@ -299,6 +298,17 @@ __device__ __forceinline__ float4 nph_scaled_gaussian(const DevModelView& mv, co
     const float sd = (float)__dmul_rn(mv.stdv[r], rd.var);
     const float lsd = (float)__dadd_rn(mv.log_stdv[r], rd.log_var);
     return make_float4(mu, sd, __fsub_rn(log_inv_sqrt_2pi, lsd), __frcp_rn(sd));
+}
+
+// the Gaussian of a padding column (no k-mer): z-score and log-density stay finite, and the column's cells are never live
+__device__ __forceinline__ float4 nph_pad_gaussian() { return make_float4(0.f, 1.f, 0.f, 1.f); }
+
+// Persistent warps: the warp's next n slots of a work queue (lane 0 pops, every lane gets the first slot's index)
+__device__ __forceinline__ uint32_t nph_warp_pop(unsigned int* counter, unsigned int n, int lane)
+{
+    uint32_t base = 0;
+    if (lane == 0) base = atomicAdd(counter, n);
+    return __shfl_sync(0xffffffffu, base, 0);
 }
 
 // Inclusive sum of v over the block (blockDim.x a multiple of 32; every thread calls it), s: 32 values of shared memory.

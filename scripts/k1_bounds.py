@@ -21,6 +21,7 @@ replayed on the same look-ups, per site (m1..m4 the match fold, b the bad state,
                word; a bound on what a sink word for no-op look-ups could give, not a form the kernel has.
 
 Usage: python scripts/k1_bounds.py [--jobs N] [--object path/to/hmm_forward_w32.o]
+       python scripts/k1_bounds.py --compare parent/csrc/build new/csrc/build
 """
 from __future__ import annotations
 
@@ -176,6 +177,46 @@ def issue_side(obj: str) -> dict[int, dict]:
     return res
 
 
+_KERNEL = re.compile(r"hmm_forward_kernelILi(\d+)ELi(\d+)ELb([01])E")
+
+
+def _normalised(insns):
+    """instructions without register numbers, branch targets and constant-bank offsets"""
+    def norm(t):
+        return re.sub(r"\b(U?[RP])\d+\b", r"\1", re.sub(r"0x[0-9a-f]+", "0x", t))
+    return [(norm(pred), op, norm(ops)) for _, pred, op, ops in insns]
+
+
+def compare_objects(parent_dir: str, new_dir: str) -> int:
+    """Every hmm_forward_kernel<C, W, CHAIN> of the hmm_forward_w*.o in two build directories: same SASS or not, and the
+    steady-state step's instruction count.  Returns the number of kernels that differ in more than instruction order."""
+    rows, worse = [], 0
+    for name in sorted(f for f in os.listdir(new_dir) if re.fullmatch(r"hmm_forward_w\d+c?\.o", f)):
+        old, new = sass_functions(os.path.join(parent_dir, name)), sass_functions(os.path.join(new_dir, name))
+        for fn in sorted(new, key=lambda f: tuple(int(x) for x in _KERNEL.search(f).groups()[::-1]) if _KERNEL.search(f) else ()):
+            m = _KERNEL.search(fn)
+            if not m or fn not in old:
+                continue
+            C, W, chain = int(m.group(1)), int(m.group(2)), m.group(3) == "1"
+            a, b = _normalised(old[fn]), _normalised(new[fn])
+            if a == b:
+                verdict = "identical"
+            elif collections.Counter(x[1] for x in a) == collections.Counter(x[1] for x in b):
+                verdict = "same opcode histogram"
+            else:
+                verdict = "differs"
+            steps = [len(steady_step(f[fn], 7 * C)) for f in (old, new)]
+            worse += verdict == "differs" or steps[1] > steps[0]
+            rows.append((C, W, chain, verdict, len(a), len(b), steps[0], steps[1]))
+    print("| C | W | chained | SASS, registers and addresses normalised | instructions parent / new | steady step parent / new |")
+    print("|---|---|---|---|---|---|")
+    for C, W, chain, verdict, na, nb, sa, sb in rows:
+        print(f"| {C} | {W} | {'yes' if chain else 'no'} | {verdict} | {na} / {nb} | {sa} / {sb} |")
+    tally = collections.Counter(r[3] for r in rows)
+    print(f"{len(rows)} kernels: " + ", ".join(f"{v} {k}" for k, v in sorted(tally.items())))
+    return worse
+
+
 # ---------------------------------------------------------------------------------------------------------
 # shared-memory side
 def _lsum(a, b, tbl):
@@ -327,7 +368,11 @@ def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--jobs", type=int, default=180, help="bench scorereads jobs replayed for the shared-memory side")
     ap.add_argument("--object", default=None, help="compiled hmm_forward_w32.o (default: compile the current source)")
+    ap.add_argument("--compare", nargs=2, metavar=("PARENT_OBJECTS", "NEW_OBJECTS"), default=None,
+                    help="two directories of hmm_forward_w*.o: compare every forward kernel's SASS and steady-state step, then exit")
     args = ap.parse_args()
+    if args.compare:
+        sys.exit(1 if compare_objects(*args.compare) else 0)
     obj = args.object
     if obj is None:
         import tempfile
