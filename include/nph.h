@@ -308,6 +308,56 @@ int nph_eventalign_chain(nph_ctx* ctx,
                          const uint32_t* ref_ranks_fwd, const uint32_t* ref_ranks_rc, size_t n_ranks_total,
                          const nph_ea_chain* chains, size_t n_chains, double indel_bias,
                          nph_ea_record* records_out, size_t records_total, nph_ea_result* results_out);
+/* The staged form: the same inputs, checks and launch, but only the results come back; the records stay on the device, where
+ * nph_eventalign_tsv formats them and nph_eventalign_records_fetch copies them out (nph_eventalign_chain is the two in one
+ * call).  They stay valid until the next call on this context that loads reads or uses the alignment scratch (any alignment,
+ * ABEA or raw-read call); after that the two consumers return NPH_ERR_STATE. */
+int nph_eventalign_chain_run(nph_ctx* ctx,
+                             const nph_aligned_pair* pairs, size_t n_pairs_total,
+                             const int32_t* event_map_start, size_t n_map_total,
+                             const uint32_t* ref_ranks_fwd, const uint32_t* ref_ranks_rc, size_t n_ranks_total,
+                             const nph_ea_chain* chains, size_t n_chains, double indel_bias,
+                             size_t records_total, nph_ea_result* results_out);
+int nph_eventalign_records_fetch(nph_ctx* ctx, nph_ea_record* records_out, size_t records_total);
+
+/* ---- eventalign.tsv on the device -----------------------------------------------------------------------
+ * The rows of emit_event_alignment_tsv (src/alignment/nanopolish_eventalign.cpp:398-484) for the records of the last
+ * nph_eventalign_chain_run, formatted where they are: one row per record, chains in the order given, records in order, the
+ * bytes of consecutive rows adjacent.  What a row needs beyond the resident records, rank tables, models and reads comes in
+ * flat arrays: per output read (one BAM record: all its chains) the names, the upper-cased, disambiguated reference and its
+ * reverse complement, the strand's unscaled event means, stdv and duration (one per event of the read), and for
+ * --signal-index / --samples the events' start times and the raw samples. */
+typedef struct {
+    uint64_t contig_off, name_off;       /* in text[] */
+    uint64_t ref_off;                    /* in ref[] and rc_ref[]: ref_len characters, as the read's chains index them */
+    uint64_t event_off;                  /* in ev_mean[], ev_stdv[], ev_duration[], ev_start_time[]: n_events entries */
+    uint64_t sample_off, n_samples;      /* in samples[] (--samples) */
+    uint64_t read_idx;                   /* printed as %zu without -n */
+    uint64_t sample_start_time;          /* SquiggleRead::sample_start_time */
+    double   sample_rate, drift;
+    uint32_t contig_len, name_len, ref_len, n_events;
+    uint32_t strand_idx;                 /* 0 't', 1 'c' */
+    uint32_t reserved;
+} nph_ea_tsv_read;
+typedef struct {
+    const nph_ea_tsv_read* reads; size_t n_reads;
+    const uint32_t* chain_read;          /* per chain of the run: its output read, non-decreasing */
+    const char* text; size_t n_text;
+    const char* ref; const char* rc_ref; size_t n_ref;
+    const float* ev_mean; const float* ev_stdv; const float* ev_duration;
+    const double* ev_start_time;         /* may be NULL without --signal-index / --samples */
+    size_t n_events;
+    const float* samples; size_t n_samples;   /* may be NULL without --samples */
+} nph_ea_tsv_batch;
+typedef struct { uint8_t print_read_names, scale_events, write_signal_index, write_samples; } nph_ea_tsv_options;
+/* Refusals are per read: a read with a value the exact formatter does not take (a non-finite or huge stdv, duration, level or
+ * sample, the 0 / 0 of an event mean of exactly zero at a 'B' state, a sample range outside the read's samples under --samples)
+ * or with a chain whose status is not NPH_EA_OK gets no bytes and read_refused_out[read] = 1; the caller formats it with the C
+ * library.  read_off_out: n_reads + 1 byte offsets; row_off_out (may be NULL): one per record + 1.  tsv_out is best
+ * page-locked.  cap too small: NPH_ERR_INVALID with *n_bytes_out set and the offset tables filled.  NPH_ERR_STATE without
+ * resident records. */
+int nph_eventalign_tsv(nph_ctx* ctx, const nph_ea_tsv_batch* in, const nph_ea_tsv_options* opt, char* tsv_out, size_t cap,
+                       uint64_t* row_off_out, uint64_t* read_off_out, uint8_t* read_refused_out, uint64_t* n_bytes_out);
 
 /* ---- call-methylation: window enumeration + both scores per motif group on the device (section 8f N3) -----
  * calculate_methylation_for_read (src/basemods/nanopolish_basemods.cpp:238-457) from "Scan the sequence for motifs"

@@ -56,6 +56,9 @@ def load() -> C.CDLL:
     lib.nph_hmm_align_batch.argtypes = [vp, vp, sz, vp, vp, sz, vp, sz, vp, sz, dbl, vp, vp, vp, vp]
     lib.nph_hmm_align.argtypes = [vp, vp, sz, vp, sz, dbl, vp, vp, vp, vp]
     lib.nph_eventalign_chain.argtypes = [vp, vp, sz, vp, sz, vp, vp, sz, vp, sz, dbl, vp, sz, vp]
+    lib.nph_eventalign_chain_run.argtypes = [vp, vp, sz, vp, sz, vp, vp, sz, vp, sz, dbl, sz, vp]
+    lib.nph_eventalign_records_fetch.argtypes = [vp, vp, sz]
+    lib.nph_eventalign_tsv.argtypes = [vp, vp, vp, vp, sz, vp, vp, vp, vp]
     lib.nph_detect_events_batch.argtypes = [vp, vp, sz, vp, sz, vp, vp, sz, vp]
     lib.nph_trim_raw_batch.argtypes = [vp, vp, sz, vp, sz, C.c_int32, C.c_int32, C.c_int32, C.c_float, vp]
     lib.nph_recalibrate_batch.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, sz, u32, vp, sz, vp, vp, vp]
@@ -94,5 +97,5 @@ EXPORTS = [
     "nph_sync", "nph_stream", "nph_model_upload", "nph_hmm_score_batch", "nph_hmm_score_batch_seq", "nph_hmm_jobs_load_seq", "nph_reads_load",
     "nph_hmm_jobs_load", "nph_hmm_score", "nph_hmm_scores_fetch", "nph_score_set_combine",
     "nph_abea_batch", "nph_abea_jobs_load", "nph_abea_run", "nph_abea_fetch", "nph_mom_batch",
-    "nph_hmm_align_batch", "nph_hmm_align", "nph_eventalign_chain", "nph_detect_events_batch", "nph_trim_raw_batch", "nph_recalibrate_batch", "nph_load_from_raw_batch", "nph_last_trim_ranges", "nph_polya_batch", "nph_methylation_batch", "nph_methylation_batch_compact", "nph_methylation_load", "nph_methylation_load_compact", "nph_methylation_run", "nph_methylation_counts", "nph_methylation_fetch", "nph_methylation_sites_dev", "nph_methylation_tsv", "nph_methylation_batch_compact_tsv", "nph_methfreq_reset", "nph_methfreq_add", "nph_methfreq_counts", "nph_methfreq_tsv", "nph_screen_edits_batch", "nph_screen_load", "nph_screen_run", "nph_screen_counts", "nph_screen_fetch", "nph_screen_load_methylation", "nph_screen_edits_batch_methylation", "nph_last_kernel_ms", "nph_host_alloc", "nph_host_free",
+    "nph_hmm_align_batch", "nph_hmm_align", "nph_eventalign_chain", "nph_eventalign_chain_run", "nph_eventalign_records_fetch", "nph_eventalign_tsv", "nph_detect_events_batch", "nph_trim_raw_batch", "nph_recalibrate_batch", "nph_load_from_raw_batch", "nph_last_trim_ranges", "nph_polya_batch", "nph_methylation_batch", "nph_methylation_batch_compact", "nph_methylation_load", "nph_methylation_load_compact", "nph_methylation_run", "nph_methylation_counts", "nph_methylation_fetch", "nph_methylation_sites_dev", "nph_methylation_tsv", "nph_methylation_batch_compact_tsv", "nph_methfreq_reset", "nph_methfreq_add", "nph_methfreq_counts", "nph_methfreq_tsv", "nph_screen_edits_batch", "nph_screen_load", "nph_screen_run", "nph_screen_counts", "nph_screen_fetch", "nph_screen_load_methylation", "nph_screen_edits_batch_methylation", "nph_last_kernel_ms", "nph_host_alloc", "nph_host_free",
 ]

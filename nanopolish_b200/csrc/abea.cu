@@ -503,6 +503,7 @@ int nph_abea_stage(nph_ctx* ctx, const uint32_t* n_events, const nph_abea_job* j
 
     ctx->abea_kmax = kmax;
     ctx->abea_trace_stride = 32 * (max_bands + kTraceBlockRows);
+    ctx->ea.resident = false;            // the band trace takes the scratch an eventalign chain run left its records in
     NPH_TRY(nph_reserve(ctx, ctx->d_align_scratch, nph_layout_bytes([&](NphArena& a) { float4* q; uint8_t* t; scratch_layout(ctx, a, &q, &t); })));
     NPH_TRY(nph_reserve(ctx, ctx->d_abea_jobs, n_jobs));
     NPH_TRY(nph_reserve(ctx, ctx->d_abea_ranks, n_ranks_total));

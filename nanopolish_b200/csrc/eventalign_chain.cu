@@ -219,15 +219,15 @@ void launch_chain(const ChainParams& p, int grid, cudaStream_t stream)
 
 } // namespace
 
-extern "C" int nph_eventalign_chain(nph_ctx* ctx,
-                                    const nph_aligned_pair* pairs, size_t n_pairs_total,
-                                    const int32_t* event_map_start, size_t n_map_total,
-                                    const uint32_t* ref_ranks_fwd, const uint32_t* ref_ranks_rc, size_t n_ranks_total,
-                                    const nph_ea_chain* chains, size_t n_chains, double indel_bias,
-                                    nph_ea_record* records_out, size_t records_total, nph_ea_result* results_out)
+extern "C" int nph_eventalign_chain_run(nph_ctx* ctx,
+                                        const nph_aligned_pair* pairs, size_t n_pairs_total,
+                                        const int32_t* event_map_start, size_t n_map_total,
+                                        const uint32_t* ref_ranks_fwd, const uint32_t* ref_ranks_rc, size_t n_ranks_total,
+                                        const nph_ea_chain* chains, size_t n_chains, double indel_bias,
+                                        size_t records_total, nph_ea_result* results_out)
 {
     if (!ctx || !chains || !results_out || n_chains == 0) return NPH_ERR_INVALID;
-    if (!pairs || !event_map_start || !ref_ranks_fwd || !ref_ranks_rc || (!records_out && records_total)) return NPH_ERR_INVALID;
+    if (!pairs || !event_map_start || !ref_ranks_fwd || !ref_ranks_rc) return NPH_ERR_INVALID;
     if (!ctx->reads_loaded) return NPH_ERR_STATE;
     NPH_CUDA(ctx, cudaSetDevice(ctx->device));
 
@@ -260,7 +260,7 @@ extern "C" int nph_eventalign_chain(nph_ctx* ctx,
     const uint32_t states_stride = (uint32_t)(e_cap + strip + 8);
 
     const size_t b_pairs = sizeof(nph_aligned_pair) * n_pairs_total, b_map = sizeof(int32_t) * n_map_total;
-    const size_t b_ranks = sizeof(uint32_t) * n_ranks_total, b_rec = sizeof(nph_ea_record) * records_total;
+    const size_t b_ranks = sizeof(uint32_t) * n_ranks_total;
     nph_aligned_pair* d_pairs; int32_t* d_map; uint32_t* d_rf; uint32_t* d_rr; nph_ea_chain* d_chains; uint32_t* d_order;
     nph_ea_record* d_rec; nph_ea_result* d_res;
     ChainParams p{};
@@ -296,8 +296,39 @@ extern "C" int nph_eventalign_chain(nph_ctx* ctx,
     NPH_CUDA(ctx, cudaGetLastError());
     NPH_CUDA(ctx, cudaEventRecord(ctx->ev1, ctx->stream));
     nph_timing_events(ctx, 1);
-    if (b_rec) NPH_CUDA(ctx, cudaMemcpyAsync(records_out, d_rec, b_rec, cudaMemcpyDeviceToHost, ctx->stream));
     NPH_CUDA(ctx, cudaMemcpyAsync(results_out, d_res, sizeof(nph_ea_result) * n_chains, cudaMemcpyDeviceToHost, ctx->stream));
     NPH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    // the records stay where the kernel wrote them, for nph_eventalign_tsv and nph_eventalign_records_fetch
+    nph_ctx::EaState& ea = ctx->ea;
+    ea.records_total = records_total; ea.n_ranks = n_ranks_total;
+    ea.d_chains = d_chains; ea.d_records = d_rec; ea.d_results = d_res; ea.d_ranks_fwd = d_rf; ea.d_ranks_rc = d_rr;
+    ea.h_chains.assign(chains, chains + n_chains);
+    ea.h_results.assign(results_out, results_out + n_chains);
+    ea.resident = true;
     return NPH_OK;
+}
+
+extern "C" int nph_eventalign_records_fetch(nph_ctx* ctx, nph_ea_record* records_out, size_t records_total)
+{
+    if (!ctx || (!records_out && records_total)) return NPH_ERR_INVALID;
+    if (!ctx->ea.resident) return NPH_ERR_STATE;
+    if (records_total != ctx->ea.records_total) return NPH_ERR_INVALID;
+    if (records_total == 0) return NPH_OK;
+    NPH_CUDA(ctx, cudaSetDevice(ctx->device));
+    NPH_CUDA(ctx, cudaMemcpyAsync(records_out, ctx->ea.d_records, sizeof(nph_ea_record) * records_total, cudaMemcpyDeviceToHost, ctx->stream));
+    NPH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return NPH_OK;
+}
+
+extern "C" int nph_eventalign_chain(nph_ctx* ctx,
+                                    const nph_aligned_pair* pairs, size_t n_pairs_total,
+                                    const int32_t* event_map_start, size_t n_map_total,
+                                    const uint32_t* ref_ranks_fwd, const uint32_t* ref_ranks_rc, size_t n_ranks_total,
+                                    const nph_ea_chain* chains, size_t n_chains, double indel_bias,
+                                    nph_ea_record* records_out, size_t records_total, nph_ea_result* results_out)
+{
+    if (!records_out && records_total) return NPH_ERR_INVALID;
+    NPH_TRY(nph_eventalign_chain_run(ctx, pairs, n_pairs_total, event_map_start, n_map_total, ref_ranks_fwd, ref_ranks_rc, n_ranks_total,
+                                     chains, n_chains, indel_bias, records_total, results_out));
+    return nph_eventalign_records_fetch(ctx, records_out, records_total);
 }

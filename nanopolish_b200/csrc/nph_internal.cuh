@@ -134,6 +134,23 @@ struct nph_ctx {
     uint64_t abea_trace_stride = 0;
     bool abea_loaded = false;
 
+    // the records of the last nph_eventalign_chain_run, where the kernel wrote them in d_align_scratch (eventalign_chain.cu), and
+    // the buffers of nph_eventalign_tsv (eventalign_tsv.cu)
+    struct EaState {
+        bool resident = false;             // dropped by nph_carve_align_scratch, nph_abea_stage and nph_reads_resident
+        size_t records_total = 0, n_ranks = 0;
+        const nph_ea_chain* d_chains = nullptr;
+        const nph_ea_record* d_records = nullptr;
+        const nph_ea_result* d_results = nullptr;
+        const uint32_t* d_ranks_fwd = nullptr;
+        const uint32_t* d_ranks_rc = nullptr;
+        std::vector<nph_ea_chain> h_chains;
+        std::vector<nph_ea_result> h_results;
+        DevBuf<uint8_t> d_tsv_in;          // names, reference characters, event and sample arrays, per-read and per-chain tables
+        DevBuf<uint8_t> d_tsv_off;         // bytes of each row, their exclusive prefix, the refusal flags
+        DevBuf<uint8_t> d_tsv;             // the rows
+    } ea;
+
     // resident call-methylation batch (methylation.cu)
     struct MethState {
         bool loaded = false, ran = false;
@@ -250,11 +267,13 @@ int nph_carve(nph_ctx* ctx, DevBuf<uint8_t>& buf, Layout&& layout)
     layout(a);
     return NPH_OK;
 }
-// Carve the alignment scratch for a call other than ABEA: the staged ABEA batch keeps its band trace there, so it is dropped.
+// Carve the alignment scratch for a call other than ABEA: the staged ABEA batch keeps its band trace there and an eventalign
+// chain run its records, so both are dropped.
 template <typename Layout>
 int nph_carve_align_scratch(nph_ctx* ctx, Layout&& layout)
 {
     ctx->abea_loaded = false;
+    ctx->ea.resident = false;
     return nph_carve(ctx, ctx->d_align_scratch, layout);
 }
 
@@ -286,8 +305,8 @@ inline void nph_timing_staged(nph_ctx* ctx, float ms, int launches)
     ctx->staged_ms = ms; ctx->last_launches = launches; ctx->timing = nph_ctx::Timing::Staged;
 }
 
-// A new read batch is resident: the HMM and ABEA jobs of the previous one no longer apply.
-inline void nph_reads_resident(nph_ctx* ctx) { ctx->reads_loaded = true; ctx->jobs_loaded = false; ctx->abea_loaded = false; }
+// A new read batch is resident: the HMM and ABEA jobs and the eventalign records of the previous one no longer apply.
+inline void nph_reads_resident(nph_ctx* ctx) { ctx->reads_loaded = true; ctx->jobs_loaded = false; ctx->abea_loaded = false; ctx->ea.resident = false; }
 
 #ifdef __CUDACC__
 // get_scaled_gaussian_from_pore_model_state (ref: src/nanopolish_squiggle_read.h:217-226) of k-mer rank r, formed in FP64 and

@@ -310,6 +310,59 @@ class Engine:
                                                   indel_bias, _p(records), total, _p(results)), "nph_eventalign_chain")
         return records, results
 
+    def eventalign_chain_run(self, pairs, event_map_start, ref_ranks_fwd, ref_ranks_rc, chains, indel_bias: float = 1.0):
+        """nph_eventalign_chain_run: the chains walked as eventalign_chain walks them, the records left on the device for
+        eventalign_tsv / eventalign_records_fetch.  Returns results EA_RESULT_DT[n_chains]."""
+        from .synth import EA_RESULT_DT
+        n = chains.shape[0]
+        total = int((chains["out_off"] + chains["out_cap"]).max()) if n else 0
+        results = np.zeros(n, EA_RESULT_DT)
+        self._check(self.lib.nph_eventalign_chain_run(self.ctx, _p(pairs), pairs.shape[0], _p(event_map_start), event_map_start.shape[0],
+                                                      _p(ref_ranks_fwd), _p(ref_ranks_rc), ref_ranks_fwd.shape[0], _p(chains), n,
+                                                      indel_bias, total, _p(results)), "nph_eventalign_chain_run")
+        return results
+
+    def eventalign_records_fetch(self, records_total: int):
+        from .synth import EA_RECORD_DT
+        records = np.zeros(records_total, EA_RECORD_DT)
+        self._check(self.lib.nph_eventalign_records_fetch(self.ctx, _p(records), records_total), "nph_eventalign_records_fetch")
+        return records
+
+    def eventalign_tsv(self, inputs: dict, print_read_names=False, scale_events=False, signal_index=False, samples=False,
+                       out: np.ndarray | None = None, want_row_off: int = 0):
+        """nph_eventalign_tsv: the eventalign.tsv rows of the last eventalign_chain_run, written on the device.  inputs: what
+        synth.eventalign_tsv_inputs builds (reads EA_TSV_READ_DT, chain_read, text, ref, rc_ref, ev_mean, ev_stdv, ev_duration,
+        ev_start_time, samples).  out: a caller-owned (page-locked) uint8 buffer; without one the call is made twice, the
+        first time for the size.  want_row_off: the number of rows, to get their offsets too.  Returns (bytes, read_off u8[n_reads
+        + 1], refused u1[n_reads], row_off or None)."""
+        class Batch(C.Structure):
+            _fields_ = [("reads", C.c_void_p), ("n_reads", C.c_size_t), ("chain_read", C.c_void_p), ("text", C.c_void_p), ("n_text", C.c_size_t),
+                        ("ref", C.c_void_p), ("rc_ref", C.c_void_p), ("n_ref", C.c_size_t), ("ev_mean", C.c_void_p), ("ev_stdv", C.c_void_p),
+                        ("ev_duration", C.c_void_p), ("ev_start_time", C.c_void_p), ("n_events", C.c_size_t), ("samples", C.c_void_p),
+                        ("n_samples", C.c_size_t)]
+        i = inputs
+        adr = lambda a: a.ctypes.data if a is not None and a.size else None
+        b = Batch(adr(i["reads"]), i["reads"].shape[0], adr(i["chain_read"]), adr(i["text"]), i["text"].shape[0], adr(i["ref"]), adr(i["rc_ref"]),
+                  i["ref"].shape[0], adr(i["ev_mean"]), adr(i["ev_stdv"]), adr(i["ev_duration"]), adr(i.get("ev_start_time")), i["ev_mean"].shape[0],
+                  adr(i.get("samples")), i["samples"].shape[0] if i.get("samples") is not None else 0)
+        opt = np.array([print_read_names, scale_events, signal_index, samples], np.uint8)
+        nr = i["reads"].shape[0]
+        read_off, refused = np.zeros(nr + 1, np.uint64), np.zeros(nr, np.uint8)
+        row_off = np.zeros(want_row_off + 1, np.uint64) if want_row_off else None
+        n = C.c_uint64(0)
+
+        def call(buf):
+            return self.lib.nph_eventalign_tsv(self.ctx, C.byref(b), _p(opt), _p(buf) if buf is not None else None, buf.shape[0] if buf is not None else 0,
+                                               _p(row_off) if row_off is not None else None, _p(read_off), _p(refused), C.byref(n))
+        if out is None:
+            rc = call(None)
+            if rc == 0 or n.value == 0:                      # no rows, or an error that is not about room
+                self._check(rc, "nph_eventalign_tsv")
+                return b"", read_off, refused, row_off
+            out = np.empty(n.value, np.uint8)
+        self._check(call(out), "nph_eventalign_tsv")
+        return out[:n.value].tobytes(), read_off, refused, row_off
+
     # ---- ABEA ---------------------------------------------------------------------------
     def abea_batch(self, reads, ev_mean, ev_start_time, kmer_ranks, jobs, model_id: int, pairs_total: int):
         pairs = np.zeros(pairs_total, PAIR_DT)

@@ -140,6 +140,7 @@ static const int OUTPUT_STRIDE = 50;     // approximately how many event alignme
 void EventAligner::clear()
 {
     m_reads.clear(); m_round.clear(); m_batch.clear();
+    m_lazy = Lazy();
 }
 
 size_t EventAligner::add_read(const EventAlignmentParameters& params)
@@ -318,22 +319,16 @@ size_t EventAligner::run_rounds(Engine& engine, double indel_bias)
     return rounds;
 }
 
-// ref_seq's k-mer at offset pos and what HMMInputSequence::get_kmer hands the model for it: the k-mer itself, or for rc
-// reads rc_subseq.substr(l - kmer_idx - k, k) == rc_ref_seq.substr(n - pos - k, k)
+// the k-mer columns of a record (nph_tsv::ea_kmers_at, the statement the device writer uses too), NUL-terminated
 void EventAligner::kmers_at(const ReadState& rs, const Rec& r, char* ref_kmer, char* model_kmer)
 {
-    const size_t k = rs.k, n = rs.ref_seq.size();
-    const size_t pos = (size_t)(r.ref_position - rs.params.ref_pos);
-    size_t len = pos <= n ? std::min(k, n - pos) : 0;          // std::string::substr clips at the end
-    std::memcpy(ref_kmer, rs.ref_seq.data() + (len ? pos : 0), len);
-    ref_kmer[len] = 0;
-    if (r.state == 'B') {
-        std::memset(model_kmer, 'N', k);
-    } else {
-        const bool rc = rs.params.strand_idx == 0 ? rs.do_base_rc : !rs.do_base_rc;
-        std::memcpy(model_kmer, rc ? rs.rc_ref_seq.data() + (n - pos - k) : rs.ref_seq.data() + pos, k);   // inside the window: always k long
-    }
-    model_kmer[k] = 0;
+    const bool rc = rs.params.strand_idx == 0 ? rs.do_base_rc : !rs.do_base_rc;
+    const nph_tsv::EaKmers km = nph_tsv::ea_kmers_at(rs.ref_seq.data(), rs.rc_ref_seq.data(), rs.ref_seq.size(),
+                                                     (size_t)(r.ref_position - rs.params.ref_pos), rs.k, rc, r.state);
+    std::memcpy(ref_kmer, km.ref_kmer, km.ref_kmer_len);
+    ref_kmer[km.ref_kmer_len] = 0;
+    if (km.model_kmer) std::memcpy(model_kmer, km.model_kmer, rs.k); else std::memset(model_kmer, 'N', rs.k);
+    model_kmer[rs.k] = 0;
 }
 
 EventAlignment EventAligner::materialize(const ReadState& rs, const Rec& r) const
@@ -355,6 +350,7 @@ EventAlignment EventAligner::materialize(const ReadState& rs, const Rec& r) cons
 
 std::vector<EventAlignment> EventAligner::alignment(size_t read_idx) const
 {
+    ensure_records();
     const ReadState& rs = m_reads[read_idx];
     std::vector<EventAlignment> out;
     out.reserve(rs.output.size());
@@ -362,9 +358,135 @@ std::vector<EventAlignment> EventAligner::alignment(size_t read_idx) const
     return out;
 }
 
-size_t EventAligner::run(Engine& engine, double indel_bias)
+size_t EventAligner::run(Engine& engine, double indel_bias) { return run_device(engine, indel_bias, nullptr, nullptr); }
+
+EventalignTsv EventAligner::run_tsv(Engine& engine, double indel_bias, const EventalignOptions& opt)
+{
+    for (const ReadState& rs : m_reads) require_samples(*rs.params.sr, opt);
+    EventalignTsv out;
+    out.batches = run_device(engine, indel_bias, &opt, &out);
+    return out;
+}
+
+void EventAligner::require_samples(const SquiggleRead& sr, const EventalignOptions& opt)
+{
+    if ((opt.write_signal_index || opt.write_samples) && sr.samples.empty())
+        throw Error(NPH_ERR_STATE, "--signal-index / --samples need the raw samples on the read (load_from_raw with SRF_LOAD_RAW_SAMPLES)");
+}
+
+// Copies the records of the last chain run into the reads' output vectors: chains [chain_first[i], chain_first[i + 1]) are read i's.
+void EventAligner::scatter(const nph_ea_record* records, const std::vector<nph_ea_chain>& chains, const std::vector<nph_ea_result>& results,
+                           const std::vector<uint64_t>& chain_first, const std::vector<char>& skip)
+{
+#pragma omp parallel for schedule(dynamic, 8) num_threads(host_threads())
+    for (long long i = 0; i < (long long)m_reads.size(); ++i) {
+        if (skip[i] || chain_first[i] == chain_first[i + 1]) continue;
+        ReadState& rs = m_reads[i];
+        size_t total = 0;
+        for (size_t c = chain_first[i]; c < chain_first[i + 1]; ++c) total += results[c].n_records;
+        rs.output.reserve(rs.output.size() + total);
+        for (size_t c = chain_first[i]; c < chain_first[i + 1]; ++c) {
+            const nph_ea_record* r = records + chains[c].out_off;
+            for (uint32_t j = 0; j < results[c].n_records; ++j) rs.output.push_back(Rec{r[j].ref_position, r[j].event_idx, (char)r[j].hmm_state});
+            rs.segments_aligned += results[c].n_windows;
+        }
+    }
+}
+
+void EventAligner::ensure_records() const
+{
+    if (!m_lazy.engine) return;
+    EventAligner* self = const_cast<EventAligner*>(this);
+    Engine& engine = *m_lazy.engine;
+    self->m_lazy.engine = nullptr;
+    nph_ea_record* const records = static_cast<nph_ea_record*>(
+        engine.pinned(Engine::Staging::EventalignRecords, sizeof(nph_ea_record) * std::max<uint64_t>(m_lazy.records_total, 1)));
+    engine.check(nph_eventalign_records_fetch(engine.ctx(), records, m_lazy.records_total), "nph_eventalign_records_fetch (the engine has run another alignment since run_tsv)");
+    self->scatter(records, m_lazy.chains, m_lazy.results, m_lazy.chain_first, std::vector<char>(m_reads.size(), 0));
+    self->m_lazy = Lazy();
+}
+
+// What nph_eventalign_tsv needs beyond the resident records, staged in page-locked memory; then the call.  Returns the device's
+// bytes (in the engine's staging) with read_off and refused filled.
+const char* EventAligner::device_tsv(Engine& engine, const EventalignOptions& opt, const std::vector<uint64_t>& chain_first,
+                                     const std::vector<size_t>& owner, std::vector<uint64_t>& read_off, std::vector<uint8_t>& refused)
 {
     const size_t nr = m_reads.size();
+    const bool sample_idx = opt.write_signal_index || opt.write_samples;
+    std::vector<nph_ea_tsv_read> tr(nr);
+    uint64_t n_text = 0, n_ref = 0, n_events = 0, n_samples = 0;
+    for (size_t i = 0; i < nr; ++i) {
+        const ReadState& rs = m_reads[i];
+        const SquiggleRead& sr = *rs.params.sr;
+        nph_ea_tsv_read& t = tr[i];
+        std::memset(&t, 0, sizeof(t));
+        if (chain_first[i] == chain_first[i + 1]) continue;            // no chain, no row: empty slices
+        t.contig_off = n_text; t.contig_len = (uint32_t)rs.params.ref_name.size(); n_text += t.contig_len;
+        t.name_off = n_text; t.name_len = (uint32_t)sr.read_name.size(); n_text += t.name_len;
+        t.ref_off = n_ref; t.ref_len = (uint32_t)rs.ref_seq.size(); n_ref += t.ref_len;
+        t.event_off = n_events; t.n_events = (uint32_t)sr.events[rs.params.strand_idx].size(); n_events += t.n_events;
+        if (opt.write_samples) { t.sample_off = n_samples; t.n_samples = sr.samples.size(); n_samples += t.n_samples; }
+        t.read_idx = (uint64_t)(size_t)rs.params.read_idx;
+        t.sample_start_time = sr.sample_start_time; t.sample_rate = sr.sample_rate;
+        t.drift = sr.scalings[rs.params.strand_idx].drift;
+        t.strand_idx = (uint32_t)rs.params.strand_idx;
+    }
+    // one staging block: start times | means | stdv | durations | samples | text | ref | rc_ref
+    const size_t b_time = sizeof(double) * (sample_idx ? n_events : 0), b_f = sizeof(float) * n_events;
+    char* const in = static_cast<char*>(engine.pinned(Engine::Staging::EventalignTsvIn, b_time + 3 * b_f + sizeof(float) * n_samples + n_text + 2 * n_ref + 8));
+    double* const time = reinterpret_cast<double*>(in);
+    float* const mean = reinterpret_cast<float*>(in + b_time);
+    float* const stdv = mean + n_events;
+    float* const dur = stdv + n_events;
+    float* const samples = dur + n_events;
+    char* const text = reinterpret_cast<char*>(samples + n_samples);
+    char* const ref = text + n_text;
+    char* const rc_ref = ref + n_ref;
+    parallel_for(nr, host_threads(), 8, [&](size_t i) {
+        const nph_ea_tsv_read& t = tr[i];
+        if (chain_first[i] == chain_first[i + 1]) return;
+        const ReadState& rs = m_reads[i];
+        const SquiggleRead& sr = *rs.params.sr;
+        const std::vector<SquiggleEvent>& ev = sr.events[rs.params.strand_idx];
+        for (size_t e = 0; e < ev.size(); ++e) {
+            mean[t.event_off + e] = ev[e].mean; stdv[t.event_off + e] = ev[e].stdv; dur[t.event_off + e] = ev[e].duration;
+            if (sample_idx) time[t.event_off + e] = ev[e].start_time;
+        }
+        if (opt.write_samples) std::memcpy(samples + t.sample_off, sr.samples.data(), sizeof(float) * sr.samples.size());
+        std::memcpy(text + t.contig_off, rs.params.ref_name.data(), t.contig_len);
+        std::memcpy(text + t.name_off, sr.read_name.data(), t.name_len);
+        std::memcpy(ref + t.ref_off, rs.ref_seq.data(), t.ref_len);
+        std::memcpy(rc_ref + t.ref_off, rs.rc_ref_seq.data(), t.ref_len);
+    });
+    std::vector<uint32_t> chain_read(owner.size());
+    for (size_t c = 0; c < owner.size(); ++c) chain_read[c] = (uint32_t)owner[c];
+    nph_ea_tsv_batch b;
+    std::memset(&b, 0, sizeof(b));
+    b.reads = tr.data(); b.n_reads = nr; b.chain_read = chain_read.data();
+    b.text = text; b.n_text = n_text; b.ref = ref; b.rc_ref = rc_ref; b.n_ref = n_ref;
+    b.ev_mean = mean; b.ev_stdv = stdv; b.ev_duration = dur; b.ev_start_time = sample_idx ? time : nullptr; b.n_events = n_events;
+    b.samples = opt.write_samples ? samples : nullptr; b.n_samples = n_samples;
+    const nph_ea_tsv_options o{opt.print_read_names, opt.scale_events, opt.write_signal_index, opt.write_samples};
+    read_off.assign(nr + 1, 0);
+    refused.assign(nr, 0);
+    // the staging of the previous batch is usually large enough; when it is not, the call reports the bytes it needs
+    size_t cap = 0;
+    char* buf = static_cast<char*>(engine.pinned_if_any(Engine::Staging::EventalignTsv, &cap));
+    uint64_t n_bytes = 0;
+    int rc = nph_eventalign_tsv(engine.ctx(), &b, &o, buf, cap, nullptr, read_off.data(), refused.data(), &n_bytes);
+    if (rc == NPH_ERR_INVALID && n_bytes > cap) {
+        buf = static_cast<char*>(engine.pinned(Engine::Staging::EventalignTsv, (size_t)n_bytes));
+        rc = nph_eventalign_tsv(engine.ctx(), &b, &o, buf, (size_t)n_bytes, nullptr, read_off.data(), refused.data(), &n_bytes);
+    }
+    engine.check(rc, "nph_eventalign_tsv");
+    return buf;
+}
+
+size_t EventAligner::run_device(Engine& engine, double indel_bias, const EventalignOptions* tsv_opt, EventalignTsv* tsv_out)
+{
+    m_lazy = Lazy();
+    const size_t nr = m_reads.size();
+    if (tsv_out) { tsv_out->read_off.assign(nr + 1, 0); tsv_out->on_host.assign(nr, 0); }
     // ---- phase 1 (parallel over reads): trims and start/stop events of every BAM segment, up to the first segment
     //      that trims to nothing (where the reference returns from align_read_to_ref) ----
     std::vector<std::vector<SegmentStart>> starts(nr);
@@ -467,13 +589,10 @@ size_t EventAligner::run(Engine& engine, double indel_bias)
     // ---- the device: reads up, one launch, records back ----
     const detail::FlatReads fr = detail::flatten_reads(engine, read_table);
     engine.check(nph_reads_load(engine.ctx(), fr.reads.data(), fr.reads.size(), fr.mean, fr.time, fr.n_events), "nph_reads_load");
-    nph_ea_record* const records = static_cast<nph_ea_record*>(
-        engine.pinned(Engine::Staging::EventalignRecords, sizeof(nph_ea_record) * std::max<uint64_t>(records_total, 1)));
     std::vector<nph_ea_result> results(n_chains);
-    engine.check(nph_eventalign_chain(engine.ctx(), pairs.data(), pairs.size(), map_start.data(), map_start.size(), ranks_fwd.data(),
-                                      ranks_rc.data(), ranks_fwd.size(), chains.data(), n_chains, indel_bias, records, records_total,
-                                      results.data()),
-                 "nph_eventalign_chain");
+    engine.check(nph_eventalign_chain_run(engine.ctx(), pairs.data(), pairs.size(), map_start.data(), map_start.size(), ranks_fwd.data(),
+                                          ranks_rc.data(), ranks_fwd.size(), chains.data(), n_chains, indel_bias, records_total, results.data()),
+                 "nph_eventalign_chain_run");
 
     // ---- scatter (parallel over reads); a read with a window the chain kernel could not hold goes through the round
     //      driver instead ----
@@ -485,28 +604,54 @@ size_t EventAligner::run(Engine& engine, double indel_bias)
         if (st & NPH_EA_OUT_OVERFLOW) throw Error(NPH_ERR_STATE, "eventalign chain: record room exceeded");
         if (st & NPH_EA_WINDOW_TOO_LARGE) redo[owner[c]] = 1;
     }
-#pragma omp parallel for schedule(dynamic, 8) num_threads(host_threads())
-    for (long long i = 0; i < (long long)nr; ++i) {
-        if (redo[i] || starts[i].empty()) continue;
-        ReadState& rs = m_reads[i];
-        size_t total = 0;
-        for (size_t c = chain_first[i]; c < chain_first[i + 1]; ++c) total += results[c].n_records;
-        rs.output.reserve(rs.output.size() + total);
-        for (size_t c = chain_first[i]; c < chain_first[i + 1]; ++c) {
-            const nph_ea_record* r = records + chains[c].out_off;
-            for (uint32_t j = 0; j < results[c].n_records; ++j) rs.output.push_back(Rec{r[j].ref_position, r[j].event_idx, (char)r[j].hmm_state});
-            rs.segments_aligned += results[c].n_windows;
-        }
-    }
     size_t n_redo = 0;
+    for (size_t i = 0; i < nr; ++i) n_redo += redo[i] != 0;
+    // the rows, where the records are: every read but those the writer refuses or the round driver re-runs
+    const char* dev_text = nullptr;
+    std::vector<uint64_t> dev_off;
+    std::vector<uint8_t> refused;
+    bool any_refused = false;
+    if (tsv_opt) {
+        dev_text = device_tsv(engine, *tsv_opt, chain_first, owner, dev_off, refused);
+        for (size_t i = 0; i < nr; ++i) any_refused = any_refused || (refused[i] && !redo[i]);
+    }
+    if (tsv_opt && !n_redo && !any_refused) {
+        // nothing needs the records on the host now: they are fetched if alignment(), sam() or summarize() ask
+        m_lazy.engine = &engine; m_lazy.records_total = records_total;
+        m_lazy.chains.swap(chains); m_lazy.results.swap(results); m_lazy.chain_first = chain_first;
+        tsv_out->m_view = dev_text; tsv_out->m_size = (size_t)dev_off[nr]; tsv_out->read_off = dev_off;
+        return 1;
+    }
+    nph_ea_record* const records = static_cast<nph_ea_record*>(
+        engine.pinned(Engine::Staging::EventalignRecords, sizeof(nph_ea_record) * std::max<uint64_t>(records_total, 1)));
+    engine.check(nph_eventalign_records_fetch(engine.ctx(), records, records_total), "nph_eventalign_records_fetch");
+    scatter(records, chains, results, chain_first, redo);
     for (size_t i = 0; i < nr; ++i) {
         if (!redo[i]) continue;
         ReadState& rs = m_reads[i];
         rs.done = false; rs.in_segment = false; rs.segment_idx = 0; rs.pending = false;
         rs.output.clear(); rs.segments_aligned = 0;
-        ++n_redo;
     }
-    return 1 + (n_redo ? run_rounds(engine, indel_bias) : 0);
+    const size_t batches = 1 + (n_redo ? run_rounds(engine, indel_bias) : 0);
+    if (tsv_opt) {
+        // the reads the device did not write take the host writer; the others keep the device's bytes
+        std::vector<std::string> host_rows(nr);
+        parallel_for(nr, host_threads(), 4, [&](size_t i) { if (redo[i] || refused[i]) host_rows[i] = tsv(i, *tsv_opt); });
+        for (size_t i = 0; i < nr; ++i) {
+            const bool on_host = redo[i] || refused[i];
+            tsv_out->on_host[i] = on_host;
+            tsv_out->read_off[i + 1] = tsv_out->read_off[i] + (on_host ? host_rows[i].size() : dev_off[i + 1] - dev_off[i]);
+        }
+        tsv_out->m_owned.resize((size_t)tsv_out->read_off[nr]);
+        parallel_for(nr, host_threads(), 4, [&](size_t i) {
+            if (tsv_out->read_off[i + 1] == tsv_out->read_off[i]) return;
+            char* dst = &tsv_out->m_owned[0] + tsv_out->read_off[i];
+            if (tsv_out->on_host[i]) std::memcpy(dst, host_rows[i].data(), host_rows[i].size());
+            else std::memcpy(dst, dev_text + dev_off[i], (size_t)(dev_off[i + 1] - dev_off[i]));
+        });
+        tsv_out->m_view = nullptr; tsv_out->m_size = tsv_out->m_owned.size();
+    }
+    return batches;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -528,6 +673,7 @@ std::string EventAligner::tsv_header(const EventalignOptions& opt)
 
 std::string EventAligner::tsv(size_t read_idx, const EventalignOptions& opt) const
 {
+    ensure_records();
     const ReadState& rs = m_reads[read_idx];
     const SquiggleRead& sr = *rs.params.sr;
     const PoreModel* pore_model = rs.pore_model;
@@ -537,8 +683,7 @@ std::string EventAligner::tsv(size_t read_idx, const EventalignOptions& opt) con
     // the read column: read_idx as %zu, or the read name with -n
     const std::string who_s = opt.print_read_names ? sr.read_name : std::to_string((size_t)rs.params.read_idx);
     const double sqrt_var = std::sqrt(sr.scalings[strand].var);
-    if ((opt.write_signal_index || opt.write_samples) && sr.samples.empty())
-        throw Error(NPH_ERR_STATE, "--signal-index / --samples need the raw samples on the read (load_from_raw with SRF_LOAD_RAW_SAMPLES)");
+    require_samples(sr, opt);
     // room per row: six numbers of at most 47 characters; with the sample columns, 16 characters per raw sample of the
     // events written (%g, six significant digits) + two indices
     size_t extra = 0;
@@ -552,58 +697,62 @@ std::string EventAligner::tsv(size_t read_idx, const EventalignOptions& opt) con
     out.resize(rs.output.size() * (ref_name.size() + who_s.size() + 2 * (size_t)k + 340) + extra);
     char* const base = &out[0];
     char* o = base;
-    char ref_kmer[64], model_kmer[64];
+    const bool rc = rs.params.strand_idx == 0 ? rs.do_base_rc : !rs.do_base_rc;
+    const bool sample_idx = opt.write_signal_index || opt.write_samples;
+    const SquiggleScalings& sc = sr.scalings[strand];
+    const nph_tsv::EaRead rd{sc.scale, sc.shift, sc.drift, sc.var, sqrt_var, sr.sample_rate, sr.sample_start_time};
+    nph_tsv::EaRow w;
+    w.contig = ref_name.data(); w.contig_len = (uint32_t)ref_name.size();
+    w.k = k;
+    w.name = opt.print_read_names ? who_s.data() : nullptr; w.name_len = (uint32_t)who_s.size();
+    w.read_idx = (uint64_t)(size_t)rs.params.read_idx;
+    w.strand = "tc"[strand];
+    w.signal_index = opt.write_signal_index;
     for (const Rec& r : rs.output) {
-        kmers_at(rs, r, ref_kmer, model_kmer);
-        // contig, position, reference_kmer, read, strand
-        o = put_str(o, ref_name.data(), ref_name.size()); *o++ = '\t';
-        o = put_i64(o, r.ref_position); *o++ = '\t';
-        o = put_str(o, ref_kmer, std::strlen(ref_kmer)); *o++ = '\t';
-        o = put_str(o, who_s.data(), who_s.size()); *o++ = '\t';
-        *o++ = "tc"[strand]; *o++ = '\t';
-
-        float event_mean = sr.get_unscaled_level(r.event_idx, strand);
-        const float event_stdv = sr.get_stdv(r.event_idx, strand);
-        const float event_duration = sr.get_duration(r.event_idx, strand);
-        float model_mean = 0.0, model_stdv = 0.0;
-        if (opt.scale_events) {
-            // scale reads to the model; unscaled model parameters
-            event_mean = sr.get_fully_scaled_level(r.event_idx, strand);
-            if (r.state != 'B') {
-                const PoreModelStateParams model = pore_model->get_parameters(pore_model->pmalphabet->kmer_rank(model_kmer, k));
-                model_mean = (float)model.level_mean;
-                model_stdv = (float)model.level_stdv;
+        // the row rule of csrc/tsv_format.cuh, shared with the device writer
+        w.kmers = nph_tsv::ea_kmers_at(rs.ref_seq.data(), rs.rc_ref_seq.data(), rs.ref_seq.size(), (size_t)(r.ref_position - rs.params.ref_pos),
+                                       k, rc, r.state);
+        w.ref_position = r.ref_position;
+        w.event_idx = r.event_idx;
+        PoreModelStateParams model;
+        if (r.state != 'B') model = pore_model->get_parameters(pore_model->pmalphabet->kmer_rank(w.kmers.model_kmer, k));
+        const SquiggleEvent& ev = sr.events[strand][r.event_idx];
+        const nph_tsv::EaRowNums n = nph_tsv::ea_row_numbers(ev.mean, opt.scale_events ? sr.get_drift_scaled_level(r.event_idx, strand) : 0.0f, ev.stdv,
+                                                             ev.duration, ev.start_time, r.state, model.level_mean, model.level_stdv, rd,
+                                                             opt.scale_events, sample_idx);
+        if (n.ok) {
+            o = nph_tsv::put_ea_row(o, w, n);
+        } else {
+            // a value the exact formatter does not take: this row through the C library
+            o = put_str(o, ref_name.data(), ref_name.size()); *o++ = '\t';
+            o = put_i64(o, r.ref_position); *o++ = '\t';
+            o = put_str(o, w.kmers.ref_kmer, w.kmers.ref_kmer_len); *o++ = '\t';
+            o = put_str(o, who_s.data(), who_s.size()); *o++ = '\t';
+            *o++ = w.strand; *o++ = '\t';
+            o = put_i64(o, r.event_idx); *o++ = '\t';
+            o += format_fixed(o, n.event_mean, 2); *o++ = '\t';
+            o += format_fixed(o, ev.stdv, 3); *o++ = '\t';
+            o += format_fixed(o, ev.duration, 5); *o++ = '\t';
+            if (w.kmers.model_kmer) o = put_str(o, w.kmers.model_kmer, k); else { std::memset(o, 'N', k); o += k; }
+            *o++ = '\t';
+            o += format_fixed(o, n.model_mean, 2); *o++ = '\t';
+            o += format_fixed(o, n.model_stdv, 2); *o++ = '\t';
+            o += format_fixed(o, n.standard_level, 2);
+            if (opt.write_signal_index) {
+                const std::pair<size_t, size_t> si = sr.get_event_sample_idx(strand, r.event_idx);
+                o += snprintf(o, 48, "\t%zu\t%zu", si.first, si.second);
             }
-        } else if (r.state != 'B') {
-            // scale model to the reads
-            const GaussianParameters model = sr.get_scaled_gaussian_from_pore_model_state(*pore_model, strand, pore_model->pmalphabet->kmer_rank(model_kmer, k));
-            model_mean = model.mean;
-            model_stdv = model.stdv;
-        }
-        // float difference over a double product, narrowed to float (a 'B' state divides by zero: inf, like the reference)
-        const float standard_level = (float)((event_mean - model_mean) / (sqrt_var * model_stdv));
-        // event_index %d, event_level_mean %.2lf, event_stdv %.3lf, event_length %.5lf
-        o = put_i64(o, r.event_idx); *o++ = '\t';
-        o += format_fixed(o, event_mean, 2); *o++ = '\t';
-        o += format_fixed(o, event_stdv, 3); *o++ = '\t';
-        o += format_fixed(o, event_duration, 5); *o++ = '\t';
-        // model_kmer, model_mean %.2lf, model_stdv %.2lf, standardized_level %.2lf
-        o = put_str(o, model_kmer, k); *o++ = '\t';
-        o += format_fixed(o, model_mean, 2); *o++ = '\t';
-        o += format_fixed(o, model_stdv, 2); *o++ = '\t';
-        o += format_fixed(o, standard_level, 2);
-        if (opt.write_signal_index) {
-            const std::pair<size_t, size_t> si = sr.get_event_sample_idx(strand, r.event_idx);
-            *o++ = '\t'; o = put_i64(o, (int64_t)si.first); *o++ = '\t'; o = put_i64(o, (int64_t)si.second);
         }
         if (opt.write_samples) {
             // the reference streams the floats through an ostream (%g, 6 significant digits) with ',' after each and
             // drops the last comma (an event without samples makes it resize() to npos and throw; here: an empty column)
-            const std::vector<float> samples = sr.get_scaled_samples_for_event(strand, r.event_idx);
+            const std::pair<size_t, size_t> si = sr.get_event_sample_idx(strand, r.event_idx);
             *o++ = '\t';
-            for (size_t i = 0; i < samples.size(); ++i) {
-                if (i) *o++ = ',';
-                o += snprintf(o, 32, "%g", (double)samples[i]);
+            for (size_t i = si.first; i < si.second; ++i) {
+                if (i != si.first) *o++ = ',';
+                const float v = nph_tsv::ea_scaled_sample(sr.samples.at(i), i, rd);
+                const nph_tsv::G6 g = nph_tsv::g6_of(v);
+                if (g.ok) o = nph_tsv::put_g6(o, g); else o += snprintf(o, 32, "%g", (double)v);
             }
         }
         *o++ = '\n';
@@ -614,6 +763,7 @@ std::string EventAligner::tsv(size_t read_idx, const EventalignOptions& opt) con
 
 std::vector<std::string> EventAligner::tsv_batch(const EventalignOptions& opt) const
 {
+    ensure_records();
     std::vector<std::string> out(m_reads.size());
     // rows of different reads are independent; the reference formats them one read at a time inside an omp critical
     parallel_for(m_reads.size(), host_threads(), 4, [&](size_t i) { out[i] = tsv(i, opt); });
@@ -664,6 +814,7 @@ std::string EventAligner::event_cigar(size_t read_idx) const
 
 std::string EventAligner::sam(size_t read_idx) const
 {
+    ensure_records();
     const ReadState& rs = m_reads[read_idx];
     const std::vector<Rec>& al = rs.output;
     if (al.empty()) return std::string();
@@ -677,6 +828,7 @@ std::string EventAligner::sam(size_t read_idx) const
 
 EventalignSummary EventAligner::summarize(size_t read_idx) const
 {
+    ensure_records();
     const ReadState& rs = m_reads[read_idx];
     const SquiggleRead& sr = *rs.params.sr;
     EventalignSummary summary;

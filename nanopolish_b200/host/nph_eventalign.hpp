@@ -121,6 +121,23 @@ struct EventalignOptions {               // the reference's command-line switche
     bool write_samples = false;          // --samples: the event's scaled raw samples (both need SquiggleRead::samples)
 };
 
+// What run_tsv returns: the rows of every queued read in one buffer, read i's at [read_off[i], read_off[i + 1]).  When the device
+// wrote every read the bytes are the engine's page-locked staging and stay valid until the next run_tsv on that engine.
+class EventalignTsv {
+public:
+    const char* data() const { return m_view ? m_view : m_owned.data(); }
+    size_t size() const { return m_size; }
+    std::vector<uint64_t> read_off;      // num_reads() + 1
+    std::vector<uint8_t> on_host;        // per read: 1 = formatted by tsv() (refused by the device writer, or aligned by run_rounds)
+    size_t batches = 0;                  // kernel batches issued, as run() counts them
+
+private:
+    friend class EventAligner;
+    const char* m_view = nullptr;
+    size_t m_size = 0;
+    std::string m_owned;
+};
+
 class EventAligner {
 public:
     // queue one read strand; returns its index in this batch
@@ -130,6 +147,11 @@ public:
     // Align every queued read: one launch of the chain kernel; reads with a window too large for its scratch are
     // re-run through run_rounds().  Returns the number of kernel batches issued (1 + fallback rounds).
     size_t run(Engine& engine, double indel_bias = hmm_indel_bias_factor);
+    // run() with the TSV rows written on the device (nph_eventalign_tsv) from the records where the chain kernel left them: the
+    // bytes of tsv_batch(opt) joined, without the records crossing PCIe.  Reads the device writer refuses and reads re-run
+    // through run_rounds() take tsv().  Afterwards alignment(), sam(), summarize() and tsv() fetch the records on first use,
+    // which must come before the engine runs another alignment.  Throws what tsv() throws for a read without raw samples.
+    EventalignTsv run_tsv(Engine& engine, double indel_bias = hmm_indel_bias_factor, const EventalignOptions& opt = EventalignOptions());
     // The host-driven form: rounds of (collect next windows -> one Viterbi launch -> advance cursors) until no read has a
     // window left.  Returns the number of rounds (= the longest read's window count).
     size_t run_rounds(Engine& engine, double indel_bias = hmm_indel_bias_factor);
@@ -142,8 +164,8 @@ public:
     const std::vector<size_t>& round_reads() const { return m_round; }     // read index of each job of the open round
 
     std::vector<EventAlignment> alignment(size_t read_idx) const;          // materialised from the compact records
-    size_t num_alignments(size_t read_idx) const { return m_reads[read_idx].output.size(); }
-    size_t num_segments(size_t read_idx) const { return m_reads[read_idx].segments_aligned; }   // profile_hmm_align calls made
+    size_t num_alignments(size_t read_idx) const { ensure_records(); return m_reads[read_idx].output.size(); }
+    size_t num_segments(size_t read_idx) const { ensure_records(); return m_reads[read_idx].segments_aligned; }   // profile_hmm_align calls made
 
     static std::string tsv_header(const EventalignOptions& opt = EventalignOptions());
     std::string tsv(size_t read_idx, const EventalignOptions& opt = EventalignOptions()) const;
@@ -186,6 +208,22 @@ private:
     bool setup_segment(ReadState& rs, size_t segment_idx, SegmentStart& out);   // trims + start/stop events; false = no pairs left
     EventAlignment materialize(const ReadState& rs, const Rec& r) const;
     static void kmers_at(const ReadState& rs, const Rec& r, char* ref_kmer, char* model_kmer);   // NUL-terminated, k+1 bytes each
+    static void require_samples(const SquiggleRead& sr, const EventalignOptions& opt);
+    size_t run_device(Engine& engine, double indel_bias, const EventalignOptions* tsv_opt, EventalignTsv* tsv_out);
+    void scatter(const nph_ea_record* records, const std::vector<nph_ea_chain>& chains, const std::vector<nph_ea_result>& results,
+                 const std::vector<uint64_t>& chain_first, const std::vector<char>& skip);
+    const char* device_tsv(Engine& engine, const EventalignOptions& opt, const std::vector<uint64_t>& chain_first, const std::vector<size_t>& owner,
+                           std::vector<uint64_t>& read_off, std::vector<uint8_t>& refused);
+    // after run_tsv: the chain run whose records are still on the device
+    struct Lazy {
+        Engine* engine = nullptr;
+        uint64_t records_total = 0;
+        std::vector<nph_ea_chain> chains;
+        std::vector<nph_ea_result> results;
+        std::vector<uint64_t> chain_first;
+    };
+    void ensure_records() const;
+    Lazy m_lazy;
     std::vector<ReadState> m_reads;
     std::vector<size_t> m_round;                          // reads with a pending job, in job order
     AlignBatch m_batch;

@@ -345,8 +345,10 @@ public:
     static Engine& thread_default();                  // lazily created, device from $NPH_DEVICE (default 0)
     void check(int status, const char* what) const;
     // page-locked host staging owned by the engine, grown on demand and reused across calls: one buffer per use
-    enum class Staging { EventalignRecords, EventMeans, StartTimes, MethylationSites, Count };
+    enum class Staging { EventalignRecords, EventMeans, StartTimes, MethylationSites, EventalignTsvIn, EventalignTsv, Count };
     void* pinned(Staging use, size_t bytes);
+    // the buffer of a use as it stands (nullptr and 0 before the first pinned() for it)
+    void* pinned_if_any(Staging use, size_t* bytes) const { *bytes = m_pinned[(int)use].bytes; return m_pinned[(int)use].p; }
 
 private:
     nph_ctx* m_ctx = nullptr;

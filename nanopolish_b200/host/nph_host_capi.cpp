@@ -611,6 +611,50 @@ long long nphh_ea_tsv_all_samples(char* out, size_t cap)
     return ea_tsv_all(opt, out, cap);
 }
 
+static EventalignOptions ea_options(int switches)
+{
+    EventalignOptions opt;
+    opt.print_read_names = (switches & 1) != 0; opt.scale_events = (switches & 2) != 0;
+    opt.write_signal_index = (switches & 4) != 0; opt.write_samples = (switches & 8) != 0;
+    return opt;
+}
+
+// tsv_batch with any switches (1 = -n, 2 = --scale-events, 4 = --signal-index, 8 = --samples), read_off_out: reads + 1 offsets
+long long nphh_ea_tsv_all_opt(int switches, char* out, size_t cap, uint64_t* read_off_out)
+{
+    long long n = -1;
+    int rc = guard([&] {
+        const std::vector<std::string> parts = g_aligner.tsv_batch(ea_options(switches));
+        size_t total = 0;
+        for (size_t i = 0; i < parts.size(); ++i) { if (read_off_out) read_off_out[i] = total; total += parts[i].size(); }
+        if (read_off_out) read_off_out[parts.size()] = total;
+        n = (long long)total;
+        if (!out) return;
+        if (total > cap) throw Error(NPH_ERR_INVALID, "text buffer too small");
+        char* o = out;
+        for (const std::string& s : parts) { std::memcpy(o, s.data(), s.size()); o += s.size(); }
+    });
+    return rc ? rc : n;
+}
+
+// EventAligner::run_tsv: align and write the rows on the device.  out may be NULL (size only); read_off_out: reads + 1 offsets,
+// on_host_out: per read 1 where the host writer filled in, batches_out: kernel batches issued.  Returns the bytes.
+long long nphh_ea_run_tsv(double indel_bias, int switches, char* out, size_t cap, uint64_t* read_off_out, uint8_t* on_host_out, long long* batches_out)
+{
+    long long n = -1;
+    int rc = guard([&] {
+        const EventalignTsv t = g_aligner.run_tsv(Engine::thread_default(), indel_bias, ea_options(switches));
+        if (read_off_out) std::memcpy(read_off_out, t.read_off.data(), sizeof(uint64_t) * t.read_off.size());
+        if (on_host_out) std::memcpy(on_host_out, t.on_host.data(), t.on_host.size());
+        if (batches_out) *batches_out = (long long)t.batches;
+        n = (long long)t.size();
+        if (!out) return;
+        if (t.size() > cap) throw Error(NPH_ERR_INVALID, "text buffer too small");
+        std::memcpy(out, t.data(), t.size());
+    });
+    return rc ? rc : n;
+}
+
 // format_fixed against the C library on n float bit patterns drawn from `seed` (uniform bit patterns, then values
 // near printed-digit ties): returns the number of mismatches
 long long nphh_format_fixed_check(uint64_t seed, size_t n)

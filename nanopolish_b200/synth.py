@@ -44,6 +44,10 @@ EA_CHAIN_DT = np.dtype([("pair_off", "<u8"), ("map_off", "<u8"), ("rank_off", "<
                         ("model_id", "<u4"), ("n_pairs", "<u4"), ("map_len", "<u4"), ("ref_len", "<u4"), ("read_seq_len", "<u4"),
                         ("out_cap", "<u4"), ("ref_offset", "<i4"), ("first_event", "<i4"), ("last_event", "<i4"),
                         ("do_base_rc", "u1"), ("rc", "u1"), ("k", "u1"), ("reserved", "u1")], align=True)
+EA_TSV_READ_DT = np.dtype([("contig_off", "<u8"), ("name_off", "<u8"), ("ref_off", "<u8"), ("event_off", "<u8"), ("sample_off", "<u8"),
+                           ("n_samples", "<u8"), ("read_idx", "<u8"), ("sample_start_time", "<u8"), ("sample_rate", "<f8"), ("drift", "<f8"),
+                           ("contig_len", "<u4"), ("name_len", "<u4"), ("ref_len", "<u4"), ("n_events", "<u4"), ("strand_idx", "<u4"),
+                           ("reserved", "<u4")], align=True)
 EA_RECORD_DT = np.dtype([("ref_position", "<i4"), ("event_idx", "<i4"), ("hmm_state", "S1"), ("reserved", "u1", 3)], align=True)
 EA_RESULT_DT = np.dtype([("n_records", "<u4"), ("n_windows", "<u4"), ("status", "<i4"), ("reserved", "<u4")], align=True)
 assert EA_CHAIN_DT.itemsize == 80 and EA_RECORD_DT.itemsize == 12 and EA_RESULT_DT.itemsize == 16
@@ -476,6 +480,37 @@ def eventalign_chains(rs: ReadSet, model_id: int = 0):
         po += nk; mo += nk; ro += nk; oo += cap
     return (np.ascontiguousarray(np.concatenate(pairs)), np.concatenate(maps), np.concatenate(rf).astype(np.uint32),
             np.concatenate(rr).astype(np.uint32), chains)
+
+
+def eventalign_tsv_inputs(rs: ReadSet, seed: int = 7, with_samples: bool = False, sample_rate: float = 4000.0, contig: str = "chr_synth"):
+    """What nph_eventalign_tsv needs beyond the chain run of eventalign_chains(rs): one output read per chain, named
+    read_<i>, on one contig; stdv and duration per event; with_samples: raw samples at sample_rate whose clock starts at the
+    sample of the read's first event, enough of them to cover every event.  Returns the dict Engine.eventalign_tsv takes."""
+    rng = np.random.default_rng(seed)
+    n = rs.n_reads
+    tr = np.zeros(n, EA_TSV_READ_DT)
+    text, refs, rcs, smp = [contig.encode()], [], [], []
+    t_off, r_off, s_off = len(contig), 0, 0
+    total = int(rs.reads["n_events"].sum())
+    stdv = rng.uniform(0.5, 3.0, total).astype(np.float32)
+    for i in range(n):
+        codes = rs.seq_codes[i]
+        name = f"read_{i}".encode()
+        o, E = int(rs.reads[i]["event_off"]), int(rs.reads[i]["n_events"])
+        t = rs.ev_start_time[o:o + E]
+        first = int(t[0] * sample_rate)
+        tr[i] = (0, t_off, r_off, o, s_off, 0, i, first, sample_rate, float(rs.reads[i]["drift"]), len(contig), len(name), codes.shape[0], E, 0, 0)
+        text.append(name); t_off += len(name)
+        refs.append(_CODE2DNA[codes]); rcs.append(_CODE2DNA[3 - codes[::-1]]); r_off += codes.shape[0]
+        if with_samples:
+            ns = int((t[-1] + 0.01) * sample_rate) - first + 8
+            smp.append(rng.normal(90.0, 12.0, ns).astype(np.float32))
+            tr[i]["n_samples"] = ns; s_off += ns
+    # every event lasts until the next one starts
+    duration = np.full(total, np.float32(0.002))
+    return dict(reads=tr, chain_read=np.arange(n, dtype=np.uint32), text=np.frombuffer(b"".join(text), np.uint8).copy(),
+                ref=np.concatenate(refs), rc_ref=np.concatenate(rcs), ev_mean=rs.ev_mean, ev_stdv=stdv, ev_duration=duration,
+                ev_start_time=rs.ev_start_time, samples=np.concatenate(smp) if with_samples else None)
 
 
 _METH_ALPHABETS = {   # name: (bases, complements, sites, methylated, methylated complement); src/common/nanopolish_alphabet.cpp:15-194
