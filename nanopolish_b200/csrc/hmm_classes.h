@@ -3,8 +3,10 @@
 // A class is (C columns per lane, W lanes per job); 32/W jobs share a warp.  W < 32 classes hold
 // single-strip jobs (K <= W*C); W == 32 also chains strips for wide jobs.  A job goes to the class that
 // minimises modelled issue slots = steps x (per-step overhead + C x per-cell cost) x W/32: 46 per warp step and
-// 67 instructions per block-cell (the steady-state step of hmm_forward_kernel<9|10, 32, false> in cuobjdump -sass,
-// scripts/k1_bounds.py).
+// 67 instructions per block-cell.  These are the steady step of the general row loop of hmm_forward_kernel<9|10, 32, false> before
+// the full-warp single-strip classes streamed their jobs (cuobjdump -sass, scripts/k1_bounds.py), and the general loop still runs
+// every other class.  A streamed job of those classes costs less than the model says: about E steps of 15 + 67 per column plus its
+// transition window (DESIGN.md section 3.4); the model has not been re-fitted to it, so every job keeps the class it had before.
 #pragma once
 #include <stdint.h>
 #include "../../include/nph.h"
@@ -59,7 +61,7 @@ NPH_HD nph_wave_geom nph_wave_geometry(int K, int E, int C, int W, bool may_chai
     return g;
 }
 
-// per-step cost: 46 issue slots of per-step work plus the row update, 67 per column
+// per-step cost: 46 issue slots of per-step work plus the row update, 67 per column (the general row loop; see above)
 NPH_HD float nph_class_cost(uint32_t steps, int C, uint32_t W)
 {
     return (float)steps * (46.0f + 67.0f * C) * (W * (1.0f / 32.0f));

@@ -31,12 +31,16 @@ __global__ void read_prologue_kernel(const DevRead* __restrict__ reads, const do
 
 } // namespace
 
+// Per-warp parameter line: the Gaussians of the widest job, or two lines of 32 * C of a streamed full-warp single-strip job
+// (hmm_forward_kernel.cuh); max_kpad >= 32 * NPH_MAX_COLS.
+static uint32_t params_stride(const nph_ctx* ctx) { return ctx->max_kpad + 32 * NPH_MAX_COLS; }
+
 // One slice per side stream: classes running concurrently on different SMs index their per-warp scratch by
 // (block, warp) and must not share it.
 static void scratch_layout(const nph_ctx* ctx, NphArena& a, float4** params, float** edge)
 {
     const size_t warps = (size_t)ctx->sm_count * kMaxWarpsPerCta;
-    for (int si = 0; si < nph_ctx::kSideStreams; ++si) nph_wave_scratch(a, ctx->max_kpad, ctx->max_period, warps, &params[si], &edge[si]);
+    for (int si = 0; si < nph_ctx::kSideStreams; ++si) nph_wave_scratch(a, params_stride(ctx), ctx->max_period, warps, &params[si], &edge[si]);
 }
 
 size_t nph_hmm_scratch_bytes(const nph_ctx* ctx)
@@ -69,7 +73,7 @@ int nph_launch_hmm_forward(nph_ctx* ctx, float* scores_dev)
     p.logsum_g = ctx->d_logsum.p;
     p.flank = ctx->d_flank.p;
     p.scores = scores_dev ? scores_dev : ctx->d_scores.p;
-    p.kpad_stride = ctx->max_kpad;
+    p.kpad_stride = params_stride(ctx);
     p.edge_stride = nph_edge_stride(ctx->max_period);
     p.c = ctx->consts;
     p.lsum_bias = NPH_LOGSUM_SAT_ADDR_BIAS;

@@ -57,6 +57,222 @@ struct FwdParams {
     HmmConsts c;
 };
 
+// One row of a lane's C columns.  Mp, Bp, Kp, Tp hold the previous row on entry and this row on return (Tp[c] = lp3 + Bp[c]); lm, lt, lk
+// are the left neighbour's M, lp3 + B and K, *_prev of the previous row and *_cur of this one.  With with_soft, column 0's match also
+// folds soft() (the soft-clip start; -inf where it does not apply), in a second copy of column 0 that the usual row branches past.
+template <int C, class SoftFn>
+__device__ __forceinline__ void row_update(const float x, const float (&mu)[C], const float (&sd)[C], const float (&cc)[C], const float (&ry)[C],
+                                           float (&Mp)[C], float (&Bp)[C], float (&Kp)[C], float (&Tp)[C],
+                                           float lm_prev, float lt_prev, float lk_prev, float lm_cur, float lt_cur, float lk_cur,
+                                           const float lp_mm_self, const float lp_mm_next, const HmmConsts& k, const bool with_soft, const SoftFn& soft,
+                                           const LogsumTable& tb)
+{
+    auto cell = [&](const int c, const bool fold_soft) {
+        const float em = log_gauss(x, mu[c], sd[c], cc[c], ry[c]);
+        // match: left fold over {same M, prev M, same B, prev B, prev K, soft}
+        float m = __fadd_rn(lp_mm_self, Mp[c]);
+        m = lsum_sat(m, __fadd_rn(lp_mm_next, lm_prev), tb);
+        m = lsum_sat(m, Tp[c], tb);
+        m = lsum_sat(m, lt_prev, tb);
+        m = lsum_sat(m, __fadd_rn(k.lp_km, lk_prev), tb);
+        if (fold_soft) m = lsum_sat(m, soft(), tb);
+        m = __fadd_rn(m, em);
+        // bad event: {same M, same B}
+        const float b = lsum_sat(__fadd_rn(k.lp_mb, Mp[c]), __fadd_rn(k.lp_bb, Bp[c]), tb);
+        // k-mer skip: {prev M, prev B, prev K} of the SAME row
+        float kk = lsum_sat(__fadd_rn(k.lp_mk, lm_cur), lt_cur, tb);
+        kk = lsum_sat(kk, __fadd_rn(k.lp_kk, lk_cur), tb);
+        const float t = __fadd_rn(k.lp_bk, b);
+
+        lm_prev = Mp[c]; lt_prev = Tp[c]; lk_prev = Kp[c];
+        lm_cur = m; lt_cur = t; lk_cur = kk;
+        Mp[c] = m; Bp[c] = b; Kp[c] = kk; Tp[c] = t;
+    };
+    if (with_soft) cell(0, true);
+    else cell(0, false);
+#pragma unroll
+    for (int c = 1; c < C; ++c) cell(c, false);
+}
+
+// the end-state fold of one row on the lane holding the last k-mer (column end_slot of the lane); post = flank[E - r]
+template <int C>
+__device__ __forceinline__ float end_fold(float lp_end, const float (&Mp)[C], const float (&Bp)[C], const float (&Kp)[C], const int end_slot, const float post,
+                                          const LogsumTable& tb)
+{
+    float Me = Mp[0], Be = Bp[0], Ke = Kp[0];
+#pragma unroll
+    for (int c = 1; c < C; ++c) if (c == end_slot) { Me = Mp[c]; Be = Bp[c]; Ke = Kp[c]; }
+    lp_end = lsum_sat(lp_end, __fadd_rn(Me, post), tb);
+    lp_end = lsum_sat(lp_end, __fadd_rn(Be, post), tb);
+    return lsum_sat(lp_end, __fadd_rn(Ke, post), tb);
+}
+
+// a job record with what its read, read transitions and model hold for it; waits, when levels are still streaming in, until the
+// chunk holding the read's last event has landed (chunks land in order; the progress word is written by a copy queued behind the data)
+struct JobIn { nph_hmm_job job; DevRead rd; float2 tr; DevModelView mv; };
+__device__ __forceinline__ JobIn fetch_job(const FwdParams& p, const uint32_t job_idx, const bool has_job, const int lane)
+{
+    JobIn j;
+    j.job = p.jobs[job_idx];
+    j.rd = p.reads[j.job.read];
+    j.tr = p.trans[j.job.read];
+    j.mv = p.models[j.job.model_id];
+    if (p.progress) {
+        uint32_t need = has_job ? (uint32_t)((j.rd.event_off + j.rd.n_events - 1) / p.chunk_events) + 1u : 0u;
+        need = __reduce_max_sync(kFull, need);
+        if (lane == 0) {
+            const volatile uint32_t* pr = p.progress;
+            while (*pr < need) __nanosleep(500);
+        }
+        __syncwarp();
+    }
+    return j;
+}
+
+// Streamed jobs of the full-warp single-strip classes (W = 32, CHAIN = false).
+//
+// A job with E > 32 rows and neither pre- nor post-clipping runs in three phases: a 33-step window where its lanes enter one by one,
+// E - 33 steady steps where every lane is on a row in 1..E, and a window where its lanes leave.  Lane j of the warp does row E of job n
+// at step t = j of the window and row 1 of job n + 1 the step after, so the leaving window of job n is the entering window of job
+// n + 1, and the warp keeps its wavefront (left neighbour one step ahead on the same job) from job to job.  A warp fills
+// and drains once per stream instead of once per job, and the steady loop carries no per-lane test: three shuffles, the lane-0 edge,
+// one prefetch and the row update.  Lanes whose columns lie wholly beyond K compute on the padding Gaussians there; only lanes further
+// right read their states, and none of them reaches the end fold.
+//
+// The warp keeps pulling jobs from the class counter while they qualify; the first one that does not ends the stream (after the
+// drain) and is returned for the general loop.  The next job's Gaussians are formed after the steady loop, into the other half of the
+// warp's parameter line (two lines of 32 * C, hmm_forward.cu sizes it): the lanes' own Gaussians are read back from their half
+// afterwards instead of being held in registers through the formation, which needs more registers than the row loop leaves.
+__device__ __forceinline__ bool streams(const nph_hmm_job& job, const int E)
+{
+    return E > 32 && (job.flags & (NPH_HAF_ALLOW_PRE_CLIP | NPH_HAF_ALLOW_POST_CLIP)) == 0;
+}
+
+// what the windows need of a streamed job.  It sits in shared memory, two per warp (the leaving and the entering job), and is read
+// only where one lane enters or leaves a job, so that the window does not hold both jobs' numbers in registers next to its row states.
+struct StreamJob {
+    unsigned long long x_addr;     // address of the level of row 1
+    uint32_t idx;
+    int E, end_lane, end_slot;
+    float lp_mm_self, lp_mm_next;
+    int x_step;                    // bytes from one row's level to the next
+};
+
+// forms job_idx's Gaussians on the warp's parameter line and its record in *s (lane 0)
+template <int C>
+__device__ __forceinline__ int stream_job(const FwdParams& p, float4* params, const uint32_t job_idx, const JobIn& j, const int lane, StreamJob* s)
+{
+    const nph_wave_geom geo = nph_wave_geometry((int)j.job.n_kmers, nph_job_events(j.job), C, 32, false);
+    if (lane == 0) {
+        s->x_addr = (unsigned long long)(p.level + j.rd.event_off + j.job.event_start);
+        s->idx = job_idx;
+        s->E = geo.E; s->end_lane = geo.end_lane(); s->end_slot = geo.end_slot();
+        s->lp_mm_self = j.tr.x; s->lp_mm_next = j.tr.y;
+        s->x_step = j.job.stride * (int)sizeof(float);
+    }
+    fill_job_gaussians<32>(params, j.mv, j.rd, p.ranks + j.job.rank_off, geo.K, geo.kpad, lane, p.c.log_inv_sqrt_2pi);
+    return geo.E;
+}
+
+// Runs the stream that starts with job job_idx (which streams()); returns the slot of the job that ended it (>= p.n_jobs: none left).
+template <int C>
+__device__ uint32_t run_stream(const FwdParams& p, const LogsumTable& tb, const HmmConsts& k, float4* params, int lane, const uint32_t job_idx,
+                               const JobIn& first)
+{
+    // opaque from here: the stream's addresses and lane offsets are formed inside the stream instead of being hoisted out of the
+    // kernel's job loop, where they would hold registers through the general loop
+    asm volatile("" : "+l"(params), "+r"(lane));
+    __shared__ StreamJob s_jobs[CtaShape<C, 32>::warps][2];
+    volatile StreamJob* const sj = s_jobs[threadIdx.x >> 5];   // volatile: read at each lane's entry and exit, not kept in registers
+    // the entering job's record is sj[n & 1] and its Gaussians are line(n); the leaving job's record is sj[(n + 1) & 1]
+    auto line = [&](const int i) { return params + (i & 1) * (32 * C); };
+    int n = 0;
+    int E = stream_job<C>(p, line(0), job_idx, first, lane, const_cast<StreamJob*>(&sj[0]));
+
+    const float NEG = -CUDART_INF_F;
+    float mu[C], sd[C], cc[C], ry[C];
+    float Mp[C], Bp[C], Kp[C], Tp[C];
+#pragma unroll
+    for (int c = 0; c < C; ++c) { mu[c] = 0.f; sd[c] = 1.f; cc[c] = 0.f; ry[c] = 1.f; Mp[c] = NEG; Bp[c] = NEG; Kp[c] = NEG; Tp[c] = NEG; }
+    float Lm_prev = NEG, Lt_prev = NEG, Lk_prev = NEG;
+    // this lane's job: transitions and the level address of its next row
+    float lp_mm_self = 0.f, lp_mm_next = 0.f;
+    unsigned long long x_addr = 0;
+    int x_step = 0;
+    float x_next = 0.f;
+    bool has_a = false, has_b = true;
+    uint32_t ended_by = p.n_jobs;
+    __syncwarp();
+    for (;;) {
+        volatile StreamJob& a = sj[(n + 1) & 1];
+        volatile StreamJob& b = sj[n & 1];
+        // window: lane j is on row E + t - j of the leaving job while t <= j, and on row t - j of b after; lane 31 enters b at t = 32
+        const int window = has_b ? 33 : a.end_lane + 1;
+        for (int t = 0; t < window; ++t) {
+            float Lm = __shfl_up_sync(kFull, Mp[C - 1], 1);
+            float Lt = __shfl_up_sync(kFull, Tp[C - 1], 1);
+            float Lk = __shfl_up_sync(kFull, Kp[C - 1], 1);
+            if (lane == 0) { Lm = NEG; Lt = NEG; Lk = NEG; }
+            const float x = x_next;
+            if (has_b && t == lane + 1) {
+                // entering b (after the shuffle: the right neighbour still takes this lane's last row of the leaving job): row 0 and the
+                // start column are -inf
+#pragma unroll
+                for (int c = 0; c < C; ++c) { Mp[c] = NEG; Bp[c] = NEG; Kp[c] = NEG; Tp[c] = NEG; }
+                Lm_prev = NEG; Lt_prev = NEG; Lk_prev = NEG;
+                load_columns<C>(line(n), lane * C, mu, sd, cc, ry);
+                lp_mm_self = b.lp_mm_self; lp_mm_next = b.lp_mm_next;
+            }
+            // prefetch for the next step; at t == j that is row 1 of b
+            if (t == lane) { x_addr = b.x_addr; x_step = b.x_step; }
+            if (t < lane ? has_a : has_b) {
+                x_next = __ldca(reinterpret_cast<const float*>(x_addr));
+                x_addr += x_step;
+            }
+            if (t <= lane ? has_a : has_b) {
+                // the soft-clip start: column 0 at row 1
+                row_update<C>(x, mu, sd, cc, ry, Mp, Bp, Kp, Tp, Lm_prev, Lt_prev, Lk_prev, Lm, Lt, Lk, lp_mm_self, lp_mm_next, k, true,
+                              [&] { return (lane == 0 && t == 1) ? p.flank[0] : NEG; }, tb);
+                Lm_prev = Lm; Lt_prev = Lt; Lk_prev = Lk;
+                if (t == lane && lane == a.end_lane) p.scores[a.idx] = end_fold<C>(NEG, Mp, Bp, Kp, a.end_slot, p.flank[0], tb);   // row E
+            }
+        }
+        if (!has_b) break;
+
+        // steady: every lane on b, rows 33 - j .. E - 1 - j
+#pragma unroll 1
+        for (int g = E - 33; g > 0; --g) {
+            float Lm = __shfl_up_sync(kFull, Mp[C - 1], 1);
+            float Lt = __shfl_up_sync(kFull, Tp[C - 1], 1);
+            float Lk = __shfl_up_sync(kFull, Kp[C - 1], 1);
+            if (lane == 0) { Lm = NEG; Lt = NEG; Lk = NEG; }
+            const float x = x_next;
+            x_next = __ldca(reinterpret_cast<const float*>(x_addr));
+            x_addr += x_step;
+            row_update<C>(x, mu, sd, cc, ry, Mp, Bp, Kp, Tp, Lm_prev, Lt_prev, Lk_prev, Lm, Lt, Lk, lp_mm_self, lp_mm_next, k, false,
+                          [&] { return NEG; }, tb);
+            Lm_prev = Lm; Lt_prev = Lt; Lk_prev = Lk;
+        }
+        has_a = true;
+
+        // the next job, if it streams, into the other half line and the record of the job that left in the last window
+        __syncwarp();
+        has_b = false;
+        const uint32_t slot = nph_warp_pop(p.counter, 1u, lane);
+        if (slot < p.n_jobs) {
+            const uint32_t n_idx = p.order[slot];
+            const JobIn j = fetch_job(p, n_idx, true, lane);
+            has_b = streams(j.job, nph_job_events(j.job));
+            if (has_b) E = stream_job<C>(p, line(n + 1), n_idx, j, lane, const_cast<StreamJob*>(&sj[(n + 1) & 1]));
+            else ended_by = slot;
+        }
+        load_columns<C>(line(n), lane * C, mu, sd, cc, ry);
+        n += 1;
+        __syncwarp();
+    }
+    return ended_by;
+}
+
 // CHAIN = false: every job of the class fits one strip (K <= W*C), all strip/edge bookkeeping compiles away.
 template <int C, int W, bool CHAIN>
 __global__ void __launch_bounds__(CtaShape<C, W>::warps * 32, 1) hmm_forward_kernel(const FwdParams p)
@@ -82,34 +298,27 @@ __global__ void __launch_bounds__(CtaShape<C, W>::warps * 32, 1) hmm_forward_ker
     const float NEG = -CUDART_INF_F;
     // lp_bk, lp_bm_next and lp_bm_self are all log(p_third) (nph_api.cu checks that they are bitwise equal), so
     // lp3 + B is one float that serves K-skip at (r, c+1), M-self at (r+1, c) and M-next at (r+1, c+1)
-    const float lp_mk = p.c.lp_mk, lp_mb = p.c.lp_mb, lp_bb = p.c.lp_bb, lp3 = p.c.lp_bk;
-    const float lp_kk = p.c.lp_kk, lp_km = p.c.lp_km;
+    const HmmConsts& k = p.c;
 
+    uint32_t ended_stream = UINT_MAX;   // full-warp single strip: the job that ended a stream, not yet run
     for (;;) {
-        const uint32_t base = nph_warp_pop(p.counter, (unsigned)G, lane);
+        const uint32_t base = ended_stream != UINT_MAX ? ended_stream : nph_warp_pop(p.counter, (unsigned)G, lane);
+        ended_stream = UINT_MAX;
         if (base >= p.n_jobs) break;
         const uint32_t slot = base + grp;
         const bool has_job = slot < p.n_jobs;
         const uint32_t job_idx = p.order[has_job ? slot : base];
-        const nph_hmm_job job = p.jobs[job_idx];
-        const DevRead rd = p.reads[job.read];
-        const float2 tr = p.trans[job.read];
-        const float lp_mm_self = tr.x, lp_mm_next = tr.y;
-        const DevModelView mv = p.models[job.model_id];
-        if (p.progress) {
-            // levels still streaming in behind us: wait until the chunk holding this read's last event has landed
-            // (chunks land in order; the progress word is written by a copy queued behind the chunk's data)
-            uint32_t need = has_job ? (uint32_t)((rd.event_off + rd.n_events - 1) / p.chunk_events) + 1u : 0u;
-            need = __reduce_max_sync(kFull, need);
-            if (lane == 0) {
-                const volatile uint32_t* pr = p.progress;
-                while (*pr < need) __nanosleep(500);
-            }
-            __syncwarp();
-        }
+        const JobIn ji = fetch_job(p, job_idx, has_job, lane);
+        const nph_hmm_job& job = ji.job;
+        const DevRead& rd = ji.rd;
+        const DevModelView& mv = ji.mv;
+        const float lp_mm_self = ji.tr.x, lp_mm_next = ji.tr.y;
 
         const nph_wave_geom geo = nph_wave_geometry((int)job.n_kmers, has_job ? nph_job_events(job) : 0, C, W, CHAIN);
         const int K = geo.K, E = geo.E, stride = job.stride, n_strips = geo.n_strips, P = geo.P;
+        if constexpr (W == 32 && !CHAIN) {
+            if (streams(job, E)) { ended_stream = run_stream<C>(p, tb, k, my_params, lane, job_idx, ji); continue; }
+        }
         const bool pre_clip = (job.flags & NPH_HAF_ALLOW_PRE_CLIP) != 0;
         const bool post_clip = (job.flags & NPH_HAF_ALLOW_POST_CLIP) != 0;
 
@@ -178,46 +387,12 @@ __global__ void __launch_bounds__(CtaShape<C, W>::warps * 32, 1) hmm_forward_ker
             if (live) {
                 const bool do_end = (!CHAIN || s == last_strip) && r >= end_row;
 
-                float lm_prev = Lm_prev, lt_prev = Lt_prev, lk_prev = Lk_prev;   // left column, row r-1
-                float lm_cur = Lm, lt_cur = Lt, lk_cur = Lk;                      // left column, row r
-                auto cell = [&](const int c, const bool with_soft) {
-                    const float em = log_gauss(x, mu[c], sd[c], cc[c], ry[c]);
-                    // match: left fold over {same M, prev M, same B, prev B, prev K, soft}
-                    float m = __fadd_rn(lp_mm_self, Mp[c]);
-                    m = lsum_sat(m, __fadd_rn(lp_mm_next, lm_prev), tb);
-                    m = lsum_sat(m, Tp[c], tb);
-                    m = lsum_sat(m, lt_prev, tb);
-                    m = lsum_sat(m, __fadd_rn(lp_km, lk_prev), tb);
-                    if (with_soft) m = lsum_sat(m, (col0 == 0 && (r == 1 || pre_clip)) ? p.flank[r - 1] : NEG, tb);
-                    m = __fadd_rn(m, em);
-                    // bad event: {same M, same B}
-                    const float b = lsum_sat(__fadd_rn(lp_mb, Mp[c]), __fadd_rn(lp_bb, Bp[c]), tb);
-                    // k-mer skip: {prev M, prev B, prev K} of the SAME row
-                    float kk = lsum_sat(__fadd_rn(lp_mk, lm_cur), lt_cur, tb);
-                    kk = lsum_sat(kk, __fadd_rn(lp_kk, lk_cur), tb);
-                    const float t = __fadd_rn(lp3, b);
-
-                    lm_prev = Mp[c]; lt_prev = Tp[c]; lk_prev = Kp[c];
-                    lm_cur = m; lt_cur = t; lk_cur = kk;
-                    Mp[c] = m; Bp[c] = b; Kp[c] = kk; Tp[c] = t;
-                };
-                // two copies of column 0, so that the usual step branches past the soft fold instead of predicating it
-                if (any_pre_clip || g == 0) cell(0, true);
-                else cell(0, false);
-#pragma unroll
-                for (int c = 1; c < C; ++c) cell(c, false);
+                row_update<C>(x, mu, sd, cc, ry, Mp, Bp, Kp, Tp, Lm_prev, Lt_prev, Lk_prev, Lm, Lt, Lk, lp_mm_self, lp_mm_next, k, any_pre_clip || g == 0,
+                              [&] { return (col0 == 0 && (r == 1 || pre_clip)) ? p.flank[r - 1] : NEG; }, tb);
                 Lm_prev = Lm; Lt_prev = Lt; Lk_prev = Lk;
 
-                if (do_end) {
-                    // states of the last k-mer's column; with flags 0 this runs once per job
-                    float Me = Mp[0], Be = Bp[0], Ke = Kp[0];
-#pragma unroll
-                    for (int c = 1; c < C; ++c) if (c == end_slot) { Me = Mp[c]; Be = Bp[c]; Ke = Kp[c]; }
-                    const float post = p.flank[E - r];
-                    lp_end = lsum_sat(lp_end, __fadd_rn(Me, post), tb);
-                    lp_end = lsum_sat(lp_end, __fadd_rn(Be, post), tb);
-                    lp_end = lsum_sat(lp_end, __fadd_rn(Ke, post), tb);
-                }
+                // the states of the last k-mer's column; with flags 0 this runs once per job
+                if (do_end) lp_end = end_fold<C>(lp_end, Mp, Bp, Kp, end_slot, p.flank[E - r], tb);
                 if (CHAIN && gl == W - 1 && s < last_strip) { edge.a[r] = Mp[C - 1]; edge.b[r] = Tp[C - 1]; edge.c[r] = Kp[C - 1]; }
             }
 

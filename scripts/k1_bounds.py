@@ -84,8 +84,8 @@ def _target(ops: str) -> int | None:
     return int(m.group(1), 16) if m else None
 
 
-def steady_step(insns, min_lds: int):
-    """Shortest path (in instructions) through the innermost loop holding >= min_lds LDS, taking >= min_lds LDS."""
+def _loops(insns, min_lds: int):
+    """(length, head, tail) instruction-index ranges of the backward branches whose body holds >= min_lds LDS"""
     addr_ix = {a: i for i, (a, _, _, _) in enumerate(insns)}
     loops = []
     for i, (a, pred, op, ops) in enumerate(insns):
@@ -96,7 +96,37 @@ def steady_step(insns, min_lds: int):
                 lds = sum(1 for x in insns[lo:i + 1] if x[2].startswith("LDS"))
                 if lds >= min_lds:
                     loops.append((i - lo, lo, i))
-    _, head, tail = min(loops)
+    return loops
+
+
+def steady_step(insns, min_lds: int):
+    """Shortest path (in instructions) through the innermost loop holding >= min_lds LDS, taking >= min_lds LDS."""
+    _, head, tail = min(_loops(insns, min_lds))
+    return _loop_step(insns, head, tail, min_lds)
+
+
+def window_step(insns, C: int):
+    """Step of the streamed kernel's transition window: the innermost loop with the soft-fold copy of column 0 (>= 7*C + 1 LDS),
+    other than the steady loop, inside the smallest loop that encloses the steady loop (the stream).  None if there is none, as in
+    a kernel without streaming, where the loop enclosing the step loop is the job loop and holds no second step loop."""
+    row_loops = _loops(insns, 7 * C)
+    _, sh, st = min(row_loops)
+    outer = [(n, h, t) for n, h, t in row_loops if h <= sh and st <= t and (h, t) != (sh, st)]
+    if not outer:
+        return None
+    _, oh, ot = min(outer)
+    inner = [(n, h, t) for n, h, t in _loops(insns, 7 * C + 1)
+             if oh <= h and t <= ot and (h, t) not in ((sh, st), (oh, ot))
+             and not any(h <= h2 and t2 <= t and (h2, t2) != (h, t) for _, h2, t2 in row_loops)]
+    if not inner:
+        return None
+    _, head, tail = min(inner, key=lambda x: x[1])
+    return _loop_step(insns, head, tail, 7 * C + 1)
+
+
+def _loop_step(insns, head: int, tail: int, min_lds: int):
+    """Shortest path (in instructions) from head to tail taking >= min_lds LDS."""
+    addr_ix = {a: i for i, (a, _, _, _) in enumerate(insns)}
     # DP over (instruction, LDS taken so far): fewest instructions issued
     INF = 1 << 30
     cap = min_lds
@@ -168,12 +198,15 @@ def classify(path) -> collections.Counter:
 
 
 def issue_side(obj: str) -> dict[int, dict]:
+    """Per C: the steady step and the step of the streamed jobs' transition window (window_step; every lane live, no lane entering
+    or leaving a job)."""
     funcs = sass_functions(obj)
     res = {}
     for C in (9, 10):
         name = f"_ZN7nph_fwd18hmm_forward_kernelILi{C}ELi32ELb0EEEvNS_9FwdParamsE"
         path = steady_step(funcs[name], 7 * C)
-        res[C] = {"total": len(path), "ops": classify(path)}
+        window = window_step(funcs[name], C)
+        res[C] = {"total": len(path), "ops": classify(path), "window": len(window) if window else None}
     return res
 
 
@@ -389,6 +422,8 @@ def main():
     per_step = {t: d[9]["total"] - 9 * per_col[t] for t, d in (("before", BEFORE), ("after", after))}
     for t in ("before", "after"):
         print(f"  {t}: {per_step[t]} per warp step + {per_col[t]} per column")
+    for C in (9, 10):
+        print(f"  C={C:2d} transition window step (streamed jobs, 33 per job): {after[C]['window'] or 'no window'}")
 
     sm = smem_side(args.jobs)
     print(f"\nShared-memory side: look-up wavefronts, lockstep replay of bench scorereads jobs (seed 42)")
