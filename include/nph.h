@@ -755,6 +755,28 @@ int nph_polya_batch(nph_ctx* ctx, const float* raw, size_t n_samples_total, cons
                     const float* ev_duration, size_t n_events_total, const nph_event_range* base_to_event, size_t n_ranks_total,
                     nph_polya_result* results_out);
 
+/* ---- poly(I) / poly(A) tail detection (nanopolish detect-polyi) -------------------------------------------
+ * Per read, what dpi_estimate_polya_for_single_read computes after loading (src/nanopolish_detect_polyi.cpp:1061-1095): the
+ * segmentation, read rate, length and QC of nph_polya_batch with DPISegmentationHMM (:177-518, whose POLYA emission is an even
+ * mixture of two Gaussians, :291-295), then BernoulliHMM::segmentation over the tail's samples [adapter + 1, polya) (:728-756)
+ * and post_boolhmm_detetection_qc (:973-997).  Same jobs, inputs and refusals as nph_polya_batch, plus NPH_ERR_INVALID for a
+ * loaded job with n_samples >= 2^31: the reference passes the tail's bounds as int and would read before the samples.
+ * A READ_FAILED_LOAD result has seg as nph_polya_batch gives it and -1 in polyi_last, polya_first and detected. */
+#define NPH_POLYI_NONE       0   /* "NONE" */
+#define NPH_POLYI_POLYA_ONLY 1   /* "POLYA-ONLY": polya_first > 0 and tail samples - polya_first > 200 */
+#define NPH_POLYI_POLYI_ONLY 2   /* "POLYI-ONLY": polyi_last > 200 */
+#define NPH_POLYI_A_PLUS_I   3   /* "A+I": both */
+typedef struct {
+    nph_polya_result seg;     /* as nph_polya_batch, under DPISegmentationHMM; seg.qc is the row's qc_tag */
+    int32_t  polyi_last;      /* BernoulliSegmentation::polyi: last poly(I) index in the tail, or -1 */
+    int32_t  polya_first;     /* BernoulliSegmentation::polya: first poly(A) index in the tail, or -1 */
+    int32_t  detected;        /* NPH_POLYI_*, the row's detected column */
+    uint32_t reserved;
+} nph_polyi_result;
+int nph_detect_polyi_batch(nph_ctx* ctx, const float* raw, size_t n_samples_total, const nph_polya_job* jobs, size_t n_jobs,
+                           const float* ev_duration, size_t n_events_total, const nph_event_range* base_to_event,
+                           size_t n_ranks_total, nph_polyi_result* results_out);
+
 /* ---- measurement hooks (used by bench.py; not part of the reference surface) ------------- */
 /* Device time in ms of the most recent nph_hmm_score / nph_abea_run kernel sequence, measured
  * with CUDA events on the context's stream (valid after a sync), and the number of kernel

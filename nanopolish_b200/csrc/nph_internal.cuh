@@ -224,7 +224,7 @@ struct nph_ctx {
     std::vector<float2> h_stage_trans;
     std::vector<nph_raw_range> h_last_trim;  // surviving sample range per job of the last nph_load_from_raw_batch
 
-    DevBuf<uint8_t> d_polya;                 // nph_polya_batch: raw samples, durations, event map, jobs, order, results
+    DevBuf<uint8_t> d_polya;                 // nph_polya_batch / nph_detect_polyi_batch: raw samples, durations, event map, jobs, order, results
 };
 
 int nph_set_cuda_error(nph_ctx* ctx, cudaError_t e, const char* what);

@@ -1,5 +1,6 @@
 // polya.cu — nanopolish polya on the device: poly(A) tail segmentation and length of a batch of reads in one call
-// (src/nanopolish_polya_estimator.cpp; the per-read part of estimate_polya_for_single_read, :786-813).
+// (src/nanopolish_polya_estimator.cpp; the per-read part of estimate_polya_for_single_read, :786-813), and nanopolish
+// detect-polyi, its sibling for poly(I) tails (src/nanopolish_detect_polyi.cpp; dpi_estimate_polya_for_single_read, :1061-1095).
 //
 // One CTA per read, reads launched longest first.  Warp 0 walks the 6-state Viterbi of SegmentationHMM (:372-463) over the
 // read's samples on one lane; warps 1..3 compute the six emission log-probabilities (:259-306) of the NEXT tile of samples
@@ -17,9 +18,17 @@
 // Every floating-point operation is spelled as the reference rounds it (float for the HMM, double for the length and QC;
 // max is std::max, (a < b) ? b : a; the backpointer rules use strict < in the reference's precedence), and expf / logf are
 // glibc's (libm_exact.cuh).
+//
+// detect-polyi is the same kernel instantiated with kPolyi (DESIGN §15).  Its segmentation HMM (DPISegmentationHMM,
+// :177-518) differs from polya's only in the POLYA emission, an even mixture of two Gaussians (:291-295).  After the walk the
+// whole CTA runs BernoulliHMM::segmentation (:728-756) over the tail's samples in two passes through the same double buffer:
+// warps 1..3 scale the samples tile by tile while lane 0 takes their sequential float mean; then warps 1..3 compute each
+// centred sample's log-likelihood-ratio bit tile by tile while lane 0 walks the 2-state Viterbi one tile behind.  Its labels
+// are I..I A..A (A is absorbing), so the walk folds the backtrack into one index: the first A of the path that ends in A.
 #include "nph_internal.cuh"
 #include "libm_exact.cuh"
 
+#include <type_traits>
 #include <vector>
 
 namespace {
@@ -28,49 +37,61 @@ constexpr int kTile = 256;            // samples per emission tile
 constexpr int kEmitWarps = 3;
 constexpr int kThreads = 32 * (1 + kEmitWarps);
 enum { ST_S = 0, ST_L, ST_A, ST_P, ST_C, ST_T, N_ST };
-enum { G_S = 0, G_L, G_A0, G_A1, G_P, G_T0, G_T1, N_G };
+// G_P1 exists in detect-polyi's table only
+enum { G_S = 0, G_L, G_A0, G_A1, G_P, G_T0, G_T1, G_P1 };
+template <bool kPolyi> constexpr int n_gauss = kPolyi ? G_P1 + 1 : G_P1;
 
-// The reference's emission parameters (:232-250), before scaling
-__constant__ const float k_gauss[N_G][2] = {
+// The reference's emission parameters (:232-250; detect_polyi.cpp:233-255 adds P1), before scaling
+__constant__ const float k_gauss[G_P1 + 1][2] = {
     {70.2737f, 3.7743f}, {110.973f, 5.237f}, {79.347f, 8.3702f}, {63.3126f, 2.7464f},
-    {108.883f, 3.257f}, {79.679f, 6.966f}, {105.784f, 16.022f}};
+    {108.883f, 3.257f}, {79.679f, 6.966f}, {105.784f, 16.022f}, {108.498f, 5.257f}};
 
+template <int NG>
 struct Gauss {
-    float mean[N_G], stdv[N_G], log_stdv[N_G], coef[N_G];   // coef = inv_sqrt_2pi / stdv, as normal_pdf forms it
+    float mean[NG], stdv[NG], log_stdv[NG], coef[NG];   // coef = inv_sqrt_2pi / stdv, as normal_pdf forms it
     float log_inv_sqrt_2pi;
 };
 
+template <bool kPolyi> using TailResult = typename std::conditional<kPolyi, nph_polyi_result, nph_polya_result>::type;
+
+template <bool kPolyi>
 struct PolyaParams {
     const float* raw;
     const float* dur;
     const nph_event_range* b2e;
     const nph_polya_job* jobs;
     const uint32_t* order;
-    nph_polya_result* out;
+    TailResult<kPolyi>* out;
     float log_inv_sqrt_2pi;           // (float)log(0.3989422804014327) (hmm/nanopolish_emissions.h:43), host libm
 };
 
 // normal_pdf (emissions.h:19-24): inv_sqrt_2pi / stdv * exp(-0.5f * a * a)
-__device__ __forceinline__ float normal_pdf(float x, const Gauss& g, int k)
+template <int NG>
+__device__ __forceinline__ float normal_pdf(float x, const Gauss<NG>& g, int k)
 {
     const float a = __fdiv_rn(__fsub_rn(x, g.mean[k]), g.stdv[k]);
     return __fmul_rn(g.coef[k], nph_expf(__fmul_rn(__fmul_rn(-0.5f, a), a)));
 }
 // log_normal_pdf (emissions.h:51-55): log_inv_sqrt_2pi - log_stdv + (-0.5f * a * a)
-__device__ __forceinline__ float log_normal_pdf(float x, const Gauss& g, int k)
+template <int NG>
+__device__ __forceinline__ float log_normal_pdf(float x, const Gauss<NG>& g, int k)
 {
     const float a = __fdiv_rn(__fsub_rn(x, g.mean[k]), g.stdv[k]);
     return __fadd_rn(__fsub_rn(g.log_inv_sqrt_2pi, g.log_stdv[k]), __fmul_rn(__fmul_rn(-0.5f, a), a));
 }
 
-// emit_log_proba of all six states (:259-306)
-__device__ __forceinline__ void emissions(float x, const Gauss& g, float e[N_ST])
+// emit_log_proba of all six states (:259-306; detect_polyi.cpp:263-312)
+template <bool kPolyi>
+__device__ __forceinline__ void emissions(float x, const Gauss<n_gauss<kPolyi>>& g, float e[N_ST])
 {
     const float xx = (x > 200.0f || x < 40.0f) ? 100.0f : x;
     e[ST_S] = nph_logf(__fadd_rn(__fmul_rn(0.50f, normal_pdf(xx, g, G_S)), __fmul_rn(0.50f, 0.00476f)));
     e[ST_L] = log_normal_pdf(xx, g, G_L);
     e[ST_A] = nph_logf(__fadd_rn(__fmul_rn(0.874f, normal_pdf(xx, g, G_A0)), __fmul_rn(0.126f, normal_pdf(xx, g, G_A1))));
-    e[ST_P] = log_normal_pdf(xx, g, G_P);
+    if constexpr (kPolyi)
+        e[ST_P] = nph_logf(__fadd_rn(__fmul_rn(0.500f, normal_pdf(xx, g, G_P)), __fmul_rn(0.500f, normal_pdf(xx, g, G_P1))));
+    else
+        e[ST_P] = log_normal_pdf(xx, g, G_P);
     e[ST_C] = (xx > 70.0f && xx < 140.0f) ? -4.2485f : -INFINITY;
     e[ST_T] = nph_logf(__fadd_rn(__fmul_rn(0.346f, normal_pdf(xx, g, G_T0)), __fmul_rn(0.654f, normal_pdf(xx, g, G_T1))));
 }
@@ -79,6 +100,29 @@ __device__ __forceinline__ void emissions(float x, const Gauss& g, float e[N_ST]
 __device__ __forceinline__ float log_prob(float p) { return p > 0.00f ? nph_logf(p) : -INFINITY; }
 
 __device__ __forceinline__ float smax(float a, float b) { return (a < b) ? b : a; }   // std::max
+
+// segment_squiggle's sentinel rule (:500-506): a boundary left at its initial value moves all three to the read's end
+__device__ __forceinline__ void sentinel_rule(uint64_t& ld, uint64_t& ad, uint64_t& pa, uint32_t n)
+{
+    if (ld == 1 || ad == 2 || pa == 3) { ld = (uint64_t)n - 3; ad = (uint64_t)n - 2; pa = (uint64_t)n - 1; }
+}
+
+// BernoulliHMM's bit of one scaled tail sample (detect_polyi.cpp:663-671): recentred on 108, clamped like the segmentation,
+// then log normal_pdf under the UNSCALED poly(I) and poly(A) Gaussians (:563-564, :581-603); (lI / lA) > 1, so the NaN of
+// -inf / -inf (both densities underflow) is 0
+__device__ __forceinline__ float unscaled_pdf(float x, float mean, float stdv)
+{
+    const float a = __fdiv_rn(__fsub_rn(x, mean), stdv);
+    return __fmul_rn(__fdiv_rn((float)0.3989422804014327, stdv), nph_expf(__fmul_rn(__fmul_rn(-0.5f, a), a)));
+}
+__device__ __forceinline__ bool bernoulli_bit(float y, float mean)
+{
+    const float s = __fadd_rn(__fsub_rn(y, mean), 108.000f);
+    const float xx = (s > 200.0f || s < 40.0f) ? 100.0f : s;
+    const float lI = nph_logf(unscaled_pdf(xx, 108.498f, 5.257f));
+    const float lA = nph_logf(unscaled_pdf(xx, 108.883f, 3.257f));
+    return __fdiv_rn(lI, lA) > 1.0f;
+}
 
 // total order of doubles as unsigned keys (the median's radix selection)
 __device__ __forceinline__ uint64_t dkey(double d)
@@ -91,10 +135,11 @@ __device__ __forceinline__ double dunkey(uint64_t k)
     return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
 }
 
-__global__ void __launch_bounds__(kThreads) polya_kernel(const PolyaParams p)
+template <bool kPolyi>
+__global__ void __launch_bounds__(kThreads) polya_kernel(const PolyaParams<kPolyi> p)
 {
     __shared__ float s_em[2][N_ST][kTile];
-    __shared__ Gauss s_g;
+    __shared__ Gauss<n_gauss<kPolyi>> s_g;
     __shared__ uint32_t s_hist[256];
     __shared__ uint32_t s_sel, s_rank;
     __shared__ double s_rate;
@@ -106,7 +151,7 @@ __global__ void __launch_bounds__(kThreads) polya_kernel(const PolyaParams p)
     const float* x = p.raw + jb.sample_off;
 
     // ---- per-read constants (:310-354): (float)scale, shift, var; mean' = shift + scale*mean, stdv' = var*stdv ----
-    if (tid < N_G) {
+    if (tid < n_gauss<kPolyi>) {
         const float scale = (float)jb.scale, shift = (float)jb.shift, var = (float)jb.var;
         const float sd = __fmul_rn(var, k_gauss[tid][1]);
         s_g.mean[tid] = __fadd_rn(shift, __fmul_rn(scale, k_gauss[tid][0]));
@@ -157,7 +202,7 @@ __global__ void __launch_bounds__(kThreads) polya_kernel(const PolyaParams p)
             const uint32_t i = t * kTile + o;
             if (i >= n_steps) break;
             float e[N_ST];
-            emissions(x[i == 0 ? n - 1 : i], s_g, e);
+            emissions<kPolyi>(x[i == 0 ? n - 1 : i], s_g, e);
 #pragma unroll
             for (int s = 0; s < N_ST; ++s) em[s][o] = e[s];
         }
@@ -230,10 +275,96 @@ __global__ void __launch_bounds__(kThreads) polya_kernel(const PolyaParams p)
         __syncthreads();
     }
 
+    // ---- detect-polyi: BernoulliHMM::segmentation(sr, adapter + 1, polya) (detect_polyi.cpp:728-756) ----
+    int32_t b_polyi = -1, b_polya = -1;   // BernoulliSegmentation {-1, -1}: not found (lane 0)
+    if constexpr (kPolyi) {
+        __shared__ uint32_t s_b0, s_m;
+        __shared__ float s_mean;
+        if (tid == 0) {
+            uint64_t ld = Tl, ad = Ta, pa = Tp;
+            sentinel_rule(ld, ad, pa, n);
+            // int start / stop: exact, as the host refuses n >= 2^31; polya >= adapter + 1 always
+            s_b0 = (uint32_t)(ad + 1);
+            s_m = (uint32_t)(pa - (ad + 1));
+        }
+        __syncthreads();
+        const uint32_t b0 = s_b0, m = s_m;
+        if (m >= 100) {                                        // stop - start < 100: not found (:732-734)
+            constexpr uint32_t kFlat = N_ST * kTile;           // one half of the double buffer, as one flat tile
+            const uint32_t n_ft = (m + kFlat - 1) / kFlat;
+            // pass 0: (x - shift) / scale in double with the unrounded scalings, narrowed to float (:737-740); pass 1: the bit
+            auto fill = [&](uint32_t t, bool bits, float mean) {
+                float* buf = &s_em[t & 1][0][0];
+                for (uint32_t o = tid - 32; o < kFlat; o += 32 * kEmitWarps) {
+                    const uint32_t i = t * kFlat + o;
+                    if (i >= m) break;
+                    const float y = __double2float_rn(__ddiv_rn(__dsub_rn((double)x[b0 + i], jb.shift), jb.scale));
+                    buf[o] = bits ? (bernoulli_bit(y, mean) ? 1.0f : 0.0f) : y;
+                }
+            };
+            // pass 0: instance_mean, a sequential float sum divided by (float)size (:655-659)
+            if (warp > 0) fill(0, false, 0.0f);
+            __syncthreads();
+            float sum = 0.0f;
+            for (uint32_t t = 0; t < n_ft; ++t) {
+                if (tid == 0) {
+                    const float* buf = &s_em[t & 1][0][0];
+                    const uint32_t o1 = min(kFlat, m - t * kFlat);
+                    for (uint32_t o = 0; o < o1; ++o) sum = __fadd_rn(sum, buf[o]);
+                } else if (warp > 0 && t + 1 < n_ft) {
+                    fill(t + 1, false, 0.0f);
+                }
+                __syncthreads();
+            }
+            if (tid == 0) s_mean = __fdiv_rn(sum, __uint2float_rn(m));
+            __syncthreads();
+            const float mean = s_mean;
+            // pass 1: BernoulliHMM::viterbi (:678-725).  first_a is the first A of the backtracked path ending in A: the
+            // backpointer of step i into A is I iff a2a < i2a, and the backtrack reads those of steps 1 .. m-2 (regions[0]
+            // stays I, so a path in A at step 1 starts A there)
+            if (warp > 0) fill(0, true, mean);
+            __syncthreads();
+            float vI = 0.0f, vA = 0.0f, lII = 0.0f, lIA = 0.0f, lAA = 0.0f, eI1 = 0.0f, eI0 = 0.0f, eA1 = 0.0f, eA0 = 0.0f;
+            uint32_t first_a = 1;
+            if (tid == 0) {
+                lII = log_prob(0.90f); lIA = log_prob(0.10f); lAA = log_prob(1.00f);
+                eI1 = nph_logf(0.72304f); eI0 = nph_logf(__fsub_rn(1.0f, 0.72304f));
+                eA1 = nph_logf(0.92154f); eA0 = nph_logf(__fsub_rn(1.0f, 0.92154f));
+            }
+            for (uint32_t t = 0; t < n_ft; ++t) {
+                if (tid == 0) {
+                    const float* buf = &s_em[t & 1][0][0];
+                    const uint32_t i0 = t * kFlat, o1 = min(kFlat, m - i0);
+                    uint32_t o = 0;
+                    if (t == 0) {
+                        // row 0: log_start_probs {logf(1), -inf} + the emissions of bit 0
+                        vI = __fadd_rn(log_prob(1.00f), buf[0] != 0.0f ? eI1 : eI0);
+                        vA = -INFINITY;
+                        o = 1;
+                    }
+                    for (; o < o1; ++o) {
+                        const uint32_t i = i0 + o;
+                        const bool one = buf[o] != 0.0f;
+                        const float i2i = __fadd_rn(vI, lII), i2a = __fadd_rn(vI, lIA), a2a = __fadd_rn(vA, lAA);
+                        vI = __fadd_rn(i2i, one ? eI1 : eI0);
+                        vA = __fadd_rn(smax(i2a, a2a), one ? eA1 : eA0);
+                        if (a2a < i2a && i + 1 < m) first_a = i + 1;
+                    }
+                } else if (warp > 0 && t + 1 < n_ft) {
+                    fill(t + 1, true, mean);
+                }
+                __syncthreads();
+            }
+            // the last row's state is A iff vI < vA (:710-716); labels I..I A..A give polyi = polya - 1
+            if (vI < vA) { b_polya = (int32_t)first_a; b_polyi = (int32_t)first_a - 1; }
+            else         { b_polyi = (int32_t)m - 1; }
+        }
+    }
+
     if (tid != 0) return;
     // ---- segment_squiggle's result (:474-507), estimate_polya_length, QC (size_t arithmetic as in the reference) ----
     uint64_t st = Ts, ld = Tl, ad = Ta, pa = Tp;
-    if (ld == 1 || ad == 2 || pa == 3) { ld = (uint64_t)n - 3; ad = (uint64_t)n - 2; pa = (uint64_t)n - 1; }
+    sentinel_rule(ld, ad, pa, n);
     const double rate = s_rate;
     const double polya_duration = __ddiv_rn(__ull2double_rn(pa - (ad + 1)), jb.sample_rate);
     const double len = __dadd_rn(__dmul_rn(polya_duration, rate), -5.0);
@@ -247,15 +378,28 @@ __global__ void __launch_bounds__(kThreads) polya_kernel(const PolyaParams p)
     nph_polya_result r;
     r.start = st; r.leader = ld; r.adapter = ad; r.polya = pa; r.cliffs = Tc;
     r.read_rate = rate; r.polya_length = polya_length; r.qc = qc; r.reserved = 0;
-    p.out[jid] = r;
+    if constexpr (kPolyi) {
+        // post_boolhmm_detetection_qc(segmentation, (int)(polya - (adapter + 1))) (detect_polyi.cpp:973-997, :1095)
+        const int32_t region_length = (int32_t)(pa - (ad + 1));
+        const bool polyi_found = b_polyi > 200;
+        const bool polya_found = b_polya > 0 && region_length - b_polya > 200;
+        nph_polyi_result q;
+        q.seg = r; q.polyi_last = b_polyi; q.polya_first = b_polya; q.reserved = 0;
+        q.detected = polyi_found ? (polya_found ? NPH_POLYI_A_PLUS_I : NPH_POLYI_POLYI_ONLY)
+                                 : (polya_found ? NPH_POLYI_POLYA_ONLY : NPH_POLYI_NONE);
+        p.out[jid] = q;
+    } else {
+        p.out[jid] = r;
+    }
 }
 
-} // namespace
-
-extern "C" int nph_polya_batch(nph_ctx* ctx, const float* raw, size_t n_samples_total, const nph_polya_job* jobs, size_t n_jobs,
-                               const float* ev_duration, size_t n_events_total, const nph_event_range* base_to_event, size_t n_ranks_total,
-                               nph_polya_result* results_out)
+// Both entry points: job validation, the failed-load results, longest-first order, the d_polya carve, the uploads and the launch
+template <bool kPolyi>
+int polya_batch(nph_ctx* ctx, const float* raw, size_t n_samples_total, const nph_polya_job* jobs, size_t n_jobs,
+                const float* ev_duration, size_t n_events_total, const nph_event_range* base_to_event, size_t n_ranks_total,
+                TailResult<kPolyi>* results_out)
 {
+    using Result = TailResult<kPolyi>;
     if (!ctx) return NPH_ERR_INVALID;
     if (n_jobs == 0) return NPH_OK;
     if (!jobs || !results_out) return NPH_ERR_INVALID;
@@ -265,6 +409,7 @@ extern "C" int nph_polya_batch(nph_ctx* ctx, const float* raw, size_t n_samples_
         const nph_polya_job& jb = jobs[j];
         if (!jb.loaded || jb.n_events == 0) continue;         // events[0].empty(): READ_FAILED_LOAD (:762)
         if (!raw || !ev_duration || !base_to_event) return NPH_ERR_INVALID;
+        if (kPolyi && jb.n_samples >= (1u << 31)) return NPH_ERR_INVALID;   // BernoulliHMM::segmentation's int start / stop
         if (jb.n_samples < 2 || !nph_slice_ok(jb.sample_off, jb.n_samples, n_samples_total) ||
             !nph_kmers_ok(jb.rank_off, jb.n_kmers, n_ranks_total) || !nph_slice_ok(jb.event_off, jb.n_events, n_events_total))
             return NPH_ERR_INVALID;
@@ -278,7 +423,8 @@ extern "C" int nph_polya_batch(nph_ctx* ctx, const float* raw, size_t n_samples_
     for (size_t j = 0; j < n_jobs; ++j) {
         nph_polya_result r{};
         r.read_rate = -1.0; r.polya_length = -1.0; r.qc = NPH_POLYA_READ_FAILED_LOAD;
-        results_out[j] = r;
+        if constexpr (kPolyi) results_out[j] = nph_polyi_result{r, -1, -1, -1, 0};
+        else results_out[j] = r;
     }
     if (live.empty()) { nph_timing_events(ctx, 0); return NPH_OK; }
     NPH_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -288,14 +434,14 @@ extern "C" int nph_polya_batch(nph_ctx* ctx, const float* raw, size_t n_samples_
     std::vector<uint32_t> order(live.size());
     for (size_t t = 0; t < live.size(); ++t) order[t] = live[by_len[t]];
 
-    float* d_raw; float* d_dur; nph_event_range* d_b2e; nph_polya_job* d_jobs; uint32_t* d_order; nph_polya_result* d_out;
+    float* d_raw; float* d_dur; nph_event_range* d_b2e; nph_polya_job* d_jobs; uint32_t* d_order; Result* d_out;
     NPH_TRY(nph_carve(ctx, ctx->d_polya, [&](NphArena& a) {
         d_raw = a.take<float>(n_samples_total);
         d_dur = a.take<float>(n_events_total);
         d_b2e = a.take<nph_event_range>(n_ranks_total);
         d_jobs = a.take<nph_polya_job>(n_jobs);
         d_order = a.take<uint32_t>(order.size());
-        d_out = a.take<nph_polya_result>(n_jobs);
+        d_out = a.take<Result>(n_jobs);
     }));
     NPH_CUDA(ctx, cudaMemcpyAsync(d_raw, raw, sizeof(float) * n_samples_total, cudaMemcpyHostToDevice, ctx->stream));
     NPH_CUDA(ctx, cudaMemcpyAsync(d_dur, ev_duration, sizeof(float) * n_events_total, cudaMemcpyHostToDevice, ctx->stream));
@@ -303,17 +449,35 @@ extern "C" int nph_polya_batch(nph_ctx* ctx, const float* raw, size_t n_samples_
     NPH_CUDA(ctx, cudaMemcpyAsync(d_jobs, jobs, sizeof(nph_polya_job) * n_jobs, cudaMemcpyHostToDevice, ctx->stream));
     NPH_CUDA(ctx, cudaMemcpyAsync(d_order, order.data(), sizeof(uint32_t) * order.size(), cudaMemcpyHostToDevice, ctx->stream));
 
-    PolyaParams pp;
+    PolyaParams<kPolyi> pp;
     pp.raw = d_raw; pp.dur = d_dur; pp.b2e = d_b2e; pp.jobs = d_jobs; pp.order = d_order; pp.out = d_out;
     pp.log_inv_sqrt_2pi = (float)std::log(0.3989422804014327);
     NPH_CUDA(ctx, cudaEventRecord(ctx->ev0, ctx->stream));
-    polya_kernel<<<(unsigned)order.size(), kThreads, 0, ctx->stream>>>(pp);
+    polya_kernel<kPolyi><<<(unsigned)order.size(), kThreads, 0, ctx->stream>>>(pp);
     NPH_CUDA(ctx, cudaGetLastError());
     NPH_CUDA(ctx, cudaEventRecord(ctx->ev1, ctx->stream));
-    std::vector<nph_polya_result> res(n_jobs);
-    NPH_CUDA(ctx, cudaMemcpyAsync(res.data(), d_out, sizeof(nph_polya_result) * n_jobs, cudaMemcpyDeviceToHost, ctx->stream));
+    std::vector<Result> res(n_jobs);
+    NPH_CUDA(ctx, cudaMemcpyAsync(res.data(), d_out, sizeof(Result) * n_jobs, cudaMemcpyDeviceToHost, ctx->stream));
     NPH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // order[] and res must outlive the copies
     for (uint32_t j : live) results_out[j] = res[j];
     nph_timing_events(ctx, 1);
     return NPH_OK;
+}
+
+} // namespace
+
+extern "C" int nph_polya_batch(nph_ctx* ctx, const float* raw, size_t n_samples_total, const nph_polya_job* jobs, size_t n_jobs,
+                               const float* ev_duration, size_t n_events_total, const nph_event_range* base_to_event, size_t n_ranks_total,
+                               nph_polya_result* results_out)
+{
+    return polya_batch<false>(ctx, raw, n_samples_total, jobs, n_jobs, ev_duration, n_events_total, base_to_event, n_ranks_total,
+                              results_out);
+}
+
+extern "C" int nph_detect_polyi_batch(nph_ctx* ctx, const float* raw, size_t n_samples_total, const nph_polya_job* jobs, size_t n_jobs,
+                                      const float* ev_duration, size_t n_events_total, const nph_event_range* base_to_event,
+                                      size_t n_ranks_total, nph_polyi_result* results_out)
+{
+    return polya_batch<true>(ctx, raw, n_samples_total, jobs, n_jobs, ev_duration, n_events_total, base_to_event, n_ranks_total,
+                             results_out);
 }

@@ -10,7 +10,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from .synth import ABEA_RES_DT, ALIGN_STATE_DT, CALIBRATION_DT, EVENT_DT, EVENT_RANGE_DT, METH_SITE_DT, METHFREQ_PARAMS_DT, PAIR_DT, POLYA_RES_DT, RAW_RANGE_DT
+from .synth import ABEA_RES_DT, ALIGN_STATE_DT, CALIBRATION_DT, EVENT_DT, EVENT_RANGE_DT, METH_SITE_DT, METHFREQ_PARAMS_DT, PAIR_DT, POLYA_RES_DT, POLYI_RES_DT, RAW_RANGE_DT
 
 
 def _p(a):
@@ -451,6 +451,16 @@ class Engine:
         out = np.zeros(n, POLYA_RES_DT)
         self._check(self.lib.nph_polya_batch(self.ctx, _p(raw), raw.shape[0], _p(jobs), n, _p(ev_duration), ev_duration.shape[0],
                                              _p(base_to_event), base_to_event.shape[0], _p(out)), "nph_polya_batch")
+        return out
+
+    def detect_polyi_batch(self, raw, jobs, ev_duration, base_to_event):
+        """nanopolish detect-polyi's per-read result (polya_batch's fields under the poly(I) segmentation model, then the
+        poly(I) / poly(A) switch in the tail and its detection tag) for a batch in one call.  Takes polya_batch's inputs;
+        returns POLYI_RES_DT[n_jobs], which nanopolish_b200.detect_polyi.rows() turns into the reference's TSV rows."""
+        n = jobs.shape[0]
+        out = np.zeros(n, POLYI_RES_DT)
+        self._check(self.lib.nph_detect_polyi_batch(self.ctx, _p(raw), raw.shape[0], _p(jobs), n, _p(ev_duration), ev_duration.shape[0],
+                                                    _p(base_to_event), base_to_event.shape[0], _p(out)), "nph_detect_polyi_batch")
         return out
 
     # ---- measurement ----------------------------------------------------------------------

@@ -436,14 +436,16 @@ int nphh_load_from_raw(int model, int n, const float* samples, const uint64_t* s
 // the index) with its whole raw signal samples[sample_off[i] .. sample_off[i+1]) at sample_rate[i].  One device call; the
 // TSV (header included) goes to tsv_out.  Returns its length, or a negative status (NPH_ERR_INVALID with the length needed in
 // *n_needed if cap is too small).
-long long nphh_polya(int n, const char** names, const char** contigs, const int32_t* pos, const uint16_t* flag, const uint32_t* cigar,
-                     const uint64_t* cigar_off, const int32_t* read, const float* samples, const uint64_t* sample_off,
-                     const double* sample_rate, char* tsv_out, size_t cap, size_t* n_needed)
+// One batch of polya or detect-polyi records through Batch (PolyaBatch, DetectPolyiBatch), its TSV into tsv_out
+extern "C++" template <class Batch>
+long long polya_records_tsv(int n, const char** names, const char** contigs, const int32_t* pos, const uint16_t* flag,
+                            const uint32_t* cigar, const uint64_t* cigar_off, const int32_t* read, const float* samples,
+                            const uint64_t* sample_off, const double* sample_rate, char* tsv_out, size_t cap, size_t* n_needed)
 {
     std::string tsv;
     int rc = guard([&] {
         std::vector<RawRead> raw(n);
-        PolyaBatch batch;
+        Batch batch;
         for (int i = 0; i < n; ++i) {
             PolyaRecord r;
             r.read_name = names[i]; r.contig = contigs[i]; r.pos = pos[i]; r.flag = flag[i];
@@ -464,6 +466,23 @@ long long nphh_polya(int n, const char** names, const char** contigs, const int3
     if (tsv.size() > cap) return NPH_ERR_INVALID;
     memcpy(tsv_out, tsv.data(), tsv.size());
     return (long long)tsv.size();
+}
+
+long long nphh_polya(int n, const char** names, const char** contigs, const int32_t* pos, const uint16_t* flag, const uint32_t* cigar,
+                     const uint64_t* cigar_off, const int32_t* read, const float* samples, const uint64_t* sample_off,
+                     const double* sample_rate, char* tsv_out, size_t cap, size_t* n_needed)
+{
+    return polya_records_tsv<PolyaBatch>(n, names, contigs, pos, flag, cigar, cigar_off, read, samples, sample_off, sample_rate,
+                                         tsv_out, cap, n_needed);
+}
+
+// ---- detect-polyi over a batch of BAM records: nphh_polya's arguments, detect_polyi_main's TSV ---------------------------
+long long nphh_detect_polyi(int n, const char** names, const char** contigs, const int32_t* pos, const uint16_t* flag,
+                            const uint32_t* cigar, const uint64_t* cigar_off, const int32_t* read, const float* samples,
+                            const uint64_t* sample_off, const double* sample_rate, char* tsv_out, size_t cap, size_t* n_needed)
+{
+    return polya_records_tsv<DetectPolyiBatch>(n, names, contigs, pos, flag, cigar, cigar_off, read, samples, sample_off, sample_rate,
+                                               tsv_out, cap, n_needed);
 }
 
 // ---- N1: eventalign (segment chaining around the Viterbi kernel) -------------------------------------------

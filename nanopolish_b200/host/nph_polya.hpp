@@ -7,6 +7,11 @@
 // missing from the index or whose events load_from_raw cleared (:761-762) gives the READ_FAILED_LOAD row.  The samples are
 // the read's WHOLE raw signal (SquiggleRead::samples with SRF_LOAD_RAW_SAMPLES, squiggle_read.cpp:251-258): RawRead::samples.
 // The verbose modes (per-sample and per-k-mer dumps) are not provided.
+//
+// DetectPolyiBatch is nanopolish detect-polyi (src/nanopolish_detect_polyi.cpp) the same way: dpi_estimate_polya_for_single_read
+// (:1008-1144) for every record, with the same per-record rules (:1018-1052) and one nph_detect_polyi_batch call, and
+// detect_polyi_main's TSV (:1159 header, :1040-1041 and :1105-1108 rows).  Its verbose modes (-v: the per-sample and per-k-mer
+// dumps) are not provided either.
 #pragma once
 #include "nph_raw.hpp"
 
@@ -41,6 +46,23 @@ private:
     std::vector<PolyaRecord> m_records;
     std::vector<nph_polya_result> m_results;
     std::vector<PolyaRecord> m_done;      // the records m_results belong to
+};
+
+class DetectPolyiBatch {
+public:
+    // PolyaBatch::add's rules
+    bool add(const PolyaRecord& rec);
+    // One nph_detect_polyi_batch call over the records added since the last run; their results replace the previous ones.
+    void run(Engine& engine);
+    const std::vector<nph_polyi_result>& results() const { return m_results; }
+    // The rows of the last run in record order, preceded by detect_polyi_main's header line if header is set.
+    std::string tsv(bool header = true) const;
+    void clear();
+
+private:
+    std::vector<PolyaRecord> m_records;
+    std::vector<nph_polyi_result> m_results;
+    std::vector<PolyaRecord> m_done;
 };
 
 } // namespace nph

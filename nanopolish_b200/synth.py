@@ -70,6 +70,10 @@ POLYA_JOB_DT = np.dtype([("sample_off", "<u8"), ("event_off", "<u8"), ("rank_off
 POLYA_RES_DT = np.dtype([("start", "<u8"), ("leader", "<u8"), ("adapter", "<u8"), ("polya", "<u8"), ("cliffs", "<u8"),
                          ("read_rate", "<f8"), ("polya_length", "<f8"), ("qc", "<i4"), ("reserved", "<u4")], align=True)
 assert POLYA_JOB_DT.itemsize == 80 and POLYA_RES_DT.itemsize == 64
+# nph_polyi_result (include/nph.h)
+POLYI_RES_DT = np.dtype([("seg", POLYA_RES_DT), ("polyi_last", "<i4"), ("polya_first", "<i4"), ("detected", "<i4"),
+                         ("reserved", "<u4")], align=True)
+assert POLYI_RES_DT.itemsize == 80
 METH_RECORD_DT = np.dtype([("ref_off", "<u8"), ("pair_off", "<u8"), ("read", "<u4"), ("model_id", "<u4"), ("ref_len", "<u4"),
                            ("n_pairs", "<u4"), ("ref_start_pos", "<i4"), ("rc", "u1"), ("strand", "u1"), ("reserved", "u1", 2)], align=True)
 METH_SITE_DT = np.dtype([("start_position", "<i4"), ("end_position", "<i4"), ("n_motif", "<u4"), ("record", "<u4"),
