@@ -120,12 +120,19 @@ typedef struct { int32_t ref_pos; int32_t read_pos; } nph_aligned_pair;
 #define NPH_ABEA_MAX_GAP         4   /* more than 50 consecutive skipped k-mers */
 #define NPH_ABEA_NO_END_CELL     8   /* last k-mer column never inside the band (reference behaviour undefined) */
 #define NPH_ABEA_PAIRS_OVERFLOW 16   /* pairs_cap too small */
+/* The record of a job that fails:
+ *   NPH_ABEA_NO_END_CELL    : no path is walked.  status is that bit alone; n_aligned 0, max_gap 0, avg_log_emission 0.
+ *   NPH_ABEA_PAIRS_OVERFLOW : the whole path is walked but QC is not run.  status is that bit alone; n_aligned and max_gap
+ *                             are the path's, avg_log_emission is 0.  The job's slot holds pairs in no defined order.
+ *   otherwise               : QC ran on the whole path; status is the bit-or of the QC bits (LOW_EMISSION, NOT_SPANNED,
+ *                             MAX_GAP) and n_aligned, max_gap and avg_log_emission are the path's.
+ * n_pairs is 0 for every failure.  A job never writes outside [pairs_off, pairs_off + pairs_cap). */
 typedef struct {
     uint32_t n_pairs;         /* 0 when the reference would have returned an empty vector */
     int32_t  status;          /* bit-or of NPH_ABEA_* */
-    int32_t  max_gap;
+    int32_t  max_gap;         /* longest run of skipped k-mers on the path */
     uint32_t n_aligned;       /* path length before QC (== n_pairs when status == 0) */
-    double   avg_log_emission;
+    double   avg_log_emission;   /* mean emission over the path, summed in path order in FP64 */
 } nph_abea_result;
 
 /* One Viterbi state of profile_hmm_align.  ref: HMMAlignmentState (src/common/nanopolish_common.h:65-73);
@@ -211,7 +218,12 @@ int nph_score_set_combine(const float* scores, size_t n_groups, uint32_t n_alt, 
 /* ---- adaptive_banded_simple_event_align -------------------------------------------------
  * One-shot, host buffers (synchronous). pairs_out receives, for job j, results[j].n_pairs
  * AlignedPairs at pairs_out + jobs[j].pairs_off in the reference's order (ascending).
- * Both forms return NPH_ERR_INVALID for a k-mer rank >= the model's n_states. */
+ * Both forms return NPH_ERR_INVALID for a k-mer rank >= the model's n_states, and for a batch with an event level outside
+ * [-NPH_ABEA_MAX_LEVEL, NPH_ABEA_MAX_LEVEL] (NaN included) anywhere in the loaded events.  The device Gaussian is exact where
+ * |level - mu'| < 2^12 (exact_math.cuh), which these levels keep for any model mean below 2048 pA.  Outside it the device and
+ * the reference part: +-inf turns the device's division into NaN where the reference's gives -inf, and from
+ * |level - mu'| / sigma' >= 2^64 the device's square overflows to -inf where the reference's (-0.5f * a) * a stays finite. */
+#define NPH_ABEA_MAX_LEVEL 2048.0f
 int nph_abea_batch(nph_ctx* ctx,
                    const nph_read* reads, size_t n_reads,
                    const float* ev_mean, const double* ev_start_time, size_t n_events_total,
@@ -690,7 +702,9 @@ int nph_recalibrate_batch(nph_ctx* ctx, const nph_read* reads, size_t n_reads, c
  * clears the read's events; the arrays still hold them), base_to_event_out[rank_off + ki] (optional).
  * A read that trims to nothing (the reference aborts on it) gets no events and NPH_CAL_EMPTY_AFTER_TRIM.
  * NPH_ERR_UNSUPPORTED if events_cap is too small (n_samples_total / 3 always suffices).  NPH_ERR_INVALID for a k-mer rank
- * >= the model's n_states, before any step runs. */
+ * >= the model's n_states, and for any sample of raw[0, n_samples_total) outside [-NPH_ABEA_MAX_LEVEL, NPH_ABEA_MAX_LEVEL] (NaN
+ * included; samples outside every job's slice too), before any step runs: an event's level is a mean of its samples, so this
+ * keeps the events inside the range nph_abea_batch takes. */
 #define NPH_CAL_EMPTY_AFTER_TRIM 16
 typedef struct {
     uint64_t sample_off;      /* first raw sample (picoamps, float) of this read in raw[] */

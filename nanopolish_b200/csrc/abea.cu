@@ -404,11 +404,13 @@ __global__ void __launch_bounds__(kThreads) mom_kernel(const MomParams p)
     }
 }
 
-// nph_check_ranks: *bad = 1 if a rank is not a state of the model
-__global__ void check_ranks_kernel(const uint32_t* ranks, size_t n, uint32_t n_states, unsigned int* bad)
+// nph_check_ranks: *bad |= 1 if a rank is not a state of the model, |= 2 if a level is NaN or |level| > NPH_ABEA_MAX_LEVEL
+__global__ void check_ranks_kernel(const uint32_t* ranks, size_t n, uint32_t n_states, const float* levels, size_t n_levels, unsigned int* bad)
 {
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-        if (ranks[i] >= n_states) *bad = 1u;
+        if (ranks[i] >= n_states) atomicOr(bad, 1u);
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n_levels; i += (size_t)gridDim.x * blockDim.x)
+        if (!(fabsf(levels[i]) <= NPH_ABEA_MAX_LEVEL)) atomicOr(bad, 2u);
 }
 
 // per warp: kmax Gaussians, then trace_stride bytes of band trace
@@ -468,16 +470,18 @@ int nph_launch_mom(nph_ctx* ctx, const nph_abea_job* d_jobs, const uint32_t* d_r
     return NPH_OK;
 }
 
-int nph_check_ranks(nph_ctx* ctx, const uint32_t* d_ranks, size_t n, uint32_t n_states)
+int nph_check_ranks(nph_ctx* ctx, const uint32_t* d_ranks, size_t n, uint32_t n_states, const float* d_levels, size_t n_levels)
 {
     unsigned int* flag = ctx->d_counters.p + (NPH_NUM_COUNTERS - 2);
     unsigned int bad = 0;
+    const size_t m = std::max(n, n_levels);
     NPH_CUDA(ctx, cudaMemsetAsync(flag, 0, sizeof(unsigned int), ctx->stream));
-    if (n) check_ranks_kernel<<<(unsigned)std::min<size_t>((n + 255) / 256, (size_t)ctx->sm_count * 8), 256, 0, ctx->stream>>>(d_ranks, n, n_states, flag);
+    if (m) check_ranks_kernel<<<(unsigned)std::min<size_t>((m + 255) / 256, (size_t)ctx->sm_count * 8), 256, 0, ctx->stream>>>(d_ranks, n, n_states, d_levels, n_levels, flag);
     NPH_CUDA(ctx, cudaGetLastError());
     NPH_CUDA(ctx, cudaMemcpyAsync(&bad, flag, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));
     NPH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    if (bad) { ctx->last_error = "a k-mer rank is not a state of the model"; return NPH_ERR_INVALID; }
+    if (bad & 1u) { ctx->last_error = "a k-mer rank is not a state of the model"; return NPH_ERR_INVALID; }
+    if (bad & 2u) { ctx->last_error = "an event level is NaN or beyond NPH_ABEA_MAX_LEVEL"; return NPH_ERR_INVALID; }
     return NPH_OK;
 }
 
@@ -535,7 +539,8 @@ int nph_abea_jobs_load(nph_ctx* ctx, const uint32_t* kmer_ranks, size_t n_ranks_
         NPH_CUDA(ctx, cudaSetDevice(ctx->device));
         NPH_TRY(nph_abea_stage(ctx, ctx->h_read_n_events.data(), jobs, n_jobs, n_ranks_total, model_id, pairs_total));
         NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_abea_ranks.p, kmer_ranks, sizeof(uint32_t) * n_ranks_total, cudaMemcpyHostToDevice, ctx->stream));
-        return nph_check_ranks(ctx, ctx->d_abea_ranks.p, n_ranks_total, ctx->models[model_id].n_states);   // the call's one sync
+        // the call's one sync.  Levels outside [-NPH_ABEA_MAX_LEVEL, NPH_ABEA_MAX_LEVEL] leave the Gaussian's proven domain: refused
+        return nph_check_ranks(ctx, ctx->d_abea_ranks.p, n_ranks_total, ctx->models[model_id].n_states, ctx->d_level.p, ctx->n_events_total);
     };
     const int rc = stage();
     ctx->abea_loaded = rc == NPH_OK;      // from the first upload on, the ABEA buffers hold this batch

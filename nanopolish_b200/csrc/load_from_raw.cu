@@ -122,9 +122,10 @@ extern "C" int nph_load_from_raw_batch(nph_ctx* ctx, const float* raw, size_t n_
     }));
     NPH_TRY(nph_reserve(ctx, ctx->d_abea_ranks, n_ranks_total));       // where MoM, ABEA and the calibration read them
     NPH_CUDA(ctx, cudaMemcpyAsync(ctx->d_abea_ranks.p, kmer_ranks, sizeof(uint32_t) * n_ranks_total, cudaMemcpyHostToDevice, ctx->stream));
-    NPH_TRY(nph_check_ranks(ctx, ctx->d_abea_ranks.p, n_ranks_total, ctx->models[model_id].n_states));
-    ctx->reads_loaded = false; ctx->jobs_loaded = false;    // the resident reads are replaced
     NPH_CUDA(ctx, cudaMemcpyAsync(d_raw, raw, sizeof(float) * n_samples_total, cudaMemcpyHostToDevice, ctx->stream));
+    // samples within +-NPH_ABEA_MAX_LEVEL give event levels ABEA takes (include/nph.h); the whole buffer is checked
+    NPH_TRY(nph_check_ranks(ctx, ctx->d_abea_ranks.p, n_ranks_total, ctx->models[model_id].n_states, d_raw, n_samples_total));
+    ctx->reads_loaded = false; ctx->jobs_loaded = false;    // the resident reads are replaced
     NPH_CUDA(ctx, cudaEventRecord(ctx->ev0, ctx->stream));
     int launches = 0;
     float staged_ms = 0.0f, ms = 0.0f;          // device time of the stages, summed (each stage ends in a sync)

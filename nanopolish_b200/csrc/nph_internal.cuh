@@ -422,5 +422,7 @@ int nph_launch_mom(nph_ctx* ctx, const nph_abea_job* d_jobs, const uint32_t* d_r
 // not synchronise.
 int nph_abea_stage(nph_ctx* ctx, const uint32_t* n_events, const nph_abea_job* jobs, size_t n_jobs, size_t n_ranks_total, uint32_t model_id,
                    size_t pairs_total);
-// NPH_ERR_INVALID unless every rank of d_ranks[0, n) is below n_states: one kernel, one flag copied back (a stream sync).
-int nph_check_ranks(nph_ctx* ctx, const uint32_t* d_ranks, size_t n, uint32_t n_states);
+// NPH_ERR_INVALID unless every rank of d_ranks[0, n) is below n_states and every level of d_levels[0, n_levels) is within
+// +-NPH_ABEA_MAX_LEVEL:
+// one kernel, one flag copied back (a stream sync).
+int nph_check_ranks(nph_ctx* ctx, const uint32_t* d_ranks, size_t n, uint32_t n_states, const float* d_levels = nullptr, size_t n_levels = 0);

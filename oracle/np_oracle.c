@@ -425,9 +425,10 @@ void npo_mom(const nph_read* reads, const float* ev_mean, const npo_model* model
 #define BW 100
 enum { FROM_D = 0, FROM_U = 1, FROM_L = 2 };
 
-int64_t npo_abea(const nph_read* reads, const float* ev_mean, const double* ev_start_time,
-                 const npo_model* model, const uint32_t* kmer_ranks, const nph_abea_job* job,
-                 nph_aligned_pair* pairs_out, nph_abea_result* res)
+/* ll_k_out (n_events + n_kmers + 2 entries, or NULL): the k-mer index of each band's lower-left cell, band 0 first */
+static int64_t abea_core(const nph_read* reads, const float* ev_mean, const double* ev_start_time,
+                         const npo_model* model, const uint32_t* kmer_ranks, const nph_abea_job* job,
+                         nph_aligned_pair* pairs_out, nph_abea_result* res, int32_t* ll_k_out)
 {
     const nph_read* read = &reads[job->read];
     const uint32_t* ranks = kmer_ranks + job->rank_off;
@@ -520,10 +521,12 @@ int64_t npo_abea(const nph_read* reads, const float* ev_mean, const double* ev_s
         }
     }
 
+    /* The result record of a failed job follows include/nph.h: NO_END_CELL walks no path; PAIRS_OVERFLOW walks the whole
+     * path (n_aligned, max_gap) but skips QC.  Either carries only its own bit and avg_log_emission 0. */
     int64_t n_out = 0;
     double sum_emission = 0, n_aligned = 0;
     int cur_gap = 0, max_gap = 0, status = found ? 0 : NPH_ABEA_NO_END_CELL;
-    while (cur_k >= 0 && cur_e >= 0) {
+    while (found && cur_k >= 0 && cur_e >= 0) {
         if ((uint64_t)n_out < job->pairs_cap) { pairs_out[n_out].ref_pos = (int32_t)cur_k; pairs_out[n_out].read_pos = (int32_t)cur_e; }
         else status |= NPH_ABEA_PAIRS_OVERFLOW;
         n_out++;
@@ -540,13 +543,14 @@ int64_t npo_abea(const nph_read* reads, const float* ev_mean, const double* ev_s
         for (int64_t i = 0, j = n_out - 1; i < j; ++i, --j) { nph_aligned_pair t = pairs_out[i]; pairs_out[i] = pairs_out[j]; pairs_out[j] = t; }
     }
 
-    double avg = sum_emission / n_aligned;
-    int spanned = 0;
-    if (n_out > 0 && !(status & NPH_ABEA_PAIRS_OVERFLOW))
-        spanned = pairs_out[0].ref_pos == 0 && pairs_out[n_out - 1].ref_pos == n_kmers - 1;
-    if (avg < min_average_log_emission) status |= NPH_ABEA_LOW_EMISSION;
-    if (!spanned) status |= NPH_ABEA_NOT_SPANNED;
-    if (max_gap > max_gap_threshold) status |= NPH_ABEA_MAX_GAP;
+    double avg = 0.0;
+    if (!status) {
+        avg = sum_emission / n_aligned;
+        int spanned = pairs_out[0].ref_pos == 0 && pairs_out[n_out - 1].ref_pos == n_kmers - 1;
+        if (avg < min_average_log_emission) status |= NPH_ABEA_LOW_EMISSION;
+        if (!spanned) status |= NPH_ABEA_NOT_SPANNED;
+        if (max_gap > max_gap_threshold) status |= NPH_ABEA_MAX_GAP;
+    }
 
     if (res) {
         res->n_aligned = (uint32_t)n_out;
@@ -555,10 +559,28 @@ int64_t npo_abea(const nph_read* reads, const float* ev_mean, const double* ev_s
         res->max_gap = max_gap;
         res->avg_log_emission = avg;
     }
+    if (ll_k_out)
+        for (long bi = 0; bi < n_bands; ++bi) ll_k_out[bi] = ll_k[bi];
     free(bands); free(trace); free(ll_e); free(ll_k);
     return status ? 0 : n_out;
 #undef BAND
 #undef TRACE
+}
+
+int64_t npo_abea(const nph_read* reads, const float* ev_mean, const double* ev_start_time,
+                 const npo_model* model, const uint32_t* kmer_ranks, const nph_abea_job* job,
+                 nph_aligned_pair* pairs_out, nph_abea_result* res)
+{
+    return abea_core(reads, ev_mean, ev_start_time, model, kmer_ranks, job, pairs_out, res, NULL);
+}
+
+/* npo_abea, plus the band history: ll_k_out[bi] = k-mer index of band bi's lower-left cell for the n_events + n_kmers + 2
+ * bands (the band's columns are k-mers ll_k_out[bi] .. ll_k_out[bi] + 99; the trim column is k-mer -1) */
+int64_t npo_abea_bands(const nph_read* reads, const float* ev_mean, const double* ev_start_time,
+                       const npo_model* model, const uint32_t* kmer_ranks, const nph_abea_job* job,
+                       nph_aligned_pair* pairs_out, nph_abea_result* res, int32_t* ll_k_out)
+{
+    return abea_core(reads, ev_mean, ev_start_time, model, kmer_ranks, job, pairs_out, res, ll_k_out);
 }
 
 double npo_abea_batch(const nph_read* reads, const float* ev_mean, const double* ev_start_time,

@@ -46,6 +46,9 @@ uint32_t npo_hmm_align(const nph_read* reads, const float* ev_mean, const double
 int64_t npo_abea(const nph_read* reads, const float* ev_mean, const double* ev_start_time,
                  const npo_model* model, const uint32_t* kmer_ranks, const nph_abea_job* job,
                  nph_aligned_pair* pairs_out, nph_abea_result* res);
+int64_t npo_abea_bands(const nph_read* reads, const float* ev_mean, const double* ev_start_time,
+                       const npo_model* model, const uint32_t* kmer_ranks, const nph_abea_job* job,
+                       nph_aligned_pair* pairs_out, nph_abea_result* res, int32_t* ll_k_out);
 double npo_abea_batch(const nph_read* reads, const float* ev_mean, const double* ev_start_time,
                       const npo_model* model, const uint32_t* kmer_ranks, const nph_abea_job* jobs,
                       size_t n_jobs, int threads, nph_aligned_pair* pairs_out, nph_abea_result* res);

@@ -121,6 +121,17 @@ class PortOracle:
                                        C.c_size_t(jobs.shape[0]), C.c_int(threads), _p(pairs), _p(res))
         return pairs, res, secs
 
+    def abea_bands(self, reads, ev_mean, ev_start, model, kmer_ranks, job):
+        """npo_abea on one job with its own pairs_cap: (pairs, result, ll_k) with ll_k[bi] the k-mer of band bi's lower-left cell"""
+        from nanopolish_b200.synth import PAIR_DT, ABEA_RES_DT
+        jb = np.array([job], dtype=job.dtype)
+        n_bands = int(reads[int(job["read"])]["n_events"]) + int(job["n_kmers"]) + 2
+        pairs = np.zeros(max(int(job["pairs_cap"]), 1), PAIR_DT)
+        res = np.zeros(1, ABEA_RES_DT)
+        ll_k = np.zeros(n_bands, np.int32)
+        self.lib.npo_abea_bands(_p(reads), _p(ev_mean), _p(ev_start), self.models([model]), _p(kmer_ranks), _p(jb), _p(pairs), _p(res), _p(ll_k))
+        return pairs[:int(job["pairs_cap"])], res[0], ll_k
+
     def mom(self, reads, ev_mean, model, kmer_ranks, job):
         marr = self.models([model])
         sh, sc = C.c_double(), C.c_double()
