@@ -447,20 +447,19 @@ class Engine:
         raw: float32 whole raw signals; jobs: POLYA_JOB_DT; ev_duration: float32 event durations; base_to_event:
         EVENT_RANGE_DT (the layout of load_from_raw_batch's outputs).  Returns POLYA_RES_DT[n_jobs];
         nanopolish_b200.polya.rows() turns it into the reference's TSV rows."""
-        n = jobs.shape[0]
-        out = np.zeros(n, POLYA_RES_DT)
-        self._check(self.lib.nph_polya_batch(self.ctx, _p(raw), raw.shape[0], _p(jobs), n, _p(ev_duration), ev_duration.shape[0],
-                                             _p(base_to_event), base_to_event.shape[0], _p(out)), "nph_polya_batch")
-        return out
+        return self._tail_batch("nph_polya_batch", POLYA_RES_DT, raw, jobs, ev_duration, base_to_event)
 
     def detect_polyi_batch(self, raw, jobs, ev_duration, base_to_event):
         """nanopolish detect-polyi's per-read result (polya_batch's fields under the poly(I) segmentation model, then the
         poly(I) / poly(A) switch in the tail and its detection tag) for a batch in one call.  Takes polya_batch's inputs;
         returns POLYI_RES_DT[n_jobs], which nanopolish_b200.detect_polyi.rows() turns into the reference's TSV rows."""
+        return self._tail_batch("nph_detect_polyi_batch", POLYI_RES_DT, raw, jobs, ev_duration, base_to_event)
+
+    def _tail_batch(self, symbol, result_dt, raw, jobs, ev_duration, base_to_event):
         n = jobs.shape[0]
-        out = np.zeros(n, POLYI_RES_DT)
-        self._check(self.lib.nph_detect_polyi_batch(self.ctx, _p(raw), raw.shape[0], _p(jobs), n, _p(ev_duration), ev_duration.shape[0],
-                                                    _p(base_to_event), base_to_event.shape[0], _p(out)), "nph_detect_polyi_batch")
+        out = np.zeros(n, result_dt)
+        self._check(getattr(self.lib, symbol)(self.ctx, _p(raw), raw.shape[0], _p(jobs), n, _p(ev_duration), ev_duration.shape[0],
+                                              _p(base_to_event), base_to_event.shape[0], _p(out)), symbol)
         return out
 
     # ---- measurement ----------------------------------------------------------------------

@@ -77,89 +77,82 @@ void append_failed_row(std::string& out, std::vector<char>& buf, const PolyaReco
     append_row(out, buf, "%s\t%s\t%d\t-1.0\t-1.0\t-1.0\t-1.0\t-1.00\t-1.00\tREAD_FAILED_LOAD\n", r.read_name.c_str(), r.contig.c_str(), r.pos);
 }
 
+// What each tail caller supplies: its device call, the name add() refuses records under, its header line, where its result
+// keeps the segmentation, and its row's columns between polya_length and qc_tag
+template <class Result> struct Tail;
+
+template <> struct Tail<nph_polya_result> {
+    static constexpr auto call = nph_polya_batch;
+    static constexpr const char* call_name = "nph_polya_batch";
+    static constexpr const char* add_name = "nph::PolyaBatch::add";
+    static constexpr const char* header =       // :877
+        "readname\tcontig\tposition\tleader_start\tadapter_start\tpolya_start\ttranscript_start\tread_rate\tpolya_length\tqc_tag\n";
+    static const nph_polya_result& seg(const nph_polya_result& r) { return r; }
+    static const char* columns(const nph_polya_result&) { return ""; }
+};
+
+template <> struct Tail<nph_polyi_result> {
+    static constexpr auto call = nph_detect_polyi_batch;
+    static constexpr const char* call_name = "nph_detect_polyi_batch";
+    static constexpr const char* add_name = "nph::DetectPolyiBatch::add";     // detect_polyi.cpp:1018-1020
+    static constexpr const char* header =       // detect_polyi.cpp:1159
+        "readname\tcontig\tposition\tleader_start\tadapter_start\tpolya_start\ttranscript_start\tread_rate\tpolya_length\tdetected\tqc_tag\n";
+    static const nph_polya_result& seg(const nph_polyi_result& r) { return r.seg; }
+    // the detected column and its tab (detect_polyi.cpp:1098-1108)
+    static const char* columns(const nph_polyi_result& r)
+    {
+        static const char* const kDetected[] = {"NONE\t", "POLYA-ONLY\t", "POLYI-ONLY\t", "A+I\t"};
+        return kDetected[r.detected];
+    }
+};
+
 } // namespace
 
-bool PolyaBatch::add(const PolyaRecord& rec)
+template <class Result>
+bool TailBatch<Result>::add(const PolyaRecord& rec)
 {
-    if (!accept(rec, "nph::PolyaBatch::add")) return false;
+    if (!accept(rec, Tail<Result>::add_name)) return false;
     m_records.push_back(rec);
     return true;
 }
 
-void PolyaBatch::clear() { m_records.clear(); m_results.clear(); m_done.clear(); }
+template <class Result>
+void TailBatch<Result>::clear() { m_records.clear(); m_results.clear(); m_done.clear(); }
 
-void PolyaBatch::run(Engine& engine)
+template <class Result>
+void TailBatch<Result>::run(Engine& engine)
 {
     const size_t n = m_records.size();
     PolyaInputs in = pack(m_records);
-    std::vector<nph_polya_result> res(n);
-    engine.check(nph_polya_batch(engine.ctx(), in.raw.data(), in.raw.size(), in.jobs.data(), n, in.dur.data(), in.dur.size(), in.b2e.data(),
-                                 in.b2e.size(), res.data()), "nph_polya_batch");
+    std::vector<Result> res(n);
+    engine.check(Tail<Result>::call(engine.ctx(), in.raw.data(), in.raw.size(), in.jobs.data(), n, in.dur.data(), in.dur.size(),
+                                    in.b2e.data(), in.b2e.size(), res.data()), Tail<Result>::call_name);
     m_results.swap(res);
     m_done.swap(m_records);
     m_records.clear();
 }
 
-std::string PolyaBatch::tsv(bool header) const
+template <class Result>
+std::string TailBatch<Result>::tsv(bool header) const
 {
     std::string out;
-    if (header)     // :877
-        out += "readname\tcontig\tposition\tleader_start\tadapter_start\tpolya_start\ttranscript_start\tread_rate\tpolya_length\tqc_tag\n";
+    if (header) out += Tail<Result>::header;
     std::vector<char> buf(256);
     for (size_t i = 0; i < m_done.size(); ++i) {
         const PolyaRecord& r = m_done[i];
-        const nph_polya_result& s = m_results[i];
+        const nph_polya_result& s = Tail<Result>::seg(m_results[i]);
         if (s.qc == NPH_POLYA_READ_FAILED_LOAD)
             append_failed_row(out, buf, r);
         else                                           // :816-826, the indices + 1 in size_t
-            append_row(out, buf, "%s\t%s\t%d\t%.1lf\t%.1lf\t%.1lf\t%.1lf\t%.2lf\t%.2lf\t%s\n",
-                       r.read_name.c_str(), r.contig.c_str(), r.pos, (double)(uint64_t)(s.start + 1), (double)(uint64_t)(s.leader + 1),
-                       (double)(uint64_t)(s.adapter + 1), (double)(uint64_t)(s.polya + 1), s.read_rate, s.polya_length, kQcTags[s.qc]);
-    }
-    return out;
-}
-
-bool DetectPolyiBatch::add(const PolyaRecord& rec)
-{
-    if (!accept(rec, "nph::DetectPolyiBatch::add")) return false;   // detect_polyi.cpp:1018-1020
-    m_records.push_back(rec);
-    return true;
-}
-
-void DetectPolyiBatch::clear() { m_records.clear(); m_results.clear(); m_done.clear(); }
-
-void DetectPolyiBatch::run(Engine& engine)
-{
-    const size_t n = m_records.size();
-    PolyaInputs in = pack(m_records);
-    std::vector<nph_polyi_result> res(n);
-    engine.check(nph_detect_polyi_batch(engine.ctx(), in.raw.data(), in.raw.size(), in.jobs.data(), n, in.dur.data(), in.dur.size(),
-                                        in.b2e.data(), in.b2e.size(), res.data()), "nph_detect_polyi_batch");
-    m_results.swap(res);
-    m_done.swap(m_records);
-    m_records.clear();
-}
-
-std::string DetectPolyiBatch::tsv(bool header) const
-{
-    static const char* const kDetected[] = {"NONE", "POLYA-ONLY", "POLYI-ONLY", "A+I"};
-    std::string out;
-    if (header)     // detect_polyi.cpp:1159
-        out += "readname\tcontig\tposition\tleader_start\tadapter_start\tpolya_start\ttranscript_start\tread_rate\tpolya_length\tdetected\tqc_tag\n";
-    std::vector<char> buf(256);
-    for (size_t i = 0; i < m_done.size(); ++i) {
-        const PolyaRecord& r = m_done[i];
-        const nph_polyi_result& d = m_results[i];
-        const nph_polya_result& s = d.seg;
-        if (s.qc == NPH_POLYA_READ_FAILED_LOAD)
-            append_failed_row(out, buf, r);
-        else                                           // detect_polyi.cpp:1098-1108
-            append_row(out, buf, "%s\t%s\t%d\t%.1lf\t%.1lf\t%.1lf\t%.1lf\t%.2lf\t%.2lf\t%s\t%s\n",
+            append_row(out, buf, "%s\t%s\t%d\t%.1lf\t%.1lf\t%.1lf\t%.1lf\t%.2lf\t%.2lf\t%s%s\n",
                        r.read_name.c_str(), r.contig.c_str(), r.pos, (double)(uint64_t)(s.start + 1), (double)(uint64_t)(s.leader + 1),
                        (double)(uint64_t)(s.adapter + 1), (double)(uint64_t)(s.polya + 1), s.read_rate, s.polya_length,
-                       kDetected[d.detected], kQcTags[s.qc]);
+                       Tail<Result>::columns(m_results[i]), kQcTags[s.qc]);
     }
     return out;
 }
+
+template class TailBatch<nph_polya_result>;
+template class TailBatch<nph_polyi_result>;
 
 } // namespace nph

@@ -30,39 +30,28 @@ struct PolyaRecord {
     const RawRead* raw = nullptr;         // the read's whole raw signal and sample rate (required when read is set)
 };
 
-class PolyaBatch {
+// One tail caller over a batch of records.  Result selects the caller: nph_polya_result is polya (nph_polya_batch,
+// polya_main's TSV), nph_polyi_result is detect-polyi (nph_detect_polyi_batch, detect_polyi_main's TSV).
+template <class Result>
+class TailBatch {
 public:
     // Adds a record; returns false (no row) for a secondary alignment.  Throws Error(NPH_ERR_INVALID) for a record without a
     // CIGAR (the reference reads cigar[n_cigar - 1]).
     bool add(const PolyaRecord& rec);
-    // One nph_polya_batch call over the records added since the last run; their results replace the previous ones.
+    // One device call over the records added since the last run; their results replace the previous ones.
     void run(Engine& engine);
-    const std::vector<nph_polya_result>& results() const { return m_results; }
-    // The rows of the last run in record order, preceded by polya_main's header line if header is set.
+    const std::vector<Result>& results() const { return m_results; }
+    // The rows of the last run in record order, preceded by the caller's header line if header is set.
     std::string tsv(bool header = true) const;
     void clear();
 
 private:
     std::vector<PolyaRecord> m_records;
-    std::vector<nph_polya_result> m_results;
+    std::vector<Result> m_results;
     std::vector<PolyaRecord> m_done;      // the records m_results belong to
 };
 
-class DetectPolyiBatch {
-public:
-    // PolyaBatch::add's rules
-    bool add(const PolyaRecord& rec);
-    // One nph_detect_polyi_batch call over the records added since the last run; their results replace the previous ones.
-    void run(Engine& engine);
-    const std::vector<nph_polyi_result>& results() const { return m_results; }
-    // The rows of the last run in record order, preceded by detect_polyi_main's header line if header is set.
-    std::string tsv(bool header = true) const;
-    void clear();
-
-private:
-    std::vector<PolyaRecord> m_records;
-    std::vector<nph_polyi_result> m_results;
-    std::vector<PolyaRecord> m_done;
-};
+using PolyaBatch = TailBatch<nph_polya_result>;
+using DetectPolyiBatch = TailBatch<nph_polyi_result>;
 
 } // namespace nph

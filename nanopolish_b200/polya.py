@@ -18,13 +18,20 @@ def _size_t_plus_one(v: int) -> float:
     return float((int(v) + 1) % (1 << 64))
 
 
+def _row(name: str, contig: str, pos: int, seg, extra=()) -> str:
+    """The row of one record from its POLYA_RES_DT segmentation, with the extra columns before qc_tag; a read that failed to
+    load gets the 10-column row without them."""
+    if int(seg["qc"]) == READ_FAILED_LOAD:
+        return "%s\t%s\t%d\t-1.0\t-1.0\t-1.0\t-1.0\t-1.00\t-1.00\tREAD_FAILED_LOAD\n" % (name, contig, pos)
+    numbers = "%s\t%s\t%d\t%.1f\t%.1f\t%.1f\t%.1f\t%.2f\t%.2f" % (
+        name, contig, pos, _size_t_plus_one(seg["start"]), _size_t_plus_one(seg["leader"]), _size_t_plus_one(seg["adapter"]),
+        _size_t_plus_one(seg["polya"]), float(seg["read_rate"]), float(seg["polya_length"]))
+    return "\t".join([numbers, *extra, QC_TAGS[int(seg["qc"])]]) + "\n"
+
+
 def row(name: str, contig: str, pos: int, res) -> str:
     """The row of one record; res is one POLYA_RES_DT element."""
-    if int(res["qc"]) == READ_FAILED_LOAD:
-        return "%s\t%s\t%d\t-1.0\t-1.0\t-1.0\t-1.0\t-1.00\t-1.00\tREAD_FAILED_LOAD\n" % (name, contig, pos)
-    return "%s\t%s\t%d\t%.1f\t%.1f\t%.1f\t%.1f\t%.2f\t%.2f\t%s\n" % (
-        name, contig, pos, _size_t_plus_one(res["start"]), _size_t_plus_one(res["leader"]), _size_t_plus_one(res["adapter"]),
-        _size_t_plus_one(res["polya"]), float(res["read_rate"]), float(res["polya_length"]), QC_TAGS[int(res["qc"])])
+    return _row(name, contig, pos, res)
 
 
 def rows(names, contigs, positions, results) -> str:

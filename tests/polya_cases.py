@@ -118,40 +118,52 @@ def pack(reads):
     return cat(raw, np.float32), jobs, cat(dur, np.float32), cat(b2e, EVENT_RANGE_DT)
 
 
-class RefPolya:
-    """The reference's own poly(A) functions (oracle/polya_harness.cpp)."""
+class RefTail:
+    """The compiled reference's entry points of one tail caller (oracle/*_harness.cpp): npref_<prefix>_read, whose n_extra
+    further result pointers come after the QC one, npref_<prefix>_failed_row and npref_<prefix>_time."""
 
-    def __init__(self):
-        self.lib = C.CDLL(REF_POLYA)
+    def __init__(self, path: str, prefix: str, n_extra: int):
+        self.lib = C.CDLL(path)
         vp, sz = C.c_void_p, C.c_size_t
-        self.lib.npref_polya_read.restype = C.c_longlong
-        self.lib.npref_polya_read.argtypes = [C.c_char_p, C.c_char_p, C.c_int, C.c_uint32, vp, sz, C.c_double, C.c_double,
-                                              C.c_double, C.c_double, vp, sz, vp, vp, sz, vp, vp, vp, vp, sz]
-        self.lib.npref_polya_failed_row.restype = C.c_longlong
-        self.lib.npref_polya_failed_row.argtypes = [C.c_char_p, C.c_char_p, C.c_int, vp, sz]
-        self.lib.npref_polya_time.restype = C.c_double
-        self.lib.npref_polya_time.argtypes = [vp, sz, C.c_double, C.c_double, C.c_double, C.c_double, vp, sz, vp, vp, sz]
+        self._read = getattr(self.lib, f"npref_{prefix}_read")
+        self._read.restype = C.c_longlong
+        self._read.argtypes = [C.c_char_p, C.c_char_p, C.c_int, C.c_uint32, vp, sz, C.c_double, C.c_double, C.c_double, C.c_double,
+                               vp, sz, vp, vp, sz, vp, vp, vp] + [vp] * n_extra + [vp, sz]
+        self._failed_row = getattr(self.lib, f"npref_{prefix}_failed_row")
+        self._failed_row.restype = C.c_longlong
+        self._failed_row.argtypes = [C.c_char_p, C.c_char_p, C.c_int, vp, sz]
+        self._time = getattr(self.lib, f"npref_{prefix}_time")
+        self._time.restype = C.c_double
+        self._time.argtypes = [vp, sz, C.c_double, C.c_double, C.c_double, C.c_double, vp, sz, vp, vp, sz]
 
-    def read(self, r: PolyaRead):
-        """(seg u64[5], (read_rate, polya_length), qc, row)"""
+    def read(self, r: PolyaRead, *extra):
+        """(seg u64[5], (read_rate, polya_length), qc, row), the reference filling the extra result pointers; the numbers are
+        None for a failed load"""
         buf = C.create_string_buffer(1024)
         if not r.loaded:
-            n = self.lib.npref_polya_failed_row(r.name.encode(), r.contig.encode(), r.pos, buf, 1024)
+            n = self._failed_row(r.name.encode(), r.contig.encode(), r.pos, buf, 1024)
             return None, None, 4, buf.raw[:n].decode()
         seg = np.zeros(5, np.uint64); rl = np.zeros(2, np.float64); qc = C.c_int()
         s = np.ascontiguousarray(r.samples, np.float32); d = np.ascontiguousarray(r.duration, np.float32)
         a = np.ascontiguousarray(r.map_start, np.int32); b = np.ascontiguousarray(r.map_stop, np.int32)
-        n = self.lib.npref_polya_read(r.name.encode(), r.contig.encode(), r.pos, r.suffix_clip, s.ctypes.data, s.shape[0],
-                                      r.sample_rate, r.scale, r.shift, r.var, d.ctypes.data, d.shape[0], a.ctypes.data, b.ctypes.data,
-                                      a.shape[0], seg.ctypes.data, rl.ctypes.data, C.byref(qc), buf, 1024)
+        n = self._read(r.name.encode(), r.contig.encode(), r.pos, r.suffix_clip, s.ctypes.data, s.shape[0], r.sample_rate, r.scale,
+                       r.shift, r.var, d.ctypes.data, d.shape[0], a.ctypes.data, b.ctypes.data, a.shape[0], seg.ctypes.data,
+                       rl.ctypes.data, C.byref(qc), *extra, buf, 1024)
         assert n > 0
         return seg, (rl[0], rl[1]), qc.value, buf.raw[:n].decode()
 
     def time(self, r: PolyaRead) -> float:
         s = np.ascontiguousarray(r.samples, np.float32); d = np.ascontiguousarray(r.duration, np.float32)
         a = np.ascontiguousarray(r.map_start, np.int32); b = np.ascontiguousarray(r.map_stop, np.int32)
-        return self.lib.npref_polya_time(s.ctypes.data, s.shape[0], r.sample_rate, r.scale, r.shift, r.var, d.ctypes.data, d.shape[0],
-                                         a.ctypes.data, b.ctypes.data, a.shape[0])
+        return self._time(s.ctypes.data, s.shape[0], r.sample_rate, r.scale, r.shift, r.var, d.ctypes.data, d.shape[0],
+                          a.ctypes.data, b.ctypes.data, a.shape[0])
+
+
+class RefPolya(RefTail):
+    """The reference's own poly(A) functions (oracle/polya_harness.cpp)."""
+
+    def __init__(self):
+        super().__init__(REF_POLYA, "polya", 0)
 
 
 def edge_reads(rng):

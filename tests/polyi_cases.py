@@ -1,5 +1,5 @@
 """detect-polyi test inputs and checkers: synthetic poly(I)/poly(A) reads, crafted edge reads, the compiled reference's
-detect-polyi pieces (oracle/_ref/libnpref_polyi.so, built by oracle/detect_polyi.mk) and a plain Python restatement of its
+detect-polyi pieces (oracle/_ref/libnpref_polyi.so, built by oracle/polya.mk) and a plain Python restatement of its
 segmentation HMM and Bernoulli stage.  Reads, packing and glibc's expf / logf come from polya_cases: a read here is the same
 PolyaRead that estimate_polya_for_single_read and dpi_estimate_polya_for_single_read both see after loading."""
 from __future__ import annotations
@@ -15,40 +15,19 @@ from tests.polya_cases import PolyaRead, _expf, _logf, f32
 REF_POLYI = os.path.join(pc.ROOT, "oracle", "_ref", "libnpref_polyi.so")
 
 
-class RefPolyi:
+class RefPolyi(pc.RefTail):
     """The reference's own detect-polyi functions (oracle/detect_polyi_harness.cpp)."""
 
     def __init__(self):
-        self.lib = C.CDLL(REF_POLYI)
-        vp, sz = C.c_void_p, C.c_size_t
-        self.lib.npref_polyi_read.restype = C.c_longlong
-        self.lib.npref_polyi_read.argtypes = [C.c_char_p, C.c_char_p, C.c_int, C.c_uint32, vp, sz, C.c_double, C.c_double,
-                                              C.c_double, C.c_double, vp, sz, vp, vp, sz, vp, vp, vp, vp, vp, vp, sz]
-        self.lib.npref_polyi_failed_row.restype = C.c_longlong
-        self.lib.npref_polyi_failed_row.argtypes = [C.c_char_p, C.c_char_p, C.c_int, vp, sz]
-        self.lib.npref_polyi_time.restype = C.c_double
-        self.lib.npref_polyi_time.argtypes = [vp, sz, C.c_double, C.c_double, C.c_double, C.c_double, vp, sz, vp, vp, sz]
+        super().__init__(REF_POLYI, "polyi", 2)
 
     def read(self, r: PolyaRead):
         """(seg u64[5], (read_rate, polya_length), qc, (polyi, polya), detected, row); the numbers are None for a failed load"""
-        buf = C.create_string_buffer(1024)
-        if not r.loaded:
-            n = self.lib.npref_polyi_failed_row(r.name.encode(), r.contig.encode(), r.pos, buf, 1024)
-            return None, None, 4, None, None, buf.raw[:n].decode()
-        seg = np.zeros(5, np.uint64); rl = np.zeros(2, np.float64); qc = C.c_int(); bern = np.zeros(2, np.int32); det = C.c_int()
-        s = np.ascontiguousarray(r.samples, np.float32); d = np.ascontiguousarray(r.duration, np.float32)
-        a = np.ascontiguousarray(r.map_start, np.int32); b = np.ascontiguousarray(r.map_stop, np.int32)
-        n = self.lib.npref_polyi_read(r.name.encode(), r.contig.encode(), r.pos, r.suffix_clip, s.ctypes.data, s.shape[0],
-                                      r.sample_rate, r.scale, r.shift, r.var, d.ctypes.data, d.shape[0], a.ctypes.data, b.ctypes.data,
-                                      a.shape[0], seg.ctypes.data, rl.ctypes.data, C.byref(qc), bern.ctypes.data, C.byref(det), buf, 1024)
-        assert n > 0
-        return seg, (rl[0], rl[1]), qc.value, (int(bern[0]), int(bern[1])), det.value, buf.raw[:n].decode()
-
-    def time(self, r: PolyaRead) -> float:
-        s = np.ascontiguousarray(r.samples, np.float32); d = np.ascontiguousarray(r.duration, np.float32)
-        a = np.ascontiguousarray(r.map_start, np.int32); b = np.ascontiguousarray(r.map_stop, np.int32)
-        return self.lib.npref_polyi_time(s.ctypes.data, s.shape[0], r.sample_rate, r.scale, r.shift, r.var, d.ctypes.data, d.shape[0],
-                                         a.ctypes.data, b.ctypes.data, a.shape[0])
+        bern = np.zeros(2, np.int32); det = C.c_int()
+        seg, rl, qc, row = super().read(r, bern.ctypes.data, C.byref(det))
+        if seg is None:
+            return None, None, 4, None, None, row
+        return seg, rl, qc, (int(bern[0]), int(bern[1])), det.value, row
 
 
 # ---- synthetic reads ------------------------------------------------------------------------------------------------------

@@ -1,7 +1,8 @@
-"""nanopolish polya end to end through the C++ host mirror (nph::load_from_raw, then nph::PolyaBatch): direct-RNA raw reads
-are loaded on the device, then a batch of BAM-like records (primary and secondary, last CIGAR operations of every kind, a read
-missing from the index, a read whose load fails) goes through one nph_polya_batch call and comes back as polya_main's TSV.  The
-expected rows come from the same chain through the oracle (oracle/prep_chain.py) and the reference's own poly(A) code."""
+"""nanopolish polya and detect-polyi end to end through the C++ host mirror (nph::load_from_raw, then nph::PolyaBatch or
+nph::DetectPolyiBatch): direct-RNA raw reads are loaded on the device, then a batch of BAM-like records (primary and secondary,
+last CIGAR operations of every kind, a read missing from the index, a read whose load fails) goes through one nph_polya_batch
+or nph_detect_polyi_batch call and comes back as polya_main's or detect_polyi_main's TSV.  The expected rows come from the same
+chain through the oracle (oracle/prep_chain.py) and the reference's own poly(A) or detect-polyi code."""
 import ctypes as C
 import os
 
@@ -10,24 +11,41 @@ import pytest
 
 from nanopolish_b200 import synth
 from tests import polya_cases as pc
+from tests import polyi_cases as qc
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HOST_SO = os.path.join(ROOT, "nanopolish_b200", "libnph_host.so")
 pytestmark = pytest.mark.gpu
-HEADER = "readname\tcontig\tposition\tleader_start\tadapter_start\tpolya_start\ttranscript_start\tread_rate\tpolya_length\tqc_tag\n"
+# (C shim, header line, the reference's class)
+MODES = {
+    "polya": ("nphh_polya", "readname\tcontig\tposition\tleader_start\tadapter_start\tpolya_start\ttranscript_start\tread_rate\t"
+              "polya_length\tqc_tag\n", pc.RefPolya),
+    "detect_polyi": ("nphh_detect_polyi", "readname\tcontig\tposition\tleader_start\tadapter_start\tpolya_start\ttranscript_start\t"
+                     "read_rate\tpolya_length\tdetected\tqc_tag\n", qc.RefPolyi),
+}
 
 
 @pytest.fixture(scope="module")
 def host():
     lib = C.CDLL(HOST_SO)
     lib.nphh_last_error.restype = C.c_char_p
-    lib.nphh_polya.restype = C.c_longlong
+    for shim, _, _ in MODES.values():
+        getattr(lib, shim).restype = C.c_longlong
     return lib
 
 
 def test_polya_after_load_from_raw_like_a_caller(host, port_oracle):
+    _after_load_from_raw_like_a_caller(host, port_oracle, "polya")
+
+
+def test_detect_polyi_after_load_from_raw_like_a_caller(host, port_oracle):
+    _after_load_from_raw_like_a_caller(host, port_oracle, "detect_polyi")
+
+
+def _after_load_from_raw_like_a_caller(host, port_oracle, mode):
     from oracle.prep_chain import oracle_chain
-    ref = pc.RefPolya()
+    shim, header, ref_class = MODES[mode]
+    ref = ref_class()
     m6 = synth.load_model("nucleotide")
     sd5 = m6.level_stdv.reshape(1024, 4).mean(1)
     rna = synth.PoreModel("derived.u_to_t_rna.5mer", 5, "nucleotide", m6.level_mean.reshape(1024, 4).mean(1), sd5, np.log(sd5))
@@ -83,16 +101,16 @@ def test_polya_after_load_from_raw_like_a_caller(host, port_oracle):
     srate = np.full(m, rate)
     cap = 1 << 16
     buf = C.create_string_buffer(cap); need = C.c_size_t()
-    got = host.nphh_polya(m, names, contigs, p(pos), p(flag), p(cig), p(coff), p(handle), p(samples), p(so), p(srate), buf, cap, C.byref(need))
+    got = getattr(host, shim)(m, names, contigs, p(pos), p(flag), p(cig), p(coff), p(handle), p(samples), p(so), p(srate), buf, cap, C.byref(need))
     assert got > 0, host.nphh_last_error()
     got = buf.raw[:got].decode()
 
-    rows = [HEADER]
+    rows = [header]
     for name, contig, ps, fl, cigar, h in recs:
         if fl & 0x100:
             continue
         if h < 0:
-            rows.append(ref.read(pc.PolyaRead(name, np.zeros(0, np.float32), rate, 1, 0, 1, None, None, None, contig=contig, pos=ps, loaded=False))[3])
+            rows.append(ref.read(pc.PolyaRead(name, np.zeros(0, np.float32), rate, 1, 0, 1, None, None, None, contig=contig, pos=ps, loaded=False))[-1])
             continue
         w = want[h - first]
         loaded = w["events"] is not None and w.get("cal") is not None and int(w["cal"]["status"]) == 0
@@ -100,7 +118,7 @@ def test_polya_after_load_from_raw_like_a_caller(host, port_oracle):
                          float(w["cal"]["var"]) if loaded else 1.0, w.get("duration"),
                          w["b2e"]["start"].astype(np.int32) if loaded else None, w["b2e"]["stop"].astype(np.int32) if loaded else None,
                          suffix_clip=cigar[-1] >> 4, contig=contig, pos=ps, loaded=loaded)
-        rows.append(ref.read(r)[3])
+        rows.append(ref.read(r)[-1])
     assert sum(1 for w in want[:-1] if w["events"] is not None and int(w["cal"]["status"]) == 0) >= 4
     assert got == "".join(rows)
     # the secondary record has no row; the flat read and the missing one fail to load
