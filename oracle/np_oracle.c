@@ -624,7 +624,44 @@ static void tstat_fill(const double* sum, const double* sumsq, size_t n, size_t 
 
 typedef struct { float threshold; size_t window_length; size_t masked_to; long peak_pos; float peak_value; int valid_peak; } npo_detector;
 
-long long npo_detect_events(const float* raw, size_t n, const nph_event_params* prm, nph_event* out, size_t cap)
+/* one step of short_long_peak_detector at position i; the boundaries it emits go to peaks[*count] (and their step to
+ * step_out[*count] when given) */
+static void npo_peak_step(npo_detector* det, const float* const* sig, float peak_height, size_t i, size_t* peaks, uint64_t* step_out,
+                          size_t* count)
+{
+    for (int k = 0; k < 2; ++k) {
+        npo_detector* d = &det[k];
+        if (d->masked_to >= i) continue;
+        float cur = sig[k][i];
+        if (d->peak_pos == -1) {
+            if (cur < d->peak_value) d->peak_value = cur;
+            else if (cur - d->peak_value > peak_height) { d->peak_value = cur; d->peak_pos = (long)i; }
+        } else {
+            if (cur > d->peak_value) { d->peak_value = cur; d->peak_pos = (long)i; }
+            if (k == 0 && d->peak_value > d->threshold) {
+                det[1].masked_to = d->peak_pos + d->window_length;
+                det[1].peak_pos = -1; det[1].peak_value = FLT_MAX; det[1].valid_peak = 0;
+            }
+            if (d->peak_value - cur > peak_height && d->peak_value > d->threshold) d->valid_peak = 1;
+            if (d->valid_peak && (i - d->peak_pos) > d->window_length / 2) {
+                if (step_out) step_out[*count] = i;
+                peaks[(*count)++] = (size_t)d->peak_pos;
+                d->peak_pos = -1; d->peak_value = cur; d->valid_peak = 0;
+            }
+        }
+    }
+}
+
+static void npo_detectors_init(npo_detector* det, const nph_event_params* prm)
+{
+    const npo_detector d0 = { prm->threshold1, prm->window_length1, 0, -1, FLT_MAX, 0 }, d1 = { prm->threshold2, prm->window_length2, 0, -1, FLT_MAX, 0 };
+    det[0] = d0; det[1] = d1;
+}
+
+/* npo_detect_events, plus what it saw on the way: the two t-statistic vectors (t1_out, t2_out: n each) and the position of
+ * the detector step that emitted each boundary (emit_step_out: n entries; boundary b is the start of event b + 1) */
+long long npo_detect_events_trace(const float* raw, size_t n, const nph_event_params* prm, nph_event* out, size_t cap,
+                                  float* t1_out, float* t2_out, uint64_t* emit_step_out)
 {
     double* sum = (double*)calloc(n + 1, sizeof(double));
     double* sumsq = (double*)calloc(n + 1, sizeof(double));
@@ -634,32 +671,13 @@ long long npo_detect_events(const float* raw, size_t n, const nph_event_params* 
     for (size_t i = 0; i < n; ++i) { sum[i + 1] = sum[i] + raw[i]; sumsq[i + 1] = sumsq[i] + raw[i] * raw[i]; }
     tstat_fill(sum, sumsq, n, prm->window_length1, t1);
     tstat_fill(sum, sumsq, n, prm->window_length2, t2);
-    npo_detector det[2] = { { prm->threshold1, prm->window_length1, 0, -1, FLT_MAX, 0 }, { prm->threshold2, prm->window_length2, 0, -1, FLT_MAX, 0 } };
+    npo_detector det[2];
+    npo_detectors_init(det, prm);
     const float* sig[2] = { t1, t2 };
-    const float peak_height = prm->peak_height;
     size_t peak_count = 0;
-    for (size_t i = 0; i < n; ++i) {
-        for (int k = 0; k < 2; ++k) {
-            npo_detector* d = &det[k];
-            if (d->masked_to >= i) continue;
-            float cur = sig[k][i];
-            if (d->peak_pos == -1) {
-                if (cur < d->peak_value) d->peak_value = cur;
-                else if (cur - d->peak_value > peak_height) { d->peak_value = cur; d->peak_pos = (long)i; }
-            } else {
-                if (cur > d->peak_value) { d->peak_value = cur; d->peak_pos = (long)i; }
-                if (k == 0 && d->peak_value > d->threshold) {
-                    det[1].masked_to = d->peak_pos + d->window_length;
-                    det[1].peak_pos = -1; det[1].peak_value = FLT_MAX; det[1].valid_peak = 0;
-                }
-                if (d->peak_value - cur > peak_height && d->peak_value > d->threshold) d->valid_peak = 1;
-                if (d->valid_peak && (i - d->peak_pos) > d->window_length / 2) {
-                    peaks[peak_count++] = (size_t)d->peak_pos;
-                    d->peak_pos = -1; d->peak_value = cur; d->valid_peak = 0;
-                }
-            }
-        }
-    }
+    for (size_t i = 0; i < n; ++i) npo_peak_step(det, sig, prm->peak_height, i, peaks, emit_step_out, &peak_count);
+    if (t1_out) memcpy(t1_out, t1, n * sizeof(float));
+    if (t2_out) memcpy(t2_out, t2, n * sizeof(float));
     size_t ne = 1;
     for (size_t i = 0; i < n; ++i) if (peaks[i] > 0 && peaks[i] < n) ne++;
     long long ret = (long long)ne;
@@ -680,6 +698,39 @@ long long npo_detect_events(const float* raw, size_t n, const nph_event_params* 
     }
     free(sum); free(sumsq); free(t1); free(t2); free(peaks);
     return ret;
+}
+
+long long npo_detect_events(const float* raw, size_t n, const nph_event_params* prm, nph_event* out, size_t cap)
+{
+    return npo_detect_events_trace(raw, n, prm, out, cap, NULL, NULL, NULL);
+}
+
+/* The peak detector alone, walked over positions [from, to) of given t-statistic vectors from the state *st (updated in
+ * place).  Returns the number of boundaries emitted; the first `cap` of them go to peaks_out (position) and step_out (the
+ * step that emitted it). */
+size_t npo_peak_walk(const float* t1, const float* t2, const nph_event_params* prm, size_t from, size_t to, npo_peak_state* st,
+                     uint64_t* peaks_out, uint64_t* step_out, size_t cap)
+{
+    npo_detector det[2];
+    npo_detectors_init(det, prm);
+    for (int k = 0; k < 2; ++k) {
+        det[k].masked_to = (size_t)st->masked_to[k]; det[k].peak_pos = (long)st->peak_pos[k];
+        det[k].peak_value = st->peak_value[k]; det[k].valid_peak = st->valid_peak[k];
+    }
+    const float* sig[2] = { t1, t2 };
+    size_t count = 0, peaks[2];
+    uint64_t steps[2];
+    for (size_t i = from; i < to; ++i) {
+        size_t c = 0;
+        npo_peak_step(det, sig, prm->peak_height, i, peaks, steps, &c);
+        for (size_t e = 0; e < c; ++e, ++count)
+            if (count < cap) { peaks_out[count] = peaks[e]; step_out[count] = steps[e]; }
+    }
+    for (int k = 0; k < 2; ++k) {
+        st->masked_to[k] = det[k].masked_to; st->peak_pos[k] = det[k].peak_pos;
+        st->peak_value[k] = det[k].peak_value; st->valid_peak[k] = det[k].valid_peak;
+    }
+    return count;
 }
 
 /* ------------------------------------------------------------------------------------------

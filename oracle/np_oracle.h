@@ -55,6 +55,12 @@ double npo_abea_batch(const nph_read* reads, const float* ev_mean, const double*
 void npo_mom(const nph_read* reads, const float* ev_mean, const npo_model* model,
              const uint32_t* kmer_ranks, const nph_abea_job* job, double* shift_out, double* scale_out);
 long long npo_detect_events(const float* raw, size_t n, const nph_event_params* prm, nph_event* out, size_t cap);
+long long npo_detect_events_trace(const float* raw, size_t n, const nph_event_params* prm, nph_event* out, size_t cap,
+                                  float* t1_out, float* t2_out, uint64_t* emit_step_out);
+/* the state of short_long_peak_detector's two detectors (index 0 = short, 1 = long); peak_pos -1 = no peak yet */
+typedef struct { uint64_t masked_to[2]; int64_t peak_pos[2]; float peak_value[2]; int32_t valid_peak[2]; } npo_peak_state;
+size_t npo_peak_walk(const float* t1, const float* t2, const nph_event_params* prm, size_t from, size_t to, npo_peak_state* st,
+                     uint64_t* peaks_out, uint64_t* step_out, size_t cap);
 int npo_trim_raw(const float* raw, size_t n, int trim_start, int trim_end, int varseg_chunk, float varseg_thresh,
                  uint32_t* start_out, uint32_t* end_out);
 void npo_recalibrate(const nph_read* reads, const float* ev_mean, const npo_model* model, const uint32_t* kmer_ranks,

@@ -146,6 +146,27 @@ class PortOracle:
         n = self.lib.npo_detect_events(_p(raw), C.c_size_t(raw.shape[0]), _p(params), _p(out), C.c_size_t(out.shape[0]))
         return out[:n].copy()
 
+    def detect_events_trace(self, raw, params):
+        """npo_detect_events and what it saw: (events, t1, t2, emit_step) with emit_step[b] the detector step that emitted
+        boundary b (the start of event b + 1)"""
+        from nanopolish_b200.synth import EVENT_DT
+        n = raw.shape[0]
+        out = np.zeros(n + 1, EVENT_DT)
+        t1, t2 = np.zeros(n, np.float32), np.zeros(n, np.float32)
+        step = np.zeros(max(n, 1), np.uint64)
+        self.lib.npo_detect_events_trace.restype = C.c_longlong
+        ne = self.lib.npo_detect_events_trace(_p(raw), C.c_size_t(n), _p(params), _p(out), C.c_size_t(out.shape[0]), _p(t1), _p(t2), _p(step))
+        return out[:ne].copy(), t1, t2, step[:ne - 1].copy()
+
+    def peak_walk(self, t1, t2, params, start, stop, state):
+        """npo_peak_walk: the peak detector over positions [start, stop) from `state` (a PEAK_STATE_DT record, updated in place);
+        returns (boundary positions, emitting steps)"""
+        cap = max(stop - start, 1)
+        pk, st = np.zeros(cap, np.uint64), np.zeros(cap, np.uint64)
+        self.lib.npo_peak_walk.restype = C.c_size_t
+        c = self.lib.npo_peak_walk(_p(t1), _p(t2), _p(params), C.c_size_t(start), C.c_size_t(stop), _p(state), _p(pk), _p(st), C.c_size_t(cap))
+        return pk[:c].copy(), st[:c].copy()
+
     def trim_raw(self, raw, trim_start=200, trim_end=10, varseg_chunk=100, varseg_thresh=0.0):
         s, e = C.c_uint32(), C.c_uint32()
         ok = self.lib.npo_trim_raw(_p(raw), C.c_size_t(raw.shape[0]), C.c_int(trim_start), C.c_int(trim_end), C.c_int(varseg_chunk),
@@ -186,6 +207,10 @@ class RefOracle:
     @staticmethod
     def available() -> bool:
         return os.path.exists(REF_SO)
+
+    def has(self, entry: str) -> bool:
+        """whether this build of the library exports a harness entry point (one built before the entry existed does not)"""
+        return hasattr(self.lib, entry)
 
     def builtin_model(self, alphabet="nucleotide", kit="r9.4_450bps", strand="template", k=6):
         key = (kit, alphabet, strand, k)
@@ -395,6 +420,19 @@ class RefOracle:
         mean = np.zeros(n + 1, np.float32); stdv = np.zeros(n + 1, np.float32)
         self.lib.npref_detect_events.restype = C.c_longlong
         ne = self.lib.npref_detect_events(_p(raw), C.c_size_t(n), int(rna), _p(start), _p(length), _p(mean), _p(stdv), C.c_size_t(n + 1))
+        return start[:ne], length[:ne], mean[:ne], stdv[:ne]
+
+    def detect_events_params(self, raw, params):
+        """detect_events with the detector_param of an EVENT_PARAMS_DT record; the signal must have a boundary"""
+        n = raw.shape[0]
+        start = np.zeros(n + 1, np.uint64); length = np.zeros(n + 1, np.float32)
+        mean = np.zeros(n + 1, np.float32); stdv = np.zeros(n + 1, np.float32)
+        p = params.reshape(-1)[0]
+        self.lib.npref_detect_events_params.restype = C.c_longlong
+        ne = self.lib.npref_detect_events_params(_p(raw), C.c_size_t(n), C.c_uint32(int(p["window_length1"])), C.c_uint32(int(p["window_length2"])),
+                                                 C.c_float(p["threshold1"]), C.c_float(p["threshold2"]), C.c_float(p["peak_height"]),
+                                                 _p(start), _p(length), _p(mean), _p(stdv), C.c_size_t(n + 1))
+        assert ne > 0
         return start[:ne], length[:ne], mean[:ne], stdv[:ne]
 
     def trim_raw(self, raw, trim_start=200, trim_end=10, varseg_chunk=100, varseg_thresh=0.0):

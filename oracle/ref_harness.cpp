@@ -357,6 +357,26 @@ long long npref_detect_events(const float* raw, size_t n, int rna, uint64_t* sta
     return ne;
 }
 
+// The same with any detector_param: windows, thresholds and peak height as given.  The signal must have at least one
+// boundary (create_events reads peaks[-1] otherwise).
+long long npref_detect_events_params(const float* raw, size_t n, uint32_t window_length1, uint32_t window_length2, float threshold1,
+                                     float threshold2, float peak_height, uint64_t* start, float* length, float* mean, float* stdv, size_t cap)
+{
+    raw_table rt;
+    rt.n = n; rt.start = 0; rt.end = n; rt.raw = const_cast<float*>(raw);
+    detector_param prm = event_detection_defaults;
+    prm.window_length1 = window_length1; prm.window_length2 = window_length2;
+    prm.threshold1 = threshold1; prm.threshold2 = threshold2; prm.peak_height = peak_height;
+    event_table et = detect_events(rt, prm);
+    if (et.event == NULL) return -2;
+    long long ne = (long long)et.n;
+    if (et.n <= cap) {
+        for (size_t i = 0; i < et.n; ++i) { start[i] = et.event[i].start; length[i] = et.event[i].length; mean[i] = et.event[i].mean; stdv[i] = et.event[i].stdv; }
+    } else ne = -1;
+    free(et.event);
+    return ne;
+}
+
 // trim_and_segment_raw (src/thirdparty/scrappie/scrappie_common.c:122-138) on a table covering the whole signal.
 // The function frees rt.raw when nothing survives, so it gets its own copy.  Signals for which the reference would
 // trip its own assert (fewer samples than a chunk, no chunk above the threshold) must not be passed.
