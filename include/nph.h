@@ -791,6 +791,44 @@ int nph_detect_polyi_batch(nph_ctx* ctx, const float* raw, size_t n_samples_tota
                            const float* ev_duration, size_t n_events_total, const nph_event_range* base_to_event,
                            size_t n_ranks_total, nph_polyi_result* results_out);
 
+/* ---- phase-reads: SNP allele calls and qualities (ref: phase_single_read, src/nanopolish_phase_reads.cpp:178-347) -----------
+ * One record = one BAM record, strand 0 of its read, in the compact event alignment of nph_methylation_batch_compact: ref_bases
+ * holds the record's fetched reference, upper-cased (std::toupper) and NOT disambiguated; model_id is the read's base model (a
+ * nucleotide model); strand stays 0.  variants is the caller's list sorted by position (sortByPosition), and var_range[2r],
+ * var_range[2r + 1] the [lower_bound(pos), upper_bound(bam_endpos)) range of record r in it.
+ * Per variant of a range, in list order: skipped unless is_snp; the window [p - 30, p + 30] (opt::min_flanking_sequence) must be
+ * bounded by AlignmentDB::_find_by_ref_bounds (the reference's event/bp ratio test never skips); the centre base must equal
+ * ref_base (Haplotype::apply_variant).  Such a site gets two forward scores (the 61-base reference window and the window with
+ * alt_base at its centre; HAF_ALLOW_PRE_CLIP | HAF_ALLOW_POST_CLIP, the record's EventAlignmentRecord::stride) and one
+ * nph_phase_call.  The calls of record r are calls_out[call_off_out[r] .. call_off_out[r + 1]) in list order.
+ * NPH_ERR_INVALID: a record, model or variant range out of bounds (lo > hi included); a model that is not a nucleotide model;
+ * calls_cap too small (nph_last_error states the count needed; the sum of hi - lo always suffices); a job the scorer refuses.
+ * n_scored_events_out (optional): sum over sites of 2 * (abs(e2 - e1) + 1). */
+#define NPH_PHASE_FLANK 30
+typedef struct {
+    int32_t  ref_position;    /* Variant::ref_position */
+    char     ref_base;        /* ref_seq[0] */
+    char     alt_base;        /* alt_seq[0] */
+    uint8_t  is_snp;          /* Variant::is_snp(): both alleles one base long */
+    uint8_t  reserved;
+} nph_phase_variant;          /* 8 bytes */
+typedef struct {
+    uint32_t record;          /* index into records[] */
+    uint32_t variant;         /* index into variants[] */
+    float    ref_score;       /* profile_hmm_score of the reference window */
+    float    alt_score;       /* of the window with the alternative base */
+    char     call;            /* alt_base if alt_score > ref_score, else ref_base */
+    uint8_t  qual;            /* q_char: (int)min(30, -10 log10 p_wrong) + 33, the byte the reference stores in the record's QUAL */
+    uint8_t  reserved[2];
+} nph_phase_call;             /* 20 bytes */
+int nph_phase_reads_batch(nph_ctx* ctx, const nph_read* reads, size_t n_reads,
+                          const float* ev_mean, const double* ev_start_time, size_t n_events_total,
+                          const char* ref_bases, const int16_t* event_deltas, size_t n_ref_total, const int32_t* first_event,
+                          const nph_meth_record* records, size_t n_records,
+                          const nph_phase_variant* variants, size_t n_variants, const uint32_t* var_range,
+                          double indel_bias, uint64_t* call_off_out,
+                          nph_phase_call* calls_out, size_t calls_cap, uint64_t* n_scored_events_out);
+
 /* ---- measurement hooks (used by bench.py; not part of the reference surface) ------------- */
 /* Device time in ms of the most recent nph_hmm_score / nph_abea_run kernel sequence, measured
  * with CUDA events on the context's stream (valid after a sync), and the number of kernel

@@ -91,6 +91,14 @@ __device__ __forceinline__ float lsum_sat(float a, float b, const LogsumTable tb
     return lsum_lookup(mx, __fadd_rd(t, 512.0f), tb);
 }
 
+// ---- add_logs(a, b) = p7_FLogsum on floats (ref: src/common/logsum.h:55-66) with the reference's table below NPH_LOGSUM_CUT
+__host__ __device__ inline float nph_flogsum(float a, float b, const float* tbl)
+{
+    const float mx = a > b ? a : b, mn = a < b ? a : b;
+    const float d = mx - mn;
+    return (mn == -INFINITY || !(d < 15.7f)) ? mx : mx + tbl[(int)(d * 1000.f)];
+}
+
 // ---- profile_hmm_score_set's fold of one group of scores (ref: src/hmm/nanopolish_profile_hmm.cpp:32-56) --------------------
 // s[0] is the nucleotide sequence's score, s[1 .. n-1] those of its methylated alternatives; pen = log(n) from host libm.
 //     score = s[0] - pen;  per alternative: add_logs((float)score, (float)(s[i] - pen)) -> score (double)
@@ -102,12 +110,25 @@ __host__ __device__ inline float nph_score_set_fold(const float* s, uint32_t n, 
     double score = (double)s[0] - pen;
     for (uint32_t i = 1; i < n; ++i) {
         const double alt = (double)s[i] - pen;
-        const float a = (float)score, b = (float)alt;
-        const float mx = a > b ? a : b, mn = a < b ? a : b;
-        const float d = mx - mn;
-        score = (mn == -INFINITY || !(d < 15.7f)) ? mx : mx + tbl[(int)(d * 1000.f)];
+        score = nph_flogsum((float)score, (float)alt, tbl);
     }
     return (float)score;
+}
+
+// ---- phase-reads' call and quality of one SNP from its two scores (ref: src/nanopolish_phase_reads.cpp:293-317) ---------------
+//     log_sum = add_logs(alt, ref)   (p7_FLogsum on the float scores, as nph_score_set_fold's step)
+//     log_p_wrong = (alt > ref ? ref : alt) - log_sum;   q = std::min(30.0, -10 * log_p_wrong / log(10));   q_char = (int)q + 33
+// The call is alt_base when alt > ref, else ref_base.  std::min(30, q) returns 30 for a NaN q.  Every step is one IEEE operation
+// and log(10) is the constant the compiler folds, so host and device round alike.
+struct NphPhaseCall { char call; uint8_t q_char; };
+__host__ __device__ inline NphPhaseCall nph_phase_quality(float ref, float alt, char ref_base, char alt_base, const float* tbl)
+{
+    const double log_sum = nph_flogsum(alt, ref, tbl);
+    const bool is_alt = alt > ref;
+    const double log_p_wrong = (double)(is_alt ? ref : alt) - log_sum;
+    const double q = -10.0 * log_p_wrong / 2.302585092994045684;       // log(10), correctly rounded
+    const double qc = q < 30.0 ? q : 30.0;
+    return NphPhaseCall{is_alt ? alt_base : ref_base, (uint8_t)((int)qc + 33)};
 }
 
 // ---- correctly rounded float division with a precomputed reciprocal --------------------------

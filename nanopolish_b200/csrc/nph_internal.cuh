@@ -201,6 +201,14 @@ struct nph_ctx {
         DevBuf<uint32_t> d_alt_models;     // n_records x n_types model ids
     } screen;
 
+    // the last nph_phase_reads_batch (phase_reads.cu)
+    struct PhaseState {
+        NphEventRecords ev;                // fetched references, compact event alignments, records
+        DevBuf<uint8_t> d_in;              // variants and per-record variant ranges
+        DevBuf<uint8_t> d_counts;          // per-record sites, their offsets, the scan's scratch, the scored-event count
+        DevBuf<nph_phase_call> d_calls;
+    } phase;
+
     // measurement
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     // side streams so that the tail of one forward class overlaps the head of the next (fork/join by events)
@@ -349,6 +357,7 @@ __device__ __forceinline__ T nph_block_scan_incl(T v, T* s, int t)
     __syncthreads();
     return v;
 }
+
 #endif
 
 // where the HMM jobs in ctx->d_jobs and their ranks come from
@@ -426,3 +435,43 @@ int nph_abea_stage(nph_ctx* ctx, const uint32_t* n_events, const nph_abea_job* j
 // +-NPH_ABEA_MAX_LEVEL:
 // one kernel, one flag copied back (a stream sync).
 int nph_check_ranks(nph_ctx* ctx, const uint32_t* d_ranks, size_t n, uint32_t n_states, const float* d_levels = nullptr, size_t n_levels = 0);
+
+#ifdef __CUDACC__
+// AlignmentDB::_find_by_ref_bounds (ref: src/alignment/nanopolish_alignment_db.cpp:688-731) on one record's dense event map
+// (event index per reference offset, NPH_NO_EVENT where aligned_events has no entry; fv its first offset with an entry) for the
+// window [cs, ce] in reference coordinates: the event indices at the two lower_bounds.  Variant screening and phase-reads call it.
+__device__ __forceinline__ int nph_first_valid_from(const int32_t* __restrict__ dense, int n, int from)
+{
+    for (int o = from < 0 ? 0 : from; o < n; ++o) if (dense[o] != NPH_NO_EVENT) return o;
+    return n;
+}
+__device__ __forceinline__ bool nph_find_by_ref_bounds(const nph_meth_record& R, const int32_t* __restrict__ dense, int fv, int cs, int ce,
+                                                       int& e1, int& e2)
+{
+    const int n = (int)R.ref_len;
+    if (fv >= n) return false;                                   // aligned_events.empty()
+    const int os = cs - R.ref_start_pos, oe = ce - R.ref_start_pos;
+    if (oe >= n || os >= n) return false;                        // lower_bound(ref_stop) == end()
+    const int is = nph_first_valid_from(dense, n, os);
+    if (is >= n) return false;
+    const int ie = nph_first_valid_from(dense, n, oe);
+    if (ie >= n) return false;
+    if (!(is <= os || is != fv)) return false;                   // left_bounded; right_bounded always holds for a lower_bound
+    e1 = dense[is]; e2 = dense[ie];
+    return true;
+}
+
+// Alphabet::rank of the DNA alphabet: unknown symbols rank 0
+__device__ __forceinline__ uint8_t nph_dna_code(uint8_t c) { return c == 'C' ? 1 : c == 'G' ? 2 : c == 'T' ? 3 : 0; }
+// HMMInputSequence::get_kmer_rank(q, k, false) and (q, k, true) of a DNA sequence held as nph_dna_code ranks: the k-mer at q and the
+// rank of its reverse complement (the complement of rank c is 3 - c, so an unknown symbol complements like 'A')
+__device__ __forceinline__ void nph_dna_kmer_ranks(const uint8_t* codes, int q, int k, uint32_t& fw, uint32_t& rc)
+{
+    uint32_t f = 0, r = 0;
+    for (int t = 0; t < k; ++t) {
+        f = f * 4u + codes[q + t];
+        r = r * 4u + (3u - codes[q + k - 1 - t]);
+    }
+    fw = f; rc = r;
+}
+#endif

@@ -75,26 +75,10 @@ __device__ __forceinline__ uint64_t pool_slot(const VarDev& d, int pi, int seq, 
     return ((uint64_t)pi * kSeqs + (uint64_t)seq) * (uint64_t)(1 + d.T) + (uint64_t)a;
 }
 
-// first offset >= from with an event-alignment entry (n: none)
-__device__ __forceinline__ int first_valid_from(const int32_t* __restrict__ dense, int n, int from)
-{
-    for (int o = from < 0 ? 0 : from; o < n; ++o) if (dense[o] != NPH_NO_EVENT) return o;
-    return n;
-}
-
 // _find_by_ref_bounds + the event/bp ratio test of get_event_subsequences for one record and window [cs, ce]
 __device__ __forceinline__ bool window_events(const nph_meth_record& R, const int32_t* __restrict__ dense, int fv, int cs, int ce, int& e1, int& e2)
 {
-    const int n = (int)R.ref_len;
-    if (fv >= n) return false;                                   // aligned_events.empty()
-    const int os = cs - R.ref_start_pos, oe = ce - R.ref_start_pos;
-    if (oe >= n || os >= n) return false;                        // lower_bound(ref_stop) == end()
-    const int is = first_valid_from(dense, n, os);
-    if (is >= n) return false;
-    const int ie = first_valid_from(dense, n, oe);
-    if (ie >= n) return false;
-    if (!(is <= os || is != fv)) return false;                   // left_bounded; right_bounded always holds for a lower_bound
-    e1 = dense[is]; e2 = dense[ie];
+    if (!nph_find_by_ref_bounds(R, dense, fv, cs, ce, e1, e2)) return false;
     const double ratio = fabs((double)(e1 - e2)) / fabs((double)(ce - cs));
     return ratio < 20.0;                                         // MAX_EVENT_TO_BP_RATIO
 }
@@ -177,8 +161,6 @@ __device__ __forceinline__ int edited_window(const uint8_t* __restrict__ w, int 
     return win + 1;
 }
 
-__device__ __forceinline__ uint8_t dna_code(uint8_t c) { return c == 'C' ? 1 : c == 'G' ? 2 : c == 'T' ? 3 : 0; }   // Alphabet::rank: unknown -> 0
-
 // thread per (position, sequence, alternative): ranks of both strands into the pool; the base sequence's nucleotide thread also
 // writes candidate validity into the position state, a methylated copy that differs from its sequence sets its bit in vm.alts
 __global__ void __launch_bounds__(kBlock) var_ranks_kernel(const VarDev d, const uint8_t* __restrict__ ref, uint32_t* __restrict__ pool,
@@ -198,7 +180,7 @@ __global__ void __launch_bounds__(kBlock) var_ranks_kernel(const VarDev d, const
         for (int c = 0; c < NPH_SCREEN_SLOTS; ++c) st.total[c] = 0.0;
         st.valid = 0; st.alive = 0; st.done = 0; st.chunk = 0; st.ref_rows = 0;
         if (pos_ok) {
-            const uint8_t b = dna_code(ref[cs - d.region_start + d.flank]), bp = dna_code(ref[cs - d.region_start + d.flank - 1]);
+            const uint8_t b = nph_dna_code(ref[cs - d.region_start + d.flank]), bp = nph_dna_code(ref[cs - d.region_start + d.flank - 1]);
             uint32_t v = 0x80000000u;
             for (int j = 0; j < 4; ++j) if (j != b) v |= (1u << (2 * j)) | (1u << (2 * j + 1));   // substitution != ref; insertion "A" -> "AA" is redundant
             if (bp != b) v |= 1u << 8;                                                           // deletion "AA" -> "A" is redundant
@@ -216,15 +198,8 @@ __global__ void __launch_bounds__(kBlock) var_ranks_kernel(const VarDev d, const
     uint32_t* fw = pool + pool_slot(d, pi, seq, a) * 2 * d.stride;
     uint32_t* rc = fw + d.stride;
     if (a == 0) {
-        for (int t = 0; t < L; ++t) sq[t] = dna_code(sq[t]);
-        for (int q = 0; q < nk; ++q) {
-            uint32_t rf = 0, rr = 0;
-            for (int t = 0; t < d.k; ++t) {
-                rf = rf * 4u + sq[q + t];
-                rr = rr * 4u + (3u - sq[q + d.k - 1 - t]);      // HMMInputSequence::get_kmer_rank(q, k, true): rank of the k-mer's reverse complement
-            }
-            fw[q] = rf; rc[q] = rr;
-        }
+        for (int t = 0; t < L; ++t) sq[t] = nph_dna_code(sq[t]);
+        for (int q = 0; q < nk; ++q) nph_dna_kmer_ranks(sq, q, d.k, fw[q], rc[q]);
         return;
     }
     // methylated copy of type a - 1: fr = ranks of methylate(sq), rv = ranks of Alphabet::reverse_complement of it, where a methylated

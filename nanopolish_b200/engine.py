@@ -10,7 +10,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from .synth import ABEA_RES_DT, ALIGN_STATE_DT, CALIBRATION_DT, EVENT_DT, EVENT_RANGE_DT, METH_SITE_DT, METHFREQ_PARAMS_DT, PAIR_DT, POLYA_RES_DT, POLYI_RES_DT, RAW_RANGE_DT
+from .synth import ABEA_RES_DT, ALIGN_STATE_DT, CALIBRATION_DT, EVENT_DT, EVENT_RANGE_DT, METH_SITE_DT, METHFREQ_PARAMS_DT, PAIR_DT, PHASE_CALL_DT, PHASE_VARIANT_DT, POLYA_RES_DT, POLYI_RES_DT, RAW_RANGE_DT
 
 
 def _p(a):
@@ -78,6 +78,25 @@ class Engine:
                                                            _p(ref_bases), _p(deltas), ref_bases.shape[0], _p(first_event), _p(records), n, _p(params),
                                                            indel_bias, _p(site_off), _p(sites), sites.shape[0], C.byref(scored)), "nph_methylation_batch_compact")
         return site_off, sites[:int(site_off[n])], int(scored.value)
+
+    # ---- phase-reads: SNP calls and qualities of a record batch (include/nph.h, nph_phase_reads_batch) ----
+    def phase_reads_batch(self, reads, ev_mean, ev_start_time, ref_bases, deltas, first_event, records, variants, var_range,
+                          indel_bias: float = 1.0, calls_cap: int | None = None):
+        """nph_phase_reads_batch: records METH_RECORD_DT (compact event alignments), variants PHASE_VARIANT_DT, var_range u4[n_records, 2].
+        Returns (call_off u8[n_records + 1], calls PHASE_CALL_DT[n_calls], scored_events).  calls_cap defaults to the sum of the ranges."""
+        assert variants.dtype == PHASE_VARIANT_DT
+        n = int(records.shape[0])
+        var_range = np.ascontiguousarray(var_range, np.uint32)
+        if calls_cap is None:
+            calls_cap = int((var_range.reshape(-1, 2)[:, 1].astype(np.int64) - var_range.reshape(-1, 2)[:, 0]).clip(0).sum()) if n else 0
+        call_off = np.zeros(n + 1, np.uint64)
+        calls = np.zeros(max(calls_cap, 1), PHASE_CALL_DT)
+        scored = C.c_uint64()
+        self._check(self.lib.nph_phase_reads_batch(self.ctx, _p(reads), reads.shape[0], _p(ev_mean), _p(ev_start_time), ev_mean.shape[0],
+                                                   _p(ref_bases), _p(deltas), ref_bases.shape[0], _p(first_event), _p(records), n,
+                                                   _p(variants), variants.shape[0], _p(var_range), indel_bias, _p(call_off), _p(calls), calls_cap,
+                                                   C.byref(scored)), "nph_phase_reads_batch")
+        return call_off, calls[:int(call_off[n])], int(scored.value)
 
     def methylation_load_compact(self, ref_bases, deltas, first_event, records, params, indel_bias: float = 1.0):
         self._check(self.lib.nph_methylation_load_compact(self.ctx, _p(ref_bases), _p(deltas), ref_bases.shape[0], _p(first_event), _p(records),

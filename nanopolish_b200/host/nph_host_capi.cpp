@@ -7,6 +7,7 @@
 #include "nph_eventalign.hpp"
 #include "nph_scorereads.hpp"
 #include "nph_polya.hpp"
+#include "nph_phase_reads.hpp"
 #include <cmath>
 #include <chrono>
 #include <cstring>
@@ -318,6 +319,46 @@ long long nphh_call_methylation(int n_reads, const int32_t* read, const char** r
 {
     return nphh_call_methylation_timed(n_reads, read, read_names, is_rev, rc, ref_start, ref_seqs, pairs, pair_off, contig, indel_bias, tsv_out,
                                        cap, n_jobs_out, nullptr);
+}
+
+// ---- phase-reads for a batch of records of one contig: the SAM records, concatenated ------------------------------------
+// Read i: registered read read[i] (strand 0), flag / mapq of its BAM record, its fetched reference (upper-cased) from ref_start[i]
+// and its aligned_events as (ref_pos, event_idx) pairs at pair_off[i]; rc is flag & 16.  The variant list is sorted by position.
+long long nphh_phase_reads(int n_reads, const int32_t* read, const char** read_names, const uint16_t* flag, const uint8_t* mapq,
+                           const int32_t* ref_start, const char** ref_seqs, const int32_t* pairs, const uint64_t* pair_off, const char* contig,
+                           int n_variants, const int32_t* var_pos, const char** var_ref, const char** var_alt, double indel_bias,
+                           char* sam_out, size_t cap)
+{
+    long long n = -1;
+    int st = guard([&] {
+        std::vector<Variant> variants((size_t)n_variants);
+        for (int i = 0; i < n_variants; ++i) {
+            variants[i].ref_name = contig; variants[i].ref_position = (size_t)var_pos[i];
+            variants[i].ref_seq = var_ref[i]; variants[i].alt_seq = var_alt[i];
+        }
+        PhaseReads phase(variants);
+        for (int i = 0; i < n_reads; ++i) {
+            EventAlignedRead r;
+            r.read = g_reads[read[i]].get();
+            r.read_name = read_names[i];
+            r.is_reverse = (flag[i] & 16) != 0;
+            r.contig = contig;
+            r.ref_start_pos = ref_start[i];
+            r.ref_seq = ref_seqs[i];
+            const uint64_t np = pair_off[i + 1] - pair_off[i];
+            r.aligned_events[0].resize(np);
+            if (np) std::memcpy(r.aligned_events[0].data(), pairs + 2 * pair_off[i], sizeof(AlignedPair) * np);
+            r.rc[0] = r.is_reverse;
+            phase.add_read(r, flag[i], mapq[i]);
+        }
+        phase.run(Engine::thread_default(), indel_bias);
+        std::string all;
+        for (const std::string& line : phase.sam()) all += line;
+        if (all.size() + 1 > cap) throw Error(NPH_ERR_INVALID, "sam buffer too small");
+        std::memcpy(sam_out, all.c_str(), all.size() + 1);
+        n = (long long)all.size();
+    });
+    return st ? st : n;
 }
 
 // call-methylation from flat host buffers (the C-ABI layout) to TSV bytes: what bench.py's end-to-end arm times.

@@ -163,6 +163,23 @@ nph_meth_params make_meth_params(const MethylationCallingParameters& params, uin
     return p;
 }
 
+bool compact_event_alignment(const std::vector<AlignedPair>& ae, int ref_start_pos, size_t ref_len, int16_t* deltas, int32_t* first_event)
+{
+    const long long len = (long long)ref_len;
+    for (long long o = 0; o < len; ++o) deltas[o] = (int16_t)NPH_METH_NO_PAIR;
+    long long prev_off = -1;
+    int prev_ev = ae.empty() ? 0 : ae[0].read_pos;
+    *first_event = prev_ev;
+    for (const AlignedPair& ap : ae) {
+        const long long o = (long long)ap.ref_pos - ref_start_pos;
+        const long long step = (long long)ap.read_pos - prev_ev;
+        if (o <= prev_off || o >= len || step > 32767 || step < -32767) return false;
+        deltas[o] = (int16_t)step;
+        prev_off = o; prev_ev = ap.read_pos;
+    }
+    return true;
+}
+
 MethylationCaller::MethylationCaller(const MethylationCallingParameters& params) : m_params(params)
 {
     if (!m_params.alphabet) m_params.alphabet = get_alphabet_by_name(m_params.methylation_type);
@@ -243,21 +260,7 @@ void MethylationCaller::stage(const EventAlignedRead* const* reads, size_t n, in
             if (!ae.empty()) std::memcpy(pairs + s.pair_off[st], ae.data(), sizeof(AlignedPair) * ae.size());
             // compact form: event-index steps per reference base (nph.h); a step beyond int16, a reference position outside the
             // substring or out of order makes the whole batch fall back to the pair lists
-            int16_t* d = deltas + s.ref_off[st];
-            const long long len = (long long)r.ref_seq.size();
-            for (long long o = 0; o < len; ++o) d[o] = (int16_t)NPH_METH_NO_PAIR;
-            long long prev_off = -1;
-            int prev_ev = ae.empty() ? 0 : ae[0].read_pos;
-            m_first_event[s.rec[st]] = prev_ev;
-            bool ok = true;
-            for (const AlignedPair& ap : ae) {
-                const long long o = (long long)ap.ref_pos - r.ref_start_pos;
-                const long long step = (long long)ap.read_pos - prev_ev;
-                if (o <= prev_off || o >= len || step > 32767 || step < -32767) { ok = false; break; }
-                d[o] = (int16_t)step;
-                prev_off = o; prev_ev = ap.read_pos;
-            }
-            if (!ok) {
+            if (!compact_event_alignment(ae, r.ref_start_pos, r.ref_seq.size(), deltas + s.ref_off[st], &m_first_event[s.rec[st]])) {
 #pragma omp atomic write
                 compact_ok = 0;
             }

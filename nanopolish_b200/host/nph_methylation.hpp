@@ -53,6 +53,11 @@ struct EventAlignedRead {
     bool rc[2] = {false, false};
 };
 
+// The compact event alignment of one record (include/nph.h, nph_methylation_batch_compact): deltas[0, ref_len) and *first_event from
+// aligned_events over a reference substring starting at ref_start_pos.  false: a reference position outside the substring or out of
+// order, or an event-index step beyond int16 (the caller then needs the pair form).
+bool compact_event_alignment(const std::vector<AlignedPair>& aligned_events, int ref_start_pos, size_t ref_len, int16_t* deltas, int32_t* first_event);
+
 // ---- modBAM tags (SAM specification: Mm = delta-encoded positions of the modified base, Ml = probabilities 0..255) ----
 struct ModbamTags {
     std::string mm;                // e.g. "C+m?,3,0,12;"

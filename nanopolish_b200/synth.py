@@ -83,6 +83,10 @@ METH_PARAMS_DT = np.dtype([("min_separation", "<i4"), ("min_flank", "<i4"), ("ma
                            ("bases", "S8"), ("complements", "S8"), ("n_sites", "<u4"), ("site_len", "<u4"),
                            ("sites", "S8", 4), ("sites_methylated", "S8", 4), ("sites_methylated_complement", "S8", 4)], align=True)
 METHFREQ_PARAMS_DT = np.dtype([("call_threshold", "<f8"), ("split_groups", "<u4"), ("reserved", "<u4")], align=True)
+PHASE_VARIANT_DT = np.dtype([("ref_position", "<i4"), ("ref_base", "S1"), ("alt_base", "S1"), ("is_snp", "u1"), ("reserved", "u1")], align=True)
+PHASE_CALL_DT = np.dtype([("record", "<u4"), ("variant", "<u4"), ("ref_score", "<f4"), ("alt_score", "<f4"), ("call", "S1"), ("qual", "u1"),
+                          ("reserved", "u1", 2)], align=True)
+assert PHASE_VARIANT_DT.itemsize == 8 and PHASE_CALL_DT.itemsize == 20
 assert METH_RECORD_DT.itemsize == 40 and METH_SITE_DT.itemsize == 24 and METH_PARAMS_DT.itemsize == 152
 assert ALIGN_STATE_DT.itemsize == 16
 assert READ_DT.itemsize == 64 and HMM_JOB_DT.itemsize == 32 and ABEA_JOB_DT.itemsize == 32
@@ -614,6 +618,43 @@ def compact_event_alignment(records: np.ndarray, pairs: np.ndarray, n_ref_total:
             raise OverflowError("event-index step beyond int16: use the pair form")
         deltas[int(R["ref_off"]) + off] = d.astype(np.int16)
     return deltas, first
+
+
+def phase_batch(rs: ReadSet, model_id: int = 0, seed: int = 0, rc_every: int = 2, step=(30, 1000), p_mismatch: float = 0.05,
+                p_non_snp: float = 0.05, p_no_variants: float = 0.05, p_iupac: float = 0.002):
+    """phase-reads' inputs for reads aligned base for base to their own sequence (methylation_records), each record on its own
+    stretch of one contig: the reference bases (with N / IUPAC bytes planted at rate p_iupac), the pair lists, the records, a
+    sorted variant list PHASE_VARIANT_DT with heterozygous SNPs every step[0]..step[1] bases (REF mismatches and non-SNPs planted,
+    some records without variants) and each record's [lower_bound, upper_bound) range u4[n_records, 2]."""
+    rng = np.random.default_rng(seed)
+    ref, pairs, recs = methylation_records(rs, model_id=model_id, rc_every=rc_every)
+    ref = ref.copy()
+    start = 10_000
+    var = []
+    for i, R in enumerate(recs):
+        n = int(R["ref_len"])
+        shift = start - int(R["ref_start_pos"])
+        recs[i]["ref_start_pos"] = start
+        pairs[int(R["pair_off"]):int(R["pair_off"]) + int(R["n_pairs"])]["ref_pos"] += shift
+        seg = ref[int(R["ref_off"]):int(R["ref_off"]) + n]
+        if rng.random() >= p_no_variants:
+            p = int(rng.integers(0, step[1]))
+            while p < n:
+                base = bytes(seg[p:p + 1])
+                alt = bytes([b"ACGT"[int(rng.integers(4))]])
+                while alt == base:
+                    alt = bytes([b"ACGT"[int(rng.integers(4))]])
+                ref_base = base if rng.random() >= p_mismatch else alt
+                var.append((start + p, ref_base, alt, 0 if rng.random() < p_non_snp else 1, 0))
+                p += int(rng.integers(step[0], step[1] + 1))
+        iu = rng.random(n) < p_iupac
+        seg[iu] = np.frombuffer(b"NRYKMSW", np.uint8)[rng.integers(0, 7, int(iu.sum()))]
+        start += n + 100
+    variants = np.array(var, PHASE_VARIANT_DT) if var else np.zeros(0, PHASE_VARIANT_DT)
+    pos = variants["ref_position"]
+    lo = np.searchsorted(pos, recs["ref_start_pos"], side="left")
+    hi = np.searchsorted(pos, recs["ref_start_pos"].astype(np.int64) + recs["ref_len"].astype(np.int64) - 1, side="right")
+    return ref, pairs, recs, variants, np.stack([lo, hi], axis=1).astype(np.uint32)
 
 
 SCREEN_PARAMS_DT = np.dtype([("flank", "<i4"), ("score_threshold", "<u4"), ("alignment_flags", "<u4"), ("k", "<u4"), ("reads_per_round", "<u4"),
