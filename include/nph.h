@@ -657,7 +657,9 @@ int nph_detect_events_batch(nph_ctx* ctx, const float* raw, size_t n_samples_tot
  * reads[i].sample_off; {0, 0} where the reference returns an empty table (or would trip its assert: fewer samples
  * than one chunk, or no chunk above the threshold).  Only sample_off and n_samples of nph_raw_read are used.
  * ref: src/thirdparty/scrappie/scrappie_common.c:9-190; call site src/nanopolish_squiggle_read.cpp:226-233
- *      (trim_start 200, trim_end 10, varseg_chunk 100, varseg_thresh 0.0).  varseg_chunk <= 128. */
+ *      (trim_start 200, trim_end 10, varseg_chunk 100, varseg_thresh 0.0).  varseg_chunk <= 128.
+ * NPH_ERR_INVALID, before anything runs, for a NaN or infinite sample anywhere in raw[0, n_samples_total): the MADs are order
+ * statistics, and with a NaN the reference's order depends on the C library's qsort. */
 typedef struct { uint32_t start, end; } nph_raw_range;
 int nph_trim_raw_batch(nph_ctx* ctx, const float* raw, size_t n_samples_total, const nph_raw_read* reads, size_t n_reads,
                        int32_t trim_start, int32_t trim_end, int32_t varseg_chunk, float varseg_thresh,
@@ -670,7 +672,9 @@ int nph_trim_raw_batch(nph_ctx* ctx, const float* raw, size_t n_samples_total, c
  *   shift, scale, var                 = recalibrate_model(read, model, strand,
  *                                           get_eventalignment_for_1d_basecalls(...), scale_var=true, scale_drift=false)
  * and the QC that follows.  reads[] carries the scalings the read has before the call (the MoM estimate); they come
- * back unchanged when the read is not recalibrated.  base_to_event_out may be NULL.
+ * back unchanged when the read is not recalibrated.  base_to_event_out may be NULL; its entries at ranks no job covers are
+ * {-1,-1}.  The jobs' rank ranges [rank_off, rank_off + n_kmers) must not overlap (each job's map is built in place at its
+ * rank_off): NPH_ERR_INVALID, before anything runs, when two of them do.
  * ref: src/nanopolish_squiggle_read.cpp:270-336,340-391; src/nanopolish_methyltrain.cpp:204-307. */
 typedef struct { int32_t start, stop; } nph_event_range;      /* IndexPair, src/nanopolish_squiggle_read.h:32-37 */
 #define NPH_CAL_OK              0
@@ -704,7 +708,9 @@ int nph_recalibrate_batch(nph_ctx* ctx, const nph_read* reads, size_t n_reads, c
  * NPH_ERR_UNSUPPORTED if events_cap is too small (n_samples_total / 3 always suffices).  NPH_ERR_INVALID for a k-mer rank
  * >= the model's n_states, and for any sample of raw[0, n_samples_total) outside [-NPH_ABEA_MAX_LEVEL, NPH_ABEA_MAX_LEVEL] (NaN
  * included; samples outside every job's slice too), before any step runs: an event's level is a mean of its samples, so this
- * keeps the events inside the range nph_abea_batch takes. */
+ * keeps the events inside the range nph_abea_batch takes.  NPH_ERR_INVALID too, before any step runs, when two jobs' rank
+ * ranges [rank_off, rank_off + n_kmers) overlap (as for nph_recalibrate_batch); base_to_event_out entries no live job
+ * covers are {-1,-1}. */
 #define NPH_CAL_EMPTY_AFTER_TRIM 16
 typedef struct {
     uint64_t sample_off;      /* first raw sample (picoamps, float) of this read in raw[] */

@@ -105,6 +105,10 @@ extern "C" int nph_load_from_raw_batch(nph_ctx* ctx, const float* raw, size_t n_
         if (!nph_slice_ok(jb.sample_off, jb.n_samples, n_samples_total) || !nph_kmers_ok(jb.rank_off, jb.n_kmers, n_ranks_total) || !(jb.sample_rate > 0.0))
             return NPH_ERR_INVALID;
     }
+    if (!nph_rank_ranges_disjoint(jobs, n_jobs)) {
+        ctx->last_error = "nph_load_from_raw_batch: two jobs share k-mer ranks";
+        return NPH_ERR_INVALID;
+    }
     NPH_CUDA(ctx, cudaSetDevice(ctx->device));
 
     // ---- 1. raw samples and ranks up once, ranks checked; trim (defaults hard-coded at the reference's call site) ----

@@ -294,6 +294,23 @@ inline bool nph_kmers_ok(uint64_t rank_off, uint32_t n_kmers, uint64_t n_ranks) 
 // on the device by nph_check_ranks.
 inline bool nph_abea_job_ok(const nph_abea_job& jb, size_t n_reads, uint64_t n_ranks, uint64_t n_pairs = 0, uint64_t pairs_total = UINT64_MAX)
 { return jb.read < n_reads && nph_kmers_ok(jb.rank_off, jb.n_kmers, n_ranks) && nph_slice_ok(jb.pairs_off, n_pairs, pairs_total); }
+// No two jobs share a k-mer rank: [rank_off, rank_off + n_kmers) of the jobs are pairwise disjoint.  The calibration builds each
+// job's base_to_event map in place at its rank_off (a warp per job, with atomics over its own pair indices), so jobs that share
+// ranks would mix two jobs' pair lists; nph_recalibrate_batch and nph_load_from_raw_batch refuse them.  ABEA and MoM only read
+// the ranks and take shared ranges.
+template <typename Job>
+bool nph_rank_ranges_disjoint(const Job* jobs, size_t n_jobs)
+{
+    size_t j = 1;                       // jobs laid out in rank order (the usual batch) need one pass and no copy
+    while (j < n_jobs && jobs[j].rank_off >= jobs[j - 1].rank_off + jobs[j - 1].n_kmers) ++j;
+    if (j >= n_jobs) return true;
+    std::vector<std::pair<uint64_t, uint64_t>> r(n_jobs);
+    for (size_t i = 0; i < n_jobs; ++i) r[i] = {jobs[i].rank_off, jobs[i].rank_off + jobs[i].n_kmers};
+    std::sort(r.begin(), r.end());
+    for (size_t i = 1; i < n_jobs; ++i)
+        if (r[i].first < r[i - 1].second) return false;
+    return true;
+}
 
 // Indices 0 .. n-1 by key, largest first; equal keys keep index order.
 template <typename K>

@@ -13,6 +13,7 @@
 // (FP64, no contraction), and the 2x2 solve is Eigen's full-pivot LU written out.
 #include "nph_internal.cuh"
 
+#include <cmath>
 #include <cstdlib>
 #include <cstring>
 
@@ -431,6 +432,10 @@ extern "C" int nph_trim_raw_batch(nph_ctx* ctx, const float* raw, size_t n_sampl
     if (n_reads == 0) return NPH_OK;
     if (!raw || !reads || !ranges_out) return NPH_ERR_INVALID;
     if (varseg_chunk < 2) return NPH_ERR_INVALID;
+    // a NaN or an infinity has no place in the order statistics (the sorting network's fminf / fmaxf drop a NaN; the reference's
+    // qsort comparator makes the order with one depend on the C library's sort)
+    for (size_t i = 0; i < n_samples_total; ++i)
+        if (!std::isfinite(raw[i])) { ctx->last_error = "nph_trim_raw_batch: a sample is NaN or infinite"; return NPH_ERR_INVALID; }
     NPH_CUDA(ctx, cudaSetDevice(ctx->device));
     float* d_raw;
     uint8_t* scratch;
@@ -460,6 +465,10 @@ extern "C" int nph_recalibrate_batch(nph_ctx* ctx, const nph_read* reads, size_t
     for (size_t j = 0; j < n_jobs; ++j)     // the pairs a job has are the n_pairs its result reports
         if (results[j].n_pairs > jobs[j].pairs_cap || !nph_abea_job_ok(jobs[j], n_reads, n_ranks_total, results[j].n_pairs, pairs_total))
             return NPH_ERR_INVALID;
+    if (!nph_rank_ranges_disjoint(jobs, n_jobs)) {
+        ctx->last_error = "nph_recalibrate_batch: two jobs share k-mer ranks";
+        return NPH_ERR_INVALID;
+    }
     NPH_CUDA(ctx, cudaSetDevice(ctx->device));
     NphCalArgs a{};
     float* d_ev; nph_read* d_reads; uint32_t* d_rk; nph_abea_job* d_jobs; nph_abea_result* d_res; nph_aligned_pair* d_pairs;
@@ -483,6 +492,7 @@ extern "C" int nph_recalibrate_batch(nph_ctx* ctx, const nph_read* reads, size_t
     NPH_CUDA(ctx, cudaMemcpyAsync(d_res, results, sizeof(nph_abea_result) * n_jobs, cudaMemcpyHostToDevice, ctx->stream));
     if (pairs_total) NPH_CUDA(ctx, cudaMemcpyAsync(d_pairs, pairs, sizeof(nph_aligned_pair) * pairs_total, cudaMemcpyHostToDevice, ctx->stream));
     NPH_TRY(nph_check_ranks(ctx, d_rk, n_ranks_total, ctx->models[model_id].n_states));
+    NPH_CUDA(ctx, cudaMemsetAsync(a.b2e, 0xff, sizeof(nph_event_range) * n_ranks_total, ctx->stream));   // ranks no job covers: {-1,-1}
     NPH_CUDA(ctx, cudaEventRecord(ctx->ev0, ctx->stream));
     NPH_TRY(nph_launch_recalibrate(ctx, a));
     NPH_CUDA(ctx, cudaEventRecord(ctx->ev1, ctx->stream));

@@ -767,12 +767,16 @@ static float npo_madf(const float* x, size_t n, float* space, float* absdiff)
     return mad * mad_scaling_factor;
 }
 
-int npo_trim_raw(const float* raw, size_t n, int trim_start, int trim_end, int varseg_chunk, float varseg_thresh,
-                 uint32_t* start_out, uint32_t* end_out)
+/* npo_trim_raw and what it saw: mad_out[nchunk] the chunks' MADs, stat_out = {threshold, interpolated (0/1)},
+ * kept_out = {first chunk above the threshold, last chunk above it} ({nchunk, -1} when none is).  Returns like npo_trim_raw. */
+int npo_trim_trace(const float* raw, size_t n, int trim_start, int trim_end, int varseg_chunk, float varseg_thresh,
+                   uint32_t* start_out, uint32_t* end_out, float* mad_out, float* stat_out, int64_t* kept_out)
 {
     *start_out = 0; *end_out = 0;
     const size_t chunk = (size_t)varseg_chunk;
     const size_t nchunk = n / chunk;
+    if (stat_out) { stat_out[0] = 0.0f; stat_out[1] = 0.0f; }
+    if (kept_out) { kept_out[0] = (int64_t)nchunk; kept_out[1] = -1; }
     if (nchunk == 0) return 0;
     size_t start = 0, end = nchunk * chunk;
     float* madarr = (float*)malloc(nchunk * sizeof(float));
@@ -780,8 +784,11 @@ int npo_trim_raw(const float* raw, size_t n, int trim_start, int trim_end, int v
     float* absdiff = (float*)malloc(chunk * sizeof(float));
     for (size_t i = 0; i < nchunk; ++i) madarr[i] = npo_madf(raw + i * chunk, chunk, space, absdiff);
     const float thresh = npo_quantilef(madarr, nchunk, varseg_thresh, space);
+    if (mad_out) memcpy(mad_out, madarr, nchunk * sizeof(float));
+    if (stat_out) { stat_out[0] = thresh; stat_out[1] = (size_t)(varseg_thresh * (nchunk - 1)) < nchunk - 1 ? 1.0f : 0.0f; }
     for (size_t i = 0; i < nchunk; ++i) { if (madarr[i] > thresh) break; start += chunk; }
     for (size_t i = nchunk; i > 0; --i) { if (madarr[i - 1] > thresh) break; end -= chunk; }
+    if (kept_out) { kept_out[0] = (int64_t)(start / chunk); kept_out[1] = (int64_t)(end / chunk) - 1; }
     free(madarr); free(space); free(absdiff);
     if (!(end > start)) return 0;                /* assert(rt.end > rt.start) */
     start += (size_t)trim_start;
@@ -792,6 +799,12 @@ int npo_trim_raw(const float* raw, size_t n, int trim_start, int trim_end, int v
     return 1;
 }
 
+int npo_trim_raw(const float* raw, size_t n, int trim_start, int trim_end, int varseg_chunk, float varseg_thresh,
+                 uint32_t* start_out, uint32_t* end_out)
+{
+    return npo_trim_trace(raw, n, trim_start, trim_end, varseg_chunk, varseg_thresh, start_out, end_out, NULL, NULL, NULL);
+}
+
 /* ------------------------------------------------------------------------------------------
  * The tail of SquiggleRead::load_from_raw after ABEA: base_to_event_map + events_per_base
  * (src/nanopolish_squiggle_read.cpp:273-302), get_eventalignment_for_1d_basecalls (:340-391), recalibrate_model with
@@ -800,7 +813,7 @@ int npo_trim_raw(const float* raw, size_t n, int trim_start, int trim_end, int v
  * neither present, so the reference cannot be compiled here.  The solve restates Eigen's FullPivLU for a 2x2 system
  * (largest-entry pivot by row+column swap, rank threshold epsilon*2*maxpivot, unit-lower / upper substitution).
  * ---------------------------------------------------------------------------------------- */
-static void npo_full_piv_lu_solve_2x2(double a00, double a01, double a11, double b0, double b1, double* x0, double* x1)
+static void npo_full_piv_lu_solve_2x2(double a00, double a01, double a11, double b0, double b1, double* x0, double* x1, int* piv)
 {
     double m[2][2] = {{a00, a01}, {a01, a11}};
     double b[2] = {b0, b1};
@@ -810,6 +823,7 @@ static void npo_full_piv_lu_solve_2x2(double a00, double a01, double a11, double
     if (fabs(m[0][1]) > big) { big = fabs(m[0][1]); pr = 0; pc = 1; }
     if (fabs(m[1][1]) > big) { big = fabs(m[1][1]); pr = 1; pc = 1; }
     *x0 = 0.0; *x1 = 0.0;
+    piv[0] = pr; piv[1] = pc; piv[2] = 0;     /* pivot row, pivot column, rank */
     if (big == 0.0) return;
     double t;
     if (pr == 1) { t = m[0][0]; m[0][0] = m[1][0]; m[1][0] = t; t = m[0][1]; m[0][1] = m[1][1]; m[1][1] = t; t = b[0]; b[0] = b[1]; b[1] = t; }
@@ -821,15 +835,23 @@ static void npo_full_piv_lu_solve_2x2(double a00, double a01, double a11, double
     if (fabs(u11) > maxpivot) maxpivot = fabs(u11);
     const double thr = 2.220446049250313e-16 * 2.0 * maxpivot;
     double y0, y1;
-    if (fabs(u11) > thr) { y1 = c1 / u11; y0 = (b[0] - y1 * m[0][1]) / m[0][0]; }
-    else { y1 = 0.0; y0 = b[0] / m[0][0]; }
+    if (fabs(u11) > thr) { y1 = c1 / u11; y0 = (b[0] - y1 * m[0][1]) / m[0][0]; piv[2] = 2; }
+    else { y1 = 0.0; y0 = b[0] / m[0][0]; piv[2] = 1; }
     if (pc == 1) { *x0 = y1; *x1 = y0; } else { *x0 = y0; *x1 = y1; }
 }
 
-void npo_recalibrate(const nph_read* reads, const float* ev_mean, const npo_model* model, const uint32_t* kmer_ranks,
-                     const nph_abea_job* job, const nph_aligned_pair* pairs, uint32_t n_pairs,
-                     nph_event_range* b2e /* n_kmers */, nph_calibration* out)
+/* npo_recalibrate and what it saw: sums_out = {A00, A01, A11, B0, B1} of the normal equations, piv_out = {pivot row, pivot
+ * column, rank (0: all zero, 1, 2)} of the solve (-1 where it did not run), m_kmers_out[n_used] the k-mer of each 'M' event. */
+void npo_recalibrate_trace(const nph_read* reads, const float* ev_mean, const npo_model* model, const uint32_t* kmer_ranks,
+                           const nph_abea_job* job, const nph_aligned_pair* pairs, uint32_t n_pairs,
+                           nph_event_range* b2e /* n_kmers */, nph_calibration* out, double* sums_out, int32_t* piv_out,
+                           uint32_t* m_kmers_out /* n_kmers */)
 {
+    double sums_[5]; int32_t piv_[3];
+    double* sums = sums_out ? sums_out : sums_;
+    int32_t* pv = piv_out ? piv_out : piv_;
+    for (int i = 0; i < 5; ++i) sums[i] = 0.0;
+    pv[0] = pv[1] = pv[2] = -1;
     const nph_read* read = &reads[job->read];
     const float* m = ev_mean + read->event_off;
     const uint32_t* ranks = kmer_ranks + job->rank_off;
@@ -866,6 +888,7 @@ void npo_recalibrate(const nph_read* reads, const float* ev_mean, const npo_mode
                 raw_events[n] = m[event_idx];
                 level_means[n] = model->level_mean[kmer_rank];
                 level_stdvs[n] = model->level_stdv[kmer_rank];
+                if (m_kmers_out) m_kmers_out[n] = (uint32_t)ki;
                 ++n;
             }
             prev_kmer_rank = kmer_rank;
@@ -883,8 +906,11 @@ void npo_recalibrate(const nph_read* reads, const float* ev_mean, const npo_mode
             B0 += e * inv_var;
             B1 += mu * e * inv_var;
         }
+        sums[0] = A00; sums[1] = A01; sums[2] = A11; sums[3] = B0; sums[4] = B1;
         double shift, scale;
-        npo_full_piv_lu_solve_2x2(A00, A01, A11, B0, B1, &shift, &scale);
+        int piv[3];
+        npo_full_piv_lu_solve_2x2(A00, A01, A11, B0, B1, &shift, &scale, piv);
+        pv[0] = piv[0]; pv[1] = piv[1]; pv[2] = piv[2];
         double var = 0.;
         for (size_t i = 0; i < n; ++i) {
             double yi = (raw_events[i] - shift - scale * level_means[i]);
@@ -899,6 +925,13 @@ void npo_recalibrate(const nph_read* reads, const float* ev_mean, const npo_mode
         out->status = NPH_CAL_TOO_FEW_EVENTS;
     }
     free(raw_events); free(level_means); free(level_stdvs);
+}
+
+void npo_recalibrate(const nph_read* reads, const float* ev_mean, const npo_model* model, const uint32_t* kmer_ranks,
+                     const nph_abea_job* job, const nph_aligned_pair* pairs, uint32_t n_pairs,
+                     nph_event_range* b2e /* n_kmers */, nph_calibration* out)
+{
+    npo_recalibrate_trace(reads, ev_mean, model, kmer_ranks, job, pairs, n_pairs, b2e, out, NULL, NULL, NULL);
 }
 
 int npo_max_threads(void)

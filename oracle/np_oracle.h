@@ -66,6 +66,12 @@ int npo_trim_raw(const float* raw, size_t n, int trim_start, int trim_end, int v
 void npo_recalibrate(const nph_read* reads, const float* ev_mean, const npo_model* model, const uint32_t* kmer_ranks,
                      const nph_abea_job* job, const nph_aligned_pair* pairs, uint32_t n_pairs,
                      nph_event_range* b2e, nph_calibration* out);
+/* the same with what they saw (tests/prep_cases.py checks its edge claims on these) */
+int npo_trim_trace(const float* raw, size_t n, int trim_start, int trim_end, int varseg_chunk, float varseg_thresh,
+                   uint32_t* start_out, uint32_t* end_out, float* mad_out, float* stat_out, int64_t* kept_out);
+void npo_recalibrate_trace(const nph_read* reads, const float* ev_mean, const npo_model* model, const uint32_t* kmer_ranks,
+                           const nph_abea_job* job, const nph_aligned_pair* pairs, uint32_t n_pairs,
+                           nph_event_range* b2e, nph_calibration* out, double* sums_out, int32_t* piv_out, uint32_t* m_kmers_out);
 int npo_max_threads(void);
 
 #ifdef __cplusplus

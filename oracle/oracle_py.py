@@ -173,6 +173,33 @@ class PortOracle:
                                    C.c_float(varseg_thresh), C.byref(s), C.byref(e))
         return int(ok), s.value, e.value
 
+    def trim_trace(self, raw, trim_start, trim_end, varseg_chunk, varseg_thresh):
+        """npo_trim_trace: trim_raw's answer and what it saw, as a dict: ok, start, end, mads (f32[n_chunks]), thresh,
+        interp (whether the threshold interpolated), first / last (the first and last chunk above the threshold;
+        n_chunks and -1 when none is)"""
+        s, e = C.c_uint32(), C.c_uint32()
+        nchunk = raw.shape[0] // varseg_chunk
+        mads = np.zeros(max(nchunk, 1), np.float32)
+        stat = np.zeros(2, np.float32)
+        kept = np.zeros(2, np.int64)
+        ok = self.lib.npo_trim_trace(_p(raw), C.c_size_t(raw.shape[0]), C.c_int(trim_start), C.c_int(trim_end), C.c_int(varseg_chunk),
+                                     C.c_float(varseg_thresh), C.byref(s), C.byref(e), _p(mads), _p(stat), _p(kept))
+        return dict(ok=int(ok), start=s.value, end=e.value, mads=mads[:nchunk].copy(), thresh=stat[0], interp=bool(stat[1]),
+                    first=int(kept[0]), last=int(kept[1]))
+
+    def recalibrate_trace(self, reads, ev_mean, model, kmer_ranks, job, pairs, n_pairs):
+        """npo_recalibrate_trace: (b2e, cal, sums f64[5] = A00 A01 A11 B0 B1, piv i32[3] = pivot row, pivot column, rank
+        (-1s where the solve did not run), m_kmers u32[n_used] = the k-mer of each 'M' event)"""
+        from nanopolish_b200.synth import EVENT_RANGE_DT, CALIBRATION_DT
+        marr = self.models([model])
+        jb = np.array([job], dtype=job.dtype)
+        b2e = np.zeros(int(job["n_kmers"]), EVENT_RANGE_DT)
+        cal = np.zeros(1, CALIBRATION_DT)
+        sums = np.zeros(5); piv = np.zeros(3, np.int32); mk = np.zeros(int(job["n_kmers"]), np.uint32)
+        self.lib.npo_recalibrate_trace(_p(reads), _p(ev_mean), marr, _p(kmer_ranks), _p(jb), _p(pairs), C.c_uint32(int(n_pairs)), _p(b2e),
+                                       _p(cal), _p(sums), _p(piv), _p(mk))
+        return b2e, cal[0], sums, piv, mk[:int(cal[0]["n_used"])].copy()
+
     def recalibrate(self, reads, ev_mean, model, kmer_ranks, job, pairs, n_pairs):
         from nanopolish_b200.synth import EVENT_RANGE_DT, CALIBRATION_DT
         marr = self.models([model])
@@ -440,6 +467,14 @@ class RefOracle:
         ok = self.lib.npref_trim_raw(_p(raw), C.c_size_t(raw.shape[0]), C.c_int(trim_start), C.c_int(trim_end), C.c_int(varseg_chunk),
                                      C.c_float(varseg_thresh), C.byref(s), C.byref(e))
         return int(ok), s.value, e.value
+
+    def trim_mads(self, raw, varseg_chunk, varseg_thresh):
+        """npref_trim_mads: scrappie's own madf of every chunk and quantilef of them: (mads f32[n_chunks], threshold)"""
+        nchunk = raw.shape[0] // varseg_chunk
+        mads = np.zeros(max(nchunk, 1), np.float32)
+        self.lib.npref_trim_mads.restype = C.c_float
+        t = self.lib.npref_trim_mads(_p(raw), C.c_size_t(raw.shape[0]), C.c_int(varseg_chunk), C.c_float(varseg_thresh), _p(mads))
+        return mads[:nchunk].copy(), np.float32(t)
 
     def mom(self, read_h, model_h, seq: bytes):
         out = np.zeros(4)

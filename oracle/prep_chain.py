@@ -12,11 +12,13 @@ def squiggle_events(ev, sample_rate):
     return dur, t
 
 
-def oracle_chain(port, model, signals, seqs, sample_rate=4000.0, rna=False):
+def oracle_chain(port, model, signals, seqs, sample_rate=4000.0, rna=False, params=None):
     """Returns per read a dict: events (EVENT_DT), duration, start_time, and — when the read got that far — mom, cal
     (CALIBRATION_DT record), b2e, n_pairs.  rna: scrappie's RNA detector parameters, the MoM estimate on the events in
-    acquisition order, then the events turned around to 5'->3' before ABEA (squiggle_read.cpp:204-213,237-240,262-265)."""
-    prm = synth.event_params(rna)
+    acquisition order, then the events turned around to 5'->3' before ABEA (squiggle_read.cpp:204-213,237-240,262-265).
+    params: an EVENT_PARAMS_DT record to use instead, whose reverse_events says whether the events are turned around."""
+    prm = synth.event_params(rna) if params is None else params
+    rna = bool(prm[0]["reverse_events"])
     out = []
     for x, codes in zip(signals, seqs):
         r = {"events": None}

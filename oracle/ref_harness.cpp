@@ -394,6 +394,20 @@ int npref_trim_raw(const float* raw, size_t n, int trim_start, int trim_end, int
     return 1;
 }
 
+// What trim_raw_by_mad computes before it trims (scrappie_common.c:156-172): scrappie's own madf on every chunk of the signal
+// into mad_out[n / varseg_chunk] and its own quantilef of those MADs at varseg_thresh, returned.  Both are external functions of
+// scrappie_common.c that its header does not declare.  The signal must hold at least one chunk.
+float madf(const float* x, size_t n, const float* med);
+void quantilef(const float* x, size_t nx, float* p, size_t np);
+float npref_trim_mads(const float* raw, size_t n, int varseg_chunk, float varseg_thresh, float* mad_out)
+{
+    const size_t nchunk = n / (size_t)varseg_chunk;
+    for (size_t i = 0; i < nchunk; ++i) mad_out[i] = madf(raw + i * (size_t)varseg_chunk, (size_t)varseg_chunk, NULL);
+    float p = varseg_thresh;
+    quantilef(mad_out, nchunk, &p, 1);
+    return p;
+}
+
 int npref_max_threads(void) { return omp_get_max_threads(); }
 // process-wide settings for callers that drive several harness calls from their own threads: the entry points below save / set /
 // restore hmm_indel_bias_factor and the OpenMP thread count around each call, which is only safe concurrently when every call sets
