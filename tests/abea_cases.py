@@ -41,6 +41,7 @@ end-cell and capacity checks always ends at k-mer 0; check_edges asserts that no
 """
 from __future__ import annotations
 
+import hashlib
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -320,6 +321,21 @@ def make_batch(jobs, model, gap: int = 0, port=None) -> Batch:
 
 def batch(model, port, gap: int = 0, levels: bool = True) -> Batch:
     return make_batch([j for j in all_jobs() if levels or j.family != "levels"], model, gap=gap, port=port)
+
+
+def fingerprint(b: Batch, j: int) -> str:
+    """the inputs of job j, under which the reference's answer is recorded"""
+    jr = b.jobs[j]
+    r = b.reads[int(jr["read"])]
+    o, n = int(r["event_off"]), int(r["n_events"])
+    h = hashlib.sha1()
+    for part in (b.seqs[j], r.tobytes(), b.ev_mean[o:o + n].tobytes(), b.ev_start_time[o:o + n].tobytes()):
+        h.update(part)
+    return h.hexdigest()
+
+
+def pairs_hash(ref_pos, read_pos) -> str:
+    return hashlib.sha1(np.ascontiguousarray(ref_pos, np.int32).tobytes() + np.ascontiguousarray(read_pos, np.int32).tobytes()).hexdigest()
 
 
 # ---------------------------------------------------------------- edges seen on the oracle

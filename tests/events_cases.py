@@ -478,6 +478,13 @@ def fingerprint(x, prm) -> str:
     return hashlib.sha1(np.ascontiguousarray(x, np.float32).tobytes() + prm.tobytes()).hexdigest()
 
 
+def events_hash(start, length, mean, stdv) -> str:
+    h = hashlib.sha1()
+    for a, dt in ((start, np.uint64), (length, np.float32), (mean, np.float32), (stdv, np.float32)):
+        h.update(np.ascontiguousarray(a, dt).tobytes())
+    return h.hexdigest()
+
+
 def check_edges(port, reads=None, configs=CONFIGS):
     """Run every read under every parameter set and configuration on the port oracle, confirm each read's claims and the
     invariants, and return (coverage {(wpr, class): set of edges}, claimed cells, predictions {(read, param, config): Prediction})."""

@@ -444,6 +444,14 @@ def cal_hash(shift, scale, drift, var, epb, n_used, calibrated) -> str:
     return hashlib.sha1(np.float64([shift, scale, drift, var, epb]).tobytes() + repr((int(n_used), bool(calibrated))).encode()).hexdigest()
 
 
+def port_cal_hash(cal, n_pairs) -> str:
+    """cal_hash of an nph_calibration record (the port's or the device's), or "no-alignment" for a job without pairs"""
+    if n_pairs == 0:
+        return "no-alignment"
+    return cal_hash(cal["shift"], cal["scale"], cal["drift"], cal["var"], cal["events_per_base"], cal["n_used"],
+                    int(cal["n_used"]) >= MIN_M)
+
+
 def _model(mean, sd=1.0, name="case"):
     mean = np.asarray(mean, np.float64)
     sd = np.full(mean.shape[0], sd, np.float64) if np.isscalar(sd) else np.asarray(sd, np.float64)

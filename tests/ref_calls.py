@@ -8,6 +8,10 @@ replay checks the method name of every call and fails on a test it holds no reco
 
 Recording: run the tests with NPH_REF_RECORD=<path> where the reference is built; the recorded calls of the tests that ran
 are merged into the committed file and written to <path>.
+
+The edge suites (test_*_edges_oracle.py) keep the reference's answers per case instead, in one CaseRecord per suite
+(tests/golden/ref_*_edges.pkl.xz), keyed by a fingerprint of each case's inputs so that the GPU suites can look them up
+too (case_answers).  NPH_REF_CASES_RECORD=<dir> pytest <edge suites> writes a new record of every suite that ran to <dir>.
 """
 from __future__ import annotations
 
@@ -15,8 +19,14 @@ import copy
 import lzma
 import os
 import pickle
+import signal
 
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_calls.pkl.xz")
+import numpy as np
+import pytest
+
+GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+GOLDEN = os.path.join(GOLDEN_DIR, "ref_calls.pkl.xz")
+ASSERTS = "asserts"
 
 
 def test_key(node) -> str:
@@ -84,3 +94,104 @@ class Replay:
                 raise out
             return copy.deepcopy(out)
         return call
+
+
+def forked(fn):
+    """fn() in a forked child: its pickled result, or ASSERTS if the child died of SIGABRT (the reference aborts the process
+    on a failed assert)"""
+    rd, wr = os.pipe()
+    pid = os.fork()
+    if pid == 0:
+        os.close(rd)
+        try:
+            data = pickle.dumps(fn())
+            with os.fdopen(wr, "wb") as f:
+                f.write(data)
+        finally:
+            os._exit(0)
+    os.close(wr)
+    with os.fdopen(rd, "rb") as f:
+        data = f.read()
+    _, st = os.waitpid(pid, 0)
+    if os.WIFSIGNALED(st) and os.WTERMSIG(st) == signal.SIGABRT:
+        return ASSERTS
+    assert os.WIFEXITED(st) and data, f"reference child ended with status {st}"
+    return pickle.loads(data)
+
+
+def same(a, b) -> bool:
+    """a equals b bit for bit, through tuples, lists, numpy arrays and numpy scalars"""
+    if isinstance(a, (tuple, list)) or isinstance(b, (tuple, list)):
+        return isinstance(a, (tuple, list)) and isinstance(b, (tuple, list)) and len(a) == len(b) and all(map(same, a, b))
+    if isinstance(a, (np.ndarray, np.generic)) or isinstance(b, (np.ndarray, np.generic)):
+        a, b = np.asarray(a), np.asarray(b)
+        return a.dtype == b.dtype and a.shape == b.shape and a.tobytes() == b.tobytes()
+    return type(a) is type(b) and a == b
+
+
+class CaseRecord:
+    """The compiled reference's answers to one edge suite's cases, kept in tests/golden/<name> as {key: [row per case]}, a row
+    being (fingerprint of the case's inputs, answer), or (fingerprint, *answer) where a suite's rows are flat.  Three modes:
+      record  NPH_REF_CASES_RECORD=<dir>: every case is asked of the reference, which must exist and export every entry point
+              in `needs`, and the rows are written to <dir>/<name> at the end of the module;
+      live    the reference exists and exports `needs`: every case is asked of it, and the fingerprints and answers must equal
+              the record's, so a stale record fails here and not only where it is replayed;
+      replay  otherwise (no library, or one built from an older harness): the record's answers, whose fingerprints must equal
+              the cases'."""
+
+    def __init__(self, name: str, needs=()):
+        from oracle.oracle_py import RefOracle
+        self.path = os.path.join(GOLDEN_DIR, name)
+        out = os.environ.get("NPH_REF_CASES_RECORD")
+        self.live = RefOracle() if RefOracle.available() else None
+        if self.live is not None and not all(self.live.has(e) for e in needs):
+            self.live = None
+        if out and self.live is None:
+            pytest.fail(f"NPH_REF_CASES_RECORD needs the compiled reference (oracle/_ref/libnpref.so) exporting {list(needs)}")
+        self.out = os.path.join(out, name) if out else None
+        self.rows = {} if out else load(self.path)
+
+    def answers(self, key: str, fingerprints: list, ask, skip: dict | None = None, fork: bool = False, flat: bool = False) -> list:
+        """The reference's answer to every case, in order.  ask(i) asks the live reference about case i; while recording with
+        `fork` it runs in a forked child, and a child the reference aborts answers ASSERTS.  `skip` maps the cases never sent
+        to the reference to the answer recorded for them."""
+        skip = skip or {}
+        n = len(fingerprints)
+        if self.live is not None:
+            got = [skip[i] if i in skip else forked(lambda i=i: ask(i)) if fork and self.out else ask(i) for i in range(n)]
+            if self.out:
+                self.rows[key] = [(fp, *a) if flat else (fp, a) for fp, a in zip(fingerprints, got)]
+                return got
+        rows = self.rows.get(key)
+        assert rows is not None and len(rows) == n, f"no recorded reference answers for {key} ({self.path}); re-record"
+        want = []
+        for i, (fp, *a) in enumerate(rows):
+            assert fp == fingerprints[i], f"{key}, case {i}: inputs differ from the recorded ones; re-record"
+            want.append(tuple(a) if flat else a[0])
+        if self.live is None:
+            got = [skip.get(i, want[i]) for i in range(n)]
+        bad = [i for i in range(n) if not same(got[i], want[i])]
+        assert not bad, f"{key}: the reference's answers to cases {bad[:5]} ({len(bad)} in all) differ from the record {self.path}"
+        return got
+
+    @property
+    def recording(self) -> bool:
+        return self.out is not None
+
+
+def case_fixture(name: str, needs=()):
+    """a module-scoped fixture holding the CaseRecord of tests/golden/<name>; while recording it writes the record at the end"""
+    def fixture():
+        rec = CaseRecord(name, needs)
+        yield rec
+        if rec.out:
+            os.makedirs(os.path.dirname(rec.out), exist_ok=True)
+            save(rec.rows, rec.out)
+    return pytest.fixture(scope="module")(fixture)
+
+
+def case_answers(name: str, key: str) -> dict:
+    """{fingerprint: answer} of the rows recorded under `key` in tests/golden/<name>"""
+    rows = load(os.path.join(GOLDEN_DIR, name)).get(key)
+    assert rows is not None, f"no recorded reference answers for {key} (tests/golden/{name})"
+    return {fp: (tuple(a) if len(a) > 1 else a[0]) for fp, *a in rows}

@@ -2,40 +2,24 @@
 identical AlignedPairs, and an empty result exactly where the oracle's n_pairs is 0.  The builders' edge claims are checked on
 the oracle's results and band history here too, and the coverage table goes to the test log.
 
-The reference's answers live in tests/golden/ref_abea_edges.pkl.xz, one entry per job: a fingerprint of the job's inputs, the
-number of pairs and a hash of them.  Where oracle/_ref/libnpref.so exists the reference is called live; elsewhere the record
-is replayed.  Jobs whose oracle status is NO_END_CELL never go to the reference, which walks its trace from an unset cell
-there.  NPH_REF_ABEA_RECORD=<path> pytest tests/test_abea_edges_oracle.py writes a new record, each job in a forked child."""
-import hashlib
+The reference's answers live in tests/golden/ref_abea_edges.pkl.xz, one row per job: a fingerprint of the job's inputs, the
+number of pairs and a hash of them (a ref_calls.CaseRecord: asked live where oracle/_ref/libnpref.so exists and compared with
+the record, replayed elsewhere).  Jobs whose oracle status is NO_END_CELL never go to the reference, which walks its trace from
+an unset cell there.  NPH_REF_CASES_RECORD=<dir> pytest tests/test_abea_edges_oracle.py writes a new record to <dir>, each job
+in a forked child."""
 import os
-import pickle
 import re
 
 import numpy as np
 import pytest
 
 from nanopolish_b200 import synth
-from oracle.oracle_py import RefOracle
 from tests import abea_cases as ac
 from tests import ref_calls
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLDEN = os.path.join(ROOT, "tests", "golden", "ref_abea_edges.pkl.xz")
-KERNEL = os.path.join(ROOT, "nanopolish_b200", "csrc", "abea.cu")
+KERNEL = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "nanopolish_b200", "csrc", "abea.cu")
 
-
-def fingerprint(b, j: int) -> str:
-    jr = b.jobs[j]
-    r = b.reads[int(jr["read"])]
-    o, n = int(r["event_off"]), int(r["n_events"])
-    h = hashlib.sha1()
-    for part in (b.seqs[j], r.tobytes(), b.ev_mean[o:o + n].tobytes(), b.ev_start_time[o:o + n].tobytes()):
-        h.update(part)
-    return h.hexdigest()
-
-
-def pairs_hash(ref_pos, read_pos) -> str:
-    return hashlib.sha1(np.ascontiguousarray(ref_pos, np.int32).tobytes() + np.ascontiguousarray(read_pos, np.int32).tobytes()).hexdigest()
+reference = ref_calls.case_fixture("ref_abea_edges.pkl.xz")
 
 
 def _ref_answer(live, handles, b, j):
@@ -43,39 +27,14 @@ def _ref_answer(live, handles, b, j):
     E = int(b.reads[int(jr["read"])]["n_events"])
     pr, n = live.abea(handles[int(jr["read"])], live.builtin_model("nucleotide"), b.seqs[j], E + int(jr["n_kmers"]) + 2)
     assert n >= 0
-    return int(n), pairs_hash(pr[:, 0], pr[:, 1])
+    return int(n), ac.pairs_hash(pr[:, 0], pr[:, 1])
 
 
-def _forked(fn):
-    rd, wr = os.pipe()
-    pid = os.fork()
-    if pid == 0:
-        os.close(rd)
-        try:
-            data = pickle.dumps(fn())
-            with os.fdopen(wr, "wb") as f:
-                f.write(data)
-        finally:
-            os._exit(0)
-    os.close(wr)
-    with os.fdopen(rd, "rb") as f:
-        data = f.read()
-    _, st = os.waitpid(pid, 0)
-    assert os.WIFEXITED(st) and data, f"reference child ended with status {st}"
-    return pickle.loads(data)
-
-
-@pytest.fixture(scope="module")
-def reference():
-    """(live RefOracle or None, recorded answers, record path or None)"""
-    path = os.environ.get("NPH_REF_ABEA_RECORD")
-    live = RefOracle() if RefOracle.available() else None
-    if path and live is None:
-        pytest.fail("NPH_REF_ABEA_RECORD needs the compiled reference (oracle/_ref/libnpref.so)")
-    rec = {} if path else ref_calls.load(GOLDEN)
-    yield live, rec, path
-    if path:
-        ref_calls.save(rec, path)
+def _register(live, b):
+    if live is None:
+        return None
+    live.clear_reads()
+    return live.register_reads(b.reads, b.ev_mean, b.ev_start_time, live.builtin_model("nucleotide"))
 
 
 @pytest.fixture(scope="module")
@@ -98,31 +57,22 @@ def test_kernel_constants():
 
 def test_abea_edges_match_reference(cases, reference):
     model, b, runs, full = cases
-    live, record, path = reference
-    handles = None
-    if live is not None:
-        live.clear_reads()
-        handles = live.register_reads(b.reads, b.ev_mean, b.ev_start_time, live.builtin_model("nucleotide"))
+    live = reference.live
+    handles = _register(live, b)
     n = b.jobs.shape[0]
-    if path:
-        record["abea_edges"] = [(fingerprint(b, j), None if int(full[j][1]["status"]) & ac.NO_END_CELL
-                                 else _forked(lambda j=j: _ref_answer(live, handles, b, j))) for j in range(n)]
-    rec = record.get("abea_edges")
-    assert rec is not None and len(rec) == n, f"no recorded reference answers for these jobs ({GOLDEN}); re-record"
+    skip = {j: None for j in range(n) if int(full[j][1]["status"]) & ac.NO_END_CELL}
+    answers = reference.answers("abea_edges", [ac.fingerprint(b, j) for j in range(n)], lambda j: _ref_answer(live, handles, b, j),
+                                skip=skip, fork=True)
     n_skipped = 0
-    for j in range(n):
-        fp, want = rec[j]
-        assert fp == fingerprint(b, j), f"job {j}: inputs differ from the recorded ones; re-record"
+    for j, want in enumerate(answers):
         pairs, res = full[j][:2]
         if int(res["status"]) & ac.NO_END_CELL:
             assert want is None and int(res["n_pairs"]) == 0
             n_skipped += 1
             continue
-        if live is not None and not path:
-            want = _ref_answer(live, handles, b, j)
         wn, wh = want
         assert int(res["n_pairs"]) == wn, f"job {j}: oracle {int(res['n_pairs'])} pairs (status {int(res['status'])}), reference {wn}"
-        assert pairs_hash(pairs["ref_pos"], pairs["read_pos"]) == wh, f"job {j}: pairs differ from the reference's"
+        assert ac.pairs_hash(pairs["ref_pos"], pairs["read_pos"]) == wh, f"job {j}: pairs differ from the reference's"
     assert n_skipped == sum(int(f[1]["status"]) & ac.NO_END_CELL != 0 for f in full)
 
 
@@ -178,21 +128,13 @@ def test_window_levels_emission(port_oracle):
 def test_mom_matches_reference(port_oracle, reference):
     """npo_mom equals the reference's estimate_scalings_using_mom bit for bit at E, K in {1, 31, 32, 33, 63, 64, 65} and on a
     21 000-event read"""
-    live, record, path = reference
     model = synth.load_model("nucleotide")
     b = ac.mom_batch(model)
+    live = reference.live
+    handles = _register(live, b)
     n = b.jobs.shape[0]
-    if live is not None:
-        live.clear_reads()
-        handles = live.register_reads(b.reads, b.ev_mean, b.ev_start_time, live.builtin_model("nucleotide"))
-        answers = [tuple(live.mom(handles[int(b.jobs[j]["read"])], live.builtin_model("nucleotide"), b.seqs[j])[:2]) for j in range(n)]
-        if path:
-            record["mom"] = [(fingerprint(b, j), answers[j]) for j in range(n)]
-    else:
-        rec = record.get("mom")
-        assert rec is not None and len(rec) == n, f"no recorded reference answers for the MoM jobs ({GOLDEN}); re-record"
-        assert all(fp == fingerprint(b, j) for j, (fp, _) in enumerate(rec)), "MoM inputs differ from the recorded ones; re-record"
-        answers = [a for _, a in rec]
+    answers = reference.answers("mom", [ac.fingerprint(b, j) for j in range(n)], lambda j: tuple(
+        live.mom(handles[int(b.jobs[j]["read"])], live.builtin_model("nucleotide"), b.seqs[j])[:2]))
     for j in range(n):
         got = port_oracle.mom(b.reads, b.ev_mean, model, b.kmer_ranks, b.jobs[j])
         assert np.array_equal(np.array(got).view(np.uint64), np.array(answers[j], np.float64).view(np.uint64)), f"MoM job {j}: {got} vs {answers[j]}"

@@ -2,48 +2,22 @@
 tests/events_cases.py under every parameter set: identical starts, bit-identical length, mean and stdv.  The builders' edge
 claims are checked on the oracle's run here too, and the coverage table goes to the test log.
 
-The reference's answers live in tests/golden/ref_events_edges.pkl.xz, one entry per (read, parameter set): a fingerprint of
-the samples and parameters, and a hash of the events.  Where oracle/_ref/libnpref.so exists and exports
-npref_detect_events_params the reference is called live; elsewhere (no library, or one built from an older harness) the
-record is replayed.  A read without any boundary never goes to the reference (create_events reads peaks[-1]
-there); the port's one-event answer for it is compared with the device only.
-NPH_REF_EVENTS_RECORD=<path> pytest tests/test_events_edges_oracle.py writes a new record."""
-import hashlib
+The reference's answers live in tests/golden/ref_events_edges.pkl.xz, one row per (read, parameter set): a fingerprint of
+the samples and parameters, and a hash of the events (a ref_calls.CaseRecord: asked live where oracle/_ref/libnpref.so exists
+and exports npref_detect_events_params and compared with the record, replayed elsewhere).  A read without any boundary never
+goes to the reference (create_events reads peaks[-1] there); the port's one-event answer for it is compared with the device
+only.  NPH_REF_CASES_RECORD=<dir> pytest tests/test_events_edges_oracle.py writes a new record to <dir>."""
 import os
 import re
 
-import numpy as np
 import pytest
 
-from oracle.oracle_py import RefOracle
 from tests import events_cases as ec
 from tests import ref_calls
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLDEN = os.path.join(ROOT, "tests", "golden", "ref_events_edges.pkl.xz")
-KERNEL = os.path.join(ROOT, "nanopolish_b200", "csrc", "event_detect.cu")
+KERNEL = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "nanopolish_b200", "csrc", "event_detect.cu")
 
-
-def events_hash(start, length, mean, stdv) -> str:
-    h = hashlib.sha1()
-    for a, dt in ((start, np.uint64), (length, np.float32), (mean, np.float32), (stdv, np.float32)):
-        h.update(np.ascontiguousarray(a, dt).tobytes())
-    return h.hexdigest()
-
-
-@pytest.fixture(scope="module")
-def reference():
-    """(live RefOracle or None, recorded answers, record path or None)"""
-    path = os.environ.get("NPH_REF_EVENTS_RECORD")
-    live = RefOracle() if RefOracle.available() else None
-    if live is not None and not live.has("npref_detect_events_params"):
-        live = None                 # a library built from an older harness, without the entry point: replay the record
-    if path and live is None:
-        pytest.fail("NPH_REF_EVENTS_RECORD needs the compiled reference with npref_detect_events_params (oracle/_ref/libnpref.so)")
-    rec = {} if path else ref_calls.load(GOLDEN)
-    yield live, rec, path
-    if path:
-        ref_calls.save(rec, path)
+reference = ref_calls.case_fixture("ref_events_edges.pkl.xz", needs=("npref_detect_events_params",))
 
 
 @pytest.fixture(scope="module")
@@ -97,32 +71,17 @@ def test_sample_span_binds_only_past_2_27_samples():
 
 
 def test_events_edges_match_reference(reads, reference, port_oracle):
-    live, record, path = reference
-    rows, want_rows = [], None if path else record.get("events_edges")
-    assert path or (want_rows is not None), f"no recorded reference answers ({GOLDEN}); re-record"
-    n_ref = 0
-    for pname, prm in ec.PARAMS.items():
-        for r in reads:
-            ev = port_oracle.detect_events(r.x, prm)
-            fp = ec.fingerprint(r.x, prm)
-            mine = events_hash(ev["start"], ev["length"], ev["mean"], ev["stdv"])
-            if ev.shape[0] == 1:
-                rows.append((fp, None))
-                continue
-            if live is not None:
-                got = events_hash(*live.detect_events_params(r.x, prm))
-            else:
-                fp_w, got = want_rows[len(rows)]
-                assert fp_w == fp, f"{r.name} under {pname}: inputs differ from the recorded ones; re-record"
-            rows.append((fp, got))
-            assert mine == got, f"{r.name} under {pname}: the port's events differ from scrappie's"
-            n_ref += 1
-    if path:
-        record["events_edges"] = rows
-    elif live is not None and want_rows is not None:
-        assert [fp for fp, _ in want_rows] == [fp for fp, _ in rows], "edge reads differ from the recorded ones; re-record"
-        assert want_rows == rows, "the compiled reference's answers differ from the record"
-    assert n_ref > 1000
+    cases = [(pname, prm, r) for pname, prm in ec.PARAMS.items() for r in reads]
+    mine = []
+    for pname, prm, r in cases:
+        ev = port_oracle.detect_events(r.x, prm)
+        mine.append(None if ev.shape[0] == 1 else ec.events_hash(ev["start"], ev["length"], ev["mean"], ev["stdv"]))
+    got = reference.answers("events_edges", [ec.fingerprint(r.x, prm) for _, prm, r in cases],
+                            lambda i: ec.events_hash(*reference.live.detect_events_params(cases[i][2].x, cases[i][1])),
+                            skip={i: None for i, m in enumerate(mine) if m is None})
+    for (pname, prm, r), m, g in zip(cases, mine, got):
+        assert m == g, f"{r.name} under {pname}: the port's events differ from scrappie's"
+    assert sum(m is not None for m in mine) > 1000
 
 
 def test_builders_reach_every_edge(port_oracle):

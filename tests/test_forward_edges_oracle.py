@@ -3,35 +3,19 @@
 no k-mer can emit leaves a finite score through the bad-event state.  The builders' edge claims, the coverage of every class and
 the warp layouts the sub-warp classes need are checked here too.
 
-The reference's answers live in tests/golden/ref_forward_edges.pkl.xz, one entry per job with a fingerprint of the job's inputs.
-Where oracle/_ref/libnpref.so exists the reference is called live; elsewhere the record is replayed.  While recording each job
-runs in a forked child, so that a job the reference aborts on would show up as such instead of ending the run:
-NPH_REF_FORWARD_RECORD=<path> pytest tests/test_forward_edges_oracle.py writes a new record."""
-import os
-
+The reference's answers live in tests/golden/ref_forward_edges.pkl.xz, one row per job (a ref_calls.CaseRecord: asked live
+where oracle/_ref/libnpref.so exists and compared with the record, replayed elsewhere).  While recording each job runs in a
+forked child, so that a job the reference aborts on would show up as such instead of ending the run:
+NPH_REF_CASES_RECORD=<dir> pytest tests/test_forward_edges_oracle.py writes a new record to <dir>."""
 import numpy as np
 import pytest
 
 from nanopolish_b200 import synth
-from oracle.oracle_py import RefOracle
 from tests import forward_cases as fc
 from tests import ref_calls
-from tests.test_viterbi_edges_oracle import _fingerprint, _forked
+from tests import viterbi_cases as vc
 
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_forward_edges.pkl.xz")
-
-
-@pytest.fixture(scope="module")
-def reference():
-    """(live RefOracle or None, recorded answers, record path or None)"""
-    path = os.environ.get("NPH_REF_FORWARD_RECORD")
-    live = RefOracle() if RefOracle.available() else None
-    if path and live is None:
-        pytest.fail("NPH_REF_FORWARD_RECORD needs the compiled reference (oracle/_ref/libnpref.so)")
-    rec = {} if path else ref_calls.load(GOLDEN)
-    yield live, rec, path
-    if path:
-        ref_calls.save(rec, path)
+reference = ref_calls.case_fixture("ref_forward_edges.pkl.xz")
 
 
 @pytest.fixture(scope="module")
@@ -45,26 +29,19 @@ def _bits(a):
 
 @pytest.mark.parametrize("bias", fc.BIASES)
 def test_forward_edges_match_reference(port_oracle, reference, cases, bias):
-    live, rec, path = reference
     model = synth.load_model("nucleotide")
     b = cases[bias]
     n = b.jobs.shape[0]
+    live = reference.live
     if live is not None:
         live.clear_reads()
         handles = live.register_reads(b.reads, b.ev_mean, b.ev_start_time, live.builtin_model("nucleotide"))
         mh = [live.builtin_model("nucleotide")]
-    key = f"bias={bias}"
-    if path:
-        rec[key] = [(_fingerprint(b, j, bias), _forked(lambda j=j: live.score_batch(handles, b.jobs[j:j + 1], b.seqs[j:j + 1], mh,
-                                                                                       indel_bias=bias)[0][0]))
-                    for j in range(n)]
-        assert not any(isinstance(w, str) for _, w in rec[key]), "the reference aborts on an edge job: drop it from the builder"
-    assert key in rec and len(rec[key]) == n, f"no recorded reference answers for {key} ({GOLDEN}); re-record"
-    for j in range(n):
-        assert rec[key][j][0] == _fingerprint(b, j, bias), f"job {j}: inputs differ from the recorded ones; re-record"
-    want = np.array([w for _, w in rec[key]], np.float32)
-    if live is not None and not path:
-        want, _ = live.score_batch(handles, b.jobs, b.seqs, mh, indel_bias=bias, threads=8)
+    want = reference.answers(f"bias={bias}", [vc.fingerprint(b, j, bias) for j in range(n)],
+                             lambda j: live.score_batch(handles, b.jobs[j:j + 1], b.seqs[j:j + 1], mh, indel_bias=bias)[0][0],
+                             fork=True)
+    assert not any(isinstance(w, str) for w in want), "the reference aborts on an edge job: drop it from the builder"
+    want = np.array(want, np.float32)
     got, _ = port_oracle.hmm_score_batch(b.reads, b.ev_mean, b.ev_start_time, [model], b.kmer_ranks, b.jobs, indel_bias=bias,
                                          threads=8)
     bad = np.flatnonzero(_bits(got) != _bits(want))

@@ -9,7 +9,6 @@ import torch
 from nanopolish_b200 import synth
 from tests import abea_cases as ac
 from tests import ref_calls
-from tests.test_abea_edges_oracle import GOLDEN, fingerprint, pairs_hash
 
 pytestmark = pytest.mark.gpu
 NPH_ERR_INVALID = -3
@@ -35,13 +34,13 @@ def test_edge_jobs_match_oracle_and_reference(engine, nuc, port_oracle):
     b = ac.batch(model, port_oracle, levels=False)
     pairs, res = engine.abea_batch(b.reads, b.ev_mean, b.ev_start_time, b.kmer_ranks, b.jobs, mid, b.pairs_total)
     _compare(b, pairs, res, model, port_oracle, "edge")
-    rec = dict(ref_calls.load(GOLDEN)["abea_edges"])
+    rec = ref_calls.case_answers("ref_abea_edges.pkl.xz", "abea_edges")
     n_ref = 0
     for j in range(b.jobs.shape[0]):
-        want = rec[fingerprint(b, j)]
+        want = rec[ac.fingerprint(b, j)]
         if int(res[j]["status"]) == 0:
             o, n = int(b.jobs[j]["pairs_off"]), int(res[j]["n_pairs"])
-            assert want is not None and want[0] == n and pairs_hash(pairs["ref_pos"][o:o + n], pairs["read_pos"][o:o + n]) == want[1], \
+            assert want is not None and want[0] == n and ac.pairs_hash(pairs["ref_pos"][o:o + n], pairs["read_pos"][o:o + n]) == want[1], \
                 f"job {j}: pairs differ from the reference's"
             n_ref += 1
     assert n_ref > 150
@@ -95,11 +94,11 @@ def test_mom_edges_bit_exact(engine, nuc, port_oracle):
     model, mid = nuc
     b = ac.mom_batch(model)
     got = engine.mom_batch(b.reads, b.ev_mean, b.kmer_ranks, b.jobs, mid)
-    rec = ref_calls.load(GOLDEN)["mom"]
+    rec = ref_calls.case_answers("ref_abea_edges.pkl.xz", "mom")
     for j in range(b.jobs.shape[0]):
         want = np.array(port_oracle.mom(b.reads, b.ev_mean, model, b.kmer_ranks, b.jobs[j]))
         assert got[j].view(np.uint64).tolist() == want.view(np.uint64).tolist(), f"MoM job {j}: {got[j]} vs {want}"
-        assert rec[j][0] == fingerprint(b, j) and got[j].tolist() == list(rec[j][1])
+        assert got[j].tolist() == list(rec[ac.fingerprint(b, j)])
 
 
 @pytest.mark.parametrize("level", ac.LEVELS)

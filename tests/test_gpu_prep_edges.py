@@ -12,7 +12,6 @@ from nanopolish_b200._lib import NphError
 from oracle.prep_chain import oracle_chain, squiggle_events
 from tests import prep_cases as pc
 from tests import ref_calls
-from tests.test_prep_edges_oracle import GOLDEN, port_cal_hash
 
 pytestmark = pytest.mark.gpu
 
@@ -23,13 +22,6 @@ NPH_ERR_UNSUPPORTED = -6
 @pytest.fixture(scope="module")
 def sm_count():
     return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-@pytest.fixture(scope="module")
-def record():
-    rec = ref_calls.load(GOLDEN)
-    assert "trim" in rec and "cal" in rec, f"no recorded reference answers ({GOLDEN})"
-    return rec
 
 
 def _pack(signals):
@@ -51,9 +43,9 @@ def _status(fn, *a, **k):
 
 
 # ---- trim --------------------------------------------------------------------------------------------------------------
-def test_trim_edges_identical(engine, port_oracle, record):
+def test_trim_edges_identical(engine, port_oracle):
     cases = pc.trim_cases()
-    rows = record["trim"]
+    rec = ref_calls.case_answers("ref_prep_edges.pkl.xz", "trim")
     groups = {}
     for i, c in enumerate(cases):
         groups.setdefault(c.params, []).append(i)
@@ -66,8 +58,9 @@ def test_trim_edges_identical(engine, port_oracle, record):
             t = pc.TrimTrace(port_oracle, c)
             g = (int(got[r]["start"]), int(got[r]["end"]))
             assert g == (t.start, t.end), f"{c.name}: device {g}, port {(t.start, t.end)}"
-            fp, want, _ = rows[i]
-            assert fp == pc.fingerprint(c.x, *c.params), f"{c.name}: inputs differ from the recorded ones"
+            fp = pc.fingerprint(c.x, *c.params)
+            assert fp in rec, f"{c.name}: inputs differ from the recorded ones"
+            want = rec[fp][0]
             if want is not None:
                 assert pc.range_hash(g[1] > g[0], *g) == want, f"{c.name}: device range differs from the reference's"
                 n_ref += 1
@@ -161,13 +154,13 @@ def _check_cal_job(c, t, b2e_dev, cal_dev, ref_hash):
         assert np.float64(cal_dev[f]).view(np.uint64) == np.float64(t.cal[f]).view(np.uint64), f"{c.name}: {f} {cal_dev[f]!r} != {t.cal[f]!r}"
     assert (int(cal_dev["n_used"]), int(cal_dev["status"])) == (int(t.cal["n_used"]), int(t.cal["status"])), \
         f"{c.name}: n_used/status {(int(cal_dev['n_used']), int(cal_dev['status']))} != {(int(t.cal['n_used']), int(t.cal['status']))}"
-    assert port_cal_hash(cal_dev, c.pairs.shape[0]) == ref_hash, f"{c.name}: device calibration differs from the reference's"
+    assert pc.port_cal_hash(cal_dev, c.pairs.shape[0]) == ref_hash, f"{c.name}: device calibration differs from the reference's"
     assert b2e_dev.shape[0] == n
 
 
-def test_calibration_edges_identical(engine, port_oracle, record):
+def test_calibration_edges_identical(engine, port_oracle):
     cases = pc.cal_cases()
-    rows = record["cal"]
+    rec = ref_calls.case_answers("ref_prep_edges.pkl.xz", "cal")
     for idx in _by_model(cases):
         group = [cases[i] for i in idx]
         mid = engine.model_upload(group[0].model)
@@ -176,11 +169,11 @@ def test_calibration_edges_identical(engine, port_oracle, record):
         covered = np.zeros(ranks.shape[0], bool)
         for j, i in enumerate(idx):
             c = cases[i]
-            fp, want = rows[i]
-            assert fp == pc.cal_fingerprint(c), f"{c.name}: inputs differ from the recorded ones"
+            fp = pc.cal_fingerprint(c)
+            assert fp in rec, f"{c.name}: inputs differ from the recorded ones"
             o, n = int(jobs[j]["rank_off"]), int(jobs[j]["n_kmers"])
             covered[o:o + n] = True
-            _check_cal_job(c, pc.CalTrace(port_oracle, c), b2e[o:o + n], cal[j], want)
+            _check_cal_job(c, pc.CalTrace(port_oracle, c), b2e[o:o + n], cal[j], rec[fp])
         assert (b2e["start"][~covered] == -1).all() and (b2e["stop"][~covered] == -1).all(), "ranks no job covers must be {-1,-1}"
 
 

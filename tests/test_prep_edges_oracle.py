@@ -5,38 +5,23 @@ the calibrated flag (get_eventalignment_for_1d_basecalls + recalibrate_model thr
 builders' edge claims are checked on the oracle's traces here too, and the coverage tables go to the test log.
 
 The reference's answers live in tests/golden/ref_prep_edges.pkl.xz: per case a fingerprint of the inputs and hashes of the
-answers.  Where oracle/_ref/libnpref.so exists and exports npref_trim_mads the reference is called live; elsewhere the record
-is replayed.  Trim cases the reference asserts or wraps on (see prep_cases.trim_deviations) are never sent to it.
-NPH_REF_PREP_RECORD=<path> pytest tests/test_prep_edges_oracle.py writes a new record."""
+answers (a ref_calls.CaseRecord: asked live where oracle/_ref/libnpref.so exists and exports npref_trim_mads and
+npref_calibrate and compared with the record, replayed elsewhere).  Trim cases the reference asserts or wraps on (see
+prep_cases.trim_deviations) are never sent to it.
+NPH_REF_CASES_RECORD=<dir> pytest tests/test_prep_edges_oracle.py writes a new record to <dir>."""
 import os
 import re
 
 import numpy as np
-import pytest
 
-from oracle.oracle_py import RefOracle
 from tests import prep_cases as pc
 from tests import ref_calls
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLDEN = os.path.join(ROOT, "tests", "golden", "ref_prep_edges.pkl.xz")
 PREP = os.path.join(ROOT, "nanopolish_b200", "csrc", "squiggle_prep.cu")
 LFR = os.path.join(ROOT, "nanopolish_b200", "csrc", "load_from_raw.cu")
 
-
-@pytest.fixture(scope="module")
-def reference():
-    """(live RefOracle or None, recorded answers, record path or None)"""
-    path = os.environ.get("NPH_REF_PREP_RECORD")
-    live = RefOracle() if RefOracle.available() else None
-    if live is not None and not live.has("npref_trim_mads"):
-        live = None                 # a library built from an older harness, without the entry point: replay the record
-    if path and live is None:
-        pytest.fail("NPH_REF_PREP_RECORD needs the compiled reference with npref_trim_mads (oracle/_ref/libnpref.so)")
-    rec = {} if path else ref_calls.load(GOLDEN)
-    yield live, rec, path
-    if path:
-        ref_calls.save(rec, path)
+reference = ref_calls.case_fixture("ref_prep_edges.pkl.xz", needs=("npref_trim_mads", "npref_calibrate"))
 
 
 def test_kernel_constants():
@@ -63,36 +48,24 @@ def test_kernel_constants():
         assert pc.trim_grid(n, sm) == min(n, 1056)
 
 
+def _ref_trim(live, c):
+    ok, s, e = live.trim_raw(c.x, *c.params)
+    mads, thr = live.trim_mads(c.x, c.chunk, c.perc)
+    return pc.range_hash(ok, s, e), pc.mads_hash(mads, thr)
+
+
 def test_trim_edges_match_reference(reference, port_oracle):
-    live, record, path = reference
-    want_rows = None if path else record.get("trim")
-    assert path or want_rows is not None, f"no recorded reference answers ({GOLDEN}); re-record"
     cases = pc.trim_cases()
-    rows, n_ref = [], 0
-    for i, c in enumerate(cases):
-        t = pc.TrimTrace(port_oracle, c)
-        fp = pc.fingerprint(c.x, *c.params)
-        if not t.ref_ok(c):
-            rows.append((fp, None, None))
-            continue
-        mine = (pc.range_hash(t.ok, t.start, t.end), pc.mads_hash(t.mads, t.thresh))
-        if live is not None:
-            ok, s, e = live.trim_raw(c.x, *c.params)
-            mads, thr = live.trim_mads(c.x, c.chunk, c.perc)
-            got = (pc.range_hash(ok, s, e), pc.mads_hash(mads, thr))
-            assert np.array_equal(mads.view(np.uint32), t.mads.view(np.uint32)), f"{c.name}: MADs differ from scrappie's"
-        else:
-            fp_w, *got = want_rows[i]
-            assert fp_w == fp, f"{c.name}: inputs differ from the recorded ones; re-record"
-            got = tuple(got)
-        rows.append((fp, *got))
-        assert mine == got, f"{c.name}: the port's trim differs from scrappie's"
-        n_ref += 1
-    if path:
-        record["trim"] = rows
-    elif live is not None and want_rows is not None:
-        assert want_rows == rows, "the compiled reference's answers differ from the record"
-    assert n_ref >= len(cases) - len(pc.trim_deviations(cases, {c.name: pc.TrimTrace(port_oracle, c) for c in cases}))
+    traces = [pc.TrimTrace(port_oracle, c) for c in cases]
+    got = reference.answers("trim", [pc.fingerprint(c.x, *c.params) for c in cases], lambda i: _ref_trim(reference.live, cases[i]),
+                            skip={i: (None, None) for i, (c, t) in enumerate(zip(cases, traces)) if not t.ref_ok(c)}, flat=True)
+    n_ref = 0
+    for c, t, g in zip(cases, traces, got):
+        if t.ref_ok(c):
+            mine = (pc.range_hash(t.ok, t.start, t.end), pc.mads_hash(t.mads, t.thresh))
+            assert mine == g, f"{c.name}: the port's trim differs from scrappie's"
+            n_ref += 1
+    assert n_ref >= len(cases) - len(pc.trim_deviations(cases, {c.name: t for c, t in zip(cases, traces)}))
     assert n_ref > 150
 
 
@@ -108,33 +81,12 @@ def _ref_cal(live, c, handles):
                                                          w["n_used"], w["calibrated"])
 
 
-def port_cal_hash(cal, n_pairs):
-    if n_pairs == 0:
-        return "no-alignment"
-    return pc.cal_hash(cal["shift"], cal["scale"], cal["drift"], cal["var"], cal["events_per_base"], cal["n_used"],
-                       int(cal["n_used"]) >= pc.MIN_M)
-
-
 def test_calibration_edges_match_reference(reference, port_oracle):
-    live, record, path = reference
-    want_rows = None if path else record.get("cal")
-    assert path or want_rows is not None, f"no recorded reference answers ({GOLDEN}); re-record"
-    rows, handles = [], {}
-    for i, c in enumerate(pc.cal_cases()):
+    cases, handles = pc.cal_cases(), {}
+    got = reference.answers("cal", [pc.cal_fingerprint(c) for c in cases], lambda i: _ref_cal(reference.live, cases[i], handles))
+    for c, g in zip(cases, got):
         t = pc.CalTrace(port_oracle, c)
-        fp = pc.cal_fingerprint(c)
-        mine = port_cal_hash(t.cal, c.pairs.shape[0])
-        if live is not None:
-            got = _ref_cal(live, c, handles)
-        else:
-            fp_w, got = want_rows[i]
-            assert fp_w == fp, f"{c.name}: inputs differ from the recorded ones; re-record"
-        rows.append((fp, got))
-        assert mine == got, f"{c.name}: the port's calibration differs from the reference's ({t.cal})"
-    if path:
-        record["cal"] = rows
-    elif live is not None and want_rows is not None:
-        assert want_rows == rows, "the compiled reference's answers differ from the record"
+        assert pc.port_cal_hash(t.cal, c.pairs.shape[0]) == g, f"{c.name}: the port's calibration differs from the reference's ({t.cal})"
 
 
 def test_builders_reach_every_edge(port_oracle):

@@ -20,6 +20,7 @@ Every builder returns jobs tagged with the edges they claim, and `check_edges` c
 """
 from __future__ import annotations
 
+import hashlib
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -347,6 +348,18 @@ def batches(model) -> dict:
     """all builder jobs, one batch per indel bias (the C ABI takes one bias per call)"""
     js = all_jobs()
     return {b: make_batch([j for j in js if j.indel_bias == b], model, seed=int(b * 10)) for b in (1.0, 0.9)}
+
+
+def fingerprint(b, j: int, bias: float) -> str:
+    """the inputs of job j of a batch (this module's or forward_cases'), under which the reference's answer is recorded"""
+    jr = b.jobs[j]
+    r = b.reads[int(jr["read"])]
+    o, n = int(r["event_off"]), int(r["n_events"])
+    h = hashlib.sha1()
+    for part in (b.seqs[j], jr.tobytes(), r.tobytes(), b.ev_mean[o:o + n].tobytes(), b.ev_start_time[o:o + n].tobytes(),
+                 np.float64(bias).tobytes()):
+        h.update(part)
+    return h.hexdigest()
 
 
 # ---------------------------------------------------------------- edges seen on a path
