@@ -743,7 +743,9 @@ int nph_last_trim_ranges(nph_ctx* ctx, nph_raw_range* ranges_out, size_t n_jobs)
  * A job with loaded == 0 (the read is missing from the index) or n_events == 0 (load_from_raw cleared its events: any
  * NPH_CAL_* status != 0) is not computed: its result carries NPH_POLYA_READ_FAILED_LOAD and -1 values (:760-777).  NPH_ERR_INVALID, before anything runs, for a loaded job with fewer than 2 samples
  * (the reference's backtrack loop wraps), no k-mer, a sample, event or map slice outside the call's arrays, or a map entry
- * other than {-1, *} or {start, stop} with 0 <= start <= stop < n_events (the reference asserts).  Secondary records and the
+ * other than {-1, *} or {start, stop} with 0 <= start <= stop < n_events (the reference asserts), or a NaN duration in a mapped
+ * span (the reference sorts the per-k-mer durations with std::sort, whose order with a NaN is undefined; +-inf durations and NaN
+ * samples are computed as the reference computes them).  Secondary records and the
  * suffix clip (the length of the record's LAST CIGAR operation, whatever its type) are the caller's to take from the BAM. */
 #define NPH_POLYA_PASS             0
 #define NPH_POLYA_NOREGION         1   /* fewer than 200 adapter or poly(A) samples */

@@ -28,6 +28,7 @@
 #include "nph_internal.cuh"
 #include "libm_exact.cuh"
 
+#include <cmath>
 #include <type_traits>
 #include <vector>
 
@@ -416,6 +417,10 @@ int polya_batch(nph_ctx* ctx, const float* raw, size_t n_samples_total, const np
         for (uint32_t k = 0; k < jb.n_kmers; ++k) {
             const nph_event_range r = base_to_event[jb.rank_off + k];
             if (r.start != -1 && !(r.start >= 0 && r.start <= r.stop && (uint32_t)r.stop < jb.n_events)) return NPH_ERR_INVALID;
+            // a NaN duration in a mapped span: the reference's sort of the per-k-mer durations has no defined order
+            if (r.start != -1)
+                for (int32_t e = r.start; e <= r.stop; ++e)
+                    if (std::isnan(ev_duration[jb.event_off + e])) return NPH_ERR_INVALID;
         }
         live.push_back((uint32_t)j);
         len.push_back(jb.n_samples);

@@ -942,3 +942,209 @@ int npo_max_threads(void)
     return 1;
 #endif
 }
+
+/* ------------------------------------------------------------------------------------------
+ * The poly(A) and detect-polyi tail callers, per read after loading: SegmentationHMM / DPISegmentationHMM ::segment_squiggle,
+ * the read rate, estimate_polya_length and the QC, and for detect-polyi BernoulliHMM::segmentation and
+ * post_boolhmm_detetection_qc.
+ * ref: src/nanopolish_polya_estimator.cpp:204-509, :564-599, :638-722; src/nanopolish_detect_polyi.cpp:177-518, :563-756, :973-997.
+ * Textbook form, on purpose unlike the device's walk: the full backpointer table, the explicit backtrack (p[n-1] = TRANSCRIPT,
+ * p[j] = bptr[j][p[j+1]] for j = n-2 .. 1, p[0] = START), the boundary scan over the labels, the read rate through a sort
+ * and, for poly(I), the Bernoulli Viterbi with its own stored backpointers.
+ * ---------------------------------------------------------------------------------------- */
+enum { TL_S = 0, TL_L, TL_A, TL_P, TL_C, TL_T };
+
+static float tl_pdf(float x, float mean, float sd)          /* normal_pdf */
+{
+    const float a = (x - mean) / sd;
+    return ((float)0.3989422804014327 / sd) * expf((-0.5f * a) * a);
+}
+
+static float tl_log_prob(float p) { return p > 0.00f ? logf(p) : -INFINITY; }
+static float tl_max(float a, float b) { return (a < b) ? b : a; }   /* std::max */
+
+static int tl_dcmp(const void* x, const void* y)
+{
+    const double a = *(const double*)x, b = *(const double*)y;
+    return (a > b) - (a < b);
+}
+
+int npo_polya_trace(int polyi, const float* x, uint32_t n, const float* dur, uint32_t n_events,
+                    const int32_t* map_start, const int32_t* map_stop, uint32_t n_kmers, double sample_rate,
+                    double scale, double shift, double var, uint32_t suffix_clip, npo_tail_result* out,
+                    uint8_t* labels_out, uint16_t* ties_out, uint8_t* bits_out)
+{
+    if (n < 2 || n_kmers == 0) return 0;
+    for (uint32_t k = 0; k < n_kmers; ++k)
+        if (map_start[k] != -1 && !(map_start[k] >= 0 && map_start[k] <= map_stop[k] && (uint32_t)map_stop[k] < n_events)) return 0;
+    /* a NaN duration in a mapped span makes the sort's order undefined */
+    for (uint32_t k = 0; k < n_kmers; ++k)
+        if (map_start[k] != -1)
+            for (int32_t e = map_start[k]; e <= map_stop[k]; ++e)
+                if (isnan(dur[e])) return 0;
+
+    /* the emission Gaussians (:232-250, detect_polyi.cpp:233-255), scaled as the HMM's constructor does (:310-354) */
+    static const float G[8][2] = {{70.2737f, 3.7743f}, {110.973f, 5.237f}, {79.347f, 8.3702f}, {63.3126f, 2.7464f},
+                                  {108.883f, 3.257f}, {79.679f, 6.966f}, {105.784f, 16.022f}, {108.498f, 5.257f}};
+    float gm[8], gs[8], gl[8];
+    for (int g = 0; g < 8; ++g) {
+        gm[g] = (float)shift + (float)scale * G[g][0];
+        gs[g] = (float)var * G[g][1];
+        gl[g] = logf(gs[g]);
+    }
+    const float lisp = (float)log(0.3989422804014327);
+#define TL_LPDF(xx, g) ((lisp - gl[g]) + ((-0.5f * (((xx) - gm[g]) / gs[g])) * (((xx) - gm[g]) / gs[g])))
+    const float lSS = tl_log_prob(0.10f), lSL = tl_log_prob(0.90f), lLL = tl_log_prob(0.90f), lLA = tl_log_prob(0.10f);
+    const float lAA = tl_log_prob(0.95f), lAP = tl_log_prob(0.05f), lPP = tl_log_prob(0.89f), lPC = tl_log_prob(0.01f);
+    const float lPT = tl_log_prob(0.10f), lCP = tl_log_prob(0.99f), lCC = tl_log_prob(0.01f), lTT = tl_log_prob(1.00f);
+
+    uint8_t (*bp)[6] = (uint8_t (*)[6])malloc((size_t)n * 6);
+    uint8_t* reg = (uint8_t*)malloc(n);
+    float v[6];
+    for (uint32_t i = 0; i < n; ++i) {
+        /* row 0 emits the LAST sample (:385-386) */
+        const float xi = x[i == 0 ? n - 1 : i];
+        const float xx = (xi > 200.0f || xi < 40.0f) ? 100.0f : xi;
+        float e[6];
+        e[TL_S] = logf(0.50f * tl_pdf(xx, gm[0], gs[0]) + 0.50f * 0.00476f);
+        e[TL_L] = TL_LPDF(xx, 1);
+        e[TL_A] = logf(0.874f * tl_pdf(xx, gm[2], gs[2]) + 0.126f * tl_pdf(xx, gm[3], gs[3]));
+        e[TL_P] = polyi ? logf(0.500f * tl_pdf(xx, gm[4], gs[4]) + 0.500f * tl_pdf(xx, gm[7], gs[7])) : TL_LPDF(xx, 4);
+        e[TL_C] = (xx > 70.0f && xx < 140.0f) ? -4.2485f : -INFINITY;
+        e[TL_T] = logf(0.346f * tl_pdf(xx, gm[5], gs[5]) + 0.654f * tl_pdf(xx, gm[6], gs[6]));
+        if (i == 0) {
+            v[TL_S] = tl_log_prob(1.00f) + e[TL_S];
+            v[TL_L] = -INFINITY + e[TL_L];
+            v[TL_A] = v[TL_P] = v[TL_C] = v[TL_T] = -INFINITY;
+            memset(bp[0], 0, 6);
+            if (ties_out) ties_out[0] = 0;
+            continue;
+        }
+        const float s_s = v[TL_S] + lSS, s_l = v[TL_S] + lSL, l_l = v[TL_L] + lLL, l_a = v[TL_L] + lLA;
+        const float a_a = v[TL_A] + lAA, a_p = v[TL_A] + lAP, p_p = v[TL_P] + lPP, p_c = v[TL_P] + lPC, p_t = v[TL_P] + lPT;
+        const float c_c = v[TL_C] + lCC, c_p = v[TL_C] + lCP, t_t = v[TL_T] + lTT;
+        v[TL_S] = s_s + e[TL_S];
+        v[TL_L] = tl_max(l_l, s_l) + e[TL_L];
+        v[TL_A] = tl_max(a_a, l_a) + e[TL_A];
+        v[TL_P] = tl_max(p_p, tl_max(a_p, c_p)) + e[TL_P];
+        v[TL_C] = tl_max(c_c, p_c) + e[TL_C];
+        v[TL_T] = tl_max(p_t, t_t) + e[TL_T];
+        /* the backpointers of step i (:411-444): strict <, POLYA's in its precedence P, A, C */
+        bp[i][TL_S] = TL_S;
+        bp[i][TL_L] = s_l < l_l ? TL_L : TL_S;
+        bp[i][TL_A] = l_a < a_a ? TL_A : TL_L;
+        bp[i][TL_P] = (a_p < p_p && c_p < p_p) ? TL_P : (p_p < a_p && c_p < a_p) ? TL_A : TL_C;
+        bp[i][TL_C] = p_c < c_c ? TL_C : TL_P;
+        bp[i][TL_T] = p_t < t_t ? TL_T : TL_P;
+        if (ties_out) {
+            /* bit 2r: rule r's comparison tied at finite scores, bit 2r + 1: at -inf; rules L, A, P-is-P, P-is-A, C, T */
+            const float pa[6][2][2] = {{{s_l, l_l}, {s_l, l_l}}, {{l_a, a_a}, {l_a, a_a}}, {{a_p, p_p}, {c_p, p_p}},
+                                       {{p_p, a_p}, {c_p, a_p}}, {{p_c, c_c}, {p_c, c_c}}, {{p_t, t_t}, {p_t, t_t}}};
+            uint16_t m = 0;
+            for (int r = 0; r < 6; ++r)
+                for (int q = 0; q < 2; ++q)
+                    if (pa[r][q][0] == pa[r][q][1]) m |= (uint16_t)(isinf(pa[r][q][0]) ? 2u << (2 * r) : 1u << (2 * r));
+            ties_out[i] = m;
+        }
+    }
+#undef TL_LPDF
+    reg[n - 1] = TL_T;
+    for (uint32_t j = n - 2; j >= 1 && j < n; --j) reg[j] = bp[j][reg[j + 1]];
+    reg[0] = TL_S;
+    free(bp);
+
+    /* the boundary scan (:474-499) and the sentinel rule (:500-506) */
+    uint64_t ix[5] = {0, 1, 2, 3, 0};
+    for (uint32_t i = 0; i < n; ++i) {
+        const int nx = i + 1 < n ? reg[i + 1] : -1;
+        if (reg[i] == TL_S && nx == TL_L) ix[0] = i;
+        if (reg[i] == TL_L && nx == TL_A) ix[1] = i;
+        if (reg[i] == TL_A && nx == TL_P) ix[2] = i;
+        if (reg[i] == TL_P && nx == TL_T) ix[3] = i;
+        if (reg[i] == TL_C) ix[4] += 1;
+    }
+    out->sentinel = (ix[1] == 1 || ix[2] == 2 || ix[3] == 3);
+    if (out->sentinel) { ix[1] = (uint64_t)n - 3; ix[2] = (uint64_t)n - 2; ix[3] = (uint64_t)n - 1; }
+    if (labels_out) memcpy(labels_out, reg, n);
+    free(reg);
+    for (int k = 0; k < 5; ++k) out->seg[k] = ix[k];
+
+    /* the read rate (:564-599): per-k-mer durations summed in event order, sorted, 1 / element [n / 2] */
+    double* d = (double*)malloc(sizeof(double) * n_kmers);
+    for (uint32_t k = 0; k < n_kmers; ++k) {
+        double s = 0.0;
+        if (map_start[k] != -1)
+            for (int32_t e = map_start[k]; e <= map_stop[k]; ++e) s += (double)dur[e];
+        d[k] = s;
+    }
+    qsort(d, n_kmers, sizeof(double), tl_dcmp);
+    const uint32_t r = n_kmers / 2;
+    out->median[0] = r > 0 ? d[r - 1] : NAN;
+    out->median[1] = d[r];
+    out->median[2] = r + 1 < n_kmers ? d[r + 1] : NAN;
+    const double rate = 1.0 / d[r];
+    free(d);
+
+    /* estimate_polya_length (:638-662) and the QC (:672-722), in size_t and double as the reference has them */
+    const uint64_t ld = ix[1], ad = ix[2], pa = ix[3];
+    const double len = (double)(pa - (ad + 1)) / sample_rate * rate + -5.0;
+    out->read_rate = rate;
+    out->polya_length = (0.0 < len) ? len : 0.0;
+    const double n_adapter = (double)((ad + 1) - ld), n_polya = (double)(pa - (ad + 1));
+    const double adapter_length = (double)(ad - (ld - 1)) / sample_rate * rate;
+    out->qc = NPH_POLYA_PASS;
+    if (n_adapter < 200.0 || n_polya < 200.0) out->qc = NPH_POLYA_NOREGION;
+    else if (adapter_length > 300.0) out->qc = NPH_POLYA_ADAPTER;
+    else if (suffix_clip > 200) out->qc = NPH_POLYA_SUFFCLIP;
+
+    out->polyi_last = out->polya_first = out->detected = -1;
+    out->bernoulli = 0;
+    out->tail_mean = NAN;
+    if (!polyi) return 1;
+
+    /* BernoulliHMM::segmentation(samples, adapter + 1, polya) (detect_polyi.cpp:728-756) */
+    const int start = (int)(ad + 1), stop = (int)pa;
+    out->polyi_last = out->polya_first = -1;
+    if (stop - start >= 100) {
+        const int m = stop - start;
+        float* y = (float*)malloc(sizeof(float) * m);
+        uint8_t* b = (uint8_t*)malloc(m);
+        uint8_t* bpA = (uint8_t*)malloc(m);
+        uint8_t* lab = (uint8_t*)malloc(m);
+        float sum = 0.0f;
+        for (int i = 0; i < m; ++i) { y[i] = (float)(((double)x[start + i] - shift) / scale); sum += y[i]; }
+        const float mean = sum / (float)m;                         /* instance_mean (:655-659) */
+        out->bernoulli = 1;
+        out->tail_mean = mean;
+        for (int i = 0; i < m; ++i) {                               /* log_lkhd_ratio_sequence (:652-675) */
+            const float s = (y[i] - mean) + 108.000f;
+            const float xx = (s > 200.0f || s < 40.0f) ? 100.0f : s;
+            const float lI = logf(tl_pdf(xx, 108.498f, 5.257f)), lA = logf(tl_pdf(xx, 108.883f, 3.257f));
+            b[i] = (lI / lA) > 1.0f;
+        }
+        const float lII = tl_log_prob(0.90f), lIA = tl_log_prob(0.10f), lAA = tl_log_prob(1.00f);
+        const float eI[2] = {logf(1.0f - 0.72304f), logf(0.72304f)}, eA[2] = {logf(1.0f - 0.92154f), logf(0.92154f)};
+        float vI = tl_log_prob(1.00f) + eI[b[0]], vA = -INFINITY + eA[b[0]];
+        bpA[0] = 0;
+        for (int i = 1; i < m; ++i) {                               /* viterbi (:678-725) */
+            const float i2i = vI + lII, i2a = vI + lIA, a2a = vA + lAA;
+            vI = i2i + eI[b[i]];
+            vA = tl_max(i2a, a2a) + eA[b[i]];
+            bpA[i] = a2a < i2a ? 0 : 1;
+        }
+        lab[m - 1] = vI < vA ? 1 : 0;
+        for (int j = m - 2; j >= 1; --j) lab[j] = lab[j + 1] == 0 ? 0 : bpA[j];
+        lab[0] = 0;
+        for (int i = 0; i < m; ++i) {
+            if (lab[i] == 0) out->polyi_last = i;
+            if (lab[i] == 1 && out->polya_first < 0) out->polya_first = i;
+        }
+        if (bits_out) memcpy(bits_out, b, m);
+        free(y); free(b); free(bpA); free(lab);
+    }
+    const int region_length = (int)(pa - (ad + 1));
+    const int polyi_found = out->polyi_last > 200, polya_found = out->polya_first > 0 && region_length - out->polya_first > 200;
+    out->detected = polyi_found ? (polya_found ? NPH_POLYI_A_PLUS_I : NPH_POLYI_POLYI_ONLY)
+                                : (polya_found ? NPH_POLYI_POLYA_ONLY : NPH_POLYI_NONE);
+    return 1;
+}

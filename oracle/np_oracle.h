@@ -73,6 +73,27 @@ void npo_recalibrate_trace(const nph_read* reads, const float* ev_mean, const np
                            const nph_abea_job* job, const nph_aligned_pair* pairs, uint32_t n_pairs,
                            nph_event_range* b2e, nph_calibration* out, double* sums_out, int32_t* piv_out, uint32_t* m_kmers_out);
 int npo_max_threads(void);
+/* one read of the poly(A) (polyi = 0) or detect-polyi (polyi = 1) tail caller: the answer and what it saw.  seg, read_rate,
+ * polya_length, qc, polyi_last, polya_first and detected are the nph_polyi_result fields (-1 for the last three under poly(A));
+ * sentinel: whether segment_squiggle's sentinel rule fired; median: the sorted per-k-mer durations at n_kmers / 2 - 1, n_kmers / 2
+ * and n_kmers / 2 + 1 (NaN where absent); bernoulli: whether the Bernoulli stage ran (poly(I), a tail of 100 samples or more);
+ * tail_mean: its float mean (NaN where it did not run; a tail holding a NaN sample also has a NaN mean). */
+typedef struct {
+    uint64_t seg[5];
+    double   read_rate, polya_length;
+    int32_t  qc, polyi_last, polya_first, detected;
+    int32_t  sentinel, bernoulli;
+    float    tail_mean;
+    double   median[3];
+} npo_tail_result;
+/* Returns 0, computing nothing, where nph_polya_batch refuses the job (n < 2, no k-mer, a bad map entry, a NaN duration in a
+ * mapped span).  Optional traces: labels_out[n] the backtracked state of every sample (0..5 = S L A P C T); ties_out[n] per step,
+ * bit 2r for a tie of rule r's comparison at finite scores and bit 2r + 1 for one at -inf, rules L, A, P-from-P, P-from-A, C,
+ * T; bits_out[polya - adapter - 1] the Bernoulli stage's bits. */
+int npo_polya_trace(int polyi, const float* x, uint32_t n, const float* dur, uint32_t n_events,
+                    const int32_t* map_start, const int32_t* map_stop, uint32_t n_kmers, double sample_rate,
+                    double scale, double shift, double var, uint32_t suffix_clip, npo_tail_result* out,
+                    uint8_t* labels_out, uint16_t* ties_out, uint8_t* bits_out);
 
 #ifdef __cplusplus
 }

@@ -209,8 +209,36 @@ class PortOracle:
         self.lib.npo_recalibrate(_p(reads), _p(ev_mean), marr, _p(kmer_ranks), _p(jb), _p(pairs), C.c_uint32(int(n_pairs)), _p(b2e), _p(cal))
         return b2e, cal[0]
 
+    def tail_trace(self, r, polyi: bool):
+        """npo_polya_trace on one tests.polya_cases.PolyaRead: None where the device refuses the job, else a dict of the answer
+        (seg u64[5], read_rate, polya_length, qc, polyi_last, polya_first, detected) and what it saw (sentinel, median f64[3],
+        bernoulli (whether the Bernoulli stage ran), tail_mean, labels u8[n], ties u16[n], bits u8[tail])"""
+        out = _NpoTailResult()
+        x = np.ascontiguousarray(r.samples, np.float32); d = np.ascontiguousarray(r.duration, np.float32)
+        ms = np.ascontiguousarray(r.map_start, np.int32); me = np.ascontiguousarray(r.map_stop, np.int32)
+        n = x.shape[0]
+        labels = np.zeros(max(n, 1), np.uint8); ties = np.zeros(max(n, 1), np.uint16); bits = np.zeros(max(n, 1), np.uint8)
+        ok = self.lib.npo_polya_trace(C.c_int(int(polyi)), _p(x), C.c_uint32(n), _p(d), C.c_uint32(d.shape[0]), _p(ms), _p(me),
+                                      C.c_uint32(ms.shape[0]), C.c_double(r.sample_rate), C.c_double(r.scale), C.c_double(r.shift),
+                                      C.c_double(r.var), C.c_uint32(r.suffix_clip), C.byref(out), _p(labels), _p(ties), _p(bits))
+        if not ok:
+            return None
+        seg = np.array(out.seg[:], np.uint64)
+        m = int(seg[3]) - int(seg[2]) - 1 if out.bernoulli else 0
+        return dict(seg=seg, read_rate=out.read_rate, polya_length=out.polya_length, qc=out.qc, polyi_last=out.polyi_last,
+                    polya_first=out.polya_first, detected=out.detected, sentinel=bool(out.sentinel),
+                    bernoulli=bool(out.bernoulli), median=np.array(out.median[:]), tail_mean=np.float32(out.tail_mean),
+                    labels=labels[:n].copy(),
+                    ties=ties[:n].copy(), bits=bits[:max(m, 0)].copy())
+
     def max_threads(self):
         return int(self.lib.npo_max_threads())
+
+
+class _NpoTailResult(C.Structure):
+    _fields_ = [("seg", C.c_uint64 * 5), ("read_rate", C.c_double), ("polya_length", C.c_double), ("qc", C.c_int32),
+                ("polyi_last", C.c_int32), ("polya_first", C.c_int32), ("detected", C.c_int32), ("sentinel", C.c_int32), ("bernoulli", C.c_int32),
+                ("tail_mean", C.c_float), ("median", C.c_double * 3)]
 
 
 class RefOracle:

@@ -11,7 +11,9 @@ are merged into the committed file and written to <path>.
 
 The edge suites (test_*_edges_oracle.py) keep the reference's answers per case instead, in one CaseRecord per suite
 (tests/golden/ref_*_edges.pkl.xz), keyed by a fingerprint of each case's inputs so that the GPU suites can look them up
-too (case_answers).  NPH_REF_CASES_RECORD=<dir> pytest <edge suites> writes a new record of every suite that ran to <dir>.
+too (case_answers).  A suite may ask another reference library (the tail callers' oracle/_ref/libnpref_polya.so and
+libnpref_polyi.so) by giving case_fixture its own `ref`.  NPH_REF_CASES_RECORD=<dir> pytest <edge suites> writes a new record of
+every suite that ran to <dir>.
 """
 from __future__ import annotations
 
@@ -139,15 +141,22 @@ class CaseRecord:
       replay  otherwise (no library, or one built from an older harness): the record's answers, whose fingerprints must equal
               the cases'."""
 
-    def __init__(self, name: str, needs=()):
-        from oracle.oracle_py import RefOracle
+    def __init__(self, name: str, needs=(), ref=None):
+        """ref: where the suite asks another library than oracle/_ref/libnpref.so, a callable returning its live handle, or
+        None where that library is not built"""
         self.path = os.path.join(GOLDEN_DIR, name)
         out = os.environ.get("NPH_REF_CASES_RECORD")
-        self.live = RefOracle() if RefOracle.available() else None
-        if self.live is not None and not all(self.live.has(e) for e in needs):
-            self.live = None
+        if ref is None:
+            from oracle.oracle_py import RefOracle
+            self.live = RefOracle() if RefOracle.available() else None
+            if self.live is not None and not all(self.live.has(e) for e in needs):
+                self.live = None
+            what = f"the compiled reference (oracle/_ref/libnpref.so) exporting {list(needs)}"
+        else:
+            self.live = ref()
+            what = f"the compiled reference {getattr(ref, '__doc__', None) or ''}".rstrip()
         if out and self.live is None:
-            pytest.fail(f"NPH_REF_CASES_RECORD needs the compiled reference (oracle/_ref/libnpref.so) exporting {list(needs)}")
+            pytest.fail(f"NPH_REF_CASES_RECORD needs {what}")
         self.out = os.path.join(out, name) if out else None
         self.rows = {} if out else load(self.path)
 
@@ -179,10 +188,10 @@ class CaseRecord:
         return self.out is not None
 
 
-def case_fixture(name: str, needs=()):
+def case_fixture(name: str, needs=(), ref=None):
     """a module-scoped fixture holding the CaseRecord of tests/golden/<name>; while recording it writes the record at the end"""
     def fixture():
-        rec = CaseRecord(name, needs)
+        rec = CaseRecord(name, needs, ref)
         yield rec
         if rec.out:
             os.makedirs(os.path.dirname(rec.out), exist_ok=True)
