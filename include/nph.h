@@ -837,6 +837,80 @@ int nph_phase_reads_batch(nph_ctx* ctx, const nph_read* reads, size_t n_reads,
                           double indel_bias, uint64_t* call_off_out,
                           nph_phase_call* calls_out, size_t calls_cap, uint64_t* n_scored_events_out);
 
+/* ---- variants --fix-homopolymers: the length likelihoods of every homopolymer of a haplotype (ref: fix_homopolymers,
+ * src/nanopolish_call_variants.cpp:541-780) ------------------------------------------------------------------------------
+ * The reference scans the haplotype for runs of 3..9 equal bases and, per run that passes its skip tests, scores every candidate
+ * length L = 3..9 against the run's event sequences.  The scan, the calling range (Haplotype::
+ * get_enclosing_reference_range_for_haplotype_range, substr_by_reference), the call and its application stay with the caller;
+ * this call takes one nph_hp_window per surviving run and returns the two likelihood vectors the reference builds for it:
+ *   the window's event sequences  AlignmentDB::get_event_subsequences over [ref_calling_start, ref_calling_end] (the records of
+ *                                 nph_screen_edits_batch, in record order: bounded by _find_by_ref_bounds, event/bp ratio below 20);
+ *                                 total_reads counts them (the TotalReads INFO value)
+ *   per sequence, in record order, skipped when abs(e_start - e_stop) < 10 (scored_reads counts the rest):
+ *     local_avg = fabs(get_time(e_start) - get_time(e_stop)) / seq_len, get_time(e) = float(start_time[e] - start_time[0]);
+ *     rate = (1 / local_avg) * 2.461964
+ *     per L: the variant sequence = the calling sequence with the run erased to, or extended to, L bases at edit_offset;
+ *       event_lik[L - 3]    += profile_hmm_score(variant, sequence, 0)                    (K1)
+ *       sum_duration         = sum over k-mer slots k0 + 2 .. k0 + L + 1, ascending, of each slot's durations: the float
+ *                              ev_duration of every non-K state of profile_hmm_align(variant, sequence, 0) (K3) on that k-mer,
+ *                              added in double in path order (DurationModel::generate_aligned_durations)
+ *       duration_lik[L - 3] += sum_duration > 0.00025 ? log_gamma_sum(sum_duration, {2.461964, rate}, L) : 0
+ * all in double with the reference's operation order; the log-gamma terms run on the host with its libm (DESIGN.md).
+ * Records: nph_meth_record in the compact form of nph_screen_edits_batch, model_id a nucleotide 6-mer model.  The reads must be
+ * PORETYPE_R9 reads: the reference adds the duration term only for those, and this call always adds it.
+ * ref_bases: the region's reference, ref_bases[p] = base at region_start + p (AlignmentDB's m_region_start .. m_region_end).
+ * NPH_ERR_INVALID: a window with k != 6 (the reference asserts), hp_length outside 3..9, a calling sequence outside calling_seqs,
+ * edit_offset + hp_length past the calling sequence (the reference throws or reads out of bounds), k0 + hp_length + k + 1 past
+ * it (slot k0 + L + 1 would index past the variant sequence's k-mers), a calling range outside the region;
+ * min_flanking_sequence < 7; a record or model out of bounds or not a nucleotide 6-mer model; a job the forward scorer refuses;
+ * a job profile_hmm_align finds no path for (the reference asserts).  NPH_ERR_UNSUPPORTED: a window so long that one CTA's
+ * Viterbi movement trace would exceed 16 GiB (the limit of nph_hmm_align).  The Viterbi states of the jobs are held in consecutive
+ * chunks of (window, read) pairs under 1 GiB of device memory, (E_max + K_max) x 16 bytes per job. */
+#define NPH_HP_MIN_LENGTH 3
+#define NPH_HP_MAX_LENGTH 9
+#define NPH_HP_LENGTHS 7
+typedef struct {
+    int32_t  region_start;            /* AlignmentDB::m_region_start */
+    int32_t  min_flanking_sequence;   /* opt::min_flanking_sequence (30); the caller's scan used it, checked >= 7 */
+    uint32_t max_chunk_pairs;         /* (window, read) pairs per chunk of Viterbi states: 0 = as many as fit the 1 GiB budget */
+    uint32_t reserved;
+} nph_hp_params;                      /* 16 bytes */
+typedef struct {
+    uint64_t seq_off;                 /* first byte of the calling sequence in calling_seqs[] */
+    uint32_t seq_len;                 /* calling_sequence.size() */
+    int32_t  ref_calling_start;       /* the enclosing reference range of the calling window */
+    int32_t  ref_calling_end;
+    uint32_t edit_offset;             /* hap_hp_start - hap_calling_start (after the enclosing range moved hap_calling_start) */
+    uint32_t k0;                      /* hap_hp_start - hap_calling_start - k + 1 */
+    uint32_t hp_length;               /* 3..9 */
+    char     hp_base;
+    uint8_t  reserved[3];
+    uint32_t k;                       /* the reads' base-model k: 6 */
+} nph_hp_window;                      /* 40 bytes */
+typedef struct {
+    uint32_t total_reads;             /* event sequences of the window (TotalReads) */
+    uint32_t scored_reads;            /* of those, the ones with abs(e_start - e_stop) >= 10 */
+    double   event_lik[NPH_HP_LENGTHS];     /* event_likelihoods[L], L = 3..9 */
+    double   duration_lik[NPH_HP_LENGTHS];  /* duration_likelihoods[L] */
+} nph_hp_likelihoods;                 /* 120 bytes */
+typedef struct {
+    uint64_t n_windows, n_pairs;      /* windows; scored (window, read) pairs */
+    uint64_t n_jobs;                  /* 7 per pair, each one forward and one Viterbi fill */
+    uint64_t n_dp_rows;               /* event rows of both fills over all jobs */
+    uint32_t n_chunks;                /* chunks of Viterbi states */
+    uint32_t reserved;
+    double   host_ms;                 /* the host's log-gamma terms and fold.  nph_last_kernel_ms after the call: the forward kernels,
+                                         K3 and the duration kernel of every chunk (not the pair, scan, emit or scheduling kernels) */
+} nph_hp_counts;                      /* 48 bytes */
+int nph_homopolymer_likelihoods_batch(nph_ctx* ctx, const nph_read* reads, size_t n_reads,
+                                      const float* ev_mean, const double* ev_start_time, const float* ev_duration, size_t n_events_total,
+                                      const char* ref_bases, size_t n_ref_bases,
+                                      const int16_t* event_deltas, size_t n_deltas_total, const int32_t* first_event,
+                                      const nph_meth_record* records, size_t n_records,
+                                      const nph_hp_params* params, const char* calling_seqs, size_t n_seq_bytes,
+                                      const nph_hp_window* windows, size_t n_windows, double indel_bias,
+                                      nph_hp_likelihoods* out, nph_hp_counts* counts_out);
+
 /* ---- measurement hooks (used by bench.py; not part of the reference surface) ------------- */
 /* Device time in ms of the most recent nph_hmm_score / nph_abea_run kernel sequence, measured
  * with CUDA events on the context's stream (valid after a sync), and the number of kernel

@@ -38,7 +38,7 @@ struct VitParams {
     const uint32_t* ranks;
     const nph_hmm_job* jobs;
     const uint64_t* states_off;      // n_jobs + 1
-    const uint32_t* order;
+    const uint32_t* order;           // nullptr: jobs in index order
     uint32_t n_jobs;
     unsigned int* counter;
     const float* flank;
@@ -69,7 +69,7 @@ __global__ void __launch_bounds__(kThreads, 1) hmm_viterbi_kernel(const VitParam
     for (;;) {
         const uint32_t slot = nph_warp_pop(p.counter, 1u, lane);
         if (slot >= p.n_jobs) break;
-        const uint32_t job_idx = p.order[slot];
+        const uint32_t job_idx = p.order ? p.order[slot] : slot;
         const nph_hmm_job job = p.jobs[job_idx];
         VitJob j;
         j.rd = p.reads[job.read];
@@ -114,8 +114,73 @@ int launch_vit(nph_ctx* ctx, const VitParams& base, const uint32_t* order, size_
 
 const int kVitCols[] = {1, 2, 3, 4, 6, 8};
 const int kNumVit = 6;
+const uint64_t kTraceBudget = 16ull << 30;
+
+int launch_vit_class(nph_ctx* ctx, int cols, const VitParams& p, const uint32_t* order, size_t count, unsigned int* counter, int max_ctas)
+{
+    switch (cols) {
+        case 1: return launch_vit<1>(ctx, p, order, count, counter, max_ctas);
+        case 2: return launch_vit<2>(ctx, p, order, count, counter, max_ctas);
+        case 3: return launch_vit<3>(ctx, p, order, count, counter, max_ctas);
+        case 4: return launch_vit<4>(ctx, p, order, count, counter, max_ctas);
+        case 6: return launch_vit<6>(ctx, p, order, count, counter, max_ctas);
+        case 8: return launch_vit<8>(ctx, p, order, count, counter, max_ctas);
+    }
+    return NPH_ERR_STATE;
+}
+
+// the cheapest class for a K x E job and its geometry
+int vit_class(uint32_t K, uint32_t E, nph_wave_geom& geo, uint32_t& steps)
+{
+    double best = 1e300; int bi = 0;
+    for (int i = 0; i < kNumVit; ++i) {
+        const nph_wave_geom g = nph_wave_geometry((int)K, (int)E, kVitCols[i], 32, true);
+        const double cost = (double)g.total_steps() * (120.0 + 70.0 * kVitCols[i]);
+        if (cost < best) { best = cost; bi = i; steps = (uint32_t)g.total_steps(); geo = g; }
+    }
+    return bi;
+}
+
+// CTAs whose movement traces fit kTraceBudget, or NPH_ERR_UNSUPPORTED when not even one CTA's do
+int vit_max_ctas(nph_ctx* ctx, size_t trace_stride, int& max_ctas)
+{
+    const uint64_t per_cta = (uint64_t)sizeof(uint16_t) * trace_stride * kWarps;
+    if (per_cta > kTraceBudget) {
+        ctx->last_error = "profile_hmm_align window too large: its movement trace needs " + std::to_string(per_cta >> 20) + " MiB per CTA (limit 16 GiB)";
+        return NPH_ERR_UNSUPPORTED;
+    }
+    max_ctas = (int)std::min<uint64_t>((uint64_t)ctx->sm_count, std::max<uint64_t>(1, kTraceBudget / per_cta));
+    return NPH_OK;
+}
 
 } // namespace
+
+int nph_viterbi_device_jobs(nph_ctx* ctx, size_t n_jobs, uint32_t max_K, uint32_t max_E, const uint64_t* d_states_off,
+                            nph_align_state* d_states, uint32_t* d_n_states)
+{
+    if (n_jobs == 0) return NPH_OK;
+    // one class for the whole batch, chosen for its largest job: the jobs a caller emits here come from windows of one shape
+    // (homopolymer calling windows), so the class a per-job choice would make differs little, and no job needs a host pass
+    nph_wave_geom geo{};
+    uint32_t steps = 0;
+    const int ci = vit_class(max_K, max_E, geo, steps);
+    const size_t trace_stride = (((uint64_t)(steps + 1) * geo.strip + 63) / 64) * 64;
+    int max_ctas = 0;
+    NPH_TRY(vit_max_ctas(ctx, trace_stride, max_ctas));
+    const int warps = max_ctas * kWarps;
+    const uint32_t kpad = std::max<uint32_t>(32, (uint32_t)geo.kpad), period = std::max<uint32_t>(NPH_MIN_PERIOD, (uint32_t)geo.P);
+    VitParams p{};
+    NPH_TRY(nph_carve_align_scratch(ctx, [&](NphArena& a) {
+        nph_wave_scratch(a, kpad, period, warps, &p.scratch_params, &p.scratch_edge);
+        p.scratch_trace = a.take<uint16_t>(trace_stride * warps);
+    }));
+    p.states_off = d_states_off; p.states = d_states; p.n_states = d_n_states; p.scores = nullptr;
+    p.level = ctx->d_level.p; p.reads = ctx->d_reads.p; p.trans = ctx->d_trans.p; p.models = ctx->d_models.p;
+    p.ranks = ctx->d_ranks.p; p.jobs = ctx->d_jobs.p; p.flank = ctx->d_flank.p;
+    p.kpad_stride = kpad; p.edge_stride = nph_edge_stride(period); p.trace_stride = trace_stride; p.c = ctx->consts;
+    NPH_CUDA(ctx, cudaMemsetAsync(ctx->d_counters.p, 0, sizeof(unsigned int), ctx->stream));
+    return launch_vit_class(ctx, kVitCols[ci], p, nullptr, n_jobs, ctx->d_counters.p, max_ctas);
+}
 
 extern "C" int nph_hmm_align_batch(nph_ctx* ctx,
                                    const nph_read* reads, size_t n_reads,
@@ -148,16 +213,10 @@ extern "C" int nph_hmm_align(nph_ctx* ctx,
     uint64_t max_trace = 1;
     for (size_t j = 0; j < n_jobs; ++j) {
         const nph_hmm_job& jb = jobs[j];
-        const uint32_t E = (uint32_t)nph_job_events(jb);
-        const uint32_t K = jb.n_kmers;
         if (states_off[j + 1] < states_off[j]) return NPH_ERR_INVALID;
-        double best = 1e300; int bi = 0; uint32_t bsteps = 0;
+        uint32_t bsteps = 0;
         nph_wave_geom geo{};
-        for (int i = 0; i < kNumVit; ++i) {
-            const nph_wave_geom g = nph_wave_geometry((int)K, (int)E, kVitCols[i], 32, true);
-            const double cost = (double)g.total_steps() * (120.0 + 70.0 * kVitCols[i]);
-            if (cost < best) { best = cost; bi = i; bsteps = (uint32_t)g.total_steps(); geo = g; }
-        }
+        const int bi = vit_class(jb.n_kmers, (uint32_t)nph_job_events(jb), geo, bsteps);
         key[j] = (uint64_t)(kNumVit - 1 - bi) << 32 | bsteps;
         ++first[bi + 1];
         max_kpad = std::max(max_kpad, (uint32_t)geo.kpad);
@@ -172,13 +231,8 @@ extern "C" int nph_hmm_align(nph_ctx* ctx,
     // the trace arena stays within kTraceBudget, and a job whose trace does not fit a single CTA's 16 warps within
     // that budget is refused with NPH_ERR_UNSUPPORTED (documented in include/nph.h) instead of a NOMEM surprise.
     const size_t trace_stride = ((max_trace + 63) / 64) * 64;
-    const uint64_t kTraceBudget = 16ull << 30;
-    const uint64_t per_cta = (uint64_t)sizeof(uint16_t) * trace_stride * kWarps;
-    if (per_cta > kTraceBudget) {
-        ctx->last_error = "profile_hmm_align window too large: its movement trace needs " + std::to_string(per_cta >> 20) + " MiB per CTA (limit 16 GiB)";
-        return NPH_ERR_UNSUPPORTED;
-    }
-    const int max_ctas = (int)std::min<uint64_t>((uint64_t)ctx->sm_count, std::max<uint64_t>(1, kTraceBudget / per_cta));
+    int max_ctas = 0;
+    NPH_TRY(vit_max_ctas(ctx, trace_stride, max_ctas));
     const int warps = max_ctas * kWarps;
     const size_t total_states = (size_t)states_off[n_jobs];
     VitParams p{};
@@ -204,16 +258,7 @@ extern "C" int nph_hmm_align(nph_ctx* ctx,
     for (int i = 0; i < kNumVit; ++i) {
         const size_t count = first[i + 1] - first[i];
         if (!count) continue;
-        int rc = NPH_ERR_STATE;
-        switch (kVitCols[i]) {
-            case 1: rc = launch_vit<1>(ctx, p, d_order + first[i], count, ctx->d_counters.p + i, max_ctas); break;
-            case 2: rc = launch_vit<2>(ctx, p, d_order + first[i], count, ctx->d_counters.p + i, max_ctas); break;
-            case 3: rc = launch_vit<3>(ctx, p, d_order + first[i], count, ctx->d_counters.p + i, max_ctas); break;
-            case 4: rc = launch_vit<4>(ctx, p, d_order + first[i], count, ctx->d_counters.p + i, max_ctas); break;
-            case 6: rc = launch_vit<6>(ctx, p, d_order + first[i], count, ctx->d_counters.p + i, max_ctas); break;
-            case 8: rc = launch_vit<8>(ctx, p, d_order + first[i], count, ctx->d_counters.p + i, max_ctas); break;
-        }
-        if (rc != NPH_OK) return rc;
+        NPH_TRY(launch_vit_class(ctx, kVitCols[i], p, d_order + first[i], count, ctx->d_counters.p + i, max_ctas));
         ++launches;
     }
     NPH_CUDA(ctx, cudaEventRecord(ctx->ev1, ctx->stream));

@@ -209,6 +209,15 @@ struct nph_ctx {
         DevBuf<nph_phase_call> d_calls;
     } phase;
 
+    // the last nph_homopolymer_likelihoods_batch (homopolymer.cu)
+    struct HpState {
+        NphEventRecords ev;                // region reference, compact event alignments, records
+        DevBuf<uint8_t> d_in;              // windows, calling sequences, event durations
+        DevBuf<uint8_t> d_counts;          // per-window read counts, scored-pair offsets, the scan's scratch, two flags
+        DevBuf<uint8_t> d_pairs;           // scored pairs, their windows, per job the forward score and sum_duration
+        DevBuf<uint8_t> d_states;          // one chunk's state offsets, state counts and Viterbi states
+    } hp;
+
     // measurement
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     // side streams so that the tail of one forward class overlaps the head of the next (fork/join by events)
@@ -411,6 +420,12 @@ int nph_jobs_schedule(nph_ctx* ctx, size_t n_jobs, size_t n_ranks_total, NphJobS
 // Scores n_jobs jobs that emit() writes into ctx->d_jobs (ranks already in ctx->d_ranks, written by a kernel of ours): reserves
 // the job, order and score arrays, uploads the read transitions, runs emit(), schedules and launches the forward kernels.
 int nph_score_device_jobs(nph_ctx* ctx, size_t n_jobs, size_t n_ranks_total, double indel_bias, const std::function<int()>& emit);
+// K3 on the n_jobs jobs a kernel of ours wrote into ctx->d_jobs / d_ranks, read transitions and flank table already in place (as
+// nph_score_device_jobs leaves them; hmm_viterbi.cu): one class and trace size for the bounds max_K x max_E, jobs in index order.
+// Job j's path goes to d_states[d_states_off[j] ..) (room d_states_off[j + 1] - d_states_off[j]), its length to d_n_states[j]
+// (0 where the reference would assert).  Device pointers; nothing is read back.
+int nph_viterbi_device_jobs(nph_ctx* ctx, size_t n_jobs, uint32_t max_K, uint32_t max_E, const uint64_t* d_states_off,
+                            nph_align_state* d_states, uint32_t* d_n_states);
 // One-shot calls (read batch, work and results in one call).  Begin: read records on the main stream, then upload() (the
 // jobs or records), then the event levels in chunks on the copy stream behind progress words the forward kernel polls —
 // enumeration and scheduling run while the levels still cross PCIe.  Finish, on every path: wait for the copy stream.
@@ -476,6 +491,15 @@ __device__ __forceinline__ bool nph_find_by_ref_bounds(const nph_meth_record& R,
     if (!(is <= os || is != fv)) return false;                   // left_bounded; right_bounded always holds for a lower_bound
     e1 = dense[is]; e2 = dense[ie];
     return true;
+}
+// AlignmentDB::get_event_subsequences (ref: src/alignment/nanopolish_alignment_db.cpp:172-221) for one record and the window
+// [cs, ce]: nph_find_by_ref_bounds plus the event/bp ratio test.  Variant screening and homopolymer fixing call it.
+__device__ __forceinline__ bool nph_event_subsequence(const nph_meth_record& R, const int32_t* __restrict__ dense, int fv, int cs, int ce,
+                                                      int& e1, int& e2)
+{
+    if (!nph_find_by_ref_bounds(R, dense, fv, cs, ce, e1, e2)) return false;
+    const double ratio = fabs((double)(e1 - e2)) / fabs((double)(ce - cs));
+    return ratio < 20.0;                                         // MAX_EVENT_TO_BP_RATIO
 }
 
 // Alphabet::rank of the DNA alphabet: unknown symbols rank 0

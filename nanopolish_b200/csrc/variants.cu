@@ -75,14 +75,6 @@ __device__ __forceinline__ uint64_t pool_slot(const VarDev& d, int pi, int seq, 
     return ((uint64_t)pi * kSeqs + (uint64_t)seq) * (uint64_t)(1 + d.T) + (uint64_t)a;
 }
 
-// _find_by_ref_bounds + the event/bp ratio test of get_event_subsequences for one record and window [cs, ce]
-__device__ __forceinline__ bool window_events(const nph_meth_record& R, const int32_t* __restrict__ dense, int fv, int cs, int ce, int& e1, int& e2)
-{
-    if (!nph_find_by_ref_bounds(R, dense, fv, cs, ce, e1, e2)) return false;
-    const double ratio = fabs((double)(e1 - e2)) / fabs((double)(ce - cs));
-    return ratio < 20.0;                                         // MAX_EVENT_TO_BP_RATIO
-}
-
 // pass 0: counts per position; pass 1: fills pos_reads behind pos_off
 template <bool FILL>
 __global__ void __launch_bounds__(kBlock) var_bounds_kernel(const VarDev d, const nph_meth_record* __restrict__ records, uint32_t n_records,
@@ -134,7 +126,7 @@ __global__ void __launch_bounds__(kBlock) var_bounds_kernel(const VarDev d, cons
             const uint32_t r = use_list ? s_list[t] : t;
             const nph_meth_record R = records[r];
             int e1, e2;
-            if (window_events(R, dense + R.ref_off, first_valid[r], cs, ce, e1, e2)) {
+            if (nph_event_subsequence(R, dense + R.ref_off, first_valid[r], cs, ce, e1, e2)) {
                 if (FILL) out[cnt] = PosRead{r, e1, e2};
                 ++cnt;
             }

@@ -10,7 +10,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from .synth import ABEA_RES_DT, ALIGN_STATE_DT, CALIBRATION_DT, EVENT_DT, EVENT_RANGE_DT, METH_SITE_DT, METHFREQ_PARAMS_DT, PAIR_DT, PHASE_CALL_DT, PHASE_VARIANT_DT, POLYA_RES_DT, POLYI_RES_DT, RAW_RANGE_DT
+from .synth import ABEA_RES_DT, ALIGN_STATE_DT, CALIBRATION_DT, EVENT_DT, EVENT_RANGE_DT, METH_SITE_DT, METHFREQ_PARAMS_DT, HP_COUNTS_DT, HP_LIK_DT, HP_WINDOW_DT, PAIR_DT, PHASE_CALL_DT, PHASE_VARIANT_DT, POLYA_RES_DT, POLYI_RES_DT, RAW_RANGE_DT
 
 
 def _p(a):
@@ -191,6 +191,21 @@ class Engine:
             self._check(self.lib.nph_screen_edits_batch_methylation(*head, _p(meth), _p(ids), _p(q), _p(nr), C.byref(scored)),
                         "nph_screen_edits_batch_methylation")
         return q, nr, int(scored.value)
+
+    # ---- variants --fix-homopolymers: length likelihoods of every calling window (include/nph.h, nph_homopolymer_likelihoods_batch) ----
+    def homopolymer_likelihoods_batch(self, reads, ev_mean, ev_start_time, ev_duration, ref_bases, deltas, first_event, records, params,
+                                      calling_seqs, windows, indel_bias: float = 1.0):
+        """records METH_RECORD_DT (compact event alignments, as screening's), params HP_PARAMS_DT[1], calling_seqs u1, windows
+        HP_WINDOW_DT.  Returns (HP_LIK_DT[n_windows], HP_COUNTS_DT scalar)."""
+        assert windows.dtype == HP_WINDOW_DT
+        out = np.zeros(max(windows.shape[0], 1), HP_LIK_DT)
+        cnt = np.zeros(1, HP_COUNTS_DT)
+        self._check(self.lib.nph_homopolymer_likelihoods_batch(self.ctx, _p(reads), reads.shape[0], _p(ev_mean), _p(ev_start_time), _p(ev_duration),
+                                                               ev_mean.shape[0], _p(ref_bases), ref_bases.shape[0], _p(deltas), deltas.shape[0],
+                                                               _p(first_event), _p(records), records.shape[0], _p(params), _p(calling_seqs),
+                                                               calling_seqs.shape[0], _p(windows), windows.shape[0], indel_bias, _p(out), _p(cnt)),
+                    "nph_homopolymer_likelihoods_batch")
+        return out[:windows.shape[0]], cnt[0]
 
     def screen_load(self, ref_bases, deltas, first_event, records, params, indel_bias: float = 1.0, methylation=None):
         head = (self.ctx, _p(ref_bases), ref_bases.shape[0], _p(deltas), deltas.shape[0], _p(first_event), _p(records), records.shape[0], _p(params),

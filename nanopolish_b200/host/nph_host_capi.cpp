@@ -834,4 +834,96 @@ long long nphh_aligned_segments(int ref_pos, const uint32_t* cigar, int n_cigar,
     return rc ? rc : n;
 }
 
+// nph::homopolymer_call on the vectors e_lik[7], d_lik[7] (L = 3..9) of a run of hp_length bases: returns 1 when the call is kept
+int nphh_homopolymer_call(const double* e_lik, const double* d_lik, uint32_t hp_length, uint64_t* call, double* quality, int* size_diff)
+{
+    nph_hp_likelihoods lik;
+    std::memset(&lik, 0, sizeof(lik));
+    std::memcpy(lik.event_lik, e_lik, sizeof(lik.event_lik));
+    std::memcpy(lik.duration_lik, d_lik, sizeof(lik.duration_lik));
+    const HomopolymerCall c = homopolymer_call(lik, hp_length);
+    *call = c.call; *quality = c.quality; *size_diff = c.size_diff;
+    return c.kept ? 1 : 0;
+}
+
+// the event durations of read `read` (SquiggleEvent::duration, strand 0)
+void nphh_read_set_durations(int read, const float* duration)
+{
+    std::vector<SquiggleEvent>& ev = g_reads[read]->events[0];
+    for (size_t i = 0; i < ev.size(); ++i) ev[i].duration = duration[i];
+}
+
+// nph::fix_homopolymers on Haplotype(contig, hap_pos, hap_ref) + the variants applied in order, over the region [region_start,
+// region_start + strlen(region_ref) - 1] with one record per entry (registered read read[r], strand 0, rc, aligned_events as
+// (ref_pos, event_idx) pairs [pair_off[r], pair_off[r + 1])).  out: the fixed sequence, a newline, then one line per variant the
+// call added: ref_position \t ref_seq \t alt_seq \t quality as 16 hex digits of its bits \t info.  Returns the length written, or
+// a negative nph_status (-2 .. -6; NPH_ERR_INVALID also when a variant of the input does not apply or out is too small).
+long long nphh_fix_homopolymers(const char* contig, int region_start, const char* region_ref, int n_records, const int32_t* read, const uint8_t* rc,
+                                const int32_t* pairs, const uint64_t* pair_off, int hap_pos, const char* hap_ref, int n_variants,
+                                const int32_t* var_pos, const char** var_ref, const char** var_alt, int min_flank, double indel_bias,
+                                char* out, size_t cap)
+{
+    long long n = -1;
+    int st = guard([&] {
+        HomopolymerRegion region;
+        region.contig = contig; region.region_start = region_start; region.reference = region_ref;
+        for (int r = 0; r < n_records; ++r) {
+            EventAlignedRead e;
+            e.read = g_reads[read[r]].get();
+            e.contig = contig;
+            e.rc[0] = rc[r] != 0;
+            const uint64_t np = pair_off[r + 1] - pair_off[r];
+            e.aligned_events[0].resize(np);
+            if (np) std::memcpy(e.aligned_events[0].data(), pairs + 2 * pair_off[r], sizeof(AlignedPair) * np);
+            region.records.push_back(std::move(e));
+        }
+        Haplotype hap(contig, (size_t)hap_pos, hap_ref);
+        for (int i = 0; i < n_variants; ++i) {
+            Variant v;
+            v.ref_name = contig; v.ref_position = (size_t)var_pos[i]; v.ref_seq = var_ref[i]; v.alt_seq = var_alt[i];
+            if (!hap.apply_variant(v)) throw Error(NPH_ERR_INVALID, "an input variant does not apply");
+        }
+        const Haplotype fixed = fix_homopolymers(hap, region, min_flank, Engine::thread_default(), indel_bias);
+        std::string s = fixed.get_sequence() + "\n";
+        for (size_t i = (size_t)n_variants; i < fixed.get_variants().size(); ++i) {
+            const Variant& v = fixed.get_variants()[i];
+            uint64_t bits;
+            std::memcpy(&bits, &v.quality, sizeof(bits));
+            char q[32];
+            std::snprintf(q, sizeof(q), "%016llx", (unsigned long long)bits);
+            s += std::to_string(v.ref_position) + "\t" + v.ref_seq + "\t" + v.alt_seq + "\t" + q + "\t" + v.info + "\n";
+        }
+        if (s.size() + 1 > cap) throw Error(NPH_ERR_INVALID, "output buffer too small");
+        std::memcpy(out, s.c_str(), s.size() + 1);
+        n = (long long)s.size();
+    });
+    return st ? st : n;
+}
+
+// the mirror's Haplotype::substr_by_reference and enclosing range on Haplotype(contig, hap_pos, hap_ref) + the variants:
+// out = the substring's sequence; range = {hap_lower, hap_upper, ref_lower, ref_upper} of the enclosing range of [lo, hi]
+// (npos as -1).  Returns the substring's reference position, or a negative nph_status where the reference asserts.
+long long nphh_haplotype_ranges(int hap_pos, const char* hap_ref, int n_variants, const int32_t* var_pos, const char** var_ref, const char** var_alt,
+                                long long start, long long end, long long lo, long long hi, long long* range, char* out, size_t cap)
+{
+    long long pos = -1;
+    int st = guard([&] {
+        Haplotype hap("ctg", (size_t)hap_pos, hap_ref);
+        for (int i = 0; i < n_variants; ++i) {
+            Variant v;
+            v.ref_name = "ctg"; v.ref_position = (size_t)var_pos[i]; v.ref_seq = var_ref[i]; v.alt_seq = var_alt[i];
+            if (!hap.apply_variant(v)) throw Error(NPH_ERR_INVALID, "an input variant does not apply");
+        }
+        size_t a = (size_t)lo, b = (size_t)hi, ra = 0, rb = 0;
+        hap.get_enclosing_reference_range_for_haplotype_range(a, b, ra, rb);
+        const size_t r4[4] = {a, b, ra, rb};
+        for (int i = 0; i < 4; ++i) range[i] = r4[i] == std::string::npos ? -1 : (long long)r4[i];
+        const Haplotype sub = hap.substr_by_reference((size_t)start, (size_t)end);
+        if (sub.get_sequence().size() + 1 > cap) throw Error(NPH_ERR_INVALID, "output buffer too small");
+        std::memcpy(out, sub.get_sequence().c_str(), sub.get_sequence().size() + 1);
+        pos = (long long)sub.get_reference_position();
+    });
+    return st ? st : pos;
+}
+
 } // extern "C"

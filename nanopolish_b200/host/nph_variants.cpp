@@ -2,6 +2,7 @@
 #include "nph_variants.hpp"
 
 #include <cmath>
+#include <cstring>
 
 namespace nph {
 
@@ -14,11 +15,19 @@ Haplotype::Haplotype(const std::string& ref_name, size_t ref_position, const std
     for (size_t i = 0; i < m_coordinate_map.size(); ++i) m_coordinate_map[i] = m_ref_position + i;
 }
 
+// The first base with a reference position >= ref_index (the reference scans linearly).  The positions of the bases that have one
+// ascend, so the position of the first such base at or after i is a non-decreasing function of i: a bisection over i finds it.
 size_t Haplotype::find_derived_index_by_ref_lower_bound(size_t ref_index) const
 {
-    for (size_t i = 0; i < m_coordinate_map.size(); ++i)
-        if (m_coordinate_map[i] != INSERTED_POSITION && m_coordinate_map[i] >= ref_index) return i;
-    return m_coordinate_map.size();
+    const size_t n = m_coordinate_map.size();
+    const auto next = [&](size_t i) { while (i < n && m_coordinate_map[i] == INSERTED_POSITION) ++i; return i; };
+    size_t lo = 0, hi = n;
+    while (lo < hi) {
+        const size_t mid = lo + (hi - lo) / 2, j = next(mid);
+        if (j == n || m_coordinate_map[j] >= ref_index) hi = mid;
+        else lo = j + 1;
+    }
+    return next(lo);
 }
 
 // Replace ref_seq by alt_seq at the haplotype position that still maps to v.ref_position; refuse (leaving the
@@ -47,6 +56,37 @@ bool Haplotype::apply_variants(const std::vector<Variant>& variants)
 size_t Haplotype::get_reference_position_for_haplotype_base(size_t i) const
 {
     return m_coordinate_map[i] == INSERTED_POSITION ? std::string::npos : m_coordinate_map[i];
+}
+
+Haplotype Haplotype::substr_by_reference(size_t start, size_t end) const
+{
+    if (start < m_ref_position || start > get_reference_end() || end < m_ref_position || end > get_reference_end())
+        throw Error(NPH_ERR_INVALID, "substr_by_reference: range outside the haplotype");
+    size_t s = find_derived_index_by_ref_lower_bound(start);
+    const size_t e = find_derived_index_by_ref_lower_bound(end);
+    while (s >= m_coordinate_map.size() || m_coordinate_map[s] == INSERTED_POSITION || m_coordinate_map[s] > start) {
+        if (s == 0) throw Error(NPH_ERR_INVALID, "substr_by_reference: no base at or before the start");
+        --s;
+    }
+    if (e == m_coordinate_map.size()) throw Error(NPH_ERR_INVALID, "substr_by_reference: no base at or after the end");
+    start = m_coordinate_map[s];
+    end = m_coordinate_map[e];
+    Haplotype ret(m_ref_name, start, m_reference.substr(start - m_ref_position, end - start + 1));
+    ret.m_sequence = m_sequence.substr(s, e - s + 1);
+    ret.m_coordinate_map.assign(m_coordinate_map.begin() + s, m_coordinate_map.begin() + e + 1);
+    return ret;
+}
+
+void Haplotype::get_enclosing_reference_range_for_haplotype_range(size_t& hap_lower, size_t& hap_upper, size_t& ref_lower, size_t& ref_upper) const
+{
+    while (hap_lower > 0 && m_coordinate_map[hap_lower] == INSERTED_POSITION) --hap_lower;
+    while (hap_upper < m_coordinate_map.size() && m_coordinate_map[hap_upper] == INSERTED_POSITION) ++hap_upper;
+    if (hap_lower == 0 || hap_upper >= m_coordinate_map.size()) {
+        hap_lower = hap_upper = ref_lower = ref_upper = std::string::npos;
+    } else {
+        ref_lower = m_coordinate_map[hap_lower];
+        ref_upper = m_coordinate_map[hap_upper];
+    }
 }
 
 std::vector<HMMInputSequence> generate_methylated_alternatives(const HMMInputSequence& sequence,
@@ -209,6 +249,145 @@ Variant score_variant_thresholded(const Variant& input_variant, Haplotype base_h
 {
     return score_variants_thresholded({input_variant}, base_haplotype, input, alignment_flags, score_threshold, methylation_types,
                                       Engine::thread_default())[0];
+}
+
+std::vector<HomopolymerWindow> homopolymer_windows(const Haplotype& haplotype, int region_start, int region_end, int min_flanking_sequence)
+{
+    const std::string& s = haplotype.get_sequence();
+    const size_t flank = (size_t)min_flanking_sequence, k = 6;
+    std::vector<HomopolymerWindow> out;
+    size_t i = 0;
+    while (i < s.size()) {
+        const char hp_base = s[i];
+        const size_t hap_hp_start = i;
+        while (i < s.size() && s[i] == hp_base) ++i;
+        if (i >= s.size()) break;                                           // the last run is never considered
+        const size_t hap_hp_end = i, hp_length = hap_hp_end - hap_hp_start;
+        if (hp_length < NPH_HP_MIN_LENGTH || hp_length > NPH_HP_MAX_LENGTH) continue;
+        if (hap_hp_start < flank || hap_hp_end + flank >= s.size()) continue;
+        size_t hap_calling_start = hap_hp_start - flank, hap_calling_end = hap_hp_end + flank, ref_calling_start, ref_calling_end;
+        haplotype.get_enclosing_reference_range_for_haplotype_range(hap_calling_start, hap_calling_end, ref_calling_start, ref_calling_end);
+        if (ref_calling_start == std::string::npos || ref_calling_end == std::string::npos) continue;
+        if (ref_calling_start < (size_t)region_start || ref_calling_end >= (size_t)region_end) continue;
+        if (ref_calling_start < haplotype.get_reference_position() || ref_calling_end >= haplotype.get_reference_end()) continue;
+        HomopolymerWindow w;
+        w.hp_start = hap_hp_start; w.hp_end = hap_hp_end;
+        w.calling = haplotype.substr_by_reference(ref_calling_start, ref_calling_end).get_sequence();
+        std::memset(&w.dev, 0, sizeof(w.dev));
+        w.dev.seq_len = (uint32_t)w.calling.size();
+        w.dev.ref_calling_start = (int32_t)ref_calling_start; w.dev.ref_calling_end = (int32_t)ref_calling_end;
+        w.dev.edit_offset = (uint32_t)(hap_hp_start - hap_calling_start);
+        w.dev.k0 = (uint32_t)(hap_hp_start - hap_calling_start - k + 1);
+        w.dev.hp_length = (uint32_t)hp_length; w.dev.hp_base = hp_base; w.dev.k = (uint32_t)k;
+        out.push_back(std::move(w));
+    }
+    return out;
+}
+
+HomopolymerCall homopolymer_call(const nph_hp_likelihoods& lik, size_t hp_length)
+{
+    double score_by_length[NPH_HP_MAX_LENGTH + 1] = {};
+    double max_score = -INFINITY;
+    size_t call = (size_t)-1;
+    for (size_t len = NPH_HP_MIN_LENGTH; len <= NPH_HP_MAX_LENGTH; ++len) {
+        const double score = lik.duration_lik[len - NPH_HP_MIN_LENGTH] + lik.event_lik[len - NPH_HP_MIN_LENGTH];
+        score_by_length[len] = score;
+        if (score > max_score) { max_score = score; call = len; }
+    }
+    HomopolymerCall out;
+    out.call = call;
+    out.quality = max_score - score_by_length[hp_length];
+    out.size_diff = (int)(call - hp_length);
+    out.kept = !(out.quality < 10);
+    return out;
+}
+
+Haplotype fix_homopolymers(const Haplotype& input, const HomopolymerRegion& region, int min_flanking_sequence, Engine& engine, double indel_bias,
+                           nph_hp_counts* counts_out)
+{
+    const int region_end = region.region_start + (int)region.reference.size() - 1;
+    std::vector<HomopolymerWindow> wins = homopolymer_windows(input, region.region_start, region_end, min_flanking_sequence);
+    std::string seqs;
+    std::vector<nph_hp_window> dev(wins.size());
+    for (size_t i = 0; i < wins.size(); ++i) {
+        wins[i].dev.seq_off = seqs.size();
+        seqs += wins[i].calling;
+        dev[i] = wins[i].dev;
+    }
+    // the region in screening's flat layout: per record its compact event alignment over the span of its aligned_events
+    detail::ReadTable reads;
+    std::vector<nph_meth_record> recs;
+    std::vector<int16_t> deltas;
+    std::vector<int32_t> first;
+    for (const EventAlignedRead& r : region.records) {
+        const std::vector<AlignedPair>& ae = r.aligned_events[0];
+        nph_meth_record rec;
+        std::memset(&rec, 0, sizeof(rec));
+        rec.read = reads.index(r.read, 0);
+        rec.model_id = engine.model_id(r.read->get_base_model(0));
+        rec.rc = r.rc[0] ? 1 : 0;
+        rec.ref_off = deltas.size();
+        int32_t f = 0;
+        if (!ae.empty() && r.read->has_events_for_strand(0)) {
+            rec.ref_start_pos = ae.front().ref_pos;
+            rec.ref_len = (uint32_t)(ae.back().ref_pos - ae.front().ref_pos + 1);
+            deltas.resize(deltas.size() + rec.ref_len);
+            if (!compact_event_alignment(ae, rec.ref_start_pos, rec.ref_len, deltas.data() + rec.ref_off, &f))
+                throw Error(NPH_ERR_UNSUPPORTED, "fix_homopolymers: an event alignment with a step beyond int16");
+        }
+        first.push_back(f);
+        recs.push_back(rec);
+    }
+    const detail::FlatReads fr = detail::flatten_reads(engine, reads);
+    std::vector<double> time(std::max<size_t>(fr.n_events, 1));
+    std::vector<float> duration(std::max<size_t>(fr.n_events, 1));
+    for (size_t i = 0; i < reads.size(); ++i) {
+        const std::vector<SquiggleEvent>& ev = reads.reads()[i].first->events[reads.reads()[i].second];
+        for (size_t e = 0; e < ev.size(); ++e) { time[fr.reads[i].event_off + e] = ev[e].start_time; duration[fr.reads[i].event_off + e] = ev[e].duration; }
+    }
+    nph_hp_params params;
+    std::memset(&params, 0, sizeof(params));
+    params.region_start = region.region_start;
+    params.min_flanking_sequence = min_flanking_sequence;
+    std::vector<nph_hp_likelihoods> lik(std::max<size_t>(wins.size(), 1));
+    nph_hp_counts counts;
+    engine.check(nph_homopolymer_likelihoods_batch(engine.ctx(), fr.reads.data(), fr.reads.size(), fr.mean, time.data(), duration.data(), fr.n_events,
+                                                   region.reference.data(), region.reference.size(), deltas.data(), deltas.size(), first.data(),
+                                                   recs.data(), recs.size(), &params, seqs.data(), seqs.size(), dev.data(), dev.size(), indel_bias,
+                                                   lik.data(), &counts),
+                 "nph_homopolymer_likelihoods_batch");
+    if (counts_out) *counts_out = counts;
+
+    Haplotype fixed = input;
+    for (size_t wi = 0; wi < wins.size(); ++wi) {
+        const HomopolymerWindow& w = wins[wi];
+        const nph_hp_likelihoods& L = lik[wi];
+        const char hp_base = w.dev.hp_base;
+        const HomopolymerCall hc = homopolymer_call(L, w.dev.hp_length);
+        if (!hc.kept) continue;
+        const int size_diff = hc.size_diff;
+        const double score = hc.quality;
+        Variant v;
+        v.ref_name = fixed.get_reference_name();
+        v.add_info("TotalReads", (size_t)L.total_reads);
+        v.add_info("AlleleCount", 1);
+        for (size_t k = w.hp_start; k <= w.hp_end && size_diff != 0; ++k) {
+            v.ref_position = input.get_reference_position_for_haplotype_base(k);
+            if (v.ref_position == std::string::npos) continue;
+            if (size_diff > 0) {
+                v.ref_seq = fixed.substr_by_reference(v.ref_position, v.ref_position).get_sequence();
+                if (v.ref_seq.size() != 1 || v.ref_seq[0] != hp_base) continue;
+                v.alt_seq = v.ref_seq + hp_base;
+            } else {
+                v.ref_seq = fixed.substr_by_reference(v.ref_position, v.ref_position + 1).get_sequence();
+                if (v.ref_seq.size() != 2 || v.ref_seq[0] != hp_base || v.ref_seq[1] != hp_base) continue;
+                v.alt_seq = v.ref_seq.substr(0, 1);
+            }
+            v.quality = score;
+            if (fixed.apply_variant(v)) break;
+        }
+    }
+    return fixed;
 }
 
 } // namespace nph

@@ -6,6 +6,8 @@
 //   generate_methylated_alternatives             ref: src/common/nanopolish_variant.cpp:158-178
 //   score_variant_thresholded                    ref: src/common/nanopolish_variant.cpp:765-799
 //   the scoring loop of score_variant_group      ref: src/common/nanopolish_variant.cpp:242-258
+//   fix_homopolymers                             ref: src/nanopolish_call_variants.cpp:541-780 (its likelihoods on the device,
+//                                                nph_homopolymer_likelihoods_batch)
 //
 // The reference scores one (read, sequence) pair per profile_hmm_score call inside an OpenMP loop.  Here every
 // (read, haplotype, alphabet alternative) triple of a whole candidate set becomes one job of ONE launch; the base
@@ -14,6 +16,7 @@
 // in read order) is applied afterwards, unchanged.
 #pragma once
 #include "nph_host.hpp"
+#include "nph_methylation.hpp"
 
 namespace nph {
 
@@ -25,6 +28,12 @@ struct Variant {
     double quality = 0.0;
     std::string info, genotype, filter;
     std::string key() const { return ref_name + ":" + std::to_string(ref_position) + ":" + ref_seq + ":" + alt_seq; }
+    // Variant::add_info (ref: src/common/nanopolish_variant.h:82-92): key=value, ';'-separated
+    template <typename T> void add_info(const std::string& k, T value)
+    {
+        const std::string kv = k + "=" + std::to_string(value);
+        info = info.empty() ? kv : info + ";" + kv;
+    }
 };
 
 class Haplotype {
@@ -38,6 +47,16 @@ public:
     size_t get_reference_position() const { return m_ref_position; }
     size_t get_reference_position_for_haplotype_base(size_t i) const;
     const std::vector<Variant>& get_variants() const { return m_variants; }
+    const std::string& get_reference_name() const { return m_ref_name; }
+    size_t get_reference_end() const { return m_ref_position + m_reference.length(); }
+    // the reference positions of the haplotype's bases (INSERTED_POSITION for an inserted base)
+    const std::vector<size_t>& coordinate_map() const { return m_coordinate_map; }
+    // the haplotype over reference [start, end] (ref: src/nanopolish_haplotype.cpp:88-140): its first base is the last one at or
+    // before start that has a reference position; throws Error(NPH_ERR_INVALID) where the reference asserts
+    Haplotype substr_by_reference(size_t start, size_t end) const;
+    // ref: src/nanopolish_haplotype.cpp:141-158.  Moves hap_lower down and hap_upper up over inserted bases and returns their
+    // reference positions; all four npos when hap_lower reaches 0 or hap_upper the end
+    void get_enclosing_reference_range_for_haplotype_range(size_t& hap_lower, size_t& hap_upper, size_t& ref_lower, size_t& ref_upper) const;
 
 private:
     size_t find_derived_index_by_ref_lower_bound(size_t ref_index) const;
@@ -87,5 +106,36 @@ std::vector<Variant> score_variants_thresholded(const std::vector<Variant>& inpu
 // the reference's single-candidate signature
 Variant score_variant_thresholded(const Variant& input_variant, Haplotype base_haplotype, const std::vector<HMMInputData>& input,
                                   uint32_t alignment_flags, uint32_t score_threshold, const std::vector<std::string>& methylation_types);
+
+// The AlignmentDB fix_homopolymers reads: the region [region_start, region_start + reference.size() - 1] of one contig and its event
+// alignment records in AlignmentDB's order, each strand 0 of its read (read->events[0] with durations; rc[0], aligned_events[0]).
+struct HomopolymerRegion {
+    std::string contig;
+    int region_start = 0;
+    std::string reference;
+    std::vector<EventAlignedRead> records;
+};
+
+// One homopolymer fix_homopolymers scores, in scan order: the run, its calling window and the nph_hp_window it becomes.
+struct HomopolymerWindow {
+    size_t hp_start, hp_end;        // [hp_start, hp_end) in the input haplotype
+    std::string calling;            // substr_by_reference(ref_calling_start, ref_calling_end)
+    nph_hp_window dev;
+};
+// the scan of :552-616: every run of 3..9 bases (the last run never) that passes the flank, enclosing-range and region tests
+std::vector<HomopolymerWindow> homopolymer_windows(const Haplotype& haplotype, int region_start, int region_end, int min_flanking_sequence);
+
+// The call of one window (ref: src/nanopolish_call_variants.cpp:686-727): the first strict maximum of d_lik + e_lik from -inf (call
+// stays npos when nothing beats it), quality = max - score[hp_length], kept unless quality < 10 (a NaN is kept), and
+// size_diff = int(call - hp_length) (npos: a deletion).
+struct HomopolymerCall { size_t call; double quality; int size_diff; bool kept; };
+HomopolymerCall homopolymer_call(const nph_hp_likelihoods& lik, size_t hp_length);
+
+// fix_homopolymers (ref: src/nanopolish_call_variants.cpp:541-780): the scan and its skip tests here, every window's likelihood
+// vectors in one nph_homopolymer_likelihoods_batch, then the call (strict argmax from -inf, quality max - score[hp_length], kept
+// unless < 10) and its 1-base insertion or deletion, tried at each base of the run until apply_variant accepts one, window by
+// window.  counts_out (optional): the device call's counters.
+Haplotype fix_homopolymers(const Haplotype& input, const HomopolymerRegion& region, int min_flanking_sequence, Engine& engine,
+                           double indel_bias = hmm_indel_bias_factor, nph_hp_counts* counts_out = nullptr);
 
 } // namespace nph

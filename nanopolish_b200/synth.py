@@ -729,6 +729,132 @@ def gen_pileup(ref_len: int, depth: int, read_bases: int, model: PoreModel, seed
     return ref, rs, recs, np.concatenate(prs)
 
 
+# ---- variants --fix-homopolymers (nph_homopolymer_likelihoods_batch) -------------------------------------------------------
+HP_PARAMS_DT = np.dtype([("region_start", "<i4"), ("min_flanking_sequence", "<i4"), ("max_chunk_pairs", "<u4"), ("reserved", "<u4")], align=True)
+HP_WINDOW_DT = np.dtype([("seq_off", "<u8"), ("seq_len", "<u4"), ("ref_calling_start", "<i4"), ("ref_calling_end", "<i4"), ("edit_offset", "<u4"),
+                         ("k0", "<u4"), ("hp_length", "<u4"), ("hp_base", "S1"), ("reserved", "u1", 3), ("k", "<u4")], align=True)
+HP_LIK_DT = np.dtype([("total_reads", "<u4"), ("scored_reads", "<u4"), ("event_lik", "<f8", 7), ("duration_lik", "<f8", 7)], align=True)
+HP_COUNTS_DT = np.dtype([("n_windows", "<u8"), ("n_pairs", "<u8"), ("n_jobs", "<u8"), ("n_dp_rows", "<u8"), ("n_chunks", "<u4"), ("reserved", "<u4"),
+                         ("host_ms", "<f8")], align=True)
+assert HP_PARAMS_DT.itemsize == 16 and HP_WINDOW_DT.itemsize == 40 and HP_LIK_DT.itemsize == 120 and HP_COUNTS_DT.itemsize == 48
+
+
+def gen_durations(rs: ReadSet, seed: int = 0, rate: float = 587.2858):
+    """per event a float duration: each k-mer's dwell drawn from the reference's gamma duration model (shape 2.461964, rate
+    DurationModel::log_gamma_sum's 587.2858 per second), split evenly over its events; the start times follow the durations"""
+    rng = np.random.default_rng(seed)
+    dur = np.zeros(rs.total_events, np.float32)
+    times = rs.ev_start_time.copy()
+    for r in range(rs.n_reads):
+        off, n = int(rs.reads[r]["event_off"]), int(rs.reads[r]["n_events"])
+        which = rs.ev_kmer[r]
+        nk = int(which.max()) + 1 if n else 0
+        dwell = rng.gamma(2.461964, 1.0 / rate, nk)
+        cnt = np.bincount(which, minlength=nk)
+        d = (dwell[which] / np.maximum(cnt[which], 1)).astype(np.float32)
+        dur[off:off + n] = d
+        times[off:off + n] = times[off] + np.concatenate([[0.0], np.cumsum(d[:-1].astype(np.float64))])
+    return dur, times
+
+
+def gen_hp_pileup(ref_len: int, depth: int, read_bases: int, model: PoreModel, seed: int = 42, region_start: int = 5000, n_hp_errors: int = 4,
+                  rc_every: int = 2, margin: int = 40, long_runs: int = 0, plant=()):
+    """A draft reference and reads sampled from a TRUTH that differs from it by homopolymer-length indels: n_hp_errors runs of 3..8
+    equal draft bases (at least `margin` bases from either end) each get one base more or one less in the truth.  Each read's
+    aligned_events map its truth positions through those indels onto the draft (an inserted truth base has no pair, a deleted draft
+    base none either), built like gen_pileup's.  Event durations follow the reference's gamma duration model (gen_durations), and the
+    start times follow the durations.  Returns (draft codes u1, ReadSet, records METH_RECORD_DT, pairs PAIR_DT, durations f4,
+    edits [(draft index of the run's first base, run length, +1 / -1)]).  long_runs: that many runs of 6..8 bases are planted in the
+    draft first, evenly spaced, and take the first edits (in long runs the k-mers of L and L + 1 bases barely differ, so the
+    duration term decides more calls).  plant: (draft index, length) runs written into the draft after those, each bounded by other
+    bases and never edited (crafted edges of the homopolymer scan)."""
+    rng = np.random.default_rng(seed)
+    k = model.k
+    ref = rng.integers(0, 4, ref_len, dtype=np.uint8)
+    planted = []
+    for q in range(long_runs):
+        at, n = margin + (q + 1) * (ref_len - 2 * margin) // (long_runs + 1), int(rng.integers(6, 9))
+        b = int(rng.integers(4))
+        ref[at:at + n] = b
+        ref[at - 1] = (b + 1) % 4; ref[at + n] = (b + 2) % 4
+        planted.append((at, n))
+    for at, n in plant:
+        b = int(ref[at])
+        ref[at:at + n] = b
+        if at > 0:
+            ref[at - 1] = (b + 1) % 4
+        if at + n < ref_len:
+            ref[at + n] = (b + 2) % 4
+    fixed_runs = set(plant)
+    runs, i = [], 0
+    while i < ref_len:
+        j = i
+        while j < ref_len and ref[j] == ref[i]:
+            j += 1
+        if 3 <= j - i <= 8 and i >= margin and j + margin <= ref_len and (i, j - i) not in fixed_runs:
+            runs.append((i, j - i))
+        i = j
+    first = [j for j, r in enumerate(runs) if r in planted]
+    rest = [j for j in range(len(runs)) if runs[j] not in planted]
+    pick = first[:n_hp_errors]
+    if len(pick) < n_hp_errors and rest:
+        pick += list(rng.choice(rest, min(n_hp_errors - len(pick), len(rest)), replace=False))
+    pick = sorted(int(j) for j in pick)
+    edits = [(runs[p][0], runs[p][1], 1 if (e % 2 == 0) else -1) for e, p in enumerate(pick)]
+    truth, t2d, last = [], [], 0
+    for start, length, d in edits:
+        truth += list(ref[last:start]); t2d += list(range(last, start))
+        if d > 0:
+            truth += [ref[start]] * (length + 1); t2d += [-1] + list(range(start, start + length))
+        else:
+            truth += [ref[start]] * (length - 1); t2d += list(range(start + 1, start + length))
+        last = start + length
+    truth += list(ref[last:]); t2d += list(range(last, ref_len))
+    truth = np.array(truth, np.uint8); t2d = np.array(t2d, np.int64)
+    n_reads = max(1, int(round(depth * truth.shape[0] / read_bases)))
+    starts = np.sort(rng.integers(0, truth.shape[0] - read_bases + 1, n_reads))
+    reads = np.zeros(n_reads, READ_DT)
+    recs = np.zeros(n_reads, METH_RECORD_DT)
+    means, times, seqs, evk, kfe, prs = [], [], [], [], [], []
+    p_nev = np.array([0.03, 0.35, 0.45, 0.17])
+    eoff = doff = poff = 0
+    for r in range(n_reads):
+        rr = np.random.default_rng(seed * 7919 + r)
+        s0 = int(starts[r])
+        seg = truth[s0:s0 + read_bases]
+        rc = 1 if (rc_every and r % rc_every == rc_every - 1) else 0
+        codes = (3 - seg[::-1]).astype(np.uint8) if rc else seg.copy()
+        nk = codes.shape[0] - k + 1
+        ranks = kmer_ranks_from_codes(codes, k, 4)
+        nev = rr.choice(4, nk, p=p_nev)
+        nev[0] = max(nev[0], 1); nev[-1] = max(nev[-1], 1)
+        which = np.repeat(np.arange(nk, dtype=np.int32), nev)
+        E = which.shape[0]
+        shift, scale, var = rr.uniform(-5.0, 5.0), rr.uniform(0.9, 1.1), rr.uniform(0.9, 1.3)
+        t = np.arange(E, dtype=np.float64) * 0.002 + rr.uniform(0.0, 100.0)
+        m = (scale * model.level_mean[ranks[which]] + shift + var * model.level_stdv[ranks[which]] * rr.standard_normal(E)).astype(np.float32)
+        reads[r] = (eoff, E, 0, scale, shift, 0.0, var, np.log(var), E / float(nk))
+        _, _, closest = closest_event_map(which, nk)
+        q = np.arange(k, read_bases - k)
+        q = q[q < nk]
+        ev = closest[read_bases - q - k] if rc else closest[q]
+        dpos = t2d[s0 + q]
+        keep = dpos >= 0
+        pr = np.zeros(int(keep.sum()), PAIR_DT)
+        pr["ref_pos"], pr["read_pos"] = region_start + dpos[keep], ev[keep]
+        if pr.shape[0] and pr["read_pos"][0] == pr["read_pos"][-1]:
+            pr = pr[:0]
+        d_lo = int(dpos[keep][0]) if pr.shape[0] else 0
+        d_len = int(dpos[keep][-1]) - d_lo + 1 if pr.shape[0] else 1
+        recs[r] = (doff, poff, r, 0, d_len, pr.shape[0], region_start + d_lo, rc, 0, (0, 0))
+        means.append(m); times.append(t); seqs.append(codes); evk.append(which)
+        kfe.append(np.searchsorted(which, np.arange(nk), side="left").astype(np.int32)); prs.append(pr)
+        eoff += E; doff += d_len; poff += pr.shape[0]
+    rs = ReadSet(reads, np.concatenate(means), np.concatenate(times), seqs, evk, kfe, k)
+    dur, rs.ev_start_time = gen_durations(rs, seed)
+    return ref, rs, recs, np.concatenate(prs), dur, edits
+
+
 # ---- methylation-aware screening (`variants -q cpg`, `-q dam,dcm`) -------------------------------------------------------
 SCREEN_METH_DT = np.dtype([("n_types", "<u4"), ("reserved", "<u4"), ("alphabets", METH_PARAMS_DT, 4)], align=True)
 assert SCREEN_METH_DT.itemsize == 616
