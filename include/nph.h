@@ -900,7 +900,8 @@ typedef struct {
     uint32_t n_chunks;                /* chunks of Viterbi states */
     uint32_t reserved;
     double   host_ms;                 /* the host's log-gamma terms and fold.  nph_last_kernel_ms after the call: the forward kernels,
-                                         K3 and the duration kernel of every chunk (not the pair, scan, emit or scheduling kernels) */
+                                         the state-offset kernel, K3 and the duration kernel of every chunk (not the pair, scan, emit
+                                         or scheduling kernels) */
 } nph_hp_counts;                      /* 48 bytes */
 int nph_homopolymer_likelihoods_batch(nph_ctx* ctx, const nph_read* reads, size_t n_reads,
                                       const float* ev_mean, const double* ev_start_time, const float* ev_duration, size_t n_events_total,
@@ -910,6 +911,57 @@ int nph_homopolymer_likelihoods_batch(nph_ctx* ctx, const nph_read* reads, size_
                                       const nph_hp_params* params, const char* calling_seqs, size_t n_seq_bytes,
                                       const nph_hp_window* windows, size_t n_windows, double indel_bias,
                                       nph_hp_likelihoods* out, nph_hp_counts* counts_out);
+
+/* ---- scorereads --train-transitions: forward scores and transition training counts of a job batch ----------------------------
+ * `nanopolish scorereads --train-transitions` runs, for every segment model_score scores (src/nanopolish_scorereads.cpp:116-203),
+ * profile_hmm_align(sequence, data) (K3, flags 0) after the forward score, and folds the path into
+ * TransitionParameters::add_training_from_alignment (src/hmm/nanopolish_transition_parameters.cpp:294-368) of the segment's strand.
+ * This call takes the batch of nph_hmm_score_batch_seq (reads, events, base codes, jobs) and returns both halves:
+ *   scores_out[j]        == what nph_hmm_score_batch_seq gives for job j (K1, the same scheduler and kernels)
+ *   counts_out[g]        the training counts of the jobs whose group (groups[j], NULL: all 0) is g, g < n_groups
+ * Per job, over its path p of n states (nothing when n <= ignore_edge_length), prev_s = 'M', kmer_move = i == 0 ||
+ * p[i-1].kmer_idx != p[i].kmer_idx:
+ *   state_transitions[prev_s][2 * s + kmer_move] += 1 for every state, and once more for 5 < i < n - 5 (ignore_edge_length 5)
+ *   in that interior, a state s != 'B' is one skip observation between k-mers from = p[i-1].kmer_idx and to = p[i].kmer_idx
+ *   (to = from + 1 for 'K' after 'M'): the bin b = min(29, (size_t)(|l1 - l2| / 0.5)) of the two scaled means
+ *   l = float(scale * level_mean[rank] + shift) (get_scaled_gaussian_from_pore_model_state) gets skip_total[b] += 1 and
+ *   skip_count[b] += (s == 'K')
+ *   n_matches += s == 'M', n_skips += s == 'K' (n_merges stays 0: an R9 path has no 'E' state)
+ * Every count is an integer sum, so the records do not depend on the order the device visits the states in.  The reference counts
+ * in uint32_t and this call in uint64_t: the two differ once a count passes 2^32.  TransitionParameters::train() needs, per bin,
+ * exactly skip_count and skip_total (its observations add is_skip and 1 to the bin's doubles), so the records carry everything the
+ * reference's observation vector does.
+ * NPH_ERR_INVALID: a group >= n_groups, n_groups outside 1..256; a job nph_hmm_score_batch_seq refuses; and where the reference
+ * asserts: a job profile_hmm_align finds no path for, a skip observation with to >= n_kmers, a state other than M, B, K; and a
+ * skip observation whose scaled mean is not finite (the reference's bin is then undefined).  One more difference: the
+ * reference's (size_t) of |l1 - l2| / 0.5 >= 2^64 (means beyond 2^62 pA) wraps to bin 0, this call clamps it to bin 29.
+ * The Viterbi states stay on the device, in consecutive chunks of jobs under 1 GiB ((E_max + K_max) x 16 bytes per job), at most
+ * max_chunk_jobs jobs each (0: no cap).  nph_last_kernel_ms after the call: the forward kernels, and K3, the state-offset kernel
+ * and the observation kernel of every chunk (not the scheduler or the uploads); params->viterbi_ms_out and observe_ms_out split the
+ * chunks' share. */
+#define NPH_TT_BINS 30
+#define NPH_TT_MAX_GROUPS 256
+typedef struct {
+    uint64_t state_transitions[3][6]; /* rows M, B, K (from); column 2 * to + kmer_move */
+    uint64_t n_matches, n_merges, n_skips;
+    uint64_t skip_total[NPH_TT_BINS]; /* skip observations per bin of |l1 - l2| (width 0.5, the last bin open) */
+    uint64_t skip_count[NPH_TT_BINS]; /* of those, the ones whose state is 'K' */
+} nph_transition_counts;              /* 648 bytes */
+typedef struct {
+    uint32_t n_groups;                /* counts records written: 2 (NUM_STRANDS) for scorereads */
+    uint32_t ignore_edge_length;      /* add_training_from_alignment's default: 5 */
+    uint32_t max_chunk_jobs;          /* jobs per chunk of Viterbi states: 0 = as many as fit the 1 GiB budget */
+    uint32_t n_chunks_out;            /* written by the call: the chunks it ran */
+    float    viterbi_ms_out;          /* written by the call: device ms of K3 and its state-offset kernel over all chunks */
+    float    observe_ms_out;          /* written by the call: device ms of the observation kernel over all chunks */
+} nph_tt_params;                      /* 24 bytes */
+int nph_train_transitions_batch(nph_ctx* ctx,
+                                const nph_read* reads, size_t n_reads,
+                                const float* ev_mean, const double* ev_start_time, size_t n_events_total,
+                                const uint8_t* seq_codes, size_t n_codes_total,
+                                const nph_hmm_job* jobs, size_t n_jobs, const uint8_t* groups,
+                                nph_tt_params* params, double indel_bias,
+                                float* scores_out, nph_transition_counts* counts_out);
 
 /* ---- measurement hooks (used by bench.py; not part of the reference surface) ------------- */
 /* Device time in ms of the most recent nph_hmm_score / nph_abea_run kernel sequence, measured

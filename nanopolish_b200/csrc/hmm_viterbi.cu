@@ -153,14 +153,64 @@ int vit_max_ctas(nph_ctx* ctx, size_t trace_stride, int& max_ctas)
     return NPH_OK;
 }
 
+// off[i] = i * stride, i = 0 .. n
+__global__ void states_off_kernel(uint64_t* __restrict__ off, uint64_t n, uint64_t stride)
+{
+    const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+    if (i <= n) off[i] = i * stride;
+}
+
+// device memory for the Viterbi states of one chunk of nph_viterbi_chunks (16 B per state, max_K + max_E states per job)
+constexpr uint64_t kStatesBudget = 1ull << 30;
+
 } // namespace
 
+int nph_viterbi_chunks(nph_ctx* ctx, DevBuf<uint8_t>& buf, uint64_t n_jobs, uint64_t max_chunk, uint64_t unit, uint32_t max_K, uint32_t max_E,
+                       const std::function<int(uint64_t j0, uint64_t nj, uint64_t& first)>& prepare,
+                       const std::function<int(const NphVitChunk&)>& fold, float* ms, int* launches, uint32_t* n_chunks,
+                       float* fold_ms)
+{
+    const uint64_t stride = (uint64_t)max_K + max_E;
+    uint64_t chunk = std::min<uint64_t>(max_chunk ? max_chunk : UINT64_MAX, kStatesBudget / (sizeof(nph_align_state) * stride));
+    chunk = std::max<uint64_t>(unit, chunk / unit * unit);
+    cudaStream_t st = ctx->stream;
+    *ms = 0.f; *launches = 0; *n_chunks = 0;
+    if (fold_ms) *fold_ms = 0.f;
+    for (uint64_t j0 = 0; j0 < n_jobs; j0 += chunk) {
+        const uint64_t nj = std::min(chunk, n_jobs - j0);
+        uint64_t* d_off; uint32_t* d_n; nph_align_state* d_states;
+        NPH_TRY(nph_carve(ctx, buf, [&](NphArena& c) {
+            d_off = c.take<uint64_t>(nj + 1);
+            d_n = c.take<uint32_t>(nj);
+            d_states = c.take<nph_align_state>(nj * stride);
+        }));
+        uint64_t first = 0;
+        NPH_TRY(prepare(j0, nj, first));
+        NPH_CUDA(ctx, cudaEventRecord(ctx->ev0, st));
+        states_off_kernel<<<(unsigned)((nj + 1 + 255) / 256), 256, 0, st>>>(d_off, nj, stride);
+        NPH_CUDA(ctx, cudaGetLastError());
+        NPH_TRY(nph_viterbi_device_jobs(ctx, (size_t)nj, max_K, max_E, d_off, d_states, d_n, (size_t)first));
+        NPH_CUDA(ctx, cudaEventRecord(ctx->ev_mid, st));
+        NPH_TRY(fold(NphVitChunk{j0, nj, d_states, d_off, d_n}));
+        NPH_CUDA(ctx, cudaEventRecord(ctx->ev1, st));
+        NPH_CUDA(ctx, cudaEventSynchronize(ctx->ev1));
+        float t = 0.f, f = 0.f;
+        NPH_CUDA(ctx, cudaEventElapsedTime(&t, ctx->ev0, ctx->ev1));
+        NPH_CUDA(ctx, cudaEventElapsedTime(&f, ctx->ev_mid, ctx->ev1));
+        *ms += t; *launches += 3; *n_chunks += 1;
+        if (fold_ms) *fold_ms += f;
+    }
+    return NPH_OK;
+}
+
 int nph_viterbi_device_jobs(nph_ctx* ctx, size_t n_jobs, uint32_t max_K, uint32_t max_E, const uint64_t* d_states_off,
-                            nph_align_state* d_states, uint32_t* d_n_states)
+                            nph_align_state* d_states, uint32_t* d_n_states, size_t first_job)
 {
     if (n_jobs == 0) return NPH_OK;
-    // one class for the whole batch, chosen for its largest job: the jobs a caller emits here come from windows of one shape
-    // (homopolymer calling windows), so the class a per-job choice would make differs little, and no job needs a host pass
+    // one class for the whole batch, chosen for its largest job, and no host pass over the jobs.  Homopolymer calling windows all
+    // have one shape, so a per-job choice would differ little there; scorereads segments of 500 events vary in K (a long deletion
+    // makes one segment's sequence longer), and one outlier then sets the class, the trace size and, in nph_viterbi_chunks, the
+    // state stride of every job of the chunk (a cost not measured: the benchmark's segments are uniform)
     nph_wave_geom geo{};
     uint32_t steps = 0;
     const int ci = vit_class(max_K, max_E, geo, steps);
@@ -176,7 +226,7 @@ int nph_viterbi_device_jobs(nph_ctx* ctx, size_t n_jobs, uint32_t max_K, uint32_
     }));
     p.states_off = d_states_off; p.states = d_states; p.n_states = d_n_states; p.scores = nullptr;
     p.level = ctx->d_level.p; p.reads = ctx->d_reads.p; p.trans = ctx->d_trans.p; p.models = ctx->d_models.p;
-    p.ranks = ctx->d_ranks.p; p.jobs = ctx->d_jobs.p; p.flank = ctx->d_flank.p;
+    p.ranks = ctx->d_ranks.p; p.jobs = ctx->d_jobs.p + first_job; p.flank = ctx->d_flank.p;
     p.kpad_stride = kpad; p.edge_stride = nph_edge_stride(period); p.trace_stride = trace_stride; p.c = ctx->consts;
     NPH_CUDA(ctx, cudaMemsetAsync(ctx->d_counters.p, 0, sizeof(unsigned int), ctx->stream));
     return launch_vit_class(ctx, kVitCols[ci], p, nullptr, n_jobs, ctx->d_counters.p, max_ctas);

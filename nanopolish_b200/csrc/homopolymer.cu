@@ -17,7 +17,7 @@
 //   hp_pairs_kernel<true>   the same walk, writing the scored pairs {record, e1, e2} in record order
 //   hp_emit_kernel          thread per (pair, L) of a chunk: the k-mer ranks of the variant sequence, strand-resolved, and ONE
 //                           nph_hmm_job — the forward and the Viterbi call of the reference are the same triple
-//   K1 (nph_score_device_jobs), then K3 on the same jobs (nph_viterbi_device_jobs)
+//   K1 (nph_score_device_jobs), then K3 on the same jobs (nph_viterbi_chunks, which runs the emit and K1 per chunk)
 //   hp_duration_kernel      a warp per job: sum_duration over the path, slot by slot in path order, slots ascending
 // The log-gamma terms and the fold in record order run on the host with the host's libm (DESIGN: glibc's double log and
 // lgamma are not correctly rounded, and unlike expf / logf in libm_exact.cuh they cannot be checked exhaustively).
@@ -37,9 +37,6 @@ constexpr int kL = NPH_HP_LENGTHS;
 constexpr int kMinEvents = 10;                       // abs(e_start - e_stop) < 10 skips the read (:637)
 constexpr double kShape = 2.461964;                  // GammaParameters::shape (:643)
 constexpr double kMinDuration = 0.00025;             // MIN_DURATION, src/hmm/nanopolish_duration_model.h:17
-// device memory for the Viterbi states of one chunk of jobs (16 B per state, E + K states per job); the descriptors run in
-// consecutive chunks under it
-constexpr uint64_t kStatesBudget = 1ull << 30;
 
 struct HpPair { uint32_t record; int32_t e1, e2; };
 
@@ -102,10 +99,9 @@ __global__ void __launch_bounds__(kThreads) hp_pairs_kernel(const HpArgs a, uint
     }
 }
 
-// thread per (pair, L) of the chunk [p0, p0 + n_pairs): job p * 7 + (L - 3), ranks at kmer_stride per job, states at states_stride
+// thread per (pair, L) of the chunk [p0, p0 + n_pairs): job p * 7 + (L - 3), ranks at kmer_stride per job
 __global__ void hp_emit_kernel(const HpArgs a, const HpPair* __restrict__ pairs, const uint32_t* __restrict__ pair_window, uint64_t p0,
-                               uint64_t n_pairs, uint32_t kmer_stride, uint64_t states_stride, nph_hmm_job* __restrict__ jobs,
-                               uint32_t* __restrict__ ranks, uint64_t* __restrict__ states_off)
+                               uint64_t n_pairs, uint32_t kmer_stride, nph_hmm_job* __restrict__ jobs, uint32_t* __restrict__ ranks)
 {
     const uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
     if (t >= n_pairs * kL) return;
@@ -132,8 +128,6 @@ __global__ void hp_emit_kernel(const HpArgs a, const HpPair* __restrict__ pairs,
     jb.stride = R.rc ? -1 : 1;                    // EventAlignmentRecord::stride agrees with rc for every read the HMM accepts
     jb.rc = R.rc; jb.flags = 0; jb.reserved = 0;  // alignment_flags = 0 (:543)
     jobs[t] = jb;
-    states_off[t] = t * states_stride;
-    if (t + 1 == n_pairs * kL) states_off[t + 1] = (t + 1) * states_stride;
 }
 
 // a warp per job: slots k0 + 2 .. k0 + L + 1 of generate_aligned_durations (each the durations of the path's non-K states of that
@@ -283,45 +277,39 @@ extern "C" int nph_homopolymer_likelihoods_batch(nph_ctx* ctx, const nph_read* r
         NPH_CUDA(ctx, cudaMemcpyAsync(d_pair_window, pair_window.data(), sizeof(uint32_t) * n_pairs, cudaMemcpyHostToDevice, st));
         hp_pairs_kernel<true><<<grid, kThreads, 0, st>>>(a, nullptr, nullptr, nullptr, d_off, d_pairs);
         NPH_CUDA(ctx, cudaGetLastError());
-        // chunks of whole pairs whose states fit kStatesBudget; every job gets room for the batch's largest path
+        // chunks of whole pairs (kL jobs each) whose states fit the budget; every job gets room for the batch's largest path
         const uint32_t kmer_stride = max_len - 6 + 1;
-        const uint64_t states_stride = (uint64_t)max_e + kmer_stride;
-        const uint64_t chunk_pairs = std::max<uint64_t>(1, std::min<uint64_t>(params->max_chunk_pairs ? params->max_chunk_pairs : UINT64_MAX,
-                                                                              kStatesBudget / (sizeof(nph_align_state) * states_stride * kL)));
-        // what nph_last_kernel_ms reports: the forward kernels (timed inside nph_score_device_jobs), K3 and the duration kernel of
-        // every chunk; the pair kernels, the scan, the emit kernel and the forward scheduler run outside those windows (in the
+        // what nph_last_kernel_ms reports: the forward kernels (timed inside nph_score_device_jobs), the state-offset kernel, K3 and
+        // the duration kernel of every chunk; the pair kernels, the scan, the emit kernel and the forward scheduler run outside those windows (in the
         // whole-call time only).  launches counts every launch of the call.
-        float kernel_ms = 0.f;
-        int launches = 6;
-        for (uint64_t p0 = 0; p0 < n_pairs; p0 += chunk_pairs) {
-            const uint64_t np = std::min(chunk_pairs, n_pairs - p0), nj = np * kL;
-            NPH_TRY(nph_reserve(ctx, ctx->d_ranks, (size_t)(nj * kmer_stride)));
-            uint64_t* d_states_off; uint32_t* d_n_states; nph_align_state* d_states;
-            NPH_TRY(nph_carve(ctx, hs.d_states, [&](NphArena& c) {
-                d_states_off = c.take<uint64_t>(nj + 1);
-                d_n_states = c.take<uint32_t>(nj);
-                d_states = c.take<nph_align_state>(nj * states_stride);
-            }));
-            NPH_TRY(nph_score_device_jobs(ctx, (size_t)nj, (size_t)(nj * kmer_stride), indel_bias, [&]() -> int {
-                hp_emit_kernel<<<(unsigned)((nj + 127) / 128), 128, 0, st>>>(a, d_pairs, d_pair_window, p0, np, kmer_stride, states_stride,
-                                                                               ctx->d_jobs.p, ctx->d_ranks.p, d_states_off);
+        float kernel_ms = 0.f, vit_ms = 0.f;
+        int launches = 6, vit_launches = 0;
+        NPH_TRY(nph_viterbi_chunks(ctx, hs.d_states, n_jobs, (uint64_t)params->max_chunk_pairs * kL, kL, kmer_stride, max_e,
+            [&](uint64_t j0, uint64_t nj, uint64_t& first) -> int {
+                const uint64_t p0 = j0 / kL, np = nj / kL;
+                NPH_TRY(nph_reserve(ctx, ctx->d_ranks, (size_t)(nj * kmer_stride)));
+                NPH_TRY(nph_score_device_jobs(ctx, (size_t)nj, (size_t)(nj * kmer_stride), indel_bias, [&]() -> int {
+                    hp_emit_kernel<<<(unsigned)((nj + 127) / 128), 128, 0, st>>>(a, d_pairs, d_pair_window, p0, np, kmer_stride,
+                                                                                   ctx->d_jobs.p, ctx->d_ranks.p);
+                    NPH_CUDA(ctx, cudaGetLastError());
+                    return NPH_OK;
+                }));
+                float ms = 0.f; int nl = 0;
+                if (nph_last_kernel_ms(ctx, &ms, &nl) == NPH_OK) { kernel_ms += ms; launches += nl + 1; }
+                NPH_CUDA(ctx, cudaMemcpyAsync(d_fwd + j0, ctx->d_scores.p, sizeof(float) * nj, cudaMemcpyDeviceToDevice, st));
+                first = 0;                                // each chunk's jobs are emitted from index 0
+                return NPH_OK;
+            },
+            [&](const NphVitChunk& c) -> int {
+                hp_duration_kernel<<<(unsigned)((c.n + kWarps - 1) / kWarps), kThreads, 0, st>>>(a, d_pairs, d_pair_window, c.j0 / kL, c.n, c.states,
+                                                                                               c.states_off, c.n_states, ctx->d_reads.p, d_dur,
+                                                                                               d_sum, d_flags + 1);
                 NPH_CUDA(ctx, cudaGetLastError());
                 return NPH_OK;
-            }));
-            float ms = 0.f; int nl = 0;
-            if (nph_last_kernel_ms(ctx, &ms, &nl) == NPH_OK) { kernel_ms += ms; launches += nl + 1; }
-            NPH_CUDA(ctx, cudaMemcpyAsync(d_fwd + p0 * kL, ctx->d_scores.p, sizeof(float) * nj, cudaMemcpyDeviceToDevice, st));
-            NPH_CUDA(ctx, cudaEventRecord(ctx->ev0, st));
-            NPH_TRY(nph_viterbi_device_jobs(ctx, (size_t)nj, kmer_stride, max_e, d_states_off, d_states, d_n_states));
-            hp_duration_kernel<<<(unsigned)((nj + kWarps - 1) / kWarps), kThreads, 0, st>>>(a, d_pairs, d_pair_window, p0, nj, d_states, d_states_off,
-                                                                                          d_n_states, ctx->d_reads.p, d_dur, d_sum, d_flags + 1);
-            NPH_CUDA(ctx, cudaGetLastError());
-            NPH_CUDA(ctx, cudaEventRecord(ctx->ev1, st));
-            NPH_CUDA(ctx, cudaEventSynchronize(ctx->ev1));
-            NPH_CUDA(ctx, cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1));
-            kernel_ms += ms; launches += 2;
-            cnt.n_chunks += 1;
-        }
+            },
+            &vit_ms, &vit_launches, &cnt.n_chunks));
+        kernel_ms += vit_ms;
+        launches += vit_launches;
         // the reference's host arithmetic on what the device found: per pair local_avg, per job the log-gamma term, folded per
         // window in record order
         std::vector<HpPair> h_pairs(n_pairs);

@@ -94,7 +94,7 @@ int create_common(nph_ctx** out, int device, bool own_stream, cudaStream_t strea
     }
     // every allocation below is checked; a failure releases what exists so far through nph_destroy
     auto fail = [&](int rc) { nph_destroy(ctx); return rc; };
-    if (cudaEventCreate(&ctx->ev0) != cudaSuccess || cudaEventCreate(&ctx->ev1) != cudaSuccess ||
+    if (cudaEventCreate(&ctx->ev0) != cudaSuccess || cudaEventCreate(&ctx->ev1) != cudaSuccess || cudaEventCreate(&ctx->ev_mid) != cudaSuccess ||
         cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&ctx->ev_reset, cudaEventDisableTiming) != cudaSuccess ||
         cudaStreamCreateWithFlags(&ctx->cstream, cudaStreamNonBlocking) != cudaSuccess) return fail(NPH_ERR_CUDA);
@@ -170,6 +170,7 @@ int nph_destroy(nph_ctx* ctx)
     if (ctx->stream || !ctx->own_stream) cudaStreamSynchronize(ctx->stream);
     if (ctx->ev0) cudaEventDestroy(ctx->ev0);
     if (ctx->ev1) cudaEventDestroy(ctx->ev1);
+    if (ctx->ev_mid) cudaEventDestroy(ctx->ev_mid);
     if (ctx->ev_fork) cudaEventDestroy(ctx->ev_fork);
     if (ctx->ev_reset) cudaEventDestroy(ctx->ev_reset);
     if (ctx->cstream) { cudaStreamSynchronize(ctx->cstream); cudaStreamDestroy(ctx->cstream); }

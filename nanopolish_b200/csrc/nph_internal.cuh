@@ -218,8 +218,15 @@ struct nph_ctx {
         DevBuf<uint8_t> d_states;          // one chunk's state offsets, state counts and Viterbi states
     } hp;
 
+    // the last nph_train_transitions_batch (transitions.cu)
+    struct TtState {
+        DevBuf<uint8_t> d_work;            // the group records, the refusal flags, the jobs' groups
+        DevBuf<uint8_t> d_states;          // one chunk's state offsets, state counts and Viterbi states
+    } tt;
+
     // measurement
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    cudaEvent_t ev_mid = nullptr;    // nph_viterbi_chunks: between K3 and the fold of a chunk
     // side streams so that the tail of one forward class overlaps the head of the next (fork/join by events)
     static const int kSideStreams = 4;
     cudaStream_t side[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -422,10 +429,27 @@ int nph_jobs_schedule(nph_ctx* ctx, size_t n_jobs, size_t n_ranks_total, NphJobS
 int nph_score_device_jobs(nph_ctx* ctx, size_t n_jobs, size_t n_ranks_total, double indel_bias, const std::function<int()>& emit);
 // K3 on the n_jobs jobs a kernel of ours wrote into ctx->d_jobs / d_ranks, read transitions and flank table already in place (as
 // nph_score_device_jobs leaves them; hmm_viterbi.cu): one class and trace size for the bounds max_K x max_E, jobs in index order.
-// Job j's path goes to d_states[d_states_off[j] ..) (room d_states_off[j + 1] - d_states_off[j]), its length to d_n_states[j]
-// (0 where the reference would assert).  Device pointers; nothing is read back.
+// Job j = ctx->d_jobs[first_job + j]: its path goes to d_states[d_states_off[j] ..) (room d_states_off[j + 1] - d_states_off[j]),
+// its length to d_n_states[j] (0 where the reference would assert).  Device pointers; nothing is read back.
 int nph_viterbi_device_jobs(nph_ctx* ctx, size_t n_jobs, uint32_t max_K, uint32_t max_E, const uint64_t* d_states_off,
-                            nph_align_state* d_states, uint32_t* d_n_states);
+                            nph_align_state* d_states, uint32_t* d_n_states, size_t first_job);
+// One chunk of nph_viterbi_chunks: jobs [j0, j0 + n) of the caller's numbering, job j0 + i's path at states + states_off[i]
+// (n_states[i] states, 0 where the reference asserts).  Device pointers.
+struct NphVitChunk {
+    uint64_t j0, n;
+    const nph_align_state* states;
+    const uint64_t* states_off;
+    const uint32_t* n_states;
+};
+// K3 over n_jobs jobs in consecutive chunks whose Viterbi states, max_K + max_E per job, fit 1 GiB of buf, at most max_chunk jobs
+// each (0: no cap), rounded down to a multiple of unit (at least unit).  Per chunk: prepare(j0, nj, first) puts the chunk's jobs in
+// ctx->d_jobs from index `first` on (with their ranks, transitions and flank table, as nph_score_device_jobs leaves them), then K3
+// runs on them and fold(chunk) launches the kernels that consume the paths.  *ms: the device time of the offset kernel, K3 and fold
+// over all chunks, *fold_ms (optional) the fold's share of it; *launches: their launches; *n_chunks: the chunks.
+int nph_viterbi_chunks(nph_ctx* ctx, DevBuf<uint8_t>& buf, uint64_t n_jobs, uint64_t max_chunk, uint64_t unit, uint32_t max_K, uint32_t max_E,
+                       const std::function<int(uint64_t j0, uint64_t nj, uint64_t& first)>& prepare,
+                       const std::function<int(const NphVitChunk&)>& fold, float* ms, int* launches, uint32_t* n_chunks,
+                       float* fold_ms = nullptr);
 // One-shot calls (read batch, work and results in one call).  Begin: read records on the main stream, then upload() (the
 // jobs or records), then the event levels in chunks on the copy stream behind progress words the forward kernel polls —
 // enumeration and scheduling run while the levels still cross PCIe.  Finish, on every path: wait for the copy stream.

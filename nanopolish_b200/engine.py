@@ -283,6 +283,23 @@ class Engine:
         self.n_jobs = int(jobs.shape[0])
         return out
 
+    def train_transitions_batch(self, reads, ev_mean, ev_start_time, seq_codes, jobs, groups=None, n_groups: int = 2,
+                                ignore_edge_length: int = 5, max_chunk_jobs: int = 0, indel_bias: float = 1.0):
+        """scorereads --train-transitions (nph_train_transitions_batch): the forward scores of the jobs, TT_COUNTS_DT[n_groups] counts
+        of their Viterbi paths, and the number of chunks of Viterbi states; last_tt_ms then holds the device ms of K3 (with its
+        state-offset kernel) and of the observation kernel"""
+        from .synth import TT_COUNTS_DT, TT_PARAMS_DT
+        scores = np.empty(jobs.shape[0], np.float32)
+        counts = np.zeros(n_groups, TT_COUNTS_DT)
+        params = np.zeros(1, TT_PARAMS_DT)
+        params[0] = (n_groups, ignore_edge_length, max_chunk_jobs, 0, 0.0, 0.0)
+        g = None if groups is None else np.ascontiguousarray(groups, np.uint8)
+        self._check(self.lib.nph_train_transitions_batch(self.ctx, _p(reads), reads.shape[0], _p(ev_mean), _p(ev_start_time), ev_mean.shape[0],
+                                                         _p(seq_codes), seq_codes.shape[0], _p(jobs), jobs.shape[0], _p(g), _p(params),
+                                                         indel_bias, _p(scores), _p(counts)), "nph_train_transitions_batch")
+        self.last_tt_ms = (float(params[0]["viterbi_ms_out"]), float(params[0]["observe_ms_out"]))     # K3 + offsets, observation
+        return scores, counts, int(params[0]["n_chunks_out"])
+
     def hmm_jobs_load_seq(self, seq_codes, jobs, indel_bias: float = 1.0):
         self._check(self.lib.nph_hmm_jobs_load_seq(self.ctx, _p(seq_codes), seq_codes.shape[0], _p(jobs), jobs.shape[0], indel_bias),
                     "nph_hmm_jobs_load_seq")

@@ -500,6 +500,25 @@ std::vector<float> HmmBatch::run(Engine& engine, double indel_bias)
     return scores;
 }
 
+std::vector<float> HmmBatch::run_training(Engine& engine, const std::vector<uint8_t>& groups, nph_tt_params& params, nph_transition_counts* counts,
+                                          double indel_bias)
+{
+    if (!groups.empty() && groups.size() != m_jobs.size()) throw Error(NPH_ERR_INVALID, "one group per job");
+    std::vector<float> scores(m_jobs.size());
+    if (m_jobs.empty()) {
+        engine.check(nph_train_transitions_batch(engine.ctx(), nullptr, 0, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, &params, indel_bias,
+                                                 nullptr, counts), "nph_train_transitions_batch");
+        return scores;
+    }
+    detail::resolve_model_ids(engine, m_job_models, m_jobs);
+    const detail::FlatReads fr = flatten_reads(engine, m_reads);
+    engine.check(nph_train_transitions_batch(engine.ctx(), fr.reads.data(), fr.reads.size(), fr.mean, fr.time, fr.n_events, m_codes.data(),
+                                             m_codes.size(), m_jobs.data(), m_jobs.size(), groups.empty() ? nullptr : groups.data(), &params,
+                                             indel_bias, scores.data(), counts),
+                 "nph_train_transitions_batch");
+    return scores;
+}
+
 size_t AbeaBatch::add(SquiggleRead& read, const PoreModel& pore_model, const std::string& sequence)
 {
     if (m_model && m_model != &pore_model) throw Error(NPH_ERR_INVALID, "one pore model per AbeaBatch");

@@ -449,6 +449,10 @@ public:
     size_t size() const { return m_jobs.size(); }
     void clear();
     std::vector<float> run(Engine& engine, double indel_bias = hmm_indel_bias_factor);
+    // run() plus profile_hmm_align's transition training counts of the same jobs (nph_train_transitions_batch): job j in group
+    // groups[j] (empty: all in group 0), params.n_groups records into counts
+    std::vector<float> run_training(Engine& engine, const std::vector<uint8_t>& groups, nph_tt_params& params, nph_transition_counts* counts,
+                                    double indel_bias = hmm_indel_bias_factor);
     const std::vector<nph_hmm_job>& jobs() const { return m_jobs; }
     // the k-mer ranks of the queued jobs, ranks()[job.rank_off + i] = get_kmer_rank(i, k, rc) — derived from the codes on request
     // (the batch itself ships one byte per base; for inspection and tests)

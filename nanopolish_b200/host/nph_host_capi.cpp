@@ -815,6 +815,63 @@ long long nphh_scorereads(int n_reads, const int32_t* read, const char** ref_seq
     return rc ? rc : n;
 }
 
+// scorereads with ScoreReads(events_per_segment, train) over the reads queued in the aligner (strand 0), in n_batches batches of
+// consecutive reads (one add_read per read, one run() and clear() per batch, as scorereads' batches of BAM records), as
+// nphh_scorereads mode 1: scores3_out per read; with train, counts_out = the two strands' nph_transition_counts accumulated over
+// the batches and text_out = TransitionTraining::report().  max_chunk_jobs: ScoreReads::set_max_chunk_jobs.  Returns the text's
+// length.
+long long nphh_scorereads_train(int n_reads, const int32_t* read, const char** ref_seqs, const int32_t* ref_offsets, int events_per_segment,
+                                int train, uint32_t max_chunk_jobs, int n_batches, double* scores3_out, void* counts_out, char* text_out,
+                                size_t cap)
+{
+    long long n = -1;
+    int rc = guard([&] {
+        if (n_batches < 1) throw Error(NPH_ERR_INVALID, "n_batches < 1");
+        ScoreReads sr((size_t)events_per_segment, train != 0);
+        sr.set_max_chunk_jobs(max_chunk_jobs);
+        for (int b = 0; b < n_batches; ++b) {
+            const int i0 = (int)((long long)n_reads * b / n_batches), i1 = (int)((long long)n_reads * (b + 1) / n_batches);
+            for (int i = i0; i < i1; ++i) sr.add_read(*g_reads[read[i]], 0, g_aligner.alignment((size_t)i), ref_seqs[i], ref_offsets[i]);
+            sr.run(Engine::thread_default());
+            for (int i = i0; i < i1; ++i) {
+                const ReadScore& s = sr.score((size_t)(i - i0));
+                scores3_out[3 * i] = s.score;
+                scores3_out[3 * i + 1] = (double)s.n_events;
+                scores3_out[3 * i + 2] = (double)s.n_segments;
+            }
+            sr.clear();
+        }
+        const std::string text = train ? sr.training().report() : std::string();
+        if (text.size() >= cap) throw Error(NPH_ERR_INVALID, "text buffer too small");
+        std::memcpy(text_out, text.c_str(), text.size() + 1);
+        if (train)
+            for (size_t g = 0; g < TransitionTraining::kStrands; ++g)
+                std::memcpy((char*)counts_out + g * sizeof(nph_transition_counts), &sr.training().counts(g), sizeof(nph_transition_counts));
+        n = (long long)text.size();
+    });
+    return rc ? rc : n;
+}
+
+// TransitionTraining over two given records (counts2): train(strand, prior) into probs_out (30), and report() into text_out.
+// Returns the text's length.
+long long nphh_transition_training(const void* counts2, int strand, const double* prior, double* probs_out, char* text_out, size_t cap)
+{
+    long long n = -1;
+    int rc = guard([&] {
+        TransitionTraining tt;
+        tt.add(static_cast<const nph_transition_counts*>(counts2));
+        TransitionTraining::Probs pr;
+        for (size_t b = 0; b < NPH_TT_BINS; ++b) pr[b] = prior[b];
+        const TransitionTraining::Probs p = tt.train((size_t)strand, pr);
+        for (size_t b = 0; b < NPH_TT_BINS; ++b) probs_out[b] = p[b];
+        const std::string text = tt.report();
+        if (text.size() >= cap) throw Error(NPH_ERR_INVALID, "text buffer too small");
+        std::memcpy(text_out, text.c_str(), text.size() + 1);
+        n = (long long)text.size();
+    });
+    return rc ? rc : n;
+}
+
 // get_aligned_segments on a packed CIGAR: pairs_out = (ref_pos, read_pos) interleaved, seg_off[n_segments + 1]
 long long nphh_aligned_segments(int ref_pos, const uint32_t* cigar, int n_cigar, int32_t* pairs_out, size_t cap_pairs, uint64_t* seg_off, size_t cap_segs)
 {

@@ -1,13 +1,54 @@
 // nph_scorereads.cpp — see nph_scorereads.hpp.
 #include "nph_scorereads.hpp"
 
+#include <cstdio>
 #include <cstdlib>
 
 namespace nph {
 
 void ScoreReads::clear()
 {
-    m_batch.clear(); m_segments.clear(); m_scores.clear();
+    m_batch.clear(); m_segments.clear(); m_scores.clear(); m_strands.clear();
+}
+
+void TransitionTraining::add(const nph_transition_counts* counts)
+{
+    for (size_t g = 0; g < kStrands; ++g) {
+        const uint64_t* in = reinterpret_cast<const uint64_t*>(&counts[g]);
+        uint64_t* acc = reinterpret_cast<uint64_t*>(&m_counts[g]);
+        for (size_t i = 0; i < sizeof(nph_transition_counts) / sizeof(uint64_t); ++i) acc[i] += in[i];
+    }
+}
+
+TransitionTraining::Probs TransitionTraining::train(size_t strand, const Probs& prior) const
+{
+    const nph_transition_counts& c = m_counts[strand];
+    const uint32_t pseudocount = 100;
+    Probs p;
+    for (size_t b = 0; b < NPH_TT_BINS; ++b) {
+        double skip = prior[b] * pseudocount;
+        // the reference's observations of a bin in any order: +1.0 per skip, +0.0 (no change) per other; total += 1 is exact
+        for (uint64_t i = 0; i < c.skip_count[b]; ++i) skip += 1.0;
+        const double total = (double)pseudocount + (double)c.skip_total[b];
+        p[b] = skip / total;
+    }
+    return p;
+}
+
+std::string TransitionTraining::report() const
+{
+    std::string out;
+    char line[96];
+    for (size_t strand = 0; strand < kStrands; ++strand) {
+        std::snprintf(line, sizeof(line), "Transition parameters for %zu\n", strand);
+        out += line;
+        const Probs p = train(strand);
+        for (size_t b = 0; b < NPH_TT_BINS; ++b) {
+            std::snprintf(line, sizeof(line), "skip_probabilities[%zu] = %.3lf;\n", b, p[b]);
+            out += line;
+        }
+    }
+    return out;
 }
 
 size_t ScoreReads::add_read(SquiggleRead& sr, size_t strand_idx, const std::vector<EventAlignment>& alignment_output,
@@ -41,13 +82,22 @@ size_t ScoreReads::add_read(SquiggleRead& sr, size_t strand_idx, const std::vect
         HMMInputSequence sequence(seg, alphabet->reverse_complement(seg), alphabet);
         const int events_in_segment = std::abs((int)data.event_start_idx - (int)data.event_stop_idx) + 1;
         m_segments.push_back(Segment{read_idx, m_batch.add(sequence, data, 0), events_in_segment});
+        m_strands.push_back((uint8_t)strand_idx);
     }
     return read_idx;
 }
 
 void ScoreReads::run(Engine& engine, double indel_bias)
 {
-    const std::vector<float> s = m_batch.run(engine, indel_bias);
+    std::vector<float> s;
+    if (m_train) {
+        nph_tt_params params{(uint32_t)TransitionTraining::kStrands, 5, m_max_chunk_jobs, 0, 0.f, 0.f};   // ignore_edge_length = 5
+        nph_transition_counts counts[TransitionTraining::kStrands];
+        s = m_batch.run_training(engine, m_strands, params, counts, indel_bias);
+        m_training.add(counts);
+    } else {
+        s = m_batch.run(engine, indel_bias);
+    }
     std::vector<double> sum(m_scores.size(), 0.0);
     for (const Segment& g : m_segments) {
         sum[g.read] += s[g.job];                    // double accumulation of the float segment scores, in segment order
@@ -57,6 +107,7 @@ void ScoreReads::run(Engine& engine, double indel_bias)
     for (size_t i = 0; i < m_scores.size(); ++i)
         m_scores[i].score = m_scores[i].n_events == 0 ? 1.0 : sum[i] / (double)m_scores[i].n_events;
     m_segments.clear();
+    m_strands.clear();
     m_batch.clear();
 }
 

@@ -92,6 +92,10 @@ assert ALIGN_STATE_DT.itemsize == 16
 assert READ_DT.itemsize == 64 and HMM_JOB_DT.itemsize == 32 and ABEA_JOB_DT.itemsize == 32
 assert PAIR_DT.itemsize == 8 and ABEA_RES_DT.itemsize == 24
 
+TT_COUNTS_DT = np.dtype([("state_transitions", "<u8", (3, 6)), ("n_matches", "<u8"), ("n_merges", "<u8"), ("n_skips", "<u8"),
+                         ("skip_total", "<u8", 30), ("skip_count", "<u8", 30)])
+TT_PARAMS_DT = np.dtype([("n_groups", "<u4"), ("ignore_edge_length", "<u4"), ("max_chunk_jobs", "<u4"), ("n_chunks_out", "<u4"),
+                         ("viterbi_ms_out", "<f4"), ("observe_ms_out", "<f4")])
 HAF_ALLOW_PRE_CLIP = 1
 HAF_ALLOW_POST_CLIP = 2
 
