@@ -912,6 +912,61 @@ int nph_homopolymer_likelihoods_batch(nph_ctx* ctx, const nph_read* reads, size_
                                       const nph_hp_window* windows, size_t n_windows, double indel_bias,
                                       nph_hp_likelihoods* out, nph_hp_counts* counts_out);
 
+/* ---- variants --calculate-all-support: the A/C/G/T read support of every called variant (ref: annotate_variants_with_all_support,
+ * src/common/nanopolish_variant.cpp:801-859) -------------------------------------------------------------------------------------
+ * Per variant, in input order and each on its own:
+ *   the window                    calling_start = ref_position - flank, calling_end = ref_position + flank: the 2 * flank + 1 bases
+ *                                 ref_bases[calling_start - region_start ..] (substr_by_reference of the unedited region)
+ *   four haplotypes, b in "ACGT"  apply_variant of {ref_seq, alt_seq = b} on a fresh window: it applies when window.substr(flank,
+ *                                 ref_seq_len) == ref_seq byte for byte (substr clamps, so a ref_seq longer than flank + 1 bases never
+ *                                 applies), and then ref_seq is replaced by b; otherwise the haplotype is the window.  `applied`
+ *                                 reports the outcome (it does not depend on b)
+ *   the window's event sequences  AlignmentDB::get_event_subsequences over [calling_start, calling_end] (the records of
+ *                                 nph_screen_edits_batch, in record order: bounded by _find_by_ref_bounds, event/bp ratio below 20);
+ *                                 n_reads counts them
+ *   per sequence, in record order s[hi] = profile_hmm_score(haplotype hi, sequence, alignment_flags) (K1), a float;
+ *                                 sum = s[0], then sum = add_logs(s[hi], sum) for hi = 1..3 (p7_FLogsum on floats);
+ *                                 support[hi] += exp(double(s[hi]) - double(sum)), in double
+ *   support[hi] /= n_reads        (0 / 0 with no sequence: a NaN, which the reference prints as -nan)
+ * K1 and the log-sum run on the device, exp, the sum over sequences and the division on the host with its libm (DESIGN.md).
+ * Records: nph_meth_record in the compact form of nph_screen_edits_batch, model_id a nucleotide model of k = params->k.
+ * ref_bases: the region's reference, ref_bases[p] = base at region_start + p (AlignmentDB's m_region_start .. m_region_end).
+ * NPH_ERR_INVALID: k outside 1..8; flank + 1 < k (a haplotype without a k-mer); alignment_flags other than NPH_HAF_*; a ref_seq
+ * outside ref_seqs; a window outside the region (substr_by_reference asserts: calling_start < region_start or calling_end >
+ * region_end); a record or model out of bounds or not a nucleotide model of k; a job the forward scorer refuses.  The contig test
+ * of get_event_subsequences (a variant on another contig asserts) is the caller's. */
+typedef struct {
+    int32_t  region_start;            /* AlignmentDB::m_region_start */
+    int32_t  flank;                   /* min_flanking_sequence (variants: 30) */
+    uint32_t alignment_flags;         /* NPH_HAF_* (variants: NPH_HAF_ALLOW_PRE_CLIP | NPH_HAF_ALLOW_POST_CLIP) */
+    uint32_t k;                       /* the reads' base-model k */
+} nph_support_params;                 /* 16 bytes */
+typedef struct {
+    int32_t  ref_position;            /* Variant::ref_position */
+    uint32_t ref_seq_len;             /* ref_seq.size() */
+    uint64_t ref_seq_off;             /* first byte of ref_seq in ref_seqs[] */
+} nph_support_variant;                /* 16 bytes */
+typedef struct {
+    double   support[4];              /* SupportFractionByBase for A, C, G, T */
+    uint32_t n_reads;                 /* event sequences of the window (the divisor) */
+    uint32_t applied;                 /* 1: apply_variant replaced ref_seq; 0: the four haplotypes are the window */
+} nph_support_result;                 /* 40 bytes */
+typedef struct {
+    uint64_t n_variants, n_pairs;     /* variants; (variant, event sequence) pairs */
+    uint64_t n_jobs;                  /* 4 per pair, one forward fill each */
+    uint64_t n_dp_rows;               /* event rows over all jobs */
+    double   host_ms;                 /* the host's exp, sums and divisions.  nph_last_kernel_ms after the call: the forward kernels
+                                         (not the pair, scan, emit, scheduling or log-sum kernels) */
+} nph_support_counts;                 /* 40 bytes */
+int nph_all_support_batch(nph_ctx* ctx, const nph_read* reads, size_t n_reads,
+                          const float* ev_mean, const double* ev_start_time, size_t n_events_total,
+                          const char* ref_bases, size_t n_ref_bases,
+                          const int16_t* event_deltas, size_t n_deltas_total, const int32_t* first_event,
+                          const nph_meth_record* records, size_t n_records,
+                          const nph_support_params* params, const char* ref_seqs, size_t n_seq_bytes,
+                          const nph_support_variant* variants, size_t n_variants, double indel_bias,
+                          nph_support_result* out, nph_support_counts* counts_out);
+
 /* ---- scorereads --train-transitions: forward scores and transition training counts of a job batch ----------------------------
  * `nanopolish scorereads --train-transitions` runs, for every segment model_score scores (src/nanopolish_scorereads.cpp:116-203),
  * profile_hmm_align(sequence, data) (K3, flags 0) after the forward score, and folds the path into

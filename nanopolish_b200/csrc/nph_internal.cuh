@@ -218,6 +218,13 @@ struct nph_ctx {
         DevBuf<uint8_t> d_states;          // one chunk's state offsets, state counts and Viterbi states
     } hp;
 
+    // the last nph_all_support_batch (all_support.cu)
+    struct SupportState {
+        NphEventRecords ev;                // region reference, compact event alignments, records
+        DevBuf<uint8_t> d_counts;          // per-variant windows, pair counts, their offsets, the scan's scratch
+        DevBuf<uint8_t> d_pairs;           // pairs, their variants, per job the difference score - log-sum
+    } sup;
+
     // the last nph_train_transitions_batch (transitions.cu)
     struct TtState {
         DevBuf<uint8_t> d_work;            // the group records, the refusal flags, the jobs' groups

@@ -10,7 +10,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from .synth import ABEA_RES_DT, ALIGN_STATE_DT, CALIBRATION_DT, EVENT_DT, EVENT_RANGE_DT, METH_SITE_DT, METHFREQ_PARAMS_DT, HP_COUNTS_DT, HP_LIK_DT, HP_WINDOW_DT, PAIR_DT, PHASE_CALL_DT, PHASE_VARIANT_DT, POLYA_RES_DT, POLYI_RES_DT, RAW_RANGE_DT
+from .synth import ABEA_RES_DT, ALIGN_STATE_DT, CALIBRATION_DT, EVENT_DT, EVENT_RANGE_DT, METH_SITE_DT, METHFREQ_PARAMS_DT, HP_COUNTS_DT, HP_LIK_DT, HP_WINDOW_DT, PAIR_DT, PHASE_CALL_DT, PHASE_VARIANT_DT, POLYA_RES_DT, POLYI_RES_DT, RAW_RANGE_DT, SUPPORT_COUNTS_DT, SUPPORT_RESULT_DT, SUPPORT_VARIANT_DT
 
 
 def _p(a):
@@ -206,6 +206,21 @@ class Engine:
                                                                calling_seqs.shape[0], _p(windows), windows.shape[0], indel_bias, _p(out), _p(cnt)),
                     "nph_homopolymer_likelihoods_batch")
         return out[:windows.shape[0]], cnt[0]
+
+    # ---- variants --calculate-all-support: A/C/G/T read support of every variant (include/nph.h, nph_all_support_batch) ----
+    def all_support_batch(self, reads, ev_mean, ev_start_time, ref_bases, deltas, first_event, records, params, ref_seqs, variants,
+                          indel_bias: float = 1.0):
+        """records METH_RECORD_DT (compact event alignments, as screening's), params SUPPORT_PARAMS_DT[1], ref_seqs u1, variants
+        SUPPORT_VARIANT_DT.  Returns (SUPPORT_RESULT_DT[n_variants], SUPPORT_COUNTS_DT scalar)."""
+        assert variants.dtype == SUPPORT_VARIANT_DT
+        out = np.zeros(max(variants.shape[0], 1), SUPPORT_RESULT_DT)
+        cnt = np.zeros(1, SUPPORT_COUNTS_DT)
+        self._check(self.lib.nph_all_support_batch(self.ctx, _p(reads), reads.shape[0], _p(ev_mean), _p(ev_start_time), ev_mean.shape[0],
+                                                   _p(ref_bases), ref_bases.shape[0], _p(deltas), deltas.shape[0], _p(first_event), _p(records),
+                                                   records.shape[0], _p(params), _p(ref_seqs), ref_seqs.shape[0], _p(variants), variants.shape[0],
+                                                   indel_bias, _p(out), _p(cnt)),
+                    "nph_all_support_batch")
+        return out[:variants.shape[0]], cnt[0]
 
     def screen_load(self, ref_bases, deltas, first_event, records, params, indel_bias: float = 1.0, methylation=None):
         head = (self.ctx, _p(ref_bases), ref_bases.shape[0], _p(deltas), deltas.shape[0], _p(first_event), _p(records), records.shape[0], _p(params),

@@ -957,6 +957,44 @@ long long nphh_fix_homopolymers(const char* contig, int region_start, const char
     return st ? st : n;
 }
 
+// nph::annotate_variants_with_all_support over the region [region_start, region_start + strlen(region_ref) - 1] of `contig`, records
+// as nphh_fix_homopolymers takes them, on the variants {var_contig, var_pos[i], var_ref[i], var_alt[i]} in order.  out: one line per
+// variant, its INFO after the call.  Returns the length written, or a negative nph_status (NPH_ERR_INVALID also when out is too
+// small).
+long long nphh_all_support(const char* contig, int region_start, const char* region_ref, int n_records, const int32_t* read, const uint8_t* rc,
+                           const int32_t* pairs, const uint64_t* pair_off, const char* var_contig, int n_variants, const int32_t* var_pos,
+                           const char** var_ref, const char** var_alt, int min_flank, uint32_t alignment_flags, double indel_bias,
+                           char* out, size_t cap)
+{
+    long long n = -1;
+    int st = guard([&] {
+        RegionAlignments region;
+        region.contig = contig; region.region_start = region_start; region.reference = region_ref;
+        for (int r = 0; r < n_records; ++r) {
+            EventAlignedRead e;
+            e.read = g_reads[read[r]].get();
+            e.contig = contig;
+            e.rc[0] = rc[r] != 0;
+            const uint64_t np = pair_off[r + 1] - pair_off[r];
+            e.aligned_events[0].resize(np);
+            if (np) std::memcpy(e.aligned_events[0].data(), pairs + 2 * pair_off[r], sizeof(AlignedPair) * np);
+            region.records.push_back(std::move(e));
+        }
+        std::vector<Variant> variants(n_variants);
+        for (int i = 0; i < n_variants; ++i) {
+            variants[i].ref_name = var_contig; variants[i].ref_position = (size_t)var_pos[i];
+            variants[i].ref_seq = var_ref[i]; variants[i].alt_seq = var_alt[i];
+        }
+        annotate_variants_with_all_support(variants, region, min_flank, alignment_flags, Engine::thread_default(), indel_bias);
+        std::string s;
+        for (const Variant& v : variants) s += v.info + "\n";
+        if (s.size() + 1 > cap) throw Error(NPH_ERR_INVALID, "output buffer too small");
+        std::memcpy(out, s.c_str(), s.size() + 1);
+        n = (long long)s.size();
+    });
+    return st ? st : n;
+}
+
 // the mirror's Haplotype::substr_by_reference and enclosing range on Haplotype(contig, hap_pos, hap_ref) + the variants:
 // out = the substring's sequence; range = {hap_lower, hap_upper, ref_lower, ref_upper} of the enclosing range of [lo, hi]
 // (npos as -1).  Returns the substring's reference position, or a negative nph_status where the reference asserts.

@@ -3,6 +3,8 @@
 
 #include <cmath>
 #include <cstring>
+#include <iomanip>
+#include <sstream>
 
 namespace nph {
 
@@ -302,6 +304,52 @@ HomopolymerCall homopolymer_call(const nph_hp_likelihoods& lik, size_t hp_length
     return out;
 }
 
+namespace {
+
+// The region in screening's flat layout: per record its compact event alignment over the span of its aligned_events, the reads
+// its records name, and their event start times
+struct RegionLayout {
+    detail::ReadTable reads;
+    std::vector<nph_meth_record> recs;
+    std::vector<int16_t> deltas;
+    std::vector<int32_t> first;
+    detail::FlatReads fr;
+    std::vector<double> time;
+};
+
+RegionLayout region_layout(const HomopolymerRegion& region, Engine& engine, const char* caller)
+{
+    RegionLayout rl;
+    for (const EventAlignedRead& r : region.records) {
+        const std::vector<AlignedPair>& ae = r.aligned_events[0];
+        nph_meth_record rec;
+        std::memset(&rec, 0, sizeof(rec));
+        rec.read = rl.reads.index(r.read, 0);
+        rec.model_id = engine.model_id(r.read->get_base_model(0));
+        rec.rc = r.rc[0] ? 1 : 0;
+        rec.ref_off = rl.deltas.size();
+        int32_t f = 0;
+        if (!ae.empty() && r.read->has_events_for_strand(0)) {
+            rec.ref_start_pos = ae.front().ref_pos;
+            rec.ref_len = (uint32_t)(ae.back().ref_pos - ae.front().ref_pos + 1);
+            rl.deltas.resize(rl.deltas.size() + rec.ref_len);
+            if (!compact_event_alignment(ae, rec.ref_start_pos, rec.ref_len, rl.deltas.data() + rec.ref_off, &f))
+                throw Error(NPH_ERR_UNSUPPORTED, std::string(caller) + ": an event alignment with a step beyond int16");
+        }
+        rl.first.push_back(f);
+        rl.recs.push_back(rec);
+    }
+    rl.fr = detail::flatten_reads(engine, rl.reads);
+    rl.time.resize(std::max<size_t>(rl.fr.n_events, 1));
+    for (size_t i = 0; i < rl.reads.size(); ++i) {
+        const std::vector<SquiggleEvent>& ev = rl.reads.reads()[i].first->events[rl.reads.reads()[i].second];
+        for (size_t e = 0; e < ev.size(); ++e) rl.time[rl.fr.reads[i].event_off + e] = ev[e].start_time;
+    }
+    return rl;
+}
+
+} // namespace
+
 Haplotype fix_homopolymers(const Haplotype& input, const HomopolymerRegion& region, int min_flanking_sequence, Engine& engine, double indel_bias,
                            nph_hp_counts* counts_out)
 {
@@ -314,36 +362,12 @@ Haplotype fix_homopolymers(const Haplotype& input, const HomopolymerRegion& regi
         seqs += wins[i].calling;
         dev[i] = wins[i].dev;
     }
-    // the region in screening's flat layout: per record its compact event alignment over the span of its aligned_events
-    detail::ReadTable reads;
-    std::vector<nph_meth_record> recs;
-    std::vector<int16_t> deltas;
-    std::vector<int32_t> first;
-    for (const EventAlignedRead& r : region.records) {
-        const std::vector<AlignedPair>& ae = r.aligned_events[0];
-        nph_meth_record rec;
-        std::memset(&rec, 0, sizeof(rec));
-        rec.read = reads.index(r.read, 0);
-        rec.model_id = engine.model_id(r.read->get_base_model(0));
-        rec.rc = r.rc[0] ? 1 : 0;
-        rec.ref_off = deltas.size();
-        int32_t f = 0;
-        if (!ae.empty() && r.read->has_events_for_strand(0)) {
-            rec.ref_start_pos = ae.front().ref_pos;
-            rec.ref_len = (uint32_t)(ae.back().ref_pos - ae.front().ref_pos + 1);
-            deltas.resize(deltas.size() + rec.ref_len);
-            if (!compact_event_alignment(ae, rec.ref_start_pos, rec.ref_len, deltas.data() + rec.ref_off, &f))
-                throw Error(NPH_ERR_UNSUPPORTED, "fix_homopolymers: an event alignment with a step beyond int16");
-        }
-        first.push_back(f);
-        recs.push_back(rec);
-    }
-    const detail::FlatReads fr = detail::flatten_reads(engine, reads);
-    std::vector<double> time(std::max<size_t>(fr.n_events, 1));
+    const RegionLayout rl = region_layout(region, engine, "fix_homopolymers");
+    const detail::FlatReads& fr = rl.fr;
     std::vector<float> duration(std::max<size_t>(fr.n_events, 1));
-    for (size_t i = 0; i < reads.size(); ++i) {
-        const std::vector<SquiggleEvent>& ev = reads.reads()[i].first->events[reads.reads()[i].second];
-        for (size_t e = 0; e < ev.size(); ++e) { time[fr.reads[i].event_off + e] = ev[e].start_time; duration[fr.reads[i].event_off + e] = ev[e].duration; }
+    for (size_t i = 0; i < rl.reads.size(); ++i) {
+        const std::vector<SquiggleEvent>& ev = rl.reads.reads()[i].first->events[rl.reads.reads()[i].second];
+        for (size_t e = 0; e < ev.size(); ++e) duration[fr.reads[i].event_off + e] = ev[e].duration;
     }
     nph_hp_params params;
     std::memset(&params, 0, sizeof(params));
@@ -351,9 +375,9 @@ Haplotype fix_homopolymers(const Haplotype& input, const HomopolymerRegion& regi
     params.min_flanking_sequence = min_flanking_sequence;
     std::vector<nph_hp_likelihoods> lik(std::max<size_t>(wins.size(), 1));
     nph_hp_counts counts;
-    engine.check(nph_homopolymer_likelihoods_batch(engine.ctx(), fr.reads.data(), fr.reads.size(), fr.mean, time.data(), duration.data(), fr.n_events,
-                                                   region.reference.data(), region.reference.size(), deltas.data(), deltas.size(), first.data(),
-                                                   recs.data(), recs.size(), &params, seqs.data(), seqs.size(), dev.data(), dev.size(), indel_bias,
+    engine.check(nph_homopolymer_likelihoods_batch(engine.ctx(), fr.reads.data(), fr.reads.size(), fr.mean, rl.time.data(), duration.data(), fr.n_events,
+                                                   region.reference.data(), region.reference.size(), rl.deltas.data(), rl.deltas.size(), rl.first.data(),
+                                                   rl.recs.data(), rl.recs.size(), &params, seqs.data(), seqs.size(), dev.data(), dev.size(), indel_bias,
                                                    lik.data(), &counts),
                  "nph_homopolymer_likelihoods_batch");
     if (counts_out) *counts_out = counts;
@@ -388,6 +412,51 @@ Haplotype fix_homopolymers(const Haplotype& input, const HomopolymerRegion& regi
         }
     }
     return fixed;
+}
+
+void annotate_variants_with_all_support(std::vector<Variant>& input, const RegionAlignments& alignments, int min_flanking_sequence,
+                                        uint32_t alignment_flags, Engine& engine, double indel_bias, nph_support_counts* counts_out)
+{
+    std::string ref_seqs;
+    std::vector<nph_support_variant> dev(std::max<size_t>(input.size(), 1));
+    for (size_t i = 0; i < input.size(); ++i) {
+        const Variant& v = input[i];
+        if (v.ref_name != alignments.contig)
+            throw Error(NPH_ERR_INVALID, "annotate_variants_with_all_support: variant " + std::to_string(i) + " is on another contig than the region");
+        if (v.ref_position > (size_t)INT32_MAX)
+            throw Error(NPH_ERR_INVALID, "annotate_variants_with_all_support: variant " + std::to_string(i) + " lies beyond int32");
+        std::memset(&dev[i], 0, sizeof(dev[i]));
+        dev[i].ref_position = (int32_t)v.ref_position;
+        dev[i].ref_seq_len = (uint32_t)v.ref_seq.size();
+        dev[i].ref_seq_off = ref_seqs.size();
+        ref_seqs += v.ref_seq;
+    }
+    const RegionLayout rl = region_layout(alignments, engine, "annotate_variants_with_all_support");
+    const detail::FlatReads& fr = rl.fr;
+    nph_support_params params;
+    std::memset(&params, 0, sizeof(params));
+    params.region_start = alignments.region_start;
+    params.flank = min_flanking_sequence;
+    params.alignment_flags = alignment_flags;
+    // every record's base model has this k (the device call checks); the DNA models of the reads are 6-mers
+    params.k = alignments.records.empty() ? 6 : alignments.records[0].read->get_base_model(0)->k;
+    std::vector<nph_support_result> out(std::max<size_t>(input.size(), 1));
+    nph_support_counts counts;
+    engine.check(nph_all_support_batch(engine.ctx(), fr.reads.data(), fr.reads.size(), fr.mean, rl.time.data(), fr.n_events,
+                                       alignments.reference.data(), alignments.reference.size(), rl.deltas.data(), rl.deltas.size(), rl.first.data(),
+                                       rl.recs.data(), rl.recs.size(), &params, ref_seqs.data(), ref_seqs.size(), dev.data(), input.size(), indel_bias,
+                                       out.data(), &counts),
+                 "nph_all_support_batch");
+    if (counts_out) *counts_out = counts;
+    for (size_t i = 0; i < input.size(); ++i) {
+        std::stringstream ss;
+        ss << std::fixed << std::setprecision(3);
+        for (int hi = 0; hi < 4; ++hi) {
+            ss << out[i].support[hi];
+            if (hi != 3) ss << ",";
+        }
+        input[i].add_info("SupportFractionByBase", ss.str());
+    }
 }
 
 } // namespace nph

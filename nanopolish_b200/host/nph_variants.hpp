@@ -8,6 +8,8 @@
 //   the scoring loop of score_variant_group      ref: src/common/nanopolish_variant.cpp:242-258
 //   fix_homopolymers                             ref: src/nanopolish_call_variants.cpp:541-780 (its likelihoods on the device,
 //                                                nph_homopolymer_likelihoods_batch)
+//   annotate_variants_with_all_support           ref: src/common/nanopolish_variant.cpp:801-859 (its scores on the device,
+//                                                nph_all_support_batch)
 //
 // The reference scores one (read, sequence) pair per profile_hmm_score call inside an OpenMP loop.  Here every
 // (read, haplotype, alphabet alternative) triple of a whole candidate set becomes one job of ONE launch; the base
@@ -32,6 +34,11 @@ struct Variant {
     template <typename T> void add_info(const std::string& k, T value)
     {
         const std::string kv = k + "=" + std::to_string(value);
+        info = info.empty() ? kv : info + ";" + kv;
+    }
+    void add_info(const std::string& k, const std::string& value)
+    {
+        const std::string kv = k + "=" + value;
         info = info.empty() ? kv : info + ";" + kv;
     }
 };
@@ -137,5 +144,20 @@ HomopolymerCall homopolymer_call(const nph_hp_likelihoods& lik, size_t hp_length
 // window.  counts_out (optional): the device call's counters.
 Haplotype fix_homopolymers(const Haplotype& input, const HomopolymerRegion& region, int min_flanking_sequence, Engine& engine,
                            double indel_bias = hmm_indel_bias_factor, nph_hp_counts* counts_out = nullptr);
+
+// The AlignmentDB of annotate_variants_with_all_support: the same view of a region and its records as fix_homopolymers reads
+typedef HomopolymerRegion RegionAlignments;
+
+// annotate_variants_with_all_support (ref: src/common/nanopolish_variant.cpp:801-859): per variant, the window [ref_position -
+// min_flanking_sequence, ref_position + min_flanking_sequence] of the region's reference with its ref_seq replaced by A, C, G and T
+// (apply_variant, or the window where it does not apply) scored against every event sequence of the window, all variants in one
+// nph_all_support_batch; then INFO gets SupportFractionByBase=a,c,g,t, each "%.3f" (std::fixed, precision 3) of the mean over the
+// reads of exp(score - log-sum of the four), in input order.  Throws Error(NPH_ERR_INVALID) where the reference asserts: a window
+// outside the region, a variant on another contig; also for a ref_position beyond int32 (the reference narrows the window's ends to
+// int).  The variants call it with alignment_flags NPH_HAF_ALLOW_PRE_CLIP | NPH_HAF_ALLOW_POST_CLIP.  counts_out (optional): the
+// device call's counters.
+void annotate_variants_with_all_support(std::vector<Variant>& input, const RegionAlignments& alignments, int min_flanking_sequence,
+                                        uint32_t alignment_flags, Engine& engine, double indel_bias = hmm_indel_bias_factor,
+                                        nph_support_counts* counts_out = nullptr);
 
 } // namespace nph

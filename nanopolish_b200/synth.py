@@ -859,6 +859,14 @@ def gen_hp_pileup(ref_len: int, depth: int, read_bases: int, model: PoreModel, s
     return ref, rs, recs, np.concatenate(prs), dur, edits
 
 
+# ---- variants --calculate-all-support (nph_all_support_batch) ------------------------------------------------------------------
+SUPPORT_PARAMS_DT = np.dtype([("region_start", "<i4"), ("flank", "<i4"), ("alignment_flags", "<u4"), ("k", "<u4")], align=True)
+SUPPORT_VARIANT_DT = np.dtype([("ref_position", "<i4"), ("ref_seq_len", "<u4"), ("ref_seq_off", "<u8")], align=True)
+SUPPORT_RESULT_DT = np.dtype([("support", "<f8", 4), ("n_reads", "<u4"), ("applied", "<u4")], align=True)
+SUPPORT_COUNTS_DT = np.dtype([("n_variants", "<u8"), ("n_pairs", "<u8"), ("n_jobs", "<u8"), ("n_dp_rows", "<u8"), ("host_ms", "<f8")], align=True)
+assert SUPPORT_PARAMS_DT.itemsize == 16 and SUPPORT_VARIANT_DT.itemsize == 16 and SUPPORT_RESULT_DT.itemsize == 40 and SUPPORT_COUNTS_DT.itemsize == 40
+
+
 # ---- methylation-aware screening (`variants -q cpg`, `-q dam,dcm`) -------------------------------------------------------
 SCREEN_METH_DT = np.dtype([("n_types", "<u4"), ("reserved", "<u4"), ("alphabets", METH_PARAMS_DT, 4)], align=True)
 assert SCREEN_METH_DT.itemsize == 616
