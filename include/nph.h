@@ -967,6 +967,67 @@ int nph_all_support_batch(nph_ctx* ctx, const nph_read* reads, size_t n_reads,
                           const nph_support_variant* variants, size_t n_variants, double indel_bias,
                           nph_support_result* out, nph_support_counts* counts_out);
 
+/* ---- variants: screen_variants_by_score on a candidate list (ref: src/nanopolish_call_variants.cpp:364-402) ------------------
+ * Each candidate of the list on its own, in input order (the reference's semantics on one OpenMP thread):
+ *   the window        calling_start = ref_position - flank, calling_end = ref_position + ref_seq_len + flank, narrowed to int; a
+ *                     window with calling_start < region_start or calling_end > region_end is skipped (are_coordinates_valid):
+ *                     status NPH_SCREEN_OUTSIDE, quality NaN.  The base haplotype is the ref_seq_len + 2 * flank + 1 bases
+ *                     ref_bases[calling_start - region_start ..]
+ *   the variant       apply_variant on a fresh window: when window[flank, flank + ref_seq_len) == ref_seq byte for byte
+ *                     (case-sensitive; an empty ref_seq always matches) ref_seq is replaced by alt_seq.  Otherwise the haplotype is
+ *                     the window and the quality is exactly 0.0: status NPH_SCREEN_NOT_APPLIED, nothing is scored
+ *   the reads         get_event_subsequences(calling_start, calling_end): the records of nph_screen_edits_batch in record order,
+ *                     bounded by _find_by_ref_bounds, event/bp ratio below 20
+ *   the quality       total = 0.0, then per read: if (fabs(total) < score_threshold) total += set(variant) - set(base), each side
+ *                     profile_hmm_score_set over the sequence and its -q alternatives (as nph_screen_load_methylation forms them)
+ * screen_variants_by_score keeps the candidates whose quality is > 0.
+ * Candidates with the same window (calling_start and ref_seq_len) share their reads and their base scores: the device scores the
+ * base set once per (window, read) for all the window's candidates still inside the threshold, reads_per_round reads at a time.
+ * Records: nph_meth_record in the compact form of nph_screen_edits_batch, model_id a nucleotide model of k = params->k.
+ * meth (NULL: no types) and alt_model_ids: as nph_screen_load_methylation takes them, with exactly its checks.
+ * NPH_ERR_INVALID: k outside 1..8; 2 * flank + 1 < k; reads_per_round == 0; alignment_flags other than NPH_HAF_*; an allele outside
+ * alleles; ref_position + ref_seq_len + flank > INT32_MAX; a record or model out of range or not a nucleotide model of k; a job the
+ * forward scorer refuses. */
+#define NPH_SCREEN_SCREENED    0u     /* scored: quality = the thresholded total */
+#define NPH_SCREEN_OUTSIDE     1u     /* the window leaves the region: the reference skips the candidate (quality NaN) */
+#define NPH_SCREEN_NOT_APPLIED 2u     /* ref_seq is not the window's: the variant haplotype is the base, quality 0.0 */
+typedef struct {
+    int32_t  region_start;            /* AlignmentDB::m_region_start */
+    int32_t  flank;                   /* opt::screen_flanking_sequence (10) */
+    uint32_t score_threshold;         /* opt::screen_score_threshold (100; --faster: 25) */
+    uint32_t alignment_flags;         /* NPH_HAF_* */
+    uint32_t k;                       /* the reads' base-model k */
+    uint32_t reads_per_round;         /* reads of a window scored between two early-exit tests (8) */
+} nph_screen_list_params;             /* 24 bytes */
+typedef struct {
+    int64_t  ref_position;            /* Variant::ref_position (>= 0) */
+    uint32_t ref_seq_len, alt_seq_len;
+    uint64_t ref_seq_off, alt_seq_off;   /* first byte of each allele in alleles[] */
+} nph_screen_candidate;               /* 32 bytes */
+typedef struct {
+    double   quality;                 /* Variant::quality after score_variant_thresholded (NaN: NPH_SCREEN_OUTSIDE) */
+    uint32_t n_reads;                 /* event sequences of the window */
+    uint32_t status;                  /* NPH_SCREEN_SCREENED, _OUTSIDE or _NOT_APPLIED */
+} nph_screen_result;                  /* 16 bytes */
+typedef struct {
+    uint64_t n_candidates, n_windows; /* candidates; distinct windows among those inside the region */
+    uint64_t n_rounds;                /* early-exit rounds */
+    uint64_t n_jobs, n_dp_rows;       /* forward jobs run and their event rows */
+    uint64_t n_jobs_without_exit;     /* jobs every read of every applied candidate would take: per window reads x (n(base) + sum n(c)) */
+    uint64_t n_reference_rows;        /* the reference's DP rows: (n(base) + n(variant)) x E per (candidate, read) until its exit,
+                                         n(s) = 1 + alternatives of s; candidates that do not apply count too (the reference scores them) */
+    double   kernel_ms;               /* device time of the forward kernels of every round (not the pair, rank, emit or accumulate kernels) */
+} nph_screen_list_counts;             /* 64 bytes */
+int nph_screen_variants_batch(nph_ctx* ctx, const nph_read* reads, size_t n_reads,
+                              const float* ev_mean, const double* ev_start_time, size_t n_events_total,
+                              const char* ref_bases, size_t n_ref_bases,
+                              const int16_t* event_deltas, size_t n_deltas_total, const int32_t* first_event,
+                              const nph_meth_record* records, size_t n_records,
+                              const nph_screen_list_params* params, const char* alleles, size_t n_allele_bytes,
+                              const nph_screen_candidate* candidates, size_t n_candidates, double indel_bias,
+                              const nph_screen_methylation* meth, const uint32_t* alt_model_ids,
+                              nph_screen_result* out, nph_screen_list_counts* counts_out);
+
 /* ---- scorereads --train-transitions: forward scores and transition training counts of a job batch ----------------------------
  * `nanopolish scorereads --train-transitions` runs, for every segment model_score scores (src/nanopolish_scorereads.cpp:116-203),
  * profile_hmm_align(sequence, data) (K3, flags 0) after the forward score, and folds the path into

@@ -18,6 +18,15 @@ struct MethDev {
 // and the three site arrays.  NPH_ERR_INVALID for a malformed alphabet, NPH_ERR_UNSUPPORTED for sites that can overlap each other.
 int nph_meth_alphabet(nph_ctx* ctx, const nph_meth_params& p, MethDev& d);
 
+// The -q types of a screening (variants.cu; nph_screen_load_methylation and nph_screen_variants_batch): at most
+// NPH_SCREEN_MAX_TYPES, alt_model_ids present when there are types and records, each alphabet well formed and of k.
+int nph_screen_types(nph_ctx* ctx, uint32_t k, const nph_screen_methylation& meth, size_t n_records, const uint32_t* alt_model_ids,
+                     std::vector<MethDev>& md);
+// A screening record: its model is a nucleotide model of k, and its model of each type (alt_model_ids[r * T + t]) is in range and
+// of that type's alphabet.
+int nph_screen_record_check(nph_ctx* ctx, uint32_t k, const std::vector<MethDev>& md, const uint32_t* alt_model_ids, size_t r,
+                            const nph_meth_record& R);
+
 #ifdef __CUDACC__
 // does a complete recognition site start at s[i]?  (is_motif_match reports complete sites only; the partial
 // matches match_to_site also knows — string end, string inside a site — never have the full length for len >= site_len)

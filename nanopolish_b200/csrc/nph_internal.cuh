@@ -225,6 +225,15 @@ struct nph_ctx {
         DevBuf<uint8_t> d_pairs;           // pairs, their variants, per job the difference score - log-sum
     } sup;
 
+    // the last nph_screen_variants_batch (screen_variants.cu)
+    struct ScreenListState {
+        NphEventRecords ev;                // region reference, compact event alignments, records
+        DevBuf<uint8_t> d_in;              // windows, sequences, the window's candidates, alleles, methylation tables and model ids
+        DevBuf<uint8_t> d_counts;          // per-window read counts and event sums, their offsets, job counts and offsets, scan scratch
+        DevBuf<uint8_t> d_pairs;           // the windows' reads
+        DevBuf<uint8_t> d_state;           // per-window round state, per-candidate state, methylated-alternative masks, counters
+    } sl;
+
     // the last nph_train_transitions_batch (transitions.cu)
     struct TtState {
         DevBuf<uint8_t> d_work;            // the group records, the refusal flags, the jobs' groups

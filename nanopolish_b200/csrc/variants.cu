@@ -380,6 +380,37 @@ ScreenStateLayout screen_state_layout(NphArena& a, size_t n_pos)
 
 } // namespace
 
+int nph_screen_types(nph_ctx* ctx, uint32_t k, const nph_screen_methylation& meth, size_t n_records, const uint32_t* alt_model_ids,
+                     std::vector<MethDev>& md)
+{
+    const uint32_t T = meth.n_types;
+    if (T > NPH_SCREEN_MAX_TYPES) { ctx->last_error = "nph_screen_methylation: more than NPH_SCREEN_MAX_TYPES types"; return NPH_ERR_INVALID; }
+    if (T && n_records && !alt_model_ids) return NPH_ERR_INVALID;
+    md.assign(T, MethDev{});
+    for (uint32_t t = 0; t < T; ++t) {
+        NPH_TRY(nph_meth_alphabet(ctx, meth.alphabets[t], md[t]));
+        if (md[t].k != k) { ctx->last_error = "nph_screen_methylation: type " + std::to_string(t) + " has k != params.k"; return NPH_ERR_INVALID; }
+    }
+    return NPH_OK;
+}
+
+int nph_screen_record_check(nph_ctx* ctx, uint32_t k, const std::vector<MethDev>& md, const uint32_t* alt_model_ids, size_t r,
+                            const nph_meth_record& R)
+{
+    const size_t T = md.size();
+    const DevModel& mod = ctx->models[R.model_id];
+    if (mod.k != k || mod.alphabet_size != 4) { ctx->last_error = "screening record " + std::to_string(r) + ": its model is not a nucleotide model of k = params.k"; return NPH_ERR_INVALID; }
+    for (size_t t = 0; t < T; ++t) {
+        const uint32_t id = alt_model_ids[r * T + t];
+        if (id >= ctx->models.size() || ctx->models[id].k != md[t].k || ctx->models[id].alphabet_size != md[t].asize) {
+            ctx->last_error = "screening record " + std::to_string(r) + ": its model of methylation type " + std::to_string(t) +
+                              " is out of range or not a model of that alphabet";
+            return NPH_ERR_INVALID;
+        }
+    }
+    return NPH_OK;
+}
+
 extern "C" int nph_screen_load_methylation(nph_ctx* ctx, const char* ref_bases, size_t n_ref_bases, const int16_t* event_deltas, size_t n_deltas_total,
                                            const int32_t* first_event, const nph_meth_record* records, size_t n_records,
                                            const nph_screen_params* params, double indel_bias,
@@ -393,27 +424,12 @@ extern "C" int nph_screen_load_methylation(nph_ctx* ctx, const char* ref_bases, 
     VarDev d;
     NPH_TRY(make_dev(ctx, *params, n_ref_bases, meth->n_types, d));
     const uint32_t T = meth->n_types;
-    if (T > NPH_SCREEN_MAX_TYPES) { ctx->last_error = "nph_screen_methylation: more than NPH_SCREEN_MAX_TYPES types"; return NPH_ERR_INVALID; }
-    if (T && n_records && !alt_model_ids) return NPH_ERR_INVALID;
-    std::vector<MethDev> md(T);
-    for (uint32_t t = 0; t < T; ++t) {
-        NPH_TRY(nph_meth_alphabet(ctx, meth->alphabets[t], md[t]));
-        if (md[t].k != params->k) { ctx->last_error = "nph_screen_methylation: type " + std::to_string(t) + " has k != params.k"; return NPH_ERR_INVALID; }
-    }
+    std::vector<MethDev> md;
+    NPH_TRY(nph_screen_types(ctx, params->k, *meth, n_records, alt_model_ids, md));
     // records index the event deltas, not the region's reference
     NPH_TRY(nph_event_records_load(ctx, m.ev, ref_bases, n_ref_bases, n_deltas_total, true, event_deltas, first_event, nullptr, 0,
                                    records, n_records, 0x3fffffffu, [&](size_t r, const nph_meth_record& R) {
-        const DevModel& mod = ctx->models[R.model_id];
-        if (mod.k != params->k || mod.alphabet_size != 4) { ctx->last_error = "screening record " + std::to_string(r) + ": its model is not a nucleotide model of k = params.k"; return NPH_ERR_INVALID; }
-        for (uint32_t t = 0; t < T; ++t) {
-            const uint32_t id = alt_model_ids[r * T + t];
-            if (id >= ctx->models.size() || ctx->models[id].k != md[t].k || ctx->models[id].alphabet_size != md[t].asize) {
-                ctx->last_error = "screening record " + std::to_string(r) + ": its model of methylation type " + std::to_string(t) +
-                                  " is out of range or not a model of that alphabet";
-                return NPH_ERR_INVALID;
-            }
-        }
-        return NPH_OK;
+        return nph_screen_record_check(ctx, params->k, md, alt_model_ids, r, R);
     }));
     m.h_meth.resize(sizeof(MethDev) * T);
     if (T) {

@@ -10,7 +10,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from .synth import ABEA_RES_DT, ALIGN_STATE_DT, CALIBRATION_DT, EVENT_DT, EVENT_RANGE_DT, METH_SITE_DT, METHFREQ_PARAMS_DT, HP_COUNTS_DT, HP_LIK_DT, HP_WINDOW_DT, PAIR_DT, PHASE_CALL_DT, PHASE_VARIANT_DT, POLYA_RES_DT, POLYI_RES_DT, RAW_RANGE_DT, SUPPORT_COUNTS_DT, SUPPORT_RESULT_DT, SUPPORT_VARIANT_DT
+from .synth import ABEA_RES_DT, ALIGN_STATE_DT, CALIBRATION_DT, EVENT_DT, EVENT_RANGE_DT, METH_SITE_DT, METHFREQ_PARAMS_DT, HP_COUNTS_DT, HP_LIK_DT, HP_WINDOW_DT, PAIR_DT, PHASE_CALL_DT, PHASE_VARIANT_DT, POLYA_RES_DT, POLYI_RES_DT, RAW_RANGE_DT, SCREEN_CANDIDATE_DT, SCREEN_LIST_COUNTS_DT, SCREEN_RESULT_DT, SUPPORT_COUNTS_DT, SUPPORT_RESULT_DT, SUPPORT_VARIANT_DT
 
 
 def _p(a):
@@ -221,6 +221,23 @@ class Engine:
                                                    indel_bias, _p(out), _p(cnt)),
                     "nph_all_support_batch")
         return out[:variants.shape[0]], cnt[0]
+
+    # ---- screen_variants_by_score on a candidate list (include/nph.h, nph_screen_variants_batch) ----
+    def screen_variants_batch(self, reads, ev_mean, ev_start_time, ref_bases, deltas, first_event, records, params, alleles, candidates,
+                              indel_bias: float = 1.0, methylation=None):
+        """records METH_RECORD_DT (compact event alignments, as screening's), params SCREEN_LIST_PARAMS_DT[1], alleles u1, candidates
+        SCREEN_CANDIDATE_DT, methylation None or (SCREEN_METH_DT[1], alt model ids n_records x n_types).  Returns
+        (SCREEN_RESULT_DT[n_candidates], SCREEN_LIST_COUNTS_DT scalar)."""
+        assert candidates.dtype == SCREEN_CANDIDATE_DT
+        out = np.zeros(max(candidates.shape[0], 1), SCREEN_RESULT_DT)
+        cnt = np.zeros(1, SCREEN_LIST_COUNTS_DT)
+        meth, ids = (None, None) if methylation is None else (methylation[0], np.ascontiguousarray(methylation[1], np.uint32))
+        self._check(self.lib.nph_screen_variants_batch(self.ctx, _p(reads), reads.shape[0], _p(ev_mean), _p(ev_start_time), ev_mean.shape[0],
+                                                       _p(ref_bases), ref_bases.shape[0], _p(deltas), deltas.shape[0], _p(first_event), _p(records),
+                                                       records.shape[0], _p(params), _p(alleles), alleles.shape[0], _p(candidates),
+                                                       candidates.shape[0], indel_bias, _p(meth), _p(ids), _p(out), _p(cnt)),
+                    "nph_screen_variants_batch")
+        return out[:candidates.shape[0]], cnt[0]
 
     def screen_load(self, ref_bases, deltas, first_event, records, params, indel_bias: float = 1.0, methylation=None):
         head = (self.ctx, _p(ref_bases), ref_bases.shape[0], _p(deltas), deltas.shape[0], _p(first_event), _p(records), records.shape[0], _p(params),

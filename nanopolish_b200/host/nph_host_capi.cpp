@@ -40,6 +40,43 @@ HMMInputData input_data(int read, const PoreModel* model, uint32_t e_start, uint
 }
 }
 
+namespace {
+RegionAlignments region_of(const char* contig, int region_start, const char* region_ref, int n_records, const int32_t* read, const uint8_t* rc,
+                           const int32_t* pairs, const uint64_t* pair_off)
+{
+    RegionAlignments region;
+    region.contig = contig; region.region_start = region_start; region.reference = region_ref;
+    for (int r = 0; r < n_records; ++r) {
+        EventAlignedRead e;
+        e.read = g_reads[read[r]].get();
+        e.contig = contig;
+        e.rc[0] = rc[r] != 0;
+        const uint64_t np = pair_off[r + 1] - pair_off[r];
+        e.aligned_events[0].resize(np);
+        if (np) std::memcpy(e.aligned_events[0].data(), pairs + 2 * pair_off[r], sizeof(AlignedPair) * np);
+        region.records.push_back(std::move(e));
+    }
+    return region;
+}
+
+std::vector<Variant> variants_of(const char* var_contig, int n_variants, const int32_t* var_pos, const char** var_ref, const char** var_alt)
+{
+    std::vector<Variant> variants(n_variants);
+    for (int i = 0; i < n_variants; ++i) {
+        variants[i].ref_name = var_contig; variants[i].ref_position = (size_t)var_pos[i];
+        variants[i].ref_seq = var_ref[i]; variants[i].alt_seq = var_alt[i];
+    }
+    return variants;
+}
+
+long long write_out(const std::string& s, char* out, size_t cap)
+{
+    if (s.size() + 1 > cap) throw Error(NPH_ERR_INVALID, "output buffer too small");
+    std::memcpy(out, s.c_str(), s.size() + 1);
+    return (long long)s.size();
+}
+} // namespace
+
 extern "C" {
 
 const char* nphh_last_error() { return g_err.c_str(); }
@@ -991,6 +1028,57 @@ long long nphh_all_support(const char* contig, int region_start, const char* reg
         if (s.size() + 1 > cap) throw Error(NPH_ERR_INVALID, "output buffer too small");
         std::memcpy(out, s.c_str(), s.size() + 1);
         n = (long long)s.size();
+    });
+    return st ? st : n;
+}
+
+// nph::screen_variants_by_score over the region and records of nphh_all_support, on the candidates {var_contig, var_pos[i], var_ref[i],
+// var_alt[i]} in order, with opt::methylation_types = types_csv split at commas ("" = none; the reads' models of each type are
+// registered with nphh_read_add_model).  out: one line per kept variant, "ref_position \t ref_seq \t alt_seq \t the 16 hex digits
+// of the quality's bits \t info".  Returns the length written, or a negative nph_status.
+long long nphh_screen_variants(const char* contig, int region_start, const char* region_ref, int n_records, const int32_t* read, const uint8_t* rc,
+                               const int32_t* pairs, const uint64_t* pair_off, const char* var_contig, int n_variants, const int32_t* var_pos,
+                               const char** var_ref, const char** var_alt, int flank, uint32_t score_threshold, const char* types_csv,
+                               uint32_t alignment_flags, double indel_bias, char* out, size_t cap)
+{
+    long long n = -1;
+    int st = guard([&] {
+        const RegionAlignments region = region_of(contig, region_start, region_ref, n_records, read, rc, pairs, pair_off);
+        std::vector<std::string> types;
+        for (std::string s = types_csv; !s.empty(); ) {
+            const size_t c = s.find(',');
+            types.push_back(s.substr(0, c));
+            s = c == std::string::npos ? std::string() : s.substr(c + 1);
+        }
+        const std::vector<Variant> kept = screen_variants_by_score(region, variants_of(var_contig, n_variants, var_pos, var_ref, var_alt),
+                                                                   alignment_flags, flank, score_threshold, types, Engine::thread_default(),
+                                                                   indel_bias);
+        std::string s;
+        char bits[17];
+        for (const Variant& v : kept) {
+            uint64_t u;
+            std::memcpy(&u, &v.quality, 8);
+            std::snprintf(bits, sizeof(bits), "%016llx", (unsigned long long)u);
+            s += std::to_string(v.ref_position) + "\t" + v.ref_seq + "\t" + v.alt_seq + "\t" + bits + "\t" + v.info + "\n";
+        }
+        n = write_out(s, out, cap);
+    });
+    return st ? st : n;
+}
+
+// nph::expand_variants over the region of nphh_all_support (no records) on the candidates {var_contig, var_pos[i], var_ref[i],
+// var_alt[i]}.  out: one line per output variant, "ref_position \t ref_seq \t alt_seq".  Returns the length written, or a negative
+// nph_status.
+long long nphh_expand_variants(const char* contig, int region_start, const char* region_ref, const char* var_contig, int n_variants,
+                               const int32_t* var_pos, const char** var_ref, const char** var_alt, int min_flank, char* out, size_t cap)
+{
+    long long n = -1;
+    int st = guard([&] {
+        const RegionAlignments region = region_of(contig, region_start, region_ref, 0, nullptr, nullptr, nullptr, nullptr);
+        std::string s;
+        for (const Variant& v : expand_variants(region, variants_of(var_contig, n_variants, var_pos, var_ref, var_alt), min_flank))
+            s += std::to_string(v.ref_position) + "\t" + v.ref_seq + "\t" + v.alt_seq + "\n";
+        n = write_out(s, out, cap);
     });
     return st ? st : n;
 }

@@ -459,4 +459,102 @@ void annotate_variants_with_all_support(std::vector<Variant>& input, const Regio
     }
 }
 
+std::vector<Variant> screen_variants_by_score(const RegionAlignments& alignments, const std::vector<Variant>& candidate_variants,
+                                              uint32_t alignment_flags, int flank, uint32_t score_threshold,
+                                              const std::vector<std::string>& methylation_types, Engine& engine, double indel_bias,
+                                              nph_screen_list_counts* counts_out)
+{
+    std::string alleles;
+    std::vector<nph_screen_candidate> dev(std::max<size_t>(candidate_variants.size(), 1));
+    for (size_t i = 0; i < candidate_variants.size(); ++i) {
+        const Variant& v = candidate_variants[i];
+        if (v.ref_position > (size_t)INT32_MAX)
+            throw Error(NPH_ERR_INVALID, "screen_variants_by_score: candidate " + std::to_string(i) + " lies beyond int32");
+        std::memset(&dev[i], 0, sizeof(dev[i]));
+        dev[i].ref_position = (int64_t)v.ref_position;
+        dev[i].ref_seq_len = (uint32_t)v.ref_seq.size();
+        dev[i].alt_seq_len = (uint32_t)v.alt_seq.size();
+        dev[i].ref_seq_off = alleles.size();
+        alleles += v.ref_seq;
+        dev[i].alt_seq_off = alleles.size();
+        alleles += v.alt_seq;
+    }
+    const RegionLayout rl = region_layout(alignments, engine, "screen_variants_by_score");
+    const detail::FlatReads& fr = rl.fr;
+    nph_screen_list_params params;
+    std::memset(&params, 0, sizeof(params));
+    params.region_start = alignments.region_start;
+    params.flank = flank;
+    params.score_threshold = score_threshold;
+    params.alignment_flags = alignment_flags;
+    // every record's base model has this k (the device call checks); the DNA models of the reads are 6-mers
+    params.k = alignments.records.empty() ? 6 : alignments.records[0].read->get_base_model(0)->k;
+    params.reads_per_round = 8;
+    // -q types: each alphabet, and per record the read's model of each type (SquiggleRead::get_model, as profile_hmm_score_set asks)
+    nph_screen_methylation meth;
+    std::memset(&meth, 0, sizeof(meth));
+    if (methylation_types.size() > NPH_SCREEN_MAX_TYPES) throw Error(NPH_ERR_INVALID, "screen_variants_by_score: more than NPH_SCREEN_MAX_TYPES methylation types");
+    meth.n_types = (uint32_t)methylation_types.size();
+    std::vector<uint32_t> alt_models;
+    for (size_t t = 0; t < methylation_types.size(); ++t) {
+        MethylationCallingParameters mp;
+        mp.methylation_type = methylation_types[t];
+        meth.alphabets[t] = make_meth_params(mp, params.k, 0, 0);
+    }
+    for (const EventAlignedRead& r : alignments.records)
+        for (const std::string& type : methylation_types) {
+            const PoreModel* m = r.read->get_model(0, type);
+            if (!m) throw Error(NPH_ERR_INVALID, "screen_variants_by_score: a read without a model of methylation type " + type);
+            alt_models.push_back(engine.model_id(m));
+        }
+    alt_models.push_back(0);
+    std::vector<nph_screen_result> out(std::max<size_t>(candidate_variants.size(), 1));
+    nph_screen_list_counts counts;
+    engine.check(nph_screen_variants_batch(engine.ctx(), fr.reads.data(), fr.reads.size(), fr.mean, rl.time.data(), fr.n_events,
+                                           alignments.reference.data(), alignments.reference.size(), rl.deltas.data(), rl.deltas.size(),
+                                           rl.first.data(), rl.recs.data(), rl.recs.size(), &params, alleles.data(), alleles.size(), dev.data(),
+                                           candidate_variants.size(), indel_bias, methylation_types.empty() ? nullptr : &meth, alt_models.data(),
+                                           out.data(), &counts),
+                 "nph_screen_variants_batch");
+    if (counts_out) *counts_out = counts;
+    std::vector<Variant> kept;
+    for (size_t i = 0; i < candidate_variants.size(); ++i) {
+        if (out[i].status == NPH_SCREEN_OUTSIDE || !(out[i].quality > 0)) continue;
+        Variant v = candidate_variants[i];
+        v.quality = out[i].quality;
+        v.info = "";
+        kept.push_back(v);
+    }
+    return kept;
+}
+
+std::vector<Variant> expand_variants(const RegionAlignments& alignments, const std::vector<Variant>& candidate_variants, int min_flanking_sequence)
+{
+    const int region_start = alignments.region_start;
+    const int region_end = alignments.region_start + (int)alignments.reference.size() - 1;
+    std::vector<Variant> out;
+    for (size_t vi = 0; vi < candidate_variants.size(); ++vi) {
+        const Variant& in = candidate_variants[vi];
+        out.push_back(in);
+        if (in.ref_seq.size() == 1 && in.alt_seq.size() == 1) continue;
+        // the deletion extended by one base, where it stays in the region and more than min_flanking_sequence bases from its end
+        const int start = (int)in.ref_position;
+        const int deletion_end = (int)(in.ref_position + in.ref_seq.size());
+        if (in.ref_name == alignments.contig && start >= region_start && deletion_end <= region_end &&
+            region_end - deletion_end > min_flanking_sequence) {
+            Variant v = in;
+            v.ref_seq = alignments.reference.substr((size_t)(start - region_start), (size_t)(deletion_end - start + 1));
+            if (v.ref_seq.compare(0, in.ref_seq.size(), in.ref_seq) != 0)
+                throw Error(NPH_ERR_INVALID, "expand_variants: candidate " + std::to_string(vi) + "'s ref_seq is not the region's (the reference asserts)");
+            out.push_back(v);
+        }
+        for (int j = 0; j < 4; ++j) {
+            Variant v = in;
+            v.alt_seq.append(1, "ACGT"[j]);
+            out.push_back(v);
+        }
+    }
+    return out;
+}
+
 } // namespace nph

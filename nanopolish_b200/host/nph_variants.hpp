@@ -10,6 +10,9 @@
 //                                                nph_homopolymer_likelihoods_batch)
 //   annotate_variants_with_all_support           ref: src/common/nanopolish_variant.cpp:801-859 (its scores on the device,
 //                                                nph_all_support_batch)
+//   screen_variants_by_score                     ref: src/nanopolish_call_variants.cpp:364-402 (on the device,
+//                                                nph_screen_variants_batch)
+//   expand_variants                              ref: src/nanopolish_call_variants.cpp:406-450 (host only)
 //
 // The reference scores one (read, sequence) pair per profile_hmm_score call inside an OpenMP loop.  Here every
 // (read, haplotype, alphabet alternative) triple of a whole candidate set becomes one job of ONE launch; the base
@@ -159,5 +162,24 @@ typedef HomopolymerRegion RegionAlignments;
 void annotate_variants_with_all_support(std::vector<Variant>& input, const RegionAlignments& alignments, int min_flanking_sequence,
                                         uint32_t alignment_flags, Engine& engine, double indel_bias = hmm_indel_bias_factor,
                                         nph_support_counts* counts_out = nullptr);
+
+// screen_variants_by_score (ref: src/nanopolish_call_variants.cpp:364-402) with opt::screen_flanking_sequence = flank,
+// opt::screen_score_threshold = score_threshold and opt::methylation_types = methylation_types: every candidate in its own window
+// [ref_position - flank, ref_position + |ref_seq| + flank], scored by score_variant_thresholded against the window's event
+// sequences, all candidates in one nph_screen_variants_batch.  Returns the candidates whose quality is > 0, in input order, with
+// their quality and INFO cleared; a window outside the region skips its candidate.  Like the reference, the contig of a candidate is
+// not checked.  Throws Error(NPH_ERR_INVALID) for a ref_position + |ref_seq| + flank beyond int32 (the reference narrows the window's
+// ends to int).  counts_out (optional): the device call's counters.
+std::vector<Variant> screen_variants_by_score(const RegionAlignments& alignments, const std::vector<Variant>& candidate_variants,
+                                              uint32_t alignment_flags, int flank, uint32_t score_threshold,
+                                              const std::vector<std::string>& methylation_types, Engine& engine,
+                                              double indel_bias = hmm_indel_bias_factor, nph_screen_list_counts* counts_out = nullptr);
+
+// expand_variants (ref: src/nanopolish_call_variants.cpp:406-450): each candidate, then for every one that is not a single-base
+// substitution its deletion extended by one reference base (only if [ref_position, ref_position + |ref_seq|] lies in the region on
+// the candidate's contig and region_end - (ref_position + |ref_seq|) > min_flanking_sequence) and its four insertions alt_seq + b,
+// b in ACGT.  Throws Error(NPH_ERR_INVALID) where the reference asserts: an extended deletion whose first |ref_seq| bases are not
+// ref_seq.
+std::vector<Variant> expand_variants(const RegionAlignments& alignments, const std::vector<Variant>& candidate_variants, int min_flanking_sequence);
 
 } // namespace nph

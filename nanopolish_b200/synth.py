@@ -867,6 +867,18 @@ SUPPORT_COUNTS_DT = np.dtype([("n_variants", "<u8"), ("n_pairs", "<u8"), ("n_job
 assert SUPPORT_PARAMS_DT.itemsize == 16 and SUPPORT_VARIANT_DT.itemsize == 16 and SUPPORT_RESULT_DT.itemsize == 40 and SUPPORT_COUNTS_DT.itemsize == 40
 
 
+# ---- screen_variants_by_score on a candidate list (nph_screen_variants_batch) --------------------------------------------------
+SCREEN_LIST_PARAMS_DT = np.dtype([("region_start", "<i4"), ("flank", "<i4"), ("score_threshold", "<u4"), ("alignment_flags", "<u4"), ("k", "<u4"),
+                                  ("reads_per_round", "<u4")], align=True)
+SCREEN_CANDIDATE_DT = np.dtype([("ref_position", "<i8"), ("ref_seq_len", "<u4"), ("alt_seq_len", "<u4"), ("ref_seq_off", "<u8"), ("alt_seq_off", "<u8")],
+                               align=True)
+SCREEN_RESULT_DT = np.dtype([("quality", "<f8"), ("n_reads", "<u4"), ("status", "<u4")], align=True)
+SCREEN_LIST_COUNTS_DT = np.dtype([("n_candidates", "<u8"), ("n_windows", "<u8"), ("n_rounds", "<u8"), ("n_jobs", "<u8"), ("n_dp_rows", "<u8"),
+                                  ("n_jobs_without_exit", "<u8"), ("n_reference_rows", "<u8"), ("kernel_ms", "<f8")], align=True)
+assert SCREEN_LIST_PARAMS_DT.itemsize == 24 and SCREEN_CANDIDATE_DT.itemsize == 32 and SCREEN_RESULT_DT.itemsize == 16 and SCREEN_LIST_COUNTS_DT.itemsize == 64
+SCREEN_SCREENED, SCREEN_OUTSIDE, SCREEN_NOT_APPLIED = 0, 1, 2
+
+
 # ---- methylation-aware screening (`variants -q cpg`, `-q dam,dcm`) -------------------------------------------------------
 SCREEN_METH_DT = np.dtype([("n_types", "<u4"), ("reserved", "<u4"), ("alphabets", METH_PARAMS_DT, 4)], align=True)
 assert SCREEN_METH_DT.itemsize == 616
