@@ -209,29 +209,31 @@ struct nph_ctx {
         DevBuf<nph_phase_call> d_calls;
     } phase;
 
+    // the batch of the last one-shot region call (nph_homopolymer_likelihoods_batch, nph_all_support_batch,
+    // nph_screen_variants_batch; window_reads.cu).  None of them is staged, so each may take over what the one before it left.
+    struct RegionState {
+        NphEventRecords ev;                // region reference, compact event alignments, records
+        DevBuf<uint8_t> d_counts;          // the windows' bounds, per-window counts, pair offsets, the scan's scratch, the largest rows
+        DevBuf<uint8_t> d_pairs;           // the windows' pairs and the window of each
+    } region;
+
     // the last nph_homopolymer_likelihoods_batch (homopolymer.cu)
     struct HpState {
-        NphEventRecords ev;                // region reference, compact event alignments, records
         DevBuf<uint8_t> d_in;              // windows, calling sequences, event durations
-        DevBuf<uint8_t> d_counts;          // per-window read counts, scored-pair offsets, the scan's scratch, two flags
-        DevBuf<uint8_t> d_pairs;           // scored pairs, their windows, per job the forward score and sum_duration
+        DevBuf<uint8_t> d_jobs;            // per job the forward score and sum_duration, the no-path flag
         DevBuf<uint8_t> d_states;          // one chunk's state offsets, state counts and Viterbi states
     } hp;
 
     // the last nph_all_support_batch (all_support.cu)
     struct SupportState {
-        NphEventRecords ev;                // region reference, compact event alignments, records
-        DevBuf<uint8_t> d_counts;          // per-variant windows, pair counts, their offsets, the scan's scratch
-        DevBuf<uint8_t> d_pairs;           // pairs, their variants, per job the difference score - log-sum
+        DevBuf<uint8_t> d_jobs;            // per variant its window, per job the difference score - log-sum
     } sup;
 
     // the last nph_screen_variants_batch (screen_variants.cu)
     struct ScreenListState {
-        NphEventRecords ev;                // region reference, compact event alignments, records
         DevBuf<uint8_t> d_in;              // windows, sequences, the window's candidates, alleles, methylation tables and model ids
-        DevBuf<uint8_t> d_counts;          // per-window read counts and event sums, their offsets, job counts and offsets, scan scratch
-        DevBuf<uint8_t> d_pairs;           // the windows' reads
-        DevBuf<uint8_t> d_state;           // per-window round state, per-candidate state, methylated-alternative masks, counters
+        DevBuf<uint8_t> d_state;           // per-window round state, job counts and offsets, scan scratch, per-candidate state,
+                                           // methylated-alternative masks, counters
     } sl;
 
     // the last nph_train_transitions_batch (transitions.cu)
@@ -438,6 +440,30 @@ constexpr int32_t NPH_NO_EVENT = INT32_MIN;
 // nph_scan_scratch(n) values from the caller's arena.
 size_t nph_scan_scratch(size_t n);
 int nph_scan_exclusive(nph_ctx* ctx, const uint64_t* in, uint32_t n, uint64_t* out, uint64_t* scratch);
+
+// One event sequence of a calling window: the record and its events e1 (window start) and e2 (window end).
+struct NphWinPair { uint32_t record; int32_t e1, e2; };
+// The profile HMM's DP rows of a pair's job: one per event of [e1, e2] or [e2, e1].
+__host__ __device__ inline uint32_t nph_pair_rows(int32_t e1, int32_t e2) { return (uint32_t)(e1 > e2 ? e1 - e2 : e2 - e1) + 1u; }
+
+// The region calls (window_reads.cu).  nph_region_load: nph_reads_load, then the records into ctx->region.ev in compact form
+// (records index the event deltas), each record also passing check(r, R).
+int nph_region_load(nph_ctx* ctx, const nph_read* reads, size_t n_reads, const float* ev_mean, const double* ev_start_time,
+                    size_t n_events_total, const char* ref, size_t n_ref, const int16_t* deltas, size_t n_deltas, const int32_t* first_event,
+                    const nph_meth_record* records, size_t n_records, const std::function<int(size_t, const nph_meth_record&)>& check);
+// What nph_window_reads found for n windows: AlignmentDB::get_event_subsequences of each, keeping the pairs with |e1 - e2| >= min_span.
+struct NphWindowReads {
+    std::vector<uint64_t> off;             // n + 1: each window's first kept pair, then their total
+    std::vector<uint32_t> met;             // per window: every event sequence found, kept or not
+    std::vector<uint64_t> rows;            // per window: nph_pair_rows summed over its kept pairs
+    uint32_t max_rows = 0;                 // the largest nph_pair_rows of a kept pair (0: none)
+    const uint64_t* d_off = nullptr;       // device copies of off, and the kept pairs window by window, each window's in record
+    const NphWinPair* d_pairs = nullptr;   // order, with the window of each pair
+    const uint32_t* d_pair_win = nullptr;
+    uint64_t n_pairs() const { return off.back(); }
+};
+// The reads of n >= 1 windows [bounds[w].x, bounds[w].y] over the records in ctx->region.ev: count, scan, one read-back, fill.
+int nph_window_reads(nph_ctx* ctx, const std::vector<int2>& bounds, int min_span, NphWindowReads& wr);
 // validate + classify + schedule the n_jobs jobs already sitting in ctx->d_jobs / d_ranks (one stream sync), size the scratch
 int nph_jobs_schedule(nph_ctx* ctx, size_t n_jobs, size_t n_ranks_total, NphJobSource src);
 // Scores n_jobs jobs that emit() writes into ctx->d_jobs (ranks already in ctx->d_ranks, written by a kernel of ours): reserves
@@ -511,7 +537,7 @@ int nph_check_ranks(nph_ctx* ctx, const uint32_t* d_ranks, size_t n, uint32_t n_
 #ifdef __CUDACC__
 // AlignmentDB::_find_by_ref_bounds (ref: src/alignment/nanopolish_alignment_db.cpp:688-731) on one record's dense event map
 // (event index per reference offset, NPH_NO_EVENT where aligned_events has no entry; fv its first offset with an entry) for the
-// window [cs, ce] in reference coordinates: the event indices at the two lower_bounds.  Variant screening and phase-reads call it.
+// window [cs, ce] in reference coordinates: the event indices at the two lower_bounds.  nph_event_subsequence and phase-reads call it.
 __device__ __forceinline__ int nph_first_valid_from(const int32_t* __restrict__ dense, int n, int from)
 {
     for (int o = from < 0 ? 0 : from; o < n; ++o) if (dense[o] != NPH_NO_EVENT) return o;
@@ -533,7 +559,8 @@ __device__ __forceinline__ bool nph_find_by_ref_bounds(const nph_meth_record& R,
     return true;
 }
 // AlignmentDB::get_event_subsequences (ref: src/alignment/nanopolish_alignment_db.cpp:172-221) for one record and the window
-// [cs, ce]: nph_find_by_ref_bounds plus the event/bp ratio test.  Variant screening and homopolymer fixing call it.
+// [cs, ce]: nph_find_by_ref_bounds plus the event/bp ratio test.  The edit screen's var_bounds_kernel and the window-read walk of the
+// region calls (window_reads.cu) call it.
 __device__ __forceinline__ bool nph_event_subsequence(const nph_meth_record& R, const int32_t* __restrict__ dense, int fv, int cs, int ce,
                                                       int& e1, int& e2)
 {
@@ -554,5 +581,28 @@ __device__ __forceinline__ void nph_dna_kmer_ranks(const uint8_t* codes, int q, 
         r = r * 4u + (3u - codes[q + k - 1 - t]);
     }
     fw = f; rc = r;
+}
+// The job header of pair P of record R; the caller fills in rank_off, model_id and n_kmers.
+__device__ __forceinline__ nph_hmm_job nph_window_job(const nph_meth_record& R, const NphWinPair& P, uint8_t flags)
+{
+    nph_hmm_job jb;
+    jb.read = R.read;
+    jb.event_start = (uint32_t)P.e1; jb.event_stop = (uint32_t)P.e2;
+    jb.stride = R.rc ? -1 : 1;          // EventAlignmentRecord::stride agrees with rc for every read the HMM accepts (profile_hmm_r9.inl:275)
+    jb.rc = R.rc; jb.flags = flags; jb.reserved = 0;
+    return jb;
+}
+// HMMInputSequence::get_kmer_rank(q, k, rc) of the DNA alphabet, one k-mer at a time, for the nk k-mers of an edited window whose
+// base v has the nph_dna_code code(v): the ranks of strand rc into rk
+template <typename Code>
+__device__ __forceinline__ void nph_window_ranks(Code code, int nk, int k, bool rc, uint32_t* rk)
+{
+    for (int q = 0; q < nk; ++q) {
+        uint8_t c[8];
+        for (int i = 0; i < k; ++i) c[i] = code(q + i);
+        uint32_t f, r;
+        nph_dna_kmer_ranks(c, 0, k, f, r);
+        rk[q] = rc ? r : f;
+    }
 }
 #endif

@@ -89,7 +89,7 @@ __global__ void __launch_bounds__(kThreads) phase_count_kernel(const PhaseArgs a
             int e1 = 0, e2 = 0;
             const bool s = v < hi && phase_site(a, R, dense, fv, a.variants[v], e1, e2);
             count += __popc(__ballot_sync(kFull, s));
-            if (s) ev += 2ull * (unsigned long long)((e2 > e1 ? e2 - e1 : e1 - e2) + 1);
+            if (s) ev += 2ull * nph_pair_rows(e1, e2);
         }
         for (int o = 16; o; o >>= 1) ev += __shfl_xor_sync(kFull, ev, o);
         if (lane == 0) {

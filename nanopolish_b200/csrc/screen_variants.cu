@@ -3,17 +3,14 @@
 //
 // Replaces, for a whole candidate list at once:
 //   screen_variants_by_score                  ref: src/nanopolish_call_variants.cpp:364-402
-//   AlignmentDB::get_event_subsequences       ref: src/alignment/nanopolish_alignment_db.cpp:172-221 (nph_event_subsequence, shared
-//                                             with the edit screen, homopolymer fixing and all-support)
+//   AlignmentDB::get_event_subsequences       ref: src/alignment/nanopolish_alignment_db.cpp:172-221 (nph_window_reads)
 //   Haplotype::apply_variant on the window    ref: src/nanopolish_haplotype.cpp:33-75 (decided on the host, per candidate)
 //   score_variant_thresholded                 ref: src/common/nanopolish_variant.cpp:765-799, with the -q sets of
 //                                             generate_methylated_alternatives (:158-178) as nph_screen_load_methylation forms them
 //
-// Candidates with the same window (calling_start, |ref_seq|) share its reads and base haplotype.  Kernels, in the count -> scan ->
-// fill shape of all_support.cu, then the round loop of variants.cu:
-//   sv_pairs_kernel<false>  a warp per window, the records 32 at a time: the window's event sequences and their event rows
-//   (nph_scan_exclusive: each window's first pair; one read-back sizes the pairs)
-//   sv_pairs_kernel<true>   the same walk, writing the pairs {record, e1, e2} in record order
+// Candidates with the same window (calling_start, |ref_seq|) share its reads and base haplotype.  Kernels, after the window-read
+// walk of window_reads.cu (count -> scan -> fill: each window's event sequences and their event rows), then the round loop of
+// variants.cu:
 //   sv_ranks_kernel         a warp per (sequence, alternative): the k-mer ranks of both strands into a variable-length pool (the
 //                           base window of every window, the edited window of every candidate that applies), and whether the
 //                           methylated copy of each type differs from its sequence
@@ -39,8 +36,6 @@ constexpr int kThreads = kWarps * 32;
 constexpr unsigned kFull = 0xffffffffu;
 constexpr uint32_t kNoSeq = 0xffffffffu;
 
-struct SvPair { uint32_t record; int32_t e1, e2; };
-
 // a window: [cs, cs + len - 1], its candidates wcand[cand_first, cand_first + n_cand), its base sequence
 struct SvWin { int32_t cs, len; uint32_t cand_first, n_cand, base_seq, pad; };
 
@@ -59,15 +54,13 @@ struct SvCounters { unsigned long long events, ref_events; unsigned int any_left
 
 struct SvArgs {
     const nph_meth_record* records;
-    const int32_t* dense;
-    const int32_t* first_valid;
     const SvWin* wins;
     const SvSeq* seqs;
     const uint32_t* wcand;
     SvCand* cands;
     const uint8_t* ref;                 // the region reference
     const uint8_t* alleles;
-    uint32_t n_records, n_wins, n_seqs;
+    uint32_t n_wins, n_seqs;
     int flank, k, T, rpr;
     uint32_t flags;
     double threshold;
@@ -83,39 +76,6 @@ struct SvMeth {
 };
 
 __device__ __forceinline__ uint32_t set_size(uint32_t mask) { return 1u + (uint32_t)__popc(mask); }
-
-// FILL = false: per window the number of event sequences and their event rows; FILL = true: the pairs
-template <bool FILL>
-__global__ void __launch_bounds__(kThreads) sv_pairs_kernel(const SvArgs a, uint64_t* __restrict__ n_pairs, unsigned long long* __restrict__ sum_e,
-                                                            const uint64_t* __restrict__ pair_off, SvPair* __restrict__ pairs)
-{
-    const int lane = threadIdx.x & 31;
-    const uint32_t warp = blockIdx.x * kWarps + (threadIdx.x >> 5);
-    const uint32_t n_warps = gridDim.x * kWarps;
-    for (uint32_t wi = warp; wi < a.n_wins; wi += n_warps) {
-        const int cs = a.wins[wi].cs, ce = cs + a.wins[wi].len - 1;
-        uint64_t n = 0;
-        unsigned long long e = 0;
-        SvPair* out = FILL ? pairs + pair_off[wi] : nullptr;
-        for (uint32_t base = 0; base < a.n_records; base += 32) {
-            const uint32_t r = base + lane;
-            int e1 = 0, e2 = 0;
-            bool in = false;
-            if (r < a.n_records) {
-                const nph_meth_record R = a.records[r];
-                in = nph_event_subsequence(R, a.dense + R.ref_off, a.first_valid[r], cs, ce, e1, e2);
-            }
-            const unsigned m = __ballot_sync(kFull, in);
-            if (FILL && in) out[n + __popc(m & ((1u << lane) - 1u))] = SvPair{r, e1, e2};
-            if (in) e += (unsigned long long)(e1 > e2 ? e1 - e2 : e2 - e1) + 1ull;
-            n += __popc(m);
-        }
-        if (!FILL) {
-            for (int o = 16; o; o >>= 1) e += __shfl_xor_sync(kFull, e, o);
-            if (lane == 0) { n_pairs[wi] = n; sum_e[wi] = e; }
-        }
-    }
-}
 
 // character i of sequence S
 __device__ __forceinline__ uint8_t seq_char(const SvArgs& a, const SvSeq& S, int i)
@@ -236,7 +196,7 @@ __device__ __forceinline__ nph_hmm_job* emit_set(const SvArgs& a, const SvMeth& 
 }
 
 __global__ void sv_emit_kernel(const SvArgs a, const SvWinState* __restrict__ ws, const uint64_t* __restrict__ pair_off,
-                               const SvPair* __restrict__ pairs, const uint64_t* __restrict__ job_off, nph_hmm_job* __restrict__ jobs,
+                               const NphWinPair* __restrict__ pairs, const uint64_t* __restrict__ job_off, nph_hmm_job* __restrict__ jobs,
                                unsigned long long* __restrict__ events, const SvMeth sm)
 {
     const uint32_t wi = blockIdx.x * blockDim.x + threadIdx.x;
@@ -244,23 +204,19 @@ __global__ void sv_emit_kernel(const SvArgs a, const SvWinState* __restrict__ ws
     if (wi < a.n_wins && ws[wi].chunk) {
         const SvWinState s = ws[wi];
         const SvWin W = a.wins[wi];
-        const SvPair* rd = pairs + pair_off[wi] + s.done;
+        const NphWinPair* rd = pairs + pair_off[wi] + s.done;
         nph_hmm_job* out = jobs + job_off[wi];
         for (uint32_t r = 0; r < s.chunk; ++r) {
-            const SvPair P = rd[r];
+            const NphWinPair P = rd[r];
             const nph_meth_record R = a.records[P.record];
-            nph_hmm_job jb;
-            jb.read = R.read;
-            jb.event_start = (uint32_t)P.e1; jb.event_stop = (uint32_t)P.e2;
-            jb.stride = R.rc ? -1 : 1;                    // EventAlignmentRecord::stride agrees with rc for every read the HMM accepts
-            jb.rc = R.rc; jb.flags = (uint8_t)a.flags; jb.reserved = 0;
+            const nph_hmm_job jb = nph_window_job(R, P, (uint8_t)a.flags);
             nph_hmm_job* const first = out;
             out = emit_set(a, sm, jb, R, P.record, W.base_seq, out);
             for (uint32_t c = 0; c < W.n_cand; ++c) {
                 const SvCand& C = a.cands[a.wcand[W.cand_first + c]];
                 if (C.alive) out = emit_set(a, sm, jb, R, P.record, C.seq, out);
             }
-            ev += (unsigned long long)(out - first) * ((unsigned long long)(P.e1 > P.e2 ? P.e1 - P.e2 : P.e2 - P.e1) + 1ull);
+            ev += (unsigned long long)(out - first) * nph_pair_rows(P.e1, P.e2);
         }
     }
     for (int o = 16; o; o >>= 1) ev += __shfl_xor_sync(kFull, ev, o);
@@ -270,7 +226,7 @@ __global__ void sv_emit_kernel(const SvArgs a, const SvWinState* __restrict__ ws
 // thread per window: the round's reads in order, per read the base set's fold once and, for every live candidate, the sequential
 // `if (fabs(total) < threshold) total += variant - base` (var_accumulate_kernel's arithmetic, NaN included)
 __global__ void sv_accumulate_kernel(const SvArgs a, SvWinState* __restrict__ ws, const uint64_t* __restrict__ pair_off,
-                                     const SvPair* __restrict__ pairs, const uint64_t* __restrict__ job_off, const float* __restrict__ scores,
+                                     const NphWinPair* __restrict__ pairs, const uint64_t* __restrict__ job_off, const float* __restrict__ scores,
                                      SvCounters* __restrict__ ctr, const SvMeth sm)
 {
     const uint32_t wi = blockIdx.x * blockDim.x + threadIdx.x;
@@ -279,14 +235,14 @@ __global__ void sv_accumulate_kernel(const SvArgs a, SvWinState* __restrict__ ws
     if (!s.chunk) return;
     const SvWin W = a.wins[wi];
     const float* sc = scores + job_off[wi];
-    const SvPair* rd = pairs + pair_off[wi] + s.done;
+    const NphWinPair* rd = pairs + pair_off[wi] + s.done;
     const uint32_t nb = set_size(a.T ? sm.alts[W.base_seq] : 0u);
     unsigned long long ref_ev = 0;
     for (uint32_t r = 0; r < s.chunk; ++r) {
         // double base_score = profile_hmm_score_set(...) (a float); a set of one is its score
         const double base_score = (double)nph_score_set_fold(sc, nb, sm.pen[nb - 1], sm.tbl);
         sc += nb;
-        const unsigned long long E = (unsigned long long)(rd[r].e1 > rd[r].e2 ? rd[r].e1 - rd[r].e2 : rd[r].e2 - rd[r].e1) + 1ull;
+        const unsigned long long E = nph_pair_rows(rd[r].e1, rd[r].e2);
         for (uint32_t c = 0; c < W.n_cand; ++c) {
             SvCand& C = a.cands[a.wcand[W.cand_first + c]];
             if (!C.alive) continue;
@@ -428,10 +384,8 @@ extern "C" int nph_screen_variants_batch(nph_ctx* ctx, const nph_read* reads, si
     nph_ctx::ScreenListState& ss = ctx->sl;
     const size_t n_wins = pl.wins.size(), n_seqs = pl.seqs.size(), n_cand = n_candidates;
     const auto run = [&]() -> int {
-        NPH_TRY(nph_reads_load(ctx, reads, n_reads, ev_mean, ev_start_time, n_events_total));
-        // records index the event deltas, as the edit screen's do
-        NPH_TRY(nph_event_records_load(ctx, ss.ev, ref_bases, n_ref_bases, n_deltas_total, true, event_deltas, first_event, nullptr, 0,
-                                       records, n_records, 0x3fffffffu, [&](size_t r, const nph_meth_record& R) {
+        NPH_TRY(nph_region_load(ctx, reads, n_reads, ev_mean, ev_start_time, n_events_total, ref_bases, n_ref_bases, event_deltas, n_deltas_total,
+                                first_event, records, n_records, [&](size_t r, const nph_meth_record& R) {
             return nph_screen_record_check(ctx, p.k, md, alt_model_ids, r, R);
         }));
         cudaStream_t st = ctx->stream;
@@ -444,18 +398,12 @@ extern "C" int nph_screen_variants_batch(nph_ctx* ctx, const nph_read* reads, si
             d_meth = c.take<MethDev>((size_t)T + 1);
             d_alt_models = c.take<uint32_t>(n_records * (size_t)T + 1);
         }));
-        uint64_t* d_n; unsigned long long* d_sum_e; uint64_t* d_off; uint64_t* d_job_cnt; uint64_t* d_job_off; uint64_t* d_scratch;
-        NPH_TRY(nph_carve(ctx, ss.d_counts, [&](NphArena& c) {
-            d_n = c.take<uint64_t>(n_wins);
-            d_sum_e = c.take<unsigned long long>(n_wins);
-            d_off = c.take<uint64_t>(n_wins + 1);
+        SvWinState* d_ws; uint64_t* d_job_cnt; uint64_t* d_job_off; uint64_t* d_scratch; SvCand* d_cands; uint32_t* d_alts; SvCounters* d_ctr;
+        NPH_TRY(nph_carve(ctx, ss.d_state, [&](NphArena& c) {
+            d_ws = c.take<SvWinState>(n_wins);
             d_job_cnt = c.take<uint64_t>(n_wins);
             d_job_off = c.take<uint64_t>(n_wins + 1);
             d_scratch = c.take<uint64_t>(nph_scan_scratch(n_wins));
-        }));
-        SvWinState* d_ws; SvCand* d_cands; uint32_t* d_alts; SvCounters* d_ctr;
-        NPH_TRY(nph_carve(ctx, ss.d_state, [&](NphArena& c) {
-            d_ws = c.take<SvWinState>(n_wins);
             d_cands = c.take<SvCand>(n_cand);
             d_alts = c.take<uint32_t>(n_seqs);
             d_ctr = c.take<SvCounters>(1);
@@ -475,29 +423,19 @@ extern "C" int nph_screen_variants_batch(nph_ctx* ctx, const nph_read* reads, si
         NPH_CUDA(ctx, cudaMemsetAsync(d_ws, 0, sizeof(SvWinState) * n_wins, st));
         NPH_CUDA(ctx, cudaMemsetAsync(d_alts, 0, sizeof(uint32_t) * n_seqs, st));
         NPH_CUDA(ctx, cudaMemsetAsync(d_ctr, 0, sizeof(SvCounters), st));
-        const int32_t* dense;
-        const int32_t* first_valid;
-        NPH_TRY(nph_event_records_expand(ctx, ss.ev, &dense, &first_valid));
-        SvArgs a{ss.ev.d_records.p, dense, first_valid, d_wins, d_seqs, d_wcand, d_cands, ss.ev.d_ref.p, d_alleles, (uint32_t)n_records,
-                 (uint32_t)n_wins, (uint32_t)n_seqs, p.flank, (int)p.k, T, (int)p.reads_per_round, p.alignment_flags, (double)p.score_threshold};
+        SvArgs a{ctx->region.ev.d_records.p, d_wins, d_seqs, d_wcand, d_cands, ctx->region.ev.d_ref.p, d_alleles, (uint32_t)n_wins,
+                 (uint32_t)n_seqs, p.flank, (int)p.k, T, (int)p.reads_per_round, p.alignment_flags, (double)p.score_threshold};
         SvMeth sm{};
         sm.types = d_meth; sm.alt_model = d_alt_models; sm.alts = d_alts; sm.tbl = ctx->d_logsum.p;
         for (int n = 1; n <= 1 + T; ++n) sm.pen[n - 1] = log((double)n);      // profile_hmm_score_set's log(num_models), host libm
         // the windows' reads
-        const int grid = (int)std::min<size_t>((n_wins + kWarps - 1) / kWarps, (size_t)ctx->sm_count * 8);
-        sv_pairs_kernel<false><<<grid, kThreads, 0, st>>>(a, d_n, d_sum_e, nullptr, nullptr);
-        NPH_CUDA(ctx, cudaGetLastError());
-        NPH_TRY(nph_scan_exclusive(ctx, d_n, (uint32_t)n_wins, d_off, d_scratch));
-        std::vector<uint64_t> off(n_wins + 1);
-        NPH_CUDA(ctx, cudaMemcpyAsync(off.data(), d_off, sizeof(uint64_t) * (n_wins + 1), cudaMemcpyDeviceToHost, st));
-        NPH_CUDA(ctx, cudaStreamSynchronize(st));                     // the one read-back that sizes the pairs
-        const uint64_t n_pairs = off[n_wins];
-        NPH_TRY(nph_reserve(ctx, ss.d_pairs, sizeof(SvPair) * (size_t)(n_pairs + 1)));
-        SvPair* d_pairs = reinterpret_cast<SvPair*>(ss.d_pairs.p);
-        if (n_pairs) {
-            sv_pairs_kernel<true><<<grid, kThreads, 0, st>>>(a, nullptr, nullptr, d_off, d_pairs);
-            NPH_CUDA(ctx, cudaGetLastError());
-        }
+        std::vector<int2> bounds(n_wins);
+        for (size_t w = 0; w < n_wins; ++w) bounds[w] = make_int2(pl.wins[w].cs, pl.wins[w].cs + pl.wins[w].len - 1);
+        NphWindowReads wr;
+        NPH_TRY(nph_window_reads(ctx, bounds, 0, wr));
+        const std::vector<uint64_t>& off = wr.off;
+        const uint64_t* d_off = wr.d_off;
+        const NphWinPair* d_pairs = wr.d_pairs;
         NPH_TRY(nph_reserve(ctx, ctx->d_ranks, (size_t)pl.pool));
         const size_t n_items = n_seqs * (size_t)(1 + T);
         const int rgrid = (int)std::min<size_t>((n_items + kWarps - 1) / kWarps, (size_t)ctx->sm_count * 16);
@@ -528,11 +466,9 @@ extern "C" int nph_screen_variants_batch(nph_ctx* ctx, const nph_read* reads, si
         }
         std::vector<SvCand> h_cands(n_cand);
         std::vector<uint32_t> h_alts(n_seqs);
-        std::vector<unsigned long long> h_sum_e(n_wins);
         SvCounters h_ctr{};
         NPH_CUDA(ctx, cudaMemcpyAsync(h_cands.data(), d_cands, sizeof(SvCand) * n_cand, cudaMemcpyDeviceToHost, st));
         NPH_CUDA(ctx, cudaMemcpyAsync(h_alts.data(), d_alts, sizeof(uint32_t) * n_seqs, cudaMemcpyDeviceToHost, st));
-        NPH_CUDA(ctx, cudaMemcpyAsync(h_sum_e.data(), d_sum_e, sizeof(unsigned long long) * n_wins, cudaMemcpyDeviceToHost, st));
         NPH_CUDA(ctx, cudaMemcpyAsync(&h_ctr, d_ctr, sizeof(h_ctr), cudaMemcpyDeviceToHost, st));
         NPH_CUDA(ctx, cudaStreamSynchronize(st));
         finish(off, h_cands);
@@ -548,7 +484,7 @@ extern "C" int nph_screen_variants_batch(nph_ctx* ctx, const nph_read* reads, si
             bool any = false;
             for (uint32_t c = 0; c < W.n_cand; ++c) {
                 const uint32_t i = pl.wcand[W.cand_first + c];
-                if (!pl.applied[i]) { if (0.0 < thr) cnt.n_reference_rows += 2u * nb * h_sum_e[w]; continue; }
+                if (!pl.applied[i]) { if (0.0 < thr) cnt.n_reference_rows += 2u * nb * wr.rows[w]; continue; }
                 any = true;
                 per_read += 1u + (uint64_t)__builtin_popcount(h_alts[pl.cands[i].seq]);
             }

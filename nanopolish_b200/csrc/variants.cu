@@ -35,8 +35,6 @@ constexpr int kSeqs = NPH_SCREEN_SLOTS + 1;      // nine candidates + the base h
 constexpr int kBlock = 256;
 constexpr int kListCap = 2048;                   // records overlapping one block of positions, kept in shared memory
 
-struct PosRead { uint32_t record; int32_t e1, e2; };
-
 struct PosState {
     double total[NPH_SCREEN_SLOTS];
     uint32_t valid;       // bit c: candidate c exists (bit 31: the position is screened at all)
@@ -80,7 +78,7 @@ template <bool FILL>
 __global__ void __launch_bounds__(kBlock) var_bounds_kernel(const VarDev d, const nph_meth_record* __restrict__ records, uint32_t n_records,
                                                             const int32_t* __restrict__ dense, const int32_t* __restrict__ first_valid,
                                                             uint64_t* __restrict__ counts, const uint64_t* __restrict__ pos_off,
-                                                            PosRead* __restrict__ pos_reads)
+                                                            NphWinPair* __restrict__ pos_reads)
 {
     __shared__ uint32_t s_list[kListCap];
     __shared__ uint32_t s_n, s_warp[kBlock / 32];
@@ -119,7 +117,7 @@ __global__ void __launch_bounds__(kBlock) var_bounds_kernel(const VarDev d, cons
     const int cs = i - d.flank, ce = i + 1 + d.flank;
     const bool pos_ok = cs >= d.region_start && ce <= d.region_start + d.n_ref - 1;       // are_coordinates_valid
     uint64_t cnt = 0;
-    PosRead* out = FILL ? pos_reads + pos_off[pi] : nullptr;
+    NphWinPair* out = FILL ? pos_reads + pos_off[pi] : nullptr;
     if (pos_ok) {
         const uint32_t n_it = use_list ? s_n : n_records;
         for (uint32_t t = 0; t < n_it; ++t) {
@@ -127,7 +125,7 @@ __global__ void __launch_bounds__(kBlock) var_bounds_kernel(const VarDev d, cons
             const nph_meth_record R = records[r];
             int e1, e2;
             if (nph_event_subsequence(R, dense + R.ref_off, first_valid[r], cs, ce, e1, e2)) {
-                if (FILL) out[cnt] = PosRead{r, e1, e2};
+                if (FILL) out[cnt] = NphWinPair{r, e1, e2};
                 ++cnt;
             }
         }
@@ -239,7 +237,7 @@ __global__ void var_round_count_kernel(const VarDev d, PosState* __restrict__ st
 }
 
 __global__ void var_emit_kernel(const VarDev d, const PosState* __restrict__ state, const uint64_t* __restrict__ pos_off,
-                                const PosRead* __restrict__ pos_reads, const nph_meth_record* __restrict__ records,
+                                const NphWinPair* __restrict__ pos_reads, const nph_meth_record* __restrict__ records,
                                 const uint64_t* __restrict__ job_off, nph_hmm_job* __restrict__ jobs, unsigned long long* __restrict__ events,
                                 const VarMeth vm)
 {
@@ -249,17 +247,13 @@ __global__ void var_emit_kernel(const VarDev d, const PosState* __restrict__ sta
         const PosState st = state[pi];
         if (st.chunk) {
             const unsigned long long am = d.T ? vm.alts[pi] : 0ull;
-            const PosRead* rd = pos_reads + pos_off[pi] + st.done;
+            const NphWinPair* rd = pos_reads + pos_off[pi] + st.done;
             nph_hmm_job* out = jobs + job_off[pi];
             for (uint32_t r = 0; r < st.chunk; ++r) {
-                const PosRead pr = rd[r];
+                const NphWinPair pr = rd[r];
                 const nph_meth_record R = records[pr.record];
-                nph_hmm_job jb;
-                jb.read = R.read;
-                jb.event_start = (uint32_t)pr.e1; jb.event_stop = (uint32_t)pr.e2;
-                jb.stride = R.rc ? -1 : 1;                    // EventAlignmentRecord::stride agrees with rc for every read the HMM accepts (profile_hmm_r9.inl:275)
-                jb.rc = R.rc; jb.flags = (uint8_t)d.flags; jb.reserved = 0;
-                const unsigned long long E = (unsigned long long)(pr.e1 > pr.e2 ? pr.e1 - pr.e2 : pr.e2 - pr.e1) + 1ull;
+                nph_hmm_job jb = nph_window_job(R, pr, (uint8_t)d.flags);
+                const unsigned long long E = nph_pair_rows(pr.e1, pr.e2);
                 // the base haplotype first, then the live candidates in slot order; each sequence followed by its methylated copies
                 // in type order (generate_methylated_alternatives)
                 for (int seq = NPH_SCREEN_SLOTS; ; ) {
@@ -286,7 +280,7 @@ __global__ void var_emit_kernel(const VarDev d, const PosState* __restrict__ sta
 
 __global__ void var_accumulate_kernel(const VarDev d, PosState* __restrict__ state, const uint64_t* __restrict__ job_off,
                                       const float* __restrict__ scores, unsigned int* __restrict__ any_left, const uint64_t* __restrict__ pos_off,
-                                      const PosRead* __restrict__ pos_reads, unsigned long long* __restrict__ ref_events, const VarMeth vm)
+                                      const NphWinPair* __restrict__ pos_reads, unsigned long long* __restrict__ ref_events, const VarMeth vm)
 {
     const int pi = blockIdx.x * blockDim.x + threadIdx.x;
     if (pi >= d.n_pos) return;
@@ -294,7 +288,7 @@ __global__ void var_accumulate_kernel(const VarDev d, PosState* __restrict__ sta
     if (!st.chunk) return;
     const unsigned long long am = d.T ? vm.alts[pi] : 0ull;
     const float* s = scores + job_off[pi];
-    const PosRead* rd = pos_reads + pos_off[pi] + st.done;
+    const NphWinPair* rd = pos_reads + pos_off[pi] + st.done;
     const double thr = (double)d.threshold;
     const uint32_t nb = set_size(am, NPH_SCREEN_SLOTS, d.T);
     unsigned long long ref_ev = 0;
@@ -302,7 +296,7 @@ __global__ void var_accumulate_kernel(const VarDev d, PosState* __restrict__ sta
         // double base_score = profile_hmm_score_set(...) (a float); a set of one is its score
         const double base_score = (double)nph_score_set_fold(s, nb, vm.pen[nb - 1], vm.tbl);
         s += nb;
-        const unsigned long long E = (unsigned long long)(rd[r].e1 > rd[r].e2 ? rd[r].e1 - rd[r].e2 : rd[r].e2 - rd[r].e1) + 1ull;
+        const unsigned long long E = nph_pair_rows(rd[r].e1, rd[r].e2);
         for (int c = 0; c < NPH_SCREEN_SLOTS; ++c) {
             if (!((st.alive >> c) & 1u)) continue;
             const uint32_t nc = set_size(am, c, d.T);
@@ -485,8 +479,8 @@ extern "C" int nph_screen_run(nph_ctx* ctx)
     uint64_t n_pos_reads = 0;
     NPH_CUDA(ctx, cudaMemcpyAsync(&n_pos_reads, m.d_pos_off.p + n_pos, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
     NPH_CUDA(ctx, cudaStreamSynchronize(st));
-    NPH_TRY(nph_reserve(ctx, m.d_pos_reads, sizeof(PosRead) * ((size_t)n_pos_reads + 1)));
-    PosRead* pos_reads = reinterpret_cast<PosRead*>(m.d_pos_reads.p);
+    NPH_TRY(nph_reserve(ctx, m.d_pos_reads, sizeof(NphWinPair) * ((size_t)n_pos_reads + 1)));
+    NphWinPair* pos_reads = reinterpret_cast<NphWinPair*>(m.d_pos_reads.p);
     var_bounds_kernel<true><<<pgrid, kBlock, 0, st>>>(d, records, n_rec, dense, first_valid, nullptr, m.d_pos_off.p, pos_reads);
     NPH_CUDA(ctx, cudaGetLastError());
     // rank pool (K1's d_ranks for this batch: per position, sequence and alternative both strands) and position state

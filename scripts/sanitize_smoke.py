@@ -76,4 +76,11 @@ for env in ({"NPH_EVENTS_WPR": "1"}, {"NPH_EVENTS_WPR": "2"}, {"NPH_EVENTS_WPR":
     assert all(x.tobytes() == y.tobytes() for x, y in zip(evs, ev2))
     for k_ in env: del os.environ[k_]
 print("round-2 kernels ok", sites1.shape[0], int(np.isfinite(q).sum()), [x.shape[0] for x in evs])
+# the region calls of `variants` over one window-read walk: fix-homopolymers, all-support and list screening
+from tests import hp_cases as hc, screen_cases as scc, support_cases as suc
+_, hcnt = hc.device(eng, hc.build(hc.CASES[1]))
+_, ucnt = suc.device(eng, suc.build(suc.CASES[0]))
+_, lcnt = scc.device(eng, scc.build(scc.CASES[1]))
+assert int(hcnt["n_pairs"]) > 0 and int(ucnt["n_pairs"]) > 0 and int(lcnt["n_jobs"]) > 0
+print("region calls ok", int(hcnt["n_pairs"]), int(ucnt["n_pairs"]), int(lcnt["n_jobs"]))
 eng.close()

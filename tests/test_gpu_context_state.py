@@ -232,6 +232,43 @@ def test_kernel_time_needs_a_timed_call(ctx):
     assert launches >= 1 and ms > 0.0
 
 
+def test_region_calls_reuse_one_batch_state(ctx):
+    """All-support, fix-homopolymers and list screening share one batch state (records and the window-read walk's buffers).  Run
+    one after another between a staged edit screen's run and its fetch, on a large pile-up, then a small one, then a medium one,
+    every result and counter is bit-equal to the same call on a fresh context, and so is the edit screen's."""
+    from tests import hp_cases as hc
+    from tests import screen_cases as scc
+    from tests import support_cases as suc
+    rs, ref_chars, deltas, first, recs, params = _screen_inputs()
+    sup, hp, lst = suc.random_case(61), hc.build(hc.CASES[1]), scc.build(scc.CASES[1])
+    calls = [lambda e: suc.device(e, sup), lambda e: hc.device(e, hp), lambda e: scc.device(e, lst)]
+
+    def edit_screen_run(e):
+        e.reads_load(rs.reads, rs.ev_mean, rs.ev_start_time)
+        e.screen_load(ref_chars, deltas, first, recs, params)
+        e.screen_run()
+
+    def bits(res, cnt):
+        return res.tobytes(), {f: int(cnt[f]) for f in cnt.dtype.names if not f.endswith("_ms")}
+
+    want = []
+    for call in calls + [None]:
+        fresh = _fresh()
+        try:
+            if call is None:
+                edit_screen_run(fresh)
+                want.append(tuple(x.tobytes() for x in fresh.screen_fetch()))
+            else:
+                want.append(bits(*call(fresh)))
+        finally:
+            fresh.close()
+    edit_screen_run(ctx)
+    got = [bits(*call(ctx)) for call in calls]
+    got.append(tuple(x.tobytes() for x in ctx.screen_fetch()))
+    assert got == want
+    assert want[0][1]["n_pairs"] > want[1][1]["n_pairs"] > 0 and want[2][1]["n_jobs"] > 0
+
+
 @pytest.mark.parametrize("device_jobs", ["methylation", "screening"])
 def test_device_written_jobs_do_not_vouch_for_host_jobs(ctx, device_jobs):
     if device_jobs == "methylation":
