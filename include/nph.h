@@ -1028,6 +1028,88 @@ int nph_screen_variants_batch(nph_ctx* ctx, const nph_read* reads, size_t n_read
                               const nph_screen_methylation* meth, const uint32_t* alt_model_ids,
                               nph_screen_result* out, nph_screen_list_counts* counts_out);
 
+/* ---- variants: the haplotype scores and genotype choice of call_haplotype_from_candidates ------------------------------------
+ * (ref: src/nanopolish_call_variants.cpp:782-880, score_variant_group and simple_call of src/common/nanopolish_variant.cpp:182-493)
+ * The caller groups the candidates and builds each group's haplotypes: combination c of group g is haplotype hap_first + c, its
+ * bases haplotype_bases[seq_off, seq_off + seq_len) and its variant ids (group-local, < n_variants) combination_variants[var_off, ..).
+ * Combination 0 is the empty one (the base haplotype); every other combination names at least one variant.  Per group, on one OpenMP
+ * thread's semantics:
+ *   the reads     get_event_subsequences(calling_start, calling_end) in record order, as nph_screen_variants_batch walks them
+ *   the keys      VariantGroup keys a read by "read_name:strand".  key_rank[read] is the rank of that string among the call's reads
+ *                 (equal strings, equal ranks): a group's keys are its distinct ranks, ascending.  Per key, s[c][key] is the score
+ *                 of its last record, read_sum[key] the add_logs chain over (record, combination) in order, is_rc the last record's
+ *   the scores    s = profile_hmm_score_set(generate_methylated_alternatives(haplotype, -q types), record, alignment_flags), a float
+ *   the sets      the multisets of ploidy combination ids in Combinations(n, ploidy, CO_WITH_REPLACEMENT) order (non-decreasing
+ *                 tuples, lexicographic); set_score = sum over keys of add_logs(..., s - log(2)) chained from -inf; best = the first
+ *                 set whose score exceeds the best so far (from -inf), base = set 0.  best - base < 20 keeps the base set
+ *   per variant   the posterior exp(s - read_sum) summed per (key, variant) and per variant in simple_call's loop order, the strand
+ *                 sums (1 - pp, pp) and the variant's count in the best set
+ * The device runs the walk, K1, the key fold and the genotype search; exp and the sums run on the host with its libm (host_ms).
+ * Records, meth and alt_model_ids: as nph_screen_variants_batch takes them.  NPH_ERR_INVALID: k outside 1..8; ploidy outside
+ * 1..NPH_CALL_MAX_PLOIDY; alignment_flags other than NPH_HAF_*; a group with fewer than 2 haplotypes or fewer than ploidy (the
+ * reference's Combinations asserts), a window outside the region or
+ * calling_start > calling_end, a haplotype or variant range outside its array; a haplotype with fewer than k bases, its bases or
+ * variant ids outside their arrays, a variant id >= the group's n_variants, a non-empty combination 0 or an empty later one; more
+ * than 2^60 genotype sets in a group; a record, model or -q type the screening calls refuse; a job the forward scorer refuses. */
+#define NPH_CALL_MAX_PLOIDY 8
+#define NPH_CALL_CALLED    0u         /* best - base >= 20 (or a NaN difference): the best set stands */
+#define NPH_CALL_BASE_KEPT 1u         /* best - base < 20: the base set is the call */
+#define NPH_CALL_NO_BEST   2u         /* no set scored above -inf: no best set, every count is 0 */
+typedef struct {
+    int32_t  region_start;            /* AlignmentDB::m_region_start */
+    uint32_t ploidy;                  /* opt::ploidy */
+    uint32_t genotype_all;            /* opt::genotype_only: emit every variant, not only those with var_count > 0 */
+    uint32_t alignment_flags;         /* NPH_HAF_* (variants: NPH_HAF_ALLOW_PRE_CLIP | NPH_HAF_ALLOW_POST_CLIP) */
+    uint32_t k;                       /* the reads' base-model k */
+} nph_call_params;                    /* 20 bytes */
+typedef struct {
+    int32_t  calling_start, calling_end;   /* the group's window in reference coordinates */
+    uint32_t hap_first, n_haplotypes;      /* haplotypes [hap_first, hap_first + n_haplotypes): one per combination */
+    uint32_t var_first, n_variants;        /* results of variants [var_first, var_first + n_variants) go to variants_out */
+} nph_call_group;                     /* 24 bytes */
+typedef struct {
+    uint64_t seq_off;                 /* first base in haplotype_bases[] */
+    uint32_t seq_len;                 /* bases */
+    uint32_t n_var;                   /* variant ids of its combination */
+    uint64_t var_off;                 /* first id in combination_variants[] */
+} nph_call_haplotype;                 /* 24 bytes */
+typedef struct {
+    uint32_t n_keys, n_combinations;  /* TotalReads; combinations (= n_haplotypes) */
+    uint32_t status;                  /* NPH_CALL_* */
+    uint32_t ploidy;                  /* entries of best_set written (0 with NPH_CALL_NO_BEST) */
+    uint32_t best_set[NPH_CALL_MAX_PLOIDY];   /* the called set's combination ids (the base set's zeros after NPH_CALL_BASE_KEPT) */
+    double   best_score, base_score;  /* the highest set score (-inf: none) and set 0's */
+} nph_call_group_result;              /* 64 bytes */
+typedef struct {
+    uint32_t var_count;               /* AlleleCount: the variant's occurrences in the called set */
+    uint32_t emit;                    /* genotype_all || var_count > 0: simple_call outputs it */
+    double   support_sum;             /* read_variant_support: SupportFraction = support_sum / n_keys */
+    double   strand[4];               /* ref_fwd, ref_rev, alt_fwd, alt_rev */
+} nph_call_variant_result;            /* 48 bytes */
+typedef struct {
+    uint64_t n_groups, n_haplotypes;  /* groups; haplotypes over all groups */
+    uint64_t n_pairs;                 /* (group, event sequence) pairs */
+    uint64_t n_jobs, n_dp_rows;       /* forward jobs (one per pair, haplotype and alternative) and their event rows */
+    uint64_t n_sets, n_set_terms;     /* genotype sets over all groups; sets x keys */
+    double   forward_ms;              /* device time of the forward kernels */
+    double   genotype_ms;             /* device time of the genotype kernels */
+    double   host_ms;                 /* the host's exp and sums */
+} nph_call_counts;                    /* 80 bytes */
+int nph_call_variant_groups_batch(nph_ctx* ctx, const nph_read* reads, size_t n_reads,
+                                  const float* ev_mean, const double* ev_start_time, size_t n_events_total,
+                                  const char* ref_bases, size_t n_ref_bases,
+                                  const int16_t* event_deltas, size_t n_deltas_total, const int32_t* first_event,
+                                  const nph_meth_record* records, size_t n_records, const uint32_t* key_rank,
+                                  const nph_call_params* params,
+                                  const nph_call_group* groups, size_t n_groups,
+                                  const nph_call_haplotype* haplotypes, size_t n_haplotypes,
+                                  const char* haplotype_bases, size_t n_bases,
+                                  const uint32_t* combination_variants, size_t n_combination_variants,
+                                  size_t n_variants, double indel_bias,
+                                  const nph_screen_methylation* meth, const uint32_t* alt_model_ids,
+                                  nph_call_group_result* groups_out, nph_call_variant_result* variants_out,
+                                  nph_call_counts* counts_out);
+
 /* ---- scorereads --train-transitions: forward scores and transition training counts of a job batch ----------------------------
  * `nanopolish scorereads --train-transitions` runs, for every segment model_score scores (src/nanopolish_scorereads.cpp:116-203),
  * profile_hmm_align(sequence, data) (K3, flags 0) after the forward score, and folds the path into

@@ -210,7 +210,8 @@ struct nph_ctx {
     } phase;
 
     // the batch of the last one-shot region call (nph_homopolymer_likelihoods_batch, nph_all_support_batch,
-    // nph_screen_variants_batch; window_reads.cu).  None of them is staged, so each may take over what the one before it left.
+    // nph_screen_variants_batch, nph_call_variant_groups_batch; window_reads.cu).  None of them is staged, so each may take over
+    // what the one before it left.
     struct RegionState {
         NphEventRecords ev;                // region reference, compact event alignments, records
         DevBuf<uint8_t> d_counts;          // the windows' bounds, per-window counts, pair offsets, the scan's scratch, the largest rows
@@ -235,6 +236,12 @@ struct nph_ctx {
         DevBuf<uint8_t> d_state;           // per-window round state, job counts and offsets, scan scratch, per-candidate state,
                                            // methylated-alternative masks, counters
     } sl;
+
+    // the last nph_call_variant_groups_batch (call_variants.cu)
+    struct CallState {
+        DevBuf<uint8_t> d_in;              // groups, haplotypes, their bases and variant ids, key ranks, methylation tables and model ids
+        DevBuf<uint8_t> d_work;            // per-group offsets, masks, pair scores, key tables, partial maxima, group results
+    } call;
 
     // the last nph_train_transitions_batch (transitions.cu)
     struct TtState {

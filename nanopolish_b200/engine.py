@@ -10,7 +10,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from .synth import ABEA_RES_DT, ALIGN_STATE_DT, CALIBRATION_DT, EVENT_DT, EVENT_RANGE_DT, METH_SITE_DT, METHFREQ_PARAMS_DT, HP_COUNTS_DT, HP_LIK_DT, HP_WINDOW_DT, PAIR_DT, PHASE_CALL_DT, PHASE_VARIANT_DT, POLYA_RES_DT, POLYI_RES_DT, RAW_RANGE_DT, SCREEN_CANDIDATE_DT, SCREEN_LIST_COUNTS_DT, SCREEN_RESULT_DT, SUPPORT_COUNTS_DT, SUPPORT_RESULT_DT, SUPPORT_VARIANT_DT
+from .synth import CALL_COUNTS_DT, CALL_GROUP_DT, CALL_GROUP_RESULT_DT, CALL_HAPLOTYPE_DT, CALL_VARIANT_RESULT_DT, ABEA_RES_DT, ALIGN_STATE_DT, CALIBRATION_DT, EVENT_DT, EVENT_RANGE_DT, METH_SITE_DT, METHFREQ_PARAMS_DT, HP_COUNTS_DT, HP_LIK_DT, HP_WINDOW_DT, PAIR_DT, PHASE_CALL_DT, PHASE_VARIANT_DT, POLYA_RES_DT, POLYI_RES_DT, RAW_RANGE_DT, SCREEN_CANDIDATE_DT, SCREEN_LIST_COUNTS_DT, SCREEN_RESULT_DT, SUPPORT_COUNTS_DT, SUPPORT_RESULT_DT, SUPPORT_VARIANT_DT
 
 
 def _p(a):
@@ -238,6 +238,27 @@ class Engine:
                                                        candidates.shape[0], indel_bias, _p(meth), _p(ids), _p(out), _p(cnt)),
                     "nph_screen_variants_batch")
         return out[:candidates.shape[0]], cnt[0]
+
+    def call_variant_groups_batch(self, reads, ev_mean, ev_start_time, ref_bases, deltas, first_event, records, key_rank, params, groups,
+                                  haplotypes, bases, combination_variants, n_variants: int, indel_bias: float = 1.0, methylation=None):
+        """records METH_RECORD_DT (compact event alignments, as screening's), key_rank u4 per read (the rank of its "name:strand"), params
+        CALL_PARAMS_DT[1], groups CALL_GROUP_DT, haplotypes CALL_HAPLOTYPE_DT, bases u1, combination_variants u4, methylation None or
+        (SCREEN_METH_DT[1], alt model ids n_records x n_types).  Returns (CALL_GROUP_RESULT_DT[n_groups], CALL_VARIANT_RESULT_DT[n_variants],
+        CALL_COUNTS_DT scalar)."""
+        assert groups.dtype == CALL_GROUP_DT and haplotypes.dtype == CALL_HAPLOTYPE_DT
+        gout = np.zeros(max(groups.shape[0], 1), CALL_GROUP_RESULT_DT)
+        vout = np.zeros(max(n_variants, 1), CALL_VARIANT_RESULT_DT)
+        cnt = np.zeros(1, CALL_COUNTS_DT)
+        kr = np.ascontiguousarray(key_rank, np.uint32)
+        cv = np.ascontiguousarray(combination_variants, np.uint32)
+        meth, ids = (None, None) if methylation is None else (methylation[0], np.ascontiguousarray(methylation[1], np.uint32))
+        self._check(self.lib.nph_call_variant_groups_batch(self.ctx, _p(reads), reads.shape[0], _p(ev_mean), _p(ev_start_time), ev_mean.shape[0],
+                                                           _p(ref_bases), ref_bases.shape[0], _p(deltas), deltas.shape[0], _p(first_event),
+                                                           _p(records), records.shape[0], _p(kr), _p(params), _p(groups), groups.shape[0],
+                                                           _p(haplotypes), haplotypes.shape[0], _p(bases), bases.shape[0], _p(cv), cv.shape[0],
+                                                           n_variants, indel_bias, _p(meth), _p(ids), _p(gout), _p(vout), _p(cnt)),
+                    "nph_call_variant_groups_batch")
+        return gout[:groups.shape[0]], vout[:n_variants], cnt[0]
 
     def screen_load(self, ref_bases, deltas, first_event, records, params, indel_bias: float = 1.0, methylation=None):
         head = (self.ctx, _p(ref_bases), ref_bases.shape[0], _p(deltas), deltas.shape[0], _p(first_event), _p(records), records.shape[0], _p(params),

@@ -1066,6 +1066,45 @@ long long nphh_screen_variants(const char* contig, int region_start, const char*
     return st ? st : n;
 }
 
+// nph::call_haplotype_from_candidates over the region of nphh_all_support, record r's read named read_names[r], on the candidates
+// {var_contig, var_pos[i], var_ref[i], var_alt[i]} with types_csv the -q types ("" = none).  out: the derived sequence, then one line
+// per variant of the derived haplotype, "ref_position \t ref_seq \t alt_seq \t the 16 hex digits of the quality's bits \t info \t
+// genotype".  Returns the length written, or a negative nph_status.
+long long nphh_call_haplotype(const char* contig, int region_start, const char* region_ref, int n_records, const int32_t* read, const uint8_t* rc,
+                              const int32_t* pairs, const uint64_t* pair_off, const char** read_names, const char* var_contig, int n_variants,
+                              const int32_t* var_pos, const char** var_ref, const char** var_alt, int flank, int min_distance, int max_haplotypes,
+                              int ploidy, int genotype_only, const char* types_csv, int calculate_all_support, uint32_t alignment_flags,
+                              double indel_bias, char* out, size_t cap)
+{
+    long long n = -1;
+    int st = guard([&] {
+        for (int r = 0; r < n_records; ++r) g_reads[read[r]]->read_name = read_names[r];
+        const RegionAlignments region = region_of(contig, region_start, region_ref, n_records, read, rc, pairs, pair_off);
+        std::vector<std::string> types;
+        for (std::string s = types_csv; !s.empty(); ) {
+            const size_t c = s.find(',');
+            types.push_back(s.substr(0, c));
+            s = c == std::string::npos ? std::string() : s.substr(c + 1);
+        }
+        const Haplotype derived = call_haplotype_from_candidates(region, variants_of(var_contig, n_variants, var_pos, var_ref, var_alt), alignment_flags,
+                                                                 flank, min_distance, max_haplotypes, ploidy, genotype_only != 0, types,
+                                                                 calculate_all_support != 0, Engine::thread_default(), indel_bias);
+        std::string s = derived.get_sequence() + "\n";
+        char bits[17];
+        for (const Variant& v : derived.get_variants()) {
+            uint64_t u;
+            std::memcpy(&u, &v.quality, 8);
+            std::snprintf(bits, sizeof(bits), "%016llx", (unsigned long long)u);
+            s += std::to_string(v.ref_position) + "\t" + v.ref_seq + "\t" + v.alt_seq + "\t" + bits + "\t" + v.info + "\t" + v.genotype + "\n";
+        }
+        n = write_out(s, out, cap);
+    });
+    return st ? st : n;
+}
+
+// nph::fisher_exact_two_sided
+double nphh_fisher_exact(int n11, int n12, int n21, int n22) { return fisher_exact_two_sided(n11, n12, n21, n22); }
+
 // nph::expand_variants over the region of nphh_all_support (no records) on the candidates {var_contig, var_pos[i], var_ref[i],
 // var_alt[i]}.  out: one line per output variant, "ref_position \t ref_seq \t alt_seq".  Returns the length written, or a negative
 // nph_status.

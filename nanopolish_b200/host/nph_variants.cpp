@@ -1,6 +1,7 @@
 // nph_variants.cpp — see nph_variants.hpp (SURVEY.md section 8f, row N2).
 #include "nph_variants.hpp"
 
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <iomanip>
@@ -165,9 +166,7 @@ size_t nChoosek(size_t n, size_t k)
     return (size_t)result;
 }
 
-VariantGroupScores score_variant_group(const std::vector<Variant>& variants, const Haplotype& base_haplotype,
-                                       const std::vector<HMMInputData>& input, int max_haplotypes, uint32_t alignment_flags,
-                                       const std::vector<std::string>& methylation_types, Engine& engine, double indel_bias)
+VariantCombinations variant_combinations(const std::vector<Variant>& variants, const Haplotype& base_haplotype, int max_haplotypes)
 {
     const size_t num_variants = variants.size();
     // the largest number of variants that can be tested jointly without exceeding max_haplotypes
@@ -179,9 +178,8 @@ VariantGroupScores score_variant_group(const std::vector<Variant>& variants, con
         max_r += 1;
     }
     max_r -= 1;
-    VariantGroupScores out;
+    VariantCombinations out;
     out.max_r = max_r;
-    std::vector<Haplotype> haplotypes;
     for (size_t r = 0; r <= max_r; ++r) {
         std::vector<size_t> idx(r);
         for (size_t i = 0; i < r; ++i) idx[i] = i;
@@ -189,7 +187,7 @@ VariantGroupScores score_variant_group(const std::vector<Variant>& variants, con
             Haplotype current = base_haplotype;
             std::vector<Variant> subset;
             for (size_t i : idx) subset.push_back(variants[i]);
-            if (current.apply_variants(subset)) { out.combinations.push_back(idx); haplotypes.push_back(current); }
+            if (current.apply_variants(subset)) { out.combinations.push_back(idx); out.haplotypes.push_back(current); }
             // next r-subset of {0..n-1} in lexicographic order
             int i = (int)r - 1;
             while (i >= 0 && idx[i] == num_variants - r + (size_t)i) --i;
@@ -198,6 +196,18 @@ VariantGroupScores score_variant_group(const std::vector<Variant>& variants, con
             for (size_t j = (size_t)i + 1; j < r; ++j) idx[j] = idx[j - 1] + 1;
         }
     }
+    return out;
+}
+
+VariantGroupScores score_variant_group(const std::vector<Variant>& variants, const Haplotype& base_haplotype,
+                                       const std::vector<HMMInputData>& input, int max_haplotypes, uint32_t alignment_flags,
+                                       const std::vector<std::string>& methylation_types, Engine& engine, double indel_bias)
+{
+    VariantCombinations vc = variant_combinations(variants, base_haplotype, max_haplotypes);
+    VariantGroupScores out;
+    out.max_r = vc.max_r;
+    out.combinations = std::move(vc.combinations);
+    const std::vector<Haplotype>& haplotypes = vc.haplotypes;
     const std::vector<std::vector<double>> by_read = score_haplotypes(haplotypes, input, alignment_flags, methylation_types, engine, indel_bias);
     out.scores.assign(haplotypes.size(), std::vector<double>(input.size()));
     for (size_t ri = 0; ri < input.size(); ++ri)
@@ -348,6 +358,28 @@ RegionLayout region_layout(const HomopolymerRegion& region, Engine& engine, cons
     return rl;
 }
 
+// The -q types as the device calls take them: each alphabet, and per record the read's model of each type (SquiggleRead::get_model,
+// as profile_hmm_score_set asks), plus one trailing id so that the array is never empty
+void methylation_args(const RegionAlignments& alignments, const std::vector<std::string>& methylation_types, uint32_t k, Engine& engine,
+                      const char* caller, nph_screen_methylation& meth, std::vector<uint32_t>& alt_models)
+{
+    std::memset(&meth, 0, sizeof(meth));
+    if (methylation_types.size() > NPH_SCREEN_MAX_TYPES) throw Error(NPH_ERR_INVALID, std::string(caller) + ": more than NPH_SCREEN_MAX_TYPES methylation types");
+    meth.n_types = (uint32_t)methylation_types.size();
+    for (size_t t = 0; t < methylation_types.size(); ++t) {
+        MethylationCallingParameters mp;
+        mp.methylation_type = methylation_types[t];
+        meth.alphabets[t] = make_meth_params(mp, k, 0, 0);
+    }
+    for (const EventAlignedRead& r : alignments.records)
+        for (const std::string& type : methylation_types) {
+            const PoreModel* m = r.read->get_model(0, type);
+            if (!m) throw Error(NPH_ERR_INVALID, std::string(caller) + ": a read without a model of methylation type " + type);
+            alt_models.push_back(engine.model_id(m));
+        }
+    alt_models.push_back(0);
+}
+
 } // namespace
 
 Haplotype fix_homopolymers(const Haplotype& input, const HomopolymerRegion& region, int min_flanking_sequence, Engine& engine, double indel_bias,
@@ -490,24 +522,9 @@ std::vector<Variant> screen_variants_by_score(const RegionAlignments& alignments
     // every record's base model has this k (the device call checks); the DNA models of the reads are 6-mers
     params.k = alignments.records.empty() ? 6 : alignments.records[0].read->get_base_model(0)->k;
     params.reads_per_round = 8;
-    // -q types: each alphabet, and per record the read's model of each type (SquiggleRead::get_model, as profile_hmm_score_set asks)
     nph_screen_methylation meth;
-    std::memset(&meth, 0, sizeof(meth));
-    if (methylation_types.size() > NPH_SCREEN_MAX_TYPES) throw Error(NPH_ERR_INVALID, "screen_variants_by_score: more than NPH_SCREEN_MAX_TYPES methylation types");
-    meth.n_types = (uint32_t)methylation_types.size();
     std::vector<uint32_t> alt_models;
-    for (size_t t = 0; t < methylation_types.size(); ++t) {
-        MethylationCallingParameters mp;
-        mp.methylation_type = methylation_types[t];
-        meth.alphabets[t] = make_meth_params(mp, params.k, 0, 0);
-    }
-    for (const EventAlignedRead& r : alignments.records)
-        for (const std::string& type : methylation_types) {
-            const PoreModel* m = r.read->get_model(0, type);
-            if (!m) throw Error(NPH_ERR_INVALID, "screen_variants_by_score: a read without a model of methylation type " + type);
-            alt_models.push_back(engine.model_id(m));
-        }
-    alt_models.push_back(0);
+    methylation_args(alignments, methylation_types, params.k, engine, "screen_variants_by_score", meth, alt_models);
     std::vector<nph_screen_result> out(std::max<size_t>(candidate_variants.size(), 1));
     nph_screen_list_counts counts;
     engine.check(nph_screen_variants_batch(engine.ctx(), fr.reads.data(), fr.reads.size(), fr.mean, rl.time.data(), fr.n_events,
@@ -555,6 +572,209 @@ std::vector<Variant> expand_variants(const RegionAlignments& alignments, const s
         }
     }
     return out;
+}
+
+namespace {
+
+// The probability of the 2x2 table whose first cell is x, its margins fixed: exp of log-binomials, or, when x is next to the
+// previous x and neither a multiple of 11 nor a table with an empty fourth cell, the previous probability times the ratio of the
+// two tables' probabilities, in kt_fisher_exact's operation order
+struct TableProbability {
+    int row1, col1, n, x;
+    double p;
+    static double log_choose(int a, int b) { return (b == 0 || a == b) ? 0 : std::lgamma(a + 1) - std::lgamma(b + 1) - std::lgamma(a - b + 1); }
+    double direct(int v) const { return std::exp(log_choose(row1, v) + log_choose(n - row1, col1 - v) - log_choose(n, col1)); }
+    double at(int v)
+    {
+        const int n22 = v + n - row1 - col1;
+        if (v % 11 && n22) {
+            if (v == x + 1) { p *= (double)(row1 - x) / v * (col1 - x) / n22; x = v; return p; }
+            if (v == x - 1) { p *= (double)x / (row1 - v) * (x + n - row1 - col1) / (col1 - v); x = v; return p; }
+        }
+        x = v;
+        p = direct(v);
+        return p;
+    }
+};
+
+std::string format_double(double v)
+{
+    std::stringstream ss;
+    ss << v;
+    return ss.str();
+}
+
+} // namespace
+
+double fisher_exact_two_sided(int n11, int n12, int n21, int n22)
+{
+    const int row1 = n11 + n12, col1 = n11 + n21, n = n11 + n12 + n21 + n22;
+    const int hi = col1 < row1 ? col1 : row1;
+    const int lo = std::max(0, row1 + col1 - n);
+    if (lo == hi) return 1.0;
+    TableProbability t{row1, col1, n, n11, 0.0};
+    t.p = t.direct(n11);
+    const double q = t.p;
+    double left = 0.0, right = 0.0;
+    double p = t.at(lo);
+    for (int i = lo + 1; p < 0.99999999 * q; ++i) { left += p; p = t.at(i); }
+    if (p < 1.00000001 * q) left += p;
+    p = t.at(hi);
+    for (int j = hi - 1; p < 0.99999999 * q; --j) { right += p; p = t.at(j); }
+    if (p < 1.00000001 * q) right += p;
+    const double two = left + right;
+    return two > 1.0 ? 1.0 : two;
+}
+
+double calculate_sor(double ref_fwd, double ref_rev, double alt_fwd, double alt_rev)
+{
+    ref_fwd += 1; ref_rev += 1; alt_fwd += 1; alt_rev += 1;                    // no zeros
+    const double r = (ref_fwd * alt_rev) / (alt_fwd * ref_rev);
+    const double sym_ratio = r + (1.0 / r);
+    const double ref_ratio = std::min(ref_fwd, ref_rev) / std::max(ref_fwd, ref_rev);
+    const double alt_ratio = std::min(alt_fwd, alt_rev) / std::max(alt_fwd, alt_rev);
+    return std::log(sym_ratio) + std::log(ref_ratio) - std::log(alt_ratio);
+}
+
+std::string make_genotype(size_t alt_alleles, size_t ploidy)
+{
+    if (alt_alleles > ploidy) throw Error(NPH_ERR_INVALID, "make_genotype: more alternative alleles than the ploidy");
+    std::string out(2 * ploidy - 1, '/');
+    for (size_t a = 0; a < ploidy; ++a) out[2 * a] = a < ploidy - alt_alleles ? '0' : '1';
+    return out;
+}
+
+Haplotype call_haplotype_from_candidates(const RegionAlignments& alignments, const std::vector<Variant>& candidate_variants,
+                                         uint32_t alignment_flags, int flank, int min_distance, int max_haplotypes, int ploidy,
+                                         bool genotype_only, const std::vector<std::string>& methylation_types, bool calculate_all_support,
+                                         Engine& engine, double indel_bias, nph_call_counts* counts_out)
+{
+    const Haplotype region_haplotype(alignments.contig, (size_t)alignments.region_start, alignments.reference);
+    for (size_t i = 0; i < candidate_variants.size(); ++i)
+        if (candidate_variants[i].ref_position > (size_t)INT32_MAX)
+            throw Error(NPH_ERR_INVALID, "call_haplotype_from_candidates: candidate " + std::to_string(i) + " lies beyond int32");
+    // the groups of :790-854 that get called, with their combinations
+    struct Group { size_t first, n; VariantCombinations vc; };
+    std::vector<Group> called;
+    std::vector<nph_call_group> dev_groups;
+    std::vector<nph_call_haplotype> dev_haps;
+    std::string bases;
+    std::vector<uint32_t> cvars;
+    size_t n_var_results = 0;
+    for (size_t cur = 0; cur < candidate_variants.size();) {
+        size_t end = cur + 1;
+        while (end < candidate_variants.size()) {
+            const int distance = (int)candidate_variants[end].ref_position - (int)candidate_variants[end - 1].ref_position;
+            if (distance > min_distance) break;
+            end++;
+        }
+        const int calling_start = (int)candidate_variants[cur].ref_position - flank;
+        const int calling_end = (int)(candidate_variants[end - 1].ref_position + candidate_variants[end - 1].ref_seq.length()) + flank;
+        if (calling_end - calling_start <= 200) {
+            if (calling_start < 0) throw Error(NPH_ERR_INVALID, "call_haplotype_from_candidates: a window before the contig's start");
+            const Haplotype calling = region_haplotype.substr_by_reference((size_t)calling_start, (size_t)calling_end);
+            const std::vector<Variant> vs(candidate_variants.begin() + cur, candidate_variants.begin() + end);
+            Group g{cur, end - cur, variant_combinations(vs, calling, max_haplotypes)};
+            if (g.vc.combinations.size() > 1) {                                   // simple_call skips a group with one combination
+                nph_call_group d;
+                std::memset(&d, 0, sizeof(d));
+                d.calling_start = calling_start; d.calling_end = calling_end;
+                d.hap_first = (uint32_t)dev_haps.size(); d.n_haplotypes = (uint32_t)g.vc.combinations.size();
+                d.var_first = (uint32_t)n_var_results; d.n_variants = (uint32_t)g.n;
+                n_var_results += g.n;
+                for (size_t c = 0; c < g.vc.combinations.size(); ++c) {
+                    nph_call_haplotype h;
+                    std::memset(&h, 0, sizeof(h));
+                    const std::string& seq = g.vc.haplotypes[c].get_sequence();
+                    h.seq_off = bases.size(); h.seq_len = (uint32_t)seq.size();
+                    h.var_off = cvars.size(); h.n_var = (uint32_t)g.vc.combinations[c].size();
+                    bases += seq;
+                    for (size_t id : g.vc.combinations[c]) cvars.push_back((uint32_t)id);
+                    dev_haps.push_back(h);
+                }
+                dev_groups.push_back(d);
+                called.push_back(std::move(g));
+            }
+        }
+        cur = end;
+    }
+    const RegionLayout rl = region_layout(alignments, engine, "call_haplotype_from_candidates");
+    const detail::FlatReads& fr = rl.fr;
+    // VariantGroup's read keys "read_name:strand" (every record is strand 0 of its read), ranked as std::map orders them
+    std::vector<std::string> keys(rl.reads.size());
+    for (size_t i = 0; i < rl.reads.size(); ++i) keys[i] = rl.reads.reads()[i].first->read_name + ":" + std::to_string(rl.reads.reads()[i].second);
+    std::vector<std::string> sorted = keys;
+    std::sort(sorted.begin(), sorted.end());
+    sorted.erase(std::unique(sorted.begin(), sorted.end()), sorted.end());
+    std::vector<uint32_t> key_rank(std::max<size_t>(keys.size(), 1));
+    for (size_t i = 0; i < keys.size(); ++i) key_rank[i] = (uint32_t)(std::lower_bound(sorted.begin(), sorted.end(), keys[i]) - sorted.begin());
+    nph_call_params params;
+    std::memset(&params, 0, sizeof(params));
+    params.region_start = alignments.region_start;
+    params.ploidy = (uint32_t)ploidy;
+    params.genotype_all = genotype_only ? 1u : 0u;
+    params.alignment_flags = alignment_flags;
+    // every record's base model has this k (the device call checks); the DNA models of the reads are 6-mers
+    params.k = alignments.records.empty() ? 6 : alignments.records[0].read->get_base_model(0)->k;
+    nph_screen_methylation meth;
+    std::vector<uint32_t> alt_models;
+    methylation_args(alignments, methylation_types, params.k, engine, "call_haplotype_from_candidates", meth, alt_models);
+    if (ploidy < 1) throw Error(NPH_ERR_INVALID, "call_haplotype_from_candidates: ploidy below 1");
+    std::vector<nph_call_group_result> gres(std::max<size_t>(dev_groups.size(), 1));
+    std::vector<nph_call_variant_result> vres(std::max<size_t>(n_var_results, 1));
+    nph_call_counts counts;
+    if (bases.empty()) bases.push_back('\0');
+    if (cvars.empty()) cvars.push_back(0);
+    if (dev_haps.empty()) dev_haps.emplace_back();
+    engine.check(nph_call_variant_groups_batch(engine.ctx(), fr.reads.data(), fr.reads.size(), fr.mean, rl.time.data(), fr.n_events,
+                                               alignments.reference.data(), alignments.reference.size(), rl.deltas.data(), rl.deltas.size(),
+                                               rl.first.data(), rl.recs.data(), rl.recs.size(), key_rank.data(), &params, dev_groups.data(),
+                                               dev_groups.size(), dev_haps.data(), dev_haps.size(), bases.data(), bases.size(), cvars.data(),
+                                               cvars.size(), n_var_results, indel_bias, methylation_types.empty() ? nullptr : &meth,
+                                               alt_models.data(), gres.data(), vres.data(), &counts),
+                 "nph_call_variant_groups_batch");
+    if (counts_out) *counts_out = counts;
+    // simple_call's output per group (ref: src/common/nanopolish_variant.cpp:416-488)
+    std::vector<std::vector<Variant>> calls(called.size());
+    std::vector<Variant> all_calls;
+    for (size_t gi = 0; gi < called.size(); ++gi) {
+        const nph_call_group_result& R = gres[gi];
+        const nph_call_variant_result* V = vres.data() + dev_groups[gi].var_first;
+        const size_t total_reads = R.n_keys;
+        for (size_t vi = 0; vi < called[gi].n; ++vi) {
+            if (!V[vi].emit) continue;
+            Variant v = candidate_variants[called[gi].first + vi];
+            const size_t var_count = V[vi].var_count;
+            v.quality = var_count > 0 ? R.best_score - R.base_score : 0.0;
+            v.add_info("TotalReads", total_reads);
+            v.add_info("AlleleCount", var_count);
+            v.add_info("SupportFraction", format_double(V[vi].support_sum / total_reads));
+            const double ref_fwd = V[vi].strand[0], ref_rev = V[vi].strand[1], alt_fwd = V[vi].strand[2], alt_rev = V[vi].strand[3];
+            v.add_info("SupportFractionByStrand", format_double(alt_fwd / (ref_fwd + alt_fwd)) + "," + format_double(alt_rev / (ref_rev + alt_rev)));
+            v.add_info("StrandSupport", std::to_string((int)std::round(ref_fwd)) + "," + std::to_string((int)std::round(ref_rev)) + "," +
+                                        std::to_string((int)std::round(alt_fwd)) + "," + std::to_string((int)std::round(alt_rev)));
+            // kt_fisher_exact takes int cells: the sums are truncated
+            const double two = fisher_exact_two_sided((int)ref_fwd, (int)ref_rev, (int)alt_fwd, (int)alt_rev);
+            int fisher_scaled = (int)(-4.343 * std::log(two) + .499);
+            if (fisher_scaled < 0) fisher_scaled = 1000;                        // underflow
+            v.add_info("StrandFisherTest", fisher_scaled);
+            v.add_info("SOR", format_double(calculate_sor(ref_fwd, ref_rev, alt_fwd, alt_rev)));
+            v.genotype = total_reads > 0 ? make_genotype(var_count, (size_t)ploidy) : ".";
+            calls[gi].push_back(v);
+        }
+        all_calls.insert(all_calls.end(), calls[gi].begin(), calls[gi].end());
+    }
+    // per-variant results do not depend on the batch: one annotation of every called variant, split back into its groups
+    if (calculate_all_support && !all_calls.empty()) {
+        annotate_variants_with_all_support(all_calls, alignments, flank, alignment_flags, engine, indel_bias);
+        size_t at = 0;
+        for (std::vector<Variant>& c : calls)
+            for (Variant& v : c) v = all_calls[at++];
+    }
+    Haplotype derived = region_haplotype;
+    for (const std::vector<Variant>& c : calls)
+        for (const Variant& v : c) derived.apply_variant(v);
+    return derived;
 }
 
 } // namespace nph

@@ -13,6 +13,9 @@
 //   screen_variants_by_score                     ref: src/nanopolish_call_variants.cpp:364-402 (on the device,
 //                                                nph_screen_variants_batch)
 //   expand_variants                              ref: src/nanopolish_call_variants.cpp:406-450 (host only)
+//   call_haplotype_from_candidates               ref: src/nanopolish_call_variants.cpp:782-880 (its scores and genotype choice on
+//                                                the device, nph_call_variant_groups_batch), with simple_call's output
+//                                                (src/common/nanopolish_variant.cpp:279-493)
 //
 // The reference scores one (read, sequence) pair per profile_hmm_score call inside an OpenMP loop.  Here every
 // (read, haplotype, alphabet alternative) triple of a whole candidate set becomes one job of ONE launch; the base
@@ -87,12 +90,20 @@ std::vector<std::vector<double>> score_haplotypes(const std::vector<Haplotype>& 
                                                   uint32_t alignment_flags, const std::vector<std::string>& methylation_types,
                                                   Engine& engine, double indel_bias = hmm_indel_bias_factor);
 
-// score_variant_group (ref: src/common/nanopolish_variant.cpp:182-262): every combination of up to max_r of the group's variants
-// (max_r = the largest r for which the haplotype count stays below max_haplotypes, :193-206) that applies cleanly to the base
-// haplotype — r = 0, the base haplotype, included — scored against every read with profile_hmm_score_set, all as ONE batch.
-// combinations[c] lists the variant ids of combination c (ascending ids, combinations of size r in lexicographic order; the
-// reference's Combinations generator visits the same sets in a different order), scores[c][read] is what
-// VariantGroup::set_combination_read_score receives.
+// The combinations of score_variant_group (ref: src/common/nanopolish_variant.cpp:193-232): max_r is the largest r for which the
+// haplotype count stays below max_haplotypes; for r = 0..max_r the r-subsets of the group's variants in the order of the reference's
+// Combinations generator (prev_permutation on a bool mask: ascending ids, lexicographic), each kept with its haplotype when
+// apply_variants succeeds on base_haplotype.  Combination 0 is the empty one.
+struct VariantCombinations {
+    std::vector<std::vector<size_t>> combinations;
+    std::vector<Haplotype> haplotypes;
+    size_t max_r = 0;
+};
+VariantCombinations variant_combinations(const std::vector<Variant>& variants, const Haplotype& base_haplotype, int max_haplotypes);
+
+// score_variant_group (ref: src/common/nanopolish_variant.cpp:182-262): every combination of variant_combinations scored against
+// every read with profile_hmm_score_set, all as ONE batch.  combinations[c] lists the variant ids of combination c, scores[c][read]
+// is what VariantGroup::set_combination_read_score receives.
 struct VariantGroupScores {
     std::vector<std::vector<size_t>> combinations;
     std::vector<std::vector<double>> scores;
@@ -181,5 +192,36 @@ std::vector<Variant> screen_variants_by_score(const RegionAlignments& alignments
 // b in ACGT.  Throws Error(NPH_ERR_INVALID) where the reference asserts: an extended deletion whose first |ref_seq| bases are not
 // ref_seq.
 std::vector<Variant> expand_variants(const RegionAlignments& alignments, const std::vector<Variant>& candidate_variants, int min_flanking_sequence);
+
+// The two-sided p-value of Fisher's exact test on the 2x2 table {{n11, n12}, {n21, n22}} as simple_call's kt_fisher_exact computes
+// it (ref: src/thirdparty/fet.c): 1 when the table's margins allow one table only; otherwise the probabilities of the tables from
+// each end inwards while they stay below 0.99999999 times the observed table's, plus the one that stops each walk when it is below
+// 1.00000001 times it, capped at 1.  Each probability is exp of log-binomials (lgamma) or, between multiples of 11, the previous
+// one times the hypergeometric ratio, so the result is the reference's bit for bit.
+double fisher_exact_two_sided(int n11, int n12, int n21, int n22);
+// ref: src/common/nanopolish_variant.cpp:264-277 (GATK's StrandOddsRatio)
+double calculate_sor(double ref_fwd, double ref_rev, double alt_fwd, double alt_rev);
+// ref: src/common/nanopolish_variant.cpp:148-158: ploidy alleles, the reference ones first, '/'-separated
+std::string make_genotype(size_t alt_alleles, size_t ploidy);
+
+// call_haplotype_from_candidates (ref: src/nanopolish_call_variants.cpp:782-880) with opt::min_flanking_sequence = flank,
+// opt::min_distance_between_variants = min_distance, opt::max_haplotypes, opt::ploidy, opt::genotype_only, opt::methylation_types
+// and opt::calculate_all_support as given, on one OpenMP thread:
+//   the groups      the candidates in the given order (unsorted lists included) while ref_position minus the previous one's is at
+//                   most min_distance; window [first - flank, last + |last.ref_seq| + flank], cut from the unedited region; a window
+//                   wider than 200 is not called
+//   the haplotypes  variant_combinations of each group; a group with one combination is not called
+//   the call        every group's scores and genotype search in one nph_call_variant_groups_batch (the reads keyed by
+//                   "read_name:0" as VariantGroup keys them); then per group simple_call's output: quality best - base (0 for a
+//                   variant outside the called set), INFO TotalReads, AlleleCount, SupportFraction, SupportFractionByStrand,
+//                   StrandSupport, StrandFisherTest, SOR, and the genotype ("." without reads); with calculate_all_support, one
+//                   annotate_variants_with_all_support over every called variant appends SupportFractionByBase
+//   the result      the region's haplotype with every group's called variants applied in order (apply_variant's refusals ignored)
+// Throws Error(NPH_ERR_INVALID) where the reference asserts (a window outside the region, a called group with fewer combinations
+// than the ploidy) and for a ref_position beyond int32.  counts_out (optional): the device call's counters.
+Haplotype call_haplotype_from_candidates(const RegionAlignments& alignments, const std::vector<Variant>& candidate_variants,
+                                         uint32_t alignment_flags, int flank, int min_distance, int max_haplotypes, int ploidy,
+                                         bool genotype_only, const std::vector<std::string>& methylation_types, bool calculate_all_support,
+                                         Engine& engine, double indel_bias = hmm_indel_bias_factor, nph_call_counts* counts_out = nullptr);
 
 } // namespace nph

@@ -879,6 +879,22 @@ assert SCREEN_LIST_PARAMS_DT.itemsize == 24 and SCREEN_CANDIDATE_DT.itemsize == 
 SCREEN_SCREENED, SCREEN_OUTSIDE, SCREEN_NOT_APPLIED = 0, 1, 2
 
 
+# ---- call_haplotype_from_candidates (nph_call_variant_groups_batch) ------------------------------------------------------
+CALL_MAX_PLOIDY = 8
+CALL_PARAMS_DT = np.dtype([("region_start", "<i4"), ("ploidy", "<u4"), ("genotype_all", "<u4"), ("alignment_flags", "<u4"), ("k", "<u4")], align=True)
+CALL_GROUP_DT = np.dtype([("calling_start", "<i4"), ("calling_end", "<i4"), ("hap_first", "<u4"), ("n_haplotypes", "<u4"), ("var_first", "<u4"),
+                          ("n_variants", "<u4")], align=True)
+CALL_HAPLOTYPE_DT = np.dtype([("seq_off", "<u8"), ("seq_len", "<u4"), ("n_var", "<u4"), ("var_off", "<u8")], align=True)
+CALL_GROUP_RESULT_DT = np.dtype([("n_keys", "<u4"), ("n_combinations", "<u4"), ("status", "<u4"), ("ploidy", "<u4"),
+                                 ("best_set", "<u4", CALL_MAX_PLOIDY), ("best_score", "<f8"), ("base_score", "<f8")], align=True)
+CALL_VARIANT_RESULT_DT = np.dtype([("var_count", "<u4"), ("emit", "<u4"), ("support_sum", "<f8"), ("strand", "<f8", 4)], align=True)
+CALL_COUNTS_DT = np.dtype([("n_groups", "<u8"), ("n_haplotypes", "<u8"), ("n_pairs", "<u8"), ("n_jobs", "<u8"), ("n_dp_rows", "<u8"), ("n_sets", "<u8"),
+                           ("n_set_terms", "<u8"), ("forward_ms", "<f8"), ("genotype_ms", "<f8"), ("host_ms", "<f8")], align=True)
+assert CALL_PARAMS_DT.itemsize == 20 and CALL_GROUP_DT.itemsize == 24 and CALL_HAPLOTYPE_DT.itemsize == 24
+assert CALL_GROUP_RESULT_DT.itemsize == 64 and CALL_VARIANT_RESULT_DT.itemsize == 48 and CALL_COUNTS_DT.itemsize == 80
+CALL_CALLED, CALL_BASE_KEPT, CALL_NO_BEST = 0, 1, 2
+
+
 # ---- methylation-aware screening (`variants -q cpg`, `-q dam,dcm`) -------------------------------------------------------
 SCREEN_METH_DT = np.dtype([("n_types", "<u4"), ("reserved", "<u4"), ("alphabets", METH_PARAMS_DT, 4)], align=True)
 assert SCREEN_METH_DT.itemsize == 616

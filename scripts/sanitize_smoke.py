@@ -83,4 +83,9 @@ _, ucnt = suc.device(eng, suc.build(suc.CASES[0]))
 _, lcnt = scc.device(eng, scc.build(scc.CASES[1]))
 assert int(hcnt["n_pairs"]) > 0 and int(ucnt["n_pairs"]) > 0 and int(lcnt["n_jobs"]) > 0
 print("region calls ok", int(hcnt["n_pairs"]), int(ucnt["n_pairs"]), int(lcnt["n_jobs"]))
+# call_haplotype_from_candidates' scores and genotype search: groups of two candidates at ploidy 2
+from tests import call_cases as ccs
+cg, _, ccnt = ccs.device(eng, ccs.build(ccs.CASES[1]))
+assert int(ccnt["n_jobs"]) > 0 and (cg["n_keys"] > 0).any()
+print("variant groups ok", int(ccnt["n_groups"]), int(ccnt["n_jobs"]), int(ccnt["n_sets"]))
 eng.close()
