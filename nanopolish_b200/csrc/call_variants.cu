@@ -9,10 +9,9 @@
 //   simple_call's read support                ref: src/common/nanopolish_variant.cpp:369-414 (on the host, with its libm)
 // The groups, their combinations and haplotypes come from the caller (the host Haplotype applies the variants).
 //
-// Kernels, after the window-read walk of window_reads.cu (count -> scan -> fill, a window per group):
-//   cv_ranks_kernel      thread per (haplotype, alternative): both strands' k-mer ranks (nph_window_ranks for the nucleotides), and
-//                        whether the methylated copy of each -q type differs from the haplotype
-//   (one read-back of those masks sizes every group's jobs)
+// Kernels, after the window-read walk of window_reads.cu (count -> scan -> fill, a window per group) and the rank pool of
+// score_sets.cu (nph_set_ranks: both strands of every haplotype and of each methylated copy, and which copies differ; one read-back
+// of those masks sizes every group's jobs):
 //   cv_emit_kernel       thread per (pair, haplotype): the jobs of its score set; then K1 (nph_score_device_jobs)
 //   cv_combine_kernel    thread per (pair, haplotype): nph_score_set_fold of its jobs
 //   cv_keys_kernel       warp per group: its pairs mapped to keys in key order, the last record's score per (combination, key),
@@ -50,16 +49,6 @@ struct CvGroup {
     uint32_t n_pairs, n_haps, hap_first, jobs_per_pair;
 };
 
-// per haplotype: its bases, its rank-pool offset (alternative a, strand s at rank_off + (2a + s) * nk), its first job in a pair's jobs
-struct CvHap { uint64_t seq_off, rank_off; uint32_t len, job_off; };
-
-struct CvMeth {
-    const MethDev* types;
-    const uint32_t* alt_model;          // n_records x T
-    uint32_t* alts;                     // per haplotype: bit t set when its methylated copy of type t differs from it
-    int T;
-};
-
 __host__ __device__ inline uint64_t gt_binom(uint64_t n, uint32_t r)
 {
     if (r > n) return 0;
@@ -82,52 +71,6 @@ __host__ __device__ inline void gt_unrank(uint64_t idx, uint32_t n, int p, uint3
     }
 }
 
-// rank of character p of methylate(s) (fw) or of Alphabet::reverse_complement(methylate(s)) (!fw, p indexing that string), as
-// screen_variants.cu's meth_rank on a plain byte string
-__device__ __forceinline__ uint32_t cv_meth_rank(const MethDev& md, const uint8_t* s, int L, int p, bool fw)
-{
-    const int rl = (int)md.site_len;
-    const int t = fw ? p : L - 1 - p;
-    for (int q0 = t - rl + 1; q0 <= t; ++q0) {
-        const int q = site_at(md, s, q0, L);
-        if (q < 0) continue;
-        return fw ? md.site_m_rank[q][t - q0] : md.site_mrc_rank[q][p - (L - q0 - rl)];
-    }
-    return fw ? md.rank_of[s[t]] : md.comp_rank_of[s[t]];
-}
-
-__global__ void cv_ranks_kernel(const CvHap* __restrict__ haps, uint32_t n_haps, const uint8_t* __restrict__ bases, int k,
-                                uint32_t* __restrict__ pool, const CvMeth cm)
-{
-    const uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-    const uint32_t na = 1u + (uint32_t)cm.T;
-    if (t >= (uint64_t)n_haps * na) return;
-    const CvHap H = haps[t / na];
-    const int alt = (int)(t % na);
-    const uint8_t* s = bases + H.seq_off;
-    const int L = (int)H.len, nk = L - k + 1;
-    uint32_t* fw = pool + H.rank_off + (uint64_t)alt * 2u * (uint64_t)nk;
-    uint32_t* rc = fw + nk;
-    if (alt == 0) {
-        const auto code = [&](int v) { return nph_dna_code(s[v]); };
-        nph_window_ranks(code, nk, k, false, fw);
-        nph_window_ranks(code, nk, k, true, rc);
-        return;
-    }
-    const MethDev& md = cm.types[alt - 1];
-    bool site = false;
-    for (int p = 0; p < L && !site; ++p) site = site_at(md, s, p, L) >= 0;
-    if (site) atomicOr(cm.alts + t / na, 1u << (alt - 1));
-    for (int p = 0; p < nk; ++p) {
-        uint32_t f = 0, r = 0;
-        for (int i = 0; i < k; ++i) {
-            f = f * md.asize + cv_meth_rank(md, s, L, p + i, true);
-            r = r * md.asize + cv_meth_rank(md, s, L, L - p - k + i, false);
-        }
-        fw[p] = f; rc[p] = r;
-    }
-}
-
 __device__ __forceinline__ uint32_t cv_group_of(const uint64_t* __restrict__ off, uint32_t n, uint64_t x)
 {
     uint32_t lo = 0, hi = n;                // the last g with off[g] <= x
@@ -141,13 +84,15 @@ __device__ __forceinline__ uint32_t cv_group_of(const uint64_t* __restrict__ off
 struct CvArgs {
     const CvGroup* groups;
     const uint64_t* item_off;           // n_groups + 1: each group's item_base, then the total
-    const CvHap* haps;
+    const NphSetSeq* haps;              // per haplotype: its bases and rank-pool offset
+    const uint32_t* job_off;            // per haplotype: its first job in a pair's jobs
     const NphWinPair* pairs;
     const nph_meth_record* records;
     uint32_t n_groups, flags;
 };
 
-__global__ void cv_emit_kernel(const CvArgs a, uint64_t n_items, int k, nph_hmm_job* __restrict__ jobs, const CvMeth cm)
+__global__ void cv_emit_kernel(const CvArgs a, uint64_t n_items, int k, nph_hmm_job* __restrict__ jobs, const NphSetTypes ty,
+                               const uint32_t* __restrict__ alts)
 {
     const uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
     if (t >= n_items) return;
@@ -157,23 +102,15 @@ __global__ void cv_emit_kernel(const CvArgs a, uint64_t n_items, int k, nph_hmm_
     const uint32_t pl = (uint32_t)(local / G.n_haps), h = G.hap_first + (uint32_t)(local % G.n_haps);
     const NphWinPair P = a.pairs[G.pair_first + pl];
     const nph_meth_record R = a.records[P.record];
-    const CvHap H = a.haps[h];
+    const NphSetSeq H = a.haps[h];
     nph_hmm_job jb = nph_window_job(R, P, (uint8_t)a.flags);
-    const uint32_t nk = H.len - (uint32_t)k + 1u;
-    const uint32_t mask = cm.T ? cm.alts[h] : 0u;
-    jb.n_kmers = nk;
-    nph_hmm_job* out = jobs + G.job_base + (uint64_t)pl * G.jobs_per_pair + H.job_off;
-    for (int alt = 0; alt <= cm.T; ++alt) {
-        if (alt && !((mask >> (alt - 1)) & 1u)) continue;
-        jb.model_id = alt ? cm.alt_model[(size_t)P.record * cm.T + (alt - 1)] : R.model_id;
-        jb.rank_off = H.rank_off + (uint64_t)alt * 2u * nk + (R.rc ? nk : 0u);
-        *out++ = jb;
-    }
+    jb.n_kmers = H.len - (uint32_t)k + 1u;
+    set_jobs(ty, jb, R, P.record, ty.T ? alts[h] : 0u, H.rank_off, jb.n_kmers, jobs + G.job_base + (uint64_t)pl * G.jobs_per_pair + a.job_off[h]);
 }
 
 // s[item] = profile_hmm_score_set of the item's jobs (a float)
-__global__ void cv_combine_kernel(const CvArgs a, uint64_t n_items, const float* __restrict__ scores, const uint32_t* __restrict__ alts,
-                                  const double* __restrict__ pen, const float* __restrict__ tbl, float* __restrict__ s)
+__global__ void cv_combine_kernel(const CvArgs a, uint64_t n_items, const float* __restrict__ scores, const NphSetTypes ty,
+                                  const uint32_t* __restrict__ alts, float* __restrict__ s)
 {
     const uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
     if (t >= n_items) return;
@@ -181,8 +118,8 @@ __global__ void cv_combine_kernel(const CvArgs a, uint64_t n_items, const float*
     const CvGroup G = a.groups[g];
     const uint64_t local = t - G.item_base;
     const uint32_t pl = (uint32_t)(local / G.n_haps), h = G.hap_first + (uint32_t)(local % G.n_haps);
-    const uint32_t n = 1u + (uint32_t)__popc(alts[h]);
-    s[t] = nph_score_set_fold(scores + G.job_base + (uint64_t)pl * G.jobs_per_pair + a.haps[h].job_off, n, pen[n - 1], tbl);
+    const uint32_t n = set_size(alts[h]);
+    s[t] = nph_score_set_fold(scores + G.job_base + (uint64_t)pl * G.jobs_per_pair + a.job_off[h], n, ty.pen[n - 1], ty.tbl);
 }
 
 // warp per group.  Pair p of the group has key_rank kr(p); its key is the number of distinct ranks below kr(p).  A pair is its key's
@@ -394,11 +331,8 @@ extern "C" int nph_call_variant_groups_batch(nph_ctx* ctx, const nph_read* reads
     if (p.ploidy < 1 || p.ploidy > NPH_CALL_MAX_PLOIDY) { ctx->last_error = "ploidy outside 1..NPH_CALL_MAX_PLOIDY"; return NPH_ERR_INVALID; }
     if (p.alignment_flags & ~(NPH_HAF_ALLOW_PRE_CLIP | NPH_HAF_ALLOW_POST_CLIP)) { ctx->last_error = "unknown alignment_flags"; return NPH_ERR_INVALID; }
     if (n_haplotypes > 0xffffffffu || n_groups > 0xffffffffu) { ctx->last_error = "more than 2^32 - 1 groups or haplotypes"; return NPH_ERR_INVALID; }
-    static const nph_screen_methylation none{};
-    const nph_screen_methylation& mt = meth ? *meth : none;
     std::vector<MethDev> md;
-    NPH_TRY(nph_screen_types(ctx, p.k, mt, n_records, alt_model_ids, md));
-    const int T = (int)md.size();
+    NPH_TRY(nph_region_types(ctx, p.k, meth, n_records, alt_model_ids, md));
     std::vector<uint64_t> n_sets;
     NPH_TRY(check_groups(ctx, p, n_ref_bases, groups, n_groups, haplotypes, n_haplotypes, n_bases, combination_variants, n_combination_variants,
                          n_variants, n_sets));
@@ -411,20 +345,16 @@ extern "C" int nph_call_variant_groups_batch(nph_ctx* ctx, const nph_read* reads
         nph_timing_staged(ctx, 0.f, 0);
         return NPH_OK;
     }
-    NPH_TRY(nph_region_load(ctx, reads, n_reads, ev_mean, ev_start_time, n_events_total, ref_bases, n_ref_bases, event_deltas, n_deltas_total,
-                            first_event, records, n_records, [&](size_t r, const nph_meth_record& R) {
-        return nph_screen_record_check(ctx, p.k, md, alt_model_ids, r, R);
-    }));
+    NphSetTypes ty;
+    NPH_TRY(nph_region_load_types(ctx, reads, n_reads, ev_mean, ev_start_time, n_events_total, ref_bases, n_ref_bases, event_deltas, n_deltas_total,
+                                  first_event, records, n_records, p.k, md, alt_model_ids, ty));
     cudaStream_t st = ctx->stream;
     const size_t G = n_groups;
-    // the haplotypes: the rank pool, per haplotype (1 + T) alternatives x both strands
-    std::vector<CvHap> hv(n_haplotypes);
-    uint64_t pool = 0;
+    std::vector<NphSetSeq> hv(n_haplotypes);
     for (size_t h = 0; h < n_haplotypes; ++h) {
         const nph_call_haplotype& H = haplotypes[h];
         if (H.seq_len < p.k || !nph_slice_ok(H.seq_off, H.seq_len, n_bases)) { ctx->last_error = "a haplotype outside haplotype_bases or with fewer than k bases"; return NPH_ERR_INVALID; }
-        hv[h] = CvHap{H.seq_off, pool, H.seq_len, 0u};
-        pool += (uint64_t)(1 + T) * 2u * (uint64_t)(H.seq_len - p.k + 1);
+        hv[h] = NphSetSeq{H.seq_off, 0, H.seq_len, 0u};
     }
     // the groups' reads
     std::vector<int2> bounds(G);
@@ -448,19 +378,17 @@ extern "C" int nph_call_variant_groups_batch(nph_ctx* ctx, const nph_read* reads
     blk_off[G] = blocks;
     if (blocks > (uint64_t)INT32_MAX) { ctx->last_error = "more genotype sets than one launch covers"; return NPH_ERR_INVALID; }
     nph_ctx::CallState& cs = ctx->call;
-    CvGroup* d_groups; uint64_t* d_item_off; uint64_t* d_blk_off; CvHap* d_haps; uint8_t* d_bases; uint32_t* d_key_rank; MethDev* d_meth;
-    uint32_t* d_alt_models; uint32_t* d_alts; double* d_pen;
+    CvGroup* d_groups; uint64_t* d_item_off; uint64_t* d_blk_off; NphSetSeq* d_haps; uint32_t* d_job_off; uint8_t* d_bases; uint32_t* d_key_rank;
+    uint32_t* d_alts;
     NPH_TRY(nph_carve(ctx, cs.d_in, [&](NphArena& c) {
         d_groups = c.take<CvGroup>(G);
         d_item_off = c.take<uint64_t>(G + 1);
         d_blk_off = c.take<uint64_t>(G + 1);
-        d_haps = c.take<CvHap>(n_haplotypes);
+        d_haps = c.take<NphSetSeq>(n_haplotypes);
+        d_job_off = c.take<uint32_t>(n_haplotypes);
         d_bases = c.take<uint8_t>(n_bases + 1);
         d_key_rank = c.take<uint32_t>(n_reads + 1);
-        d_meth = c.take<MethDev>((size_t)T + 1);
-        d_alt_models = c.take<uint32_t>(n_records * (size_t)T + 1);
         d_alts = c.take<uint32_t>(n_haplotypes);
-        d_pen = c.take<double>(NPH_SCREEN_MAX_TYPES + 1);
     }));
     float* d_s; float* d_ks; float* d_read_sum; uint32_t* d_key_rc; uint32_t* d_flag; uint32_t* d_key; uint32_t* d_n_keys;
     GtBest* d_partial; GtBest* d_best; double* d_base;
@@ -476,21 +404,11 @@ extern "C" int nph_call_variant_groups_batch(nph_ctx* ctx, const nph_read* reads
         d_best = c.take<GtBest>(G);
         d_base = c.take<double>(G);
     }));
-    double pen[NPH_SCREEN_MAX_TYPES + 1];
-    for (int n = 1; n <= NPH_SCREEN_MAX_TYPES + 1; ++n) pen[n - 1] = log((double)n);     // profile_hmm_score_set's log(num_models), host libm
-    NPH_CUDA(ctx, cudaMemcpyAsync(d_haps, hv.data(), sizeof(CvHap) * n_haplotypes, cudaMemcpyHostToDevice, st));
     if (n_bases) NPH_CUDA(ctx, cudaMemcpyAsync(d_bases, haplotype_bases, n_bases, cudaMemcpyHostToDevice, st));
     if (n_reads) NPH_CUDA(ctx, cudaMemcpyAsync(d_key_rank, key_rank, sizeof(uint32_t) * n_reads, cudaMemcpyHostToDevice, st));
-    if (T) NPH_CUDA(ctx, cudaMemcpyAsync(d_meth, md.data(), sizeof(MethDev) * T, cudaMemcpyHostToDevice, st));
-    if (T && n_records) NPH_CUDA(ctx, cudaMemcpyAsync(d_alt_models, alt_model_ids, sizeof(uint32_t) * n_records * T, cudaMemcpyHostToDevice, st));
-    NPH_CUDA(ctx, cudaMemcpyAsync(d_pen, pen, sizeof(pen), cudaMemcpyHostToDevice, st));
-    NPH_CUDA(ctx, cudaMemsetAsync(d_alts, 0, sizeof(uint32_t) * n_haplotypes, st));
-    const CvMeth cm{d_meth, d_alt_models, d_alts, T};
-    NPH_TRY(nph_reserve(ctx, ctx->d_ranks, (size_t)pool));
-    const uint64_t n_rank_items = (uint64_t)n_haplotypes * (1u + T);
-    cv_ranks_kernel<<<(unsigned)((n_rank_items + 127) / 128), 128, 0, st>>>(d_haps, (uint32_t)n_haplotypes, d_bases, (int)p.k, ctx->d_ranks.p, cm);
-    NPH_CUDA(ctx, cudaGetLastError());
-    std::vector<uint32_t> alts(n_haplotypes);
+    uint64_t pool = 0;
+    NPH_TRY(nph_set_ranks(ctx, hv, d_haps, d_bases, p.k, ty, d_alts, &pool));
+    std::vector<uint32_t> alts(n_haplotypes), job_off(n_haplotypes);
     NPH_CUDA(ctx, cudaMemcpyAsync(alts.data(), d_alts, sizeof(uint32_t) * n_haplotypes, cudaMemcpyDeviceToHost, st));
     NPH_CUDA(ctx, cudaStreamSynchronize(st));                         // read-back: each haplotype's set size lays out the jobs
     uint64_t n_jobs = 0;
@@ -498,7 +416,7 @@ extern "C" int nph_call_variant_groups_batch(nph_ctx* ctx, const nph_read* reads
         uint32_t J = 0;
         for (uint32_t c = 0; c < groups[g].n_haplotypes; ++c) {
             const uint32_t h = groups[g].hap_first + c;
-            hv[h].job_off = J;
+            job_off[h] = J;
             J += 1u + (uint32_t)__builtin_popcount(alts[h]);
         }
         gv[g].jobs_per_pair = J;
@@ -507,22 +425,22 @@ extern "C" int nph_call_variant_groups_batch(nph_ctx* ctx, const nph_read* reads
         cnt.n_dp_rows += wr.rows[g] * J;
     }
     cnt.n_jobs = n_jobs;
-    NPH_CUDA(ctx, cudaMemcpyAsync(d_haps, hv.data(), sizeof(CvHap) * n_haplotypes, cudaMemcpyHostToDevice, st));
+    NPH_CUDA(ctx, cudaMemcpyAsync(d_job_off, job_off.data(), sizeof(uint32_t) * n_haplotypes, cudaMemcpyHostToDevice, st));
     NPH_CUDA(ctx, cudaMemcpyAsync(d_groups, gv.data(), sizeof(CvGroup) * G, cudaMemcpyHostToDevice, st));
     NPH_CUDA(ctx, cudaMemcpyAsync(d_item_off, item_off.data(), sizeof(uint64_t) * (G + 1), cudaMemcpyHostToDevice, st));
     NPH_CUDA(ctx, cudaMemcpyAsync(d_blk_off, blk_off.data(), sizeof(uint64_t) * (G + 1), cudaMemcpyHostToDevice, st));
-    const CvArgs a{d_groups, d_item_off, d_haps, wr.d_pairs, ctx->region.ev.d_records.p, (uint32_t)G, p.alignment_flags};
+    const CvArgs a{d_groups, d_item_off, d_haps, d_job_off, wr.d_pairs, ctx->region.ev.d_records.p, (uint32_t)G, p.alignment_flags};
     float forward_ms = 0.f;
     int launches = 5;
     if (n_jobs) {
         NPH_TRY(nph_score_device_jobs(ctx, (size_t)n_jobs, (size_t)pool, indel_bias, [&]() -> int {
-            cv_emit_kernel<<<(unsigned)((items + 127) / 128), 128, 0, st>>>(a, items, (int)p.k, ctx->d_jobs.p, cm);
+            cv_emit_kernel<<<(unsigned)((items + 127) / 128), 128, 0, st>>>(a, items, (int)p.k, ctx->d_jobs.p, ty, d_alts);
             NPH_CUDA(ctx, cudaGetLastError());
             return NPH_OK;
         }));
         int nl = 0;
         if (nph_last_kernel_ms(ctx, &forward_ms, &nl) == NPH_OK) launches += nl + 1;
-        cv_combine_kernel<<<(unsigned)((items + 255) / 256), 256, 0, st>>>(a, items, ctx->d_scores.p, d_alts, d_pen, ctx->d_logsum.p, d_s);
+        cv_combine_kernel<<<(unsigned)((items + 255) / 256), 256, 0, st>>>(a, items, ctx->d_scores.p, ty, d_alts, d_s);
         NPH_CUDA(ctx, cudaGetLastError());
     }
     cv_keys_kernel<<<(unsigned)((G + kWarps - 1) / kWarps), kThreads, 0, st>>>(a, d_key_rank, d_s, ctx->d_logsum.p, d_flag, d_key, d_ks, d_read_sum,

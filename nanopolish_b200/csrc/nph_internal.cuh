@@ -216,6 +216,7 @@ struct nph_ctx {
         NphEventRecords ev;                // region reference, compact event alignments, records
         DevBuf<uint8_t> d_counts;          // the windows' bounds, per-window counts, pair offsets, the scan's scratch, the largest rows
         DevBuf<uint8_t> d_pairs;           // the windows' pairs and the window of each
+        DevBuf<uint8_t> d_types;           // the -q types' MethDev tables and n_records x T model ids (score_sets.cu)
     } region;
 
     // the last nph_homopolymer_likelihoods_batch (homopolymer.cu)
@@ -232,14 +233,14 @@ struct nph_ctx {
 
     // the last nph_screen_variants_batch (screen_variants.cu)
     struct ScreenListState {
-        DevBuf<uint8_t> d_in;              // windows, sequences, the window's candidates, alleles, methylation tables and model ids
+        DevBuf<uint8_t> d_in;              // windows, sequences and their bytes, the window's candidates
         DevBuf<uint8_t> d_state;           // per-window round state, job counts and offsets, scan scratch, per-candidate state,
                                            // methylated-alternative masks, counters
     } sl;
 
     // the last nph_call_variant_groups_batch (call_variants.cu)
     struct CallState {
-        DevBuf<uint8_t> d_in;              // groups, haplotypes, their bases and variant ids, key ranks, methylation tables and model ids
+        DevBuf<uint8_t> d_in;              // groups, haplotypes and their bases, key ranks
         DevBuf<uint8_t> d_work;            // per-group offsets, masks, pair scores, key tables, partial maxima, group results
     } call;
 

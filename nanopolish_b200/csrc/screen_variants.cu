@@ -8,12 +8,10 @@
 //   score_variant_thresholded                 ref: src/common/nanopolish_variant.cpp:765-799, with the -q sets of
 //                                             generate_methylated_alternatives (:158-178) as nph_screen_load_methylation forms them
 //
-// Candidates with the same window (calling_start, |ref_seq|) share its reads and base haplotype.  Kernels, after the window-read
-// walk of window_reads.cu (count -> scan -> fill: each window's event sequences and their event rows), then the round loop of
-// variants.cu:
-//   sv_ranks_kernel         a warp per (sequence, alternative): the k-mer ranks of both strands into a variable-length pool (the
-//                           base window of every window, the edited window of every candidate that applies), and whether the
-//                           methylated copy of each type differs from its sequence
+// Candidates with the same window (calling_start, |ref_seq|) share its reads and base haplotype.  The host writes the base window of
+// every window and the edited window of every candidate that applies as bytes.  Kernels, after the window-read walk of
+// window_reads.cu (count -> scan -> fill: each window's event sequences and their event rows) and the rank pool of score_sets.cu
+// (nph_set_ranks: both strands of every sequence and of each methylated copy, and which copies differ), the round loop of variants.cu:
 //   per round, while any candidate is inside the threshold and has reads left:
 //     sv_round_count_kernel   thread per window: the next reads_per_round reads, each scoring the base set and the set of every
 //                             live candidate of the window
@@ -31,18 +29,11 @@
 
 namespace {
 
-constexpr int kWarps = 8;
-constexpr int kThreads = kWarps * 32;
 constexpr unsigned kFull = 0xffffffffu;
 constexpr uint32_t kNoSeq = 0xffffffffu;
 
 // a window: [cs, cs + len - 1], its candidates wcand[cand_first, cand_first + n_cand), its base sequence
 struct SvWin { int32_t cs, len; uint32_t cand_first, n_cand, base_seq, pad; };
-
-// a sequence of the rank pool: window bytes [0, flank), the allele (al bytes at alleles[alt_off]), window bytes from flank + rl on.
-// The base window has rl = al = 0.  Alternative a (0: nucleotides, 1 + t: methylated copy of type t) has its forward ranks at
-// rank_off + a * 2 * nk and its reverse-strand ranks nk further, nk = L - k + 1.
-struct SvSeq { uint64_t rank_off, alt_off; int32_t win_off, rl, al, L; };
 
 // per candidate: the thresholded total, the reference's DP rows, its variant sequence (kNoSeq: outside the region or not applied),
 // whether its total is inside the threshold at the start of the round
@@ -55,106 +46,14 @@ struct SvCounters { unsigned long long events, ref_events; unsigned int any_left
 struct SvArgs {
     const nph_meth_record* records;
     const SvWin* wins;
-    const SvSeq* seqs;
+    const NphSetSeq* seqs;
     const uint32_t* wcand;
     SvCand* cands;
-    const uint8_t* ref;                 // the region reference
-    const uint8_t* alleles;
-    uint32_t n_wins, n_seqs;
-    int flank, k, T, rpr;
+    uint32_t n_wins;
+    int k, rpr;
     uint32_t flags;
     double threshold;
 };
-
-// the -q types (T = 0: none)
-struct SvMeth {
-    const MethDev* types;
-    const uint32_t* alt_model;          // n_records x T
-    uint32_t* alts;                     // per sequence: bit t set when its methylated copy of type t differs from it
-    const float* tbl;
-    double pen[NPH_SCREEN_MAX_TYPES + 1];   // log(n) for a set of n sequences, host libm
-};
-
-__device__ __forceinline__ uint32_t set_size(uint32_t mask) { return 1u + (uint32_t)__popc(mask); }
-
-// character i of sequence S
-__device__ __forceinline__ uint8_t seq_char(const SvArgs& a, const SvSeq& S, int i)
-{
-    const uint8_t* w = a.ref + S.win_off;
-    if (i < a.flank) return w[i];
-    if (i < a.flank + S.al) return a.alleles[S.alt_off + (uint64_t)(i - a.flank)];
-    return w[i - S.al + S.rl];
-}
-
-// site_at (meth_dev.cuh) on the characters of S
-__device__ __forceinline__ int seq_site_at(const SvArgs& a, const MethDev& md, const SvSeq& S, int i)
-{
-    if (i < 0 || i + (int)md.site_len > S.L) return -1;
-    for (uint32_t q = 0; q < md.n_sites; ++q) {
-        bool eq = true;
-        for (uint32_t t = 0; t < md.site_len && eq; ++t) eq = seq_char(a, S, i + (int)t) == (uint8_t)md.site[q][t];
-        if (eq) return (int)q;
-    }
-    return -1;
-}
-
-// rank of character p of methylate(S) (fw) or of Alphabet::reverse_complement(methylate(S)) (!fw, p indexing that string): a
-// methylated site at s covers [s, s + rl) forward and [L - s - rl, L - s) reversed.  Recognition sites never overlap
-// (nph_meth_alphabet), so at most one site covers a position.
-__device__ __forceinline__ uint32_t meth_rank(const SvArgs& a, const MethDev& md, const SvSeq& S, int p, bool fw)
-{
-    const int rl = (int)md.site_len;
-    const int t = fw ? p : S.L - 1 - p;                          // the forward position the character comes from
-    for (int s = t - rl + 1; s <= t; ++s) {
-        const int q = seq_site_at(a, md, S, s);
-        if (q < 0) continue;
-        return fw ? md.site_m_rank[q][t - s] : md.site_mrc_rank[q][p - (S.L - s - rl)];
-    }
-    const uint8_t c = seq_char(a, S, t);
-    return fw ? md.rank_of[c] : md.comp_rank_of[c];
-}
-
-// a warp per (sequence, alternative): both strands' ranks of every k-mer; an alternative's lanes also look for a site at each
-// position, and a sequence with one gets its type's bit in sm.alts (generate_methylated_alternatives keeps a copy that differs)
-__global__ void __launch_bounds__(kThreads) sv_ranks_kernel(const SvArgs a, uint32_t* __restrict__ pool, const SvMeth sm)
-{
-    const int lane = threadIdx.x & 31;
-    const uint32_t warp = blockIdx.x * kWarps + (threadIdx.x >> 5);
-    const uint32_t n_warps = gridDim.x * kWarps;
-    const uint32_t na = 1u + (uint32_t)a.T;
-    for (uint32_t item = warp; item < a.n_seqs * na; item += n_warps) {
-        const uint32_t si = item / na;
-        const int alt = (int)(item % na);
-        const SvSeq S = a.seqs[si];
-        const int nk = S.L - a.k + 1;
-        uint32_t* fw = pool + S.rank_off + (uint64_t)alt * 2u * (uint64_t)nk;
-        uint32_t* rc = fw + nk;
-        bool site = false;
-        for (int p = lane; p < S.L; p += 32) {
-            if (alt == 0) {
-                if (p >= nk) continue;
-                // HMMInputSequence::get_kmer_rank(p, k, rc) of the DNA alphabet (nph_dna_kmer_ranks)
-                uint32_t f = 0, r = 0;
-                for (int t = 0; t < a.k; ++t) {
-                    f = f * 4u + nph_dna_code(seq_char(a, S, p + t));
-                    r = r * 4u + (3u - nph_dna_code(seq_char(a, S, p + a.k - 1 - t)));
-                }
-                fw[p] = f; rc[p] = r;
-                continue;
-            }
-            const MethDev& md = sm.types[alt - 1];
-            site = site || seq_site_at(a, md, S, p) >= 0;
-            if (p >= nk) continue;
-            uint32_t f = 0, r = 0;
-            for (int t = 0; t < a.k; ++t) {
-                f = f * md.asize + meth_rank(a, md, S, p + t, true);
-                r = r * md.asize + meth_rank(a, md, S, S.L - p - a.k + t, false);
-            }
-            fw[p] = f; rc[p] = r;
-        }
-        if (__any_sync(kFull, site) && lane == 0) atomicOr(sm.alts + si, 1u << (alt - 1));
-    }
-}
 
 // thread per window: how many jobs it contributes this round (per read the base set and the set of every live candidate)
 __global__ void sv_round_count_kernel(const SvArgs a, SvWinState* __restrict__ ws, const uint64_t* __restrict__ pair_off,
@@ -178,26 +77,18 @@ __global__ void sv_round_count_kernel(const SvArgs a, SvWinState* __restrict__ w
     job_cnt[wi] = (uint64_t)s.chunk * per_read;
 }
 
-// appends the jobs of sequence si's set for one read: the sequence, then its methylated copies in type order
-__device__ __forceinline__ nph_hmm_job* emit_set(const SvArgs& a, const SvMeth& sm, nph_hmm_job jb, const nph_meth_record& R, uint32_t record,
-                                                 uint32_t si, nph_hmm_job* out)
+// appends the jobs of sequence si's set for one read
+__device__ __forceinline__ nph_hmm_job* emit_seq(const SvArgs& a, const NphSetTypes& ty, const uint32_t* alts, nph_hmm_job jb,
+                                                 const nph_meth_record& R, uint32_t record, uint32_t si, nph_hmm_job* out)
 {
-    const SvSeq S = a.seqs[si];
-    const uint32_t nk = (uint32_t)(S.L - a.k + 1);
-    const uint32_t mask = a.T ? sm.alts[si] : 0u;
-    jb.n_kmers = nk;
-    for (int alt = 0; alt <= a.T; ++alt) {
-        if (alt && !((mask >> (alt - 1)) & 1u)) continue;
-        jb.model_id = alt ? sm.alt_model[(size_t)record * a.T + (alt - 1)] : R.model_id;
-        jb.rank_off = S.rank_off + (uint64_t)alt * 2u * nk + (R.rc ? nk : 0u);
-        *out++ = jb;
-    }
-    return out;
+    const NphSetSeq S = a.seqs[si];
+    jb.n_kmers = S.len - (uint32_t)a.k + 1u;
+    return set_jobs(ty, jb, R, record, ty.T ? alts[si] : 0u, S.rank_off, jb.n_kmers, out);
 }
 
 __global__ void sv_emit_kernel(const SvArgs a, const SvWinState* __restrict__ ws, const uint64_t* __restrict__ pair_off,
                                const NphWinPair* __restrict__ pairs, const uint64_t* __restrict__ job_off, nph_hmm_job* __restrict__ jobs,
-                               unsigned long long* __restrict__ events, const SvMeth sm)
+                               unsigned long long* __restrict__ events, const NphSetTypes ty, const uint32_t* __restrict__ alts)
 {
     const uint32_t wi = blockIdx.x * blockDim.x + threadIdx.x;
     unsigned long long ev = 0;
@@ -211,10 +102,10 @@ __global__ void sv_emit_kernel(const SvArgs a, const SvWinState* __restrict__ ws
             const nph_meth_record R = a.records[P.record];
             const nph_hmm_job jb = nph_window_job(R, P, (uint8_t)a.flags);
             nph_hmm_job* const first = out;
-            out = emit_set(a, sm, jb, R, P.record, W.base_seq, out);
+            out = emit_seq(a, ty, alts, jb, R, P.record, W.base_seq, out);
             for (uint32_t c = 0; c < W.n_cand; ++c) {
                 const SvCand& C = a.cands[a.wcand[W.cand_first + c]];
-                if (C.alive) out = emit_set(a, sm, jb, R, P.record, C.seq, out);
+                if (C.alive) out = emit_seq(a, ty, alts, jb, R, P.record, C.seq, out);
             }
             ev += (unsigned long long)(out - first) * nph_pair_rows(P.e1, P.e2);
         }
@@ -227,7 +118,7 @@ __global__ void sv_emit_kernel(const SvArgs a, const SvWinState* __restrict__ ws
 // `if (fabs(total) < threshold) total += variant - base` (var_accumulate_kernel's arithmetic, NaN included)
 __global__ void sv_accumulate_kernel(const SvArgs a, SvWinState* __restrict__ ws, const uint64_t* __restrict__ pair_off,
                                      const NphWinPair* __restrict__ pairs, const uint64_t* __restrict__ job_off, const float* __restrict__ scores,
-                                     SvCounters* __restrict__ ctr, const SvMeth sm)
+                                     SvCounters* __restrict__ ctr, const NphSetTypes ty, const uint32_t* __restrict__ alts)
 {
     const uint32_t wi = blockIdx.x * blockDim.x + threadIdx.x;
     if (wi >= a.n_wins) return;
@@ -236,18 +127,18 @@ __global__ void sv_accumulate_kernel(const SvArgs a, SvWinState* __restrict__ ws
     const SvWin W = a.wins[wi];
     const float* sc = scores + job_off[wi];
     const NphWinPair* rd = pairs + pair_off[wi] + s.done;
-    const uint32_t nb = set_size(a.T ? sm.alts[W.base_seq] : 0u);
+    const uint32_t nb = set_size(ty.T ? alts[W.base_seq] : 0u);
     unsigned long long ref_ev = 0;
     for (uint32_t r = 0; r < s.chunk; ++r) {
         // double base_score = profile_hmm_score_set(...) (a float); a set of one is its score
-        const double base_score = (double)nph_score_set_fold(sc, nb, sm.pen[nb - 1], sm.tbl);
+        const double base_score = (double)nph_score_set_fold(sc, nb, ty.pen[nb - 1], ty.tbl);
         sc += nb;
         const unsigned long long E = nph_pair_rows(rd[r].e1, rd[r].e2);
         for (uint32_t c = 0; c < W.n_cand; ++c) {
             SvCand& C = a.cands[a.wcand[W.cand_first + c]];
             if (!C.alive) continue;
-            const uint32_t nc = set_size(a.T ? sm.alts[C.seq] : 0u);
-            const double variant_score = (double)nph_score_set_fold(sc, nc, sm.pen[nc - 1], sm.tbl);
+            const uint32_t nc = set_size(ty.T ? alts[C.seq] : 0u);
+            const double variant_score = (double)nph_score_set_fold(sc, nc, ty.pen[nc - 1], ty.tbl);
             sc += nc;
             if (fabs(C.total) < a.threshold) {
                 C.total = __dadd_rn(C.total, __dsub_rn(variant_score, base_score));
@@ -272,15 +163,15 @@ __global__ void sv_accumulate_kernel(const SvArgs a, SvWinState* __restrict__ ws
     if (left) atomicOr(&ctr->any_left, 1u);
 }
 
-// the host's view of the list: windows, sequences, the windows' candidate lists, the initial candidate states
+// the host's view of the list: windows, sequences and their bytes, the windows' candidate lists, the initial candidate states
 struct SvPlan {
     std::vector<SvWin> wins;
-    std::vector<SvSeq> seqs;
+    std::vector<NphSetSeq> seqs;
+    std::vector<uint8_t> bytes;
     std::vector<uint32_t> wcand;
     std::vector<SvCand> cands;
     std::vector<uint32_t> cand_win;           // per candidate: its window (kNoSeq: outside the region)
     std::vector<uint8_t> applied;
-    uint64_t pool = 0;                        // rank pool entries
 };
 
 int plan_list(nph_ctx* ctx, const nph_screen_list_params& p, const char* ref, size_t n_ref, const char* alleles, size_t n_allele_bytes,
@@ -313,7 +204,8 @@ int plan_list(nph_ctx* ctx, const nph_screen_list_params& p, const char* ref, si
             w = (uint32_t)pl.wins.size();
             win_of.emplace(key, w);
             pl.wins.push_back(SvWin{(int32_t)cs, len, 0u, 0u, (uint32_t)pl.seqs.size(), 0u});
-            pl.seqs.push_back(SvSeq{0, 0, win_off, 0, 0, len});
+            pl.seqs.push_back(NphSetSeq{pl.bytes.size(), 0, (uint32_t)len, 0u});
+            pl.bytes.insert(pl.bytes.end(), ref + win_off, ref + win_off + len);
             members.emplace_back();
         } else {
             w = it->second;
@@ -325,8 +217,11 @@ int plan_list(nph_ctx* ctx, const nph_screen_list_params& p, const char* ref, si
         pl.applied[i] = 1;
         pl.cands[i].seq = (uint32_t)pl.seqs.size();
         pl.cands[i].alive = 0.0 < (double)p.score_threshold ? 1u : 0u;
-        pl.seqs.push_back(SvSeq{0, c.alt_seq_off, win_off, (int32_t)c.ref_seq_len, (int32_t)c.alt_seq_len,
-                                len - (int32_t)c.ref_seq_len + (int32_t)c.alt_seq_len});
+        // the edited window: its first flank bases, alt_seq, the bases after ref_seq
+        pl.seqs.push_back(NphSetSeq{pl.bytes.size(), 0, (uint32_t)(len - (int32_t)c.ref_seq_len + (int32_t)c.alt_seq_len), 0u});
+        pl.bytes.insert(pl.bytes.end(), ref + win_off, ref + win_off + p.flank);
+        pl.bytes.insert(pl.bytes.end(), alleles + c.alt_seq_off, alleles + c.alt_seq_off + c.alt_seq_len);
+        pl.bytes.insert(pl.bytes.end(), ref + win_off + p.flank + c.ref_seq_len, ref + win_off + len);
     }
     for (size_t w = 0; w < pl.wins.size(); ++w) {
         pl.wins[w].cand_first = (uint32_t)pl.wcand.size();
@@ -357,11 +252,8 @@ extern "C" int nph_screen_variants_batch(nph_ctx* ctx, const nph_read* reads, si
     if (p.flank < 0 || 2 * (int64_t)p.flank + 1 < (int64_t)p.k) { ctx->last_error = "2 * flank + 1 below k (a haplotype without a k-mer)"; return NPH_ERR_INVALID; }
     if (p.reads_per_round == 0) { ctx->last_error = "reads_per_round is 0"; return NPH_ERR_INVALID; }
     if (p.alignment_flags & ~(NPH_HAF_ALLOW_PRE_CLIP | NPH_HAF_ALLOW_POST_CLIP)) { ctx->last_error = "unknown alignment_flags"; return NPH_ERR_INVALID; }
-    static const nph_screen_methylation none{};
-    const nph_screen_methylation& mt = meth ? *meth : none;
     std::vector<MethDev> md;
-    NPH_TRY(nph_screen_types(ctx, p.k, mt, n_records, alt_model_ids, md));
-    const int T = (int)md.size();
+    NPH_TRY(nph_region_types(ctx, p.k, meth, n_records, alt_model_ids, md));
     SvPlan pl;
     NPH_TRY(plan_list(ctx, p, ref_bases, n_ref_bases, alleles, n_allele_bytes, candidates, n_candidates, pl));
     nph_screen_list_counts cnt{};
@@ -384,19 +276,16 @@ extern "C" int nph_screen_variants_batch(nph_ctx* ctx, const nph_read* reads, si
     nph_ctx::ScreenListState& ss = ctx->sl;
     const size_t n_wins = pl.wins.size(), n_seqs = pl.seqs.size(), n_cand = n_candidates;
     const auto run = [&]() -> int {
-        NPH_TRY(nph_region_load(ctx, reads, n_reads, ev_mean, ev_start_time, n_events_total, ref_bases, n_ref_bases, event_deltas, n_deltas_total,
-                                first_event, records, n_records, [&](size_t r, const nph_meth_record& R) {
-            return nph_screen_record_check(ctx, p.k, md, alt_model_ids, r, R);
-        }));
+        NphSetTypes ty;
+        NPH_TRY(nph_region_load_types(ctx, reads, n_reads, ev_mean, ev_start_time, n_events_total, ref_bases, n_ref_bases, event_deltas,
+                                      n_deltas_total, first_event, records, n_records, p.k, md, alt_model_ids, ty));
         cudaStream_t st = ctx->stream;
-        SvWin* d_wins; SvSeq* d_seqs; uint32_t* d_wcand; uint8_t* d_alleles; MethDev* d_meth; uint32_t* d_alt_models;
+        SvWin* d_wins; NphSetSeq* d_seqs; uint32_t* d_wcand; uint8_t* d_bytes;
         NPH_TRY(nph_carve(ctx, ss.d_in, [&](NphArena& c) {
             d_wins = c.take<SvWin>(n_wins);
-            d_seqs = c.take<SvSeq>(n_seqs);
+            d_seqs = c.take<NphSetSeq>(n_seqs);
             d_wcand = c.take<uint32_t>(pl.wcand.size());
-            d_alleles = c.take<uint8_t>(n_allele_bytes + 1);
-            d_meth = c.take<MethDev>((size_t)T + 1);
-            d_alt_models = c.take<uint32_t>(n_records * (size_t)T + 1);
+            d_bytes = c.take<uint8_t>(pl.bytes.size());
         }));
         SvWinState* d_ws; uint64_t* d_job_cnt; uint64_t* d_job_off; uint64_t* d_scratch; SvCand* d_cands; uint32_t* d_alts; SvCounters* d_ctr;
         NPH_TRY(nph_carve(ctx, ss.d_state, [&](NphArena& c) {
@@ -408,26 +297,14 @@ extern "C" int nph_screen_variants_batch(nph_ctx* ctx, const nph_read* reads, si
             d_alts = c.take<uint32_t>(n_seqs);
             d_ctr = c.take<SvCounters>(1);
         }));
-        // the rank pool: per sequence (1 + T) alternatives x both strands
-        for (SvSeq& s : pl.seqs) {
-            s.rank_off = pl.pool;
-            pl.pool += (uint64_t)(1 + T) * 2u * (uint64_t)(s.L - (int)p.k + 1);
-        }
         NPH_CUDA(ctx, cudaMemcpyAsync(d_wins, pl.wins.data(), sizeof(SvWin) * n_wins, cudaMemcpyHostToDevice, st));
-        NPH_CUDA(ctx, cudaMemcpyAsync(d_seqs, pl.seqs.data(), sizeof(SvSeq) * n_seqs, cudaMemcpyHostToDevice, st));
         NPH_CUDA(ctx, cudaMemcpyAsync(d_wcand, pl.wcand.data(), sizeof(uint32_t) * pl.wcand.size(), cudaMemcpyHostToDevice, st));
         NPH_CUDA(ctx, cudaMemcpyAsync(d_cands, pl.cands.data(), sizeof(SvCand) * n_cand, cudaMemcpyHostToDevice, st));
-        if (n_allele_bytes) NPH_CUDA(ctx, cudaMemcpyAsync(d_alleles, alleles, n_allele_bytes, cudaMemcpyHostToDevice, st));
-        if (T) NPH_CUDA(ctx, cudaMemcpyAsync(d_meth, md.data(), sizeof(MethDev) * T, cudaMemcpyHostToDevice, st));
-        if (T && n_records) NPH_CUDA(ctx, cudaMemcpyAsync(d_alt_models, alt_model_ids, sizeof(uint32_t) * n_records * T, cudaMemcpyHostToDevice, st));
+        NPH_CUDA(ctx, cudaMemcpyAsync(d_bytes, pl.bytes.data(), pl.bytes.size(), cudaMemcpyHostToDevice, st));
         NPH_CUDA(ctx, cudaMemsetAsync(d_ws, 0, sizeof(SvWinState) * n_wins, st));
-        NPH_CUDA(ctx, cudaMemsetAsync(d_alts, 0, sizeof(uint32_t) * n_seqs, st));
         NPH_CUDA(ctx, cudaMemsetAsync(d_ctr, 0, sizeof(SvCounters), st));
-        SvArgs a{ctx->region.ev.d_records.p, d_wins, d_seqs, d_wcand, d_cands, ctx->region.ev.d_ref.p, d_alleles, (uint32_t)n_wins,
-                 (uint32_t)n_seqs, p.flank, (int)p.k, T, (int)p.reads_per_round, p.alignment_flags, (double)p.score_threshold};
-        SvMeth sm{};
-        sm.types = d_meth; sm.alt_model = d_alt_models; sm.alts = d_alts; sm.tbl = ctx->d_logsum.p;
-        for (int n = 1; n <= 1 + T; ++n) sm.pen[n - 1] = log((double)n);      // profile_hmm_score_set's log(num_models), host libm
+        SvArgs a{ctx->region.ev.d_records.p, d_wins, d_seqs, d_wcand, d_cands, (uint32_t)n_wins, (int)p.k, (int)p.reads_per_round,
+                 p.alignment_flags, (double)p.score_threshold};
         // the windows' reads
         std::vector<int2> bounds(n_wins);
         for (size_t w = 0; w < n_wins; ++w) bounds[w] = make_int2(pl.wins[w].cs, pl.wins[w].cs + pl.wins[w].len - 1);
@@ -436,11 +313,8 @@ extern "C" int nph_screen_variants_batch(nph_ctx* ctx, const nph_read* reads, si
         const std::vector<uint64_t>& off = wr.off;
         const uint64_t* d_off = wr.d_off;
         const NphWinPair* d_pairs = wr.d_pairs;
-        NPH_TRY(nph_reserve(ctx, ctx->d_ranks, (size_t)pl.pool));
-        const size_t n_items = n_seqs * (size_t)(1 + T);
-        const int rgrid = (int)std::min<size_t>((n_items + kWarps - 1) / kWarps, (size_t)ctx->sm_count * 16);
-        sv_ranks_kernel<<<rgrid, kThreads, 0, st>>>(a, ctx->d_ranks.p, sm);
-        NPH_CUDA(ctx, cudaGetLastError());
+        uint64_t pool = 0;
+        NPH_TRY(nph_set_ranks(ctx, pl.seqs, d_seqs, d_bytes, p.k, ty, d_alts, &pool));
         const unsigned wgrid = (unsigned)((n_wins + 255) / 256);
         float kernel_ms = 0.f;
         int launches = 6;
@@ -452,12 +326,12 @@ extern "C" int nph_screen_variants_batch(nph_ctx* ctx, const nph_read* reads, si
             NPH_CUDA(ctx, cudaMemcpyAsync(&n_jobs, d_job_off + n_wins, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
             NPH_CUDA(ctx, cudaStreamSynchronize(st));                 // read-back: the round's job count
             if (n_jobs == 0) break;
-            NPH_TRY(nph_score_device_jobs(ctx, (size_t)n_jobs, (size_t)pl.pool, indel_bias, [&]() -> int {
-                sv_emit_kernel<<<wgrid, 256, 0, st>>>(a, d_ws, d_off, d_pairs, d_job_off, ctx->d_jobs.p, &d_ctr->events, sm);
+            NPH_TRY(nph_score_device_jobs(ctx, (size_t)n_jobs, (size_t)pool, indel_bias, [&]() -> int {
+                sv_emit_kernel<<<wgrid, 256, 0, st>>>(a, d_ws, d_off, d_pairs, d_job_off, ctx->d_jobs.p, &d_ctr->events, ty, d_alts);
                 NPH_CUDA(ctx, cudaGetLastError());
                 return NPH_OK;
             }));
-            sv_accumulate_kernel<<<wgrid, 256, 0, st>>>(a, d_ws, d_off, d_pairs, d_job_off, ctx->d_scores.p, d_ctr, sm);
+            sv_accumulate_kernel<<<wgrid, 256, 0, st>>>(a, d_ws, d_off, d_pairs, d_job_off, ctx->d_scores.p, d_ctr, ty, d_alts);
             NPH_CUDA(ctx, cudaGetLastError());
             float ms = 0.f; int nl = 0;
             if (nph_last_kernel_ms(ctx, &ms, &nl) == NPH_OK) { kernel_ms += ms; launches += nl + 4; }

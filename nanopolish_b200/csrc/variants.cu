@@ -19,7 +19,9 @@
 //   var_accumulate_kernel  per position: the sequential `if (fabs(total) < threshold) total += variant - base` over the
 //                       round's reads in order (each side profile_hmm_score_set's fold of its sequence and alternatives);
 //                       candidates inside the threshold stay live
-// The host drives the rounds; per round one read-back (job count) plus the scheduler's summary.
+// The host drives the rounds; per round one read-back (job count) plus the scheduler's summary.  The -q sets (a sequence and its
+// methylated copies) use the set description and helpers of meth_dev.cuh and score_sets.cu, shared with list screening and group
+// calling; the pool, the masks and the -q tables stay this screen's own.
 #include "nph_internal.cuh"
 #include "exact_math.cuh"
 #include "meth_dev.cuh"
@@ -52,19 +54,10 @@ struct VarDev {
     int T;                // methylation types; alternative a = 0 is the nucleotide sequence, a = 1 + t its methylated copy of type t
 };
 
-// the methylation types of a screening (T = 0: none)
-struct VarMeth {
-    const MethDev* types;               // T alphabets, -q order
-    const uint32_t* alt_model;          // n_records x T: read->get_model(strand, type t)
-    unsigned long long* alts;           // per position: bit seq * T + t set when sequence seq has a methylated copy of type t
-    const float* tbl;                   // the context's log-sum table
-    double pen[NPH_SCREEN_MAX_TYPES + 1];   // log(n) for a set of n = 1 .. 1 + T sequences, host libm
-};
-
-// profile_hmm_score_set's set size of sequence seq: itself + its methylated copies
-__device__ __forceinline__ uint32_t set_size(unsigned long long alts, int seq, int T)
+// the copies of sequence seq in a position's mask (bit seq * T + t: its methylated copy of type t differs from it)
+__device__ __forceinline__ uint32_t seq_mask(unsigned long long alts, int seq, int T)
 {
-    return 1u + (uint32_t)__popcll((alts >> (seq * T)) & ((1ull << T) - 1ull));
+    return (uint32_t)((alts >> (seq * T)) & ((1ull << T) - 1ull));
 }
 
 // pool slot of (position, sequence, alternative): 2 * stride ranks (forward, reverse strand)
@@ -152,9 +145,10 @@ __device__ __forceinline__ int edited_window(const uint8_t* __restrict__ w, int 
 }
 
 // thread per (position, sequence, alternative): ranks of both strands into the pool; the base sequence's nucleotide thread also
-// writes candidate validity into the position state, a methylated copy that differs from its sequence sets its bit in vm.alts
+// writes candidate validity into the position state, a methylated copy that differs from its sequence sets its bit in alts
 __global__ void __launch_bounds__(kBlock) var_ranks_kernel(const VarDev d, const uint8_t* __restrict__ ref, uint32_t* __restrict__ pool,
-                                                           PosState* __restrict__ state, const uint64_t* __restrict__ pos_off, const VarMeth vm)
+                                                           PosState* __restrict__ state, const uint64_t* __restrict__ pos_off, const NphSetTypes st,
+                                                           unsigned long long* __restrict__ alts)
 {
     const long long gid = (long long)blockIdx.x * kBlock + threadIdx.x;
     const int na = 1 + d.T;
@@ -192,22 +186,19 @@ __global__ void __launch_bounds__(kBlock) var_ranks_kernel(const VarDev d, const
         for (int q = 0; q < nk; ++q) nph_dna_kmer_ranks(sq, q, d.k, fw[q], rc[q]);
         return;
     }
-    // methylated copy of type a - 1: fr = ranks of methylate(sq), rv = ranks of Alphabet::reverse_complement of it, where a methylated
-    // site at q comes out as the methylated complement back to front at [L - q - rl, L - q)
-    const MethDev& md = vm.types[a - 1];
-    const int rl = (int)md.site_len;
+    // methylated copy of type a - 1: fr = ranks of methylate(sq), rv = ranks of Alphabet::reverse_complement of it
+    const MethDev& md = st.types[a - 1];
+    bool changed = false;
+    for (int q = 0; q < L && !changed; ++q) changed = site_at(md, sq, q, L) >= 0;
+    if (!changed) return;                                        // generate_methylated_alternatives keeps only a copy that differs
+    atomicOr(alts + pi, 1ull << (seq * d.T + a - 1));
     uint8_t* fr = w;
     uint8_t rv[NPH_SCREEN_MAX_WINDOW + 1];
-    for (int t = 0; t < L; ++t) { fr[t] = md.rank_of[sq[t]]; rv[L - 1 - t] = md.comp_rank_of[sq[t]]; }
-    bool changed = false;
-    for (int q = 0; q + rl <= L; ++q) {
-        const int s = site_at(md, sq, q, L);
-        if (s < 0) continue;
-        changed = true;
-        for (int t = 0; t < rl; ++t) { fr[q + t] = md.site_m_rank[s][t]; rv[L - q - rl + t] = md.site_mrc_rank[s][t]; }
+    for (int t = 0; t < L; ++t) {
+        uint32_t f, r;
+        meth_copy_rank(md, sq, L, t, f, r);
+        fr[t] = (uint8_t)f; rv[L - 1 - t] = (uint8_t)r;
     }
-    if (!changed) return;                                        // generate_methylated_alternatives keeps only a copy that differs
-    atomicOr(vm.alts + pi, 1ull << (seq * d.T + a - 1));
     for (int q = 0; q < nk; ++q) {
         uint32_t rf = 0, rr = 0;
         for (int t = 0; t < d.k; ++t) { rf = rf * md.asize + fr[q + t]; rr = rr * md.asize + rv[L - q - d.k + t]; }
@@ -230,8 +221,8 @@ __global__ void var_round_count_kernel(const VarDev d, PosState* __restrict__ st
     uint32_t per_read = 1u + __popc(st.alive);
     if (d.T) {
         const unsigned long long am = alts[pi];
-        per_read = set_size(am, NPH_SCREEN_SLOTS, d.T);
-        for (int c = 0; c < NPH_SCREEN_SLOTS; ++c) if ((st.alive >> c) & 1u) per_read += set_size(am, c, d.T);
+        per_read = set_size(seq_mask(am, NPH_SCREEN_SLOTS, d.T));
+        for (int c = 0; c < NPH_SCREEN_SLOTS; ++c) if ((st.alive >> c) & 1u) per_read += set_size(seq_mask(am, c, d.T));
     }
     job_cnt[pi] = (uint64_t)chunk * per_read;
 }
@@ -239,37 +230,31 @@ __global__ void var_round_count_kernel(const VarDev d, PosState* __restrict__ st
 __global__ void var_emit_kernel(const VarDev d, const PosState* __restrict__ state, const uint64_t* __restrict__ pos_off,
                                 const NphWinPair* __restrict__ pos_reads, const nph_meth_record* __restrict__ records,
                                 const uint64_t* __restrict__ job_off, nph_hmm_job* __restrict__ jobs, unsigned long long* __restrict__ events,
-                                const VarMeth vm)
+                                const NphSetTypes ty, const unsigned long long* __restrict__ alts)
 {
     const int pi = blockIdx.x * blockDim.x + threadIdx.x;
     unsigned long long ev = 0;
     if (pi < d.n_pos) {
         const PosState st = state[pi];
         if (st.chunk) {
-            const unsigned long long am = d.T ? vm.alts[pi] : 0ull;
+            const unsigned long long am = d.T ? alts[pi] : 0ull;
             const NphWinPair* rd = pos_reads + pos_off[pi] + st.done;
             nph_hmm_job* out = jobs + job_off[pi];
             for (uint32_t r = 0; r < st.chunk; ++r) {
                 const NphWinPair pr = rd[r];
                 const nph_meth_record R = records[pr.record];
                 nph_hmm_job jb = nph_window_job(R, pr, (uint8_t)d.flags);
-                const unsigned long long E = nph_pair_rows(pr.e1, pr.e2);
-                // the base haplotype first, then the live candidates in slot order; each sequence followed by its methylated copies
-                // in type order (generate_methylated_alternatives)
+                nph_hmm_job* const first = out;
+                // the base haplotype first, then the live candidates in slot order
                 for (int seq = NPH_SCREEN_SLOTS; ; ) {
                     const int L = seq == NPH_SCREEN_SLOTS ? d.win : (seq == 8 ? d.win - 1 : ((seq & 1) ? d.win + 1 : d.win));
                     jb.n_kmers = (uint32_t)(L - d.k + 1);
-                    for (int a = 0; a <= d.T; ++a) {
-                        if (a && !((am >> (seq * d.T + a - 1)) & 1ull)) continue;
-                        jb.model_id = a ? vm.alt_model[(size_t)pr.record * d.T + (a - 1)] : R.model_id;
-                        jb.rank_off = pool_slot(d, pi, seq, a) * 2 * d.stride + (R.rc ? d.stride : 0);
-                        *out++ = jb;
-                        ev += E;
-                    }
+                    out = set_jobs(ty, jb, R, pr.record, seq_mask(am, seq, d.T), pool_slot(d, pi, seq, 0) * 2 * d.stride, (uint32_t)d.stride, out);
                     if (seq == NPH_SCREEN_SLOTS) seq = -1;
                     do { ++seq; } while (seq < NPH_SCREEN_SLOTS && !((st.alive >> seq) & 1u));
                     if (seq >= NPH_SCREEN_SLOTS) break;
                 }
+                ev += (unsigned long long)(out - first) * nph_pair_rows(pr.e1, pr.e2);
             }
         }
     }
@@ -280,27 +265,28 @@ __global__ void var_emit_kernel(const VarDev d, const PosState* __restrict__ sta
 
 __global__ void var_accumulate_kernel(const VarDev d, PosState* __restrict__ state, const uint64_t* __restrict__ job_off,
                                       const float* __restrict__ scores, unsigned int* __restrict__ any_left, const uint64_t* __restrict__ pos_off,
-                                      const NphWinPair* __restrict__ pos_reads, unsigned long long* __restrict__ ref_events, const VarMeth vm)
+                                      const NphWinPair* __restrict__ pos_reads, unsigned long long* __restrict__ ref_events, const NphSetTypes ty,
+                                      const unsigned long long* __restrict__ alts)
 {
     const int pi = blockIdx.x * blockDim.x + threadIdx.x;
     if (pi >= d.n_pos) return;
     PosState st = state[pi];
     if (!st.chunk) return;
-    const unsigned long long am = d.T ? vm.alts[pi] : 0ull;
+    const unsigned long long am = d.T ? alts[pi] : 0ull;
     const float* s = scores + job_off[pi];
     const NphWinPair* rd = pos_reads + pos_off[pi] + st.done;
     const double thr = (double)d.threshold;
-    const uint32_t nb = set_size(am, NPH_SCREEN_SLOTS, d.T);
+    const uint32_t nb = set_size(seq_mask(am, NPH_SCREEN_SLOTS, d.T));
     unsigned long long ref_ev = 0;
     for (uint32_t r = 0; r < st.chunk; ++r) {
         // double base_score = profile_hmm_score_set(...) (a float); a set of one is its score
-        const double base_score = (double)nph_score_set_fold(s, nb, vm.pen[nb - 1], vm.tbl);
+        const double base_score = (double)nph_score_set_fold(s, nb, ty.pen[nb - 1], ty.tbl);
         s += nb;
         const unsigned long long E = nph_pair_rows(rd[r].e1, rd[r].e2);
         for (int c = 0; c < NPH_SCREEN_SLOTS; ++c) {
             if (!((st.alive >> c) & 1u)) continue;
-            const uint32_t nc = set_size(am, c, d.T);
-            const double variant_score = (double)nph_score_set_fold(s, nc, vm.pen[nc - 1], vm.tbl);
+            const uint32_t nc = set_size(seq_mask(am, c, d.T));
+            const double variant_score = (double)nph_score_set_fold(s, nc, ty.pen[nc - 1], ty.tbl);
             s += nc;
             if (fabs(st.total[c]) < thr) {
                 st.total[c] = __dadd_rn(st.total[c], __dsub_rn(variant_score, base_score));
@@ -332,12 +318,12 @@ __global__ void var_output_kernel(const VarDev d, const PosState* __restrict__ s
         const unsigned long long am = d.T ? alts[pi] : 0ull;
         const uint32_t nr = (uint32_t)(pos_off[pi + 1] - pos_off[pi]);
         ref_rows[pi] = st.ref_rows;
-        uint32_t per_read = set_size(am, NPH_SCREEN_SLOTS, d.T);
+        uint32_t per_read = set_size(seq_mask(am, NPH_SCREEN_SLOTS, d.T));
         bool any = false;
         for (int c = 0; c < NPH_SCREEN_SLOTS; ++c) {
             const double q = ((st.valid >> c) & 1u) ? st.total[c] : __longlong_as_double(0x7ff8000000000000ll);
             qual[(size_t)pi * NPH_SCREEN_SLOTS + c] = q;
-            if (!isnan(q)) { any = true; per_read += set_size(am, c, d.T); }
+            if (!isnan(q)) { any = true; per_read += set_size(seq_mask(am, c, d.T)); }
         }
         n_reads[pi] = nr;
         if (any) full = (unsigned long long)nr * per_read;
@@ -373,37 +359,6 @@ ScreenStateLayout screen_state_layout(NphArena& a, size_t n_pos)
 }
 
 } // namespace
-
-int nph_screen_types(nph_ctx* ctx, uint32_t k, const nph_screen_methylation& meth, size_t n_records, const uint32_t* alt_model_ids,
-                     std::vector<MethDev>& md)
-{
-    const uint32_t T = meth.n_types;
-    if (T > NPH_SCREEN_MAX_TYPES) { ctx->last_error = "nph_screen_methylation: more than NPH_SCREEN_MAX_TYPES types"; return NPH_ERR_INVALID; }
-    if (T && n_records && !alt_model_ids) return NPH_ERR_INVALID;
-    md.assign(T, MethDev{});
-    for (uint32_t t = 0; t < T; ++t) {
-        NPH_TRY(nph_meth_alphabet(ctx, meth.alphabets[t], md[t]));
-        if (md[t].k != k) { ctx->last_error = "nph_screen_methylation: type " + std::to_string(t) + " has k != params.k"; return NPH_ERR_INVALID; }
-    }
-    return NPH_OK;
-}
-
-int nph_screen_record_check(nph_ctx* ctx, uint32_t k, const std::vector<MethDev>& md, const uint32_t* alt_model_ids, size_t r,
-                            const nph_meth_record& R)
-{
-    const size_t T = md.size();
-    const DevModel& mod = ctx->models[R.model_id];
-    if (mod.k != k || mod.alphabet_size != 4) { ctx->last_error = "screening record " + std::to_string(r) + ": its model is not a nucleotide model of k = params.k"; return NPH_ERR_INVALID; }
-    for (size_t t = 0; t < T; ++t) {
-        const uint32_t id = alt_model_ids[r * T + t];
-        if (id >= ctx->models.size() || ctx->models[id].k != md[t].k || ctx->models[id].alphabet_size != md[t].asize) {
-            ctx->last_error = "screening record " + std::to_string(r) + ": its model of methylation type " + std::to_string(t) +
-                              " is out of range or not a model of that alphabet";
-            return NPH_ERR_INVALID;
-        }
-    }
-    return NPH_OK;
-}
 
 extern "C" int nph_screen_load_methylation(nph_ctx* ctx, const char* ref_bases, size_t n_ref_bases, const int16_t* event_deltas, size_t n_deltas_total,
                                            const int32_t* first_event, const nph_meth_record* records, size_t n_records,
@@ -489,23 +444,18 @@ extern "C" int nph_screen_run(nph_ctx* ctx)
     ScreenStateLayout sl;
     NPH_TRY(nph_carve(ctx, m.d_state, [&](NphArena& a) { sl = screen_state_layout(a, n_pos); }));
     PosState* state = sl.state;
-    VarMeth vm{};
-    vm.types = reinterpret_cast<const MethDev*>(m.d_meth.p);
-    vm.alt_model = m.d_alt_models.p;
-    vm.alts = sl.alts;
-    vm.tbl = ctx->d_logsum.p;
-    for (int n = 1; n <= 1 + d.T; ++n) vm.pen[n - 1] = log((double)n);      // profile_hmm_score_set's log(num_models), host libm
+    const NphSetTypes ty = nph_set_types(reinterpret_cast<const MethDev*>(m.d_meth.p), m.d_alt_models.p, ctx->d_logsum.p, d.T);
     NPH_CUDA(ctx, cudaMemsetAsync(ctx->d_ranks.p, 0, sizeof(uint32_t) * pool, st));
-    if (d.T) NPH_CUDA(ctx, cudaMemsetAsync(vm.alts, 0, sizeof(unsigned long long) * (size_t)n_pos, st));
+    if (d.T) NPH_CUDA(ctx, cudaMemsetAsync(sl.alts, 0, sizeof(unsigned long long) * (size_t)n_pos, st));
     const long long n_thr = (long long)n_pos * kSeqs * (1 + d.T);
-    var_ranks_kernel<<<(unsigned)((n_thr + kBlock - 1) / kBlock), kBlock, 0, st>>>(d, m.ev.d_ref.p, ctx->d_ranks.p, state, m.d_pos_off.p, vm);
+    var_ranks_kernel<<<(unsigned)((n_thr + kBlock - 1) / kBlock), kBlock, 0, st>>>(d, m.ev.d_ref.p, ctx->d_ranks.p, state, m.d_pos_off.p, ty, sl.alts);
     NPH_CUDA(ctx, cudaGetLastError());
     ScreenCounters* ctr = sl.counters;
     NPH_CUDA(ctx, cudaMemsetAsync(ctr, 0, sizeof(ScreenCounters), st));
     float kernel_ms_total = 0.f;
     int launches_total = 0;
     for (;;) {
-        var_round_count_kernel<<<pgrid, kBlock, 0, st>>>(d, state, m.d_pos_off.p, counts, vm.alts);
+        var_round_count_kernel<<<pgrid, kBlock, 0, st>>>(d, state, m.d_pos_off.p, counts, sl.alts);
         NPH_CUDA(ctx, cudaGetLastError());
         NPH_TRY(nph_scan_exclusive(ctx, counts, n_pos, job_off, scan_scratch));
         uint64_t n_jobs = 0;
@@ -514,12 +464,12 @@ extern "C" int nph_screen_run(nph_ctx* ctx)
         if (n_jobs == 0) break;
         // var_emit_kernel writes the round's jobs over the pool var_ranks_kernel wrote; the schedule is one more read-back
         NPH_TRY(nph_score_device_jobs(ctx, (size_t)n_jobs, pool, m.indel_bias, [&]() -> int {
-            var_emit_kernel<<<pgrid, kBlock, 0, st>>>(d, state, m.d_pos_off.p, pos_reads, records, job_off, ctx->d_jobs.p, &ctr->events, vm);
+            var_emit_kernel<<<pgrid, kBlock, 0, st>>>(d, state, m.d_pos_off.p, pos_reads, records, job_off, ctx->d_jobs.p, &ctr->events, ty, sl.alts);
             NPH_CUDA(ctx, cudaGetLastError());
             return NPH_OK;
         }));
         NPH_CUDA(ctx, cudaMemsetAsync(&ctr->any_left, 0, sizeof(unsigned int), st));
-        var_accumulate_kernel<<<pgrid, kBlock, 0, st>>>(d, state, job_off, ctx->d_scores.p, &ctr->any_left, m.d_pos_off.p, pos_reads, &ctr->ref_events, vm);
+        var_accumulate_kernel<<<pgrid, kBlock, 0, st>>>(d, state, job_off, ctx->d_scores.p, &ctr->any_left, m.d_pos_off.p, pos_reads, &ctr->ref_events, ty, sl.alts);
         NPH_CUDA(ctx, cudaGetLastError());
         float ms = 0.f; int nl = 0;
         if (nph_last_kernel_ms(ctx, &ms, &nl) == NPH_OK) { kernel_ms_total += ms; launches_total += nl + 6; }

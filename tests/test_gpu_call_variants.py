@@ -72,6 +72,15 @@ def test_random_region_equals_restatement(host, eng, seed, ploidy):
     assert len(got) > 40
 
 
+def test_dam_dcm_equals_restatement(host, eng):
+    """-q dam,dcm on the planted-site pile-up: sets of up to three sequences per haplotype"""
+    c = cc.build(("meth_dam_dcm_p2", ("meth", 130, 10, 100, 73), 2, 1, 64, ("dam", "dcm"), 0, "meth", "plain"))
+    st, got = cc.mirror(host, c)
+    assert st >= 0, host.nphh_last_error()
+    assert got == cc.restated(c, cc.hmm_scores(eng, c))
+    assert len(got) > 3
+
+
 def test_thousand_haplotypes_equal_brute_force(host, eng):
     """one group of 10 variants with max_haplotypes 1000: 968 haplotypes, 468 996 sets at ploidy 2"""
     c = cc.build(("h1000", ("snp", 700, 8, 240, 6, 10), 2, 1, 1000, (), 0, "cluster10", "plain"))

@@ -233,15 +233,22 @@ def test_kernel_time_needs_a_timed_call(ctx):
 
 
 def test_region_calls_reuse_one_batch_state(ctx):
-    """All-support, fix-homopolymers and list screening share one batch state (records and the window-read walk's buffers).  Run
-    one after another between a staged edit screen's run and its fetch, on a large pile-up, then a small one, then a medium one,
-    every result and counter is bit-equal to the same call on a fresh context, and so is the edit screen's."""
+    """All-support, fix-homopolymers, list screening and group calling share one batch state (records, the window-read walk's
+    buffers and the -q tables).  Run one after another between a staged edit screen's run and its fetch, on a large pile-up, then a
+    small one, then a medium one, then one with -q cpg, every result and counter is bit-equal to the same call on a fresh context, and
+    so is the edit screen's."""
+    from tests import call_cases as cc
     from tests import hp_cases as hc
     from tests import screen_cases as scc
     from tests import support_cases as suc
     rs, ref_chars, deltas, first, recs, params = _screen_inputs()
-    sup, hp, lst = suc.random_case(61), hc.build(hc.CASES[1]), scc.build(scc.CASES[1])
-    calls = [lambda e: suc.device(e, sup), lambda e: hc.device(e, hp), lambda e: scc.device(e, lst)]
+    sup, hp, lst, grp = suc.random_case(61), hc.build(hc.CASES[1]), scc.build(scc.CASES[1]), cc.build(cc.CASES[-1])
+
+    def group_call(e):
+        g, v, cnt = cc.device(e, grp, methylation=scc.meth_arg(grp))
+        return np.frombuffer(g.tobytes() + v.tobytes(), np.uint8), cnt
+
+    calls = [lambda e: suc.device(e, sup), lambda e: hc.device(e, hp), lambda e: scc.device(e, lst), group_call]
 
     def edit_screen_run(e):
         e.reads_load(rs.reads, rs.ev_mean, rs.ev_start_time)
@@ -266,7 +273,7 @@ def test_region_calls_reuse_one_batch_state(ctx):
     got = [bits(*call(ctx)) for call in calls]
     got.append(tuple(x.tobytes() for x in ctx.screen_fetch()))
     assert got == want
-    assert want[0][1]["n_pairs"] > want[1][1]["n_pairs"] > 0 and want[2][1]["n_jobs"] > 0
+    assert want[0][1]["n_pairs"] > want[1][1]["n_pairs"] > 0 and want[2][1]["n_jobs"] > 0 and want[3][1]["n_jobs"] > 0
 
 
 @pytest.mark.parametrize("device_jobs", ["methylation", "screening"])

@@ -116,10 +116,11 @@ def test_random_list_equals_restatement(eng, seed, threshold, flags):
     assert int(cnt["n_windows"]) < int((st != scr.OUTSIDE).sum())                      # candidates share windows
 
 
-@pytest.mark.parametrize("types", [(), ("cpg",)], ids=["none", "cpg"])
+@pytest.mark.parametrize("types", [(), ("cpg",), ("dam", "dcm")], ids=["none", "cpg", "dam_dcm"])
 def test_edits_equal_the_edit_screen(eng, types):
     """a substitution or insertion at position i has the edit screen's window [i - flank, i + 1 + flank] and reads, so both calls
-    give the same quality bits"""
+    give the same quality bits (with dam,dcm: sets of up to three sequences, through the edit screen's fixed rank pool and the list's
+    variable one)"""
     from tests.test_variants_methylation_oracle import methylated_pileup
     if types:
         _, _, _, ref_chars, rs, recs, pairs = methylated_pileup(list(types), 240, 10, 120, seed=91)
