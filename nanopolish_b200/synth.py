@@ -258,9 +258,10 @@ def gen_reads(n_reads: int, n_events: int, model: PoreModel, seed: int = 42, dri
     return ReadSet(reads, np.concatenate(means), np.concatenate(times), seqs, evk, kfe, k)
 
 
-def gen_reads_from_sequence(codes: np.ndarray, n_reads: int, model: PoreModel, seed: int = 42) -> ReadSet:
+def gen_reads_from_sequence(codes: np.ndarray, n_reads: int, model: PoreModel, seed: int = 42, nev=None) -> ReadSet:
     """n_reads reads that all traverse the same base sequence (a pile-up over one reference window), each with its own
-    event counts, noise and scalings — the input shape of variant scoring (SURVEY.md 8d, config 5)."""
+    event counts, noise and scalings — the input shape of variant scoring (SURVEY.md 8d, config 5).  nev: the events each
+    k-mer emits in every read (0: the k-mer is skipped), instead of random counts."""
     k = model.k
     nk = codes.shape[0] - k + 1
     ranks = kmer_ranks_from_codes(codes, k, 4)
@@ -270,9 +271,13 @@ def gen_reads_from_sequence(codes: np.ndarray, n_reads: int, model: PoreModel, s
     p_nev = np.array([0.03, 0.35, 0.45, 0.17])
     for r in range(n_reads):
         rng = np.random.default_rng(seed + r)
-        nev = rng.choice(4, nk, p=p_nev)
-        nev[0] = max(nev[0], 1); nev[-1] = max(nev[-1], 1)
-        which = np.repeat(np.arange(nk, dtype=np.int32), nev)
+        if nev is None:
+            ne = rng.choice(4, nk, p=p_nev)
+            ne[0] = max(ne[0], 1); ne[-1] = max(ne[-1], 1)
+        else:
+            ne = np.asarray(nev, np.int64)
+            assert ne.shape == (nk,) and ne.min() >= 0 and ne.sum() > 0
+        which = np.repeat(np.arange(nk, dtype=np.int32), ne)
         E = which.shape[0]
         shift, scale, var = rng.uniform(-5.0, 5.0), rng.uniform(0.9, 1.1), rng.uniform(0.9, 1.3)
         t = (np.arange(E, dtype=np.float64) * 0.002) + rng.uniform(0.0, 100.0)

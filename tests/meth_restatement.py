@@ -36,15 +36,18 @@ def is_motif_match(a, s, i):
     return any(match_to_site(s, i, site, rl)[1] == rl for site in a["sites"])
 
 
-def methylate(a, s):
+def methylate(a, s, fit=0, tail=""):
+    """fit: moves the test that a site lies inside the string (i + rl <= len(s)) by that many bases; a site that then reaches
+    past the end is matched against `tail`, the bases that follow the string, and methylated as far as the string goes"""
     rl = len(a["sites"][0])
+    t = s + tail
     out = list(s)
     i = 0
     while i < len(s):
         stride = 1
         for site, site_m in zip(a["sites"], a["sites_m"]):
-            if match_to_site(s, i, site, rl)[1] == rl:
-                out[i:i + rl] = list(site_m)
+            if i + rl <= len(s) + fit and match_to_site(t, i, site, rl)[1] == rl:
+                out[i:i + rl] = list(site_m)[:len(s) - i]
                 stride = rl
                 break
         i += stride
@@ -102,31 +105,38 @@ def find_by_ref_bounds(ref_pos, read_pos, ref_start, ref_stop):
     return int(read_pos[i]), int(read_pos[j])
 
 
+# the boundary comparisons of enumerate_record, each of which `moved` may shift by a number of bases
+MOVABLE = ("separation", "sub_start", "max_span", "event_span", "region_start", "region_end", "site_fit", "substr")
+
+
 def enumerate_record(ref, ref_start_pos, pr_ref, pr_read, rc, alphabet, k, min_separation=10, min_flank=10, max_span=200,
-                     min_event_span=10, region_start=-1, region_end=-1):
-    """-> list of (start_position, end_position, n_motif, e1, e2, ranks_u, ranks_m, site_sequence)"""
+                     min_event_span=10, region_start=-1, region_end=-1, moved=None):
+    """-> list of (start_position, end_position, n_motif, e1, e2, ranks_u, ranks_m, site_sequence).
+    moved: {name in MOVABLE: shift}, the restatement with those comparisons moved (a check that test cases sit on them)"""
+    mv = (moved or {}).get
     a = ALPHABETS[alphabet]
     motif_sites = [i for i in range(len(ref) - 1) if is_motif_match(a, ref, i)] if len(ref) else []
     groups, cur = [], 0
     while cur < len(motif_sites):
         end = cur + 1
-        while end < len(motif_sites) and motif_sites[end] - motif_sites[end - 1] <= min_separation:
+        while end < len(motif_sites) and motif_sites[end] - motif_sites[end - 1] <= min_separation + mv("separation", 0):
             end += 1
         groups.append((cur, end)); cur = end
     out = []
     for gs, ge in groups:
         first, last = motif_sites[gs], motif_sites[ge - 1]
         sub_start, sub_end, span = first - min_flank, last + min_flank, last - first
-        if sub_start <= min_separation or span > max_span:
+        if sub_start <= min_separation + mv("sub_start", 0) or span > max_span + mv("max_span", 0):
             continue
-        subseq = ref[sub_start:sub_end + 1]                       # substr: cut at the end of the string
+        subseq = ref[sub_start:min(sub_end + 1, len(ref) + mv("substr", 0))]     # substr: cut at the end of the string
         b = find_by_ref_bounds(pr_ref, pr_read, sub_start + ref_start_pos, sub_end + ref_start_pos)
-        if b is None or abs(b[1] - b[0]) <= min_event_span:
+        if b is None or abs(b[1] - b[0]) <= min_event_span + mv("event_span", 0):
             continue
         start_position, end_position = first + ref_start_pos, last + ref_start_pos
-        if (region_start != -1 and start_position < region_start) or (region_end != -1 and end_position >= region_end):
+        if (region_start != -1 and start_position < region_start + mv("region_start", 0)) or \
+                (region_end != -1 and end_position >= region_end + mv("region_end", 0)):
             continue
-        m_subseq = methylate(a, subseq)
+        m_subseq = methylate(a, subseq, mv("site_fit", 0), ref[sub_start + len(subseq):sub_start + len(subseq) + max(mv("site_fit", 0), 0)])
         ru = kmer_ranks(a, subseq, reverse_complement(a, subseq), k, rc)
         rm = kmer_ranks(a, m_subseq, reverse_complement(a, m_subseq), k, rc)
         out.append((start_position, end_position, ge - gs, b[0], b[1], ru, rm, ref[first - k + 1:last + k]))
