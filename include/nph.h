@@ -1110,6 +1110,61 @@ int nph_call_variant_groups_batch(nph_ctx* ctx, const nph_read* reads, size_t n_
                                   nph_call_group_result* groups_out, nph_call_variant_result* variants_out,
                                   nph_call_counts* counts_out);
 
+/* ---- variants: the basecall candidates of a region (AlignmentDB::get_variants_in_region) -------------------------------------
+ * (ref: src/alignment/nanopolish_alignment_db.cpp:259-368)  The pile-up of the base-space alignments of a loaded region: every
+ * mismatch or gap the reads show between reference positions start and stop, merged on (position, ref_seq, alt_seq), with its
+ * instance count and the read depth at its position.  Per record, in record order, over aligned_bases (the record's
+ * get_aligned_segments()[0]: (ref_pos, read_pos) pairs, both strictly increasing):
+ *   the bounds    start_iter = lower_bound(start), stop_iter = lower_bound(stop) by ref_pos
+ *   the depth     +1 over [max(start_iter->ref_pos, start), min(stop_iter == end ? back().ref_pos : stop_iter->ref_pos, stop)):
+ *                 deleted reference bases count, the record's last aligned base does not
+ *   the walk      from start_iter to stop_iter: is_gap = the next pair is not (ref + 1, read + 1) and is not stop_iter; on a gap,
+ *                 next = the first later pair whose read base equals its reference base (byte compare), else stop_iter; without
+ *                 one, next = the next pair.  (mismatch || gap) && next != stop_iter && next->ref_pos < stop - 1 is one instance:
+ *                 ref_seq = region_ref[i.ref, next.ref), alt_seq = bases[i.read, next.read)
+ * A record without a pair at or after start adds no depth and no instance (the reference dereferences end() there).
+ * A record's alignment comes in the compact form of nph_methylation_batch_compact, read positions in place of event indices:
+ * base_deltas[map_off + o] belongs to reference position ref_start_pos + o, NPH_METH_NO_PAIR where the record has no pair, else
+ * its read position minus the previous pair's (first_read_pos for the first pair, whose own delta is then 0).  A read-position
+ * step beyond int16 (an insertion of more than 32 767 bases) cannot be written in this form: the host mirror returns
+ * NPH_ERR_UNSUPPORTED for it.
+ * Out: one nph_region_candidate per distinct (ref_position, ref_seq, alt_seq), alt_seq = bases[alt_off, alt_off + alt_len) of one of
+ * its instances; in ascending ref_position, otherwise in no documented order (the reference's std::map order and its filter are the
+ * caller's: nph::get_variants_in_region).  count is exact; neither field depends on the order of the device's atomics.
+ * out_cap too small: NPH_ERR_INVALID with *n_out set to the count needed.  NPH_ERR_INVALID also for stop < start (the reference
+ * asserts), [start, stop] not inside [region_start, region_start + n_ref - 1], a record whose bases or alignment slice leave their
+ * arrays, whose read positions leave its bases or do not strictly increase (a non-first delta below 1).
+ * Counts: records, the pairs the walks visited, instances, distinct variants, and the device time of the call's kernels
+ * (region_candidates.cu: cand_walk_kernel, cand_rep_kernel, cand_emit_kernel, the scans, the radix sort). */
+typedef struct {
+    uint64_t seq_off;                 /* first base of the record's read in bases[] (seq_nt16_str characters, '=' and 'N' included) */
+    uint64_t map_off;                 /* first entry of its compact alignment in base_deltas[] */
+    uint32_t seq_len;                 /* bases of the read */
+    uint32_t map_len;                 /* reference positions its compact alignment covers (0: no pairs) */
+    int32_t  ref_start_pos;           /* reference position of base_deltas[map_off] */
+    int32_t  first_read_pos;          /* read position of the record's first pair */
+} nph_seq_record;                     /* 32 bytes */
+typedef struct {
+    int32_t  ref_position;            /* Variant::ref_position */
+    uint32_t ref_len;                 /* |ref_seq|: ref_seq = region_ref[ref_position - region_start, + ref_len) */
+    uint32_t alt_len;                 /* |alt_seq| */
+    uint32_t count;                   /* instances over all records */
+    uint32_t depth;                   /* the depth at ref_position */
+    uint32_t record;                  /* the record of the instance alt_off points into */
+    uint64_t alt_off;                 /* alt_seq = bases[alt_off, alt_off + alt_len) */
+} nph_region_candidate;               /* 32 bytes */
+typedef struct {
+    uint64_t n_records;               /* records of the call */
+    uint64_t n_pairs;                 /* pairs in [start_iter, stop_iter) over all records */
+    uint64_t n_instances;             /* mismatch or gap instances before the merge */
+    uint64_t n_variants;              /* distinct variants */
+    double   kernel_ms;               /* device time from the first kernel to the last (one read-back of the instance total between) */
+} nph_candidate_counts;               /* 40 bytes */
+int nph_region_candidates_batch(nph_ctx* ctx, const char* region_ref, size_t n_ref, int32_t region_start,
+                                const char* bases, size_t n_bases, const int16_t* base_deltas, size_t n_deltas,
+                                const nph_seq_record* records, size_t n_records, int32_t start, int32_t stop,
+                                nph_region_candidate* out, size_t out_cap, uint64_t* n_out, nph_candidate_counts* counts_out);
+
 /* ---- scorereads --train-transitions: forward scores and transition training counts of a job batch ----------------------------
  * `nanopolish scorereads --train-transitions` runs, for every segment model_score scores (src/nanopolish_scorereads.cpp:116-203),
  * profile_hmm_align(sequence, data) (K3, flags 0) after the forward score, and folds the path into

@@ -399,6 +399,13 @@ int nph_event_records_load(nph_ctx* ctx, NphEventRecords& ev, const char* ref, s
         if (!ok) { ctx->last_error = "record " + std::to_string(r) + " is out of range (read, model, reference or event-alignment slice)"; return NPH_ERR_INVALID; }
         NPH_TRY(check(r, R));
     }
+    return nph_event_records_upload(ctx, ev, ref, n_ref, n_map, compact, deltas, first_event, pairs, n_pairs, records, n_records);
+}
+
+int nph_event_records_upload(nph_ctx* ctx, NphEventRecords& ev, const char* ref, size_t n_ref, size_t n_map, bool compact,
+                             const int16_t* deltas, const int32_t* first_event, const nph_aligned_pair* pairs, size_t n_pairs,
+                             const nph_meth_record* records, size_t n_records)
+{
     NPH_CUDA(ctx, cudaSetDevice(ctx->device));
     ev.n_records = n_records; ev.n_ref = n_ref; ev.n_map = n_map; ev.compact = compact;
     NPH_TRY(nph_reserve(ctx, ev.d_ref, n_ref + 16));

@@ -244,6 +244,14 @@ struct nph_ctx {
         DevBuf<uint8_t> d_work;            // per-group offsets, masks, pair scores, key tables, partial maxima, group results
     } call;
 
+    // the last nph_region_candidates_batch (region_candidates.cu)
+    struct CandState {
+        NphEventRecords ev;                // region reference, compact base alignments (read position per reference base), records
+        DevBuf<uint8_t> d_seq;             // the records' read bases
+        DevBuf<uint8_t> d_work;            // depth differences and depth, per-record instance counts and offsets, scan scratch, flags
+        DevBuf<uint8_t> d_inst;            // instances, their sort keys and order, representatives, counts, output offsets, cub scratch
+    } cand;
+
     // the last nph_train_transitions_batch (transitions.cu)
     struct TtState {
         DevBuf<uint8_t> d_work;            // the group records, the refusal flags, the jobs' groups
@@ -440,6 +448,11 @@ int nph_event_records_load(nph_ctx* ctx, NphEventRecords& ev, const char* ref, s
                            const int16_t* deltas, const int32_t* first_event, const nph_aligned_pair* pairs, size_t n_pairs,
                            const nph_meth_record* records, size_t n_records, uint32_t max_len,
                            const std::function<int(size_t, const nph_meth_record&)>& check);
+// The upload half of nph_event_records_load, without its checks: the caller has checked every record's slices (region
+// candidates, whose records carry base alignments and name no read or model, call it directly).
+int nph_event_records_upload(nph_ctx* ctx, NphEventRecords& ev, const char* ref, size_t n_ref, size_t n_map, bool compact,
+                             const int16_t* deltas, const int32_t* first_event, const nph_aligned_pair* pairs, size_t n_pairs,
+                             const nph_meth_record* records, size_t n_records);
 // Compact form: the event index of every base (NPH_NO_EVENT: no entry) at dense[ref_off + o] and each record's first base with
 // an entry (ref_len: none) at first_valid[record].  Pair form: both nullptr, nothing launched.
 int nph_event_records_expand(nph_ctx* ctx, NphEventRecords& ev, const int32_t** dense, const int32_t** first_valid);

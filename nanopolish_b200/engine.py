@@ -10,7 +10,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from .synth import CALL_COUNTS_DT, CALL_GROUP_DT, CALL_GROUP_RESULT_DT, CALL_HAPLOTYPE_DT, CALL_VARIANT_RESULT_DT, ABEA_RES_DT, ALIGN_STATE_DT, CALIBRATION_DT, EVENT_DT, EVENT_RANGE_DT, METH_SITE_DT, METHFREQ_PARAMS_DT, HP_COUNTS_DT, HP_LIK_DT, HP_WINDOW_DT, PAIR_DT, PHASE_CALL_DT, PHASE_VARIANT_DT, POLYA_RES_DT, POLYI_RES_DT, RAW_RANGE_DT, SCREEN_CANDIDATE_DT, SCREEN_LIST_COUNTS_DT, SCREEN_RESULT_DT, SUPPORT_COUNTS_DT, SUPPORT_RESULT_DT, SUPPORT_VARIANT_DT
+from .synth import CANDIDATE_COUNTS_DT, REGION_CANDIDATE_DT, CALL_COUNTS_DT, CALL_GROUP_DT, CALL_GROUP_RESULT_DT, CALL_HAPLOTYPE_DT, CALL_VARIANT_RESULT_DT, ABEA_RES_DT, ALIGN_STATE_DT, CALIBRATION_DT, EVENT_DT, EVENT_RANGE_DT, METH_SITE_DT, METHFREQ_PARAMS_DT, HP_COUNTS_DT, HP_LIK_DT, HP_WINDOW_DT, PAIR_DT, PHASE_CALL_DT, PHASE_VARIANT_DT, POLYA_RES_DT, POLYI_RES_DT, RAW_RANGE_DT, SCREEN_CANDIDATE_DT, SCREEN_LIST_COUNTS_DT, SCREEN_RESULT_DT, SUPPORT_COUNTS_DT, SUPPORT_RESULT_DT, SUPPORT_VARIANT_DT
 
 
 def _p(a):
@@ -259,6 +259,28 @@ class Engine:
                                                            n_variants, indel_bias, _p(meth), _p(ids), _p(gout), _p(vout), _p(cnt)),
                     "nph_call_variant_groups_batch")
         return gout[:groups.shape[0]], vout[:n_variants], cnt[0]
+
+    def region_candidates_batch(self, region_ref, region_start: int, seq, deltas, records, start: int, stop: int, cap: int | None = None):
+        """nph_region_candidates_batch: region_ref u1 (or bytes), seq u1 (the records' bases), deltas i2, records SEQ_RECORD_DT.  Returns
+        (REGION_CANDIDATE_DT[n_variants], CANDIDATE_COUNTS_DT scalar); a first cap that is too small is retried once at the size needed."""
+        if isinstance(region_ref, str):
+            region_ref = region_ref.encode()
+        ref = np.frombuffer(region_ref, np.uint8) if isinstance(region_ref, bytes) else np.ascontiguousarray(region_ref, np.uint8)
+        seq = np.ascontiguousarray(seq, np.uint8)
+        deltas = np.ascontiguousarray(deltas, np.int16)
+        cnt = np.zeros(1, CANDIDATE_COUNTS_DT)
+        n = C.c_uint64(0)
+        cap = 1024 if cap is None else cap
+        for _ in range(2):
+            out = np.zeros(max(cap, 1), REGION_CANDIDATE_DT)
+            st = self.lib.nph_region_candidates_batch(self.ctx, _p(ref), ref.shape[0], region_start, _p(seq), seq.shape[0], _p(deltas), deltas.shape[0],
+                                                      _p(records), records.shape[0], start, stop, _p(out), cap, C.byref(n), _p(cnt))
+            if st == _lib.NPH_ERR_INVALID and n.value > cap:
+                cap = n.value
+                continue
+            self._check(st, "nph_region_candidates_batch")
+            return out[:n.value], cnt[0]
+        raise AssertionError("nph_region_candidates_batch: the retried cap was too small")
 
     def screen_load(self, ref_bases, deltas, first_event, records, params, indel_bias: float = 1.0, methylation=None):
         head = (self.ctx, _p(ref_bases), ref_bases.shape[0], _p(deltas), deltas.shape[0], _p(first_event), _p(records), records.shape[0], _p(params),

@@ -1148,4 +1148,73 @@ long long nphh_haplotype_ranges(int hap_pos, const char* hap_ref, int n_variants
     return st ? st : pos;
 }
 
+// the base-space records of a region: record r's bases seq_bases[r], strand seq_rc[r], aligned_bases the (ref_pos, read_pos) pairs
+// seq_pairs[2 * seq_pair_off[r] ..) up to seq_pair_off[r + 1]
+static void add_sequence_records(RegionAlignments& region, int n_seq, const char** seq_bases, const uint8_t* seq_rc, const int32_t* seq_pairs,
+                                 const uint64_t* seq_pair_off)
+{
+    for (int r = 0; r < n_seq; ++r) {
+        SequenceAlignedRead sr;
+        sr.read_name = "seq" + std::to_string(r);
+        sr.rc = seq_rc[r] != 0;
+        sr.sequence = seq_bases[r];
+        const uint64_t np = seq_pair_off[r + 1] - seq_pair_off[r];
+        sr.aligned_bases.resize(np);
+        if (np) std::memcpy(sr.aligned_bases.data(), seq_pairs + 2 * seq_pair_off[r], sizeof(AlignedPair) * np);
+        region.sequence_records.push_back(std::move(sr));
+    }
+}
+
+// nph::get_variants_in_region over the region [region_start, region_start + strlen(region_ref) - 1] of `contig` and the base-space
+// records of add_sequence_records.  out: one line per variant in the returned order, "ref_position \t ref_seq \t alt_seq \t info";
+// counts (optional): nph_candidate_counts.  Returns the length written, or a negative nph_status.
+long long nphh_variants_in_region(const char* contig, int region_start, const char* region_ref, int n_seq, const char** seq_bases, const uint8_t* seq_rc,
+                                  const int32_t* seq_pairs, const uint64_t* seq_pair_off, int start, int stop, double min_frequency, int min_depth,
+                                  nph_candidate_counts* counts, char* out, size_t cap)
+{
+    long long n = -1;
+    int st = guard([&] {
+        RegionAlignments region = region_of(contig, region_start, region_ref, 0, nullptr, nullptr, nullptr, nullptr);
+        add_sequence_records(region, n_seq, seq_bases, seq_rc, seq_pairs, seq_pair_off);
+        std::string s;
+        for (const Variant& v : get_variants_in_region(region, start, stop, min_frequency, min_depth, Engine::thread_default(), counts))
+            s += std::to_string(v.ref_position) + "\t" + v.ref_seq + "\t" + v.alt_seq + "\t" + v.info + "\n";
+        n = write_out(s, out, cap);
+    });
+    return st ? st : n;
+}
+
+// `nanopolish variants` on one window in its default mode: nph::call_variants_for_region then nph::write_variants_vcf, over the
+// region [region_start, ...] of nphh_call_haplotype's event records (record r's read named read_names[r]) and add_sequence_records'
+// base-space records.  candidates_vcf: NULL, or the --candidates file's text; types_csv: the -q types.  out: the VCF.  Returns the
+// length written, or a negative nph_status.
+long long nphh_call_region(const char* contig, int contig_length, int start_base, int end_base, int region_start, const char* region_ref,
+                           int n_records, const int32_t* read, const uint8_t* rc, const int32_t* pairs, const uint64_t* pair_off, const char** read_names,
+                           int n_seq, const char** seq_bases, const uint8_t* seq_rc, const int32_t* seq_pairs, const uint64_t* seq_pair_off,
+                           int flank, int min_distance, int max_haplotypes, int ploidy, int genotype_only, const char* types_csv,
+                           int calculate_all_support, int snps_only, double min_frequency, int min_depth, const char* candidates_vcf,
+                           double indel_bias, char* out, size_t cap)
+{
+    long long n = -1;
+    int st = guard([&] {
+        for (int r = 0; r < n_records; ++r) g_reads[read[r]]->read_name = read_names[r];
+        RegionAlignments region = region_of(contig, region_start, region_ref, n_records, read, rc, pairs, pair_off);
+        add_sequence_records(region, n_seq, seq_bases, seq_rc, seq_pairs, seq_pair_off);
+        CallVariantsOptions o;
+        o.min_flanking_sequence = flank; o.min_distance_between_variants = min_distance; o.max_haplotypes = max_haplotypes;
+        o.ploidy = ploidy; o.genotype_only = genotype_only != 0; o.calculate_all_support = calculate_all_support != 0;
+        o.snps_only = snps_only != 0; o.min_candidate_frequency = min_frequency; o.min_candidate_depth = min_depth;
+        for (std::string s = types_csv; !s.empty(); ) {
+            const size_t c = s.find(',');
+            o.methylation_types.push_back(s.substr(0, c));
+            s = c == std::string::npos ? std::string() : s.substr(c + 1);
+        }
+        if (candidates_vcf) { o.use_candidates = true; o.candidates_vcf = candidates_vcf; }
+        const int end = std::min(end_base, contig_length - 1);
+        const Haplotype called = call_variants_for_region(region, start_base, end, contig_length, o, Engine::thread_default(), indel_bias);
+        n = write_out(write_variants_vcf(region, start_base, end, contig_length, o, called), out, cap);
+    });
+    return st ? st : n;
+}
+
 } // extern "C"

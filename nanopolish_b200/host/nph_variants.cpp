@@ -4,7 +4,9 @@
 #include <algorithm>
 #include <cmath>
 #include <cstring>
+#include <cstdio>
 #include <iomanip>
+#include <map>
 #include <sstream>
 
 namespace nph {
@@ -597,14 +599,14 @@ struct TableProbability {
     }
 };
 
+} // namespace
+
 std::string format_double(double v)
 {
     std::stringstream ss;
     ss << v;
     return ss.str();
 }
-
-} // namespace
 
 double fisher_exact_two_sided(int n11, int n12, int n21, int n22)
 {
@@ -775,6 +777,146 @@ Haplotype call_haplotype_from_candidates(const RegionAlignments& alignments, con
     for (const std::vector<Variant>& c : calls)
         for (const Variant& v : c) derived.apply_variant(v);
     return derived;
+}
+
+std::vector<Variant> get_variants_in_region(const RegionAlignments& alignments, int start, int stop, double min_frequency, int min_depth,
+                                            Engine& engine, nph_candidate_counts* counts_out)
+{
+    std::string seq;
+    std::vector<int16_t> deltas;
+    std::vector<nph_seq_record> recs(alignments.sequence_records.size());
+    for (size_t r = 0; r < recs.size(); ++r) {
+        const SequenceAlignedRead& sr = alignments.sequence_records[r];
+        const std::vector<AlignedPair>& ab = sr.aligned_bases;
+        nph_seq_record& R = recs[r];
+        std::memset(&R, 0, sizeof(R));
+        R.seq_off = seq.size(); R.seq_len = (uint32_t)sr.sequence.size();
+        seq += sr.sequence;
+        if (ab.empty()) continue;
+        for (size_t i = 1; i < ab.size(); ++i)
+            if (ab[i].ref_pos <= ab[i - 1].ref_pos || ab[i].read_pos <= ab[i - 1].read_pos)
+                throw Error(NPH_ERR_INVALID, "get_variants_in_region: record " + std::to_string(r) + ": its pairs do not strictly increase");
+        R.ref_start_pos = ab.front().ref_pos;
+        R.map_len = (uint32_t)(ab.back().ref_pos - ab.front().ref_pos + 1);
+        R.map_off = deltas.size();
+        deltas.resize(deltas.size() + R.map_len);
+        if (!compact_event_alignment(ab, R.ref_start_pos, R.map_len, deltas.data() + R.map_off, &R.first_read_pos))
+            throw Error(NPH_ERR_UNSUPPORTED, "get_variants_in_region: record " + std::to_string(r) + ": a read-position step beyond int16");
+    }
+    if (seq.empty()) seq.push_back('\0');
+    if (deltas.empty()) deltas.push_back(0);
+    std::vector<nph_region_candidate> cand(1024);
+    uint64_t n = 0;
+    nph_candidate_counts counts;
+    int st = nph_region_candidates_batch(engine.ctx(), alignments.reference.data(), alignments.reference.size(), alignments.region_start, seq.data(),
+                                         seq.size(), deltas.data(), deltas.size(), recs.data(), recs.size(), start, stop, cand.data(), cand.size(), &n, &counts);
+    if (st == NPH_ERR_INVALID && n > cand.size()) {
+        cand.resize(n);
+        st = nph_region_candidates_batch(engine.ctx(), alignments.reference.data(), alignments.reference.size(), alignments.region_start, seq.data(),
+                                         seq.size(), deltas.data(), deltas.size(), recs.data(), recs.size(), start, stop, cand.data(), cand.size(), &n, &counts);
+    }
+    engine.check(st, "nph_region_candidates_batch");
+    if (counts_out) *counts_out = counts;
+    // the reference's filter, then its std::map<std::string, ...> order over Variant::key() and its sort (ref: :346-366).  The filter
+    // reads only the count and the depth, so it runs first: the map then holds the kept variants alone, in the same relative order
+    std::map<std::string, Variant> by_key;
+    for (size_t i = 0; i < n; ++i) {
+        const nph_region_candidate& c = cand[i];
+        const size_t count = c.count, d = c.depth;
+        const double f = (double)count / d;
+        if (!(f >= min_frequency && (int)d >= min_depth)) continue;
+        Variant v;
+        v.ref_name = alignments.contig;
+        v.ref_position = (size_t)c.ref_position;
+        v.ref_seq = alignments.reference.substr((size_t)(c.ref_position - alignments.region_start), c.ref_len);
+        v.alt_seq = seq.substr((size_t)c.alt_off, c.alt_len);
+        v.add_info("BaseCalledReadsWithVariant", count);
+        v.add_info("BaseCalledFraction", format_double(f));
+        by_key.emplace(v.key(), std::move(v));
+    }
+    std::vector<Variant> variants;
+    variants.reserve(by_key.size());
+    for (auto& kv : by_key) variants.push_back(std::move(kv.second));
+    std::sort(variants.begin(), variants.end(), [](const Variant& a, const Variant& b) {
+        return a.ref_name == b.ref_name ? a.ref_position < b.ref_position : a.ref_name < b.ref_name;
+    });
+    return variants;
+}
+
+std::vector<Variant> read_variants_for_region(const std::string& text, const std::string& contig, int region_start, int region_end)
+{
+    std::vector<Variant> out;
+    std::istringstream in(text);
+    std::string line;
+    while (std::getline(in, line)) {
+        if (!line.empty() && line[0] == '#') continue;
+        std::stringstream ss(line);
+        std::string dummy;
+        Variant v;
+        ss >> v.ref_name >> v.ref_position >> dummy >> v.ref_seq >> v.alt_seq >> v.quality >> v.filter >> v.info >> dummy >> v.genotype;
+        v.ref_position -= 1;
+        if (v.ref_name.empty() || v.ref_seq.empty() || v.alt_seq.empty() || v.quality < 0.0f)
+            throw Error(NPH_ERR_INVALID, "read_variants_for_region: a line Variant::read_vcf asserts on");
+        if (v.ref_name == contig && (int)v.ref_position >= region_start && (int)v.ref_position <= region_end) {
+            v.info.clear();
+            out.push_back(v);
+        }
+    }
+    return out;
+}
+
+Haplotype call_variants_for_region(const RegionAlignments& alignments, int start_base, int end_base, int contig_length,
+                                   const CallVariantsOptions& o, Engine& engine, double indel_bias)
+{
+    if (start_base > end_base) throw Error(NPH_ERR_INVALID, "call_variants_for_region: the window's start is after its end");
+    if (contig_length - start_base < 40) throw Error(NPH_ERR_INVALID, "call_variants_for_region: the window starts within 40 bases of the contig's end");
+    const int BUFFER = o.min_flanking_sequence + 10;
+    const int region_start = std::max(start_base, BUFFER);
+    if (alignments.region_start != region_start - BUFFER || alignments.reference.empty())
+        throw Error(NPH_ERR_INVALID, "call_variants_for_region: the region is not loaded at region_start - BUFFER");
+    const int region_end = alignments.region_start + (int)alignments.reference.size() - 1 - BUFFER;
+    const std::vector<Variant> candidates = o.use_candidates
+        ? read_variants_for_region(o.candidates_vcf, alignments.contig, region_start, region_end)
+        : get_variants_in_region(alignments, region_start, region_end, o.min_candidate_frequency, o.min_candidate_depth, engine);
+    return call_haplotype_from_candidates(alignments, candidates, NPH_HAF_ALLOW_PRE_CLIP | NPH_HAF_ALLOW_POST_CLIP, o.min_flanking_sequence,
+                                          o.min_distance_between_variants, o.max_haplotypes, o.ploidy, o.genotype_only, o.methylation_types,
+                                          o.calculate_all_support, engine, indel_bias);
+}
+
+std::string write_variants_vcf(const RegionAlignments& alignments, int start_base, int end_base, int contig_length,
+                               const CallVariantsOptions& o, const Haplotype& called)
+{
+    const auto tag = [](const char* t, const char* id, int count, const char* type, const char* desc) {
+        return std::string("##") + t + "=<ID=" + id + ",Number=" + std::to_string(count) + ",Type=" + type + ",Description=\"" + desc + "\">\n";
+    };
+    std::string s = "##fileformat=VCFv4.2\n";
+    s += "##nanopolish_window=" + alignments.contig + ":" + std::to_string(start_base) + "-" + std::to_string(std::min(end_base, contig_length - 1)) + "\n";
+    s += tag("INFO", "TotalReads", 1, "Integer", "The number of event-space reads used to call the variant");
+    s += tag("INFO", "SupportFraction", 1, "Float", "The fraction of event-space reads that support the variant");
+    s += tag("INFO", "SupportFractionByStrand", 2, "Float", "Fraction of event-space reads that support the variant for each strand");
+    s += tag("INFO", "BaseCalledReadsWithVariant", 1, "Integer", "The number of base-space reads that support the variant");
+    s += tag("INFO", "BaseCalledFraction", 1, "Float", "The fraction of base-space reads that support the variant");
+    s += tag("INFO", "AlleleCount", 1, "Integer", "The inferred number of copies of the allele");
+    s += tag("INFO", "StrandSupport", 4, "Integer", "Number of reads supporting the REF and ALT allele, by strand");
+    s += tag("INFO", "StrandFisherTest", 1, "Integer", "Strand bias fisher test");
+    s += tag("INFO", "SOR", 1, "Float", "StrandOddsRatio test from GATK");
+    s += tag("INFO", "RefContext", 1, "String", "The reference sequence context surrounding the variant call");
+    if (o.calculate_all_support) s += tag("INFO", "SupportFractionByBase", 4, "Float", "The fraction of reads supporting A,C,G,T at this position");
+    s += tag("FORMAT", "GT", 1, "String", "Genotype");
+    s += "#CHROM\tPOS\tID\tREF\tALT\tQUAL\tFILTER\tINFO\tFORMAT\tsample\n";
+    for (Variant v : called.get_variants()) {
+        if (o.snps_only && !(v.ref_seq.size() == 1 && v.alt_seq.size() == 1)) continue;
+        const int cs = std::max((int)v.ref_position - 5, 0);
+        const int ce = std::min((int)(v.ref_position + v.ref_seq.length() + 4), contig_length - 1);
+        const int lo = alignments.region_start, hi = alignments.region_start + (int)alignments.reference.size() - 1;
+        if (cs < lo || ce > hi || ce < cs) throw Error(NPH_ERR_INVALID, "write_variants_vcf: a RefContext outside the loaded region");
+        v.add_info("RefContext", alignments.reference.substr((size_t)(cs - lo), (size_t)(ce - cs + 1)));
+        char q[64];
+        std::snprintf(q, sizeof(q), "%.1lf", v.quality);
+        s += v.ref_name + "\t" + std::to_string(v.ref_position + 1) + "\t.\t" + v.ref_seq + "\t" + v.alt_seq + "\t" + q + "\t" +
+             (v.filter.empty() ? std::string("PASS") : v.filter) + "\t" + v.info + "\tGT\t" + (v.genotype.empty() ? std::string(".") : v.genotype) + "\n";
+    }
+    return s;
 }
 
 } // namespace nph

@@ -128,13 +128,24 @@ std::vector<Variant> score_variants_thresholded(const std::vector<Variant>& inpu
 Variant score_variant_thresholded(const Variant& input_variant, Haplotype base_haplotype, const std::vector<HMMInputData>& input,
                                   uint32_t alignment_flags, uint32_t score_threshold, const std::vector<std::string>& methylation_types);
 
+// One SequenceAlignmentRecord of AlignmentDB (ref: src/alignment/nanopolish_alignment_db.h): the read's name and strand, its bases as
+// stored in the BAM (seq_nt16_str characters, '=' and 'N' included) and aligned_bases = get_aligned_segments(record)[0]
+struct SequenceAlignedRead {
+    std::string read_name;
+    bool rc = false;
+    std::string sequence;
+    std::vector<AlignedPair> aligned_bases;
+};
+
 // The AlignmentDB fix_homopolymers reads: the region [region_start, region_start + reference.size() - 1] of one contig and its event
 // alignment records in AlignmentDB's order, each strand 0 of its read (read->events[0] with durations; rc[0], aligned_events[0]).
+// sequence_records: the base-space records (get_variants_in_region reads them; the event-space calls do not).
 struct HomopolymerRegion {
     std::string contig;
     int region_start = 0;
     std::string reference;
     std::vector<EventAlignedRead> records;
+    std::vector<SequenceAlignedRead> sequence_records;
 };
 
 // One homopolymer fix_homopolymers scores, in scan order: the run, its calling window and the nph_hp_window it becomes.
@@ -223,5 +234,59 @@ Haplotype call_haplotype_from_candidates(const RegionAlignments& alignments, con
                                          uint32_t alignment_flags, int flank, int min_distance, int max_haplotypes, int ploidy,
                                          bool genotype_only, const std::vector<std::string>& methylation_types, bool calculate_all_support,
                                          Engine& engine, double indel_bias = hmm_indel_bias_factor, nph_call_counts* counts_out = nullptr);
+
+// std::stringstream << v with the stream's defaults (precision 6: 0.333333, 1, 5e-05), as the reference's Variant::add_info writes a double
+std::string format_double(double v);
+
+// AlignmentDB::get_variants_in_region(contig, start, stop, min_frequency, min_depth) (ref: src/alignment/nanopolish_alignment_db.cpp:
+// 259-368) over alignments.sequence_records: the pile-up and merge in one nph_region_candidates_batch, then the reference's order on the
+// host: the distinct variants in std::map order of their keys "contig:pos:ref:alt" (bytewise: "1000:..." < "100:..."), kept when
+// (double)count / depth >= min_frequency && depth >= min_depth, INFO BaseCalledReadsWithVariant=count;BaseCalledFraction=f
+// (format_double), then std::sort by position (not stable: the order among variants at one position is std::sort's, which reaches
+// the VCF through call_haplotype_from_candidates' grouping).  Throws Error(NPH_ERR_INVALID) for stop < start, [start, stop] outside
+// the region, a record whose pairs do not strictly increase or leave its bases; Error(NPH_ERR_UNSUPPORTED) for a read-position step
+// beyond int16 (an insertion of more than 32 767 bases).  counts_out (optional): the device call's counters.
+std::vector<Variant> get_variants_in_region(const RegionAlignments& alignments, int start, int stop, double min_frequency, int min_depth,
+                                            Engine& engine, nph_candidate_counts* counts_out = nullptr);
+
+// read_variants_for_region (ref: src/common/nanopolish_variant.cpp:81-108): the VCF lines of `text` (headers skipped) parsed as
+// Variant::read_vcf parses them, kept when on `contig` with (int)ref_position in [region_start, region_end], INFO cleared.  Throws
+// Error(NPH_ERR_INVALID) where read_vcf asserts: an empty contig, REF or ALT, a negative quality (an empty line included).
+std::vector<Variant> read_variants_for_region(const std::string& text, const std::string& contig, int region_start, int region_end);
+
+// The options of `nanopolish variants` that its default (non-consensus) mode reads, with the reference's defaults
+// (ref: src/nanopolish_call_variants.cpp:115-140).  min_candidate_frequency is the float literal 0.2f widened to double.
+struct CallVariantsOptions {
+    int min_flanking_sequence = 30;
+    int min_distance_between_variants = 10;
+    int max_haplotypes = 1000;
+    int ploidy = 0;                             // -p: required by the reference
+    bool genotype_only = false;
+    bool calculate_all_support = false;
+    bool snps_only = false;
+    double min_candidate_frequency = 0.2f;
+    int min_candidate_depth = 20;
+    std::vector<std::string> methylation_types;
+    bool use_candidates = false;                // --candidates: candidates_vcf holds the file's text
+    std::string candidates_vcf;
+};
+
+// call_variants_for_region (ref: src/nanopolish_call_variants.cpp:882-1011) in its default mode, with main's window checks
+// (:1131-1170): start_base and end_base as main has them (end clamped to contig_length - 1).  BUFFER = min_flanking_sequence + 10,
+// region_start = max(start_base, BUFFER); `alignments` is the region loaded over [region_start - BUFFER, min(end_base + BUFFER,
+// contig_length - 1)], region_end = its last base - BUFFER.  Candidates: get_variants_in_region(region_start, region_end,
+// min_candidate_frequency, min_candidate_depth), or read_variants_for_region over candidates_vcf; then call_haplotype_from_candidates
+// with NPH_HAF_ALLOW_PRE_CLIP | NPH_HAF_ALLOW_POST_CLIP.  Throws Error(NPH_ERR_INVALID) for start_base > end_base, contig_length -
+// start_base < 40, and a region not loaded at region_start - BUFFER.
+Haplotype call_variants_for_region(const RegionAlignments& alignments, int start_base, int end_base, int contig_length,
+                                   const CallVariantsOptions& options, Engine& engine, double indel_bias = hmm_indel_bias_factor);
+
+// The VCF call_variants_main writes (ref: src/nanopolish_call_variants.cpp:1172-1278): the header (##fileformat, ##nanopolish_window=
+// contig:start_base-end_base, the INFO and FORMAT tag lines in the reference's order, SupportFractionByBase only with
+// calculate_all_support, the #CHROM line), then per variant of `called` (SNPs only with snps_only) INFO RefContext = the reference
+// over [max(pos - 5, 0), min(pos + |ref| + 4, contig_length - 1)], taken from `alignments`, and Variant::write_vcf's line.  Throws
+// Error(NPH_ERR_INVALID) for a context outside the loaded region.
+std::string write_variants_vcf(const RegionAlignments& alignments, int start_base, int end_base, int contig_length,
+                               const CallVariantsOptions& options, const Haplotype& called);
 
 } // namespace nph

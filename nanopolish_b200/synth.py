@@ -982,3 +982,96 @@ def gen_pileup_methylated(ref_len: int, depth: int, read_bases: int, model: Pore
 
     return gen_pileup(ref_len, depth, read_bases, model, seed=seed, region_start=region_start, n_true_variants=0, rc_every=rc_every,
                       sequences=plant, read_levels=levels)
+
+
+# ---- get_variants_in_region (nph_region_candidates_batch) ------------------------------------------------------------------
+SEQ_RECORD_DT = np.dtype([("seq_off", "<u8"), ("map_off", "<u8"), ("seq_len", "<u4"), ("map_len", "<u4"), ("ref_start_pos", "<i4"),
+                          ("first_read_pos", "<i4")], align=True)
+REGION_CANDIDATE_DT = np.dtype([("ref_position", "<i4"), ("ref_len", "<u4"), ("alt_len", "<u4"), ("count", "<u4"), ("depth", "<u4"),
+                                ("record", "<u4"), ("alt_off", "<u8")], align=True)
+CANDIDATE_COUNTS_DT = np.dtype([("n_records", "<u8"), ("n_pairs", "<u8"), ("n_instances", "<u8"), ("n_variants", "<u8"), ("kernel_ms", "<f8")],
+                               align=True)
+assert SEQ_RECORD_DT.itemsize == 32 and REGION_CANDIDATE_DT.itemsize == 32 and CANDIDATE_COUNTS_DT.itemsize == 40
+
+
+def seq_records(bases: list, aligned: list):
+    """Base-space records -> the inputs of nph_region_candidates_batch: (bases u1, deltas i2, SEQ_RECORD_DT).  bases[r] is record r's
+    read (bytes), aligned[r] its aligned_bases as an (n, 2) array of (ref_pos, read_pos); the compact form is compact_event_alignment's
+    over [first ref_pos, last ref_pos].  Raises OverflowError for a read-position step beyond int16."""
+    n = len(bases)
+    recs = np.zeros(n, SEQ_RECORD_DT)
+    tmp = np.zeros(n, METH_RECORD_DT)
+    pairs, seq = [], []
+    soff = poff = moff = 0
+    for r in range(n):
+        a = np.asarray(aligned[r], np.int64).reshape(-1, 2)
+        recs[r]["seq_off"], recs[r]["seq_len"] = soff, len(bases[r])
+        seq.append(np.frombuffer(bytes(bases[r]), np.uint8))
+        soff += len(bases[r])
+        if a.shape[0]:
+            ml = int(a[-1, 0] - a[0, 0] + 1)
+            recs[r]["ref_start_pos"], recs[r]["map_len"], recs[r]["map_off"] = int(a[0, 0]), ml, moff
+            recs[r]["first_read_pos"] = int(a[0, 1])
+            tmp[r]["ref_off"], tmp[r]["ref_len"], tmp[r]["ref_start_pos"] = moff, ml, int(a[0, 0])
+            tmp[r]["pair_off"], tmp[r]["n_pairs"] = poff, a.shape[0]
+            pr = np.zeros(a.shape[0], PAIR_DT)
+            pr["ref_pos"], pr["read_pos"] = a[:, 0], a[:, 1]
+            pairs.append(pr)
+            poff += a.shape[0]
+            moff += ml
+    pr = np.concatenate(pairs) if pairs else np.zeros(0, PAIR_DT)
+    deltas, _ = compact_event_alignment(tmp, pr, moff) if moff else (np.zeros(0, np.int16), None)
+    flat = np.concatenate(seq) if seq else np.zeros(0, np.uint8)
+    return flat, deltas, recs
+
+
+def basecall_of(truth: str, t0: int, n: int, rng, p_sub: float = 0.0, p_ins: float = 0.0, p_del: float = 0.0, clip=(0, 0)):
+    """A basecall of truth[t0, t0 + n) with substitutions, 1-3 base insertions and deletions at the given per-base rates and soft clips
+    of clip[0] / clip[1] random bases, and its aligned_bases against the truth coordinates (offset t0 = reference position t0): the
+    M/=/X columns of its alignment, (ref, read) strictly increasing."""
+    out, pairs = [rng.choice(list("ACGT"), clip[0]).tolist()], []
+    out = list(out[0])
+    for i in range(t0, t0 + n):
+        u = rng.random()
+        if u < p_del and i not in (t0, t0 + n - 1):
+            continue
+        b = truth[i]
+        if rng.random() < p_sub:
+            b = "ACGT"[("ACGT".index(b) + int(rng.integers(1, 4))) % 4] if b in "ACGT" else "A"
+        pairs.append((i, len(out)))
+        out.append(b)
+        if rng.random() < p_ins and i != t0 + n - 1:
+            out += rng.choice(list("ACGT"), int(rng.integers(1, 4))).tolist()
+    out += rng.choice(list("ACGT"), clip[1]).tolist()
+    return "".join(out).encode(), np.array(pairs, np.int64).reshape(-1, 2)
+
+
+def gen_basecall_pileup(ref_len: int, depth: int, read_bases: int, model: PoreModel, seed: int = 42, region_start: int = 5000,
+                        n_true_variants: int = 0, rc_every: int = 2, p_sub: float = 0.03, p_ins: float = 0.03, p_del: float = 0.03,
+                        max_clip: int = 0):
+    """gen_pileup's draft, truth, reads and event alignments, plus each read's basecall: its truth slice with seeded substitution,
+    insertion and deletion rates and soft clips of up to max_clip bases, aligned to the draft coordinates.  Returns a dict with draft
+    (str), truth (str), region_start, rs, recs, pairs (gen_pileup's), names, rc, bases (list of bytes), aligned (list of (n, 2)
+    aligned_bases) and the flat inputs seq, deltas, seq_recs (seq_records)."""
+    seqs = {}
+
+    def keep(draft, truth):
+        seqs["draft"], seqs["truth"] = draft, truth
+        return draft, truth
+    ref, rs, recs, pairs = gen_pileup(ref_len, depth, read_bases, model, seed=seed, region_start=region_start, n_true_variants=n_true_variants,
+                                      rc_every=rc_every, sequences=keep)
+    draft = bytes(b"ACGT"[c] for c in seqs["draft"]).decode()
+    truth = bytes(b"ACGT"[c] for c in seqs["truth"]).decode()
+    rng = np.random.default_rng(seed * 31337 + 5)
+    bases, aligned = [], []
+    for R in recs:
+        t0 = int(R["ref_start_pos"]) - region_start
+        n = int(R["ref_len"])
+        clip = (int(rng.integers(0, max_clip + 1)), int(rng.integers(0, max_clip + 1))) if max_clip else (0, 0)
+        b, a = basecall_of(truth, t0, n, rng, p_sub, p_ins, p_del, clip)
+        a[:, 0] += region_start
+        bases.append(b)
+        aligned.append(a)
+    seq, deltas, seq_recs = seq_records(bases, aligned)
+    return dict(draft=draft, truth=truth, region_start=region_start, rs=rs, recs=recs, pairs=pairs, names=[f"read{r}" for r in range(recs.shape[0])],
+                rc=[int(x) for x in recs["rc"]], bases=bases, aligned=aligned, seq=seq, deltas=deltas, seq_recs=seq_recs)
