@@ -242,12 +242,13 @@ class _NpoTailResult(C.Structure):
 
 
 class RefOracle:
-    """The compiled reference.  Reads are registered once (npref_read_create) and addressed by handle."""
+    """The compiled reference: libnpref.so, or another library linked from its objects plus a harness (path).  Reads are registered
+    once (npref_read_create) and addressed by handle."""
 
-    def __init__(self):
-        if not os.path.exists(REF_SO):
-            raise FileNotFoundError(REF_SO + " (run `make -C oracle ref` where /root/reference exists)")
-        self.lib = L = C.CDLL(REF_SO)
+    def __init__(self, path: str = REF_SO):
+        if not os.path.exists(path):
+            raise FileNotFoundError(path + " (built by oracle/'s make files where the reference sources exist)")
+        self.lib = L = C.CDLL(path)
         L.npref_score_batch.restype = C.c_double
         L.npref_abea_batch.restype = C.c_double
         L.npref_abea.restype = C.c_int64
@@ -260,8 +261,8 @@ class RefOracle:
         self._models = {}
 
     @staticmethod
-    def available() -> bool:
-        return os.path.exists(REF_SO)
+    def available(path: str = REF_SO) -> bool:
+        return os.path.exists(path)
 
     def has(self, entry: str) -> bool:
         """whether this build of the library exports a harness entry point (one built before the entry existed does not)"""

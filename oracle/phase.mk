@@ -3,8 +3,7 @@
 # Builds oracle/_ref/libnpref_phase.so: libnpref.so's objects (the UNMODIFIED reference translation units oracle/Makefile compiles
 # in place from $(REF), and ref_harness.o), the reference's src/common/nanopolish_bam_utils.cpp (write_bam_vardata), and
 # phase_reads_harness.cpp, which compiles src/nanopolish_phase_reads.cpp in place (it #includes it) so that the reference's own
-# phase_single_read runs.  Two symbols are wrapped (-Wl,--wrap): the SquiggleRead constructor that loads from a ReadDB, and
-# adaptive_banded_simple_event_align, through whose call in npref_abea the harness finds a read by its handle.  Same flags, one
+# phase_single_read runs.  One symbol is wrapped (-Wl,--wrap): the SquiggleRead constructor that loads from a ReadDB.  Same flags, one
 # section per function, the same --gc-sections link and export list as libnpref.so: phase_reads_main and the ReadDB / BAM code
 # it reaches are dropped.
 # Usage: make -C oracle -f phase.mk
@@ -20,11 +19,10 @@ phase:
 	@echo "oracle: $(REF) not present (GPU box): using prebuilt $(OUT)/libnpref_phase.so if any"
 endif
 
-PHASE_WRAP := _ZN12SquiggleReadC1ERKNSt7__cxx1112basic_stringIcSt11char_traitsIcESaIcEEERK6ReadDBj \
-              _Z34adaptive_banded_simple_event_alignR12SquiggleReadRK9PoreModelRKNSt7__cxx1112basic_stringIcSt11char_traitsIcESaIcEEE
+PHASE_WRAP := _ZN12SquiggleReadC1ERKNSt7__cxx1112basic_stringIcSt11char_traitsIcESaIcEEERK6ReadDBj
 
 $(OUT)/obj/phase_reads_harness.o $(OUT)/obj/nanopolish_bam_utils.o: REFFLAGS += -ffunction-sections -fdata-sections
-$(OUT)/obj/phase_reads_harness.o: phase_reads_harness.cpp $(REF)/src/nanopolish_phase_reads.cpp
+$(OUT)/obj/phase_reads_harness.o: phase_reads_harness.cpp ref_harness.h $(REF)/src/nanopolish_phase_reads.cpp
 	@mkdir -p $(OUT)/obj
 	$(CXX) $(REFFLAGS) $(REFINC) -c $< -o $@
 $(OUT)/obj/nanopolish_bam_utils.o: $(REF)/src/common/nanopolish_bam_utils.cpp

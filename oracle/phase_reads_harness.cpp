@@ -3,8 +3,8 @@
 //
 // What the function reaches outside its computation is answered by test doubles:
 //   SquiggleRead(name, read_db)  the constructor that loads a read from a ReadDB is routed (-Wl,--wrap, oracle/phase.mk) to a copy
-//                                of a read assembled by npref_read_create + npref_read_set_eventalign (ref_harness.cpp); its
-//                                handle is taken through npref_abea, whose call of adaptive_banded_simple_event_align is wrapped too
+//                                of a read assembled by npref_read_create + npref_read_set_eventalign (ref_harness.cpp), found by
+//                                its handle through npref_read_of
 //   faidx_fetch_seq, bam_endpos  ref_harness.cpp's doubles (the contig held in memory)
 //   bam_init1, bam_destroy1      calloc / free of a record
 //   sam_write1                   keeps the record; npref_phase_read prints it as a SAM line (the mandatory fields of the SAM
@@ -13,17 +13,15 @@
 //                                either case; every other byte is N)
 // Nothing of the reference or of htslib is copied.
 #include "nanopolish_phase_reads.cpp"
+#include "ref_harness.h"
 
 #include <cstdio>
 #include <new>
 
 extern double hmm_indel_bias_factor;                  // src/hmm/nanopolish_profile_hmm_r9.cpp:19
-struct NprefContig { std::string name, seq; };       // ref_harness.cpp: what its faidx_fetch_seq double reads behind a faidx_t*
-extern "C" long long npref_abea(int read_h, int model_h, const char* seq, int32_t* pairs_out, size_t cap);   // ref_harness.cpp
 
 namespace {
-thread_local bool g_capture = false;
-thread_local const SquiggleRead* g_read = nullptr;
+thread_local int g_read_h = -1;                       // the handle whose read the wrapped constructor copies
 thread_local std::string g_sam;                       // the last record sam_write1 received, as a SAM line
 thread_local bool g_written = false;
 
@@ -40,22 +38,14 @@ constexpr unsigned char nt16(int c, int i = 0)
 #define NT16_64(c) NT16_16(c), NT16_16(c + 16), NT16_16(c + 32), NT16_16(c + 48)
 extern "C" const unsigned char seq_nt16_table[256] = { NT16_64(0), NT16_64(64), NT16_64(128), NT16_64(192) };
 
-// ---- wrapped symbols (oracle/phase.mk links with --wrap=<mangled name> for both) ----
-extern "C" std::vector<AlignedPair> __real__Z34adaptive_banded_simple_event_alignR12SquiggleReadRK9PoreModelRKNSt7__cxx1112basic_stringIcSt11char_traitsIcESaIcEEE(
-    SquiggleRead&, const PoreModel&, const std::string&);
-extern "C" std::vector<AlignedPair> __wrap__Z34adaptive_banded_simple_event_alignR12SquiggleReadRK9PoreModelRKNSt7__cxx1112basic_stringIcSt11char_traitsIcESaIcEEE(
-    SquiggleRead& sr, const PoreModel& pm, const std::string& seq)
-{
-    if (g_capture) { g_read = &sr; return std::vector<AlignedPair>(); }
-    return __real__Z34adaptive_banded_simple_event_alignR12SquiggleReadRK9PoreModelRKNSt7__cxx1112basic_stringIcSt11char_traitsIcESaIcEEE(sr, pm, seq);
-}
+// ---- the wrapped constructor (oracle/phase.mk links with --wrap=<its mangled name>) ----
 extern "C" void __wrap__ZN12SquiggleReadC1ERKNSt7__cxx1112basic_stringIcSt11char_traitsIcESaIcEEERK6ReadDBj(SquiggleRead* self, const std::string&,
                                                                                                          const ReadDB&, uint32_t)
 {
     // what npref_read_create / npref_read_set_eventalign set, member by member (TransitionParameters owns raw buffers, so the
     // whole object is not assigned)
     SquiggleRead* sr = new (self) SquiggleRead();
-    const SquiggleRead& src = *g_read;
+    const SquiggleRead& src = *npref_read_of(g_read_h);
     sr->pore_type = src.pore_type; sr->read_type = src.read_type; sr->nucleotide_type = src.nucleotide_type;
     sr->read_name = src.read_name; sr->read_sequence = src.read_sequence;
     for (int s = 0; s < 2; ++s) {
@@ -94,9 +84,7 @@ long long npref_phase_read(int read_h, const char* read_name, const char* contig
                            const uint32_t* cigar, int n_cigar, int n_variants, const int32_t* var_pos, const char** var_ref, const char** var_alt,
                            double indel_bias, char* sam_out, size_t cap)
 {
-    g_capture = true;
-    npref_abea(read_h, 0, "", nullptr, 0);
-    g_capture = false;
+    g_read_h = read_h;
     NprefContig contig{contig_name, contig_seq};
     bam_hdr_t hdr;
     std::memset(&hdr, 0, sizeof(hdr));

@@ -43,6 +43,7 @@
 extern "C" {
 #include "event_detection.h"   // src/thirdparty/scrappie (C99)
 }
+#include "ref_harness.h"
 
 extern double hmm_indel_bias_factor;   // src/hmm/nanopolish_profile_hmm_r9.cpp:19
 
@@ -53,7 +54,6 @@ extern double hmm_indel_bias_factor;   // src/hmm/nanopolish_profile_hmm_r9.cpp:
 
 // htslib is not built here; eventalign needs two of its calls.  Test doubles: the "FASTA index" is a contig held
 // in memory, bam_endpos is pos + reference length of the CIGAR (what htslib computes for a mapped record).
-struct NprefContig { std::string name, seq; };
 extern "C" char* faidx_fetch_seq(const faidx_t* fai, const char* c_name, int p_beg_i, int p_end_i, int* len)
 {
     const NprefContig* c = reinterpret_cast<const NprefContig*>(fai);
@@ -119,6 +119,8 @@ std::vector<const PoreModel*> g_models;
 std::vector<std::unique_ptr<PoreModel>> g_owned_models;
 std::vector<std::unique_ptr<SquiggleRead>> g_reads;
 }
+
+SquiggleRead* npref_read_of(int h) { return g_reads[h].get(); }
 
 extern "C" {
 

@@ -4,42 +4,14 @@
 //
 // What model_score reaches outside its computation:
 //   the faidx handle     the in-memory contig of ref_harness.cpp's faidx_fetch_seq test double (an NprefContig)
-//   the SquiggleRead     a handle of ref_harness.cpp (npref_read_create), strand 0, taken through npref_abea, whose call of
-//                        adaptive_banded_simple_event_align is wrapped (-Wl,--wrap, oracle/scorereads.mk) as in hp_harness.cpp
+//   the SquiggleRead     a handle of ref_harness.cpp (npref_read_create, found by npref_read_of), strand 0
 //   stdout               its SEGMENT lines, written to a memory stream and dropped
 //   stderr               print()'s lines, written to a memory stream and returned
 // Nothing of the reference is copied.
 #include "nanopolish_scorereads.cpp"
+#include "ref_harness.h"
 
 #include <cstdio>
-
-extern "C" long long npref_abea(int read_h, int model_h, const char* seq, int32_t* pairs_out, size_t cap);   // ref_harness.cpp
-
-namespace {
-
-struct NprefContig { std::string name, seq; };      // the layout ref_harness.cpp's faidx_fetch_seq reads
-
-thread_local bool g_capture = false;
-thread_local SquiggleRead* g_read = nullptr;
-
-SquiggleRead* read_of(int h)
-{
-    g_capture = true;
-    npref_abea(h, 0, "", nullptr, 0);
-    g_capture = false;
-    return g_read;
-}
-
-} // namespace
-
-extern "C" std::vector<AlignedPair> __real__Z34adaptive_banded_simple_event_alignR12SquiggleReadRK9PoreModelRKNSt7__cxx1112basic_stringIcSt11char_traitsIcESaIcEEE(
-    SquiggleRead&, const PoreModel&, const std::string&);
-extern "C" std::vector<AlignedPair> __wrap__Z34adaptive_banded_simple_event_alignR12SquiggleReadRK9PoreModelRKNSt7__cxx1112basic_stringIcSt11char_traitsIcESaIcEEE(
-    SquiggleRead& sr, const PoreModel& pm, const std::string& seq)
-{
-    if (g_capture) { g_read = &sr; return std::vector<AlignedPair>(); }
-    return __real__Z34adaptive_banded_simple_event_alignR12SquiggleReadRK9PoreModelRKNSt7__cxx1112basic_stringIcSt11char_traitsIcESaIcEEE(sr, pm, seq);
-}
 
 extern "C" {
 
@@ -57,7 +29,7 @@ long long npref_model_score_train(int read_h, const char* contig, const char* co
                                   const int32_t* event_idx, int rc, int eps, int r9_prior, double* score_out, uint64_t* counts_out,
                                   double* probs_out, char* text_out, size_t cap)
 {
-    SquiggleRead* sr = read_of(read_h);
+    SquiggleRead* sr = npref_read_of(read_h);
     NprefContig fai{contig, contig_seq};
     std::vector<EventAlignment> ao(n_align);
     for (int i = 0; i < n_align; ++i) {

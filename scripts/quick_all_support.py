@@ -2,7 +2,7 @@
 draft region at depth 50, reads of 2 000 bases on both strands, a truth that differs from the draft by 400 homopolymer-length
 indels), min_flanking_sequence 30, HAF_ALLOW_PRE_CLIP | HAF_ALLOW_POST_CLIP, with the truth's seeded edits as the variants.
 Reports the variants, (variant, read) pairs, jobs and DP rows, the kernel time (nph_last_kernel_ms), the host's exp and fold time
-and the whole call, the card's name, power limit and SM clock read in the same run, and — where oracle/_ref/libnpref_support.so is
+and the whole call, the card's name, power limit and SM clock read in the same run, and — where oracle/_ref/libnpref_variants.so is
 built — the compiled reference's own annotate_variants_with_all_support on one CPU thread over a sub-region of the same pile-up, per
 (variant, read) pair.  Prints one JSON line.
 
@@ -15,13 +15,13 @@ import sys
 import time
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import ctypes as C  # noqa: E402
 
 import numpy as np  # noqa: E402
 
 from nanopolish_b200 import synth  # noqa: E402
 from nanopolish_b200.engine import Engine  # noqa: E402
 from tests import support_cases as sc  # noqa: E402
+from tests.ref_variants import RefVariants  # noqa: E402
 
 reps = int(sys.argv[1]) if len(sys.argv) > 1 else 5
 gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
@@ -55,9 +55,9 @@ row = dict(region_bases=len(c["draft"]), depth=50, reads=int(c["recs"].shape[0])
            kernel_ms_median=float(np.median(kern_ms)), host_ms_median=float(np.median(host_ms)),
            call_ms_median=float(np.median(call_ms)), call_ms_min=float(np.min(call_ms)), call_ms_max=float(np.max(call_ms)))
 row["pairs_per_s"] = row["pairs"] / (row["call_ms_median"] / 1e3)
-if sc.RefSupport.available():
-    ref = sc.RefSupport()
-    ref.lib.npref_set_globals(C.c_double(1.0), 1)                       # annotate_variants_with_all_support has no OpenMP; one thread all the same
+if RefVariants.available():
+    ref = RefVariants()
+    ref.set_globals(1.0, 1)                                             # annotate_variants_with_all_support has no OpenMP; one thread all the same
     sub = case(3_000, 24, seed=78)
     hs, _ = ref.register(sub)
     t0 = time.perf_counter()

@@ -3,7 +3,7 @@ whose truth differs from it by 400 substitutions.  The candidates are the truth'
 each (the pair forms one group) and 400 wrong substitutions on their own; min_flanking_sequence 30, min_distance_between_variants 10,
 max_haplotypes 1000, HAF_ALLOW_PRE_CLIP | HAF_ALLOW_POST_CLIP, ploidy 1 and 2.  Reports per ploidy the groups, haplotypes, jobs, DP rows,
 genotype sets and set x key terms, the forward-kernel, genotype-kernel and host times and the whole call, with the card's name, power
-limit and SM clock read in the same run.  Where oracle/_ref/libnpref_call.so is built (and no GPU is needed for it), --reference
+limit and SM clock read in the same run.  Where oracle/_ref/libnpref_variants.so is built (and no GPU is needed for it), --reference
 times the compiled reference's own call_haplotype_from_candidates on one CPU thread over the first 60 candidates instead.  Prints one
 JSON line.
 
@@ -21,6 +21,7 @@ import numpy as np  # noqa: E402
 
 from nanopolish_b200 import synth  # noqa: E402
 from tests import call_cases as cc  # noqa: E402
+from tests.ref_variants import RefVariants  # noqa: E402
 
 args = [a for a in sys.argv[1:] if not a.startswith("--")]
 reps = int(args[0]) if args else 5
@@ -42,7 +43,7 @@ c = dict(draft=draft, rs=rs, recs=recs, pairs=pairs, dur=dur, region_start=cc.RE
 row = dict(region_bases=len(draft), depth=50, reads=int(recs.shape[0]), candidates=len(cands))
 
 if "--reference" in sys.argv:
-    ref = cc.RefCall()
+    ref = RefVariants()
     sub = dict(c, candidates=cands[:60], ploidy=2)
     hs, _ = ref.register(sub)
     t0 = time.perf_counter()

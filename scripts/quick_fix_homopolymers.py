@@ -1,13 +1,12 @@
 """Timing of nph_homopolymer_likelihoods_batch on a `variants --fix-homopolymers` workload: a 50 kb draft region at depth 50 (reads
 of 2 000 bases on both strands) whose truth differs from the draft by 400 homopolymer-length indels, min_flanking_sequence 30.
 Reports the homopolymers, (homopolymer, read) pairs, jobs and DP rows, the kernel time (nph_last_kernel_ms), the host's log-gamma
-time and the whole call, the card's name, power limit and SM clock read in the same run, and — where oracle/_ref/libnpref_hp.so
+time and the whole call, the card's name, power limit and SM clock read in the same run, and — where oracle/_ref/libnpref_variants.so
 is built — the compiled reference's own fix_homopolymers on one CPU thread over a sub-region of the same pile-up, per
 (homopolymer, read) pair.  Prints one JSON line.
 
   python scripts/quick_fix_homopolymers.py [reps]
 """
-import ctypes as C
 import json
 import os
 import subprocess
@@ -21,6 +20,7 @@ from nanopolish_b200 import synth  # noqa: E402
 from nanopolish_b200.engine import Engine  # noqa: E402
 from tests import hp_cases as hc  # noqa: E402
 from tests import hp_restatement as hr  # noqa: E402
+from tests.ref_variants import RefVariants  # noqa: E402
 
 reps = int(sys.argv[1]) if len(sys.argv) > 1 else 5
 gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
@@ -53,9 +53,9 @@ row = dict(region_bases=len(c["draft"]), depth=50, reads=int(c["recs"].shape[0])
            kernel_ms_median=float(np.median(kern_ms)), host_lgamma_ms_median=float(np.median(host_ms)),
            call_ms_median=float(np.median(call_ms)), call_ms_min=float(np.min(call_ms)), call_ms_max=float(np.max(call_ms)))
 row["pairs_per_s"] = row["pairs"] / (row["call_ms_median"] / 1e3)
-if hc.RefHp.available():
-    ref = hc.RefHp()
-    ref.lib.npref_set_globals(C.c_double(1.0), 1)                       # fix_homopolymers has no OpenMP; one thread all the same
+if RefVariants.available():
+    ref = RefVariants()
+    ref.set_globals(1.0, 1)                                             # fix_homopolymers has no OpenMP; one thread all the same
     sub = case(3_000, 24, seed=78)
     hs, mh = ref.register(sub)
     t0 = time.perf_counter()

@@ -6,7 +6,7 @@ vcf_50k_p1).  Reports the device time of the candidate kernels and the whole dev
 share beyond the device call, the instances and distinct variants, and nph::call_variants_for_region + nph::write_variants_vcf at
 ploidy 1 (the VCF's bytes equal the compiled reference's, tests/test_gpu_region_candidates.py), with the card's name, power limit and
 SM clock read in the same run.  --reference times the compiled reference's own AlignmentDB::get_variants_in_region
-(oracle/_ref/libnpref_region.so) on one CPU thread instead.  Prints one JSON line.
+(oracle/_ref/libnpref_variants.so) on one CPU thread instead.  Prints one JSON line.
 
   python scripts/quick_region_candidates.py [reps] [--reference]
 """
@@ -23,6 +23,7 @@ import numpy as np  # noqa: E402
 
 from nanopolish_b200 import synth  # noqa: E402
 from tests import candidate_cases as cc  # noqa: E402
+from tests.ref_variants import RefVariants  # noqa: E402
 
 args = [a for a in sys.argv[1:] if not a.startswith("--")]
 reps = int(args[0]) if args else 5
@@ -32,11 +33,11 @@ cand = dict(c, start=c["region_start"] + buffer, stop=c["region_end"] - buffer) 
 row = dict(region_bases=len(c["region_ref"]), depth=50, records=len(c["bases"]), record_bases=int(sum(len(b) for b in c["bases"])))
 
 if "--reference" in sys.argv:
-    ref = cc.RefCand()
+    ref = RefVariants()
     t = []
     for _ in range(max(1, min(reps, 3))):
         t0 = time.perf_counter()
-        got = ref.variants(cand)
+        got = ref.variants_in_region(cand)
         t.append(time.perf_counter() - t0)
     row.update(ref_get_variants_in_region_s_1thread=float(np.median(t)), ref_kept=len(got),
                cpu=subprocess.run(["sh", "-c", "grep -m1 'model name' /proc/cpuinfo"], capture_output=True, text=True).stdout.strip())

@@ -5,7 +5,7 @@ quick_all_support.py (a 50 kb draft region at depth 50, reads of 2 000 bases on 
   round1  the truth expanded by expand_variants (min_flanking_sequence 30): each indel, its one-base-longer deletion, four insertions
 Reports per list the candidates, windows, rounds, jobs with and without the early exit, the reference's DP rows and their rate, the
 kernel time and the whole call, the card's name, power limit and SM clock read in the same run, and — where
-oracle/_ref/libnpref_screen.so is built — the compiled reference's own screen_variants_by_score on one CPU thread over the first
+oracle/_ref/libnpref_variants.so is built — the compiled reference's own screen_variants_by_score on one CPU thread over the first
 candidates of the round-1 list, per candidate.  Prints one JSON line.
 
   python scripts/quick_screen_variants.py [reps]
@@ -24,6 +24,7 @@ from nanopolish_b200 import synth  # noqa: E402
 from nanopolish_b200.engine import Engine  # noqa: E402
 from tests import screen_cases as sc  # noqa: E402
 from tests import screen_restatement as scr  # noqa: E402
+from tests.ref_variants import RefVariants  # noqa: E402
 
 reps = int(sys.argv[1]) if len(sys.argv) > 1 else 5
 gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
@@ -70,8 +71,8 @@ for name, cands in (("round0", round0), ("round1", round1)):
                      jobs_without_exit=int(cnt["n_jobs_without_exit"]), reference_rows=int(cnt["n_reference_rows"]),
                      kernel_ms_median=float(np.median(kern_ms)), call_ms_median=ms, call_ms_min=float(np.min(call_ms)),
                      call_ms_max=float(np.max(call_ms)), reference_rows_per_s=int(cnt["n_reference_rows"]) / (ms / 1e3))
-if sc.RefScreen.available():
-    refo = sc.RefScreen()
+if RefVariants.available():
+    refo = RefVariants()
     sub = dict(c, candidates=round1[:60])
     hs, _ = refo.register(sub)
     t0 = time.perf_counter()

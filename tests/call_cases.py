@@ -3,26 +3,23 @@
 A case is a seeded pile-up (tests/support_cases.py's substitution pile-ups, or tests/screen_cases.py's planted recognition sites),
 reads on both strands, a region over it, the read names, the options of the call (ploidy, genotype_only, max_haplotypes, -q types,
 calculate_all_support) and a candidate list.  Its answers come from
-  reference     the compiled reference's own call_haplotype_from_candidates (oracle/_ref/libnpref_call.so, oracle/call_harness.cpp)
+  reference     the compiled reference's own call_haplotype_from_candidates (tests/ref_variants.py: oracle/_ref/libnpref_variants.so)
   restated      tests/call_restatement.py over the compiled reference's profile_hmm_score (the same library), or over
                 nph_hmm_score_batch
   mirror        nph::call_haplotype_from_candidates through the nphh_call_haplotype shim (nph_call_variant_groups_batch).
 Every answer is the derived sequence, then per variant of the derived haplotype "position, alleles, quality bits, INFO, genotype"."""
 import ctypes as C
 import hashlib
-import os
 
 import numpy as np
 
 from nanopolish_b200 import synth
-from oracle.oracle_py import RefOracle
 from tests import call_restatement as cr
 from tests import hp_cases as hc
 from tests import screen_cases as sc
 from tests import support_cases as suc
 from tests import var_meth_restatement as vmr
 
-REF_CALL = os.path.join(hc.ROOT, "oracle", "_ref", "libnpref_call.so")
 REGION_START = hc.REGION_START
 CONTIG = hc.CONTIG
 FLAGS = 3                               # HAF_ALLOW_PRE_CLIP | HAF_ALLOW_POST_CLIP, what `variants` passes
@@ -150,66 +147,17 @@ def strip_all_support(lines):
     return out
 
 
-class RefCall(RefOracle):
-    """RefOracle over oracle/_ref/libnpref_call.so: its own reads, profile_hmm_score, call_haplotype_from_candidates, kt_fisher_exact
-    and Combinations"""
+def ref_restated(ref, c, hs, mh):
+    """restated over the profile_hmm_score of `ref` (a tests/ref_variants.py RefVariants holding the case's reads as registered: hs,
+    mh), the type models being its built-in ones"""
+    models = [mh] + [ref.builtin_model(alphabet=t) for t in c["types"]]
+    recs = c["recs"]
 
-    def __init__(self):
-        super().__init__()
-        L = self.lib = C.CDLL(REF_CALL)
-        L.npref_score_batch.restype = C.c_double
-        L.npref_call_haplotype.restype = C.c_longlong
-        L.npref_fisher_exact.restype = C.c_double
-        L.npref_fisher_exact.argtypes = [C.c_int] * 4
-        L.npref_combinations.restype = C.c_longlong
-
-    @staticmethod
-    def available() -> bool:
-        return os.path.exists(REF_CALL) and RefOracle.available()
-
-    register = hc.RefHp.register
-
-    def called(self, c, hs):
-        recs, pairs = c["recs"], c["pairs"]
-        p = lambda a: a.ctypes.data_as(C.c_void_p)
-        rh = np.ascontiguousarray(hs[recs["read"]], np.int32)
-        rc = np.ascontiguousarray(recs["rc"], np.uint8)
-        stride = np.where(rc == 1, -1, 1).astype(np.int8)
-        po = np.ascontiguousarray(recs["pair_off"], np.uint64)
-        npair = np.ascontiguousarray(recs["n_pairs"], np.uint32)
-        pp = np.ascontiguousarray(np.stack([pairs["ref_pos"], pairs["read_pos"]], 1).astype(np.int32))
-        vs = c["candidates"]
-        vp = np.array([x[0] for x in vs] or [0], np.int32)
-        cap = 1 << 22
-        out = C.create_string_buffer(cap)
-        n = self.lib.npref_call_haplotype(CONTIG.encode(), c["region_start"], c["region_end"], c["region_ref"].encode(), int(recs.shape[0]), p(rh),
-                                          _cstrs(record_names(c)), p(rc), p(stride), p(po), p(npair), p(pp), len(vs), p(vp),
-                                          _cstrs([x[1] for x in vs]), _cstrs([x[2] for x in vs]), FLANK, MIN_DISTANCE, c["max_haplotypes"],
-                                          c["ploidy"], c["genotype_only"], ",".join(c["types"]).encode(), c["all_support"], C.c_uint32(FLAGS),
-                                          out, C.c_size_t(cap))
-        assert n >= 0, n
-        return _lines(out.raw[:n])
-
-    def restated(self, c, hs, mh):
-        """cr.restated over this library's profile_hmm_score, the type models being its built-in ones"""
-        models = [mh] + [self.builtin_model(alphabet=t) for t in c["types"]]
-        recs = c["recs"]
-
-        def score(reqs):
-            jobs = [(0, int(recs[r]["read"]), 1 + t, e1, e2, len(s) - 5, -1 if recs[r]["rc"] else 1, int(recs[r]["rc"]), FLAGS, 0)
-                    for r, e1, e2, t, s in reqs]
-            return self.score_batch(hs, np.array(jobs, synth.HMM_JOB_DT), [s.encode() for *_, s in reqs], models)[0]
-        return restated(c, score)
-
-    def fisher(self, n11, n12, n21, n22):
-        return self.lib.npref_fisher_exact(n11, n12, n21, n22)
-
-    def combinations(self, n, k, with_replacement):
-        cap = 1 << 20
-        out = np.zeros(cap, np.uint32)
-        m = self.lib.npref_combinations(n, k, int(with_replacement), out.ctypes.data_as(C.c_void_p), C.c_size_t(cap))
-        assert m >= 0
-        return out[:m * k].reshape(m, k).tolist() if k else [[]] * m
+    def score(reqs):
+        jobs = [(0, int(recs[r]["read"]), 1 + t, e1, e2, len(s) - 5, -1 if recs[r]["rc"] else 1, int(recs[r]["rc"]), FLAGS, 0)
+                for r, e1, e2, t, s in reqs]
+        return ref.score_batch(hs, np.array(jobs, synth.HMM_JOB_DT), [s.encode() for *_, s in reqs], models)[0]
+    return restated(c, score)
 
 
 def restated(c, score):

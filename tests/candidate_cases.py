@@ -6,7 +6,6 @@ bounds [start, stop] and the filter (min_frequency, min_depth).  Records are wri
 and `claims(case, distinct)` checks it on the restatement's answer.  Cases with `before_start` records (aligned entirely before
 start, where the reference dereferences end()) are never sent to the compiled reference."""
 import hashlib
-import os
 
 import numpy as np
 
@@ -213,66 +212,6 @@ def claims(c, dist):
     assert c["claim"] is None or c["claim"](dist), f"{c['name']}: the case does not reach the edge it was built for"
 
 
-REF_REGION = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref", "libnpref_region.so")
-
-
-class RefCand:
-    """oracle/_ref/libnpref_region.so (oracle/region.mk): npref_variants_in_region, the reference's own
-    AlignmentDB::get_variants_in_region, and npref_call_region, its default-mode region call and VCF"""
-
-    def __init__(self):
-        import ctypes as C
-        self.C = C
-        self.lib = C.CDLL(REF_REGION)
-        self.lib.npref_variants_in_region.restype = C.c_longlong
-        self._call = None
-
-    @property
-    def call(self):
-        """tests/call_cases.py's RefCall with this library in place of libnpref_call.so (its reads, registered in this library, are the
-        ones npref_call_region's call_haplotype_from_candidates sees)"""
-        if self._call is None:
-            from tests.call_cases import RefCall
-            from oracle.oracle_py import RefOracle
-
-            C = self.C
-
-            class RefRegionCall(RefCall):
-                def __init__(inner):
-                    RefOracle.__init__(inner)
-                    # the entry points RefOracle typed on libnpref.so, typed alike on this library
-                    for name, f in list(vars(inner.lib).items()):
-                        if isinstance(f, C._CFuncPtr):
-                            g = getattr(self.lib, name)
-                            g.restype, g.argtypes = f.restype, f.argtypes
-                    inner.lib = self.lib
-                    inner.lib.npref_call_haplotype.restype = C.c_longlong
-            self._call = RefRegionCall()
-        return self._call
-
-    @staticmethod
-    def available() -> bool:
-        if not os.path.exists(REF_REGION):
-            return False
-        from oracle.oracle_py import RefOracle
-        return RefOracle.available()
-
-    def variants(self, c):
-        """the reference's ordered list: one (ref_position, ref_seq, alt_seq, info) per variant"""
-        C = self.C
-        pp, off = flat_pairs(c)
-        bases = (C.c_char_p * max(len(c["bases"]), 1))(*c["bases"])
-        rc = np.array(c["rc"] or [0], np.uint8)
-        cap = 1 << 26
-        out = C.create_string_buffer(cap)
-        region_end = c["region_start"] + len(c["region_ref"]) - 1
-        n = self.lib.npref_variants_in_region(CONTIG.encode(), c["region_start"], region_end, c["region_ref"].encode(), len(c["bases"]), bases,
-                                              rc.ctypes.data_as(C.c_void_p), pp.ctypes.data_as(C.c_void_p), off.ctypes.data_as(C.c_void_p),
-                                              c["start"], c["stop"], C.c_double(c["min_frequency"]), c["min_depth"], out, C.c_size_t(cap))
-        assert n >= 0, n
-        return parse(out.raw[:n])
-
-
 def parse(raw: bytes):
     return [tuple(int(f) if i == 0 else f for i, f in enumerate(l.split("\t"))) for l in raw.decode("latin-1").splitlines()]
 
@@ -327,10 +266,11 @@ def call_fingerprint(c) -> str:
 
 
 def call_args(c):
-    """the arrays both region calls take: event records (read index per record, rc, flat pairs, offsets) and base-space records"""
+    """the arrays the host mirror's region call takes: event records (read index per record, rc, flat pairs, offsets) and base-space
+    records"""
     recs, pairs = c["recs"], c["pairs"]
     pp, off = flat_pairs(c)
-    return dict(rc=np.ascontiguousarray(recs["rc"], np.uint8), stride=np.where(recs["rc"] == 1, -1, 1).astype(np.int8),
+    return dict(rc=np.ascontiguousarray(recs["rc"], np.uint8),
                 po=np.ascontiguousarray(recs["pair_off"], np.uint64), npair=np.ascontiguousarray(recs["n_pairs"], np.uint32),
                 ep=np.ascontiguousarray(np.stack([pairs["ref_pos"], pairs["read_pos"]], 1).astype(np.int32)),
                 seq_bases=c["bases"], seq_rc=np.array(c["rc"] or [0], np.uint8), sp=pp, soff=off,
@@ -341,22 +281,3 @@ def _cstrs(xs):
     import ctypes as C
     return (C.c_char_p * max(len(xs), 1))(*[x if isinstance(x, bytes) else x.encode() for x in xs])
 
-
-def ref_call_region(live, c):
-    """npref_call_region of oracle/_ref/libnpref_call.so: the VCF bytes"""
-    import ctypes as C
-    hs, _ = live.register(c)
-    a = call_args(c)
-    p = lambda x: x.ctypes.data_as(C.c_void_p)
-    rh = np.ascontiguousarray(hs[c["recs"]["read"]], np.int32)
-    cap = 1 << 24
-    out = C.create_string_buffer(cap)
-    live.lib.npref_call_region.restype = C.c_longlong
-    n = live.lib.npref_call_region("ctg".encode(), c["contig_length"], c["start_base"], c["end_base"], c["region_start"], c["region_end"],
-                                   c["region_ref"].encode(), int(c["recs"].shape[0]), p(rh), _cstrs(a["names"]), p(a["rc"]), p(a["stride"]),
-                                   p(a["po"]), p(a["npair"]), p(a["ep"]), len(c["bases"]), _cstrs(a["seq_bases"]), p(a["seq_rc"]), p(a["sp"]),
-                                   p(a["soff"]), CALL_FLANK, CALL_MIN_DISTANCE, CALL_MAX_HAPLOTYPES, c["ploidy"], 0, b"", c["all_support"],
-                                   c["snps_only"], C.c_double(c["min_frequency"]), c["min_depth"],
-                                   None if c["candidates"] is None else c["candidates"].encode(), out, C.c_size_t(cap))
-    assert n >= 0, n
-    return out.raw[:n]

@@ -3,7 +3,7 @@
 A case is a seeded pile-up of synth.gen_hp_pileup (reads from a truth that differs from the draft by homopolymer-length indels,
 event durations from the reference's gamma model) plus a haplotype over the draft (the draft with some variants applied) and
 min_flanking_sequence.  Its answers come from
-  ref_fixed     the compiled reference's own fix_homopolymers (oracle/_ref/libnpref_hp.so, oracle/hp_harness.cpp)
+  ref_fixed     the compiled reference's own fix_homopolymers (tests/ref_variants.py: oracle/_ref/libnpref_variants.so)
   restated      tests/hp_restatement.py over the compiled reference's profile_hmm_score / profile_hmm_align (the same library)
   device        nph_homopolymer_likelihoods_batch for the restatement's windows."""
 import ctypes as C
@@ -13,11 +13,9 @@ import os
 import numpy as np
 
 from nanopolish_b200 import synth
-from oracle.oracle_py import RefOracle
 from tests import hp_restatement as hr
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_HP = os.path.join(ROOT, "oracle", "_ref", "libnpref_hp.so")
 CONTIG = "ctg"
 REGION_START = 5000
 
@@ -147,74 +145,30 @@ def fingerprint(c) -> str:
     return h.hexdigest()
 
 
-class RefHp(RefOracle):
-    """RefOracle over oracle/_ref/libnpref_hp.so: its own reads, profile_hmm_score / _align, and fix_homopolymers"""
+def ref_restated(ref, c, hs, mh):
+    """per window (total_reads, e_lik, d_lik) over the HMMs of `ref` (a tests/ref_variants.py RefVariants holding the case's reads
+    as registered: hs, mh), and the fixed text"""
+    recs, rs = c["recs"], c["rs"]
+    rec_reads = rs.reads[recs["read"]]
 
-    def __init__(self):
-        super().__init__()
-        L = self.lib = C.CDLL(REF_HP)
-        L.npref_score_batch.restype = C.c_double
-        L.npref_fix_homopolymers.restype = C.c_longlong
+    def job(seq, r, e1, e2):
+        jb = np.zeros(1, synth.HMM_JOB_DT)
+        jb[0]["read"], jb[0]["event_start"], jb[0]["event_stop"], jb[0]["rc"] = int(recs[r]["read"]), e1, e2, int(recs[r]["rc"])
+        return jb
 
-    @staticmethod
-    def available() -> bool:
-        return os.path.exists(REF_HP) and RefOracle.available()
+    score = lambda seq, r, e1, e2: ref.score_batch(hs, job(seq, r, e1, e2), [seq.encode()], [mh])[0][0]
 
-    def register(self, c):
-        self.clear_reads()
-        rs = c["rs"]
-        mh = self.builtin_model()
-        hs = self.register_reads(rs.reads, rs.ev_mean, rs.ev_start_time, mh)
-        for i, r in enumerate(rs.reads):
-            o, n = int(r["event_off"]), int(r["n_events"])
-            self.read_set_eventalign(hs[i], f"r{i}", "", np.zeros(0, np.int32), np.zeros(0, np.int32), np.ones(n, np.float32), c["dur"][o:o + n])
-        return hs, mh
+    def align(seq, r, e1, e2):
+        ek, _, st = ref.align(hs[int(recs[r]["read"])], mh, seq.encode(), e1, e2, int(recs[r]["rc"]), 0)
+        return [(int(e), int(k), chr(s)) for (e, k), s in zip(ek, st)]
 
-    def fixed(self, c, hs) -> str:
-        recs, pairs = c["recs"], c["pairs"]
-        rh = np.ascontiguousarray(hs[recs["read"]], np.int32)
-        rc = np.ascontiguousarray(recs["rc"], np.uint8)
-        stride = np.where(rc == 1, -1, 1).astype(np.int8)
-        po = np.ascontiguousarray(recs["pair_off"], np.uint64)
-        npair = np.ascontiguousarray(recs["n_pairs"], np.uint32)
-        pp = np.ascontiguousarray(np.stack([pairs["ref_pos"], pairs["read_pos"]], 1).astype(np.int32))
-        vp = np.array([REGION_START + o for o, _, _ in c["variants"]] or [0], np.int32)
-        vr = (C.c_char_p * max(1, len(c["variants"])))(*[r.encode() for _, r, _ in c["variants"]])
-        va = (C.c_char_p * max(1, len(c["variants"])))(*[a.encode() for _, _, a in c["variants"]])
-        cap = 1 << 20
-        out = C.create_string_buffer(cap)
-        p = lambda a: a.ctypes.data_as(C.c_void_p)
-        n = self.lib.npref_fix_homopolymers(CONTIG.encode(), c["region_start"], c["region_end"], c["region_ref"].encode(), int(recs.shape[0]), p(rh), p(rc),
-                                            p(stride), p(po), p(npair), p(pp), REGION_START, c["draft"].encode(), len(c["variants"]), p(vp), vr, va,
-                                            c["min_flank"], out, C.c_size_t(cap))
-        assert n >= 0, n
-        text = out.raw[:n].decode()
-        seq, *lines = text.split("\n")
-        return seq + "\n" + "".join(l + "\n" for l in lines[len(c["variants"]):] if l)
-
-    def restated(self, c, hs, mh):
-        """per window (total_reads, e_lik, d_lik) over the reference's HMMs, and the fixed text"""
-        recs, rs = c["recs"], c["rs"]
-        rec_reads = rs.reads[recs["read"]]
-
-        def job(seq, r, e1, e2):
-            jb = np.zeros(1, synth.HMM_JOB_DT)
-            jb[0]["read"], jb[0]["event_start"], jb[0]["event_stop"], jb[0]["rc"] = int(recs[r]["read"]), e1, e2, int(recs[r]["rc"])
-            return jb
-
-        score = lambda seq, r, e1, e2: self.score_batch(hs, job(seq, r, e1, e2), [seq.encode()], [mh])[0][0]
-
-        def align(seq, r, e1, e2):
-            ek, _, st = self.align(hs[int(recs[r]["read"])], mh, seq.encode(), e1, e2, int(recs[r]["rc"]), 0)
-            return [(int(e), int(k), chr(s)) for (e, k), s in zip(ek, st)]
-
-        vectors = []
-        for w in c["wins"]:
-            seqs = hr.event_sequences(recs, c["pairs"], w["rcs"], w["rce"])
-            e, d = hr.likelihoods(w, seqs, rec_reads, rs.ev_start_time, c["dur"], score, align)
-            vectors.append((len(seqs), e, d))
-        fixed = hr.fix_homopolymers(c["hap"], c["wins"], vectors)
-        return vectors, hr.fixed_text(fixed, len(c["variants"]))
+    vectors = []
+    for w in c["wins"]:
+        seqs = hr.event_sequences(recs, c["pairs"], w["rcs"], w["rce"])
+        e, d = hr.likelihoods(w, seqs, rec_reads, rs.ev_start_time, c["dur"], score, align)
+        vectors.append((len(seqs), e, d))
+    fixed = hr.fix_homopolymers(c["hap"], c["wins"], vectors)
+    return vectors, hr.fixed_text(fixed, len(c["variants"]))
 
 
 def event_edges(c):

@@ -4,24 +4,21 @@ A case is a seeded pile-up — synth.gen_pileup (a truth with substitutions), sy
 with homopolymer-length indels) or synth.gen_pileup_methylated (planted recognition sites), reads on both strands — plus a region
 over it, opt::screen_flanking_sequence, alignment_flags, opt::screen_score_threshold, opt::methylation_types and a candidate list.
 Its answers come from
-  reference     the compiled reference's own screen_variants_by_score (oracle/_ref/libnpref_screen.so, oracle/screen_harness.cpp)
+  reference     the compiled reference's own screen_variants_by_score (tests/ref_variants.py: oracle/_ref/libnpref_variants.so)
   restated      tests/screen_restatement.py over the compiled reference's profile_hmm_score (the same library)
   device        nph_screen_variants_batch
   mirror        nph::screen_variants_by_score through the nphh_screen_variants shim (the device call)."""
 import ctypes as C
 import hashlib
-import os
 
 import numpy as np
 
 from nanopolish_b200 import synth
-from oracle.oracle_py import RefOracle
 from tests import hp_cases as hc
 from tests import screen_restatement as scr
 from tests import support_cases as suc
 from tests import var_meth_restatement as vmr
 
-REF_SCREEN = os.path.join(hc.ROOT, "oracle", "_ref", "libnpref_screen.so")
 REGION_START = hc.REGION_START
 CONTIG = hc.CONTIG
 FLAGS = 3                               # HAF_ALLOW_PRE_CLIP | HAF_ALLOW_POST_CLIP, what `variants` passes
@@ -173,63 +170,17 @@ def plan(c, candidates=None):
                     c["flank"], c["types"])
 
 
-class RefScreen(RefOracle):
-    """RefOracle over oracle/_ref/libnpref_screen.so: its own reads, profile_hmm_score, screen_variants_by_score and expand_variants"""
+def ref_restated(ref, c, hs, mh):
+    """scr.screened over the profile_hmm_score of `ref` (a tests/ref_variants.py RefVariants holding the case's reads as registered:
+    hs, mh), the type models being its built-in ones"""
+    models = [mh] + [ref.builtin_model(alphabet=t) for t in c["types"]]
+    recs = c["recs"]
 
-    def __init__(self):
-        super().__init__()
-        L = self.lib = C.CDLL(REF_SCREEN)
-        L.npref_score_batch.restype = C.c_double
-        L.npref_screen_variants.restype = C.c_longlong
-        L.npref_expand_variants.restype = C.c_longlong
-
-    @staticmethod
-    def available() -> bool:
-        return os.path.exists(REF_SCREEN) and RefOracle.available()
-
-    register = hc.RefHp.register
-
-    def screened(self, c, hs):
-        """the reference's output list, one line per kept variant"""
-        recs, pairs = c["recs"], c["pairs"]
-        p = lambda a: a.ctypes.data_as(C.c_void_p)
-        rh = np.ascontiguousarray(hs[recs["read"]], np.int32)
-        rc = np.ascontiguousarray(recs["rc"], np.uint8)
-        stride = np.where(rc == 1, -1, 1).astype(np.int8)
-        po = np.ascontiguousarray(recs["pair_off"], np.uint64)
-        npair = np.ascontiguousarray(recs["n_pairs"], np.uint32)
-        pp = np.ascontiguousarray(np.stack([pairs["ref_pos"], pairs["read_pos"]], 1).astype(np.int32))
-        vs = c["candidates"]
-        vp = np.array([x[0] for x in vs] or [0], np.int32)
-        cap = 1 << 22
-        out = C.create_string_buffer(cap)
-        n = self.lib.npref_screen_variants(CONTIG.encode(), c["region_start"], c["region_end"], c["region_ref"].encode(), int(recs.shape[0]),
-                                           p(rh), p(rc), p(stride), p(po), p(npair), p(pp), len(vs), p(vp), _cstrs([x[1] for x in vs]),
-                                           _cstrs([x[2] for x in vs]), c["flank"], int(c["threshold"]), ",".join(c["types"]).encode(),
-                                           C.c_uint32(c["flags"]), out, C.c_size_t(cap))
-        assert n >= 0, n
-        return out.raw[:n].decode().split("\n")[:-1]
-
-    def expanded(self, region_start, region_ref, cands, min_flank):
-        p = lambda a: a.ctypes.data_as(C.c_void_p)
-        vp = np.array([x[0] for x in cands] or [0], np.int32)
-        cap = 1 << 22
-        out = C.create_string_buffer(cap)
-        n = self.lib.npref_expand_variants(CONTIG.encode(), region_start, region_start + len(region_ref) - 1, region_ref.encode(), len(cands),
-                                           p(vp), _cstrs([x[1] for x in cands]), _cstrs([x[2] for x in cands]), min_flank, out, C.c_size_t(cap))
-        assert n >= 0, n
-        return out.raw[:n].decode().split("\n")[:-1]
-
-    def restated(self, c, hs, mh):
-        """scr.screened over this library's profile_hmm_score, the type models being its built-in ones"""
-        models = [mh] + [self.builtin_model(alphabet=t) for t in c["types"]]
-        recs = c["recs"]
-
-        def score(reqs):
-            jobs = [(0, int(recs[r]["read"]), 1 + t, e1, e2, len(s) - 5, -1 if recs[r]["rc"] else 1, int(recs[r]["rc"]), c["flags"], 0)
-                    for r, e1, e2, t, s in reqs]
-            return self.score_batch(hs, np.array(jobs, synth.HMM_JOB_DT), [s.encode() for *_, s in reqs], models)[0]
-        return scr.screened(plan(c), score, c["threshold"])
+    def score(reqs):
+        jobs = [(0, int(recs[r]["read"]), 1 + t, e1, e2, len(s) - 5, -1 if recs[r]["rc"] else 1, int(recs[r]["rc"]), c["flags"], 0)
+                for r, e1, e2, t, s in reqs]
+        return ref.score_batch(hs, np.array(jobs, synth.HMM_JOB_DT), [s.encode() for *_, s in reqs], models)[0]
+    return scr.screened(plan(c), score, c["threshold"])
 
 
 def meth_arg(c):

@@ -3,24 +3,21 @@
 A case is a seeded pile-up — synth.gen_hp_pileup through tests/hp_cases.py (a truth with homopolymer-length indels) or
 synth.gen_pileup (a truth with substitutions), reads on both strands — plus a region over it, min_flanking_sequence, alignment_flags
 and a variant list.  Its answers come from
-  reference     the compiled reference's own annotate_variants_with_all_support (oracle/_ref/libnpref_support.so,
-                oracle/support_harness.cpp)
+  reference     the compiled reference's own annotate_variants_with_all_support (tests/ref_variants.py:
+                oracle/_ref/libnpref_variants.so)
   restated      tests/support_restatement.py over the compiled reference's profile_hmm_score and add_logs (the same library)
   device        nph_all_support_batch
   mirror        nph::annotate_variants_with_all_support through the nphh_all_support shim (the device call)."""
 import ctypes as C
 import hashlib
-import os
 
 import numpy as np
 
 from nanopolish_b200 import synth
-from oracle.oracle_py import RefOracle
 from tests import hp_cases as hc
 from tests import hp_restatement as hr
 from tests import support_restatement as sr
 
-REF_SUPPORT = os.path.join(hc.ROOT, "oracle", "_ref", "libnpref_support.so")
 REGION_START = hc.REGION_START
 CONTIG = hc.CONTIG
 FLAGS = 3                               # HAF_ALLOW_PRE_CLIP | HAF_ALLOW_POST_CLIP, what `variants` passes
@@ -193,46 +190,10 @@ def restated(c, score_jobs, add_logs):
     return out
 
 
-class RefSupport(RefOracle):
-    """RefOracle over oracle/_ref/libnpref_support.so: its own reads, profile_hmm_score, add_logs and
-    annotate_variants_with_all_support"""
-
-    def __init__(self):
-        super().__init__()
-        L = self.lib = C.CDLL(REF_SUPPORT)
-        L.npref_score_batch.restype = C.c_double
-        self.lib.npref_all_support.restype = C.c_longlong
-        self.lib.npref_add_logs.restype = C.c_float
-        self.lib.npref_add_logs.argtypes = [C.c_float, C.c_float]
-
-    @staticmethod
-    def available() -> bool:
-        return os.path.exists(REF_SUPPORT) and RefOracle.available()
-
-    register = hc.RefHp.register
-
-    def infos(self, c, hs):
-        """the INFO of every variant after the reference's call"""
-        recs, pairs = c["recs"], c["pairs"]
-        p = lambda a: a.ctypes.data_as(C.c_void_p)
-        rh = np.ascontiguousarray(hs[recs["read"]], np.int32)
-        rc = np.ascontiguousarray(recs["rc"], np.uint8)
-        stride = np.where(rc == 1, -1, 1).astype(np.int8)
-        po = np.ascontiguousarray(recs["pair_off"], np.uint64)
-        npair = np.ascontiguousarray(recs["n_pairs"], np.uint32)
-        pp = np.ascontiguousarray(np.stack([pairs["ref_pos"], pairs["read_pos"]], 1).astype(np.int32))
-        vs = c["variants"]
-        vp = np.array([x[0] for x in vs] or [0], np.int32)
-        cap = 1 << 20
-        out = C.create_string_buffer(cap)
-        n = self.lib.npref_all_support(CONTIG.encode(), c["region_start"], c["region_end"], c["region_ref"].encode(), int(recs.shape[0]), p(rh),
-                                       p(rc), p(stride), p(po), p(npair), p(pp), len(vs), p(vp), _cstrs([x[1] for x in vs]),
-                                       _cstrs([x[2] for x in vs]), c["flank"], C.c_uint32(c["flags"]), out, C.c_size_t(cap))
-        assert n >= 0, n
-        return out.raw[:n].decode().split("\n")[:-1]
-
-    def restated(self, c, hs, mh):
-        return restated(c, lambda jobs, seqs: self.score_batch(hs, jobs, seqs, [mh])[0], self.lib.npref_add_logs)
+def ref_restated(ref, c, hs, mh):
+    """restated over the profile_hmm_score and add_logs of `ref` (a tests/ref_variants.py RefVariants holding the case's reads as
+    registered: hs, mh)"""
+    return restated(c, lambda jobs, seqs: ref.score_batch(hs, jobs, seqs, [mh])[0], ref.lib.npref_add_logs)
 
 
 def device(eng, c, variants=None, params=None):

@@ -1,5 +1,5 @@
 """The compiled reference's own annotate_variants_with_all_support (src/common/nanopolish_variant.cpp:801-859, run unmodified by
-oracle/support_harness.cpp) against the restatement in tests/support_restatement.py over the reference's profile_hmm_score and add_logs:
+oracle/variants_harness.cpp) against the restatement in tests/support_restatement.py over the reference's profile_hmm_score and add_logs:
 the SupportFractionByBase INFO of every variant, byte for byte, on the cases of tests/support_cases.py.  Each case asserts the
 edges it was built to reach.  The reference's INFO and the restated support fractions, read counts and apply_variant outcomes are
 kept in tests/golden/ref_all_support.pkl.xz for the device suite (tests/test_gpu_all_support.py).  Also: the restatement refuses a
@@ -11,8 +11,9 @@ from tests import forward_cases as fc
 from tests import hp_restatement as hr
 from tests import support_cases as sc
 from tests.ref_calls import case_fixture
+from tests.ref_variants import RefVariants
 
-ref_sup = case_fixture("ref_all_support.pkl.xz", ref=lambda: sc.RefSupport() if sc.RefSupport.available() else None)
+ref_sup = case_fixture("ref_all_support.pkl.xz", ref=lambda: RefVariants() if RefVariants.available() else None)
 
 
 @pytest.mark.parametrize("spec", sc.CASES, ids=[s[0] for s in sc.CASES])
@@ -23,7 +24,7 @@ def test_restatement_equals_reference(ref_sup, spec):
     def ask(_):
         hs, mh = live.register(c)
         want = live.infos(c, hs)
-        got = live.restated(c, hs, mh)
+        got = sc.ref_restated(live, c, hs, mh)
         assert [g[3] for g in got] == want, f"{spec[0]}: the restated INFO differs from the reference's"
         return [(w, np.asarray(g[0], np.float64), g[1], g[2]) for w, g in zip(want, got)]
 

@@ -1,5 +1,5 @@
 """The compiled reference's own call_haplotype_from_candidates (src/nanopolish_call_variants.cpp:782-880, run unmodified by
-oracle/call_harness.cpp) against the restatement in tests/call_restatement.py over the reference's profile_hmm_score: the derived
+oracle/variants_harness.cpp) against the restatement in tests/call_restatement.py over the reference's profile_hmm_score: the derived
 sequence and, per variant, position, alleles, quality bits, INFO and genotype on every case of tests/call_cases.py (INFO without
 SupportFractionByBase, which is not restated).  Each case asserts the edges it was built to reach.  Also: the host mirror's Fisher test
 against the reference's kt_fisher_exact on every table of at most 60 reads and on large and underflowing tables, and the visit orders of
@@ -15,9 +15,10 @@ import pytest
 from tests import call_cases as cc
 from tests import call_restatement as cr
 from tests.ref_calls import case_fixture
+from tests.ref_variants import RefVariants
 from tests.test_host_mirror import HOST_SO
 
-ref_call = case_fixture("ref_call_haplotype.pkl.xz", ref=lambda: cc.RefCall() if cc.RefCall.available() else None)
+ref_call = case_fixture("ref_call_haplotype.pkl.xz", ref=lambda: RefVariants() if RefVariants.available() else None)
 
 # large tables, and tables whose probabilities underflow (StrandFisherTest clamps those to 1000)
 BIG_TABLES = [(500, 3, 7, 900), (2000, 1, 1, 2000), (0, 1000, 1000, 0), (1000, 0, 0, 1000), (33, 77, 121, 11), (250, 250, 250, 250),
@@ -32,7 +33,7 @@ def test_restatement_equals_reference(ref_call, spec):
     def ask(_):
         hs, mh = live.register(c)
         want = live.called(c, hs)
-        got = live.restated(c, hs, mh)
+        got = cc.ref_restated(live, c, hs, mh)
         assert got == (cc.strip_all_support(want) if c["all_support"] else want), f"{spec[0]}: the restated call differs from the reference's"
         return want
 

@@ -1,4 +1,4 @@
-"""The compiled reference's own fix_homopolymers (src/nanopolish_call_variants.cpp:541-780, run unmodified by oracle/hp_harness.cpp)
+"""The compiled reference's own fix_homopolymers (src/nanopolish_call_variants.cpp:541-780, run unmodified by oracle/variants_harness.cpp)
 against the restatement in tests/hp_restatement.py over the reference's profile_hmm_score / profile_hmm_align: the fixed sequence
 and every variant it adds (position, REF / ALT, the bits of its quality, INFO), on pile-ups whose truth differs from the draft by
 homopolymer insertions and deletions, reads of both strands, a haplotype with inserted and substituted bases in the calling
@@ -16,9 +16,10 @@ import pytest
 from tests import hp_cases as hc
 from tests import hp_restatement as hr
 from tests.ref_calls import case_fixture
+from tests.ref_variants import RefVariants
 from tests.test_host_mirror import HOST_SO
 
-ref_hp = case_fixture("ref_fix_homopolymers.pkl.xz", ref=lambda: hc.RefHp() if hc.RefHp.available() else None)
+ref_hp = case_fixture("ref_fix_homopolymers.pkl.xz", ref=lambda: RefVariants() if RefVariants.available() else None)
 
 
 @pytest.mark.parametrize("spec", hc.CASES, ids=[s[0] for s in hc.CASES])
@@ -29,7 +30,7 @@ def test_restatement_equals_reference(ref_hp, spec):
     def ask(_):
         hs, mh = live.register(c)
         want = live.fixed(c, hs)
-        vectors, got = live.restated(c, hs, mh)
+        vectors, got = hc.ref_restated(live, c, hs, mh)
         assert got == want, f"{spec[0]}: the restatement's fixed haplotype differs from the reference's"
         # the vectors as float64 arrays: recorded and compared by their bits (NaN included)
         return want, [(n, np.array(e, np.float64), np.array(d, np.float64)) for n, e, d in vectors]

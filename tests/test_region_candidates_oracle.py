@@ -1,5 +1,5 @@
 """The compiled reference's own AlignmentDB::get_variants_in_region (src/alignment/nanopolish_alignment_db.cpp:259-368, run
-unmodified by oracle/call_harness.cpp) against the plain-Python walk of tests/candidate_restatement.py on every case of
+unmodified by oracle/variants_harness.cpp) against the plain-Python walk of tests/candidate_restatement.py on every case of
 tests/candidate_cases.py that the reference is defined on: the kept variants' positions and, per position, the multiset of
 (ref_seq, alt_seq, INFO), and the full order wherever no position repeats.  Each case asserts the edge it was built to reach; the
 sort_ties case shows that the reference's order among variants at one position is not key order (std::sort's ties reach the
@@ -12,8 +12,9 @@ import pytest
 from tests import candidate_cases as cc
 from tests import candidate_restatement as cr
 from tests.ref_calls import case_fixture
+from tests.ref_variants import RefVariants
 
-ref_cand = case_fixture("ref_region_candidates.pkl.xz", ref=lambda: cc.RefCand() if cc.RefCand.available() else None)
+ref_cand = case_fixture("ref_region_candidates.pkl.xz", ref=lambda: RefVariants() if RefVariants.available() else None)
 
 
 def restated_lines(c):
@@ -33,7 +34,7 @@ def by_position(lines):
 def test_restatement_equals_reference(ref_cand, name):
     c = cc.build(name)
     cc.claims(c, cc.restated(c))
-    want = ref_cand.answers(name, [cc.fingerprint(c)], lambda _: ref_cand.live.variants(c))[0]
+    want = ref_cand.answers(name, [cc.fingerprint(c)], lambda _: ref_cand.live.variants_in_region(c))[0]
     got = restated_lines(c)
     assert [w[0] for w in want] == sorted(g[0] for g in got), f"{name}: positions differ"
     assert by_position(want) == by_position(got), f"{name}: the variants at some position differ"
@@ -60,7 +61,7 @@ def test_fraction_format():
 def test_reference_region_call(ref_cand, spec):
     """the reference's default-mode region call and VCF (npref_call_region), recorded for the device suite; each case reaches its edge"""
     c = cc.build_call(spec)
-    vcf = ref_cand.answers(spec[0], [cc.call_fingerprint(c)], lambda _: cc.ref_call_region(ref_cand.live.call, c))[0]
+    vcf = ref_cand.answers(spec[0], [cc.call_fingerprint(c)], lambda _: ref_cand.live.call_region(c))[0]
     lines = vcf.decode().splitlines()
     records = [l.split("\t") for l in lines if not l.startswith("#")]
     end = min(c["end_base"], c["contig_length"] - 1)

@@ -1,5 +1,5 @@
 """The compiled reference's own screen_variants_by_score and expand_variants (src/nanopolish_call_variants.cpp:364-450, run unmodified by
-oracle/screen_harness.cpp) against the restatement in tests/screen_restatement.py over the reference's profile_hmm_score: the output
+oracle/variants_harness.cpp) against the restatement in tests/screen_restatement.py over the reference's profile_hmm_score: the output
 list (positions, alleles, quality bits, empty INFO) on every case of tests/screen_cases.py, and expand_variants' list.  Each case
 asserts the edges it was built to reach.  The reference's lists and the restated quality, read count, status and DP rows of every
 candidate are kept in tests/golden/ref_screen_variants.pkl.xz for the device suite (tests/test_gpu_screen_variants.py)."""
@@ -10,8 +10,9 @@ from tests import hp_restatement as hr
 from tests import screen_cases as sc
 from tests import screen_restatement as scr
 from tests.ref_calls import case_fixture
+from tests.ref_variants import RefVariants
 
-ref_screen = case_fixture("ref_screen_variants.pkl.xz", ref=lambda: sc.RefScreen() if sc.RefScreen.available() else None)
+ref_screen = case_fixture("ref_screen_variants.pkl.xz", ref=lambda: RefVariants() if RefVariants.available() else None)
 
 
 @pytest.mark.parametrize("spec", sc.CASES, ids=[s[0] for s in sc.CASES])
@@ -22,7 +23,7 @@ def test_restatement_equals_reference(ref_screen, spec):
     def ask(_):
         hs, mh = live.register(c)
         want = live.screened(c, hs)
-        got = live.restated(c, hs, mh)
+        got = sc.ref_restated(live, c, hs, mh)
         assert scr.kept_lines(c["candidates"], got) == want, f"{spec[0]}: the restated list differs from the reference's"
         return want, [(np.float64(q), n, st, rows) for q, n, st, rows in got]
 

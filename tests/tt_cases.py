@@ -90,14 +90,12 @@ class RefTT(RefOracle):
     """RefOracle over oracle/_ref/libnpref_scorereads.so: its reads, profile_hmm_score / _align, and model_score with training"""
 
     def __init__(self):
-        super().__init__()
-        L = self.lib = C.CDLL(REF_SR)
-        L.npref_score_batch.restype = C.c_double
-        L.npref_model_score_train.restype = C.c_longlong
+        super().__init__(REF_SR)
+        self.lib.npref_model_score_train.restype = C.c_longlong
 
     @staticmethod
     def available() -> bool:
-        return os.path.exists(REF_SR) and RefOracle.available()
+        return RefOracle.available(REF_SR)
 
     def model_score(self, c):
         """(score, counts[81], probs[30], print() text) of the reference"""
