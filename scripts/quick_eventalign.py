@@ -14,7 +14,7 @@ import numpy as np  # noqa: E402
 
 from oracle import eventalign_py as EP  # noqa: E402
 from tests import eventalign_cases as EC  # noqa: E402
-from tests.test_host_mirror import HOST_SO, _register, _register_reads  # noqa: E402
+from tests import host_mirror as hm  # noqa: E402
 
 n_reads = int(sys.argv[1]) if len(sys.argv) > 1 else 256
 n_events = int(sys.argv[2]) if len(sys.argv) > 2 else 4000
@@ -22,13 +22,10 @@ n_ref = int(sys.argv[3]) if len(sys.argv) > 3 else 32
 
 model, rs, cases = EC.build_cases(n_reads, n_events, seed=91)
 cases = cases[:n_reads]                                   # without the unmapped / windowed extras
-host = C.CDLL(HOST_SO)
-host.nphh_last_error.restype = C.c_char_p
-for f in ("nphh_ea_run", "nphh_ea_run_rounds", "nphh_ea_text", "nphh_ea_num_segments", "nphh_ea_tsv_all"):
-    getattr(host, f).restype = C.c_longlong
-p = lambda a: a.ctypes.data_as(C.c_void_p)
-mh = _register(host, model)
-rh = _register_reads(host, rs, mh)
+host = hm.load()
+p = hm.p
+mh = hm.register_model(host, model)
+rh = hm.register_reads(host, rs, mh)
 
 
 def setup():

@@ -23,12 +23,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from nanopolish_b200 import synth                                  # noqa: E402
 from nanopolish_b200.engine import Engine                          # noqa: E402
+from tests import host_mirror as hm                                # noqa: E402
 
 SWITCH_SETS = [("none", 0), ("--signal-index --scale-events", 2 | 4), ("--samples", 8)]
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
 
 
 def card():
@@ -43,37 +40,33 @@ def spread(xs):
 def host_arms(host, model, rs, inp, switches, repeats):
     """wall time of the two EventAligner paths; returns (a, b, bytes)"""
     host.nphh_clear()
-    mean, sd, lsd = (np.ascontiguousarray(x) for x in (model.level_mean, model.level_stdv, model.level_log_stdv))
-    mh = host.nphh_model_create(model.alphabet.encode(), model.k, mean.shape[0], _p(mean), _p(sd), _p(lsd))
-    rh, seqs = [], []
-    for i, r in enumerate(rs.reads):
+    rh = hm.register_reads(host, rs, hm.register_model(host, model))
+    seqs = []
+    for i, (r, h) in enumerate(zip(rs.reads, rh)):
         o, n = int(r["event_off"]), int(r["n_events"])
-        m, t = np.ascontiguousarray(rs.ev_mean[o:o + n]), np.ascontiguousarray(rs.ev_start_time[o:o + n])
-        h = host.nphh_read_create(n, _p(m), _p(t), C.c_double(r["shift"]), C.c_double(r["scale"]), C.c_double(r["drift"]), C.c_double(r["var"]),
-                                  C.c_double(r["events_per_base"]), mh)
         seq = synth._CODE2DNA[rs.seq_codes[i]].tobytes()
         nk = len(seq) - model.k + 1
         start, stop, _ = synth.closest_event_map(rs.ev_kmer[i], nk)
         a, b = np.ascontiguousarray(start, np.int32), np.ascontiguousarray(stop, np.int32)
         tr = inp["reads"][i]
         stdv, dur = np.ascontiguousarray(inp["ev_stdv"][o:o + n]), np.ascontiguousarray(inp["ev_duration"][o:o + n])
-        assert host.nphh_read_set_eventalign(h, f"read_{i}".encode(), seq, _p(a), _p(b), C.c_size_t(nk), _p(stdv), _p(dur)) == 0
+        assert host.nphh_read_set_eventalign(h, f"read_{i}".encode(), seq, hm.p(a), hm.p(b), C.c_size_t(nk), hm.p(stdv), hm.p(dur)) == 0
         if inp["samples"] is not None:
             # the host mirror's sample clock starts at 0: shift the read's samples to where its events index them
             first = int(tr["sample_start_time"])
             smp = np.zeros(first + int(tr["n_samples"]), np.float32)
             smp[first:] = inp["samples"][int(tr["sample_off"]):int(tr["sample_off"]) + int(tr["n_samples"])]
-            assert host.nphh_read_set_samples(h, _p(smp), C.c_size_t(smp.shape[0]), C.c_double(4000.0)) == 0
+            assert host.nphh_read_set_samples(h, hm.p(smp), C.c_size_t(smp.shape[0]), C.c_double(4000.0)) == 0
         elif switches & 4:
             one = np.zeros(1, np.float32)                            # --signal-index wants samples on the read and reads none
-            assert host.nphh_read_set_samples(h, _p(one), C.c_size_t(1), C.c_double(4000.0)) == 0
-        rh.append(h); seqs.append(seq)
+            assert host.nphh_read_set_samples(h, hm.p(one), C.c_size_t(1), C.c_double(4000.0)) == 0
+        seqs.append(seq)
 
     def queue():
         host.nphh_ea_begin()
         for i, seq in enumerate(seqs):
             cigar = np.array([(len(seq) << 4) | 0], np.uint32)
-            assert host.nphh_ea_add_read(rh[i], b"chr_synth", 0, 0, 60, _p(cigar), 1, seq, i, -1, -1) == i, host.nphh_last_error()
+            assert host.nphh_ea_add_read(rh[i], b"chr_synth", 0, 0, 60, hm.p(cigar), 1, seq, i, -1, -1) == i, host.nphh_last_error()
 
     def arm_a(out=None, cap=0):
         queue()
@@ -95,7 +88,7 @@ def host_arms(host, model, rs, inp, switches, repeats):
     # equal bytes first (this is also each arm's warm-up)
     _, n = arm_a()
     ba, bb = np.zeros(n, np.uint8), np.zeros(n, np.uint8)
-    assert arm_a(_p(ba), n)[1] == n and arm_b(_p(bb), n)[1] == n
+    assert arm_a(hm.p(ba), n)[1] == n and arm_b(hm.p(bb), n)[1] == n
     assert np.array_equal(ba, bb), "the device's bytes differ from the host writer's"
     del ba, bb
     ta, tb = [], []
@@ -140,10 +133,7 @@ def main():
     args = ap.parse_args()
     eng = Engine(0)                                                  # raises without a GPU
     print(json.dumps({"card_and_power_limit": card()}))
-    host = C.CDLL(os.path.join(ROOT, "nanopolish_b200", "libnph_host.so"))
-    host.nphh_last_error.restype = C.c_char_p
-    for f in ("nphh_ea_run", "nphh_ea_run_tsv", "nphh_ea_tsv_all_opt"):
-        getattr(host, f).restype = C.c_longlong
+    host = hm.load()
     model = synth.load_model("nucleotide")
     for shape in args.shapes.split(","):
         n_reads, n_events = (int(v) for v in shape.split("x"))

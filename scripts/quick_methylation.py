@@ -14,18 +14,16 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np  # noqa: E402
 
 from nanopolish_b200 import synth  # noqa: E402
-from tests.test_host_mirror import HOST_SO, _register, _register_reads  # noqa: E402
+from tests import host_mirror as hm  # noqa: E402
 
 K = 6
 n_reads = int(sys.argv[1]) if len(sys.argv) > 1 else 512
 n_events = int(sys.argv[2]) if len(sys.argv) > 2 else 4000
-host = C.CDLL(HOST_SO)
-host.nphh_last_error.restype = C.c_char_p
-host.nphh_call_methylation_timed.restype = C.c_longlong
+host = hm.load()
 nuc, cpg = synth.load_model("nucleotide"), synth.load_model("cpg")
 rs = synth.gen_reads(n_reads, n_events, nuc, seed=2024, cpg_keep=0.3)
-mh, ch = _register(host, nuc), _register(host, cpg)
-rh = _register_reads(host, rs, mh)
+mh, ch = hm.register_model(host, nuc), hm.register_model(host, cpg)
+rh = hm.register_reads(host, rs, mh)
 for r in rh:
     host.nphh_read_add_model(r, b"cpg", ch)
 refs_s, pairs_l = [], []
@@ -39,7 +37,7 @@ flat = np.concatenate(pairs_l).reshape(-1)
 off = np.zeros(n_reads + 1, np.uint64); off[1:] = np.cumsum([p.shape[0] for p in pairs_l])
 names = (C.c_char_p * n_reads)(*[f"read_{i}".encode() for i in range(n_reads)])
 refs = (C.c_char_p * n_reads)(*refs_s)
-p = lambda a: a.ctypes.data_as(C.c_void_p)
+p = hm.p
 z = np.zeros(n_reads, np.uint8)
 cap = 400 * 45 * n_reads
 buf = C.create_string_buffer(cap)

@@ -10,7 +10,6 @@ SM clock read in the same run.  --reference times the compiled reference's own A
 
   python scripts/quick_region_candidates.py [reps] [--reference]
 """
-import ctypes as C
 import json
 import os
 import subprocess
@@ -45,8 +44,7 @@ if "--reference" in sys.argv:
     sys.exit(0)
 
 from nanopolish_b200.engine import Engine  # noqa: E402
-from tests.test_gpu_region_candidates import call_region, mirror  # noqa: E402
-from tests.test_host_mirror import HOST_SO  # noqa: E402
+from tests import host_mirror as hm  # noqa: E402
 
 row["gpu"] = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
                             capture_output=True, text=True).stdout.strip()
@@ -61,14 +59,12 @@ for _ in range(reps):
     kern.append(float(cnt["kernel_ms"]))
 row.update(pairs=int(cnt["n_pairs"]), instances=int(cnt["n_instances"]), distinct=int(cnt["n_variants"]),
            device_kernel_ms_median=float(np.median(kern)), device_call_ms_median=float(np.median(call)))
-host = C.CDLL(HOST_SO)
-host.nphh_last_error.restype = C.c_char_p
-host.nphh_variants_in_region.restype = C.c_longlong
-mirror(host, cand)
+host = hm.load()
+cc.mirror(host, cand)
 mir = []
 for _ in range(reps):
     t0 = time.perf_counter()
-    n, kept = mirror(host, cand)
+    n, kept = cc.mirror(host, cand)
     mir.append((time.perf_counter() - t0) * 1e3)
     assert n >= 0, host.nphh_last_error()
 row.update(kept=len(kept), mirror_call_ms_median=float(np.median(mir)),
@@ -76,7 +72,7 @@ row.update(kept=len(kept), mirror_call_ms_median=float(np.median(mir)),
 region = []
 for _ in range(max(1, min(reps, 3))):
     t0 = time.perf_counter()
-    n, vcf = call_region(host, c)
+    n, vcf = cc.call_region(host, c)
     region.append((time.perf_counter() - t0) * 1e3)
     assert n >= 0, host.nphh_last_error()
 row.update(vcf_records=sum(1 for l in vcf.decode().splitlines() if not l.startswith("#")), region_call_and_vcf_with_read_registration_ms_median=float(np.median(region)))

@@ -15,6 +15,7 @@ import numpy as np
 
 from nanopolish_b200 import synth
 from tests import call_restatement as cr
+from tests import host_mirror as hm
 from tests import hp_cases as hc
 from tests import screen_cases as sc
 from tests import support_cases as suc
@@ -129,14 +130,6 @@ def fingerprint(c) -> str:
     return h.hexdigest()
 
 
-def _cstrs(xs):
-    return (C.c_char_p * max(1, len(xs)))(*[x.encode() for x in xs])
-
-
-def _lines(raw):
-    return raw.decode().split("\n")[:-1]
-
-
 def strip_all_support(lines):
     """the lines without ;SupportFractionByBase=... (not restated)"""
     out = [lines[0]]
@@ -187,39 +180,13 @@ def hmm_scores(eng, c):
 def mirror(host, c, candidates=None, ploidy=None, all_support=None):
     """nph::call_haplotype_from_candidates through the nphh_call_haplotype shim: (status, lines).  With types, the reads get the device
     suite's type models (nphh_read_add_model)"""
-    from tests.test_host_mirror import _register, _register_reads
-    p = lambda a: a.ctypes.data_as(C.c_void_p)
-    host.nphh_clear()
-    rs = c["rs"]
-    mh = _register(host, synth.load_model("nucleotide"))
-    hs = _register_reads(host, rs, mh)
-    if c["types"]:
-        from tests.test_variants_methylation_oracle import type_models
-        tm = type_models(c["types"])
-        for t in c["types"]:
-            h = _register(host, tm[t])
-            for r in hs:
-                host.nphh_read_add_model(int(r), t.encode(), h)
-    recs, pairs = c["recs"], c["pairs"]
-    read = np.array([hs[int(x)] for x in recs["read"]], np.int32)
-    rc = np.ascontiguousarray(recs["rc"], np.uint8)
-    pp = np.ascontiguousarray(np.stack([pairs["ref_pos"], pairs["read_pos"]], 1).astype(np.int32))
-    # records index their pairs by pair_off / n_pairs: a repeated record gets its own copy of the pairs
-    order = np.concatenate([np.arange(int(r["pair_off"]), int(r["pair_off"]) + int(r["n_pairs"])) for r in recs] or [np.zeros(0, np.int64)])
-    pp = np.ascontiguousarray(pp[order])
-    po = np.concatenate([[0], np.cumsum(recs["n_pairs"].astype(np.uint64))]).astype(np.uint64)
+    hs = hm.register_case(host, c, synth.load_model("nucleotide"), sc.type_models(c["types"]).values())
     vs = c["candidates"] if candidates is None else candidates
-    vp = np.array([x[0] for x in vs] or [0], np.int32)
-    out = C.create_string_buffer(1 << 22)
-    host.nphh_call_haplotype.restype = C.c_longlong
-    n = host.nphh_call_haplotype(CONTIG.encode(), c["region_start"], c["region_ref"].encode(), int(recs.shape[0]), p(read), p(rc), p(pp), p(po),
-                                 _cstrs(record_names(c)), CONTIG.encode(), len(vs), p(vp), _cstrs([x[1] for x in vs]), _cstrs([x[2] for x in vs]),
-                                 FLANK, MIN_DISTANCE, c["max_haplotypes"], c["ploidy"] if ploidy is None else ploidy, c["genotype_only"],
-                                 ",".join(c["types"]).encode(), c["all_support"] if all_support is None else all_support, C.c_uint32(FLAGS),
-                                 C.c_double(1.0), out, C.c_size_t(1 << 22))
-    if n < 0:
-        return int(n), None
-    return int(n), _lines(out.raw[:n])
+    n, raw = hm.text(host, "nphh_call_haplotype", CONTIG.encode(), c["region_start"], c["region_ref"].encode(), *hm.records(c, hs),
+                     hm.cstrs(record_names(c)), CONTIG.encode(), len(vs), *hm.alleles(vs), FLANK, MIN_DISTANCE, c["max_haplotypes"],
+                     c["ploidy"] if ploidy is None else ploidy, c["genotype_only"], ",".join(c["types"]).encode(),
+                     c["all_support"] if all_support is None else all_support, C.c_uint32(FLAGS), C.c_double(1.0))
+    return n, (None if raw is None else raw.decode().split("\n")[:-1])
 
 
 def device_inputs(c, genotype_all=1):

@@ -5,12 +5,14 @@ bounds [start, stop] and the filter (min_frequency, min_depth).  Records are wri
 (rec()), or drawn from a seeded truth with basecall errors (synth.basecall_of).  Each case states the edge it was built to reach
 and `claims(case, distinct)` checks it on the restatement's answer.  Cases with `before_start` records (aligned entirely before
 start, where the reference dereferences end()) are never sent to the compiled reference."""
+import ctypes as C
 import hashlib
 
 import numpy as np
 
 from nanopolish_b200 import synth
 from tests import candidate_restatement as cr
+from tests import host_mirror as hm
 
 CONTIG = "ctg1"
 F02 = float(np.float32(0.2))            # the reference's default -m: the float literal 0.2f widened to double
@@ -216,6 +218,15 @@ def parse(raw: bytes):
     return [tuple(int(f) if i == 0 else f for i, f in enumerate(l.split("\t"))) for l in raw.decode("latin-1").splitlines()]
 
 
+def mirror(host, c, counts=None):
+    """nph::get_variants_in_region through the nphh_variants_in_region shim: (status, the parsed list or None)"""
+    pp, off = flat_pairs(c)
+    n, raw = hm.text(host, "nphh_variants_in_region", CONTIG.encode(), c["region_start"], c["region_ref"].encode(), len(c["bases"]),
+                     hm.cstrs(c["bases"]), hm.p(np.array(c["rc"] or [0], np.uint8)), hm.p(pp), hm.p(off), c["start"], c["stop"],
+                     C.c_double(c["min_frequency"]), c["min_depth"], None if counts is None else hm.p(counts), cap=1 << 26)
+    return n, (None if raw is None else parse(raw))
+
+
 # ---- the default-mode region call: call_variants_for_region + call_variants_main's VCF ----------------------------------------
 # (name, ref_len, depth, read_bases, seed, n_true, ploidy, all_support, snps_only, candidates file, contig_length, end past the contig)
 CALL_CASES = [
@@ -265,19 +276,13 @@ def call_fingerprint(c) -> str:
     return h.hexdigest()
 
 
-def call_args(c):
-    """the arrays the host mirror's region call takes: event records (read index per record, rc, flat pairs, offsets) and base-space
-    records"""
-    recs, pairs = c["recs"], c["pairs"]
+def call_region(host, c):
+    """`variants` in its default mode through the nphh_call_region shim (nph::call_variants_for_region + nph::write_variants_vcf):
+    (status, the VCF bytes or None)"""
+    hs = hm.register_case(host, c, synth.load_model("nucleotide"))
     pp, off = flat_pairs(c)
-    return dict(rc=np.ascontiguousarray(recs["rc"], np.uint8),
-                po=np.ascontiguousarray(recs["pair_off"], np.uint64), npair=np.ascontiguousarray(recs["n_pairs"], np.uint32),
-                ep=np.ascontiguousarray(np.stack([pairs["ref_pos"], pairs["read_pos"]], 1).astype(np.int32)),
-                seq_bases=c["bases"], seq_rc=np.array(c["rc"] or [0], np.uint8), sp=pp, soff=off,
-                names=[c["names"][int(r)] for r in recs["read"]])
-
-
-def _cstrs(xs):
-    import ctypes as C
-    return (C.c_char_p * max(len(xs), 1))(*[x if isinstance(x, bytes) else x.encode() for x in xs])
-
+    return hm.text(host, "nphh_call_region", b"ctg", c["contig_length"], c["start_base"], c["end_base"], c["region_start"],
+                   c["region_ref"].encode(), *hm.records(c, hs), hm.cstrs([c["names"][int(r)] for r in c["recs"]["read"]]), len(c["bases"]),
+                   hm.cstrs(c["bases"]), hm.p(np.array(c["rc"] or [0], np.uint8)), hm.p(pp), hm.p(off), CALL_FLANK, CALL_MIN_DISTANCE,
+                   CALL_MAX_HAPLOTYPES, c["ploidy"], 0, b"", c["all_support"], c["snps_only"], C.c_double(c["min_frequency"]), c["min_depth"],
+                   None if c["candidates"] is None else c["candidates"].encode(), C.c_double(1.0), cap=1 << 24)

@@ -1,12 +1,17 @@
 """Synthetic eventalign inputs shared by the oracle, host-logic and GPU tests (SURVEY.md 8f N1): reads as
 load_from_raw leaves them (events, scalings, basecalled sequence, base-to-event map) plus what the reference pulls
-from the BAM record and the FASTA (position, flag, CIGAR, contig).  Seeded; no file access."""
+from the BAM record and the FASTA (position, flag, CIGAR, contig).  Seeded; no file access.  Also the ways the host
+mirror's EventAligner and ScoreReads take them: load_batch, drive_rounds and scorereads."""
+import ctypes as C
+
 import numpy as np
 
 from nanopolish_b200 import synth
 from oracle import eventalign_py as EP
+from tests import host_mirror as hm
 
 K = 6
+EPS = 200          # events per segment of scorereads (the reference uses 500 on whole reads; the test reads have ~1 500 events)
 _DNA = "ACGT"
 
 
@@ -114,3 +119,67 @@ def port_align_fn(port_oracle, rs, model, slot, indel_bias=1.0):
         st, status = port_oracle.hmm_align(rs.reads, rs.ev_mean, rs.ev_start_time, [model], ranks, jb[0], indel_bias=indel_bias)
         return [(int(s["event_idx"]), int(s["kmer_idx"]), s["state"].decode()) for s in st]
     return fn
+
+
+def raw_samples(slot):
+    """stand-in for the trimmed raw samples SRF_LOAD_RAW_SAMPLES keeps: enough of them to cover every event's time span"""
+    return np.random.default_rng(900 + slot).normal(90.0, 12.0, 420_000).astype(np.float32)
+
+
+def load_batch(host, cases, samples_of=raw_samples):
+    """clear the mirror, register the model and reads, give each case's read its eventalign data and its samples (samples_of(slot), at
+    4 kHz; none where that is None), and queue every case in a new EventAligner batch"""
+    model, rs, cs = cases
+    host.nphh_clear()
+    mh = hm.register_model(host, model)
+    rh = hm.register_reads(host, rs, mh)
+    host.nphh_ea_begin()
+    for c in cs:
+        slot, r = read_slot(c, rs.n_reads), c["read"]
+        a, b = np.ascontiguousarray(r.b2e_start, np.int32), np.ascontiguousarray(c["b2e_stop"], np.int32)
+        assert host.nphh_read_set_eventalign(rh[slot], r.name.encode(), r.read_sequence.encode(), hm.p(a), hm.p(b), C.c_size_t(a.shape[0]),
+                                             hm.p(np.ascontiguousarray(r.stdv)), hm.p(np.ascontiguousarray(r.duration))) == 0
+        smp = samples_of(slot)
+        if smp is not None:
+            assert host.nphh_read_set_samples(rh[slot], hm.p(smp), C.c_size_t(smp.shape[0]), C.c_double(4000.0)) == 0
+        idx = host.nphh_ea_add_read(rh[slot], c["contig_name"].encode(), c["ref_pos"], c["flag"], c["mapq"], hm.p(c["cigar"]),
+                                    int(c["cigar"].shape[0]), c["fetched"].encode(), c["read_idx"], c["region"][0], c["region"][1])
+        assert idx == c["read_idx"], host.nphh_last_error()
+
+
+def drive_rounds(host, cs, rs, model, port_oracle):
+    """pull every round's jobs out of the C++ cursors and feed back the plain-C Viterbi's paths"""
+    jobs = np.zeros(max(len(cs), 1), synth.HMM_JOB_DT)
+    ranks = np.zeros(len(cs) * 400 + 400, np.uint32)
+    n_ranks = C.c_uint64()
+    rounds = 0
+    while True:
+        n = host.nphh_ea_next_round(hm.p(jobs), C.c_size_t(jobs.shape[0]), hm.p(ranks), C.c_size_t(ranks.shape[0]), C.byref(n_ranks))
+        assert n >= 0, host.nphh_last_error()
+        if n == 0:
+            return rounds
+        paths, off = [], [0]
+        for j in range(n):
+            jb = jobs[j].copy()
+            jb["read"] = read_slot(cs[int(jb["read"])], rs.n_reads)
+            st, _ = port_oracle.hmm_align(rs.reads, rs.ev_mean, rs.ev_start_time, [model], ranks, jb)
+            paths.append(st); off.append(off[-1] + st.shape[0])
+        flat = np.concatenate(paths) if off[-1] else np.zeros(0, synth.ALIGN_STATE_DT)
+        assert host.nphh_ea_consume(C.c_size_t(n), hm.p(np.array(off, np.uint64)), hm.p(flat)) == 0, host.nphh_last_error()
+        rounds += 1
+
+
+def scorereads(host, cases, mode):
+    """ScoreReads over the cases' event alignments (nphh_scorereads, EPS events per segment; mode 0 builds the jobs only, 1 scores
+    them on the device): (jobs, ranks, per-read (score, events, segments))"""
+    model, rs, cs = cases
+    n = len(cs)
+    reads = np.array([read_slot(c, rs.n_reads) for c in cs], np.int32)      # g_reads handles == slots after load_batch
+    refs = (C.c_char_p * n)(*[c["fetched"].encode() for c in cs])
+    offs = np.array([c["ref_pos"] for c in cs], np.int32)
+    jobs = np.zeros(256, synth.HMM_JOB_DT); ranks = np.zeros(1 << 18, np.uint32); nr = C.c_uint64(); sc = np.zeros((n, 3))
+    p = hm.p
+    k = host.nphh_scorereads(n, p(reads), refs, p(offs), EPS, mode, p(jobs), C.c_size_t(jobs.shape[0]), p(ranks), C.c_size_t(ranks.shape[0]),
+                             C.byref(nr), p(sc))
+    assert k >= 0, host.nphh_last_error()
+    return jobs[:k].copy(), ranks[:nr.value].copy(), sc

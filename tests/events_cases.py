@@ -35,6 +35,14 @@ PEAK_STATE_DT = np.dtype([("masked_to", "<u8", 2), ("peak_pos", "<i8", 2), ("pea
 assert PEAK_STATE_DT.itemsize == 48
 
 
+def same(got, want):
+    """identical boundaries and bit-identical length / mean / stdv"""
+    assert got.shape[0] == want.shape[0]
+    assert np.array_equal(got["start"], want["start"])
+    for f in ("length", "mean", "stdv"):
+        assert np.array_equal(got[f].view(np.uint32), want[f].view(np.uint32)), f
+
+
 def params(w1, w2, t1=None, t2=9.0, ph=None):
     p = np.zeros(1, synth.EVENT_PARAMS_DT)
     rna = w2 >= 10

@@ -13,6 +13,7 @@ import os
 import numpy as np
 
 from nanopolish_b200 import synth
+from tests import host_mirror as hm
 from tests import hp_restatement as hr
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -193,36 +194,14 @@ def vectors_of(liks):
     return [(int(x["total_reads"]), [float(v) for v in x["event_lik"]], [float(v) for v in x["duration_lik"]]) for x in liks]
 
 
-def _cstrs(xs):
-    return (C.c_char_p * max(1, len(xs)))(*[x.encode() for x in xs])
-
-
 def mirror(host, c, indel_bias=1.0) -> str:
     """nph::fix_homopolymers through the nphh_fix_homopolymers shim (the device call): the fixed text"""
-    from tests.test_host_mirror import _register, _register_reads
-    p = lambda a: a.ctypes.data_as(C.c_void_p)
-    host.nphh_clear()
-    rs = c["rs"]
-    mh = _register(host, c["model"])
-    hs = _register_reads(host, rs, mh)
-    for i, r in enumerate(rs.reads):
-        o, n = int(r["event_off"]), int(r["n_events"])
-        host.nphh_read_set_durations(hs[i], p(np.ascontiguousarray(c["dur"][o:o + n])))
-    recs, pairs = c["recs"], c["pairs"]
-    read = np.array([hs[int(x)] for x in recs["read"]], np.int32)
-    rc = np.ascontiguousarray(recs["rc"], np.uint8)
-    pp = np.ascontiguousarray(np.stack([pairs["ref_pos"], pairs["read_pos"]], 1).astype(np.int32))
-    po = np.zeros(recs.shape[0] + 1, np.uint64)
-    po[:-1] = recs["pair_off"]; po[-1] = pairs.shape[0]
-    assert (po[1:-1] == po[:-2] + recs["n_pairs"][:-1]).all()
-    vp = np.array([REGION_START + o for o, _, _ in c["variants"]] or [0], np.int32)
-    out = C.create_string_buffer(1 << 20)
-    host.nphh_fix_homopolymers.restype = C.c_longlong
-    n = host.nphh_fix_homopolymers(CONTIG.encode(), c["region_start"], c["region_ref"].encode(), int(recs.shape[0]), p(read), p(rc), p(pp), p(po),
-                                   REGION_START, c["draft"].encode(), len(c["variants"]), p(vp), _cstrs([r for _, r, _ in c["variants"]]),
-                                   _cstrs([a for _, _, a in c["variants"]]), c["min_flank"], C.c_double(indel_bias), out, C.c_size_t(1 << 20))
+    hs = hm.register_case(host, c, c["model"], durations=c["dur"])
+    vs = [(REGION_START + o, r, a) for o, r, a in c["variants"]]
+    n, raw = hm.text(host, "nphh_fix_homopolymers", CONTIG.encode(), c["region_start"], c["region_ref"].encode(), *hm.records(c, hs),
+                     REGION_START, c["draft"].encode(), len(vs), *hm.alleles(vs), c["min_flank"], C.c_double(indel_bias), cap=1 << 20)
     assert n >= 0, (n, host.nphh_last_error())
-    return out.raw[:n].decode()
+    return raw.decode()
 
 
 def ranges(lib, entry: str, hap_ref: str, variants, start, end, lo, hi):
@@ -230,10 +209,8 @@ def ranges(lib, entry: str, hap_ref: str, variants, start, end, lo, hi):
     npref_haplotype_ranges (the compiled reference) or nphh_haplotype_ranges (the mirror)"""
     fn = getattr(lib, entry)
     fn.restype = C.c_longlong
-    vp = np.array([REGION_START + o for o, _, _ in variants] or [0], np.int32)
     rng = np.zeros(4, np.int64)
     out = C.create_string_buffer(1 << 16)
-    n = fn(REGION_START, hap_ref.encode(), len(variants), vp.ctypes.data_as(C.c_void_p), _cstrs([r for _, r, _ in variants]),
-           _cstrs([a for _, _, a in variants]), C.c_longlong(start), C.c_longlong(end), C.c_longlong(lo), C.c_longlong(hi),
-           rng.ctypes.data_as(C.c_void_p), out, C.c_size_t(1 << 16))
+    n = fn(REGION_START, hap_ref.encode(), len(variants), *hm.alleles([(REGION_START + o, r, a) for o, r, a in variants]),
+           C.c_longlong(start), C.c_longlong(end), C.c_longlong(lo), C.c_longlong(hi), hm.p(rng), out, C.c_size_t(1 << 16))
     return int(n), out.value.decode(), tuple(int(x) for x in rng)

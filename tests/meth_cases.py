@@ -100,3 +100,20 @@ def tsv_rows(contig_name, strand_char, read_name, rows):
         m, u = float(ll_m) + 0.0, float(ll_u) + 0.0
         out.append("%s\t%s\t%d\t%d\t%s\t%.2f\t%.2f\t%.2f\t%d\t%d\t%s\n" % (contig_name, strand_char, sp, ep, read_name, m - u, m, u, 1, nm, seq))
     return "".join(out)
+
+
+def expected_rows(sites, site_off, recs, ref, names, is_rev, contig, k):
+    """the reference's writer (src/nanopolish_call_methylation.cpp:113-140) over site records, formatted by Python's correctly
+    rounded %.2f — the C library's %.2lf"""
+    out = []
+    for r in range(recs.shape[0]):
+        R = recs[r]
+        seg = ref[int(R["ref_off"]):int(R["ref_off"]) + int(R["ref_len"])].tobytes().decode()
+        for s in sites[int(site_off[r]):int(site_off[r + 1])]:
+            ll_m, ll_u = float(s["ll_methylated"]) + 0.0, float(s["ll_unmethylated"]) + 0.0
+            b = int(s["start_position"]) - int(R["ref_start_pos"]) - k + 1
+            e = min(int(s["end_position"]) - int(R["ref_start_pos"]) + k, int(R["ref_len"]))
+            out.append("%s\t%s\t%d\t%d\t%s\t%.2f\t%.2f\t%.2f\t%d\t%d\t%s\n" % (
+                contig, "-" if is_rev[r] else "+", int(s["start_position"]), int(s["end_position"]), names[r], ll_m - ll_u, ll_m, ll_u, 1,
+                int(s["n_motif"]), seg[b:e]))
+    return "".join(out)

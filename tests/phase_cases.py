@@ -12,6 +12,7 @@ import os
 import numpy as np
 
 from nanopolish_b200 import synth
+from tests import host_mirror as hm
 from tests import meth_cases as mc
 from tests import phase_restatement as pr
 
@@ -19,10 +20,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 REF_PHASE = os.path.join(ROOT, "oracle", "_ref", "libnpref_phase.so")
 CONTIG = "chr1"
 _NT16 = "=ACMGRSVTWYHKDBN"
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
 
 
 def cases(rs, seed=7, mapq=60):
@@ -115,12 +112,12 @@ class RefPhase:
         for i, r in enumerate(rs.reads):
             o, n = int(r["event_off"]), int(r["n_events"])
             m = np.ascontiguousarray(rs.ev_mean[o:o + n]); t = np.ascontiguousarray(rs.ev_start_time[o:o + n])
-            h = self.lib.npref_read_create(C.c_uint32(n), _p(m), _p(t), C.c_double(r["shift"]), C.c_double(r["scale"]), C.c_double(r["drift"]),
+            h = self.lib.npref_read_create(C.c_uint32(n), hm.p(m), hm.p(t), C.c_double(r["shift"]), C.c_double(r["scale"]), C.c_double(r["drift"]),
                                            C.c_double(r["var"]), C.c_double(r["events_per_base"]), self.mh)
             c = case_list[i]
             a, b = np.ascontiguousarray(c["b2e_start"], np.int32), np.ascontiguousarray(c["b2e_stop"], np.int32)
             one = np.ones(n, np.float32)
-            self.lib.npref_read_set_eventalign(h, c["name"].encode(), c["read_sequence"].encode(), _p(a), _p(b), C.c_size_t(a.shape[0]), _p(one), _p(one))
+            self.lib.npref_read_set_eventalign(h, c["name"].encode(), c["read_sequence"].encode(), hm.p(a), hm.p(b), C.c_size_t(a.shape[0]), hm.p(one), hm.p(one))
             hs.append(h)
         return hs
 
@@ -130,7 +127,7 @@ class RefPhase:
         vr = (C.c_char_p * len(var))(*[v[1].encode() for v in var]); va = (C.c_char_p * len(var))(*[v[2].encode() for v in var])
         buf = C.create_string_buffer(1 << 20)
         n = self.lib.npref_phase_read(h, case["name"].encode(), CONTIG.encode(), case["contig"].encode(), case["ref_pos"], case["flag"], case["mapq"],
-                                      _p(cg), cg.shape[0], len(var), _p(vp), vr, va, C.c_double(indel_bias), buf, C.c_size_t(1 << 20))
+                                      hm.p(cg), cg.shape[0], len(var), hm.p(vp), vr, va, C.c_double(indel_bias), buf, C.c_size_t(1 << 20))
         assert n >= 0
         return buf.value.decode() if n else None
 
@@ -150,8 +147,7 @@ def mirror_sam(host, host_reads, case_list, var, indel_bias=1.0):
     rh = np.array(host_reads, np.int32)
     cap = 1 << 26
     buf = C.create_string_buffer(cap)
-    host.nphh_phase_reads.restype = C.c_longlong
-    got = host.nphh_phase_reads(n, _p(rh), names, _p(flags), _p(mapq), _p(starts), refs, _p(pairs), _p(off), CONTIG.encode(), len(var), _p(vp), vr, va,
+    got = host.nphh_phase_reads(n, hm.p(rh), names, hm.p(flags), hm.p(mapq), hm.p(starts), refs, hm.p(pairs), hm.p(off), CONTIG.encode(), len(var), hm.p(vp), vr, va,
                                 C.c_double(indel_bias), buf, C.c_size_t(cap))
     assert got >= 0, host.nphh_last_error()
     return buf.value.decode()

@@ -10,10 +10,12 @@ Its answers come from
   mirror        nph::screen_variants_by_score through the nphh_screen_variants shim (the device call)."""
 import ctypes as C
 import hashlib
+import os
 
 import numpy as np
 
 from nanopolish_b200 import synth
+from tests import host_mirror as hm
 from tests import hp_cases as hc
 from tests import screen_restatement as scr
 from tests import support_cases as suc
@@ -23,6 +25,8 @@ REGION_START = hc.REGION_START
 CONTIG = hc.CONTIG
 FLAGS = 3                               # HAF_ALLOW_PRE_CLIP | HAF_ALLOW_POST_CLIP, what `variants` passes
 ALL_TYPES = ("cpg", "dam", "dcm")       # the device suite's model ids 1, 2, 3
+TYPE_LISTS = [["cpg"], ["dam"], ["dcm"], ["dam", "dcm"], ["dcm", "dam"]]
+N_AT = (33, 71)                     # region offsets of the planted N (inside some windows' flanks, never at a screened base or its left neighbour)
 
 # (name, pile-up, trim, flank, alignment_flags, score_threshold, methylation types, candidates).  pile-up: as tests/support_cases.py,
 # or ("meth", ref_len, depth, read_bases, seed); trim (a, b): the region is the draft without its first a and last b bases.  candidates:
@@ -53,6 +57,28 @@ EXPAND = [
 ]
 
 
+def type_models(types):
+    for name in types:
+        # without its fixture load_model falls back to a synthetic table and the comparison would mean nothing
+        assert os.path.exists(os.path.join(synth._GOLDEN, f"r9.4_450bps.{name}.6mer.template.npz")), name
+    return {name: synth.load_model(name) for name in types}
+
+
+def methylated_pileup(types, ref_len, depth, read_bases, seed):
+    nuc = synth.load_model("nucleotide")
+    tm = type_models(types)
+    ref, rs, recs, pairs = synth.gen_pileup_methylated(ref_len, depth, read_bases, nuc, types, tm, seed=seed, region_start=REGION_START,
+                                                       n_true_variants=6, rc_every=2, methylated_fraction=0.6)
+    ref_chars = synth._CODE2DNA[ref].copy()
+    return nuc, tm, ref, ref_chars, rs, recs, pairs
+
+
+def with_n(ref_chars):
+    out = ref_chars.copy()
+    out[list(N_AT)] = ord("N")
+    return out
+
+
 def _other(b: str) -> str:
     return "ACGT"[("ACGT".index(b.upper()) + 1) % 4]
 
@@ -60,7 +86,6 @@ def _other(b: str) -> str:
 def _pileup(kind, types):
     if kind[0] != "meth":
         return suc._pileup(kind, synth.load_model("nucleotide"))
-    from tests.test_variants_methylation_oracle import methylated_pileup
     _, ref_len, depth, read_bases, seed = kind
     _, _, _, ref_chars, rs, recs, pairs = methylated_pileup(list(types), ref_len, depth, read_bases, seed)
     draft = ref_chars.tobytes().decode()
@@ -219,43 +244,15 @@ def hmm_scores(eng, c):
     return score
 
 
-def _cstrs(xs):
-    return (C.c_char_p * max(1, len(xs)))(*[x.encode() for x in xs])
-
-
 def mirror(host, c, candidates=None):
     """nph::screen_variants_by_score through the nphh_screen_variants shim: (status, [line per kept variant]).  With types, the reads
     get the device suite's type models (nphh_read_add_model)"""
-    from tests.test_host_mirror import _register, _register_reads
-    p = lambda a: a.ctypes.data_as(C.c_void_p)
-    host.nphh_clear()
-    rs = c["rs"]
-    mh = _register(host, synth.load_model("nucleotide"))
-    hs = _register_reads(host, rs, mh)
-    if c["types"]:
-        from tests.test_variants_methylation_oracle import type_models
-        tm = type_models(c["types"])
-        for t in c["types"]:
-            h = _register(host, tm[t])
-            for r in hs:
-                host.nphh_read_add_model(int(r), t.encode(), h)
-    recs, pairs = c["recs"], c["pairs"]
-    read = np.array([hs[int(x)] for x in recs["read"]], np.int32)
-    rc = np.ascontiguousarray(recs["rc"], np.uint8)
-    pp = np.ascontiguousarray(np.stack([pairs["ref_pos"], pairs["read_pos"]], 1).astype(np.int32))
-    po = np.zeros(recs.shape[0] + 1, np.uint64)
-    po[:-1] = recs["pair_off"]; po[-1] = pairs.shape[0]
+    hs = hm.register_case(host, c, synth.load_model("nucleotide"), type_models(c["types"]).values())
     vs = c["candidates"] if candidates is None else candidates
-    vp = np.array([x[0] for x in vs] or [0], np.int32)
-    out = C.create_string_buffer(1 << 22)
-    host.nphh_screen_variants.restype = C.c_longlong
-    n = host.nphh_screen_variants(CONTIG.encode(), c["region_start"], c["region_ref"].encode(), int(recs.shape[0]), p(read), p(rc), p(pp), p(po),
-                                  CONTIG.encode(), len(vs), p(vp), _cstrs([x[1] for x in vs]), _cstrs([x[2] for x in vs]), c["flank"],
-                                  C.c_uint32(c["threshold"]), ",".join(c["types"]).encode(), C.c_uint32(c["flags"]), C.c_double(1.0), out,
-                                  C.c_size_t(1 << 22))
-    if n < 0:
-        return int(n), None
-    return int(n), out.raw[:n].decode().split("\n")[:-1]
+    n, raw = hm.text(host, "nphh_screen_variants", CONTIG.encode(), c["region_start"], c["region_ref"].encode(), *hm.records(c, hs),
+                     CONTIG.encode(), len(vs), *hm.alleles(vs), c["flank"], C.c_uint32(c["threshold"]), ",".join(c["types"]).encode(),
+                     C.c_uint32(c["flags"]), C.c_double(1.0))
+    return n, (None if raw is None else raw.decode().split("\n")[:-1])
 
 
 def expand_candidates(c):
@@ -272,15 +269,9 @@ def expand_candidates(c):
 
 
 def host_expand(host, c, cands, min_flank, var_contig=CONTIG):
-    p = lambda a: a.ctypes.data_as(C.c_void_p)
-    vp = np.array([x[0] for x in cands] or [0], np.int32)
-    out = C.create_string_buffer(1 << 22)
-    host.nphh_expand_variants.restype = C.c_longlong
-    n = host.nphh_expand_variants(CONTIG.encode(), c["region_start"], c["region_ref"].encode(), var_contig.encode(), len(cands), p(vp),
-                                  _cstrs([x[1] for x in cands]), _cstrs([x[2] for x in cands]), min_flank, out, C.c_size_t(1 << 22))
-    if n < 0:
-        return int(n), None
-    return int(n), out.raw[:n].decode().split("\n")[:-1]
+    n, raw = hm.text(host, "nphh_expand_variants", CONTIG.encode(), c["region_start"], c["region_ref"].encode(), var_contig.encode(),
+                     len(cands), *hm.alleles(cands), min_flank)
+    return n, (None if raw is None else raw.decode().split("\n")[:-1])
 
 
 def expand_lines(xs):

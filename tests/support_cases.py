@@ -14,6 +14,7 @@ import hashlib
 import numpy as np
 
 from nanopolish_b200 import synth
+from tests import host_mirror as hm
 from tests import hp_cases as hc
 from tests import hp_restatement as hr
 from tests import support_restatement as sr
@@ -203,31 +204,10 @@ def device(eng, c, variants=None, params=None):
                                  c["first"], c["recs"], c["params"] if params is None else params, ref_seqs, varr)
 
 
-def _cstrs(xs):
-    return (C.c_char_p * max(1, len(xs)))(*[x.encode() for x in xs])
-
-
 def mirror(host, c, var_contig=CONTIG, variants=None):
     """nph::annotate_variants_with_all_support through the nphh_all_support shim: (status, [INFO per variant])"""
-    from tests.test_host_mirror import _register, _register_reads
-    p = lambda a: a.ctypes.data_as(C.c_void_p)
-    host.nphh_clear()
-    rs = c["rs"]
-    mh = _register(host, c["model"])
-    hs = _register_reads(host, rs, mh)
-    recs, pairs = c["recs"], c["pairs"]
-    read = np.array([hs[int(x)] for x in recs["read"]], np.int32)
-    rc = np.ascontiguousarray(recs["rc"], np.uint8)
-    pp = np.ascontiguousarray(np.stack([pairs["ref_pos"], pairs["read_pos"]], 1).astype(np.int32))
-    po = np.zeros(recs.shape[0] + 1, np.uint64)
-    po[:-1] = recs["pair_off"]; po[-1] = pairs.shape[0]
+    hs = hm.register_case(host, c, c["model"])
     vs = c["variants"] if variants is None else variants
-    vp = np.array([x[0] for x in vs] or [0], np.int32)
-    out = C.create_string_buffer(1 << 20)
-    host.nphh_all_support.restype = C.c_longlong
-    n = host.nphh_all_support(CONTIG.encode(), c["region_start"], c["region_ref"].encode(), int(recs.shape[0]), p(read), p(rc), p(pp), p(po),
-                              var_contig.encode(), len(vs), p(vp), _cstrs([x[1] for x in vs]), _cstrs([x[2] for x in vs]), c["flank"],
-                              C.c_uint32(c["flags"]), C.c_double(1.0), out, C.c_size_t(1 << 20))
-    if n < 0:
-        return int(n), None
-    return int(n), out.raw[:n].decode().split("\n")[:-1]
+    n, raw = hm.text(host, "nphh_all_support", CONTIG.encode(), c["region_start"], c["region_ref"].encode(), *hm.records(c, hs),
+                     var_contig.encode(), len(vs), *hm.alleles(vs), c["flank"], C.c_uint32(c["flags"]), C.c_double(1.0), cap=1 << 20)
+    return n, (None if raw is None else raw.decode().split("\n")[:-1])

@@ -5,7 +5,6 @@ SupportFractionByBase, which is not restated).  Each case asserts the edges it w
 against the reference's kt_fisher_exact on every table of at most 60 reads and on large and underflowing tables, and the visit orders of
 the reference's Combinations generator.  The reference's answers are kept in tests/golden/ref_call_haplotype.pkl.xz for the device
 suite (tests/test_gpu_call_variants.py) and for machines without the reference."""
-import ctypes as C
 import hashlib
 import itertools
 
@@ -14,9 +13,9 @@ import pytest
 
 from tests import call_cases as cc
 from tests import call_restatement as cr
+from tests import host_mirror as hm
 from tests.ref_calls import case_fixture
 from tests.ref_variants import RefVariants
-from tests.test_host_mirror import HOST_SO
 
 ref_call = case_fixture("ref_call_haplotype.pkl.xz", ref=lambda: RefVariants() if RefVariants.available() else None)
 
@@ -90,9 +89,7 @@ def _fisher_answers(fisher):
 
 
 def test_fisher_equals_reference(ref_call):
-    host = C.CDLL(HOST_SO)
-    host.nphh_fisher_exact.restype = C.c_double
-    host.nphh_fisher_exact.argtypes = [C.c_int] * 4
+    host = hm.load()
     want = ref_call.answers("fisher", [repr((60, BIG_TABLES))], lambda _: _fisher_answers(ref_call.live.fisher))[0]
     assert _fisher_answers(host.nphh_fisher_exact) == tuple(want)
     # the restatement the device suite uses, on a sample of the tables and the large ones

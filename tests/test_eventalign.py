@@ -23,7 +23,7 @@ import pytest
 from nanopolish_b200 import synth
 from oracle import eventalign_py as EP
 from tests import eventalign_cases as EC
-from tests.test_host_mirror import HOST_SO, _register, _register_reads
+from tests import host_mirror as hm
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "eventalign_golden.npz")
 
@@ -83,7 +83,7 @@ def test_sample_columns_match_compiled_reference(cases, ref_oracle):
     for c in cs[:2]:
         slot, r = EC.read_slot(c, rs.n_reads), c["read"]
         ref_oracle.read_set_eventalign(rh[slot], r.name, r.read_sequence, r.b2e_start, c["b2e_stop"], r.stdv, r.duration)
-        smp = _raw_samples(slot)
+        smp = EC.raw_samples(slot)
         ref_oracle.read_set_samples(rh[slot], smp, 4000.0)
         for e in (0, 1, 17, 400, int(rs.reads[slot]["n_events"]) - 1):
             a, b, v = ref_oracle.event_samples(rh[slot], e)
@@ -106,40 +106,7 @@ def test_restatement_matches_golden(cases, restated, golden):
 
 
 # ---- the C++ host side --------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def host():
-    lib = C.CDLL(HOST_SO)
-    lib.nphh_last_error.restype = C.c_char_p
-    for f in ("nphh_ea_run", "nphh_ea_next_round", "nphh_ea_text", "nphh_ea_num_segments", "nphh_aligned_segments"):
-        getattr(lib, f).restype = C.c_longlong
-    return lib
-
-
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
-
-
-def _setup(host, cases):
-    model, rs, cs = cases
-    host.nphh_clear()
-    mh = _register(host, model)
-    rh = _register_reads(host, rs, mh)
-    host.nphh_ea_begin()
-    for c in cs:
-        slot, r = EC.read_slot(c, rs.n_reads), c["read"]
-        a, b = np.ascontiguousarray(r.b2e_start, np.int32), np.ascontiguousarray(c["b2e_stop"], np.int32)
-        assert host.nphh_read_set_eventalign(rh[slot], r.name.encode(), r.read_sequence.encode(), _p(a), _p(b), C.c_size_t(a.shape[0]),
-                                             _p(np.ascontiguousarray(r.stdv)), _p(np.ascontiguousarray(r.duration))) == 0
-        smp = _raw_samples(slot)
-        assert host.nphh_read_set_samples(rh[slot], _p(smp), C.c_size_t(smp.shape[0]), C.c_double(4000.0)) == 0
-        idx = host.nphh_ea_add_read(rh[slot], c["contig_name"].encode(), c["ref_pos"], c["flag"], c["mapq"], _p(c["cigar"]),
-                                    int(c["cigar"].shape[0]), c["fetched"].encode(), c["read_idx"], c["region"][0], c["region"][1])
-        assert idx == c["read_idx"], host.nphh_last_error()
-
-
-def _raw_samples(slot):
-    """stand-in for the trimmed raw samples SRF_LOAD_RAW_SAMPLES keeps: enough of them to cover every event's time span"""
-    return np.random.default_rng(900 + slot).normal(90.0, 12.0, 420_000).astype(np.float32)
+host = hm.fixture()
 
 
 def _text(host, idx, what):
@@ -157,9 +124,9 @@ def _check_outputs(host, cases, restated, golden):
         assert _text(host, i, 1) == EP.tsv(r, al, print_read_names=True)                   # -n
         assert _text(host, i, 2) == EP.tsv(r, al, scale_events=True)                       # --scale-events
         hdr = _text(host, 0, 6)[:-1] + "\tstart_idx\tend_idx\tsamples\n"
-        assert _text(host, i, 7) == hdr + EP.tsv(r, al, samples=_raw_samples(EC.read_slot(c, rs.n_reads)), sample_rate=4000.0)   # --signal-index --samples
+        assert _text(host, i, 7) == hdr + EP.tsv(r, al, samples=EC.raw_samples(EC.read_slot(c, rs.n_reads)), sample_rate=4000.0)   # --signal-index --samples
         ints, dbl = np.zeros(5, np.int32), np.zeros(2)
-        assert host.nphh_ea_summary(i, _p(ints), _p(dbl)) == 0
+        assert host.nphh_ea_summary(i, hm.p(ints), hm.p(dbl)) == 0
         sm = EP.summarize(r, al)
         assert [int(v) for v in ints] == [sm["num_events"], sm["num_steps"], sm["num_stays"], sm["num_skips"], sm["reference_span"]]
         assert (float(dbl[0]), float(dbl[1])) == (sm["sum_duration"], sm["sum_z_score"])
@@ -168,7 +135,6 @@ def _check_outputs(host, cases, restated, golden):
         if _single_segment(c):
             assert _text(host, i, 4) == golden[f"cigar_{i}"]
             assert _text(host, i, 3) == EP.sam(r, al, c["mapq"])
-    host.nphh_ea_tsv_all.restype = C.c_longlong
     buf = C.create_string_buffer(1 << 22)
     assert host.nphh_ea_tsv_all(buf, C.c_size_t(1 << 22)) >= 0, host.nphh_last_error()
     assert buf.value.decode() == "".join(golden[f"tsv_{c['read_idx']}"] for c in cs)           # tsv_batch: all reads, in parallel
@@ -179,13 +145,13 @@ def _check_outputs(host, cases, restated, golden):
 def test_host_chaining_logic_on_cpu(host, cases, restated, golden, port_oracle):
     """EventAligner's cursors, fed with the plain-C Viterbi's paths (no device involved)."""
     model, rs, cs = cases
-    _setup(host, cases)
+    EC.load_batch(host, cases)
     jobs = np.zeros(len(cs), synth.HMM_JOB_DT)
     ranks = np.zeros(len(cs) * 400, np.uint32)
     n_ranks = C.c_uint64()
     rounds = 0
     while True:
-        n = host.nphh_ea_next_round(_p(jobs), C.c_size_t(jobs.shape[0]), _p(ranks), C.c_size_t(ranks.shape[0]), C.byref(n_ranks))
+        n = host.nphh_ea_next_round(hm.p(jobs), C.c_size_t(jobs.shape[0]), hm.p(ranks), C.c_size_t(ranks.shape[0]), C.byref(n_ranks))
         assert n >= 0, host.nphh_last_error()
         if n == 0:
             break
@@ -196,7 +162,7 @@ def test_host_chaining_logic_on_cpu(host, cases, restated, golden, port_oracle):
             st, status = port_oracle.hmm_align(rs.reads, rs.ev_mean, rs.ev_start_time, [model], ranks, jb)
             paths.append(st); off.append(off[-1] + st.shape[0])
         flat = np.concatenate(paths) if off[-1] else np.zeros(0, synth.ALIGN_STATE_DT)
-        assert host.nphh_ea_consume(C.c_size_t(n), _p(np.array(off, np.uint64)), _p(flat)) == 0, host.nphh_last_error()
+        assert host.nphh_ea_consume(C.c_size_t(n), hm.p(np.array(off, np.uint64)), hm.p(flat)) == 0, host.nphh_last_error()
         rounds += 1
     assert rounds == max(s for _, s in restated)          # launches = the longest read's segment count
     _check_outputs(host, cases, restated, golden)
@@ -205,11 +171,11 @@ def test_host_chaining_logic_on_cpu(host, cases, restated, golden, port_oracle):
 
 _MISSING_SAMPLES = r"""
 import ctypes as C, sys
+sys.path.insert(0, sys.argv[1])
 import numpy as np
-host = C.CDLL(sys.argv[1])
-host.nphh_last_error.restype = C.c_char_p
-host.nphh_ea_tsv_all.restype = host.nphh_ea_tsv_all_samples.restype = C.c_longlong
-p = lambda a: a.ctypes.data_as(C.c_void_p)
+from tests import host_mirror as hm
+host = hm.load()
+p = hm.p
 mean, sd = np.linspace(60.0, 120.0, 1024), np.full(1024, 2.0)
 mh = host.nphh_model_create(b"nucleotide", 5, 1024, p(mean), p(sd), None)
 ev, t = np.full(50, 90.0, np.float32), np.arange(50, dtype=np.float64) / 1000.0
@@ -233,34 +199,11 @@ def test_tsv_batch_reports_a_read_without_samples():
     parallel loop, and the batch must return an error status instead of terminating the process (run in a child)."""
     import subprocess
     import sys
-    from tests.test_host_mirror import HOST_SO
-    r = subprocess.run([sys.executable, "-c", _MISSING_SAMPLES, HOST_SO], capture_output=True, text=True, timeout=120)
+    r = subprocess.run([sys.executable, "-c", _MISSING_SAMPLES, hm.ROOT], capture_output=True, text=True, timeout=120)
     assert r.returncode == 0, r.stderr
     plain, with_samples, err = r.stdout.splitlines()
     assert int(plain) == 0                                 # without the sample columns both reads format (unmapped: no rows)
     assert int(with_samples) < 0 and "--samples" in err
-
-
-def _drive_rounds(host, cs, rs, model, port_oracle):
-    """pull every round's jobs out of the C++ cursors and feed back the plain-C Viterbi's paths"""
-    jobs = np.zeros(max(len(cs), 1), synth.HMM_JOB_DT)
-    ranks = np.zeros(len(cs) * 400 + 400, np.uint32)
-    n_ranks = C.c_uint64()
-    rounds = 0
-    while True:
-        n = host.nphh_ea_next_round(_p(jobs), C.c_size_t(jobs.shape[0]), _p(ranks), C.c_size_t(ranks.shape[0]), C.byref(n_ranks))
-        assert n >= 0, host.nphh_last_error()
-        if n == 0:
-            return rounds
-        paths, off = [], [0]
-        for j in range(n):
-            jb = jobs[j].copy()
-            jb["read"] = EC.read_slot(cs[int(jb["read"])], rs.n_reads)
-            st, _ = port_oracle.hmm_align(rs.reads, rs.ev_mean, rs.ev_start_time, [model], ranks, jb)
-            paths.append(st); off.append(off[-1] + st.shape[0])
-        flat = np.concatenate(paths) if off[-1] else np.zeros(0, synth.ALIGN_STATE_DT)
-        assert host.nphh_ea_consume(C.c_size_t(n), _p(np.array(off, np.uint64)), _p(flat)) == 0, host.nphh_last_error()
-        rounds += 1
 
 
 def test_eventalign_edge_cases_against_compiled_reference(host, cases, ref_oracle, port_oracle):
@@ -273,8 +216,8 @@ def test_eventalign_edge_cases_against_compiled_reference(host, cases, ref_oracl
     for batch in (variants[:4], variants[4:]):
         for i, v in enumerate(batch):
             v["read_idx"] = i
-        _setup(host, (model, rs, batch))
-        _drive_rounds(host, batch, rs, model, port_oracle)
+        EC.load_batch(host, (model, rs, batch))
+        EC.drive_rounds(host, batch, rs, model, port_oracle)
         ref_oracle.clear_reads()
         mh = ref_oracle.builtin_model("nucleotide")
         rh = ref_oracle.register_reads(rs.reads, rs.ev_mean, rs.ev_start_time, mh)
@@ -299,7 +242,7 @@ def test_eventalign_edge_cases_on_device(host, cases, port_oracle):
     for batch in (variants[:4], variants[4:]):
         for i, v in enumerate(batch):
             v["read_idx"] = i
-        _setup(host, (model, rs, batch))
+        EC.load_batch(host, (model, rs, batch))
         assert host.nphh_ea_run(C.c_double(1.0)) >= 0, host.nphh_last_error()
         for v in batch:
             slot, r = EC.read_slot(v, rs.n_reads), v["read"]
@@ -332,13 +275,11 @@ def _edge_variants(base):
 def test_format_fixed_matches_printf(host):
     """The TSV writer's %.2lf / %.3lf / %.5lf replacement (exact integer arithmetic on the float) against snprintf on
     6 x 600k values: uniform bit patterns, dyadic fractions, decimal ties and their neighbours, inf/nan, +-0."""
-    host.nphh_format_fixed_check.restype = C.c_longlong
     assert host.nphh_format_fixed_check(C.c_uint64(20240923), C.c_size_t(600_000)) == 0, host.nphh_last_error()
 
 
 def test_rolling_kmer_ranks(host):
     """the rank tables EventAligner::run hands the chain kernel (one rolling pass per reference) == Alphabet::kmer_rank"""
-    host.nphh_rolling_ranks_check.restype = C.c_longlong
     rng = np.random.default_rng(4)
     dna = "".join("ACGT"[c] for c in rng.integers(0, 4, 3000))
     cpg = "".join("ACGMT"[c] for c in rng.integers(0, 5, 3000))
@@ -354,21 +295,21 @@ def test_get_aligned_segments(host):
     want = EP.get_aligned_segments(1000, cigar)
     pairs = np.zeros((64, 2), np.int32)
     seg_off = np.zeros(8, np.uint64)
-    n = host.nphh_aligned_segments(1000, _p(cigar), int(cigar.shape[0]), _p(pairs), C.c_size_t(64), _p(seg_off), C.c_size_t(8))
+    n = host.nphh_aligned_segments(1000, hm.p(cigar), int(cigar.shape[0]), hm.p(pairs), C.c_size_t(64), hm.p(seg_off), C.c_size_t(8))
     assert n == len(want) == 2
     for s in range(n):
         got = [tuple(int(v) for v in p) for p in pairs[int(seg_off[s]):int(seg_off[s + 1])]]
         assert got == want[s]
     assert want[0][0] == (1000, 5) and want[1][0] == (1000 + 10 + 3 + 4 + 7, 5 + 10 + 2 + 4)
     bad = EP.pack_cigar([(3, "P")])
-    assert host.nphh_aligned_segments(0, _p(bad), 1, _p(pairs), C.c_size_t(64), _p(seg_off), C.c_size_t(8)) < 0     # the reference asserts
+    assert host.nphh_aligned_segments(0, hm.p(bad), 1, hm.p(pairs), C.c_size_t(64), hm.p(seg_off), C.c_size_t(8)) < 0     # the reference asserts
 
 
 @pytest.mark.gpu
 def test_eventalign_on_device(host, cases, restated, golden):
     """The whole thing on the device: every (read, BAM segment) chain walked start to end by one warp of
     eventalign_chain_kernel in ONE launch; text identical to the reference's."""
-    _setup(host, cases)
+    EC.load_batch(host, cases)
     batches = host.nphh_ea_run(C.c_double(1.0))
     assert batches == 1, host.nphh_last_error()            # no window needed the host-driven fallback
     _check_outputs(host, cases, restated, golden)
@@ -378,7 +319,7 @@ def test_eventalign_on_device(host, cases, restated, golden):
 @pytest.mark.gpu
 def test_eventalign_host_rounds_on_device(host, cases, restated, golden):
     """The host-driven form: one hmm_viterbi_kernel launch per round over the next window of every unfinished read."""
-    _setup(host, cases)
+    EC.load_batch(host, cases)
     rounds = host.nphh_ea_run_rounds(C.c_double(1.0))
     assert rounds >= 0, host.nphh_last_error()
     assert rounds == max(s for _, s in restated)
@@ -390,7 +331,7 @@ def test_eventalign_host_rounds_on_device(host, cases, restated, golden):
 def test_eventalign_chain_falls_back_for_large_windows(host, cases, restated, golden):
     """A window with more events than the chain kernel's scratch holds flags its read; EventAligner re-runs those reads
     through the round driver and the output does not change."""
-    _setup(host, cases)
+    EC.load_batch(host, cases)
     os.environ["NPH_EA_EVENT_CAP"] = "150"                  # most windows span ~170 events
     try:
         batches = host.nphh_ea_run(C.c_double(1.0))

@@ -13,11 +13,11 @@ import ctypes as C
 import numpy as np
 import pytest
 
+from tests import host_mirror as hm
 from tests import hp_cases as hc
 from tests import hp_restatement as hr
 from tests.ref_calls import case_fixture
 from tests.ref_variants import RefVariants
-from tests.test_host_mirror import HOST_SO
 
 ref_hp = case_fixture("ref_fix_homopolymers.pkl.xz", ref=lambda: RefVariants() if RefVariants.available() else None)
 
@@ -84,7 +84,7 @@ def _assert_edges_reached(name, c, vectors):
 def test_call_rule_edges():
     """the mirror's call rule (nph::homopolymer_call) against the restatement's on crafted vectors: quality exactly 10 and one ulp
     below, NaN scores, nothing above -inf (call npos), +inf, and ties (the first length wins)"""
-    host = C.CDLL(HOST_SO)
+    host = hm.load()
     below = float(np.nextafter(10.0, 0.0))
     nan, inf = float("nan"), float("inf")
     cases = [
@@ -101,8 +101,7 @@ def test_call_rule_edges():
     for hp, e, d in cases:
         call, q, sd = C.c_uint64(), C.c_double(), C.c_int()
         ea, da = np.array(e, np.float64), np.array(d, np.float64)
-        kept = host.nphh_homopolymer_call(ea.ctypes.data_as(C.c_void_p), da.ctypes.data_as(C.c_void_p), C.c_uint32(hp), C.byref(call),
-                                          C.byref(q), C.byref(sd))
+        kept = host.nphh_homopolymer_call(hm.p(ea), hm.p(da), C.c_uint32(hp), C.byref(call), C.byref(q), C.byref(sd))
         w_call, w_q, w_sd, w_kept = hr.call_rule(hp, e, d)
         assert (call.value, sd.value, bool(kept)) == (w_call, w_sd, w_kept), (hp, e, d)
         assert np.float64(q.value).tobytes() == np.float64(w_q).tobytes() or (q.value != q.value and w_q != w_q)
@@ -138,7 +137,7 @@ def _range_cases():
 
 
 def test_mirror_haplotype_ranges_equal_reference(ref_hp):
-    host = C.CDLL(HOST_SO)
+    host = hm.load()
     cases = _range_cases()
     assert len(cases) > 150
     fps = [repr(x[:6]) for x in cases]

@@ -4,8 +4,6 @@ reference's (restated over its own HMMs, tests/test_all_support_oracle.py, recor
 host mirror's nph::annotate_variants_with_all_support (nanopolish_b200/host/nph_variants.cpp) writes the reference's INFO byte for
 byte.  Also: a large random batch against the restatement over nph_hmm_score_batch's scores; an empty variant list and an empty
 pile-up; every refusal, by its message."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
@@ -13,20 +11,16 @@ from nanopolish_b200 import synth
 from nanopolish_b200._lib import NphError
 from nanopolish_b200.engine import Engine
 from oracle.oracle_py import PortOracle
+from tests import host_mirror as hm
 from tests import support_cases as sc
 from tests import support_restatement as sr
 from tests.ref_calls import case_answers
-from tests.test_host_mirror import HOST_SO
 
 pytestmark = pytest.mark.gpu
 GOLDEN = "ref_all_support.pkl.xz"
 
 
-@pytest.fixture(scope="module")
-def host():
-    lib = C.CDLL(HOST_SO)
-    lib.nphh_last_error.restype = C.c_char_p
-    return lib
+host = hm.fixture()
 
 
 @pytest.fixture(scope="module")

@@ -4,8 +4,6 @@ position, alleles, quality bits, INFO bytes and genotype, equal the reference's 
 tests/test_call_variants_oracle.py).  Also: two random 20 kb regions at ploidy 1 and 2, and a group of 968 haplotypes at ploidy 2,
 against the restatement (tests/call_restatement.py, its genotype search a numpy brute force) over nph_hmm_score_batch's scores; the
 device call's counters; an empty candidate list, an empty pile-up, and every refusal by its message."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
@@ -14,20 +12,15 @@ from nanopolish_b200._lib import NphError
 from nanopolish_b200.engine import Engine
 from tests import call_cases as cc
 from tests import call_restatement as cr
+from tests import host_mirror as hm
 from tests import screen_cases as sc
 from tests.ref_calls import case_answers
-from tests.test_host_mirror import HOST_SO
-from tests.test_variants_methylation_oracle import type_models
 
 pytestmark = pytest.mark.gpu
 GOLDEN = "ref_call_haplotype.pkl.xz"
 
 
-@pytest.fixture(scope="module")
-def host():
-    lib = C.CDLL(HOST_SO)
-    lib.nphh_last_error.restype = C.c_char_p
-    return lib
+host = hm.fixture()
 
 
 @pytest.fixture(scope="module")
@@ -35,7 +28,7 @@ def eng():
     e = Engine(0)
     e.model_upload(synth.load_model("nucleotide"))                       # model 0
     for t in sc.ALL_TYPES:                                               # models 1, 2, 3
-        e.model_upload(type_models([t])[t])
+        e.model_upload(sc.type_models([t])[t])
     yield e
     e.close()
 

@@ -18,7 +18,7 @@ from nanopolish_b200._lib import NphError
 from nanopolish_b200.engine import Engine
 from oracle import eventalign_py as EP
 from tests import eventalign_cases as EC
-from tests.test_host_mirror import HOST_SO, _register, _register_reads
+from tests import host_mirror as hm
 
 pytestmark = pytest.mark.gpu
 
@@ -27,15 +27,7 @@ GOLD = os.path.join(ROOT, "tests", "golden", "eventalign_golden.npz")
 NPH_ERR_INVALID, NPH_ERR_STATE = -3, -5
 NAMES, SCALE, INDEX, SAMPLES = 1, 2, 4, 8            # the switches of nphh_ea_run_tsv / nphh_ea_tsv_all_opt
 RATE = 4000.0
-
-
-@pytest.fixture(scope="module")
-def host():
-    lib = C.CDLL(HOST_SO)
-    lib.nphh_last_error.restype = C.c_char_p
-    for f in ("nphh_ea_run", "nphh_ea_run_tsv", "nphh_ea_tsv_all_opt", "nphh_ea_text", "nphh_ea_num_segments"):
-        getattr(lib, f).restype = C.c_longlong
-    return lib
+host = hm.fixture()
 
 
 @pytest.fixture(scope="module")
@@ -56,38 +48,10 @@ def restated(cases, port_oracle):
                                  EC.port_align_fn(port_oracle, rs, model, EC.read_slot(c, rs.n_reads)), *c["region"]) for c in cs]
 
 
-def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
-
-
-def _raw_samples(slot):
-    """the trimmed raw samples SRF_LOAD_RAW_SAMPLES keeps, as tests/test_eventalign.py stands in for them"""
-    return np.random.default_rng(900 + slot).normal(90.0, 12.0, 420_000).astype(np.float32)
-
-
-def _setup(host, cases, samples_of=_raw_samples):
-    model, rs, cs = cases
-    host.nphh_clear()
-    mh = _register(host, model)
-    rh = _register_reads(host, rs, mh)
-    host.nphh_ea_begin()
-    for c in cs:
-        slot, r = EC.read_slot(c, rs.n_reads), c["read"]
-        a, b = np.ascontiguousarray(r.b2e_start, np.int32), np.ascontiguousarray(c["b2e_stop"], np.int32)
-        assert host.nphh_read_set_eventalign(rh[slot], r.name.encode(), r.read_sequence.encode(), _p(a), _p(b), C.c_size_t(a.shape[0]),
-                                             _p(np.ascontiguousarray(r.stdv)), _p(np.ascontiguousarray(r.duration))) == 0
-        smp = samples_of(slot)
-        if smp is not None:
-            assert host.nphh_read_set_samples(rh[slot], _p(smp), C.c_size_t(smp.shape[0]), C.c_double(RATE)) == 0
-        idx = host.nphh_ea_add_read(rh[slot], c["contig_name"].encode(), c["ref_pos"], c["flag"], c["mapq"], _p(c["cigar"]),
-                                    int(c["cigar"].shape[0]), c["fetched"].encode(), c["read_idx"], c["region"][0], c["region"][1])
-        assert idx == c["read_idx"], host.nphh_last_error()
-
-
 def _run_tsv(host, n_reads, switches, cap=1 << 25):
     buf = np.zeros(cap, np.uint8)
     read_off, on_host, batches = np.zeros(n_reads + 1, np.uint64), np.zeros(n_reads, np.uint8), C.c_longlong(0)
-    n = host.nphh_ea_run_tsv(C.c_double(1.0), switches, _p(buf), C.c_size_t(cap), _p(read_off), _p(on_host), C.byref(batches))
+    n = host.nphh_ea_run_tsv(C.c_double(1.0), switches, hm.p(buf), C.c_size_t(cap), hm.p(read_off), hm.p(on_host), C.byref(batches))
     assert n >= 0, host.nphh_last_error()
     return buf[:n].tobytes().decode(), read_off, on_host, batches.value
 
@@ -96,7 +60,7 @@ def _host_rows(host, n_reads, switches, cap=1 << 25):
     """run() + tsv_batch: the host writer's bytes and per-read offsets"""
     assert host.nphh_ea_run(C.c_double(1.0)) >= 0, host.nphh_last_error()
     buf, read_off = np.zeros(cap, np.uint8), np.zeros(n_reads + 1, np.uint64)
-    n = host.nphh_ea_tsv_all_opt(switches, _p(buf), C.c_size_t(cap), _p(read_off))
+    n = host.nphh_ea_tsv_all_opt(switches, hm.p(buf), C.c_size_t(cap), hm.p(read_off))
     assert n >= 0, host.nphh_last_error()
     return buf[:n].tobytes().decode(), read_off
 
@@ -104,7 +68,7 @@ def _host_rows(host, n_reads, switches, cap=1 << 25):
 def _restated_rows(cases, restated, switches):
     model, rs, cs = cases
     return [EP.tsv(c["read"], al, print_read_names=bool(switches & NAMES), scale_events=bool(switches & SCALE),
-                   samples=_raw_samples(EC.read_slot(c, rs.n_reads)) if switches & SAMPLES else None, sample_rate=RATE)
+                   samples=EC.raw_samples(EC.read_slot(c, rs.n_reads)) if switches & SAMPLES else None, sample_rate=RATE)
             for c, al in zip(cs, restated)]
 
 
@@ -113,7 +77,7 @@ def test_device_rows_are_the_reference_rows(host, cases, restated, golden, switc
     """Forward, reverse-strand, two-segment, windowed and unmapped records over a soft-masked reference with an ambiguity code:
     the device's bytes are the restated reference's, the golden file's, and tsv_batch's."""
     model, rs, cs = cases
-    _setup(host, cases)
+    EC.load_batch(host, cases)
     got, read_off, on_host, batches = _run_tsv(host, len(cs), switches)
     assert batches == 1 and not on_host.any()                    # every row came from the device
     if switches & (INDEX | SAMPLES) in (0, INDEX | SAMPLES):     # the restatement writes the two sample columns together
@@ -125,7 +89,7 @@ def test_device_rows_are_the_reference_rows(host, cases, restated, golden, switc
         assert len(got) > 400_000
     # the records are fetched when something asks for them: the host writer then reproduces the device's bytes
     assert host.nphh_ea_num_segments(0) > 0
-    _setup(host, cases)
+    EC.load_batch(host, cases)
     rows, host_off = _host_rows(host, len(cs), switches)
     assert got == rows and np.array_equal(read_off, host_off)
     host.nphh_ea_begin()
@@ -140,7 +104,7 @@ def test_formatter_checks_on_device():
 
 def test_large_windows_take_the_round_driver(host, cases, golden):
     model, rs, cs = cases
-    _setup(host, cases)
+    EC.load_batch(host, cases)
     os.environ["NPH_EA_EVENT_CAP"] = "150"                       # most windows span ~170 events
     try:
         got, read_off, on_host, batches = _run_tsv(host, len(cs), 0)
@@ -159,13 +123,13 @@ def test_a_read_with_a_non_finite_stdv_takes_the_host_writer(host, cases, golden
     stdv[100::200] = np.inf
     bad[1]["read"] = dataclasses.replace(cs[1]["read"], stdv=stdv)
     bad[5]["read"] = bad[1]["read"]                              # the windowed record is built on the same read
-    _setup(host, (model, rs, bad))
+    EC.load_batch(host, (model, rs, bad))
     got, read_off, on_host, batches = _run_tsv(host, len(cs), 0)
     assert [int(v) for v in on_host] == [0, 1, 0, 0, 0, 1] and batches == 1
     for i in (0, 2, 3):                                           # the other reads are the device's, unchanged
         assert got[int(read_off[i]):int(read_off[i + 1])] == golden[f"tsv_{i}"]
     assert "\tinf\t" in got[int(read_off[1]):int(read_off[2])]
-    _setup(host, (model, rs, bad))
+    EC.load_batch(host, (model, rs, bad))
     rows, host_off = _host_rows(host, len(cs), 0)
     assert got == rows and np.array_equal(read_off, host_off)
     host.nphh_ea_begin()
@@ -173,9 +137,9 @@ def test_a_read_with_a_non_finite_stdv_takes_the_host_writer(host, cases, golden
 
 def test_run_tsv_reports_a_read_without_samples(host, cases):
     """what tsv_batch raises for such a batch (test_tsv_batch_reports_a_read_without_samples), before anything is launched"""
-    _setup(host, cases, samples_of=lambda slot: None if slot == 2 else _raw_samples(slot))
+    EC.load_batch(host, cases, samples_of=lambda slot: None if slot == 2 else EC.raw_samples(slot))
     buf = np.zeros(1 << 20, np.uint8)
-    assert host.nphh_ea_run_tsv(C.c_double(1.0), SAMPLES, _p(buf), C.c_size_t(buf.shape[0]), None, None, None) < 0
+    assert host.nphh_ea_run_tsv(C.c_double(1.0), SAMPLES, hm.p(buf), C.c_size_t(buf.shape[0]), None, None, None) < 0
     assert "--samples" in host.nphh_last_error().decode()
     host.nphh_ea_begin()
 
@@ -258,7 +222,7 @@ def test_a_batch_of_a_few_thousand_reads(host):
     rs = synth.gen_reads(3000, 400, model, seed=33, drift=True)
     rng = np.random.default_rng(34)
     host.nphh_clear()
-    rh = _register_reads(host, rs, _register(host, model))
+    rh = hm.register_reads(host, rs, hm.register_model(host, model))
     one_sample = np.zeros(1, np.float32)
 
     def queue():
@@ -267,7 +231,7 @@ def test_a_batch_of_a_few_thousand_reads(host):
             seq = synth._CODE2DNA[rs.seq_codes[i]].tobytes()
             nk = len(seq) - model.k + 1
             cigar = EP.pack_cigar([(len(seq), "M")])
-            assert host.nphh_ea_add_read(rh[i], b"chr_synth", 1000 + i, 0, 60, _p(cigar), 1, seq, i, -1, -1) == i, host.nphh_last_error()
+            assert host.nphh_ea_add_read(rh[i], b"chr_synth", 1000 + i, 0, 60, hm.p(cigar), 1, seq, i, -1, -1) == i, host.nphh_last_error()
 
     for i in range(rs.n_reads):
         seq = synth._CODE2DNA[rs.seq_codes[i]].tobytes()
@@ -276,8 +240,8 @@ def test_a_batch_of_a_few_thousand_reads(host):
         E = int(rs.reads[i]["n_events"])
         stdv, dur = rng.uniform(0.5, 3.0, E).astype(np.float32), np.full(E, 0.002, np.float32)
         a, b = np.ascontiguousarray(start, np.int32), np.ascontiguousarray(stop, np.int32)
-        assert host.nphh_read_set_eventalign(rh[i], f"read_{i}".encode(), seq, _p(a), _p(b), C.c_size_t(nk), _p(stdv), _p(dur)) == 0
-        assert host.nphh_read_set_samples(rh[i], _p(one_sample), C.c_size_t(1), C.c_double(RATE)) == 0     # --signal-index reads no sample
+        assert host.nphh_read_set_eventalign(rh[i], f"read_{i}".encode(), seq, hm.p(a), hm.p(b), C.c_size_t(nk), hm.p(stdv), hm.p(dur)) == 0
+        assert host.nphh_read_set_samples(rh[i], hm.p(one_sample), C.c_size_t(1), C.c_double(RATE)) == 0     # --signal-index reads no sample
     for switches in (0, NAMES | SCALE | INDEX):
         queue()
         got, read_off, on_host, batches = _run_tsv(host, rs.n_reads, switches, cap=1 << 28)

@@ -5,15 +5,9 @@ import numpy as np
 import pytest
 
 from nanopolish_b200 import synth
+from tests import events_cases as ec
 
 pytestmark = pytest.mark.gpu
-
-
-def _same(got, want):
-    assert got.shape[0] == want.shape[0]
-    assert np.array_equal(got["start"], want["start"])
-    for f in ("length", "mean", "stdv"):
-        assert np.array_equal(got[f].view(np.uint32), want[f].view(np.uint32)), f
 
 
 @pytest.mark.parametrize("rna,n_samples,n_reads", [(False, 36000, 40), (True, 50000, 12), (False, 700, 150)])
@@ -24,7 +18,7 @@ def test_events_identical(engine, port_oracle, rna, n_samples, n_reads):
     got = engine.detect_events_batch(raw, reads, prm)
     for r, g in zip(reads, got):
         x = np.ascontiguousarray(raw[int(r["sample_off"]):int(r["sample_off"]) + int(r["n_samples"])])
-        _same(g, port_oracle.detect_events(x, prm))
+        ec.same(g, port_oracle.detect_events(x, prm))
     assert sum(g.shape[0] for g in got) > n_reads * n_samples / (60 if rna else 25)
 
 
@@ -41,7 +35,7 @@ def test_ragged_and_degenerate(engine, port_oracle):
     got = engine.detect_events_batch(raw, reads, prm)
     for r, g in zip(reads, got):
         x = np.ascontiguousarray(raw[int(r["sample_off"]):int(r["sample_off"]) + int(r["n_samples"])])
-        _same(g, port_oracle.detect_events(x, prm))
+        ec.same(g, port_oracle.detect_events(x, prm))
     # constant signal: no peak, one event covering the read
     flat = np.full(500, 80.0, np.float32)
     rd = np.zeros(1, synth.RAW_READ_DT); rd[0] = (0, 0, 500, 16)
@@ -78,7 +72,7 @@ def test_every_walk_of_the_detector_is_exact(engine, port_oracle, monkeypatch, e
         got = engine.detect_events_batch(raw, reads, prm)
         for r, g in zip(reads, got):
             x = np.ascontiguousarray(raw[int(r["sample_off"]):int(r["sample_off"]) + int(r["n_samples"])])
-            _same(g, port_oracle.detect_events(x, prm))
+            ec.same(g, port_oracle.detect_events(x, prm))
 
 
 def test_samples_the_guard_refuses_take_the_streaming_kernel(engine, port_oracle):
@@ -98,4 +92,4 @@ def test_samples_the_guard_refuses_take_the_streaming_kernel(engine, port_oracle
     got = engine.detect_events_batch(raw, reads, prm)
     for r, g in zip(reads, got):
         x = np.ascontiguousarray(raw[int(r["sample_off"]):int(r["sample_off"]) + int(r["n_samples"])])
-        _same(g, port_oracle.detect_events(x, prm))
+        ec.same(g, port_oracle.detect_events(x, prm))

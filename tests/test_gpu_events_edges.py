@@ -12,7 +12,6 @@ import torch
 
 from nanopolish_b200 import synth
 from tests import events_cases as ec
-from tests.test_gpu_events import _same
 
 pytestmark = pytest.mark.gpu
 NPH_ERR_UNSUPPORTED = -6
@@ -50,7 +49,7 @@ def test_edge_reads_bit_exact_on_the_predicted_path(engine, port_oracle, edges, 
         got, stats = _run(engine, capfd, monkeypatch, raw, rr, prm, env)
         for r, g in zip(reads, got):
             try:
-                _same(g, port_oracle.detect_events(r.x, prm))
+                ec.same(g, port_oracle.detect_events(r.x, prm))
             except AssertionError as ex:
                 raise AssertionError(f"{r.name} under {pname}: {ex}") from ex
         assert stats == ec.batch_stats(preds, reads, pname, config), f"{pname}: (repair walks, fallback, guard/slice)"
@@ -73,7 +72,7 @@ def test_warps_per_read_heuristic(engine, port_oracle, capfd, monkeypatch, want)
     got, stats = _run(engine, capfd, monkeypatch, raw, rr, prm, {})
     want_rep = 0
     for r, g in zip(reads, got):
-        _same(g, port_oracle.detect_events(r.x, prm))
+        ec.same(g, port_oracle.detect_events(r.x, prm))
         pr = ec.predict(ec.Trace(port_oracle, r.x, prm), 32 * want, ec.FUSED_WARM, ec.room(r.x.shape[0]))
         assert pr.path == "fast"
         want_rep += pr.repairs
@@ -96,7 +95,7 @@ def test_capacity(engine, port_oracle, capfd, monkeypatch, wpr):
     rd = np.zeros(1, synth.RAW_READ_DT)
     rd[0] = (0, 0, 6000, ne)
     got, stats = _run(engine, capfd, monkeypatch, x, rd, prm, {"NPH_EVENTS_WPR": wpr})
-    _same(got[0], want)
+    ec.same(got[0], want)
     pr = ec.predict(ec.Trace(port_oracle, x, prm), 32 * int(wpr), ec.FUSED_WARM, ne)
     assert stats == (pr.repairs, int(pr.path != "fast"), int(pr.path != "fast"))
     rd[0] = (0, 0, 6000, ne - 1)
@@ -109,7 +108,7 @@ def test_capacity(engine, port_oracle, capfd, monkeypatch, wpr):
     assert 1 < ne < 32
     rd[0] = (0, 0, 100, ne)
     got, stats = _run(engine, capfd, monkeypatch, x, rd, prm, {"NPH_EVENTS_WPR": wpr})
-    _same(got[0], want)
+    ec.same(got[0], want)
     assert stats[1:] == (1, 1)
     rd[0] = (0, 0, 100, ne - 1)
     with pytest.raises(NphError):
@@ -118,7 +117,7 @@ def test_capacity(engine, port_oracle, capfd, monkeypatch, wpr):
     flat = np.full(3000, 77.25, np.float32)
     rd[0] = (0, 0, 3000, 1)
     got, stats = _run(engine, capfd, monkeypatch, flat, rd, prm, {"NPH_EVENTS_WPR": wpr})
-    _same(got[0], port_oracle.detect_events(flat, prm))
+    ec.same(got[0], port_oracle.detect_events(flat, prm))
     assert got[0].shape[0] == 1 and stats[1] == 0
 
 
@@ -145,5 +144,5 @@ def test_adc_quantised_traces_take_the_fast_path(engine, port_oracle, capfd, mon
         assert g.exact and r.x.min() >= 40 and r.x.max() <= 250
     got, stats = _run(engine, capfd, monkeypatch, raw, rr, prm, {})
     for r, g in zip(reads, got):
-        _same(g, port_oracle.detect_events(r.x, prm))
+        ec.same(g, port_oracle.detect_events(r.x, prm))
     assert stats[1:] == (0, 0)

@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 
 from nanopolish_b200 import synth
-from tests.test_gpu_events import _same
+from tests import events_cases as ec
 
 pytestmark = pytest.mark.gpu
 
@@ -35,7 +35,7 @@ def _detect_on_fallback(engine, capfd, raw, reads, prm):
 def _check(got, raw, reads, prm, port_oracle):
     for r, g in zip(reads, got):
         x = np.ascontiguousarray(raw[int(r["sample_off"]):int(r["sample_off"]) + int(r["n_samples"])])
-        _same(g, port_oracle.detect_events(x, prm))
+        ec.same(g, port_oracle.detect_events(x, prm))
 
 
 def _params(w1, w2, t1, t2, ph):

@@ -5,28 +5,22 @@ applied to them gives the reference's fixed haplotype, variant for variant; so d
 (nanopolish_b200/host/nph_variants.cpp) through its C shim.  Both insertions and deletions are called, and on the long-run pile-up
 the duration term makes calls the event term alone would not.  Also: a batch cut into many chunks of Viterbi states gives the same
 bits as one chunk; an empty pile-up and a haplotype without homopolymers; every refusal."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
 from nanopolish_b200 import synth
 from nanopolish_b200._lib import NphError
 from nanopolish_b200.engine import Engine
+from tests import host_mirror as hm
 from tests import hp_cases as hc
 from tests import hp_restatement as hr
 from tests.ref_calls import case_answers
-from tests.test_host_mirror import HOST_SO
 
 pytestmark = pytest.mark.gpu
 GOLDEN = "ref_fix_homopolymers.pkl.xz"
 
 
-@pytest.fixture(scope="module")
-def host():
-    lib = C.CDLL(HOST_SO)
-    lib.nphh_last_error.restype = C.c_char_p
-    return lib
+host = hm.fixture()
 
 
 @pytest.fixture(scope="module")

@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 
 from nanopolish_b200 import synth
+from tests import meth_cases as mc
 from tests import meth_restatement as mr
 
 pytestmark = pytest.mark.gpu
@@ -137,7 +138,7 @@ def test_record_counts_around_the_scan_block(eng2, port_oracle, n_records, compa
         site_off[1:] = np.cumsum(np.bincount(sites["record"], minlength=n_records))
         names = ["r%d" % i for i in range(n_records)]
         is_rev = (np.arange(n_records) % 2).astype(np.uint8)
-        assert eng2.methylation_tsv("chr20", names, is_rev).decode() == _expected_rows(sites, site_off, recs, ref, names, is_rev, "chr20", K)
+        assert eng2.methylation_tsv("chr20", names, is_rev).decode() == mc.expected_rows(sites, site_off, recs, ref, names, is_rev, "chr20", K)
 
 
 def test_staged_form_matches_one_shot(eng2):
@@ -190,7 +191,6 @@ def test_invalid_inputs(eng2):
 def test_device_equals_compiled_reference(eng2, ref_oracle):
     """nph_methylation_batch against the compiled reference's own calculate_methylation_for_read + TSV writer (oracle/_ref,
     which travels to the GPU box): records built the way BAM / FASTA / SquiggleRead present them (tests/meth_cases.py)."""
-    from tests import meth_cases as mc
     nuc = synth.load_model("nucleotide")
     rs = synth.gen_reads(9, 2200, nuc, seed=4242, cpg_keep=0.35)
     ref_oracle.clear_reads()
@@ -252,7 +252,6 @@ def test_compact_event_alignment_form(eng2, ref_oracle):
     off2, s2 = eng2.methylation_fetch()
     assert np.array_equal(a[0], off2) and a[1].tobytes() == s2.tobytes()
     # records with indels
-    from tests import meth_cases as mc
     nuc = synth.load_model("nucleotide")
     rs = synth.gen_reads(6, 2200, nuc, seed=77, cpg_keep=0.35)
     rng = np.random.default_rng(3)
@@ -275,23 +274,6 @@ def test_compact_event_alignment_form(eng2, ref_oracle):
     assert np.array_equal(a[0], b[0]) and a[1].tobytes() == b[1].tobytes() and a[1].shape[0] > 100
 
 
-def _expected_rows(sites, site_off, recs, ref, names, is_rev, contig, k):
-    """the reference's writer (src/nanopolish_call_methylation.cpp:113-140) over site records, formatted by Python's correctly
-    rounded %.2f — the C library's %.2lf"""
-    out = []
-    for r in range(recs.shape[0]):
-        R = recs[r]
-        seg = ref[int(R["ref_off"]):int(R["ref_off"]) + int(R["ref_len"])].tobytes().decode()
-        for s in sites[int(site_off[r]):int(site_off[r + 1])]:
-            ll_m, ll_u = float(s["ll_methylated"]) + 0.0, float(s["ll_unmethylated"]) + 0.0
-            b = int(s["start_position"]) - int(R["ref_start_pos"]) - k + 1
-            e = min(int(s["end_position"]) - int(R["ref_start_pos"]) + k, int(R["ref_len"]))
-            out.append("%s\t%s\t%d\t%d\t%s\t%.2f\t%.2f\t%.2f\t%d\t%d\t%s\n" % (
-                contig, "-" if is_rev[r] else "+", int(s["start_position"]), int(s["end_position"]), names[r], ll_m - ll_u, ll_m, ll_u, 1,
-                int(s["n_motif"]), seg[b:e]))
-    return "".join(out)
-
-
 def test_tsv_rows_formatted_on_the_device(eng2):
     """nph_methylation_tsv: every field of every row, against Python's formatting of the same site records (forward and reverse records,
     a record without sites, a window clipped by the end of the record's reference, read names of different lengths)."""
@@ -307,7 +289,7 @@ def test_tsv_rows_formatted_on_the_device(eng2):
     names = ["r%d_%s" % (i, "x" * (i % 7)) for i in range(recs.shape[0])]
     is_rev = (np.arange(recs.shape[0]) % 2).astype(np.uint8)
     got = eng2.methylation_tsv("chr20", names, is_rev).decode()
-    want = _expected_rows(sites, site_off, recs, ref, names, is_rev, "chr20", K)
+    want = mc.expected_rows(sites, site_off, recs, ref, names, is_rev, "chr20", K)
     assert want.count("\n") == sites.shape[0] > 150
     assert got == want
     # a destination that is too small reports the size needed

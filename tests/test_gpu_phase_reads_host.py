@@ -3,24 +3,17 @@ call): its SAM records, byte for byte, against the compiled reference's own phas
 that library is built, and against the restatement (tests/phase_restatement.py) always — every record-level rule (no record when no
 variant lies at or after the read, a record of the plain reference when the range is empty), last-variant-wins, the SEQ round trip
 through the 4-bit codes, and one line against a literal string."""
-import ctypes as C
 import os
 
 import numpy as np
 import pytest
 
 from nanopolish_b200 import synth
+from tests import host_mirror as hm
 from tests import phase_cases as pc
-from tests.test_host_mirror import HOST_SO, _register, _register_reads
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def host():
-    lib = C.CDLL(HOST_SO)
-    lib.nphh_last_error.restype = C.c_char_p
-    return lib
+host = hm.fixture()
 
 
 def test_mirror_sam_equals_reference(host, port_oracle):
@@ -39,8 +32,8 @@ def test_mirror_sam_equals_reference(host, port_oracle):
     var = [v for v in var if v[0] < cl[-2]["ref_pos"]]
     var.append((cl[-3]["ref_pos"] + len(cl[-3]["upper"]) + 2, "A", "C"))                       # read -3: an empty range, not at the end
     var = [v for v in var if not (cl[-3]["ref_pos"] <= v[0] < cl[-3]["ref_pos"] + len(cl[-3]["upper"]))]
-    mh = _register(host, model)
-    rh = _register_reads(host, rs, mh)
+    mh = hm.register_model(host, model)
+    rh = hm.register_reads(host, rs, mh)
     got = pc.mirror_sam(host, rh, cl, var)
     want = [pc.restated(port_oracle, rs, model, i, c, var) for i, c in enumerate(cl)]
     assert want[-1] is None and want[-2] is None and set(want[-3].split("\t")[10].strip()) == {"?"}
@@ -56,8 +49,8 @@ def test_mirror_sam_equals_reference(host, port_oracle):
 def test_mirror_literal_line(host):
     model = synth.load_model("nucleotide")
     rs = synth.gen_reads(1, 400, model, seed=1)
-    mh = _register(host, model)
-    rh = _register_reads(host, rs, mh)
+    mh = hm.register_model(host, model)
+    rh = hm.register_reads(host, rs, mh)
     case = dict(name="lit", flag=16, mapq=7, ref_pos=2, upper="ACGTNRYX=acgt0", pairs=[])
     got = pc.mirror_sam(host, rh, [case], [(1000, "A", "C")])
     assert got == "lit\t16\tchr1\t3\t7\t14M\t*\t0\t0\tACGTNRYN=ACGTA\t??????????????\n"

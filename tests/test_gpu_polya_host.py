@@ -4,17 +4,15 @@ last CIGAR operations of every kind, a read missing from the index, a read whose
 or nph_detect_polyi_batch call and comes back as polya_main's or detect_polyi_main's TSV.  The expected rows come from the same
 chain through the oracle (oracle/prep_chain.py) and the reference's own poly(A) or detect-polyi code."""
 import ctypes as C
-import os
 
 import numpy as np
 import pytest
 
 from nanopolish_b200 import synth
+from tests import host_mirror as hm
 from tests import polya_cases as pc
 from tests import polyi_cases as qc
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HOST_SO = os.path.join(ROOT, "nanopolish_b200", "libnph_host.so")
 pytestmark = pytest.mark.gpu
 # (C shim, header line, the reference's class)
 MODES = {
@@ -23,15 +21,7 @@ MODES = {
     "detect_polyi": ("nphh_detect_polyi", "readname\tcontig\tposition\tleader_start\tadapter_start\tpolya_start\ttranscript_start\t"
                      "read_rate\tpolya_length\tdetected\tqc_tag\n", qc.RefPolyi),
 }
-
-
-@pytest.fixture(scope="module")
-def host():
-    lib = C.CDLL(HOST_SO)
-    lib.nphh_last_error.restype = C.c_char_p
-    for shim, _, _ in MODES.values():
-        getattr(lib, shim).restype = C.c_longlong
-    return lib
+host = hm.fixture()
 
 
 def test_polya_after_load_from_raw_like_a_caller(host, port_oracle):
@@ -58,7 +48,7 @@ def _after_load_from_raw_like_a_caller(host, port_oracle, mode):
     rate = 3012.0
     want = oracle_chain(port_oracle, rna, signals, seqs, sample_rate=rate, rna=True)
 
-    p = lambda a: a.ctypes.data_as(C.c_void_p)
+    p = hm.p
     mean5, sd, lsd = (np.ascontiguousarray(a) for a in (rna.level_mean, rna.level_stdv, rna.level_log_stdv))
     mh = host.nphh_model_create(b"u_to_t_rna", 5, 1024, p(mean5), p(sd), p(lsd))
     assert mh >= 0, host.nphh_last_error()

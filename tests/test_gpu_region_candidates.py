@@ -4,8 +4,6 @@ the plain-Python walk of tests/candidate_restatement.py (records entirely before
 INFO bytes included, equals the compiled reference's (recorded in tests/golden/ref_region_candidates.pkl.xz by
 tests/test_region_candidates_oracle.py).  Also: the call's counters, a first output capacity that is too small, every refusal, and
 the sizes of the new ABI structs."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
@@ -13,20 +11,13 @@ from nanopolish_b200 import synth
 from nanopolish_b200._lib import NPH_ERR_INVALID, NphError
 from nanopolish_b200.engine import Engine
 from tests import candidate_cases as cc
+from tests import host_mirror as hm
 from tests.ref_calls import case_answers
-from tests.test_host_mirror import HOST_SO
 
 pytestmark = pytest.mark.gpu
 GOLDEN = "ref_region_candidates.pkl.xz"
 NPH_ERR_UNSUPPORTED = -6
-
-
-@pytest.fixture(scope="module")
-def host():
-    lib = C.CDLL(HOST_SO)
-    lib.nphh_last_error.restype = C.c_char_p
-    lib.nphh_variants_in_region.restype = C.c_longlong
-    return lib
+host = hm.fixture()
 
 
 @pytest.fixture(scope="module")
@@ -57,18 +48,6 @@ def distinct_of(c, out, seq):
     return got
 
 
-def mirror(host, c, counts=None):
-    pp, off = cc.flat_pairs(c)
-    bases = (C.c_char_p * max(len(c["bases"]), 1))(*c["bases"])
-    rc = np.array(c["rc"] or [0], np.uint8)
-    cap = 1 << 26
-    out = C.create_string_buffer(cap)
-    n = host.nphh_variants_in_region(cc.CONTIG.encode(), c["region_start"], c["region_ref"].encode(), len(c["bases"]), bases, rc.ctypes.data_as(C.c_void_p),
-                                     pp.ctypes.data_as(C.c_void_p), off.ctypes.data_as(C.c_void_p), c["start"], c["stop"], C.c_double(c["min_frequency"]),
-                                     c["min_depth"], None if counts is None else counts.ctypes.data_as(C.c_void_p), out, C.c_size_t(cap))
-    return int(n), (cc.parse(out.raw[:n]) if n >= 0 else None)
-
-
 @pytest.mark.parametrize("name", cc.CASES)
 def test_device_equals_restatement(eng, cases, name):
     c = cases[name]
@@ -85,7 +64,7 @@ def test_mirror_equals_reference(host, cases, name):
     c = cases[name]
     want = case_answers(GOLDEN, name)[cc.fingerprint(c)]
     counts = np.zeros(1, synth.CANDIDATE_COUNTS_DT)
-    n, got = mirror(host, c, counts)
+    n, got = cc.mirror(host, c, counts)
     assert n >= 0, host.nphh_last_error()
     assert got == want
     assert int(counts[0]["n_records"]) == len(c["bases"])
@@ -139,14 +118,14 @@ def test_refusals(eng, host):
     c = dict(region_start=1000, region_ref=ref, rc=[0], start=1000, stop=1150, min_frequency=0.0, min_depth=0)
     for ins, status in ((32_766, 0), (32_767, NPH_ERR_UNSUPPORTED)):
         b, a, _ = cc.rec(ref, 1000, 1010, [("M", 30), ("I", "A" * ins), ("M", 30)])
-        n, got = mirror(host, dict(c, bases=[b], aligned=[a]))
+        n, got = cc.mirror(host, dict(c, bases=[b], aligned=[a]))
         assert (n >= 0) if status == 0 else (n == status), host.nphh_last_error()
         if status == 0:
             assert [(g[0], len(g[2])) for g in got] == [(1039, ins + 1)]
     b, a, _ = cc.rec(ref, 1000, 1010, [("M", 30)])
     a = a[[0, 2, 1, 3]]
-    assert mirror(host, dict(c, bases=[b], aligned=[a]))[0] == NPH_ERR_INVALID
-    assert mirror(host, dict(c, bases=[b], aligned=[cc.rec(ref, 1000, 1010, [("M", 30)])[1]], start=1100, stop=1099))[0] == NPH_ERR_INVALID
+    assert cc.mirror(host, dict(c, bases=[b], aligned=[a]))[0] == NPH_ERR_INVALID
+    assert cc.mirror(host, dict(c, bases=[b], aligned=[cc.rec(ref, 1000, 1010, [("M", 30)])[1]], start=1100, stop=1099))[0] == NPH_ERR_INVALID
 
 
 def test_abi_sizes():
@@ -154,32 +133,11 @@ def test_abi_sizes():
     assert synth.SEQ_RECORD_DT.fields["first_read_pos"][1] == 28 and synth.REGION_CANDIDATE_DT.fields["alt_off"][1] == 24
 
 
-def call_region(host, c):
-    """`variants` in its default mode through the nphh_call_region shim (nph::call_variants_for_region + nph::write_variants_vcf)"""
-    from tests.test_host_mirror import _register, _register_reads
-    p = lambda a: a.ctypes.data_as(C.c_void_p)
-    host.nphh_clear()
-    mh = _register(host, synth.load_model("nucleotide"))
-    hs = _register_reads(host, c["rs"], mh)
-    a = cc.call_args(c)
-    read = np.array([hs[int(x)] for x in c["recs"]["read"]], np.int32)
-    cap = 1 << 24
-    out = C.create_string_buffer(cap)
-    host.nphh_call_region.restype = C.c_longlong
-    n = host.nphh_call_region(b"ctg", c["contig_length"], c["start_base"], c["end_base"], c["region_start"], c["region_ref"].encode(),
-                              int(c["recs"].shape[0]), p(read), p(a["rc"]), p(a["ep"]), p(np.concatenate([a["po"], [a["po"][-1] + a["npair"][-1]]]).astype(np.uint64)),
-                              cc._cstrs(a["names"]), len(c["bases"]), cc._cstrs(a["seq_bases"]), p(a["seq_rc"]), p(a["sp"]), p(a["soff"]),
-                              cc.CALL_FLANK, cc.CALL_MIN_DISTANCE, cc.CALL_MAX_HAPLOTYPES, c["ploidy"], 0, b"", c["all_support"], c["snps_only"],
-                              C.c_double(c["min_frequency"]), c["min_depth"], None if c["candidates"] is None else c["candidates"].encode(),
-                              C.c_double(1.0), out, C.c_size_t(cap))
-    return int(n), out.raw[:max(int(n), 0)]
-
-
 @pytest.mark.parametrize("spec", cc.CALL_CASES, ids=[s[0] for s in cc.CALL_CASES])
 def test_region_call_vcf_equals_reference(host, spec):
     c = cc.build_call(spec)
     want = case_answers(GOLDEN, spec[0])[cc.call_fingerprint(c)]
-    n, got = call_region(host, c)
+    n, got = cc.call_region(host, c)
     assert n >= 0, host.nphh_last_error()
     assert got == want
 
@@ -188,7 +146,7 @@ def test_region_call_refusals(host):
     c = cc.build_call(cc.CALL_CASES[2])
     for kw in (dict(start_base=c["end_base"] + 1), dict(start_base=c["contig_length"] - 39, end_base=c["contig_length"] + 5),
                dict(region_start=c["region_start"] + 1, region_ref=c["region_ref"][1:])):
-        n, _ = call_region(host, dict(c, **kw))
+        n, _ = cc.call_region(host, dict(c, **kw))
         assert n == NPH_ERR_INVALID, kw
-    n, _ = call_region(host, dict(c, candidates="ctg\t5100\n"))                  # read_vcf asserts on an empty REF
+    n, _ = cc.call_region(host, dict(c, candidates="ctg\t5100\n"))                  # read_vcf asserts on an empty REF
     assert n == NPH_ERR_INVALID

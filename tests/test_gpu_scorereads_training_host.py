@@ -11,11 +11,16 @@ import pytest
 from nanopolish_b200 import synth
 from nanopolish_b200.engine import Engine
 from tests import eventalign_cases as EC
-from tests import test_eventalign as TE
+from tests import host_mirror as hm
 from tests import transition_restatement as tr
-from tests.test_host_scorereads import EPS, _call, cases, host  # noqa: F401  (module fixtures)
 
 pytestmark = pytest.mark.gpu
+host = hm.fixture()
+
+
+@pytest.fixture(scope="module")
+def cases():
+    return EC.build_cases()
 
 
 def _train(host, cases, train, n_batches, max_chunk_jobs=0):
@@ -25,9 +30,8 @@ def _train(host, cases, train, n_batches, max_chunk_jobs=0):
     refs = (C.c_char_p * n)(*[c["fetched"].encode() for c in cs])
     offs = np.array([c["ref_pos"] for c in cs], np.int32)
     sc = np.zeros((n, 3)); counts = np.zeros((2, tr.WORDS), np.uint64); buf = C.create_string_buffer(1 << 14)
-    p = TE._p
-    host.nphh_scorereads_train.restype = C.c_longlong
-    k = host.nphh_scorereads_train(n, p(reads), refs, p(offs), EPS, train, C.c_uint32(max_chunk_jobs), n_batches, p(sc), p(counts), buf,
+    p = hm.p
+    k = host.nphh_scorereads_train(n, p(reads), refs, p(offs), EC.EPS, train, C.c_uint32(max_chunk_jobs), n_batches, p(sc), p(counts), buf,
                                    C.c_size_t(1 << 14))
     assert k >= 0, host.nphh_last_error()
     return sc, counts, buf.raw[:k].decode()
@@ -35,7 +39,7 @@ def _train(host, cases, train, n_batches, max_chunk_jobs=0):
 
 def test_score_reads_with_training(host, cases):
     model, rs, cs = cases
-    TE._setup(host, cases)
+    EC.load_batch(host, cases)
     assert host.nphh_ea_run(C.c_double(1.0)) >= 0, host.nphh_last_error()
     plain, _, text0 = _train(host, cases, 0, 1)
     one, c1, text1 = _train(host, cases, 1, 1)
@@ -44,7 +48,7 @@ def test_score_reads_with_training(host, cases):
     assert plain.tobytes() == one.tobytes() == two.tobytes()                 # training leaves the scores as they are
     assert c1.tobytes() == c2.tobytes() and text1 == text2                    # two batches accumulate to the one-batch counts
     # the restatement over the device's Viterbi paths of the same segments (the job list ScoreReads builds, mode 0)
-    jobs, ranks, _ = _call(host, cases, mode=0)
+    jobs, ranks, _ = EC.scorereads(host, cases, mode=0)
     slots = list(dict.fromkeys(EC.read_slot(c, rs.n_reads) for c in cs))    # the batch's read table: reads in first-use order
     jobs = jobs.copy()
     jobs["read"] = np.array(slots, np.uint32)[jobs["read"]]

@@ -4,29 +4,22 @@ HMMs, tests/test_screen_variants_oracle.py, recorded in tests/golden/ref_screen_
 nph::screen_variants_by_score returns the reference's list.  Also: reads_per_round does not change a quality; random lists of about
 2 000 candidates against the restatement over nph_hmm_score_batch's scores; the substitutions and insertions of nph_screen_edits_batch
 bit for bit; the host mirror's expand_variants; an empty list, an empty pile-up and a list outside the region; every refusal."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
 from nanopolish_b200 import synth
 from nanopolish_b200._lib import NphError
 from nanopolish_b200.engine import Engine
+from tests import host_mirror as hm
 from tests import screen_cases as sc
 from tests import screen_restatement as scr
 from tests.ref_calls import case_answers
-from tests.test_host_mirror import HOST_SO
-from tests.test_variants_methylation_oracle import type_models
 
 pytestmark = pytest.mark.gpu
 GOLDEN = "ref_screen_variants.pkl.xz"
 
 
-@pytest.fixture(scope="module")
-def host():
-    lib = C.CDLL(HOST_SO)
-    lib.nphh_last_error.restype = C.c_char_p
-    return lib
+host = hm.fixture()
 
 
 @pytest.fixture(scope="module")
@@ -34,7 +27,7 @@ def eng():
     e = Engine(0)
     e.model_upload(synth.load_model("nucleotide"))                       # model 0
     for t in sc.ALL_TYPES:                                               # models 1, 2, 3
-        e.model_upload(type_models([t])[t])
+        e.model_upload(sc.type_models([t])[t])
     yield e
     e.close()
 
@@ -121,9 +114,8 @@ def test_edits_equal_the_edit_screen(eng, types):
     """a substitution or insertion at position i has the edit screen's window [i - flank, i + 1 + flank] and reads, so both calls
     give the same quality bits (with dam,dcm: sets of up to three sequences, through the edit screen's fixed rank pool and the list's
     variable one)"""
-    from tests.test_variants_methylation_oracle import methylated_pileup
     if types:
-        _, _, _, ref_chars, rs, recs, pairs = methylated_pileup(list(types), 240, 10, 120, seed=91)
+        _, _, _, ref_chars, rs, recs, pairs = sc.methylated_pileup(list(types), 240, 10, 120, seed=91)
         draft = ref_chars.tobytes().decode()
         deltas, first = synth.compact_event_alignment(recs, pairs, int(recs["ref_len"].sum()))
     else:

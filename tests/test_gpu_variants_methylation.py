@@ -11,7 +11,7 @@ from nanopolish_b200._lib import NphError
 from tests import var_meth_restatement as vmr
 from tests import var_restatement as vr
 from tests.ref_types import _ref_types_session, ref_types  # noqa: F401  (fixtures)
-from tests.test_variants_methylation_oracle import N_AT, TYPE_LISTS, methylated_pileup, type_models, with_n
+from tests.screen_cases import N_AT, TYPE_LISTS, methylated_pileup, type_models, with_n
 
 pytestmark = pytest.mark.gpu
 K = 6

@@ -4,7 +4,7 @@ import numpy as np
 import pytest
 
 from nanopolish_b200 import synth
-from tests.test_gpu_hmm import _random_jobs
+from tests.random_cases import random_hmm_jobs
 
 pytestmark = pytest.mark.gpu
 
@@ -51,7 +51,7 @@ def test_random_shapes(engine, nuc, port_oracle, shape):
     model, mid = nuc
     rs = synth.gen_reads(6, 2200, model, seed=300 + shape["kmin"])
     rng = np.random.default_rng(shape["kmax"])
-    jobs = _random_jobs(rs, rng, shape["n"], shape["kmin"], shape["kmax"], shape["emin"], shape["emax"], [0, 1, 2, 3])
+    jobs = random_hmm_jobs(rs, rng, shape["n"], shape["kmin"], shape["kmax"], shape["emin"], shape["emax"], [0, 1, 2, 3])
     dj = jobs.jobs.copy(); dj["model_id"] = mid
     got, _ = engine.hmm_align_batch(rs.reads, rs.ev_mean, rs.ev_start_time, jobs.kmer_ranks, dj, indel_bias=0.9)
     want = [port_oracle.hmm_align(rs.reads, rs.ev_mean, rs.ev_start_time, [model], jobs.kmer_ranks, jobs.jobs[j], indel_bias=0.9)

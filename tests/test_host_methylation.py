@@ -8,19 +8,13 @@ import numpy as np
 import pytest
 
 from nanopolish_b200 import synth
+from tests import host_mirror as hm
+from tests import meth_cases as mc
 from tests import meth_restatement as mr
-from tests.test_host_mirror import HOST_SO, _register, _register_reads
 
 pytestmark = pytest.mark.gpu
 K = 6
-
-
-@pytest.fixture(scope="module")
-def host():
-    lib = C.CDLL(HOST_SO)
-    lib.nphh_last_error.restype = C.c_char_p
-    lib.nphh_call_methylation.restype = C.c_longlong
-    return lib
+host = hm.fixture()
 
 
 def _expected_tsv(port_oracle, rs, models, reads_meta):
@@ -42,8 +36,8 @@ def _expected_tsv(port_oracle, rs, models, reads_meta):
 def test_call_methylation_tsv_identical(host, port_oracle):
     nuc, cpg = synth.load_model("nucleotide"), synth.load_model("cpg")
     rs = synth.gen_reads(6, 2500, nuc, seed=2024, cpg_keep=0.3)
-    mh, ch = _register(host, nuc), _register(host, cpg)
-    rh = _register_reads(host, rs, mh)
+    mh, ch = hm.register_model(host, nuc), hm.register_model(host, cpg)
+    rh = hm.register_reads(host, rs, mh)
     for r in rh:
         host.nphh_read_add_model(r, b"cpg", ch)
     metas = []
@@ -71,7 +65,7 @@ def test_call_methylation_tsv_identical(host, port_oracle):
     off = np.zeros(n + 1, np.uint64); off[1:] = np.cumsum([len(m["pairs"]) for m in metas])
     names = (C.c_char_p * n)(*[m["name"].encode() for m in metas])
     refs = (C.c_char_p * n)(*[m["ref"].encode() for m in metas])
-    p = lambda a: a.ctypes.data_as(C.c_void_p)
+    p = hm.p
     buf = C.create_string_buffer(1 << 20)
     njobs = C.c_uint64()
     got = host.nphh_call_methylation(n, p(np.array(rh, np.int32)), names, p(np.array([m["is_rev"] for m in metas], np.uint8)),
@@ -86,7 +80,6 @@ def test_flat_call_formats_its_rows_on_the_device(host):
     """nph::call_methylation_flat with the compact event alignment: one C call, methylation_calls.tsv bytes out, the rows formatted by
     nph_methylation_tsv — against Python's formatting of the site records of the same batch."""
     from nanopolish_b200.engine import Engine
-    from tests.test_gpu_methylation import _expected_rows
     nuc, cpg = synth.load_model("nucleotide"), synth.load_model("cpg")
     rs = synth.gen_reads(40, 2500, nuc, seed=808, cpg_keep=0.3)
     ref, pairs, recs = synth.methylation_records(rs, model_id=1, rc_every=2)
@@ -101,13 +94,11 @@ def test_flat_call_formats_its_rows_on_the_device(host):
     n = rs.n_reads
     names_py = [f"read_{i}" for i in range(n)]
     is_rev = np.ascontiguousarray(recs["rc"]).astype(np.uint8)
-    want = _expected_rows(sites, site_off, recs, ref, names_py, is_rev, "chr1", K)
-    vp = lambda a: a.ctypes.data_as(C.c_void_p)
+    want = mc.expected_rows(sites, site_off, recs, ref, names_py, is_rev, "chr1", K)
+    vp = hm.p
     cm, cs, cl = (np.ascontiguousarray(x) for x in (cpg.level_mean, cpg.level_stdv, cpg.level_log_stdv))
-    host.nphh_model_create.restype = C.c_int
     mh = host.nphh_model_create(b"cpg", 6, cm.shape[0], vp(cm), vp(cs), vp(cl))
     names = (C.c_char_p * n)(*[s.encode() for s in names_py])
-    host.nphh_call_methylation_flat.restype = C.c_longlong
     buf = np.zeros(len(want) + 4096, np.uint8)
     ns, se = C.c_uint64(), C.c_uint64()
     secs = np.zeros(2)

@@ -3,25 +3,15 @@ copied from the reference's own unit test expectations (src/test/nanopolish_test
 randomised agreement with the compiled reference, and — on the GPU — profile_hmm_score /
 profile_hmm_score_set / adaptive_banded_simple_event_align called exactly like a nanopolish caller."""
 import ctypes as C
-import os
 
 import numpy as np
 import pytest
 
 from nanopolish_b200 import synth
+from tests import host_mirror as hm
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HOST_SO = os.path.join(ROOT, "nanopolish_b200", "libnph_host.so")
 OPS = {"reverse_complement": 0, "methylate": 1, "unmethylate": 2, "disambiguate": 3}
-
-
-@pytest.fixture(scope="module")
-def host():
-    lib = C.CDLL(HOST_SO)
-    lib.nphh_last_error.restype = C.c_char_p
-    lib.nphh_kmer_rank.restype = C.c_uint32
-    lib.nphh_abea.restype = C.c_longlong
-    return lib
+host = hm.fixture()
 
 
 def _op(lib, alphabet, op, s):
@@ -120,32 +110,14 @@ def test_rolling_ranks_equal_get_kmer_rank(host):
 
 
 # ---- GPU: the reference's free functions through the mirror -----------------------------------
-def _register(host, model):
-    mean = np.ascontiguousarray(model.level_mean); sd = np.ascontiguousarray(model.level_stdv)
-    lsd = np.ascontiguousarray(model.level_log_stdv)
-    p = lambda a: a.ctypes.data_as(C.c_void_p)
-    return host.nphh_model_create(model.alphabet.encode(), model.k, mean.shape[0], p(mean), p(sd), p(lsd))
-
-
-def _register_reads(host, rs, mh):
-    hs = []
-    for r in rs.reads:
-        o, n = int(r["event_off"]), int(r["n_events"])
-        m = np.ascontiguousarray(rs.ev_mean[o:o + n]); t = np.ascontiguousarray(rs.ev_start_time[o:o + n])
-        hs.append(host.nphh_read_create(n, m.ctypes.data_as(C.c_void_p), t.ctypes.data_as(C.c_void_p), C.c_double(r["shift"]),
-                                        C.c_double(r["scale"]), C.c_double(r["drift"]), C.c_double(r["var"]),
-                                        C.c_double(r["events_per_base"]), mh))
-    return hs
-
-
 @pytest.mark.gpu
 def test_profile_hmm_score_like_a_caller(host, port_oracle):
     nuc = synth.load_model("nucleotide")
     rs = synth.gen_reads(3, 900, nuc, seed=61, drift=True)
     jobs = synth.scorereads_jobs(rs, 200, rc_every=2, keep_seqs=True)
     want, _ = port_oracle.hmm_score_batch(rs.reads, rs.ev_mean, rs.ev_start_time, [nuc], jobs.kmer_ranks, jobs.jobs)
-    mh = _register(host, nuc)
-    rh = _register_reads(host, rs, mh)
+    mh = hm.register_model(host, nuc)
+    rh = hm.register_reads(host, rs, mh)
     host.nphh_set_indel_bias(C.c_double(1.0))
     # one call per job, exactly the reference's signature
     for j in range(min(4, jobs.jobs.shape[0])):
@@ -160,7 +132,7 @@ def test_profile_hmm_score_like_a_caller(host, port_oracle):
     buf = b"".join(jobs.seqs)
     off = np.zeros(n + 1, np.uint64); off[1:] = np.cumsum([len(s) for s in jobs.seqs])
     got = np.zeros(n, np.float32)
-    p = lambda a: a.ctypes.data_as(C.c_void_p)
+    p = hm.p
     reads = np.ascontiguousarray(np.array(rh, np.int32)[jobs.jobs["read"]])
     models = np.full(n, mh, np.int32)
     rc = host.nphh_profile_hmm_score_many(C.c_size_t(n), p(reads), p(models), C.c_char_p(buf), p(off),
@@ -179,8 +151,8 @@ def test_profile_hmm_score_set_like_a_caller(host, port_oracle):
     nuc, cpg = synth.load_model("nucleotide"), synth.load_model("cpg")
     rs = synth.gen_reads(2, 600, nuc, seed=88, cpg_keep=0.4)
     mj = synth.methylation_jobs(rs, model_id=1, keep_seqs=True, max_groups_per_read=3)
-    mh, ch = _register(host, nuc), _register(host, cpg)
-    rh = _register_reads(host, rs, mh)
+    mh, ch = hm.register_model(host, nuc), hm.register_model(host, cpg)
+    rh = hm.register_reads(host, rs, mh)
     for r in rh:
         host.nphh_read_add_model(r, b"cpg", ch)
     for g in range(mj.jobs.shape[0] // 2):
@@ -212,8 +184,8 @@ def test_abea_and_mom_like_a_caller(host, port_oracle):
     rs = synth.gen_reads(2, 700, nuc, seed=17, rng_scalings=False)
     jobs, ranks, total = synth.abea_jobs(rs)
     po, ro, _ = port_oracle.abea_batch(rs.reads, rs.ev_mean, rs.ev_start_time, nuc, ranks, jobs, total)
-    mh = _register(host, nuc)
-    rh = _register_reads(host, rs, mh)
+    mh = hm.register_model(host, nuc)
+    rh = hm.register_reads(host, rs, mh)
     for i in range(rs.n_reads):
         seq = synth._CODE2DNA[rs.seq_codes[i]].tobytes()
         cap = int(jobs[i]["pairs_cap"])
@@ -249,7 +221,7 @@ def test_load_from_raw_like_a_caller(host, port_oracle):
     signals.append(noise); seqs.append(seqs[1][:2000])
     n = len(signals)
     want = oracle_chain(port_oracle, nuc, signals, seqs)
-    mh = _register(host, nuc)
+    mh = hm.register_model(host, nuc)
     soff = np.zeros(n + 1, np.uint64); soff[1:] = np.cumsum([s.shape[0] for s in signals])
     qoff = np.zeros(n + 1, np.uint64); qoff[1:] = np.cumsum([c.shape[0] for c in seqs])
     seqbuf = b"".join(synth._CODE2DNA[c].tobytes() for c in seqs)
@@ -259,7 +231,7 @@ def test_load_from_raw_like_a_caller(host, port_oracle):
     mean = np.zeros(room, np.float32); stdv = np.zeros(room, np.float32); start = np.zeros(room, np.float64); dur = np.zeros(room, np.float32)
     b2e = np.full((int(qoff[-1]), 2), -7, np.int32)
     flat = np.concatenate(signals)
-    p = lambda a: a.ctypes.data_as(C.c_void_p)
+    p = hm.p
     host.nphh_set_load_flags(2)                                 # SRF_LOAD_RAW_SAMPLES: keep the trimmed samples on every read
     try:
         rc = host.nphh_load_from_raw(mh, n, p(flat), p(soff), seqbuf, p(qoff), C.c_double(4000.0), p(n_events), p(scal), p(eoff), p(mean), p(stdv),
@@ -267,8 +239,6 @@ def test_load_from_raw_like_a_caller(host, port_oracle):
     finally:
         host.nphh_set_load_flags(0)
     assert rc >= 0, host.nphh_last_error()
-    host.nphh_read_num_samples.restype = C.c_longlong
-    host.nphh_read_sample.restype = C.c_float
     for i in range(n):                                          # samples[i] = rt.raw[rt.start + i] (squiggle_read.cpp:251-258)
         s0, s1 = want[i]["range"]
         assert host.nphh_read_num_samples(rc + i) == s1 - s0
@@ -317,7 +287,7 @@ def test_load_from_raw_direct_rna_like_a_caller(host, port_oracle):
     want = oracle_chain(port_oracle, rna, signals, seqs, sample_rate=3012.0, rna=True)
     mean5, sd = np.ascontiguousarray(rna.level_mean), np.ascontiguousarray(rna.level_stdv)
     lsd = np.ascontiguousarray(rna.level_log_stdv)
-    p = lambda a: a.ctypes.data_as(C.c_void_p)
+    p = hm.p
     mh = host.nphh_model_create(b"u_to_t_rna", 5, 1024, p(mean5), p(sd), p(lsd))
     assert mh >= 0, host.nphh_last_error()
     soff = np.zeros(n + 1, np.uint64); soff[1:] = np.cumsum([s.shape[0] for s in signals])

@@ -8,17 +8,10 @@ import numpy as np
 import pytest
 
 from oracle import eventalign_py as EP
-from tests.test_host_mirror import HOST_SO
+from tests import host_mirror as hm
 
 K = 6
-
-
-@pytest.fixture(scope="module")
-def host():
-    lib = C.CDLL(HOST_SO)
-    lib.nphh_last_error.restype = C.c_char_p
-    lib.nphh_modbam_tags.restype = C.c_longlong
-    return lib
+host = hm.fixture()
 
 
 def _host_tags(host, seq, ref_pos, flag, cigar, calls, reference_mode=0):
@@ -27,7 +20,7 @@ def _host_tags(host, seq, ref_pos, flag, cigar, calls, reference_mode=0):
     seqs = (C.c_char_p * max(n, 1))(*[c[1].encode() for c in calls])
     lm = np.array([c[2] for c in calls], np.float64); lu = np.array([c[3] for c in calls], np.float64)
     mm = C.create_string_buffer(1 << 16); ml = np.zeros(1 << 14, np.uint8)
-    p = lambda a: a.ctypes.data_as(C.c_void_p)
+    p = hm.p
     cg = np.ascontiguousarray(cigar, np.uint32)
     k = host.nphh_modbam_tags(seq.encode(), int(ref_pos), int(flag), p(cg), int(cg.shape[0]), n, p(sp), seqs, p(lm), p(lu), reference_mode,
                               mm, C.c_size_t(1 << 16), p(ml), C.c_size_t(ml.shape[0]))
@@ -110,6 +103,6 @@ def test_modbam_rejects_spliced_records(host):
     ref, seq, ref_pos, flag, cigar, calls = _record(rng)
     spliced = np.concatenate([cigar[:2], EP.pack_cigar([(30, "N")]), cigar[2:]])
     mm = C.create_string_buffer(64); ml = np.zeros(8, np.uint8)
-    p = lambda a: a.ctypes.data_as(C.c_void_p)
+    p = hm.p
     assert host.nphh_modbam_tags(seq.encode(), ref_pos, 0, p(spliced), int(spliced.shape[0]), 0, None, (C.c_char_p * 1)(), None, None, 0,
                                  mm, C.c_size_t(64), p(ml), C.c_size_t(8)) < 0           # the reference exits on spliced alignments

@@ -14,19 +14,9 @@ import pytest
 from nanopolish_b200 import synth
 from oracle import eventalign_py as EP
 from tests import eventalign_cases as EC
-from tests import test_eventalign as TE
+from tests import host_mirror as hm
 
-EPS = 200          # events per segment (the reference uses 500 on whole reads; the test reads have ~1 500 events)
-
-
-@pytest.fixture(scope="module")
-def host():
-    from tests.test_host_mirror import HOST_SO
-    lib = C.CDLL(HOST_SO)
-    lib.nphh_last_error.restype = C.c_char_p
-    for f in ("nphh_ea_run", "nphh_ea_next_round", "nphh_ea_text", "nphh_ea_num_segments", "nphh_aligned_segments", "nphh_scorereads"):
-        getattr(lib, f).restype = C.c_longlong
-    return lib
+host = hm.fixture()
 
 
 @pytest.fixture(scope="module")
@@ -39,8 +29,8 @@ def _expected_segments(cs, restated, rs):
     out = []
     for c, (al, _) in zip(cs, restated):
         segs = []
-        for start in range(EPS, len(al) - EPS, EPS):
-            a0, a1 = al[start], al[start + EPS]
+        for start in range(EC.EPS, len(al) - EC.EPS, EC.EPS):
+            a0, a1 = al[start], al[start + EC.EPS]
             seg = c["fetched"][a0.ref_position - c["ref_pos"]:a1.ref_position - c["ref_pos"] + 1]
             if len(seg) <= EC.K:
                 continue
@@ -62,20 +52,6 @@ def _restate(cases, port_oracle):
     return out
 
 
-def _call(host, cases, mode):
-    model, rs, cs = cases
-    n = len(cs)
-    reads = np.array([EC.read_slot(c, rs.n_reads) for c in cs], np.int32)      # g_reads handles == slots after _setup
-    refs = (C.c_char_p * n)(*[c["fetched"].encode() for c in cs])
-    offs = np.array([c["ref_pos"] for c in cs], np.int32)
-    jobs = np.zeros(256, synth.HMM_JOB_DT); ranks = np.zeros(1 << 18, np.uint32); nr = C.c_uint64(); sc = np.zeros((n, 3))
-    p = TE._p
-    k = host.nphh_scorereads(n, p(reads), refs, p(offs), EPS, mode, p(jobs), C.c_size_t(jobs.shape[0]), p(ranks), C.c_size_t(ranks.shape[0]),
-                             C.byref(nr), p(sc))
-    assert k >= 0, host.nphh_last_error()
-    return jobs[:k].copy(), ranks[:nr.value].copy(), sc
-
-
 def _check_jobs(jobs, ranks, want):
     flat = [s for segs in want for s in segs]
     assert jobs.shape[0] == len(flat) > 10
@@ -87,9 +63,9 @@ def _check_jobs(jobs, ranks, want):
 def test_model_score_segments_on_cpu(host, cases, port_oracle):
     model, rs, cs = cases
     restated = _restate(cases, port_oracle)
-    TE._setup(host, cases)
-    TE._drive_rounds(host, cs, rs, model, port_oracle)
-    jobs, ranks, _ = _call(host, cases, mode=0)
+    EC.load_batch(host, cases)
+    EC.drive_rounds(host, cs, rs, model, port_oracle)
+    jobs, ranks, _ = EC.scorereads(host, cases, mode=0)
     _check_jobs(jobs, ranks, _expected_segments(cs, restated, rs))
     host.nphh_ea_begin()
 
@@ -98,9 +74,9 @@ def test_model_score_segments_on_cpu(host, cases, port_oracle):
 def test_model_score_on_device(host, cases, port_oracle):
     model, rs, cs = cases
     restated = _restate(cases, port_oracle)
-    TE._setup(host, cases)
+    EC.load_batch(host, cases)
     assert host.nphh_ea_run(C.c_double(1.0)) >= 0, host.nphh_last_error()
-    jobs, ranks, sc = _call(host, cases, mode=1)
+    jobs, ranks, sc = EC.scorereads(host, cases, mode=1)
     want = _expected_segments(cs, restated, rs)
     _check_jobs(jobs, ranks, want)
     # per-read score from the oracle's profile_hmm_score of the same segments (float scores summed in double, in order)

@@ -2,20 +2,14 @@
 Haplotype::apply_variant semantics, and score_variants_thresholded against an expectation composed from the
 oracle's per-sequence scores + the reference's host arithmetic (score_set logsum, read-order early exit)."""
 import ctypes as C
-import os
 
 import numpy as np
 import pytest
 
 from nanopolish_b200 import synth
-from tests.test_host_mirror import HOST_SO, _register, _register_reads
+from tests import host_mirror as hm
 
-
-@pytest.fixture(scope="module")
-def host():
-    lib = C.CDLL(HOST_SO)
-    lib.nphh_last_error.restype = C.c_char_p
-    return lib
+host = hm.fixture()
 
 
 def _apply(host, ref, pos0, variants):
@@ -107,8 +101,8 @@ def test_expectation_is_the_compiled_reference(host, port_oracle, ref_oracle, me
 @pytest.mark.parametrize("meth,threshold", [(False, 100), (True, 30)])
 def test_score_variants_thresholded(host, port_oracle, meth, threshold):
     nuc, cpg, codes, ref, rs, cands = _variant_case()
-    mh, ch = _register(host, nuc), _register(host, cpg)
-    rh = _register_reads(host, rs, mh)
+    mh, ch = hm.register_model(host, nuc), hm.register_model(host, cpg)
+    rh = hm.register_reads(host, rs, mh)
     for r in rh:
         host.nphh_read_add_model(r, b"cpg", ch)
     windows = [(0, int(rs.reads[j]["n_events"]) - 1) for j in range(rs.n_reads)]
@@ -119,7 +113,7 @@ def test_score_variants_thresholded(host, port_oracle, meth, threshold):
     assert vseqs[-1] is None and all(v is not None for v in vseqs[:-1])
     n = len(cands)
     q = np.zeros(n)
-    p = lambda a: a.ctypes.data_as(C.c_void_p)
+    p = hm.p
     reads = np.array(rh, np.int32)
     es = np.array([w[0] for w in windows], np.uint32); ee = np.array([w[1] for w in windows], np.uint32)
     rcs = np.zeros(rs.n_reads, np.uint8)
@@ -145,8 +139,8 @@ def test_score_variant_group_equals_compiled_reference(host, ref_oracle, meth, m
     (combination, read) score is the same double."""
     nuc, cpg, codes, ref, rs, cands = _variant_case()
     cands = cands[:4] + [(1000 + 20, "C", "A")]                 # the last one collides with candidate 1 (same reference base)
-    mh, ch = _register(host, nuc), _register(host, cpg)
-    rh = _register_reads(host, rs, mh)
+    mh, ch = hm.register_model(host, nuc), hm.register_model(host, cpg)
+    rh = hm.register_reads(host, rs, mh)
     for r in rh:
         host.nphh_read_add_model(r, b"cpg", ch)
     windows = [(0, int(rs.reads[j]["n_events"]) - 1) for j in range(rs.n_reads)]
@@ -155,13 +149,12 @@ def test_score_variant_group_equals_compiled_reference(host, ref_oracle, meth, m
     want = ref_oracle.score_variant_group(rrh, windows, np.zeros(rs.n_reads, np.uint8), ref, 1000, cands, max_haplotypes, 3, meth, indel_bias=0.9)
     ref_oracle.clear_reads()
     n = len(cands)
-    p = lambda a: a.ctypes.data_as(C.c_void_p)
+    p = hm.p
     reads = np.array(rh, np.int32)
     es = np.array([w[0] for w in windows], np.uint32); ee = np.array([w[1] for w in windows], np.uint32)
     rcs = np.zeros(rs.n_reads, np.uint8)
     mt = (C.c_char_p * 1)(b"cpg")
     combos = np.zeros(4096, np.uint32); scores = np.zeros(4096 * rs.n_reads)
-    host.nphh_score_variant_group.restype = C.c_longlong
     k = host.nphh_score_variant_group(rs.n_reads, p(reads), p(es), p(ee), p(rcs), mh, ref.encode(), C.c_size_t(1000), n,
                                       (C.c_size_t * n)(*[c[0] for c in cands]), (C.c_char_p * n)(*[c[1].encode() for c in cands]),
                                       (C.c_char_p * n)(*[c[2].encode() for c in cands]), max_haplotypes, 3, 1 if meth else 0, mt,

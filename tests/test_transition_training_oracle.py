@@ -81,10 +81,9 @@ def test_host_mirror_training(ref_tt):
     """nph::TransitionTraining (nanopolish_b200/host/nph_scorereads.cpp) on the recorded counts: train() with either prior equals
     the reference's trained probabilities, and report() equals its stderr for two strands"""
     import ctypes as C
-    from tests.test_host_mirror import HOST_SO
-    lib = C.CDLL(HOST_SO)
-    lib.nphh_transition_training.restype = C.c_longlong
-    p = lambda a: a.ctypes.data_as(C.c_void_p)
+    from tests import host_mirror as hm
+    lib = hm.load()
+    p = hm.p
     rows = {}
     for spec in (tc.CASES[0], tc.CASES[1], tc.CASES[3]):
         c = tc.build(spec)

@@ -1,41 +1,15 @@
 """The restatement of methylation-aware candidate screening (tests/var_meth_restatement.py) against the compiled reference's own
 score_variant_thresholded with opt::methylation_types, on methylated pile-ups: every type list, early exit on and off, both
 alignment-flag settings, forward and reverse reads, edits that create or destroy recognition sites, and windows with an N."""
-import os
-
 import numpy as np
 import pytest
 
-from nanopolish_b200 import synth
 from tests import var_meth_restatement as vmr
 from tests.ref_types import _ref_types_session, ref_types  # noqa: F401  (fixtures)
+from tests.screen_cases import N_AT, TYPE_LISTS, methylated_pileup, with_n
 
 K = 6
 REGION = 5000
-TYPE_LISTS = [["cpg"], ["dam"], ["dcm"], ["dam", "dcm"], ["dcm", "dam"]]
-N_AT = (33, 71)                     # region offsets of the planted N (inside some windows' flanks, never at a screened base or its left neighbour)
-
-
-def type_models(types):
-    for name in types:
-        # without its fixture load_model falls back to a synthetic table and the comparison would mean nothing
-        assert os.path.exists(os.path.join(synth._GOLDEN, f"r9.4_450bps.{name}.6mer.template.npz")), name
-    return {name: synth.load_model(name) for name in types}
-
-
-def methylated_pileup(types, ref_len, depth, read_bases, seed):
-    nuc = synth.load_model("nucleotide")
-    tm = type_models(types)
-    ref, rs, recs, pairs = synth.gen_pileup_methylated(ref_len, depth, read_bases, nuc, types, tm, seed=seed, region_start=REGION,
-                                                       n_true_variants=6, rc_every=2, methylated_fraction=0.6)
-    ref_chars = synth._CODE2DNA[ref].copy()
-    return nuc, tm, ref, ref_chars, rs, recs, pairs
-
-
-def with_n(ref_chars):
-    out = ref_chars.copy()
-    out[list(N_AT)] = ord("N")
-    return out
 
 
 def changes_sets(sets):
